@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- MCTS simulations/s of the fused CUDA search (BASELINE.json metric) on N B200s.
+"""bench.py -- MCTS simulations/s of the fused CUDA search (BASELINE.json metric) on N H100s.
 
 A "step" is one full collect step of the hot path over one batch of synthetic observations:
 initial_inference -> root preparation (Dirichlet noise) -> num_simulations x [PUCT traverse ->
@@ -8,6 +8,7 @@ MuZeroPolicy._forward_collect does between receiving obs and choosing actions
 (lzero/policy/muzero.py:749-779).  simulations/s = roots * num_simulations / step time.
 
   python bench.py [--gpus N --steps K --warmup W]             # our arm  (torchrun for N > 1)
+  python bench.py ... --dump-outputs DIR                       # + the last timed step's outputs as DIR/<name>.npy
   python bench.py --impl reference [--gpus N --steps K ...]   # reference arm: the reference's own
         CPU path (compiled reference ctree from oracle/_ref + PyTorch-CPU fp32 model) on host cores
 
@@ -71,7 +72,11 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the strong_scaling and extra.workloads blocks")
     ap.add_argument("--h2d-chunks", type=int, default=2)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (visits, values, ...) as DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     select_workload(args.workload)
     args.roots = args.roots or ROOTS_PER_GPU
     args.sims = args.sims or NUM_SIMULATIONS
@@ -225,20 +230,27 @@ def _peak():
     pk_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pk_path):
         peaks = json.load(open(pk_path))
-        return float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1590.0))), \
+        return float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 989.0))), \
             "measured (MEASURED_PEAKS.json bf16_tflops_sustained: kernel timed inside a long step)"
-    return 1590.0, "fallback (B200_PROFILING.md: 1.59 PFLOP/s burst)"
+    return 989.0, "H100 SXM data sheet: 989 TFLOP/s dense BF16 at 700 W (not a measured rate)"
 
 
-def _traffic(workload_key):
-    """dram__bytes_read + dram__bytes_write of the dominant kernel from the committed ncu capture (profiles/roofline_traffic.json,
-    written by profiles/summarize.py), or None when no capture of the current kernel exists."""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "roofline_traffic.json")))
-        e = t.get(workload_key)
-        return (e["bytes_per_launch"], e["source"]) if e else (None, None)
-    except Exception:
-        return None, None
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out, dirname):
+    """Writes the tensors of one search_batch result as <name>.npy: floating point as float32, integers as float64 (exact).  An
+    output larger than its share of 64 MB is replaced by a fixed, seeded sample of its rows."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    arrays = {k: v.detach().cpu().numpy() for k, v in sorted(out.items()) if hasattr(v, "detach")}
+    share = DUMP_LIMIT_BYTES // max(1, len(arrays))
+    for name, a in arrays.items():
+        a = a.astype(np.float32 if np.issubdtype(a.dtype, np.floating) else np.float64)
+        if a.nbytes > share and a.ndim >= 1:
+            rows = max(1, share // max(1, a.nbytes // a.shape[0]))
+            a = a[np.sort(np.random.default_rng(0).choice(a.shape[0], rows, replace=False))]
+        np.save(os.path.join(dirname, name + ".npy"), a)
 
 
 def ours(args, rank, local_rank, world):
@@ -374,7 +386,16 @@ def ours(args, rank, local_rank, world):
     if rank == 0:
         sampler.start()      # sampled across warm-up + timed region (same load; nvidia-smi needs ~100 ms to start)
         time.sleep(0.3)
-    dev_ms, wall_ms, launches = timed(device_step(W), args.steps, warm)
+    last = {}
+
+    def keep_last(fn):
+        def run(i):
+            last["out"] = fn(i)
+            return last["out"]
+        return run
+    dev_ms, wall_ms, launches = timed(keep_last(device_step(W)), args.steps, warm)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(last["out"], args.dump_outputs)
     clocks = sampler.stop() if rank == 0 else None
     e2e_dev_ms, e2e_wall_ms, _ = timed(e2e_step(W), args.steps, warm)
     e2e_full_wall_ms = e2e_wall_ms
@@ -395,8 +416,8 @@ def ours(args, rank, local_rank, world):
                     d_ms, k_ms = dev_ms / args.steps, graph_avg_ms
                 else:
                     W2 = build(WORKLOADS["muzero"], G // world, S2)
-                    n2 = max(3, min(args.steps, 5))
-                    d2, _, _ = timed(device_step(W2), n2, 3)
+                    n2 = args.steps
+                    d2, _, _ = timed(device_step(W2), n2, warm)
                     k_ms, _, _ = search_only(W2)
                     d_ms, k_ms = maxr(d2 / n2, k_ms)
                     del W2
@@ -408,9 +429,9 @@ def ours(args, rank, local_rank, world):
     if not args.no_extras and args.workload == "muzero":
         wl2 = WORKLOADS["efficientzero"]
         W3 = build(wl2, wl2["roots"], wl2["sims"])
-        n3 = max(3, min(args.steps, 5))
-        d3, _, _ = timed(device_step(W3), n3, 3)
-        e3, ew3, _ = timed(e2e_step(W3), n3, 3)
+        n3 = args.steps
+        d3, _, _ = timed(device_step(W3), n3, warm)
+        e3, ew3, _ = timed(e2e_step(W3), n3, warm)
         k3, _, nk3 = search_only(W3)
         d3, ew3, k3 = maxr(d3 / n3, ew3 / n3, k3)
         tot3 = wl2["roots"] * world
@@ -432,7 +453,6 @@ def ours(args, rank, local_rank, world):
         h2d_full = W["h_u8"][0].numel() + W["h_mask"].numel() + W["h_noise"].numel() * 4
         h2d = (W["h_new"][0].numel() + W["h_mask"].numel() + W["h_noise"].numel() * 4) if W["fs"] is not None else h2d_full
         d2h = B * A * 4 + B * 4 * 3 + B * A * 4
-        traffic, traffic_src = _traffic(args.workload if (B, S, A) == (WL["roots"], WL["sims"], WL["actions"]) else "none")
         achieved = B * S * FLOP_RECURRENT / (graph_avg_ms * 1e-3) / 1e12
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
@@ -443,7 +463,7 @@ def ours(args, rank, local_rank, world):
                        "step": "initial_inference + prepare + S x (traverse, recurrent_inference, backpropagate) + results"
                                + (" (EfficientZero: value-prefix trees, LSTM state reset every lstm_horizon_len steps)" if EZ else ""),
                        "deterministic": True,
-                       "math": "tcgen05 fp16 hi/lo split (fp32-accurate: A_hi x [B_hi | B_lo] as one N = 128 MMA + A_lo x B_hi, fp32 accumulate in TMEM): the 1e-5 parity mode",
+                       "math": "wgmma fp16 hi/lo split (fp32-accurate: A_hi x B_hi + A_hi x B_lo + A_lo x B_hi, fp32 accumulate in registers): the 1e-5 parity mode",
                        "weights": "random, reference state_dict layout (lightzero_b200.synthetic_weights; no checkpoints offline)",
                        "l2": f"no explicit flush: per-step working set = rotating 3 x {W['d_f32'][0].numel() * 4 / 1e6:.0f} MB observation batches + "
                              f"{(S + 1) * B * (2304 + (1024 if EZ else 0)) * 4 / 1e6:.0f} MB latent / LSTM-state pools > 126 MB L2",
@@ -468,12 +488,11 @@ def ours(args, rank, local_rank, world):
             "gpu_launches_note": "counted by the library (lz_debug_launch_count: every kernel it enqueues, graph kernel nodes included) over the timed region",
             "search_graph_kernels": num_kernels_search,
             "roofline": {"bound": "tensor",
-                         "kernel": ("search graph = 1 + num_simulations x [k_net_tc conv trunk + prediction heads (tcgen05), k_ez_lstm_tc (tcgen05 3xFP16 GEMM "
+                         "kernel": ("search graph = 1 + num_simulations x [k_net_tc conv trunk + prediction heads (wgmma), k_ez_lstm_tc (wgmma 3xFP16 GEMM "
                                     "over all roots + cell update), k_ez_head, tree back-up + descent]" if EZ else
-                                    "k_net_tc, persistent launch = num_simulations x [tree back-up/descent + fused recurrent_inference] (tcgen05)"),
+                                    "k_net_tc, persistent launch = num_simulations x [tree back-up/descent + fused recurrent_inference] (wgmma)"),
                          "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf,
                          "frac_of_peak_over_3": 3 * achieved / peak_tf,
-                         "traffic": traffic, "traffic_source": traffic_src,
                          "peak_source": peak_note, "kernel_ms": graph_avg_ms, "kernel_ms_min": graph_min_ms,
                          "kernel_share_of_step": graph_avg_ms / ms_per_step,
                          "flop_per_launch": B * S * FLOP_RECURRENT,

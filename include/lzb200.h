@@ -1,5 +1,5 @@
 /*
- * lzb200.h -- C ABI of the B200-native batched MuZero MCTS + inference engine.
+ * lzb200.h -- C ABI of the H100-native batched MuZero MCTS + inference engine.
  *
  * This is the drop-in boundary for ONE hot path of opendilab/LightZero (file:line relative to the
  * reference repository root):
@@ -177,14 +177,14 @@ int lz_model_set_tensor(lz_model *m, const char *name, const float *h_data, int6
 int lz_model_finalize(lz_model *m);
 /* Arithmetic of the latent-grid networks (recurrent_inference and the tail of initial_inference):
  *   0 = fp32 FFMA on the CUDA cores;
- *   1 = tcgen05 tensor cores with fp16 hi/lo operand splitting (3 MMAs per product, fp32 accumulate in
- *       TMEM): fp32-accurate, the mode parity is stated for;
- *   2 = tcgen05 single fp16 pass (fp32 accumulate): ~3x fewer MMAs, logits accurate to ~1e-3. */
+ *   1 = wgmma tensor cores with fp16 hi/lo operand splitting (3 MMAs per product, fp32 accumulate in
+ *       registers): fp32-accurate, the mode parity is stated for;
+ *   2 = wgmma single fp16 pass (fp32 accumulate): ~3x fewer MMAs, logits accurate to ~1e-3. */
 int lz_model_set_math(lz_model *m, int mode);
-/* Test hook: overrides the layer program of the tcgen05 kernels (see net_tc.cuh LF_* flags). */
+/* Test hook: overrides the layer program of the tensor-core kernels (see net_tc.cuh LF_* flags). */
 int lz_model_debug_tc_program(lz_model *m, int which, int nlayers, const int *layer_w, const int *layer_flags,
                               int has_reward);
-/* Test hook: 64 clock64 stamps of CTA 0 of the last tcgen05 launch made with env LZ_TC_DEBUG=1. */
+/* Test hook: 64 clock64 stamps of CTA 0 of the last tensor-core launch made with env LZ_TC_DEBUG=1. */
 int lz_debug_tc_stamps(unsigned long long *h_out);
 int lz_model_latent_hw(const lz_model *m);   /* 6 for 84/96, 8 for 64 */
 int lz_model_support_size(const lz_model *m);
@@ -258,7 +258,7 @@ int lz_search_collect_host(lz_search *q, const float *h_obs, const uint8_t *h_ma
 /* The same two entry points for uint8 frames [B,obs_c,H,W] (Atari frames as the emulator delivers them; a quarter of the
  * bytes on the wire).  The [0, 1] scaling of the reference's env wrapper (ScaledFloatFrameWrapper: obs / 255 -> float32,
  * zoo/atari/envs/atari_wrappers.py:219-220, atari_lightzero_env.py:87-88) is applied inside the first conv kernel, bit-identical
- * to that host arithmetic.  tcgen05 conv model with 84x84 / 96x96 frames only. */
+ * to that host arithmetic.  tensor-core conv model with 84x84 / 96x96 frames only. */
 int lz_search_collect_u8(lz_search *q, const uint8_t *d_obs_u8, const uint8_t *d_mask, const float *d_noise,
                          float noise_weight, const int32_t *d_to_play, int deterministic,
                          float *d_pred_value, float *d_policy_logits, lz_stream s);

@@ -1,6 +1,6 @@
-"""lightzero_b200 -- B200-native batched MuZero MCTS + model inference behind the reference's own
+"""lightzero_b200 -- H100-native batched MuZero MCTS + model inference behind the reference's own
 interfaces (lzero.mcts.tree_search.MuZeroMCTSCtree, lzero.mcts.ctree.ctree_muzero.mz_tree,
-lzero.model.MuZeroModel; plus the EfficientZero counterparts EfficientZeroMCTSCtree, ez_tree, EfficientZeroModel).  All compute is hand-written sm_100a CUDA behind the C ABI of
+lzero.model.MuZeroModel; plus the EfficientZero counterparts EfficientZeroMCTSCtree, ez_tree, EfficientZeroModel).  All compute is hand-written sm_90a CUDA behind the C ABI of
 include/lzb200.h; this package is the thin host side."""
 from .mcts_ctree import EfficientZeroMCTSCtree, MuZeroMCTSCtree, UniZeroMCTSCtree  # noqa: F401
 from .efficientzero_model import EfficientZeroModel, EZNetworkOutput  # noqa: F401

@@ -106,7 +106,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a).  lightzero_b200 has no CPU / PyTorch fallback.")
+            "(nvcc, sm_90a).  lightzero_b200 has no CPU / PyTorch fallback.")
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)   # AttributeError here == header / library mismatch

@@ -106,7 +106,7 @@ int lz_frames_push(lz_frames *f, const uint8_t *d_new_frames, const uint8_t *d_r
     LZ_REQUIRE(f && d_new_frames, LZ_EINVAL, "lz_frames_push: null argument");
     const int fq = f->frame_bytes / 16;
     const size_t n = (size_t)f->B * f->stack * fq;
-    const int blocks = (int)((n + 255) / 256 < (size_t)148 * 8 ? (n + 255) / 256 : (size_t)148 * 8);
+    const int blocks = (int)((n + 255) / 256 < (size_t)kNumSMs * 8 ? (n + 255) / 256 : (size_t)kNumSMs * 8);
     k_frames_push<<<blocks, 256, 0, (cudaStream_t)s>>>(reinterpret_cast<const uint4 *>(f->buf[f->cur]), reinterpret_cast<uint4 *>(f->buf[f->cur ^ 1]),
                                                      reinterpret_cast<const uint4 *>(d_new_frames), d_reset, f->B, f->stack, fq);
     LZ_KERNEL_CHECK();

@@ -1,8 +1,9 @@
-// conv_tc.cu -- generic tcgen05 3x3 convolution for the DownSample tower (see conv_tc.cuh for the layout).
-// One CTA = one band of image rows (or G small whole images): bulk-copies the band (+halo) of every
-// k-group plane into shared memory, runs 9 taps x (Cin/16) k-steps x 3 fp16 hi/lo passes of tcgen05.mma
-// per 128-row tile with row-shifted descriptors, and writes BN / residual / ReLU results straight from
-// TMEM to the next layer's TCL tensor (already split into fp16 hi/lo).
+// conv_tc.cu -- generic wgmma 3x3 convolution for the DownSample tower (see conv_tc.cuh for the layout).
+// One CTA = one band of image rows (or G small whole images): bulk-copies the band (+halo) of every k-group plane into shared
+// memory once, then for each 128-row tile runs 9 taps x (Cin/16) k-steps x 3 fp16 hi/lo passes of wgmma (two warpgroups, 64 rows
+// each, accumulators in registers) with row-shifted descriptors; the taps stream through a ring once per tile (L2-resident, 4-16 KB
+// each).  The epilogue applies BN / residual / ReLU straight from the accumulator fragments and writes the next layer's TCL tensor
+// (already split into fp16 hi/lo).
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -12,32 +13,14 @@
 #include "conv_tc.cuh"
 #include "tc_ptx.cuh"
 
-// The MMAs are issued from uniform control flow: the whole issuing warp runs the loop and elect.sync picks the lane
-// (48.6 cycles per N = 64 MMA, the shared-memory operand floor, against 60-78 from an `if (lane == 0)` branch, where ptxas
-// wraps every UTCHMMA in an ELECT / BRA.U.ANY loop: profiles/r01e_mma_probe.md; validated on hardware in round 2).
-// -DLZ_LANE0_ISSUE restores the round-1 single-lane branch for A/B measurements.
-#ifndef LZ_LANE0_ISSUE
-#define LZ_MMA_ISSUER_ON true
-#define LZ_UMMA umma_f16_elect
-#define LZ_UCOMMIT umma_commit_elect
-#else
-#define LZ_MMA_ISSUER_ON (lane == 0)
-#define LZ_UMMA umma_f16
-#define LZ_UCOMMIT umma_commit
-#endif
-
 namespace lz {
 
-// 8 epilogue warps (two per TMEM lane quarter, one half of the output columns each): with the CTA's phases load -> MMA -> epilogue in series and
-// only two CTAs co-resident, the epilogue (and the exposed latency of its residual loads) was the longest phase with 4 warps (clock64 stamps,
-// tests/gpu_debug_tower.py); 320 threads x <= 102 registers still fit two CTAs per SM
-constexpr int kCvEpiWarps = 8, kCvEpiThreads = kCvEpiWarps * 32, kCvThreads = kCvEpiThreads + 64;
+constexpr int kCvConsumers = 256, kCvThreads = kCvConsumers + 32;   // two MMA / epilogue warpgroups + the producer warp
 constexpr int kCvStages = 4;          // ring slots reserved in the barrier block; p.stages (2..4) are used
 
 struct CvBars {
     uint64_t full[kCvStages], empty[kCvStages];
-    uint64_t in_full, acc_ready;
-    uint32_t tmem_base, pad;
+    uint64_t in_full;
 };
 
 struct CvGeom {                   // identical on host (shared-memory size) and device
@@ -65,8 +48,20 @@ __host__ __device__ inline CvGeom cv_geom(const ConvTc &p)
     return g;
 }
 
-template <int N, bool FOLD>
-__global__ void __launch_bounds__(kCvThreads, 2) k_conv_tc(ConvTc p)
+// fp16 hi / lo of two consecutive channels (4-byte stores)
+__device__ __forceinline__ void store_split2(unsigned char *hi_ptr, unsigned char *lo_ptr, float a, float b)
+{
+    a = fminf(fmaxf(a, -65504.0f), 65504.0f);
+    b = fminf(fmaxf(b, -65504.0f), 65504.0f);
+    const __half ha = __float2half_rn(a), hb = __float2half_rn(b);
+    *reinterpret_cast<__half2 *>(hi_ptr) = __halves2half2(ha, hb);
+    *reinterpret_cast<__half2 *>(lo_ptr) = __halves2half2(__float2half_rn(a - __half2float(ha)), __float2half_rn(b - __half2float(hb)));
+}
+
+template <int N>
+// N <= 64: <= 112 registers (32 or 16 accumulators per thread), so two CTAs can share an SM and overlap one CTA's band load /
+// epilogue with the other's MMAs; N = 128 needs 64 accumulators per thread and runs one CTA per SM
+__global__ void __launch_bounds__(kCvThreads, N == 128 ? 1 : 2) k_conv_tc(ConvTc p)
 {
     extern __shared__ __align__(1024) unsigned char smem[];
     const CvGeom g = cv_geom(p);
@@ -74,38 +69,23 @@ __global__ void __launch_bounds__(kCvThreads, 2) k_conv_tc(ConvTc p)
     unsigned char *ring = smem + g.in_bytes;
     CvBars *bars = reinterpret_cast<CvBars *>(ring + p.stages * g.tap_bytes);
     const int nstages = p.stages;
-    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;   // warp-uniform value: uniform role branches (see net_tc.cu)
+    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;   // warp-uniform value: uniform role branches
     const int pitch = p.in.pitch, H = p.in.H, W = p.in.W, kg_in = p.in.C / 8;
     const int group = blockIdx.x / g.nbands, band = blockIdx.x - group * g.nbands;
     const int img0 = group * p.G, nimg = min(p.G, p.B - img0);
     const int y0 = band * p.band_h;
     const int rin0 = y0 * pitch - 1;
     const int npass = p.npass;
-    // fp32-accurate mode, N <= 64: A_hi x [B_hi | B_lo] is ONE MMA of 2N columns (the tap block stores, per k-group, the N hi rows followed
-    // by the N lo rows) and A_lo x B_hi a second one of N columns: 2 instead of 3 A-operand-bound instructions per k-step; the accumulator
-    // of a tile is then 2N columns wide ([0, N) and [N, 2N) are added at read-out).  N = 128 keeps three N-column MMAs (2N = 256 columns
-    // would gain nothing: 128.7 + 64.7 vs 3 x 64.7 cycles, profiles/r01e_mma_probe.md).
-    constexpr bool kFold = FOLD;                 // chosen per layer on the host (pick_band)
-    constexpr int NA = kFold ? 2 * N : N;
-    uint32_t tmem_cols = 32;                         // power of two >= NT * NA: lets two CTAs share the SM's 512 columns
-    while (tmem_cols < (uint32_t)(g.NT * NA)) tmem_cols <<= 1;
 
     if (tid == 0) {
-        for (int i = 0; i < kCvStages; ++i) { mbar_init(&bars->full[i], 1); mbar_init(&bars->empty[i], 1); }
+        for (int i = 0; i < kCvStages; ++i) { mbar_init(&bars->full[i], 1); mbar_init(&bars->empty[i], kCvConsumers / 32); }
         mbar_init(&bars->in_full, 1);
-        mbar_init(&bars->acc_ready, 1);
         fence_mbar_init();
     }
-    if (warp == kCvEpiWarps + 1) tmem_alloc(&bars->tmem_base, tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = __shfl_sync(0xffffffffu, bars->tmem_base, 0);
 
-    unsigned long long *dbg = (p.dbg && blockIdx.x == gridDim.x / 2) ? p.dbg : nullptr;
-    if (dbg && tid == 0) dbg[58] = clock64();
-    if (warp == kCvEpiWarps) {
-        // ================= producer: input band, then the 9 weight taps =================
+    if (warp == kCvConsumers / 32) {
+        // ================= producer: input band, then the 9 weight taps once per tile =================
         if (lane == 0) {
             const int grow0 = rin0 + 1;                                    // memory row of rho = rin0
             const int ncopy = min(g.rin, p.in.plane_rows - grow0);
@@ -120,74 +100,69 @@ __global__ void __launch_bounds__(kCvThreads, 2) k_conv_tc(ConvTc p)
                             unsigned char *dst = in_s + f * g.phase + part * g.part + kg * g.plane + (size_t)k * g.rin * 16;
                             bulk_g2s(dst, src, bytes, &bars->in_full);
                         }
-            for (int tap = 0; tap < 9; ++tap) {
-                const int st = tap % nstages;
-                if (tap >= nstages) mbar_wait(&bars->empty[st], ((tap / nstages) - 1) & 1);
+            for (int n = 0; n < 9 * g.NT; ++n) {
+                const int st = n % nstages, tap = n % 9;
+                if (n >= nstages) mbar_wait(&bars->empty[st], ((n / nstages) - 1) & 1);
                 mbar_expect_tx(&bars->full[st], (uint32_t)g.tap_bytes);
                 bulk_g2s(ring + st * g.tap_bytes, p.w + (size_t)tap * g.tap_bytes, (uint32_t)g.tap_bytes, &bars->full[st]);
             }
         }
-    } else if (warp == kCvEpiWarps + 1) {
-        // ================= MMA issuer =================
-        if (LZ_MMA_ISSUER_ON) {
-            const uint32_t idesc = make_idesc_f16(128, N), idesc2 = make_idesc_f16(128, NA);
-            const uint32_t plane16 = (uint32_t)(g.plane >> 4);
-            const uint64_t a_desc0 = make_desc(smem_u32(in_s), plane16, 8);
-            const uint64_t b_desc0 = make_desc(smem_u32(ring), 2 * N, 8);        // tap block [kg][N hi rows | N lo rows][16 B]: LBO = 2N rows
-            const uint32_t b_lo16 = (uint32_t)N;                                  // the lo rows of a k-group, in 16-byte units
-            const uint32_t a_lo16 = (uint32_t)(g.part >> 4);
-            const int nks = kg_in / 2;
-            mbar_wait(&bars->in_full, 0);
-            tc_fence_after();
-            if (dbg && lane == 0) dbg[59] = clock64();
-            for (int tap = 0; tap < 9; ++tap) {
-                const int st = tap % nstages;
-                mbar_wait(&bars->full[st], (tap / nstages) & 1);
-                tc_fence_after();
-                const uint64_t b0 = b_desc0 + (uint64_t)((st * g.tap_bytes) >> 4);
-                const uint64_t a_tap = a_desc0 + (uint64_t)((p.tap_phase[tap] * g.phase) >> 4) + (uint64_t)(g.m_lo + p.tap_shift[tap]);
-                for (int t = 0; t < g.NT; ++t) {
-                    const uint64_t a0 = a_tap + (uint64_t)(t * 128);
-                    const uint32_t d = tmem + t * NA;
-                    if (npass != 3) {
-                        for (int ks = 0; ks < nks; ++ks)
-                            LZ_UMMA(d, a0 + ks * 2 * plane16, b0 + ks * 4 * N, idesc, (tap | ks) != 0);
-                    } else if (kFold) {
-                        for (int ks = 0; ks < nks; ++ks)
-                            LZ_UMMA(d, a0 + ks * 2 * plane16, b0 + ks * 4 * N, idesc2, (tap | ks) != 0);
-                        for (int ks = 0; ks < nks; ++ks)
-                            LZ_UMMA(d, a0 + a_lo16 + ks * 2 * plane16, b0 + ks * 4 * N, idesc, 1);
-                    } else {
-                        for (int ks = 0; ks < nks; ++ks)
-                            LZ_UMMA(d, a0 + ks * 2 * plane16, b0 + ks * 4 * N, idesc, (tap | ks) != 0);
-                        for (int ks = 0; ks < nks; ++ks)
-                            LZ_UMMA(d, a0 + ks * 2 * plane16, b0 + b_lo16 + ks * 4 * N, idesc, 1);
-                        for (int ks = 0; ks < nks; ++ks)
-                            LZ_UMMA(d, a0 + a_lo16 + ks * 2 * plane16, b0 + ks * 4 * N, idesc, 1);
-                    }
+        return;
+    }
+
+    // ================= two warpgroups: rows [64 wg, 64 wg + 64) of every tile =================
+    const int wg = warp >> 2;
+    const uint32_t plane16 = (uint32_t)(g.plane >> 4);
+    const uint64_t a_desc0 = make_desc(smem_u32(in_s), plane16, 8);
+    const uint64_t b_desc0 = make_desc(smem_u32(ring), 2 * N, 8);        // tap block [kg][N hi rows | N lo rows][16 B]: LBO = 2N rows
+    const uint32_t b_lo16 = (uint32_t)N;                                  // the lo rows of a k-group, in 16-byte units
+    const uint32_t a_lo16 = (uint32_t)(g.part >> 4);
+    const int nks = kg_in / 2;
+    const int yend = min(y0 + p.band_h, H);
+    const int qc = 2 * (lane & 3);                                        // first of the thread's two columns in each 8-column group
+    mbar_wait(&bars->in_full, 0);
+    for (int t = 0; t < g.NT; ++t) {
+        float acc[N / 2];
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) acc[i] = 0.0f;
+        for (int tap = 0; tap < 9; ++tap) {
+            const int n = t * 9 + tap, st = n % nstages;
+            mbar_wait(&bars->full[st], (n / nstages) & 1);
+            const uint64_t b0 = b_desc0 + (uint64_t)((st * g.tap_bytes) >> 4);
+            const uint64_t a0 = a_desc0 + (uint64_t)((p.tap_phase[tap] * g.phase) >> 4) + (uint64_t)(g.m_lo + p.tap_shift[tap] + t * 128 + wg * 64);
+            wg_fence();
+            for (int ks = 0; ks < nks; ++ks) {
+                wgmma_f16<N>(acc, a0 + ks * 2 * plane16, b0 + ks * 4 * N);
+                if (npass == 3) {
+                    wgmma_f16<N>(acc, a0 + ks * 2 * plane16, b0 + b_lo16 + ks * 4 * N);
+                    wgmma_f16<N>(acc, a0 + a_lo16 + ks * 2 * plane16, b0 + ks * 4 * N);
                 }
-                LZ_UCOMMIT(&bars->empty[st]);
             }
-            LZ_UCOMMIT(&bars->acc_ready);
-            if (dbg && lane == 0) dbg[60] = clock64();
+            wg_commit();
+            if (tap > 0) {
+                wg_wait<1>();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&bars->empty[(n - 1) % nstages]);
+            }
         }
-    } else {
-        // ================= epilogue: TMEM -> BN (+residual) (+ReLU) -> fp16 hi/lo -> next layer's TCL =================
-        const int q4 = warp & 3, half = warp >> 2, rowid = q4 * 32 + lane;
-        const uint32_t lane_base = tmem + ((uint32_t)(q4 * 32) << 16);
-        const int yend = min(y0 + p.band_h, H);
-        mbar_wait_warp(&bars->acc_ready, 0);
-        tc_fence_after();
-        if (dbg && tid == 0) dbg[61] = clock64();
-        for (int t = 0; t < g.NT; ++t) {
-            const int m = g.m_lo + t * 128 + rowid;
+        wg_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars->empty[(t * 9 + 8) % nstages]);
+
+        // ================= epilogue from the fragment: BN (+residual) (+ReLU) -> fp16 hi/lo -> next layer's TCL =================
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            const int m = g.m_lo + t * 128 + wg * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
             const int k = m / g.rin;
             const int rho = rin0 + (m - k * g.rin);
             const int yy = rho / pitch - 1, xx = rho - (yy + 1) * pitch;
             const bool in_band = (k < nimg) && (rho >= pitch) && (yy >= y0) && (yy < yend);
             const bool valid = in_band && (xx < W);
-            {
-                const int grp = (N == 128) ? half : 0;               // N = 128: one output tensor per warp half; else one half of the columns
+#pragma unroll
+            for (int j = 0; j < N / 8; ++j) {
+                const int col = 8 * j + qc;
+                const int grp = (N == 128) ? (col >> 6) : 0;      // N = 128: columns [64, 128) are the second output tensor
+                const int c = col - grp * 64;                     // channel within the output tensor
                 const Tcl &o = p.out[grp];
                 const bool relu = p.relu[grp] != 0;
                 size_t obase = 0;
@@ -203,66 +178,24 @@ __global__ void __launch_bounds__(kCvThreads, 2) k_conv_tc(ConvTc p)
                         do_write = false;
                     }
                 }
-                constexpr int NCW = (N == 128) ? 64 : N / 2;     // columns this warp handles: [cbase, cbase + NCW) of the output tensor
-                const int cbase = (N == 128) ? 0 : half * NCW;
-#pragma unroll
-                for (int cc = 0; cc < NCW; cc += 16) {
-                    float v[16];
-                    const int c0 = cbase + cc;
-                    const int col = grp * 64 + c0;
-                    // residual operand (TCL hi / lo of the 16 columns): issued BEFORE the TMEM loads so that its L2 / HBM latency overlaps them
-                    const bool has_res = p.res.base && grp == 0 && valid;
-                    uint4 rh[2], rl[2];
-                    if (has_res) {
-#pragma unroll
-                        for (int g2 = 0; g2 < 2; ++g2) {
-                            const unsigned char *rp = p.res.base + (size_t)(img0 + k) * p.res.img_stride +
-                                                      ((size_t)(c0 / 8 + g2) * p.res.plane_rows + rho + 1) * 16;
-                            rh[g2] = __ldg(reinterpret_cast<const uint4 *>(rp));
-                            rl[g2] = __ldg(reinterpret_cast<const uint4 *>(rp + p.res.part_stride));
-                        }
-                    }
-                    tmem_ld16(lane_base + t * NA + col, v);
-                    if (kFold && npass == 3) {          // the A_hi x B_lo half of the folded accumulator
-                        float v2[16];
-                        tmem_ld16(lane_base + t * NA + N + col, v2);
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) v[i] += v2[i];
-                    }
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) v[i] = fmaf(v[i], __ldg(p.scale + col + i), __ldg(p.shift + col + i));
-                    if (has_res) {
-#pragma unroll
-                        for (int g2 = 0; g2 < 2; ++g2) {
-                            const __half2 *hh = reinterpret_cast<const __half2 *>(&rh[g2]), *hl = reinterpret_cast<const __half2 *>(&rl[g2]);
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                const float2 a = __half22float2(hh[j]), b = __half22float2(hl[j]);
-                                v[g2 * 8 + 2 * j] += a.x + b.x;
-                                v[g2 * 8 + 2 * j + 1] += a.y + b.y;
-                            }
-                        }
-                    }
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) v[i] = valid ? (relu ? fmaxf(v[i], 0.0f) : v[i]) : 0.0f;
-                    if (do_write) {
-#pragma unroll
-                        for (int g2 = 0; g2 < 2; ++g2) {
-                            const int kgi = c0 / 8 + g2;
-                            unsigned char *op = o.base + obase + (size_t)kgi * o.plane_rows * 16;
-                            store_split8(op, op + o.part_stride, v + 8 * g2);
-                        }
-                    }
+                float v0 = fmaf(acc[4 * j + 2 * hr], __ldg(p.scale + col), __ldg(p.shift + col));
+                float v1 = fmaf(acc[4 * j + 2 * hr + 1], __ldg(p.scale + col + 1), __ldg(p.shift + col + 1));
+                if (p.res.base && grp == 0 && valid) {
+                    const unsigned char *rp = p.res.base + (size_t)(img0 + k) * p.res.img_stride +
+                                              ((size_t)(c >> 3) * p.res.plane_rows + rho + 1) * 16 + (c & 7) * 2;
+                    const float2 a = __half22float2(*reinterpret_cast<const __half2 *>(rp));
+                    const float2 b = __half22float2(*reinterpret_cast<const __half2 *>(rp + p.res.part_stride));
+                    v0 += a.x + b.x;
+                    v1 += a.y + b.y;
+                }
+                v0 = valid ? (relu ? fmaxf(v0, 0.0f) : v0) : 0.0f;
+                v1 = valid ? (relu ? fmaxf(v1, 0.0f) : v1) : 0.0f;
+                if (do_write) {
+                    unsigned char *op = o.base + obase + (size_t)(c >> 3) * o.plane_rows * 16 + (c & 7) * 2;
+                    store_split2(op, op + o.part_stride, v0, v1);
                 }
             }
         }
-    }
-    if (dbg && tid == 0) { dbg[62] = clock64(); dbg[63] = ((unsigned long long)g.NT << 32) | (unsigned)gridDim.x; }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kCvEpiWarps + 1) {
-        __syncwarp();
-        tmem_dealloc(tmem, tmem_cols);
     }
 }
 
@@ -322,40 +255,23 @@ __global__ void k_pool_tcl(Tcl in, Tcl out, float *out_nchw, int B, int Hout)
 int conv_tc_prepare_launch()
 {
     const int big = 227 * 1024;
-    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
-    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
-    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
-    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
-    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
+    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
+    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
+    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
     return LZ_OK;
 }
 
-unsigned long long *tc_debug_buffer();     // net_tc.cu (env LZ_TC_DEBUG at model finalize time)
-
-int conv_tc_launch(const ConvTc &p_in, cudaStream_t s)
+int conv_tc_launch(const ConvTc &p, cudaStream_t s)
 {
-    ConvTc p = p_in;
-    p.dbg = nullptr;
-    if (const char *e = getenv("LZ_CONV_DEBUG")) {          // bring-up only: stamps of the e-th conv_tc launch of every group of 8 (one tower)
-        static int launch_idx = 0;
-        if (tc_debug_buffer() && (launch_idx++ % 8) == atoi(e)) p.dbg = tc_debug_buffer();
-    }
     const CvGeom g = cv_geom(p);
     LZ_REQUIRE(g.smem <= 227 * 1024, LZ_EINVAL, "conv_tc: band needs %zu B shared memory", g.smem);
-    LZ_REQUIRE(g.NT * conv_tc_acc_cols(p) <= 512, LZ_EINVAL, "conv_tc: %d tiles x %d columns exceed TMEM", g.NT, conv_tc_acc_cols(p));
     LZ_REQUIRE(g.tap_bytes <= 16384 && (p.in.C % 16) == 0, LZ_EINVAL, "conv_tc: unsupported channel counts");
     const int groups = (p.B + p.G - 1) / p.G;
     const int grid = groups * g.nbands;
     switch (p.N) {
-        case 32:
-            if (p.fold) k_conv_tc<32, true><<<grid, kCvThreads, g.smem, s>>>(p);
-            else k_conv_tc<32, false><<<grid, kCvThreads, g.smem, s>>>(p);
-            break;
-        case 64:
-            if (p.fold) k_conv_tc<64, true><<<grid, kCvThreads, g.smem, s>>>(p);
-            else k_conv_tc<64, false><<<grid, kCvThreads, g.smem, s>>>(p);
-            break;
-        case 128: k_conv_tc<128, false><<<grid, kCvThreads, g.smem, s>>>(p); break;
+        case 32: k_conv_tc<32><<<grid, kCvThreads, g.smem, s>>>(p); break;
+        case 64: k_conv_tc<64><<<grid, kCvThreads, g.smem, s>>>(p); break;
+        case 128: k_conv_tc<128><<<grid, kCvThreads, g.smem, s>>>(p); break;
         default: LZ_REQUIRE(false, LZ_EINVAL, "conv_tc: N must be 32, 64 or 128");
     }
     LZ_KERNEL_CHECK();
@@ -390,7 +306,7 @@ float conv_tc_pack(const float *w, int cin, int cout, int ncols, int col0, unsig
 int pool_tcl_launch(const Tcl &in, const Tcl &out, int B, cudaStream_t s)
 {
     const size_t n = (size_t)B * (in.C / 8) * out.H * out.W;
-    k_pool_tcl<<<(int)std::min<size_t>((n + 255) / 256, 148 * 32), 256, 0, s>>>(in, out, nullptr, B, out.H);
+    k_pool_tcl<<<(int)std::min<size_t>((n + 255) / 256, kNumSMs * 32), 256, 0, s>>>(in, out, nullptr, B, out.H);
     LZ_KERNEL_CHECK();
     return LZ_OK;
 }
@@ -399,7 +315,7 @@ int pool_tcl_to_nchw_launch(const Tcl &in, float *out, int B, int Hout, cudaStre
 {
     const size_t n = (size_t)B * (in.C / 8) * Hout * Hout;
     Tcl dummy = in;
-    k_pool_tcl<<<(int)std::min<size_t>((n + 255) / 256, 148 * 32), 256, 0, s>>>(in, dummy, out, B, Hout);
+    k_pool_tcl<<<(int)std::min<size_t>((n + 255) / 256, kNumSMs * 32), 256, 0, s>>>(in, dummy, out, B, Hout);
     LZ_KERNEL_CHECK();
     return LZ_OK;
 }

@@ -1,4 +1,4 @@
-// conv_tc.cuh -- tcgen05 3x3 convolutions of the DownSample tower (representation network).
+// conv_tc.cuh -- wgmma 3x3 convolutions of the DownSample tower (representation network).
 //
 // Activations between tower layers live in HBM in a tensor-core-ready layout ("TCL"): per image
 //   [part: fp16 hi | fp16 lo][k-group of 8 channels][row][8 halves]
@@ -6,7 +6,7 @@
 //   rho = (y + 1) * pitch + x,   memory row = rho + 1   (one spare zero row at each end),
 //   rows per plane R = (H + 2) * pitch + 2.
 // A band of image rows is then a handful of contiguous cp.async.bulk copies per plane, lands in shared
-// memory already in the UMMA K-major / no-swizzle canonical layout, and every 3x3 tap is the same buffer
+// memory already in the wgmma K-major / no-swizzle canonical layout, and every 3x3 tap is the same buffer
 // read through a row-shifted descriptor (see net_tc.cu).  Stride-2 convolutions read a 4-phase
 // (space-to-depth) variant written by the producing layer: phase (y&1, x&1) image of half size, so that
 // tap (ky,kx) is phase ((ky+1)&1, (kx+1)&1) shifted by (ky==0 ? -1 : 0, kx==0 ? -1 : 0).
@@ -49,15 +49,11 @@ struct ConvTc {
     int N;                        // 32, 64 or 128
     int G, band_h;                // images per CTA (band_h == H when G > 1), image rows per band
     int stages;                   // weight ring depth (2..4)
-    int fold;                     // fp32-accurate mode: A_hi x [B_hi | B_lo] as ONE 2N-column MMA (N <= 64; 2N accumulator columns per tile)
     int B, npass;
-    unsigned long long *dbg;      // bring-up instrumentation (env LZ_CONV_DEBUG=<layer>): clock64 stamps of the middle CTA, slots 58-63 of the debug buffer
 };
 
 int conv_tc_prepare_launch();
 int conv_tc_launch(const ConvTc &p, cudaStream_t s);
-// TMEM accumulator columns per 128-row tile: layers with N <= 64 output columns fold [B_hi | B_lo] into one 2N-column MMA (conv_tc.cu)
-inline int conv_tc_acc_cols(const ConvTc &p) { return (p.fold && p.N <= 64) ? 2 * p.N : p.N; }
 // weights [cout][cin][3][3] -> tap blocks with `ncols` columns, this tensor occupying columns
 // [col0, col0+cout); returns the exact power-of-two scale applied
 float conv_tc_pack(const float *w_torch, int cin, int cout, int ncols, int col0, unsigned char *dst);

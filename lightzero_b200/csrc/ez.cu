@@ -1,4 +1,4 @@
-// ez.cu -- EfficientZero value-prefix head for sm_100a: LSTM step + BatchNorm1d/ReLU/MLP/categorical expectation.
+// ez.cu -- EfficientZero value-prefix head for sm_90a: LSTM step + BatchNorm1d/ReLU/MLP/categorical expectation.
 //
 // k_ez_lstm: gates[B][4H] = [feat | h_in] (B x (nin+H)) * wcat ((nin+H) x 4H) + bias as a tiled fp32 GEMM over ALL roots
 // (the weights, 8.9 MB at nin = 576 / H = 512, are read once per 64-row tile instead of once per root), with the LSTM cell
@@ -15,20 +15,6 @@
 #include "ez.cuh"
 #include "lz_common.cuh"
 #include "tc_ptx.cuh"
-
-// The MMAs are issued from uniform control flow: the whole issuing warp runs the loop and elect.sync picks the lane
-// (48.6 cycles per N = 64 MMA, the shared-memory operand floor, against 60-78 from an `if (lane == 0)` branch, where ptxas
-// wraps every UTCHMMA in an ELECT / BRA.U.ANY loop: profiles/r01e_mma_probe.md; validated on hardware in round 2).
-// -DLZ_LANE0_ISSUE restores the round-1 single-lane branch for A/B measurements.
-#ifndef LZ_LANE0_ISSUE
-#define LZ_MMA_ISSUER_ON true
-#define LZ_UMMA umma_f16_elect
-#define LZ_UCOMMIT umma_commit_elect
-#else
-#define LZ_MMA_ISSUER_ON (lane == 0)
-#define LZ_UMMA umma_f16
-#define LZ_UCOMMIT umma_commit
-#endif
 
 namespace lz {
 
@@ -177,46 +163,38 @@ __global__ void __launch_bounds__(256) k_ez_head(EzNet net, EzIO io)
     }
 }
 
-// ---------------------------------------------------------------------------------------------- tcgen05 LSTM step
-// gates = [feat | h] * W as a tcgen05 GEMM with fp32 accuracy ("3xFP16": A_hi*W_hi + A_hi*W_lo + A_lo*W_hi, fp32
-// accumulation in TMEM).  CTA tile: 128 roots x 64 gate columns (16 hidden units), K = nin + H in chunks of 64 through a
-// 3-stage ring.  Warps 0-3: gather the fp32 A rows (features, then the leaf parent's h through ix), split them to fp16
-// hi / lo into the UMMA K-major layout [k-group][row][8 halves] -- then become the epilogue (tcgen05.ld, LSTM cell update,
-// reset).  Warp 4 lane 0: bulk-copies the pre-split weight chunks.  Warp 5 lane 0: MMA issue (+ TMEM alloc by warp 5).
+// ---------------------------------------------------------------------------------------------- wgmma LSTM step
+// gates = [feat | h] * W as a wgmma GEMM with fp32 accuracy ("3xFP16": A_hi*W_hi + A_hi*W_lo + A_lo*W_hi, fp32 accumulation in
+// registers).  CTA tile: 128 roots x 64 gate columns (16 hidden units), K = nin + H in chunks of 64 through a 3-stage ring.  Two
+// warpgroups: each gathers the fp32 A rows of every other chunk (features, then the leaf parent's h through ix), splits them to fp16
+// hi / lo into the wgmma K-major layout [k-group][row][8 halves], issues the MMAs of its 64 rows of every chunk and runs the
+// epilogue (LSTM cell update, reset) from its accumulators.  Warp 8 lane 0 bulk-copies the pre-split weight chunks.
 constexpr int kTM = 128, kTN = 64, kTK = 64, kTStages = 3;
 constexpr int kTAPart = 8 * kTM * 16;            // one hi or lo part of an A stage: [8 k-groups][128 rows][16 B] = 16 KB
 constexpr int kTWPart = 8 * kTN * 16;            // one hi or lo part of a W stage: 8 KB
 constexpr int kTStageBytes = 2 * kTAPart + 2 * kTWPart;     // 48 KB
 constexpr int kTSmem = kTStages * kTStageBytes + 256;
-constexpr int kTGroups = 3;                      // A-producer groups of 128 threads; group g converts chunks g, g+3, ... (3 chunks of L2 latency in flight)
-constexpr int kTThreads = 192 + (kTGroups - 1) * 128;
+constexpr int kTThreads = 256 + 32;
 
 struct EzTcBars {
     uint64_t full_a[kTStages], full_w[kTStages], empty[kTStages];
-    uint64_t acc_ready;
-    uint32_t tmem_base, pad;
 };
 
 __global__ void __launch_bounds__(kTThreads, 1) k_ez_lstm_tc(EzNet net, EzIO io)
 {
     extern __shared__ __align__(1024) unsigned char smem[];
     EzTcBars *bars = reinterpret_cast<EzTcBars *>(smem + kTStages * kTStageBytes);
-    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;   // warp-uniform value: uniform role branches (see net_tc.cu)
+    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;   // warp-uniform value: uniform role branches
     const int nt = blockIdx.x, m0 = blockIdx.y * kTM;
     const int H = net.H, nin = net.nin, KT = nin + H, nchunks = KT / kTK;
 
     if (tid == 0) {
-        for (int i = 0; i < kTStages; ++i) { mbar_init(&bars->full_a[i], 128); mbar_init(&bars->full_w[i], 1); mbar_init(&bars->empty[i], 1); }
-        mbar_init(&bars->acc_ready, 1);
+        for (int i = 0; i < kTStages; ++i) { mbar_init(&bars->full_a[i], 128); mbar_init(&bars->full_w[i], 1); mbar_init(&bars->empty[i], 8); }
         fence_mbar_init();
     }
-    if (warp == 5) tmem_alloc(&bars->tmem_base, 64);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = __shfl_sync(0xffffffffu, bars->tmem_base, 0);
 
-    if (warp == 4) {
+    if (warp == 8) {
         if (lane == 0) {
             const unsigned char *src = net.wtc + (size_t)nt * nchunks * (2 * kTWPart);
             for (int c = 0; c < nchunks; ++c) {
@@ -227,114 +205,105 @@ __global__ void __launch_bounds__(kTThreads, 1) k_ez_lstm_tc(EzNet net, EzIO io)
                 bulk_g2s(smem + st * kTStageBytes + 2 * kTAPart, src + (size_t)c * (2 * kTWPart), 2 * kTWPart, &bars->full_w[st]);
             }
         }
-    } else if (warp == 5) {
-        if (LZ_MMA_ISSUER_ON) {
-            const uint32_t idesc = make_idesc_f16(kTM, kTN);
-            for (int c = 0; c < nchunks; ++c) {
-                const int st = c % kTStages;
-                mbar_wait(&bars->full_a[st], (c / kTStages) & 1);
-                mbar_wait(&bars->full_w[st], (c / kTStages) & 1);
-                tc_fence_after();
-                const uint32_t a_s = smem_u32(smem + st * kTStageBytes), w_s = a_s + 2 * kTAPart;
-                const uint64_t a_hi = make_desc(a_s, (kTM * 16) >> 4, 8), a_lo = make_desc(a_s + kTAPart, (kTM * 16) >> 4, 8);
-                const uint64_t w_hi = make_desc(w_s, (kTN * 16) >> 4, 8), w_lo = make_desc(w_s + kTWPart, (kTN * 16) >> 4, 8);
+        return;
+    }
+    // ---- A production: warpgroup grp converts chunks grp, grp + 2, ...  Per pass a warp covers 8 rows x 8 k-groups: lane -> (row =
+    // lane % 8, k-groups lane / 8 and lane / 8 + 4), so one load instruction touches 8 lines (one per row) instead of 32 and each
+    // quarter-warp stores 8 consecutive rows of one k-group plane (conflict-free).
+    const int grp = warp >> 2, tg = tid & 127;
+    const int pw = tg >> 5, pl = tg & 31, prow0 = pw * 8 + (pl & 7), pkg = pl >> 3;
+    const float *fsrc[4], *hsrc[4];
+    bool pon[4];
 #pragma unroll
-                for (int ks = 0; ks < kTK / 16; ++ks) {
-                    const uint64_t ao = (uint64_t)(ks * 2 * kTM * 16 >> 4), wo = (uint64_t)(ks * 2 * kTN * 16 >> 4);
-                    LZ_UMMA(tmem, a_hi + ao, w_hi + wo, idesc, (c | ks) != 0);
-                    LZ_UMMA(tmem, a_hi + ao, w_lo + wo, idesc, 1);
-                    LZ_UMMA(tmem, a_lo + ao, w_hi + wo, idesc, 1);
-                }
-                LZ_UCOMMIT(&bars->empty[st]);
-            }
-            LZ_UCOMMIT(&bars->acc_ready);
-        }
-    } else {
-        // ---- A producers (warps 0-3 group 0, warps 6-9 group 1, warps 10-13 group 2).  Per pass a warp covers 8 rows x 8
-        // k-groups: lane -> (row = lane % 8, k-groups lane / 8 and lane / 8 + 4), so one load instruction touches 8 lines (one
-        // per row) instead of 32 and each quarter-warp stores 8 consecutive rows of one k-group plane (conflict-free).
-        const int grp = warp < 4 ? 0 : (warp - 6) / 4 + 1;
-        const int tg = warp < 4 ? tid : (tid - 192) & 127;
-        const int pw = tg >> 5, pl = tg & 31, prow0 = pw * 8 + (pl & 7), pkg = pl >> 3;
-        const float *fsrc[4], *hsrc[4];
-        bool pon[4];
+    for (int ps = 0; ps < 4; ++ps) {
+        const int bb = m0 + ps * 32 + prow0;
+        pon[ps] = bb < io.B;
+        fsrc[ps] = io.feat + (size_t)(pon[ps] ? bb : 0) * nin;
+        hsrc[ps] = io.h_base + (pon[ps] && io.ix ? (size_t)io.ix[bb] * io.slot_stride : 0) + (size_t)(pon[ps] ? bb : 0) * H;
+    }
+    auto produce = [&](int c) {
+        const int st = c % kTStages;
+        const int k0 = c * kTK;                                             // nin is a multiple of 64: a chunk never straddles feat | h
+        float4 v[16];
 #pragma unroll
         for (int ps = 0; ps < 4; ++ps) {
-            const int bb = m0 + ps * 32 + prow0;
-            pon[ps] = bb < io.B;
-            fsrc[ps] = io.feat + (size_t)(pon[ps] ? bb : 0) * nin;
-            hsrc[ps] = io.h_base + (pon[ps] && io.ix ? (size_t)io.ix[bb] * io.slot_stride : 0) + (size_t)(pon[ps] ? bb : 0) * H;
+            const float *src = (k0 < nin ? fsrc[ps] + k0 : hsrc[ps] + (k0 - nin)) + pkg * 8;
+#pragma unroll
+            for (int u = 0; u < 4; ++u)      // u: 0,1 = k-group pkg, 2,3 = k-group pkg + 4
+                v[ps * 4 + u] = (pon[ps] && !(io.dbg & 1)) ? *reinterpret_cast<const float4 *>(src + (u >> 1) * 32 + (u & 1) * 4) : make_float4(0, 0, 0, 0);
         }
-        for (int c = grp; c < nchunks; c += kTGroups) {
-            const int st = c % kTStages;
-            const int k0 = c * kTK;                                             // nin is a multiple of 64: a chunk never straddles feat | h
-            float4 v[16];
+        if (c >= kTStages) mbar_wait(&bars->empty[st], ((c / kTStages) - 1) & 1);
 #pragma unroll
-            for (int ps = 0; ps < 4; ++ps) {
-                const float *src = (k0 < nin ? fsrc[ps] + k0 : hsrc[ps] + (k0 - nin)) + pkg * 8;
+        for (int ps = 0; ps < 4; ++ps) {
+            unsigned char *a_hi = smem + st * kTStageBytes + (ps * 32 + prow0) * 16;
 #pragma unroll
-                for (int u = 0; u < 4; ++u)      // u: 0,1 = k-group pkg, 2,3 = k-group pkg + 4
-                    v[ps * 4 + u] = (pon[ps] && !(io.dbg & 1)) ? *reinterpret_cast<const float4 *>(src + (u >> 1) * 32 + (u & 1) * 4) : make_float4(0, 0, 0, 0);
-            }
-            if (c >= kTStages) mbar_wait(&bars->empty[st], ((c / kTStages) - 1) & 1);
-#pragma unroll
-            for (int ps = 0; ps < 4; ++ps) {
-                unsigned char *a_hi = smem + st * kTStageBytes + (ps * 32 + prow0) * 16;
-#pragma unroll
-                for (int h2 = 0; h2 < 2; ++h2) {
-                    const float4 x = v[ps * 4 + 2 * h2], y = v[ps * 4 + 2 * h2 + 1];
-                    const float f[8] = {x.x, x.y, x.z, x.w, y.x, y.y, y.z, y.w};
-                    const int kg = pkg + 4 * h2;
-                    store_split8(a_hi + kg * (kTM * 16), a_hi + kTAPart + kg * (kTM * 16), f);
-                }
-            }
-            fence_proxy_async();
-            mbar_arrive(&bars->full_a[st]);
-        }
-        // ---- epilogue, all three groups: warp w may read TMEM lanes 32 * (w % 4) .. +31 = rows of the tile; the 64 accumulator
-        // columns (16 hidden units x (i, f, g, o)) are dealt out in chunks of 16: group 0 takes chunks 0 and 3, groups 1 / 2
-        // chunks 1 / 2.  (A single group doing all 16 units per thread cost 10 us: one warp per scheduler, five
-        // transcendentals per unit.)  sigmoid / tanh through __expf + __fdividef: abs error ~1e-6 on values in (-1, 1).
-        {
-            const int row = (warp & 3) * 32 + lane, b = m0 + row;
-            const bool on = b < io.B;
-            const size_t hoff = (on && io.ix ? (size_t)io.ix[b] * io.slot_stride : 0) + (size_t)(on ? b : 0) * H;
-            mbar_wait_warp(&bars->acc_ready, 0);
-            tc_fence_after();
-            const uint32_t lane_base = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-            const float inv = net.wtc_inv_scale;
-            const float *c_in = io.c_base + hoff;
-            const bool reset = on && io.is_reset && io.is_reset[b] != 0;
-            for (int chunk = grp; chunk < 4; chunk += 3) {
-                float g[16];
-                tmem_ld16(lane_base + chunk * 16, g);
-                if (!on || (io.dbg & 4)) continue;
-                const int u0 = nt * 16 + chunk * 4;
-                const float4 cin4 = *reinterpret_cast<const float4 *>(c_in + u0);
-                const float cin[4] = {cin4.x, cin4.y, cin4.z, cin4.w};
-                float hn[4], cn[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const float4 bias = *reinterpret_cast<const float4 *>(net.bias + (size_t)(u0 + u) * 4);
-                    const float gi = fmaf(g[4 * u], inv, bias.x), gf = fmaf(g[4 * u + 1], inv, bias.y);
-                    const float gg = fmaf(g[4 * u + 2], inv, bias.z), go = fmaf(g[4 * u + 3], inv, bias.w);
-                    const float si = __fdividef(1.0f, 1.0f + __expf(-gi)), sf = __fdividef(1.0f, 1.0f + __expf(-gf));
-                    const float so = __fdividef(1.0f, 1.0f + __expf(-go));
-                    const float tg_ = 1.0f - __fdividef(2.0f, __expf(2.0f * gg) + 1.0f);
-                    cn[u] = sf * cin[u] + si * tg_;
-                    hn[u] = so * (1.0f - __fdividef(2.0f, __expf(2.0f * cn[u]) + 1.0f));
-                }
-                *reinterpret_cast<float4 *>(io.h_tmp + (size_t)b * H + u0) = make_float4(hn[0], hn[1], hn[2], hn[3]);
-                if (io.h_out) *reinterpret_cast<float4 *>(io.h_out + (size_t)b * H + u0) = reset ? make_float4(0, 0, 0, 0) : make_float4(hn[0], hn[1], hn[2], hn[3]);
-                if (io.c_out) *reinterpret_cast<float4 *>(io.c_out + (size_t)b * H + u0) = reset ? make_float4(0, 0, 0, 0) : make_float4(cn[0], cn[1], cn[2], cn[3]);
+            for (int h2 = 0; h2 < 2; ++h2) {
+                const float4 x = v[ps * 4 + 2 * h2], y = v[ps * 4 + 2 * h2 + 1];
+                const float f[8] = {x.x, x.y, x.z, x.w, y.x, y.y, y.z, y.w};
+                const int kg = pkg + 4 * h2;
+                store_split8(a_hi + kg * (kTM * 16), a_hi + kTAPart + kg * (kTM * 16), f);
             }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 5) {
+        fence_proxy_async();
+        mbar_arrive(&bars->full_a[st]);
+    };
+    for (int c = grp; c < kTStages && c < nchunks; c += 2) produce(c);
+    // ---- MMAs of this warpgroup's 64 rows; a chunk's slot is refilled (A by its producing warpgroup) once both have read it
+    float acc[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[i] = 0.0f;
+    for (int c = 0; c < nchunks; ++c) {
+        const int st = c % kTStages;
+        mbar_wait(&bars->full_a[st], (c / kTStages) & 1);
+        mbar_wait(&bars->full_w[st], (c / kTStages) & 1);
+        const uint32_t a_s = smem_u32(smem + st * kTStageBytes) + grp * 64 * 16, w_s = smem_u32(smem + st * kTStageBytes) + 2 * kTAPart;
+        const uint64_t a_hi = make_desc(a_s, (kTM * 16) >> 4, 8), a_lo = make_desc(a_s + kTAPart, (kTM * 16) >> 4, 8);
+        const uint64_t w_hi = make_desc(w_s, (kTN * 16) >> 4, 8), w_lo = make_desc(w_s + kTWPart, (kTN * 16) >> 4, 8);
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < kTK / 16; ++ks) {
+            const uint64_t ao = (uint64_t)(ks * 2 * kTM * 16 >> 4), wo = (uint64_t)(ks * 2 * kTN * 16 >> 4);
+            wgmma_n64(acc, a_hi + ao, w_hi + wo);
+            wgmma_n64(acc, a_hi + ao, w_lo + wo);
+            wgmma_n64(acc, a_lo + ao, w_hi + wo);
+        }
+        wg_commit();
+        wg_wait<0>();
         __syncwarp();
-        tmem_dealloc(tmem, 64);
+        if (lane == 0) mbar_arrive(&bars->empty[st]);
+        if (c + kTStages < nchunks && ((c + kTStages) & 1) == grp) produce(c + kTStages);
+    }
+    // ---- epilogue from the fragment: columns 8 j + 2 (lane % 4) + {0, 1} are gates (i, f) (even lane % 4) or (g, o) (odd) of hidden
+    // unit 2 j + (lane % 4) / 2; lane pairs swap one row's half so the even lane updates its first row, the odd lane its second.
+    // sigmoid / tanh through __expf + __fdividef: abs error ~1e-6 on values in (-1, 1).
+    {
+        const bool odd = (lane & 1) != 0;
+        const int row = grp * 64 + 16 * (warp & 3) + (lane >> 2) + (odd ? 8 : 0), b = m0 + row;
+        const bool on = b < io.B && !(io.dbg & 4);
+        const size_t hoff = (on && io.ix ? (size_t)io.ix[b] * io.slot_stride : 0) + (size_t)(on ? b : 0) * H;
+        const float inv = net.wtc_inv_scale;
+        const float *c_in = io.c_base + hoff;
+        const bool reset = on && io.is_reset && io.is_reset[b] != 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const float s0 = odd ? acc[4 * j] : acc[4 * j + 2], s1 = odd ? acc[4 * j + 1] : acc[4 * j + 3];
+            const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+            const float ai = odd ? r0 : acc[4 * j], af = odd ? r1 : acc[4 * j + 1];
+            const float ag = odd ? acc[4 * j + 2] : r0, ao = odd ? acc[4 * j + 3] : r1;
+            if (!on) continue;
+            const int u = nt * 16 + 2 * j + ((lane & 3) >> 1);
+            const float4 bias = *reinterpret_cast<const float4 *>(net.bias + (size_t)u * 4);
+            const float gi = fmaf(ai, inv, bias.x), gf = fmaf(af, inv, bias.y);
+            const float gg = fmaf(ag, inv, bias.z), go = fmaf(ao, inv, bias.w);
+            const float si = __fdividef(1.0f, 1.0f + __expf(-gi)), sf = __fdividef(1.0f, 1.0f + __expf(-gf));
+            const float so = __fdividef(1.0f, 1.0f + __expf(-go));
+            const float tg_ = 1.0f - __fdividef(2.0f, __expf(2.0f * gg) + 1.0f);
+            const float cn = sf * c_in[u] + si * tg_;
+            const float hn = so * (1.0f - __fdividef(2.0f, __expf(2.0f * cn) + 1.0f));
+            io.h_tmp[(size_t)b * H + u] = hn;
+            if (io.h_out) io.h_out[(size_t)b * H + u] = reset ? 0.0f : hn;
+            if (io.c_out) io.c_out[(size_t)b * H + u] = reset ? 0.0f : cn;
+        }
     }
 }
 

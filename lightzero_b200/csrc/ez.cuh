@@ -8,7 +8,7 @@ namespace lz {
 struct EzNet {
     const float *wcat;        // [nin + H][4H]: rows = inputs (reward features, then h_in), columns n = unit * 4 + gate (i, f, g, o)
     const float *bias;        // [4H] same column order: bias_ih + bias_hh
-    const unsigned char *wtc; // tcgen05 path: [n-tile 32][k-chunk 17][hi 8 KB | lo 8 KB], each [k-group 8][n 64][8 halves] fp16, scaled by wtc_scale
+    const unsigned char *wtc; // tensor-core path: [n-tile 32][k-chunk 17][hi 8 KB | lo 8 KB], each [k-group 8][n 64][8 halves] fp16, scaled by wtc_scale
     float wtc_inv_scale;      // 1 / (power-of-two scale applied to wtc)
     const float *vp_s, *vp_t; // norm_value_prefix folded: y = relu(h' * s + t)
     const float *fc1;         // [H][hid] input-major
@@ -33,9 +33,9 @@ struct EzIO {
     int dbg;                  // timing experiments (env LZ_EZ_DBG; wrong results): 1 = no A loads, 2 = no weight copies, 4 = no cell update
 };
 
-int ez_launch(const EzNet &net, const EzIO &io, cudaStream_t s, int math);   // math 0: fp32 FFMA GEMM, else tcgen05 3xFP16
+int ez_launch(const EzNet &net, const EzIO &io, cudaStream_t s, int math);   // math 0: fp32 FFMA GEMM, else tensor-core (wgmma) 3xFP16
 int ez_prepare_launch();
-// host: pack W ([4H][nin] and [4H][H], torch gate order) into the tcgen05 layout; returns the scale applied
+// host: pack W ([4H][nin] and [4H][H], torch gate order) into the tensor-core layout; returns the scale applied
 size_t ez_wtc_bytes(int nin, int H);
 float ez_pack_wtc(const float *w_ih, const float *w_hh, int nin, int H, unsigned char *dst);
 

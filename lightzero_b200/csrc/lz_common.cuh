@@ -49,4 +49,6 @@ inline int dev_alloc(T **p, size_t n)
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+constexpr int kNumSMs = 132;       // streaming multiprocessors of the H100 SXM the grid sizes are tuned for
+
 }  // namespace lz

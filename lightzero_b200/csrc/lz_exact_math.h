@@ -8,7 +8,7 @@
 // rounded to float once.  That result is NOT always the correctly rounded exp (max error 0.502 ULP),
 // so neither CUDA's expf nor (float)exp((double)x) matches it on every input.  Restating the same
 // double-precision operation sequence does: IEEE double add/mul/fma are exact-rounded on both x86
-// and sm_100, so the device reproduces the host bit pattern.  tests/test_exact_math.py checks this
+// and sm_90, so the device reproduces the host bit pattern.  tests/test_exact_math.py checks this
 // restatement against libm expf for EVERY float in [-104, +0] (1.12e9 inputs) on the host.
 //
 // Published algorithm restated: glibc 2.39 sysdeps/ieee754/flt-32/e_expf.c + e_exp2f_data.c

@@ -268,7 +268,7 @@ k_conv3x3_generic(ConvG L, const float *__restrict__ in, float *__restrict__ out
 
 // ------------------------------------------------------------------------------------------------
 // The stem of the DownSample tower for 4 input channels (DownSample.conv1 + norm1 + ReLU, common.py:334-366; 3x3, stride 2,
-// pad 1, 4 -> 32 channels) on the CUDA cores, written straight into the tensor-core layout (TCL) of the first tcgen05 layer.
+// pad 1, 4 -> 32 channels) on the CUDA cores, written straight into the tensor-core layout (TCL) of the first wgmma layer.
 // K = 36 is too thin for the tensor cores; the kernel is FFMA-bound by construction: the 1,152 weights and the folded BatchNorm
 // tables travel BY VALUE in the kernel parameters, so every FFMA takes its weight operand from the constant bank (no weight
 // loads at all) and the only shared-memory traffic is one activation load per 32 FFMAs.  CTA = rows_per_cta full output rows
@@ -369,7 +369,7 @@ __global__ void k_inverse_scalar(const float *logits, float *out, int B, int K, 
 // ------------------------------------------------------------------------------------------------
 static int pick_W(int B)
 {
-    // largest roots-per-CTA that still yields ~one CTA per SM (148 SMs); small batches use small CTAs
+    // largest roots-per-CTA that still yields ~one CTA per SM; small batches use small CTAs
     if (B >= 8 * 120) return 8;
     if (B >= 4 * 120) return 4;
     if (B >= 2 * 120) return 2;
@@ -476,13 +476,13 @@ static int launch_convg(const ConvG &L, const float *in, float *out, const float
 static int launch_pool(const float *in, float *out, int planes, int hin, int hout, cudaStream_t s)
 {
     const size_t n = (size_t)planes * hout * hout;
-    int blocks = (int)std::min<size_t>((n + 255) / 256, 148 * 16);
+    int blocks = (int)std::min<size_t>((n + 255) / 256, kNumSMs * 16);
     k_avgpool3s2<<<blocks, 256, 0, s>>>(in, out, planes, hin, hin, hout, hout);
     LZ_KERNEL_CHECK();
     return LZ_OK;
 }
 
-// skip scratch of the tcgen05 latent-grid kernel (grown outside stream capture: API entry points and lz_search_create)
+// skip scratch of the tensor-core latent-grid kernel (grown outside stream capture: API entry points and lz_search_create)
 static int reserve_tc_skip(lz_model *m, int B)
 {
     if (m->kind != 0 || B <= m->tc_skip_B) return LZ_OK;
@@ -523,7 +523,7 @@ int model_reserve(lz_model *m, int B)
     }
     m->ws_floats = per_root * B;
     m->ws_B = B;
-    // TCL activation workspace of the tcgen05 tower (zeroed once: pad rows / columns are never written non-zero)
+    // TCL activation workspace of the tensor-core tower (zeroed once: pad rows / columns are never written non-zero)
     {
         const int h1 = m->tower[0].hout, h2 = m->tower[3].hout, h3 = (h2 - 1) / 2 + 1, c2 = kC / 2;
         const size_t bT = tcl_bytes(B, c2, h1, h1, 1), bT2 = tcl_bytes(B, c2, h1 / 2, h1 / 2, 4);
@@ -549,39 +549,32 @@ int model_reserve(lz_model *m, int B)
     return LZ_OK;
 }
 
-// ---- tcgen05 tower ---------------------------------------------------------------------------
-// picks the band height (and, for whole small images, the images per CTA) that fits shared memory / TMEM
-// and wastes the fewest MMA rows
+// ---- tensor-core (wgmma) tower ------------------------------------------------------------------
+// picks the band height (and, for whole small images, the images per CTA) that fits shared memory and wastes the fewest MMA rows
 static void pick_band(ConvTc &p)
 {
     const int H = p.in.H, pitch = p.in.pitch, kg = p.in.C / 8;
     double best = -1.0;
-    int best_h = 1, best_g = 1, best_st = 4, best_fold = 0;
-    // fold = A_hi x [B_hi | B_lo] as ONE 2N-column MMA (conv_tc.cu): 2 instead of 3 A-operand-bound MMAs per k-step, but 2N accumulator
-    // columns per tile.  Measured on B200: +8-10 % on the 42x42 / 21x21 layers even with smaller bands, -12 % on the 11x11 layers
-    // (fewer whole images per CTA), so it is not offered below 16 rows.
-    for (int fold = 0; fold <= ((p.N <= 64 && H >= 16) ? 1 : 0); ++fold)
-        for (int G = 1; G <= 4; ++G)
-            for (int bh = (G > 1 ? H : 1); bh <= H; ++bh)
-                for (int st = 2; st <= 4; st += 2) {
-                    const int NA = fold ? 2 * p.N : p.N;
-                    const int rin = (bh + 2) * pitch + 2, mcount = (G - 1) * rin + bh * pitch, NT = (mcount + 127) / 128;
-                    int PR = pitch + 1 + NT * 128 + pitch + 2;
-                    if (PR < G * rin) PR = G * rin;
-                    const size_t smem = (((size_t)PR * 16 * kg * 2 * p.in.nphase + 127) & ~(size_t)127) + st * (size_t)2 * kg * p.N * 16 + 1024;
-                    if (smem > 227 * 1024 || NT * NA > 512) continue;
-                    const int nb = (H + bh - 1) / bh;
-                    double score = (double)(G * H * (pitch - 1)) / ((double)nb * NT * 128);       // useful / issued MMA rows
-                    const bool two_ctas = smem <= 113 * 1024 && NT * NA <= 256;                // co-residency overlaps load / MMA / epilogue
-                    score *= two_ctas ? 1.35 : 1.0;
-                    score *= (st == 4) ? 1.0 : 0.97;
-                    score *= fold ? 1.12 : 1.0;
-                    if (score > best + 1e-9) { best = score; best_h = bh; best_g = G; best_st = st; best_fold = fold; }
-                }
+    int best_h = 1, best_g = 1, best_st = 4;
+    for (int G = 1; G <= 4; ++G)
+        for (int bh = (G > 1 ? H : 1); bh <= H; ++bh)
+            for (int st = 2; st <= 4; st += 2) {
+                const int rin = (bh + 2) * pitch + 2, mcount = (G - 1) * rin + bh * pitch, NT = (mcount + 127) / 128;
+                int PR = pitch + 1 + NT * 128 + pitch + 2;
+                if (PR < G * rin) PR = G * rin;
+                const size_t smem = (((size_t)PR * 16 * kg * 2 * p.in.nphase + 127) & ~(size_t)127) + st * (size_t)2 * kg * p.N * 16 + 1024;
+                if (smem > 227 * 1024) continue;
+                const int nb = (H + bh - 1) / bh;
+                double score = (double)(G * H * (pitch - 1)) / ((double)nb * NT * 128);       // useful / issued MMA rows
+                // two co-resident CTAs (N <= 64, see k_conv_tc) overlap one band's load / epilogue with the other's MMAs: initial_inference
+                // at B = 1024 took 4.0 ms with this preference and 4.5 ms without it (H100 SXM, 700 W)
+                if (p.N <= 64 && smem <= 113 * 1024) score *= 1.35;
+                score *= (st == 4) ? 1.0 : 0.97;
+                if (score > best + 1e-9) { best = score; best_h = bh; best_g = G; best_st = st; }
+            }
     p.band_h = best_h;
     p.G = best_g;
     p.stages = best_st;
-    p.fold = best_fold;
 }
 
 static int tower_tc_run(lz_model *m, int B, const float *d_obs, float *pre_latent, cudaStream_t s, const uint8_t *d_obs_u8 = nullptr)
@@ -618,7 +611,7 @@ static int tower_tc_run(lz_model *m, int B, const float *d_obs, float *pre_laten
     return pool_tcl_to_nchw_launch(m->V2, pre_latent, B, kHW, s);                    // pooling2 -> [B][64][6][6]
 }
 
-// tcgen05 path only: the DownSample tower alone (obs -> pre-latent [B][64][36]) ...
+// tensor-core path only: the DownSample tower alone (obs -> pre-latent [B][64][36]) ...
 int model_initial_tower(lz_model *m, int B, const float *d_obs, float *pre_latent, cudaStream_t s, const uint8_t *d_obs_u8)
 {
     LZ_REQUIRE(m->kind == 0 && m->math != 0 && m->cfg.obs_h != 64, LZ_ESTATE, "model_initial_tower: tensor-core conv model only");
@@ -778,7 +771,7 @@ static bool pack_head(lz_model *m, Packer &P, const std::string &conv, const std
     return true;
 }
 
-// ---- tcgen05 tower tables (conv_tc.cu) ----
+// ---- tensor-core tower tables (conv_tc.cu) ----
 static int pack_tower_tc(lz_model *m)
 {
     const std::string R = "representation_network.downsample_net.";
@@ -860,7 +853,7 @@ static int pack_tower_tc(lz_model *m)
     return conv_tc_prepare_launch();
 }
 
-// ---- tcgen05 tables (net_tc.cu): fp16 hi/lo weights, folded BN, action-bias planes, layer programs ----
+// ---- tensor-core tables (net_tc.cu): fp16 hi/lo weights, folded BN, action-bias planes, layer programs ----
 static int pack_tc(lz_model *m, const NetDev &net)
 {
     const lz_model_config &c = m->cfg;
@@ -944,7 +937,7 @@ static int pack_tc(lz_model *m, const NetDev &net)
         const Head &H = *fc_heads[h];
         if (H.hid <= 0) continue;
         const int nin = H.hc * kP;
-        LZ_REQUIRE(H.hid <= 32 && H.K <= 608 && nin <= 576, LZ_EINVAL, "lz_model_finalize: tcgen05 path needs head hidden <= 32, head channels <= 16 and support <= 608");
+        LZ_REQUIRE(H.hid <= 32 && H.K <= 608 && nin <= 576, LZ_EINVAL, "lz_model_finalize: tensor-core path needs head hidden <= 32, head channels <= 16 and support <= 608");
         auto W0 = find(m, fc_names[h] + ".0.weight", (size_t)H.hid * nin), W3 = find(m, fc_names[h] + ".3.weight", (size_t)H.K * H.hid);
         if (!W0 || !W3) return LZ_EINVAL;
         auto pow2_scale = [](const std::vector<float> &w) {
@@ -1060,7 +1053,7 @@ int lz_model_create(const lz_model_config *cfg, lz_model **out)
     m->hw = kHW; m->P = kP; m->K = K;
     m->ws[0] = m->ws[1] = m->ws[2] = nullptr;
     m->ws_floats = 0; m->ws_B = 0;
-    m->math = 1; m->d_tc = nullptr;   // default: tcgen05 3xFP16 (fp32-accurate)
+    m->math = 1; m->d_tc = nullptr;   // default: tensor-core 3xFP16 (fp32-accurate)
     m->d_tower = nullptr; m->tws = nullptr; m->tws_bytes = 0; m->tc_skip = nullptr; m->tc_skip_B = 0;
     *out = m;
     return LZ_OK;
@@ -1159,7 +1152,7 @@ int lz_model_finalize(lz_model *m)
             for (int i = 0; i < H; ++i) fc1[(size_t)i * hid + j] = (*W0)[(size_t)j * H + i];
         for (int k = 0; k < K; ++k)
             for (int j = 0; j < hid; ++j) fc2[(size_t)j * K + k] = (*W3)[(size_t)k * hid + j];
-        {   // tcgen05 copy of the LSTM weights (fp16 hi / lo, power-of-two scaled), own allocation
+        {   // tensor-core copy of the LSTM weights (fp16 hi / lo, power-of-two scaled), own allocation
             std::vector<unsigned char> wtc(ez_wtc_bytes(nin, H));
             ez_scale = ez_pack_wtc(Wih->data(), Whh->data(), nin, H, wtc.data());
             if (m->d_ez_wtc) cudaFree(m->d_ez_wtc);
@@ -1243,15 +1236,15 @@ int lz_model_finalize(lz_model *m)
 
 int lz_model_set_math(lz_model *m, int mode)
 {
-    LZ_REQUIRE(m && mode >= 0 && mode <= 2, LZ_EINVAL, "lz_model_set_math: mode must be 0 (fp32 FFMA), 1 (tcgen05 3xFP16) or 2 (tcgen05 fp16)");
+    LZ_REQUIRE(m && mode >= 0 && mode <= 2, LZ_EINVAL, "lz_model_set_math: mode must be 0 (fp32 FFMA), 1 (tensor-core 3xFP16) or 2 (tensor-core fp16)");
     LZ_REQUIRE(m->kind == 0 || mode == 0, LZ_EINVAL, "lz_model_set_math: the MLP model only has the fp32 path");
-    LZ_REQUIRE(!(m->kind == 0 && m->cfg.efficientzero && mode == 0), LZ_EINVAL, "lz_model_set_math: the EfficientZero model runs its conv stack on the tcgen05 path only (mode 1 or 2)");
+    LZ_REQUIRE(!(m->kind == 0 && m->cfg.efficientzero && mode == 0), LZ_EINVAL, "lz_model_set_math: the EfficientZero model runs its conv stack on the tensor-core path only (mode 1 or 2)");
     if (m->math != mode) ++m->generation;      // captured search graphs bake the path (and pass count) in
     m->math = mode;
     return LZ_OK;
 }
 
-/* debug: replace the layer program of the tcgen05 recurrent kernel (which == 0) or tail kernel (which == 1) */
+/* debug: replace the layer program of the tensor-core recurrent kernel (which == 0) or tail kernel (which == 1) */
 int lz_model_debug_tc_program(lz_model *m, int which, int nlayers, const int *layer_w, const int *layer_flags, int has_reward)
 {
     LZ_REQUIRE(m && m->finalized && nlayers >= 1 && nlayers <= kTcMaxLayers, LZ_EINVAL, "lz_model_debug_tc_program: bad argument");
@@ -1263,7 +1256,7 @@ int lz_model_debug_tc_program(lz_model *m, int which, int nlayers, const int *la
     return LZ_OK;
 }
 
-/* debug: copies the 64 clock64 stamps of the last instrumented tcgen05 launch (env LZ_TC_DEBUG=1) to the host */
+/* debug: copies the 64 clock64 stamps of the last instrumented tensor-core launch (env LZ_TC_DEBUG=1) to the host */
 int lz_debug_tc_stamps(unsigned long long *h_out)
 {
     LZ_REQUIRE(h_out && tc_debug_buffer(), LZ_ESTATE, "lz_debug_tc_stamps: no instrumented launch yet");

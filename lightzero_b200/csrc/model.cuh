@@ -56,7 +56,7 @@ struct RecIO {
     float *policy_logits;             // [B][A] or nullptr
     float *reward_logits, *value_logits;   // [B][K] or nullptr
     int pdl;                          // programmatic dependent launch (search graph)
-    float *skip_scratch;              // [B][2304] scratch of the tcgen05 path (nullptr: the model's own, lz_model::tc_skip)
+    float *skip_scratch;              // [B][2304] scratch of the tensor-core path (nullptr: the model's own, lz_model::tc_skip)
     // EfficientZero (reward == value prefix): LSTM state in / out, see ez.cuh
     const float *h_base, *c_base;     // base + ix[b]*hslot_stride + b*H
     size_t hslot_stride;
@@ -81,7 +81,7 @@ struct lz_model {
     lz::EzNet ez;                     // EfficientZero value-prefix head tables (device pointers into d_weights)
     float *ez_feat, *ez_htmp;         // [ws_B][hc*36], [ws_B][H] scratch between the conv kernel and the LSTM kernels
     int ez_B;
-    unsigned char *d_ez_wtc;          // LSTM weights in the tcgen05 layout (ez.cu)
+    unsigned char *d_ez_wtc;          // LSTM weights in the tensor-core layout (ez.cu)
     int latent_floats;                // floats per root latent (64*36 or latent_dim)
     lz_mlp_config mcfg;
     lz::MlpNet mlp;
@@ -95,12 +95,12 @@ struct lz_model {
     std::vector<float> stem_params;   // host copy of the Cin = 4 stem's weights + folded BN (kernel-parameter operands of k_stem4_tcl, model.cu)
     int stem_valid;
     int hw, P, K;
-    int math;                         // 0 = fp32 FFMA (net6.cuh), 1 = tcgen05 3xFP16 (fp32-accurate), 2 = tcgen05 fp16 single pass
-    unsigned char *d_tc;              // packed fp16 hi/lo weights + tables of the tcgen05 path
+    int math;                         // 0 = fp32 FFMA (net6.cuh), 1 = tensor-core 3xFP16 (fp32-accurate), 2 = tensor-core fp16 single pass
+    unsigned char *d_tc;              // packed fp16 hi/lo weights + tables of the tensor-core path
     lz::TcNet tc_rec, tc_tail;
     float *tc_skip;                   // [tc_skip_B][2304] ResBlock skip scratch of k_net_tc for launches outside a search (model_reserve)
     int tc_skip_B;
-    // tcgen05 DownSample tower: packed weights / folded BN per layer, TCL activation workspace
+    // tensor-core DownSample tower: packed weights / folded BN per layer, TCL activation workspace
     unsigned char *d_tower;           // weights + scale/shift tables
     lz::ConvTc tower_tc[7];           // rb1.c1, rb1.c2, ds(c1+c3), ds.c2, rb2.c1, rb2.c2, rb3.c1 / rb3.c2 share [6]: see model.cu
     lz::ConvTc tower_tc_rb3[2];

@@ -1,4 +1,4 @@
-// net_tc.cuh -- interface of the tcgen05 network path (net_tc.cu).
+// net_tc.cuh -- interface of the tensor-core (wgmma) network path (net_tc.cu).
 #pragma once
 #include "lz_common.cuh"
 #include "net6.cuh"
@@ -36,7 +36,6 @@ struct TcNet {
 struct TcIO {
     int B;
     int roots_per_cta;             // filled by tc_launch
-    int split_rx;                  // filled by tc_launch: > 0 = the CTA's roots run as two independently pipelined groups {split_rx, rest} (net_tc.cu)
     int npass;                     // 3 = fp32-accurate (hi*hi + hi*lo + lo*hi), 1 = fast (hi*hi)
     int pdl;                       // launch with programmatic stream serialization (inside the search graph)
     const float *latent_base;      // input latents: base + ix[b]*slot_stride + b*2304 (NCHW [64][36])
@@ -47,7 +46,7 @@ struct TcIO {
     float *reward, *value;         // [B] scalars
     float *policy_logits;          // [B][A]
     float *reward_logits, *value_logits;   // [B][K] or nullptr
-    // persistent search (the whole num_simulations loop in one launch; tree + network per CTA of 7 roots)
+    // persistent search (the whole num_simulations loop in one launch; tree + network per CTA of up to 8 roots)
     int persistent, nsims, sim0, deterministic;
     int *ix_rw, *action_rw;        // [B] tree -> network hand-off (same arrays as ix / action)
     float *latent_pool_rw;         // == latent_base; slot s+1 receives the latents of simulation s

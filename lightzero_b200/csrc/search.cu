@@ -23,7 +23,7 @@ struct lz_search {
     float *d_policy;             // [B][A]
     float *d_root_logits;        // [B][A]
     float *d_root_value;         // [B]
-    float *d_skip;               // [B][C*P] ResBlock skip scratch of the tcgen05 network kernel (per search: searches may overlap on streams)
+    float *d_skip;               // [B][C*P] ResBlock skip scratch of the tensor-core network kernel (per search: searches may overlap on streams)
     // EfficientZero: LSTM state pools [(S+1)][B][H] (tuple element 0 / 1 of reward_hidden_state, mcts_ctree.py:775-776)
     // and the per-leaf is_reset flags handed from the traverse to the LSTM kernel and the back-up (:856-861)
     float *hpool, *cpool;
@@ -54,8 +54,8 @@ static int enqueue_search(lz_search *q, int deterministic, cudaStream_t s)
     int rc;
     lz_tree *t = q->tree;
     t->step_counter = 0;
-    // Persistent search: roots never interact, so the CTA that owns 7 roots can run their whole search -- tree
-    // back-up / descent and the network -- for all num_simulations inside ONE launch of the tcgen05 kernel.
+    // Persistent search: roots never interact, so the CTA that owns up to 8 roots can run their whole search -- tree
+    // back-up / descent and the network -- for all num_simulations inside ONE launch of the tensor-core kernel.
     const bool ez = q->model->kind == 0 && q->model->cfg.efficientzero;
     if (ez) {
         // EfficientZeroMCTSCtree.search (mcts_ctree.py:671-876): the LSTM step is a GEMM over all roots, so the network
@@ -365,7 +365,7 @@ static int collect_device(lz_search *q, const float *d_obs, const uint8_t *d_obs
     int rc;
     if (d_obs_u8) {
         LZ_REQUIRE(q->model->kind == 0 && q->model->math != 0 && q->model->cfg.obs_h != 64, LZ_EINVAL,
-                   "lz_search_collect_u8: uint8 frames need the tcgen05 conv model (84x84 / 96x96)");
+                   "lz_search_collect_u8: uint8 frames need the tensor-core conv model (84x84 / 96x96)");
         if (!q->d_pre_stage && (rc = dev_alloc(&q->d_pre_stage, (size_t)q->B * q->model->latent_floats))) return rc;
         rc = model_initial_tower(q->model, q->B, nullptr, q->d_pre_stage, (cudaStream_t)s, d_obs_u8);
         if (rc == LZ_OK) rc = model_initial_tail(q->model, q->B, q->d_pre_stage, io, (cudaStream_t)s);
@@ -400,7 +400,7 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
 {
     LZ_REQUIRE(q && h_obs, LZ_EINVAL, "lz_search_collect_host: bad argument");
     LZ_REQUIRE(!obs_u8 || (q->model->kind == 0 && q->model->math != 0 && q->model->cfg.obs_h != 64), LZ_EINVAL,
-               "lz_search_collect_host_u8: uint8 frames need the tcgen05 conv model (84x84 / 96x96)");
+               "lz_search_collect_host_u8: uint8 frames need the tensor-core conv model (84x84 / 96x96)");
     const size_t esz = obs_u8 ? 1 : sizeof(float);         // bytes per observation element on the wire and in the staging buffer
     cudaStream_t s = (cudaStream_t)s_;
     const lz_model_config &c = q->model->cfg;

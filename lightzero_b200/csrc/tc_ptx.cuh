@@ -1,6 +1,6 @@
-// tc_ptx.cuh -- thin inline-PTX wrappers for the Blackwell (sm_100a) primitives used by the tcgen05 kernels:
-// mbarrier, cp.async.bulk (TMA bulk copy), proxy / tcgen05 fences, TMEM alloc / ld / st, tcgen05.mma
-// (kind::f16, cta_group::1) and tcgen05.commit, plus the UMMA shared-memory and instruction descriptors.
+// tc_ptx.cuh -- thin inline-PTX wrappers for the Hopper (sm_90a) primitives used by the tensor-core kernels:
+// mbarrier, cp.async.bulk (TMA bulk copy), proxy fences, wgmma (m64nNk16, fp16 in, fp32 accumulate in registers) and its
+// shared-memory matrix descriptor.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -27,7 +27,8 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes)
 {
     asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}\n" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-// bounded wait: a protocol bug must trap, never hang the GPU
+// Bounded wait: a protocol bug must trap, never hang the GPU.  No printf here: a call anywhere in a kernel makes ptxas serialise
+// its wgmma pipeline (every MMA would wait for the previous one).
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)
 {
     const uint32_t a = smem_u32(bar);
@@ -37,30 +38,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)
                      : "=r"(ok) : "r"(a), "r"(parity) : "memory");
         if (ok) return;
     }
-    printf("lz net_tc: mbarrier timeout (block %d thread %d)\n", blockIdx.x, threadIdx.x);
     asm volatile("trap;\n");
-}
-// Whole-warp wait: only lane 0 polls (with back-off) so that idle warps do not compete with the tensor
-// core's operand fetch for shared-memory bandwidth; the other lanes park at the warp barrier.
-__device__ __forceinline__ void mbar_wait_warp(uint64_t *bar, uint32_t parity)
-{
-    if ((threadIdx.x & 31) == 0) {
-        const uint32_t a = smem_u32(bar);
-        uint32_t ok = 0;
-        for (uint32_t it = 0; it < (1u << 26) && !ok; ++it) {
-            asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                         : "=r"(ok) : "r"(a), "r"(parity) : "memory");
-#ifndef LZ_POLL_NS
-#define LZ_POLL_NS 64
-#endif
-            if (!ok) __nanosleep(LZ_POLL_NS);
-        }
-        if (!ok) {
-            printf("lz net_tc: mbarrier timeout (block %d warp %d)\n", blockIdx.x, threadIdx.x >> 5);
-            asm volatile("trap;\n");
-        }
-    }
-    __syncwarp();
 }
 __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar)
 {
@@ -69,148 +47,86 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t by
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t *dst_smem, uint32_t ncols)
-{
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], fp16 inputs, fp32 accumulate, issued by ONE thread
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-                 ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// The same, to be executed by ALL lanes of the issuing warp in uniform control flow: one elected lane issues.  Measured
-// (profiles/r01e_mma_probe.md): 48.6 cycles per N = 64 MMA (the shared-memory operand floor) against 60-78 when the
-// instruction sits in an `if (lane == 0)` branch, where ptxas wraps it in an ELECT / BRA.U.ANY loop.
-__device__ __forceinline__ void umma_f16_elect(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile("{\n\t.reg .pred pe;\n\t.reg .pred pa;\n\telect.sync _|pe, 0xffffffff;\n\tsetp.ne.b32 pa, %4, 0;\n\t"
-                 "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, pa;\n\t}\n"
-                 ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit_elect(uint64_t *bar)
-{
-    asm volatile("{\n\t.reg .pred pe;\n\telect.sync _|pe, 0xffffffff;\n\t"
-                 "@pe tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}\n" ::"r"(smem_u32(bar)) : "memory");
-}
-// arrives on the mbarrier once every MMA issued so far by this thread has completed
-__device__ __forceinline__ void umma_commit(uint64_t *bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// one elected lane of a converged warp (true in exactly one lane)
-__device__ __forceinline__ bool elect_one()
-{
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}\n" : "=r"(pred));
-    return pred != 0;
-}
-// whole-warp wait for a warp that must stay converged (the MMA issuer): one lane polls, the others park at the warp barrier
-__device__ __forceinline__ void mbar_wait_converged(uint64_t *bar, uint32_t parity)
-{
-#ifdef LZ_WAIT_ONE_LANE
-    if ((threadIdx.x & 31) == 0) mbar_wait(bar, parity);
-    __syncwarp();
-#else
-    // every lane polls (same address: one shared-memory access per try): no divergent branch at all in front of the elect.sync
-    // issue loop -- a lane-0-only poll followed by __syncwarp() left the warp split and every elect.sync re-converging (measured:
-    // ~330 cycles per MMA instead of 49-65)
-    mbar_wait(bar, parity);
-    __syncwarp();
-#endif
-}
-// tcgen05.ld without the wait (several loads in flight), and the wait that also pins the destination registers so the
-// compiler cannot schedule their uses above it
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32])
-{
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                   "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                   "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t (&r)[16])
-{
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
+// ---- wgmma (sm_90a): D[64 x N] (+)= A[64 x 16] * B[16 x N], fp16 inputs from shared-memory descriptors, fp32 accumulators in the
+// registers of the issuing warpgroup.  Accumulator fragment of thread (warp w of the warpgroup, lane l): d[4 j + {0, 1}] = row
+// 16 w + l / 4, columns 8 j + 2 (l % 4) + {0, 1}; d[4 j + {2, 3}] = the same columns of row 16 w + l / 4 + 8.
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
 template <int N>
-__device__ __forceinline__ void tmem_pin(uint32_t (&r)[N])
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
+
+// Pins accumulator registers at this point of the program: zeroing (or reading) them cannot be moved into a wgmma pipeline stage,
+// which would make ptxas serialise every wgmma of the kernel
+template <int N>
+__device__ __forceinline__ void wg_fence_acc(float (&d)[N])
 {
 #pragma unroll
-    for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i]));
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32])
-{
-    uint32_t r[32];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                   "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                   "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16])
-{
-    uint32_t r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float (&v)[32])
-{
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-                 "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-                 "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n"
-                 ::"r"(taddr),
-                   "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-                   "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-                   "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-                   "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15])),
-                   "r"(__float_as_uint(v[16])), "r"(__float_as_uint(v[17])), "r"(__float_as_uint(v[18])), "r"(__float_as_uint(v[19])),
-                   "r"(__float_as_uint(v[20])), "r"(__float_as_uint(v[21])), "r"(__float_as_uint(v[22])), "r"(__float_as_uint(v[23])),
-                   "r"(__float_as_uint(v[24])), "r"(__float_as_uint(v[25])), "r"(__float_as_uint(v[26])), "r"(__float_as_uint(v[27])),
-                   "r"(__float_as_uint(v[28])), "r"(__float_as_uint(v[29])), "r"(__float_as_uint(v[30])), "r"(__float_as_uint(v[31]))
-                 : "memory");
-    asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory");
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// K-major, SWIZZLE_NONE shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-// start address >> 4 in [0,14), leading byte offset >> 4 in [16,30) (between the two 16-byte K chunks of
-// one MMA), stride byte offset >> 4 in [32,46) (between 8-row core matrices), version = 1 in [46,48).
+#define LZ_WG_R8(o) "+f"(d[o + 0]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+__device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t a, uint64_t b)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
+                 : LZ_WG_R8(0) : "l"(a), "l"(b));
+}
+__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t a, uint64_t b)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
+                 "%15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
+                 : LZ_WG_R8(0), LZ_WG_R8(8) : "l"(a), "l"(b));
+}
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a, uint64_t b)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
+                 "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+                 : LZ_WG_R8(0), LZ_WG_R8(8), LZ_WG_R8(16), LZ_WG_R8(24) : "l"(a), "l"(b));
+}
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t a, uint64_t b)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
+                 "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, "
+                 "%39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, "
+                 "%63}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+                 : LZ_WG_R8(0), LZ_WG_R8(8), LZ_WG_R8(16), LZ_WG_R8(24), LZ_WG_R8(32), LZ_WG_R8(40), LZ_WG_R8(48), LZ_WG_R8(56)
+                 : "l"(a), "l"(b));
+}
+#undef LZ_WG_R8
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t a, uint64_t b)
+{
+    if constexpr (N == 16) wgmma_n16(d, a, b);
+    else if constexpr (N == 32) wgmma_n32(d, a, b);
+    else if constexpr (N == 64) wgmma_n64(d, a, b);
+    else wgmma_n128(d, a, b);
+}
+
+// Writes a warpgroup's m64nN accumulator fragment to a row-major fp32 array S[row][ld] at rows row0 .. row0 + 63, columns col0 ..
+// (the read-outs then own one row per thread, as the epilogues are written)
+template <int N>
+__device__ __forceinline__ void wg_stage(float *S, int ld, int row0, int col0, const float (&d)[N / 2])
+{
+    const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    float *p0 = S + (size_t)(row0 + 16 * w + (lane >> 2)) * ld + col0 + 2 * (lane & 3), *p1 = p0 + 8 * ld;
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+        *reinterpret_cast<float2 *>(p0 + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
+        *reinterpret_cast<float2 *>(p1 + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    }
+}
+
+// K-major, no-swizzle shared-memory matrix descriptor of wgmma: start address >> 4 in [0,14), leading byte offset >> 4 in [16,30)
+// (between the two 16-byte K core matrices of one k-step), stride byte offset >> 4 in [32,46) (between 8-row core matrices).
+// Descriptors of the same operand differ only in the start-address field: 16-byte-unit offsets are added to a base.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo16, uint32_t sbo16)
 {
-    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)(lbo16 & 0x3FFFu) << 16) | ((uint64_t)(sbo16 & 0x3FFFu) << 32) | (1ull << 46);
+    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)(lbo16 & 0x3FFFu) << 16) | ((uint64_t)(sbo16 & 0x3FFFu) << 32);
 }
-// instruction descriptor, kind::f16: D = F32 (bit 4), A = B = F16 (0), both K-major, N>>3 at [17,23), M>>4 at [24,29)
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) { return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24); }
 
 // split 8 floats into fp16 hi / lo and store them as two 16-byte vectors
 __device__ __forceinline__ void store_split8(unsigned char *hi_ptr, unsigned char *lo_ptr, const float *v)

@@ -138,7 +138,7 @@ k_tree_backprop_traverse(TreeParams p, int latent_index, const float *reward, co
                          const float *logits, int deterministic, unsigned step, int32_t *ix, int32_t *act, int32_t *is_reset)
 {
     const int b = blockIdx.x * (kTreeBlock / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    pdl_launch_dependents();      // lets the next network kernel set up (TMEM, barriers, first weight taps) meanwhile
+    pdl_launch_dependents();      // lets the next network kernel set up (barriers, first weight taps) meanwhile
     pdl_wait();                   // reward / value / logits come from the preceding network kernel
     if (b >= p.B) return;
     tree_backprop<EZ>(p, b, lane, latent_index, reward[b], value[b], logits + (size_t)b * p.A, nullptr,

@@ -1,7 +1,7 @@
 """Host-side mirror of ``lzero.model.efficientzero_model.EfficientZeroModel`` (efficientzero_model.py:20-272): same
 constructor keywords, ``initial_inference(obs)`` / ``recurrent_inference(latent_state, reward_hidden_state, action)`` with
 the same ``EZNetworkOutput``; weights come from the reference ``state_dict`` (the training-only SSL ``projection`` /
-``prediction_head`` entries are ignored).  The conv trunk and the prediction heads run on the tcgen05 kernels shared with
+``prediction_head`` entries are ignored).  The conv trunk and the prediction heads run on the wgmma kernels shared with
 ``MuZeroModel``; the value-prefix head (conv1x1 -> BN -> ReLU -> LSTM -> BN -> ReLU -> MLP, :552-569) is a batched GEMM +
 fused cell update (csrc/ez.cu).  Inference only (eval mode)."""
 from dataclasses import dataclass

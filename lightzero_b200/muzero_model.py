@@ -90,7 +90,7 @@ class MuZeroModel:
     MATH_MODES = {"fp32": 0, "tc3": 1, "tc1": 2}
 
     def set_math(self, mode):
-        """'fp32' = FFMA on CUDA cores, 'tc3' = tcgen05 3xFP16 (fp32-accurate), 'tc1' = tcgen05 single fp16 pass."""
+        """'fp32' = FFMA on CUDA cores, 'tc3' = wgmma 3xFP16 (fp32-accurate), 'tc1' = wgmma single fp16 pass."""
         code = self.MATH_MODES[mode] if isinstance(mode, str) else int(mode)
         cabi.check(self._lib.lz_model_set_math(self._h, code), "lz_model_set_math")
         self.math = code

@@ -46,14 +46,13 @@ def main():
     print("== last simulation of CTA 0, cycles since the start of the simulation (tree phase first)")
     print(f"   tree: backprop done {rel(56):8d}  traverse done (warp 0) + CTA barrier {rel(51):8d}")
     print(f"   load done                        {rel(1):8d}")
+    prev = 1
     for L in range(5):
-        print(f"   L{L}: mma issue {rel(32 + 2 * L):8d} -> {rel(33 + 2 * L):8d} | acc ready {rel(2 + 2 * L):8d}  epilogue done {rel(3 + 2 * L):8d}"
-              f"   [mma {s[2 + 2 * L] - s[32 + 2 * L]:6d}  epi {s[3 + 2 * L] - s[2 + 2 * L]:6d}]")
-    print(f"   last layer: group X epilogue done (act_ready[0]) {rel(57):8d}")
-    print(f"   early reward head done           {rel(28):8d}")
-    print(f"   hooks ready                      {rel(24):8d}")
-    print(f"   VP heads: scatter done {rel(44):8d}  FC1 {rel(45):8d}  hidden {rel(46):8d}  FC2 {rel(47):8d}  all done {rel(27):8d}")
-    print(f"   ring waits summed over the whole launch (CTA 0): MMA warp {s[52]} (+ first tap of each simulation {s[53]}), FC1 {s[54]}, FC2 {s[55]}  -> per simulation (4 calls) {s[52] // (4 * S)}, {s[53] // (4 * S)}, {s[54] // (4 * S)}, {s[55] // (4 * S)}")
+        print(f"   L{L}: MMAs done {rel(2 + 2 * L):8d}  epilogue (+ hooks) done {rel(3 + 2 * L):8d}"
+              f"   [mma {s[2 + 2 * L] - s[prev]:6d}  epi {s[3 + 2 * L] - s[2 + 2 * L]:6d}]")
+        prev = 3 + 2 * L
+    print(f"   layers done                      {rel(24):8d}")
+    print(f"   heads: B operand ready {rel(44):8d}  FC1 {rel(45):8d}  hidden {rel(46):8d}  FC2 {rel(47):8d}  all done {rel(27):8d}")
     print(f"   total kernel cycles (start stamp -> end of last sim) {s[27] - s[0]}  = {(s[27] - s[0]) / S:.0f} per simulation")
 
 

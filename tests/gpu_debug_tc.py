@@ -1,4 +1,4 @@
-"""Bring-up diagnostics for the tcgen05 path (run on the GPU box; not a pytest).  Single-layer
+"""Bring-up diagnostics for the tensor-core (wgmma) path (run on the GPU box; not a pytest).  Single-layer
 programs first (localise descriptor / epilogue bugs), then the full network against fp32 FFMA and
 the PyTorch oracle."""
 import ctypes
@@ -111,7 +111,7 @@ if __name__ == "__main__" and not os.environ.get("DBG_PHASES"):
 
 
 def phase_breakdown():
-    """clock64 stamps of CTA 0 (env LZ_TC_DEBUG=1): where does a tcgen05 launch spend its cycles?"""
+    """clock64 stamps of CTA 0 (env LZ_TC_DEBUG=1): where does a k_net_tc launch spend its cycles?"""
     os.environ["LZ_TC_DEBUG"] = "1"
     A = 6
     torch.manual_seed(0)

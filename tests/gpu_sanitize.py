@@ -46,10 +46,10 @@ eroots = emcts.roots(B, [list(range(A))] * B)
 eroots.prepare(0.25, noise, [0.] * B, eo.policy_logits, [1, 2] * (B // 2) + [1])     # two-player branch
 emcts.search(eroots, ecu, eo.latent_state, eo.reward_hidden_state, [1, 2] * (B // 2) + [1])
 print("efficientzero ok", r["values"][:3].tolist(), eroots.get_distributions()[:2])
-# round 2: a batch that takes the {5, 2} root-group split of the persistent kernel (7 roots per CTA), the fused reuse searches, the
+# a batch that leaves the last CTA of the persistent kernel partly filled (8 roots per CTA), the fused reuse searches, the
 # uint8 entry point fed by the device-resident frame stack, GameSegment statistics
 from lightzero_b200.collector import FrameStack, SegmentStats
-B2 = 148 * 6 + 5
+B2 = 132 * 7 + 5
 cu = lzb.MuZeroModel(observation_shape=(4, 84, 84), action_space_size=A).load_state_dict(ref.state_dict())
 pol = MuZeroCollectPolicy(cu, dict(num_simulations=4, deterministic=True, discount_factor=0.997))
 fs = FrameStack(B2, 4, 84, 84)

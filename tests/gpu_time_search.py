@@ -1,5 +1,5 @@
 """Times the fused MuZero search (bench size by default) with CUDA events, uninstrumented: the A/B tool for kernel variants
-(LZ_LIB_TAG=<tag> picks lightzero_b200/_lib/<tag>/liblzb200.so; LZ_TC_SPLIT / LZ_TC_ROOTS are read by tc_launch at graph capture)."""
+(LZ_LIB_TAG=<tag> picks lightzero_b200/_lib/<tag>/liblzb200.so; LZ_TC_ROOTS is read by tc_launch at graph capture)."""
 import os
 import sys
 
@@ -29,4 +29,4 @@ for it in range(int(os.environ.get("DBG_N", 8))):
     torch.cuda.synchronize()
     ms.append(a.elapsed_time(b))
 vis = np.asarray(roots.get_distributions()).sum()
-print(f"tag={os.environ.get('LZ_LIB_TAG', '-')} split={os.environ.get('LZ_TC_SPLIT', 'default')} B={B} S={S} A={A}: search ms min {min(ms[2:]):.3f} median {sorted(ms[2:])[len(ms[2:]) // 2]:.3f}  (visits {int(vis)})")
+print(f"tag={os.environ.get('LZ_LIB_TAG', '-')} B={B} S={S} A={A}: search ms min {min(ms[2:]):.3f} median {sorted(ms[2:])[len(ms[2:]) // 2]:.3f}  (visits {int(vis)})")

@@ -110,10 +110,10 @@ def test_model_rejects_unsupported_configs():
         m.initial_inference(torch.zeros(1, 4, 84, 84).cuda())
 
 
-# ------------------------------------------------------------------ tcgen05 path (lz_model_set_math)
+# ------------------------------------------------------------------ tensor-core path (lz_model_set_math)
 @pytest.mark.parametrize("B,A", [(7, 6), (50, 18), (1000, 6), (1024, 18)])
 def test_tensor_core_3xfp16_recurrent_matches_oracle(B, A):
-    """math='tc3': tcgen05 MMAs on fp16 hi/lo splits (3 passes), fp32 accumulation in TMEM -- must meet the
+    """math='tc3': wgmma MMAs on fp16 hi/lo splits (3 passes), fp32 accumulation in registers -- must meet the
     same 1e-5 bar as the fp32 FFMA path."""
     ref, cu = _models(A, seed=4)
     cu.set_math("tc3")

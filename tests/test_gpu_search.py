@@ -57,7 +57,7 @@ def test_fused_graph_search_equals_stepwise_search(B, A, S, masks, math):
         roots.clear()
     assert results[0] == results[1] == results[2]
     assert all(sum(d) == S for d in results[0][0])
-    # one persistent launch (tcgen05 path) or [traverse] + S x [network, backprop(+traverse)] kernels
+    # one persistent launch (tensor-core path) or [traverse] + S x [network, backprop(+traverse)] kernels
     assert mcts.last_num_kernels in (1, 2 * S + 1)
 
 
