@@ -265,7 +265,7 @@ int lz_search_collect_u8(lz_search *q, const uint8_t *d_obs_u8, const uint8_t *d
 int lz_search_collect_host_u8(lz_search *q, const uint8_t *h_obs_u8, const uint8_t *h_mask, const float *h_noise,
                               float noise_weight, const int32_t *h_to_play, int deterministic, int nchunks,
                               float *d_pred_value, float *d_policy_logits, lz_stream s);
-/* Number of kernel nodes one lz_search_run enqueues (for launch accounting). */
+/* Number of kernel nodes of the search graph this search launched last (any lz_search_run* / lz_search_collect* call). */
 int lz_search_num_kernels(const lz_search *q);
 /* Device pointer of the latent pool (NCHW per slot) for inspection in tests. */
 const float *lz_search_latent_pool(const lz_search *q);

@@ -200,7 +200,6 @@ __global__ void __launch_bounds__(kTThreads, 1) k_ez_lstm_tc(EzNet net, EzIO io)
             for (int c = 0; c < nchunks; ++c) {
                 const int st = c % kTStages;
                 if (c >= kTStages) mbar_wait(&bars->empty[st], ((c / kTStages) - 1) & 1);
-                if ((io.dbg & 2) && c >= kTStages) { mbar_arrive(&bars->full_w[st]); continue; }
                 mbar_expect_tx(&bars->full_w[st], 2 * kTWPart);
                 bulk_g2s(smem + st * kTStageBytes + 2 * kTAPart, src + (size_t)c * (2 * kTWPart), 2 * kTWPart, &bars->full_w[st]);
             }
@@ -230,7 +229,7 @@ __global__ void __launch_bounds__(kTThreads, 1) k_ez_lstm_tc(EzNet net, EzIO io)
             const float *src = (k0 < nin ? fsrc[ps] + k0 : hsrc[ps] + (k0 - nin)) + pkg * 8;
 #pragma unroll
             for (int u = 0; u < 4; ++u)      // u: 0,1 = k-group pkg, 2,3 = k-group pkg + 4
-                v[ps * 4 + u] = (pon[ps] && !(io.dbg & 1)) ? *reinterpret_cast<const float4 *>(src + (u >> 1) * 32 + (u & 1) * 4) : make_float4(0, 0, 0, 0);
+                v[ps * 4 + u] = pon[ps] ? *reinterpret_cast<const float4 *>(src + (u >> 1) * 32 + (u & 1) * 4) : make_float4(0, 0, 0, 0);
         }
         if (c >= kTStages) mbar_wait(&bars->empty[st], ((c / kTStages) - 1) & 1);
 #pragma unroll
@@ -279,7 +278,7 @@ __global__ void __launch_bounds__(kTThreads, 1) k_ez_lstm_tc(EzNet net, EzIO io)
     {
         const bool odd = (lane & 1) != 0;
         const int row = grp * 64 + 16 * (warp & 3) + (lane >> 2) + (odd ? 8 : 0), b = m0 + row;
-        const bool on = b < io.B && !(io.dbg & 4);
+        const bool on = b < io.B;
         const size_t hoff = (on && io.ix ? (size_t)io.ix[b] * io.slot_stride : 0) + (size_t)(on ? b : 0) * H;
         const float inv = net.wtc_inv_scale;
         const float *c_in = io.c_base + hoff;
@@ -342,13 +341,11 @@ int ez_prepare_launch()
     return LZ_OK;
 }
 
-int ez_launch(const EzNet &net, const EzIO &io_in, cudaStream_t s, int math)
+int ez_launch(const EzNet &net, const EzIO &io, cudaStream_t s, int math)
 {
-    EzIO io = io_in;
-    if (const char *e = getenv("LZ_EZ_DBG")) io.dbg = atoi(e);
     LZ_REQUIRE(net.H <= kHMaxH && net.hid <= kHMaxHid && net.K <= kHLd && (net.H % 8) == 0, LZ_EINVAL,
                "ez_launch: unsupported LSTM / head size (H=%d hid=%d K=%d)", net.H, net.hid, net.K);
-    const bool tc_ok = net.wtc && (net.nin % kTK) == 0 && (net.H % kTK) == 0 && !getenv("LZ_EZ_FP32");
+    const bool tc_ok = net.wtc && (net.nin % kTK) == 0 && (net.H % kTK) == 0;
     if (math != 0 && tc_ok) {
         dim3 grid(4 * net.H / kTN, (io.B + kTM - 1) / kTM);
         k_ez_lstm_tc<<<grid, kTThreads, kTSmem, s>>>(net, io);

@@ -30,7 +30,6 @@ struct EzIO {
     float *h_tmp;             // [B][H] un-reset h' (input of the value-prefix head)
     float *value_prefix;      // [B] scalar or nullptr
     float *vp_logits;         // [B][K] or nullptr
-    int dbg;                  // timing experiments (env LZ_EZ_DBG; wrong results): 1 = no A loads, 2 = no weight copies, 4 = no cell update
 };
 
 int ez_launch(const EzNet &net, const EzIO &io, cudaStream_t s, int math);   // math 0: fp32 FFMA GEMM, else tensor-core (wgmma) 3xFP16

@@ -424,7 +424,6 @@ int model_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
         t.latent_base = io.latent_base; t.ix = io.ix; t.slot_stride = io.slot_stride; t.action = io.action;
         t.latent_out = io.next_latent; t.reward = io.reward; t.value = io.value; t.policy_logits = io.policy_logits;
         t.reward_logits = io.reward_logits; t.value_logits = io.value_logits;
-        t.pdl = io.pdl;
         t.skip_scratch = io.skip_scratch;
         if (!t.skip_scratch) {
             LZ_REQUIRE(io.B <= m->tc_skip_B, LZ_ESTATE, "model_recurrent: scratch sized for %d roots, got %d (model_reserve)", m->tc_skip_B, io.B);
@@ -583,7 +582,7 @@ static int tower_tc_run(lz_model *m, int B, const float *d_obs, float *pre_laten
     const int npass = (m->math == 1) ? 3 : 1;
     // stem: conv1 (Cin = 4/12, stride 2) on the CUDA cores, written straight into TCL (uint8 frames are scaled to [0, 1] here)
     const ConvG &S0 = m->tower[0];
-    if (m->stem_valid && !getenv("LZ_STEM_GENERIC")) {
+    if (m->stem_valid) {
         const int rows_per_cta = std::max(1, 256 / S0.wout);
         const size_t smem = (size_t)4 * (2 * rows_per_cta + 1) * (S0.win + 4) * sizeof(float);
         dim3 grid(ceil_div(S0.hout, rows_per_cta), B);
@@ -639,7 +638,7 @@ int model_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, c
     float *a = m->ws[0], *b = m->ws[1], *c = m->ws[2];
     const std::vector<ConvG> &T = m->tower;
     int rc;
-    if (m->math != 0 && m->cfg.obs_h != 64 && !getenv("LZ_TOWER_SIMT")) {
+    if (m->math != 0 && m->cfg.obs_h != 64) {
         if ((rc = tower_tc_run(m, B, d_obs, a, s))) return rc;
         return model_initial_tail(m, B, a, io_in, s);
     }
@@ -662,18 +661,10 @@ int model_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, c
         if ((rc = launch_pool(c, a, B * kC, h3, h4, s))) return rc;
         pre = a;
     }
+    if (m->math != 0) return model_initial_tail(m, B, pre, io_in, s);
     TailIO io = io_in;
     io.B = B;
     io.pre_latent = pre;
-    if (m->math != 0) {
-        TcIO t;
-        memset(&t, 0, sizeof(t));
-        t.B = B; t.npass = (m->math == 1) ? 3 : 1;
-        t.latent_base = pre; t.latent_out = io.latent; t.latent_out2 = io.latent2;
-        t.value = io.value; t.policy_logits = io.policy_logits; t.value_logits = io.value_logits;
-        t.skip_scratch = m->tc_skip;
-        return tc_launch(m->tc_tail, t, s);
-    }
     switch (pick_W(B)) {
         case 8: return launch_tail<8>(m->net, io, s);
         case 4: return launch_tail<4>(m->net, io, s);

@@ -55,7 +55,6 @@ struct RecIO {
     float *reward, *value;            // [B] scalars or nullptr
     float *policy_logits;             // [B][A] or nullptr
     float *reward_logits, *value_logits;   // [B][K] or nullptr
-    int pdl;                          // programmatic dependent launch (search graph)
     float *skip_scratch;              // [B][2304] scratch of the tensor-core path (nullptr: the model's own, lz_model::tc_skip)
     // EfficientZero (reward == value prefix): LSTM state in / out, see ez.cuh
     const float *h_base, *c_base;     // base + ix[b]*hslot_stride + b*H

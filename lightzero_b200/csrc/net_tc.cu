@@ -393,7 +393,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
     const int nsims = io.nsims > 0 ? io.nsims : 1;     // > 1 (or persistent): the whole search loop runs inside this launch
     const bool persistent = io.persistent != 0;
 
-    pdl_launch_dependents();      // the next tree kernel may become resident; it blocks in pdl_wait() until this grid is done
     // ---- one-time setup ----
     if (tid == 0) {
         for (int i = 0; i < kStages; ++i) { mbar_init(&bars->full[i], 1); mbar_init(&bars->empty[i], kEpiWarps); }
@@ -484,7 +483,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
     unsigned char *fr = smem + kSmemMain;      // reward features (fp16 hi / lo, FC1's B-operand rows 0-7), parked from their hook
     unsigned long long *dbg = (io.dbg && blockIdx.x == 0 && tid == 0) ? io.dbg : nullptr;
     if (dbg) dbg[0] = clock64();
-    pdl_wait();                   // ix / action / the latent pool come from the preceding kernels
     // this warp's tree (tree_persist.cuh): its scalars / first path entries live in registers during the tree phase and are
     // parked in shared memory while the warp does network work
     uint32_t *tree_park = reinterpret_cast<uint32_t *>(smem + kSmemMain + kFrBytes) + warp * kTreeParkWords;
@@ -929,17 +927,9 @@ int tc_launch(const TcNet &net, const TcIO &io_in, cudaStream_t s, const TreePar
     io.dbg = g_dbg;
     io.roots_per_cta = tc_pick_roots(io.B);
     LZ_REQUIRE(!io.persistent || tp.A <= 32, LZ_EINVAL, "tc_launch: the persistent search needs A <= 32 (got %d)", tp.A);
-    if (const char *e = getenv("LZ_TC_ROOTS")) io.roots_per_cta = std::min(std::max(atoi(e), 1), kMaxRoots);
     const int grid = (io.B + io.roots_per_cta - 1) / io.roots_per_cta;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kTcThreads); cfg.dynamicSmemBytes = kSmemBytes; cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = io_in.pdl ? 1 : 0;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    count_launch();
-    LZ_CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_net_tc, net, io, tp));
+    k_net_tc<<<grid, kTcThreads, kSmemBytes, s>>>(net, io, tp);
+    LZ_KERNEL_CHECK();
     return LZ_OK;
 }
 

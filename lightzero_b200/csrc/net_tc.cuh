@@ -37,7 +37,6 @@ struct TcIO {
     int B;
     int roots_per_cta;             // filled by tc_launch
     int npass;                     // 3 = fp32-accurate (hi*hi + hi*lo + lo*hi), 1 = fast (hi*hi)
-    int pdl;                       // launch with programmatic stream serialization (inside the search graph)
     const float *latent_base;      // input latents: base + ix[b]*slot_stride + b*2304 (NCHW [64][36])
     const int *ix;                 // or nullptr
     size_t slot_stride;

@@ -4,13 +4,18 @@
 // :326-329, a duplicated recurrent_inference :338/:345, four blocking D2H copies :347-350 and three
 // .tolist() conversions :355-357) has no counterpart here: the tree hands (slot, action) to the
 // network through device memory and the network hands (reward, value, logits) back the same way.
-#include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
 
 #include "model.cuh"
 #include "tree.cuh"
+
+struct SearchGraph {              // one instantiated search graph and what it baked in
+    cudaGraphExec_t exec;
+    unsigned long long gen_model, gen_tree;   // model / tree generation at capture
+    int num_kernels;              // kernel nodes
+};
 
 struct lz_search {
     lz_tree *tree;
@@ -32,12 +37,10 @@ struct lz_search {
     // ReZero search_with_reuse: library-owned copies of the caller's per-root true action / reuse value (graph-stable addresses)
     int32_t *d_true_action;
     float *d_reuse_value;
-    cudaGraphExec_t exec_reuse;
-    cudaGraphExec_t exec[2];     // [deterministic]
-    unsigned long long gen_model[3], gen_tree[3];   // model / tree generation each graph (exec[0], exec[1], exec_reuse) was captured at
+    SearchGraph graphs[3];       // plain search with deterministic 0 / 1, search with reuse
     cudaStream_t capture_stream; // library-owned: the caller's stream may be the legacy default stream,
                                  // which cannot be captured; the instantiated graph launches on the caller's
-    int num_kernels;
+    int num_kernels;             // kernel nodes of the graph launched last
     // host-buffer collect: staging + copy stream so the H2D of chunk i+1 overlaps the tower of chunk i
     cudaStream_t copy_stream, copy_stream2;   // chunks alternate between two copy streams (two DMA engines)
     cudaEvent_t ev_chunk[8], ev_start;
@@ -49,38 +52,37 @@ struct lz_search {
 
 using namespace lz;
 
-static int enqueue_search(lz_search *q, int deterministic, cudaStream_t s)
+// recurrent_inference of simulation sim: latents (and EfficientZero LSTM state) gathered at the slots the descent left in d_ix,
+// results into pool slot sim + 1 (mcts_ctree.py:352,364) and the tree hand-off buffers
+static RecIO rec_io(const lz_search *q, int sim)
+{
+    RecIO io;
+    memset(&io, 0, sizeof(io));
+    io.B = q->B; io.latent_base = q->pool; io.ix = q->d_ix; io.slot_stride = q->slot_stride; io.action = q->d_action;
+    io.next_latent = q->pool + (size_t)(sim + 1) * q->slot_stride;
+    io.reward = q->d_reward; io.value = q->d_value; io.policy_logits = q->d_policy;
+    io.skip_scratch = q->d_skip;
+    if (q->hpool) {
+        io.h_base = q->hpool; io.c_base = q->cpool; io.hslot_stride = q->hslot_stride;
+        io.h_out = q->hpool + (size_t)(sim + 1) * q->hslot_stride; io.c_out = q->cpool + (size_t)(sim + 1) * q->hslot_stride;
+        io.is_reset = q->d_is_reset;
+    }
+    return io;
+}
+
+// MuZeroMCTSCtree.search (mcts_ctree.py:267-368), EfficientZeroMCTSCtree.search (:671-876) and their search_with_reuse variants
+// (:370-468, :878-1003): [descent] + S x [recurrent_inference, back-up (+ next descent)].  Under reuse every tree goes through the
+// network every simulation (the reference compacts the batch on the host; here the rows of "no inference" trees are computed and
+// ignored, which keeps the loop one static CUDA graph).
+static int enqueue_search(lz_search *q, int deterministic, bool reuse, cudaStream_t s)
 {
     int rc;
     lz_tree *t = q->tree;
     t->step_counter = 0;
     // Persistent search: roots never interact, so the CTA that owns up to 8 roots can run their whole search -- tree
     // back-up / descent and the network -- for all num_simulations inside ONE launch of the tensor-core kernel.
-    const bool ez = q->model->kind == 0 && q->model->cfg.efficientzero;
-    if (ez) {
-        // EfficientZeroMCTSCtree.search (mcts_ctree.py:671-876): the LSTM step is a GEMM over all roots, so the network
-        // is several launches per simulation and the loop stays a multi-kernel graph
-        if ((rc = tree_launch_traverse(t, t->p.tie_first, q->d_ix, nullptr, q->d_action, nullptr, nullptr, s, q->d_is_reset))) return rc;
-        for (int sim = 0; sim < q->S; ++sim) {
-            RecIO io;
-            memset(&io, 0, sizeof(io));
-            io.B = q->B; io.latent_base = q->pool; io.ix = q->d_ix; io.slot_stride = q->slot_stride; io.action = q->d_action;
-            io.next_latent = q->pool + (size_t)(sim + 1) * q->slot_stride;
-            io.reward = q->d_reward; io.value = q->d_value; io.policy_logits = q->d_policy;
-            io.h_base = q->hpool; io.c_base = q->cpool; io.hslot_stride = q->hslot_stride;
-            io.h_out = q->hpool + (size_t)(sim + 1) * q->hslot_stride; io.c_out = q->cpool + (size_t)(sim + 1) * q->hslot_stride;
-            io.is_reset = q->d_is_reset;
-            io.skip_scratch = q->d_skip;
-            if ((rc = model_recurrent(q->model, io, s))) return rc;
-            if (sim + 1 < q->S)
-                rc = tree_launch_backprop_traverse(t, sim + 1, q->d_reward, q->d_value, q->d_policy, t->p.tie_first, q->d_ix, q->d_action, s, q->d_is_reset);
-            else
-                rc = tree_launch_backprop(t, sim + 1, q->d_reward, q->d_value, q->d_policy, nullptr, s, q->d_is_reset);
-            if (rc) return rc;
-        }
-        return LZ_OK;
-    }
-    if (q->model->kind == 0 && q->model->math != 0 && t->p.A <= 32 && !getenv("LZ_NO_PERSIST")) {   // tree_persist.cuh: one lane per child
+    // EfficientZero stays a multi-kernel graph: its LSTM step is a GEMM over all roots (several launches per simulation).
+    if (!reuse && !q->hpool && q->model->kind == 0 && q->model->math != 0 && t->p.A <= 32) {   // tree_persist.cuh: one lane per child
         TcIO io;
         memset(&io, 0, sizeof(io));
         io.B = q->B; io.npass = (q->model->math == 1) ? 3 : 1;
@@ -92,116 +94,113 @@ static int enqueue_search(lz_search *q, int deterministic, cudaStream_t s)
         io.pool_cl = 1;      // slots >= 1 are written and read only by this kernel: channels-last (vector loads / stores); slot 0 stays NCHW
         return tc_launch(q->model->tc_rec, io, s, &t->p);
     }
-    const bool pdl = q->model->kind == 0 && q->model->math != 0 && getenv("LZ_PDL");   // opt-in: measured slower (6.26 vs 5.90 ms per 50-sim search)
-    t->pdl = pdl;
-    if ((rc = tree_launch_traverse(t, deterministic, q->d_ix, nullptr, q->d_action, nullptr, nullptr, s))) return rc;
-    for (int sim = 0; sim < q->S; ++sim) {
-        RecIO io;
-        memset(&io, 0, sizeof(io));
-        io.B = q->B;
-        io.latent_base = q->pool;
-        io.ix = q->d_ix;
-        io.slot_stride = q->slot_stride;
-        io.action = q->d_action;
-        io.next_latent = q->pool + (size_t)(sim + 1) * q->slot_stride;   // mcts_ctree.py:352,364
-        io.reward = q->d_reward;
-        io.value = q->d_value;
-        io.policy_logits = q->d_policy;
-        io.pdl = pdl ? 1 : 0;
-        io.skip_scratch = q->d_skip;
-        if ((rc = model_recurrent(q->model, io, s))) { t->pdl = false; return rc; }
-        if (sim + 1 < q->S)
-            rc = tree_launch_backprop_traverse(t, sim + 1, q->d_reward, q->d_value, q->d_policy, deterministic, q->d_ix, q->d_action, s);
-        else
-            rc = tree_launch_backprop(t, sim + 1, q->d_reward, q->d_value, q->d_policy, nullptr, s);
-        if (rc) { t->pdl = false; return rc; }
+    TreeStep descent = {};
+    descent.traverse = 1; descent.deterministic = deterministic;
+    descent.act = q->d_action; descent.is_reset = q->d_is_reset;
+    if (reuse) {
+        descent.true_action = q->d_true_action; descent.reuse_value = q->d_reuse_value;
+        descent.ix_net = q->d_ix;
+    } else {
+        descent.ix = q->d_ix;
     }
-    t->pdl = false;
-    return LZ_OK;
-}
-
-// MuZeroMCTSCtree.search_with_reuse (mcts_ctree.py:370-468): every tree goes through the network every simulation (the
-// reference compacts the batch on the host; here the rows of "no inference" trees are computed and ignored, which keeps the
-// loop one static CUDA graph): [traverse_with_reuse] + S x [recurrent_inference, backpropagate_with_reuse (+ next traverse)].
-static int enqueue_search_reuse(lz_search *q, cudaStream_t s)
-{
-    int rc;
-    lz_tree *t = q->tree;
-    t->step_counter = 0;
-    if (q->hpool) {
-        // EfficientZeroMCTSCtree.search_with_reuse (mcts_ctree.py:878-1003): value-prefix trees, the LSTM step over all roots, is_reset
-        // per tree from the descent; [traverse_with_reuse] + S x [conv trunk + heads, LSTM value-prefix head, backpropagate_with_reuse,
-        // next traverse_with_reuse]
-        if ((rc = tree_launch_traverse_reuse(t, q->d_true_action, q->d_reuse_value, nullptr, q->d_ix, nullptr, q->d_action, nullptr, nullptr, s,
-                                             q->d_is_reset))) return rc;
-        for (int sim = 0; sim < q->S; ++sim) {
-            RecIO io;
-            memset(&io, 0, sizeof(io));
-            io.B = q->B; io.latent_base = q->pool; io.ix = q->d_ix; io.slot_stride = q->slot_stride; io.action = q->d_action;
-            io.next_latent = q->pool + (size_t)(sim + 1) * q->slot_stride;
-            io.reward = q->d_reward; io.value = q->d_value; io.policy_logits = q->d_policy;
-            io.h_base = q->hpool; io.c_base = q->cpool; io.hslot_stride = q->hslot_stride;
-            io.h_out = q->hpool + (size_t)(sim + 1) * q->hslot_stride; io.c_out = q->cpool + (size_t)(sim + 1) * q->hslot_stride;
-            io.is_reset = q->d_is_reset;
-            io.skip_scratch = q->d_skip;
-            if ((rc = model_recurrent(q->model, io, s))) return rc;
-            if ((rc = tree_launch_backprop_reuse(t, sim + 1, q->d_reward, q->d_value, q->d_policy, q->d_reuse_value, nullptr, nullptr, s,
-                                                 q->d_is_reset))) return rc;
-            if (sim + 1 < q->S &&
-                (rc = tree_launch_traverse_reuse(t, q->d_true_action, q->d_reuse_value, nullptr, q->d_ix, nullptr, q->d_action, nullptr, nullptr, s,
-                                                 q->d_is_reset))) return rc;
-        }
-        return LZ_OK;
-    }
-    if ((rc = tree_launch_traverse_reuse(t, q->d_true_action, q->d_reuse_value, nullptr, q->d_ix, nullptr, q->d_action, nullptr, nullptr, s))) return rc;
+    // the EfficientZero reuse back-up and the next descent are separate launches
+    const bool fuse = !(reuse && q->hpool);
+    if ((rc = tree_launch_step(t, descent, s))) return rc;
     for (int sim = 0; sim < q->S; ++sim) {
-        RecIO io;
-        memset(&io, 0, sizeof(io));
-        io.B = q->B; io.latent_base = q->pool; io.ix = q->d_ix; io.slot_stride = q->slot_stride; io.action = q->d_action;
-        io.next_latent = q->pool + (size_t)(sim + 1) * q->slot_stride;
-        io.reward = q->d_reward; io.value = q->d_value; io.policy_logits = q->d_policy;
-        io.skip_scratch = q->d_skip;
-        if ((rc = model_recurrent(q->model, io, s))) return rc;
-        if (sim + 1 < q->S)
-            rc = tree_launch_backprop_traverse_reuse(t, sim + 1, q->d_reward, q->d_value, q->d_policy, q->d_true_action, q->d_reuse_value,
-                                                     q->d_ix, q->d_action, s);
-        else
-            rc = tree_launch_backprop_reuse(t, sim + 1, q->d_reward, q->d_value, q->d_policy, q->d_reuse_value, nullptr, nullptr, s);
-        if (rc) return rc;
+        if ((rc = model_recurrent(q->model, rec_io(q, sim), s))) return rc;
+        const bool next = sim + 1 < q->S;
+        TreeStep step = descent;
+        step.traverse = next && fuse;
+        step.latent_index = sim + 1;
+        step.reward = q->d_reward; step.value = q->d_value; step.logits = q->d_policy; step.leaf_reset = q->d_is_reset;
+        if ((rc = tree_launch_step(t, step, s))) return rc;
+        if (next && !fuse && (rc = tree_launch_step(t, descent, s))) return rc;
     }
     return LZ_OK;
 }
 
-static int run_graph(lz_search *q, int deterministic, cudaStream_t s)
+static int run_graph(lz_search *q, int deterministic, bool reuse, cudaStream_t s)
 {
-    const int d = deterministic ? 1 : 0;
+    // an EfficientZero plain search breaks ties by p.tie_first (tracked by the tree generation), not by the flag: one graph
+    SearchGraph &g = q->graphs[reuse ? 2 : (deterministic || q->hpool) ? 1 : 0];
     // a captured graph bakes in device pointers of the model's tables (passed by value in TcNet / NetDev / EzNet), the math mode
     // and the tree parameters (TreeParams by value): re-capture when any of them changed since (weight reload, set_math,
-    // model_reserve growth, lz_tree_set_params / lz_tree_set_ez)
-    if (q->exec[d] && (q->gen_model[d] != q->model->generation || q->gen_tree[d] != q->tree->generation)) {
-        cudaGraphExecDestroy(q->exec[d]);
-        q->exec[d] = nullptr;
+    // model_reserve growth, lz_tree_set_params / lz_tree_set_ez / lz_tree_set_tiebreak)
+    if (g.exec && (g.gen_model != q->model->generation || g.gen_tree != q->tree->generation)) {
+        cudaGraphExecDestroy(g.exec);
+        g.exec = nullptr;
     }
-    if (!q->exec[d]) {
-        q->gen_model[d] = q->model->generation;
-        q->gen_tree[d] = q->tree->generation;
+    if (!g.exec) {
+        g.gen_model = q->model->generation;
+        g.gen_tree = q->tree->generation;
         cudaGraph_t graph = nullptr;
         if (!q->capture_stream) LZ_CUDA_CHECK(cudaStreamCreateWithFlags(&q->capture_stream, cudaStreamNonBlocking));
         LZ_CUDA_CHECK(cudaStreamBeginCapture(q->capture_stream, cudaStreamCaptureModeThreadLocal));
-        int rc = enqueue_search(q, deterministic, q->capture_stream);
+        int rc = enqueue_search(q, deterministic, reuse, q->capture_stream);
         cudaError_t e = cudaStreamEndCapture(q->capture_stream, &graph);
         if (rc != LZ_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
         if (e != cudaSuccess) { set_error("cudaStreamEndCapture failed: %s", cudaGetErrorString(e)); return LZ_ECUDA; }
         size_t n = 0;
         LZ_CUDA_CHECK(cudaGraphGetNodes(graph, nullptr, &n));
-        q->num_kernels = (int)n;
-        e = cudaGraphInstantiate(&q->exec[d], graph, 0);
+        g.num_kernels = (int)n;
+        e = cudaGraphInstantiate(&g.exec, graph, 0);
         cudaGraphDestroy(graph);
         if (e != cudaSuccess) { set_error("cudaGraphInstantiate failed: %s", cudaGetErrorString(e)); return LZ_ECUDA; }
     }
-    LZ_CUDA_CHECK(cudaGraphLaunch(q->exec[d], s));
-    count_launch(q->num_kernels);       // the graph's kernel nodes
+    LZ_CUDA_CHECK(cudaGraphLaunch(g.exec, s));
+    q->num_kernels = g.num_kernels;
+    count_launch(g.num_kernels);       // the graph's kernel nodes
     return LZ_OK;
+}
+
+static int copy_latent_roots(lz_search *q, const float *d_latent_roots, cudaStream_t s)
+{
+    if (d_latent_roots && d_latent_roots != q->pool)
+        LZ_CUDA_CHECK(cudaMemcpyAsync(q->pool, d_latent_roots, q->slot_stride * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    return LZ_OK;
+}
+
+static int ez_root_hidden(lz_search *q, const float *d_hidden0, const float *d_hidden1, cudaStream_t s)
+{
+    const size_t bytes = q->hslot_stride * sizeof(float);
+    if (d_hidden0) LZ_CUDA_CHECK(cudaMemcpyAsync(q->hpool, d_hidden0, bytes, cudaMemcpyDeviceToDevice, s));
+    else LZ_CUDA_CHECK(cudaMemsetAsync(q->hpool, 0, bytes, s));        // efficientzero_model.py:231-236: zeros after initial_inference
+    if (d_hidden1) LZ_CUDA_CHECK(cudaMemcpyAsync(q->cpool, d_hidden1, bytes, cudaMemcpyDeviceToDevice, s));
+    else LZ_CUDA_CHECK(cudaMemsetAsync(q->cpool, 0, bytes, s));
+    return LZ_OK;
+}
+
+static int run_with_reuse(lz_search *q, const float *d_latent_roots, const int32_t *d_true_action, const float *d_reuse_value,
+                          int32_t *d_infer_count, cudaStream_t s)
+{
+    if (!q->d_true_action) {
+        int rc = dev_alloc(&q->d_true_action, (size_t)q->B);
+        if (rc == LZ_OK) rc = dev_alloc(&q->d_reuse_value, (size_t)q->B);
+        if (rc != LZ_OK) return rc;
+    }
+    int rc = copy_latent_roots(q, d_latent_roots, s);
+    if (rc) return rc;
+    LZ_CUDA_CHECK(cudaMemcpyAsync(q->d_true_action, d_true_action, (size_t)q->B * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+    LZ_CUDA_CHECK(cudaMemcpyAsync(q->d_reuse_value, d_reuse_value, (size_t)q->B * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    LZ_CUDA_CHECK(cudaMemsetAsync(q->tree->p.infer_count, 0, (size_t)q->tree->p.N * sizeof(int), s));
+    if ((rc = run_graph(q, 0, true, s))) return rc;
+    if (d_infer_count)      // per simulation: how many trees needed the network (mcts_ctree.py:433,466-467)
+        LZ_CUDA_CHECK(cudaMemcpyAsync(d_infer_count, q->tree->p.infer_count, (size_t)q->S * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+    return LZ_OK;
+}
+
+// lz_search_collect*: reset the roots to the legal mask, prepare them from the initial inference's logits (+ noise), then search
+static int collect_search(lz_search *q, const uint8_t *d_mask, const float *d_logits, const float *d_noise, float noise_weight,
+                          const int32_t *d_to_play, int deterministic, cudaStream_t s)
+{
+    int rc;
+    if ((rc = lz_tree_reset_mask(q->tree, d_mask, s))) return rc;                // policy/muzero.py:760,769
+    if ((rc = lz_tree_prepare(q->tree, d_logits, d_noise, noise_weight, nullptr, d_to_play, s))) return rc;   // :774
+    if (q->hpool) {      // EfficientZero: zero LSTM state at the roots; the tree has no deterministic argument, the collect call's flag selects its tie-breaking
+        if ((rc = ez_root_hidden(q, nullptr, nullptr, s))) return rc;
+        if ((rc = lz_tree_set_tiebreak(q->tree, deterministic))) return rc;
+    }
+    return run_graph(q, deterministic, false, s);                                // :775
 }
 
 extern "C" {
@@ -243,7 +242,7 @@ int lz_search_create(lz_tree *t, lz_model *m, int num_simulations, lz_search **o
 int lz_search_destroy(lz_search *q)
 {
     if (!q) return LZ_OK;
-    for (int d = 0; d < 2; ++d) if (q->exec[d]) cudaGraphExecDestroy(q->exec[d]);
+    for (SearchGraph &g : q->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     if (q->capture_stream) cudaStreamDestroy(q->capture_stream);
     if (q->copy_stream) {
         cudaStreamDestroy(q->copy_stream);
@@ -256,18 +255,7 @@ int lz_search_destroy(lz_search *q)
     cudaFree(q->d_policy); cudaFree(q->d_root_logits); cudaFree(q->d_root_value); cudaFree(q->d_skip);
     cudaFree(q->hpool); cudaFree(q->cpool); cudaFree(q->d_is_reset);
     cudaFree(q->d_true_action); cudaFree(q->d_reuse_value);
-    if (q->exec_reuse) cudaGraphExecDestroy(q->exec_reuse);
     delete q;
-    return LZ_OK;
-}
-
-static int ez_root_hidden(lz_search *q, const float *d_hidden0, const float *d_hidden1, cudaStream_t s)
-{
-    const size_t bytes = q->hslot_stride * sizeof(float);
-    if (d_hidden0) LZ_CUDA_CHECK(cudaMemcpyAsync(q->hpool, d_hidden0, bytes, cudaMemcpyDeviceToDevice, s));
-    else LZ_CUDA_CHECK(cudaMemsetAsync(q->hpool, 0, bytes, s));        // efficientzero_model.py:231-236: zeros after initial_inference
-    if (d_hidden1) LZ_CUDA_CHECK(cudaMemcpyAsync(q->cpool, d_hidden1, bytes, cudaMemcpyDeviceToDevice, s));
-    else LZ_CUDA_CHECK(cudaMemsetAsync(q->cpool, 0, bytes, s));
     return LZ_OK;
 }
 
@@ -275,15 +263,11 @@ int lz_search_run_ez(lz_search *q, const float *d_latent_roots, const float *d_h
 {
     LZ_REQUIRE(q && q->hpool, LZ_EINVAL, "lz_search_run_ez: not an EfficientZero search");
     LZ_REQUIRE(q->tree->prepared, LZ_ESTATE, "lz_search_run_ez: roots not prepared (call lz_tree_prepare first)");
-    if (d_latent_roots && d_latent_roots != q->pool)
-        LZ_CUDA_CHECK(cudaMemcpyAsync(q->pool, d_latent_roots, q->slot_stride * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)s));
-    int rc = ez_root_hidden(q, d_hidden0_roots, d_hidden1_roots, (cudaStream_t)s);
+    int rc = copy_latent_roots(q, d_latent_roots, (cudaStream_t)s);
+    if (rc == LZ_OK) rc = ez_root_hidden(q, d_hidden0_roots, d_hidden1_roots, (cudaStream_t)s);
     if (rc) return rc;
-    return run_graph(q, 1, (cudaStream_t)s);
+    return run_graph(q, 1, false, (cudaStream_t)s);
 }
-
-static int run_with_reuse(lz_search *q, const float *d_latent_roots, const int32_t *d_true_action, const float *d_reuse_value,
-                          int32_t *d_infer_count, cudaStream_t s);
 
 int lz_search_run_with_reuse(lz_search *q, const float *d_latent_roots, const int32_t *d_true_action, const float *d_reuse_value,
                              int32_t *d_infer_count, lz_stream s_)
@@ -305,51 +289,14 @@ int lz_search_run_ez_with_reuse(lz_search *q, const float *d_latent_roots, const
     return run_with_reuse(q, d_latent_roots, d_true_action, d_reuse_value, d_infer_count, (cudaStream_t)s_);
 }
 
-static int run_with_reuse(lz_search *q, const float *d_latent_roots, const int32_t *d_true_action, const float *d_reuse_value,
-                          int32_t *d_infer_count, cudaStream_t s)
-{
-    if (!q->d_true_action) {
-        int rc = dev_alloc(&q->d_true_action, (size_t)q->B);
-        if (rc == LZ_OK) rc = dev_alloc(&q->d_reuse_value, (size_t)q->B);
-        if (rc != LZ_OK) return rc;
-    }
-    if (d_latent_roots && d_latent_roots != q->pool)
-        LZ_CUDA_CHECK(cudaMemcpyAsync(q->pool, d_latent_roots, q->slot_stride * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    LZ_CUDA_CHECK(cudaMemcpyAsync(q->d_true_action, d_true_action, (size_t)q->B * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
-    LZ_CUDA_CHECK(cudaMemcpyAsync(q->d_reuse_value, d_reuse_value, (size_t)q->B * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    LZ_CUDA_CHECK(cudaMemsetAsync(q->tree->p.infer_count, 0, (size_t)q->tree->p.N * sizeof(int), s));
-    if (q->exec_reuse && (q->gen_model[2] != q->model->generation || q->gen_tree[2] != q->tree->generation)) {
-        cudaGraphExecDestroy(q->exec_reuse);
-        q->exec_reuse = nullptr;
-    }
-    if (!q->exec_reuse) {
-        q->gen_model[2] = q->model->generation;
-        q->gen_tree[2] = q->tree->generation;
-        cudaGraph_t graph = nullptr;
-        if (!q->capture_stream) LZ_CUDA_CHECK(cudaStreamCreateWithFlags(&q->capture_stream, cudaStreamNonBlocking));
-        LZ_CUDA_CHECK(cudaStreamBeginCapture(q->capture_stream, cudaStreamCaptureModeThreadLocal));
-        int rc = enqueue_search_reuse(q, q->capture_stream);
-        cudaError_t e = cudaStreamEndCapture(q->capture_stream, &graph);
-        if (rc != LZ_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
-        if (e != cudaSuccess) { set_error("cudaStreamEndCapture failed: %s", cudaGetErrorString(e)); return LZ_ECUDA; }
-        e = cudaGraphInstantiate(&q->exec_reuse, graph, 0);
-        cudaGraphDestroy(graph);
-        if (e != cudaSuccess) { set_error("cudaGraphInstantiate failed: %s", cudaGetErrorString(e)); return LZ_ECUDA; }
-    }
-    LZ_CUDA_CHECK(cudaGraphLaunch(q->exec_reuse, s));
-    if (d_infer_count)      // per simulation: how many trees needed the network (mcts_ctree.py:433,466-467)
-        LZ_CUDA_CHECK(cudaMemcpyAsync(d_infer_count, q->tree->p.infer_count, (size_t)q->S * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
-    return LZ_OK;
-}
-
 int lz_search_run(lz_search *q, const float *d_latent_roots, int deterministic, lz_stream s)
 {
     LZ_REQUIRE(q, LZ_EINVAL, "lz_search_run: null search");
     LZ_REQUIRE(!q->hpool, LZ_ESTATE, "lz_search_run: EfficientZero search, use lz_search_run_ez");
     LZ_REQUIRE(q->tree->prepared, LZ_ESTATE, "lz_search_run: roots not prepared (call lz_tree_prepare first)");
-    if (d_latent_roots && d_latent_roots != q->pool)
-        LZ_CUDA_CHECK(cudaMemcpyAsync(q->pool, d_latent_roots, q->slot_stride * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)s));
-    return run_graph(q, deterministic, (cudaStream_t)s);
+    int rc = copy_latent_roots(q, d_latent_roots, (cudaStream_t)s);
+    if (rc) return rc;
+    return run_graph(q, deterministic, false, (cudaStream_t)s);
 }
 
 static int collect_device(lz_search *q, const float *d_obs, const uint8_t *d_obs_u8, const uint8_t *d_mask, const float *d_noise,
@@ -373,13 +320,7 @@ static int collect_device(lz_search *q, const float *d_obs, const uint8_t *d_obs
         rc = model_initial(q->model, q->B, d_obs, io, (cudaStream_t)s);          // policy/muzero.py:749
     }
     if (rc) return rc;
-    if ((rc = lz_tree_reset_mask(q->tree, d_mask, s))) return rc;                // :760,769
-    if ((rc = lz_tree_prepare(q->tree, io.policy_logits, d_noise, noise_weight, nullptr, d_to_play, s))) return rc;   // :774
-    if (q->hpool) {      // EfficientZero: zero LSTM state at the roots; the tree has no deterministic argument, the collect call's flag selects its tie-breaking
-        if ((rc = ez_root_hidden(q, nullptr, nullptr, (cudaStream_t)s))) return rc;
-        if ((rc = lz_tree_set_tiebreak(q->tree, deterministic))) return rc;
-    }
-    return run_graph(q, deterministic, (cudaStream_t)s);                         // :775
+    return collect_search(q, d_mask, io.policy_logits, d_noise, noise_weight, d_to_play, deterministic, (cudaStream_t)s);
 }
 
 int lz_search_collect(lz_search *q, const float *d_obs, const uint8_t *d_mask, const float *d_noise, float noise_weight,
@@ -424,12 +365,11 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
     LZ_CUDA_CHECK(cudaEventRecord(q->ev_start, s));
     LZ_CUDA_CHECK(cudaStreamWaitEvent(q->copy_stream, q->ev_start, 0));
     LZ_CUDA_CHECK(cudaStreamWaitEvent(q->copy_stream2, q->ev_start, 0));
-    const bool two = !getenv("LZ_ONE_COPY_STREAM");
     const int per = (B + nchunks - 1) / nchunks;
     for (int i = 0; i < nchunks; ++i) {
         const int b0 = i * per, bc = std::min(per, B - b0);
         if (bc <= 0) { nchunks = i; break; }
-        cudaStream_t cs = (two && (i & 1)) ? q->copy_stream2 : q->copy_stream;
+        cudaStream_t cs = (i & 1) ? q->copy_stream2 : q->copy_stream;
         LZ_CUDA_CHECK(cudaMemcpyAsync(reinterpret_cast<unsigned char *>(q->d_obs_stage) + (size_t)b0 * q->obs_elems * esz,
                                       static_cast<const unsigned char *>(h_obs) + (size_t)b0 * q->obs_elems * esz,
                                       (size_t)bc * q->obs_elems * esz, cudaMemcpyHostToDevice, cs));
@@ -468,15 +408,8 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
         int rc = model_initial_tail(q->model, B, q->d_pre_stage, io, s);
         if (rc) return rc;
     }
-    int rc;
-    if ((rc = lz_tree_reset_mask(q->tree, h_mask ? q->d_mask_stage : nullptr, s))) return rc;
-    if ((rc = lz_tree_prepare(q->tree, logits, h_noise ? q->d_noise_stage : nullptr, noise_weight, nullptr,
-                              h_to_play ? q->d_tp_stage : nullptr, s))) return rc;
-    if (q->hpool) {
-        if ((rc = ez_root_hidden(q, nullptr, nullptr, s))) return rc;
-        if ((rc = lz_tree_set_tiebreak(q->tree, deterministic))) return rc;
-    }
-    return run_graph(q, deterministic, s);
+    return collect_search(q, h_mask ? q->d_mask_stage : nullptr, logits, h_noise ? q->d_noise_stage : nullptr, noise_weight,
+                          h_to_play ? q->d_tp_stage : nullptr, deterministic, s);
 }
 
 int lz_search_collect_host(lz_search *q, const float *h_obs, const uint8_t *h_mask, const float *h_noise, float noise_weight,

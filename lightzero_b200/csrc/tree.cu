@@ -9,7 +9,6 @@
 
 #include "lz_common.cuh"
 #include "tree.cuh"
-#include "tc_ptx.cuh"
 
 namespace lz {
 
@@ -105,80 +104,32 @@ k_tree_prepare(TreeParams p, const float *logits, const float *noise, float nois
     }
 }
 
-template <bool EZ>
+// One simulation boundary of every tree: the back-up of the last expansion, then the next descent (see TreeStep).  Fusing
+// both into one launch halves the tree launches of a search graph.
+template <bool EZ, bool REUSE>
 __global__ void __launch_bounds__(kTreeBlock)
-k_tree_traverse(TreeParams p, int deterministic, unsigned step, int32_t *ix, int32_t *iy, int32_t *act,
-                int32_t *len, int32_t *vtp, int32_t *is_reset)
-{
-    const int b = blockIdx.x * (kTreeBlock / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    pdl_launch_dependents();
-    pdl_wait();
-    if (b >= p.B) return;
-    tree_traverse<EZ>(p, b, lane, deterministic, step, ix, iy, act, len, vtp);
-    // mcts_ctree.py:856-861: the LSTM state of a leaf is reset every lstm_horizon_len steps of depth
-    if (EZ && is_reset && lane == 0) is_reset[b] = (p.search_len[b] % p.lstm_horizon == 0) ? 1 : 0;
-}
-
-template <bool EZ>
-__global__ void __launch_bounds__(kTreeBlock)
-k_tree_backprop(TreeParams p, int latent_index, const float *reward, const float *value, const float *logits,
-                const int32_t *to_play, const int32_t *is_reset)
-{
-    const int b = blockIdx.x * (kTreeBlock / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    pdl_launch_dependents();
-    pdl_wait();
-    if (b >= p.B) return;
-    tree_backprop<EZ>(p, b, lane, latent_index, reward[b], value[b], logits + (size_t)b * p.A, to_play,
-                      (EZ && is_reset) ? is_reset[b] : 0);
-}
-
-template <bool EZ>
-__global__ void __launch_bounds__(kTreeBlock)
-k_tree_backprop_traverse(TreeParams p, int latent_index, const float *reward, const float *value,
-                         const float *logits, int deterministic, unsigned step, int32_t *ix, int32_t *act, int32_t *is_reset)
-{
-    const int b = blockIdx.x * (kTreeBlock / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    pdl_launch_dependents();      // lets the next network kernel set up (barriers, first weight taps) meanwhile
-    pdl_wait();                   // reward / value / logits come from the preceding network kernel
-    if (b >= p.B) return;
-    tree_backprop<EZ>(p, b, lane, latent_index, reward[b], value[b], logits + (size_t)b * p.A, nullptr,
-                      (EZ && is_reset) ? is_reset[b] : 0);
-    tree_traverse<EZ>(p, b, lane, deterministic, step, ix, nullptr, act, nullptr, nullptr);
-    if (EZ && is_reset && lane == 0) is_reset[b] = (p.search_len[b] % p.lstm_horizon == 0) ? 1 : 0;
-}
-
-// ---- ReZero search_with_reuse (MuZero trees) ----
-template <bool EZ>
-__global__ void __launch_bounds__(kTreeBlock)
-k_tree_traverse_reuse(TreeParams p, unsigned step, const int32_t *true_action, const float *reuse_value, int32_t *ix, int32_t *ix_net,
-                      int32_t *iy, int32_t *act, int32_t *len, int32_t *vtp, int32_t *is_reset)
+k_tree_step(TreeParams p, TreeStep a)
 {
     const int b = blockIdx.x * (kTreeBlock / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (b >= p.B) return;
-    tree_traverse<EZ, true>(p, b, lane, p.tie_first, step, ix, iy, act, len, vtp, true_action, reuse_value, ix_net);
-    // EfficientZero, fused search: is_reset of the reached node per TREE (mcts_ctree.py:856-861 / 1040-1046: search_len % lstm_horizon_len)
-    if (EZ && is_reset && lane == 0) is_reset[b] = (p.search_len[b] % p.lstm_horizon == 0) ? 1 : 0;
-}
-
-template <bool EZ>
-__global__ void __launch_bounds__(kTreeBlock)
-k_tree_backprop_reuse(TreeParams p, int latent_index, const float *reward, const float *value, const float *logits,
-                      const float *reuse_value, const int32_t *batch_rank, const int32_t *to_play, const int32_t *is_reset)
-{
-    const int b = blockIdx.x * (kTreeBlock / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (b >= p.B) return;
-    tree_backprop<EZ, true>(p, b, lane, latent_index, reward[b], value[b], logits + (size_t)b * p.A, to_play,
-                            (EZ && is_reset) ? is_reset[b] : 0, reuse_value[b], batch_rank ? batch_rank[b] : -1);
-}
-
-__global__ void __launch_bounds__(kTreeBlock)
-k_tree_backprop_traverse_reuse(TreeParams p, int latent_index, const float *reward, const float *value, const float *logits,
-                               unsigned step, const int32_t *true_action, const float *reuse_value, int32_t *ix_net, int32_t *act)
-{
-    const int b = blockIdx.x * (kTreeBlock / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (b >= p.B) return;
-    tree_backprop<false, true>(p, b, lane, latent_index, reward[b], value[b], logits + (size_t)b * p.A, nullptr, 0, reuse_value[b], -1);
-    tree_traverse<false, true>(p, b, lane, p.tie_first, step, nullptr, nullptr, act, nullptr, nullptr, true_action, reuse_value, ix_net);
+    if (a.latent_index > 0)
+        tree_backprop<EZ, REUSE>(p, b, lane, a.latent_index, a.reward[b], a.value[b], a.logits + (size_t)b * p.A, a.to_play,
+                                 (EZ && a.leaf_reset) ? a.leaf_reset[b] : 0, REUSE ? a.reuse_value[b] : 0.0f,
+                                 (REUSE && a.batch_rank) ? a.batch_rank[b] : -1);
+    if (a.traverse) {
+        tree_traverse<EZ, REUSE>(p, b, lane, a.deterministic, a.step, a.ix, a.act, a.true_action, a.reuse_value, a.ix_net);
+        if (lane == 0) {
+            const int len = p.search_len[b];
+            // batch_index (cnode.cpp:907-923): recorded on the node the descent ended in (the last path entry), or this tree after a
+            // reuse stop on an already expanded child
+            if (a.iy)
+                a.iy[b] = (REUSE && p.reuse_state[b] != 2) ? p.n_batch[(size_t)b * p.N + p.path_slot[(size_t)b * p.N + len - 1]] : b;
+            if (a.len) a.len[b] = len;
+            if (a.vtp) a.vtp[b] = p.vtp[b];
+            // mcts_ctree.py:856-861 / 1040-1046: the LSTM state of a leaf is reset every lstm_horizon_len steps of depth (per tree)
+            if (EZ && a.is_reset) a.is_reset[b] = (len % p.lstm_horizon == 0) ? 1 : 0;
+        }
+    }
 }
 
 // get_distributions / get_values / get_trajectories (cnode.cpp:237-277,369-417)
@@ -262,90 +213,22 @@ k_tree_select_action(TreeParams p, double inv_temperature, int deterministic, un
 
 static inline dim3 tree_grid(int B) { return dim3(ceil_div(B, kTreeBlock / 32)); }
 
-template <typename... KArgs, typename... Args>
-static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, cudaStream_t s, bool pdl, Args... args)
+int tree_launch_step(lz_tree *t, const TreeStep &a_in, cudaStream_t s)
 {
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = grid; cfg.blockDim = dim3(kTreeBlock); cfg.dynamicSmemBytes = 0; cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    count_launch();
-    return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-
-int tree_launch_traverse(lz_tree *t, int deterministic, int32_t *d_ix, int32_t *d_iy, int32_t *d_action,
-                         int32_t *d_len, int32_t *d_vtp, cudaStream_t s, int32_t *d_is_reset)
-{
-    if (t->p.ez)
-        LZ_CUDA_CHECK(launch_pdl(k_tree_traverse<true>, tree_grid(t->p.B), s, t->pdl, t->p, deterministic, t->step_counter++, d_ix, d_iy,
-                                 d_action, d_len, d_vtp, d_is_reset));
-    else
-        LZ_CUDA_CHECK(launch_pdl(k_tree_traverse<false>, tree_grid(t->p.B), s, t->pdl, t->p, deterministic, t->step_counter++, d_ix, d_iy,
-                                 d_action, d_len, d_vtp, d_is_reset));
-    return LZ_OK;
-}
-
-int tree_launch_backprop(lz_tree *t, int latent_index, const float *d_reward, const float *d_value,
-                         const float *d_logits, const int32_t *d_to_play, cudaStream_t s, const int32_t *d_is_reset)
-{
-    if (t->p.ez)
-        LZ_CUDA_CHECK(launch_pdl(k_tree_backprop<true>, tree_grid(t->p.B), s, t->pdl, t->p, latent_index, d_reward, d_value, d_logits,
-                                 d_to_play, d_is_reset));
-    else
-        LZ_CUDA_CHECK(launch_pdl(k_tree_backprop<false>, tree_grid(t->p.B), s, t->pdl, t->p, latent_index, d_reward, d_value, d_logits,
-                                 d_to_play, d_is_reset));
-    return LZ_OK;
-}
-
-int tree_launch_backprop_traverse(lz_tree *t, int latent_index, const float *d_reward, const float *d_value,
-                                  const float *d_logits, int deterministic, int32_t *d_ix, int32_t *d_action,
-                                  cudaStream_t s, int32_t *d_is_reset)
-{
-    if (t->p.ez)
-        LZ_CUDA_CHECK(launch_pdl(k_tree_backprop_traverse<true>, tree_grid(t->p.B), s, t->pdl, t->p, latent_index, d_reward, d_value,
-                                 d_logits, deterministic, t->step_counter++, d_ix, d_action, d_is_reset));
-    else
-        LZ_CUDA_CHECK(launch_pdl(k_tree_backprop_traverse<false>, tree_grid(t->p.B), s, t->pdl, t->p, latent_index, d_reward, d_value,
-                                 d_logits, deterministic, t->step_counter++, d_ix, d_action, d_is_reset));
-    return LZ_OK;
-}
-
-int tree_launch_traverse_reuse(lz_tree *t, const int32_t *d_true_action, const float *d_reuse_value, int32_t *d_ix, int32_t *d_ix_net,
-                               int32_t *d_iy, int32_t *d_action, int32_t *d_len, int32_t *d_vtp, cudaStream_t s, int32_t *d_is_reset)
-{
-    if (t->p.ez)
-        k_tree_traverse_reuse<true><<<tree_grid(t->p.B), kTreeBlock, 0, s>>>(t->p, t->step_counter++, d_true_action, d_reuse_value, d_ix, d_ix_net,
-                                                                            d_iy, d_action, d_len, d_vtp, d_is_reset);
-    else
-        k_tree_traverse_reuse<false><<<tree_grid(t->p.B), kTreeBlock, 0, s>>>(t->p, t->step_counter++, d_true_action, d_reuse_value, d_ix, d_ix_net,
-                                                                             d_iy, d_action, d_len, d_vtp, nullptr);
-    LZ_KERNEL_CHECK();
-    return LZ_OK;
-}
-
-int tree_launch_backprop_reuse(lz_tree *t, int latent_index, const float *d_reward, const float *d_value, const float *d_logits,
-                               const float *d_reuse_value, const int32_t *d_batch_rank, const int32_t *d_to_play, cudaStream_t s,
-                               const int32_t *d_is_reset)
-{
-    if (t->p.ez)
-        k_tree_backprop_reuse<true><<<tree_grid(t->p.B), kTreeBlock, 0, s>>>(t->p, latent_index, d_reward, d_value, d_logits, d_reuse_value,
-                                                                            d_batch_rank, d_to_play, d_is_reset);
-    else
-        k_tree_backprop_reuse<false><<<tree_grid(t->p.B), kTreeBlock, 0, s>>>(t->p, latent_index, d_reward, d_value, d_logits, d_reuse_value,
-                                                                             d_batch_rank, d_to_play, d_is_reset);
-    LZ_KERNEL_CHECK();
-    return LZ_OK;
-}
-
-int tree_launch_backprop_traverse_reuse(lz_tree *t, int latent_index, const float *d_reward, const float *d_value, const float *d_logits,
-                                        const int32_t *d_true_action, const float *d_reuse_value, int32_t *d_ix_net, int32_t *d_action,
-                                        cudaStream_t s)
-{
-    k_tree_backprop_traverse_reuse<<<tree_grid(t->p.B), kTreeBlock, 0, s>>>(t->p, latent_index, d_reward, d_value, d_logits,
-                                                                           t->step_counter++, d_true_action, d_reuse_value, d_ix_net, d_action);
+    TreeStep a = a_in;
+    const bool reuse = a.reuse_value != nullptr;
+    if (a.traverse) {
+        if (t->p.ez || reuse) a.deterministic = t->p.tie_first;
+        a.step = t->step_counter++;
+    }
+    const dim3 grid = tree_grid(t->p.B);
+    if (t->p.ez) {
+        if (reuse) k_tree_step<true, true><<<grid, kTreeBlock, 0, s>>>(t->p, a);
+        else k_tree_step<true, false><<<grid, kTreeBlock, 0, s>>>(t->p, a);
+    } else {
+        if (reuse) k_tree_step<false, true><<<grid, kTreeBlock, 0, s>>>(t->p, a);
+        else k_tree_step<false, false><<<grid, kTreeBlock, 0, s>>>(t->p, a);
+    }
     LZ_KERNEL_CHECK();
     return LZ_OK;
 }
@@ -474,8 +357,10 @@ int lz_tree_traverse(lz_tree *t, int deterministic, int32_t *d_ix, int32_t *d_iy
     LZ_REQUIRE(t, LZ_EINVAL, "lz_tree_traverse: null tree");
     LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_traverse: roots not prepared (call lz_tree_prepare first)");
     LZ_REQUIRE(!t->p.ez, LZ_ESTATE, "lz_tree_traverse: tree is in EfficientZero mode, use lz_tree_traverse_ez");
-    return tree_launch_traverse(t, deterministic, d_ix, d_iy, d_last_action, d_search_len, d_virtual_to_play,
-                                (cudaStream_t)s);
+    TreeStep a = {};
+    a.traverse = 1; a.deterministic = deterministic;
+    a.ix = d_ix; a.iy = d_iy; a.act = d_last_action; a.len = d_search_len; a.vtp = d_virtual_to_play;
+    return tree_launch_step(t, a, (cudaStream_t)s);
 }
 
 int lz_tree_backpropagate(lz_tree *t, int latent_index, const float *d_reward, const float *d_value,
@@ -486,7 +371,9 @@ int lz_tree_backpropagate(lz_tree *t, int latent_index, const float *d_reward, c
     LZ_REQUIRE(!t->p.ez, LZ_ESTATE, "lz_tree_backpropagate: tree is in EfficientZero mode, use lz_tree_backpropagate_ez");
     LZ_REQUIRE(latent_index >= 1 && latent_index <= t->max_sims, LZ_EINVAL,
                "lz_tree_backpropagate: latent_index %d outside [1, %d]", latent_index, t->max_sims);
-    return tree_launch_backprop(t, latent_index, d_reward, d_value, d_logits, d_to_play, (cudaStream_t)s);
+    TreeStep a = {};
+    a.latent_index = latent_index; a.reward = d_reward; a.value = d_value; a.logits = d_logits; a.to_play = d_to_play;
+    return tree_launch_step(t, a, (cudaStream_t)s);
 }
 
 int lz_tree_set_ez(lz_tree *t, int efficientzero, int lstm_horizon_len)
@@ -514,7 +401,10 @@ int lz_tree_traverse_ez(lz_tree *t, int32_t *d_ix, int32_t *d_iy, int32_t *d_las
 {
     LZ_REQUIRE(t && t->p.ez, LZ_ESTATE, "lz_tree_traverse_ez: tree is not in EfficientZero mode (lz_tree_set_ez)");
     LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_traverse_ez: roots not prepared (call lz_tree_prepare first)");
-    return tree_launch_traverse(t, t->p.tie_first, d_ix, d_iy, d_last_action, d_search_len, d_virtual_to_play, (cudaStream_t)s, d_is_reset);
+    TreeStep a = {};
+    a.traverse = 1;
+    a.ix = d_ix; a.iy = d_iy; a.act = d_last_action; a.len = d_search_len; a.vtp = d_virtual_to_play; a.is_reset = d_is_reset;
+    return tree_launch_step(t, a, (cudaStream_t)s);
 }
 
 int lz_tree_backpropagate_ez(lz_tree *t, int latent_index, const float *d_value_prefix, const float *d_value,
@@ -525,7 +415,10 @@ int lz_tree_backpropagate_ez(lz_tree *t, int latent_index, const float *d_value_
     LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_backpropagate_ez: roots not prepared");
     LZ_REQUIRE(latent_index >= 1 && latent_index <= t->max_sims, LZ_EINVAL,
                "lz_tree_backpropagate_ez: latent_index %d outside [1, %d]", latent_index, t->max_sims);
-    return tree_launch_backprop(t, latent_index, d_value_prefix, d_value, d_logits, d_to_play, (cudaStream_t)s, d_is_reset);
+    TreeStep a = {};
+    a.latent_index = latent_index; a.reward = d_value_prefix; a.value = d_value; a.logits = d_logits; a.to_play = d_to_play;
+    a.leaf_reset = d_is_reset;
+    return tree_launch_step(t, a, (cudaStream_t)s);
 }
 
 int lz_tree_traverse_with_reuse(lz_tree *t, const int32_t *d_true_action, const float *d_reuse_value, int32_t *d_ix, int32_t *d_iy,
@@ -533,8 +426,10 @@ int lz_tree_traverse_with_reuse(lz_tree *t, const int32_t *d_true_action, const 
 {
     LZ_REQUIRE(t && d_true_action && d_reuse_value, LZ_EINVAL, "lz_tree_traverse_with_reuse: null argument");
     LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_traverse_with_reuse: roots not prepared");
-    return tree_launch_traverse_reuse(t, d_true_action, d_reuse_value, d_ix, nullptr, d_iy, d_last_action, d_search_len, d_virtual_to_play,
-                                      (cudaStream_t)s);
+    TreeStep a = {};
+    a.traverse = 1; a.true_action = d_true_action; a.reuse_value = d_reuse_value;
+    a.ix = d_ix; a.iy = d_iy; a.act = d_last_action; a.len = d_search_len; a.vtp = d_virtual_to_play;
+    return tree_launch_step(t, a, (cudaStream_t)s);
 }
 
 int lz_tree_backpropagate_with_reuse(lz_tree *t, int latent_index, const float *d_reward, const float *d_value, const float *d_logits,
@@ -546,8 +441,10 @@ int lz_tree_backpropagate_with_reuse(lz_tree *t, int latent_index, const float *
     LZ_REQUIRE(!t->p.ez || d_is_reset, LZ_EINVAL, "lz_tree_backpropagate_with_reuse: EfficientZero trees need d_is_reset");
     LZ_REQUIRE(latent_index >= 1 && latent_index <= t->max_sims, LZ_EINVAL,
                "lz_tree_backpropagate_with_reuse: latent_index %d outside [1, %d]", latent_index, t->max_sims);
-    return tree_launch_backprop_reuse(t, latent_index, d_reward, d_value, d_logits, d_reuse_value, d_batch_rank, d_to_play, (cudaStream_t)s,
-                                      d_is_reset);
+    TreeStep a = {};
+    a.latent_index = latent_index; a.reward = d_reward; a.value = d_value; a.logits = d_logits; a.to_play = d_to_play;
+    a.leaf_reset = d_is_reset; a.batch_rank = d_batch_rank; a.reuse_value = d_reuse_value;
+    return tree_launch_step(t, a, (cudaStream_t)s);
 }
 
 int lz_tree_select_action(lz_tree *t, float temperature, int deterministic, uint64_t seed, int32_t *d_action,

@@ -139,6 +139,7 @@ class MuZeroMCTSCtree(object):
         with torch.cuda.device(dev):
             cabi.check(t.lib.lz_search_run_with_reuse(q, lat.data_ptr(), ta.data_ptr(), rv.data_ptr(), counts.data_ptr(),
                                                       cabi.stream_ptr()), "lz_search_run_with_reuse")
+        self.last_num_kernels = t.lib.lz_search_num_kernels(q)
         c = counts.cpu().numpy()
         return int(c[-1]), float(c.sum()) / S
 
@@ -263,6 +264,7 @@ class EfficientZeroMCTSCtree(MuZeroMCTSCtree):
         with torch.cuda.device(dev):
             cabi.check(t.lib.lz_search_run_ez_with_reuse(q, lat.data_ptr(), h0.data_ptr(), h1.data_ptr(), ta.data_ptr(), rv.data_ptr(),
                                                          counts.data_ptr(), cabi.stream_ptr()), "lz_search_run_ez_with_reuse")
+        self.last_num_kernels = t.lib.lz_search_num_kernels(q)
         c = counts.cpu().numpy()
         return int(c[-1]), float(c.sum()) / S
 

@@ -46,7 +46,6 @@ def main():
         rb = dyn.resblocks[0]
         exp_c1 = rb.conv1(latent)          # relu(bn(conv(x)))
     for variant in (0,):
-        os.environ["LZ_TC_VARIANT"] = str(variant)
         print(f"==== descriptor variant {variant} ====")
         cu.set_math("tc3")
         try:
@@ -64,7 +63,6 @@ def main():
         except Exception as e:
             print("variant", variant, "FAILED:", repr(e))
             return
-    os.environ["LZ_TC_VARIANT"] = os.environ.get("DBG_VARIANT", "0")
     # full network
     cu2 = lzb.MuZeroModel(observation_shape=(4, 84, 84), action_space_size=A).load_state_dict(ref.state_dict())
     with torch.no_grad():

@@ -1,5 +1,5 @@
 """Times the fused MuZero search (bench size by default) with CUDA events, uninstrumented: the A/B tool for kernel variants
-(LZ_LIB_TAG=<tag> picks lightzero_b200/_lib/<tag>/liblzb200.so; LZ_TC_ROOTS is read by tc_launch at graph capture)."""
+(LZ_LIB_TAG=<tag> picks lightzero_b200/_lib/<tag>/liblzb200.so)."""
 import os
 import sys
 

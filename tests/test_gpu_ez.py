@@ -243,6 +243,8 @@ def test_fused_ez_search_with_reuse_equals_piecewise_drive():
     assert fused == step
     assert length == counts[-1] and abs(avg - sum(counts) / S) < 1e-9
     assert min(counts) < B
+    # traverse + S x (conv trunk, LSTM GEMM, value-prefix head, back-up) + (S - 1) x traverse
+    assert mcts.last_num_kernels == 5 * S
 
 
 def test_ez_stochastic_tiebreak_is_legal_and_reproducible():

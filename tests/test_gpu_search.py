@@ -42,7 +42,7 @@ class _Recorder:
 
 
 @pytest.mark.parametrize("math", ["fp32", "tc3"])
-@pytest.mark.parametrize("B,A,S,masks", [(16, 6, 20, False), (300, 18, 50, True), (1024, 6, 50, False)])
+@pytest.mark.parametrize("B,A,S,masks", [(16, 6, 20, False), (300, 18, 50, True), (1024, 6, 50, False), (64, 40, 20, True)])
 def test_fused_graph_search_equals_stepwise_search(B, A, S, masks, math):
     """The single-graph search and the one-simulation-at-a-time drive of the same kernels must agree
     exactly: visit counts, root values (bits), and repeated graph launches must be reproducible."""
@@ -57,8 +57,8 @@ def test_fused_graph_search_equals_stepwise_search(B, A, S, masks, math):
         roots.clear()
     assert results[0] == results[1] == results[2]
     assert all(sum(d) == S for d in results[0][0])
-    # one persistent launch (tensor-core path) or [traverse] + S x [network, backprop(+traverse)] kernels
-    assert mcts.last_num_kernels in (1, 2 * S + 1)
+    # tensor-core path with A <= 32: one persistent launch; else [traverse] + S x [network, backprop(+traverse)] kernels
+    assert mcts.last_num_kernels == (1 if math == "tc3" and A <= 32 else 2 * S + 1)
 
 
 def test_search_accepts_numpy_latents_and_host_lists():
@@ -284,6 +284,7 @@ def test_fused_search_with_reuse_equals_stepwise_drive():
     assert fused == step
     assert length == counts[-1] and abs(avg - sum(counts) / S) < 1e-9
     assert min(counts) < B       # some trees reused a value instead of calling the network
+    assert mcts.last_num_kernels == 1 + 2 * S     # traverse + S x (network, back-up(+traverse))
 
 
 def test_uint8_frames_equal_scaled_float_frames_bit_for_bit():
