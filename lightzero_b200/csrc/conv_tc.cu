@@ -3,7 +3,8 @@
 // memory once, then for each 128-row tile runs 9 taps x (Cin/16) k-steps x 3 fp16 hi/lo passes of wgmma (two warpgroups, 64 rows
 // each, accumulators in registers) with row-shifted descriptors; the taps stream through a ring once per tile (L2-resident, 4-16 KB
 // each).  The epilogue applies BN / residual / ReLU straight from the accumulator fragments and writes the next layer's TCL tensor
-// (already split into fp16 hi/lo).
+// (already split into fp16 hi/lo).  k_resblock_tc runs both convs of a plain ResBlock the same way, with conv1's output kept in
+// shared memory.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -59,8 +60,8 @@ __device__ __forceinline__ void store_split2(unsigned char *hi_ptr, unsigned cha
 }
 
 template <int N>
-// N <= 64: <= 112 registers (32 or 16 accumulators per thread), so two CTAs can share an SM and overlap one CTA's band load /
-// epilogue with the other's MMAs; N = 128 needs 64 accumulators per thread and runs one CTA per SM
+// N = 64: <= 112 registers (32 accumulators per thread), so two CTAs can share an SM and overlap one CTA's band load / epilogue
+// with the other's MMAs; N = 128 needs 64 accumulators per thread and runs one CTA per SM
 __global__ void __launch_bounds__(kCvThreads, N == 128 ? 1 : 2) k_conv_tc(ConvTc p)
 {
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -165,19 +166,6 @@ __global__ void __launch_bounds__(kCvThreads, N == 128 ? 1 : 2) k_conv_tc(ConvTc
                 const int c = col - grp * 64;                     // channel within the output tensor
                 const Tcl &o = p.out[grp];
                 const bool relu = p.relu[grp] != 0;
-                size_t obase = 0;
-                bool do_write = in_band;
-                if (in_band) {
-                    if (o.nphase == 1) {
-                        obase = (size_t)(img0 + k) * o.img_stride + (size_t)(rho + 1) * 16;
-                    } else if (valid) {                  // phase-split output for a stride-2 consumer
-                        const int ph = (yy & 1) * 2 + (xx & 1);
-                        const int rho2 = ((yy >> 1) + 1) * o.pitch + (xx >> 1);
-                        obase = (size_t)(img0 + k) * o.img_stride + ph * o.phase_stride + (size_t)(rho2 + 1) * 16;
-                    } else {
-                        do_write = false;
-                    }
-                }
                 float v0 = fmaf(acc[4 * j + 2 * hr], __ldg(p.scale + col), __ldg(p.shift + col));
                 float v1 = fmaf(acc[4 * j + 2 * hr + 1], __ldg(p.scale + col + 1), __ldg(p.shift + col + 1));
                 if (p.res.base && grp == 0 && valid) {
@@ -190,8 +178,249 @@ __global__ void __launch_bounds__(kCvThreads, N == 128 ? 1 : 2) k_conv_tc(ConvTc
                 }
                 v0 = valid ? (relu ? fmaxf(v0, 0.0f) : v0) : 0.0f;
                 v1 = valid ? (relu ? fmaxf(v1, 0.0f) : v1) : 0.0f;
+                if (in_band) {
+                    unsigned char *op = o.base + (size_t)(img0 + k) * o.img_stride + ((size_t)(c >> 3) * o.plane_rows + rho + 1) * 16 + (c & 7) * 2;
+                    store_split2(op, op + o.part_stride, v0, v1);
+                }
+            }
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------- fused ResBlock
+// k_resblock_tc runs relu(bn2(conv2(relu(bn1(conv1(x))))) + x) for one band of h output rows (or G whole images) per CTA.  Both
+// shared-memory buffers use the TCL plane layout with a per-image stride of S = (h + 4) pitch + 2 rows:
+//   input x:          row j of image k = memory row (y0 - 1) pitch + j - k S,  i.e. image rows [y0 - 2, y0 + h + 2)
+//   intermediate t1:  row i of image k = memory row y0 pitch + i - k S,        i.e. image rows [y0 - 1, y0 + h + 1)
+// conv1 computes the h + 2 rows [y0 - 1, y0 + h] (the halo rows conv2 needs are recomputed) exactly like k_conv_tc on the band
+// (y0 - 1, h + 2): its output row m is t1 row m - pitch, stored as fp16 hi/lo, and rows outside the image (or the pad column) are
+// stored as zeros, so conv2 reads t1 through the same row-shifted descriptors as an HBM band.  conv2's output row m takes its
+// residual from x row m + pitch.  Each output row's sums run in the same tap -> k-step -> pass order as two k_conv_tc launches,
+// and t1 holds the same fp16 split they pass through HBM, so the results are bit-identical to them.
+// The input band lands in 128-row chunks, each with its own mbarrier: conv1's first pair of tiles starts once its rows are in,
+// while the rest of the band is still loading (with ~200 KB of shared memory per CTA, no second CTA can hide the load).
+// Reads past a buffer's last plane (only by tile rows past the last useful one, < 128 rows) land in the next buffer or the ring.
+constexpr int kRbChunks = 16;
+
+struct RbBars {
+    uint64_t full[kCvStages], empty[kCvStages];
+    uint64_t chunk[kRbChunks];
+};
+
+struct RbGeom {                   // identical on host (shared-memory size, band picker) and device
+    int nbands, S, m_lo, NT1, NT2, PR, nchunk;
+    size_t plane, part, buf, tap_bytes, smem;
+};
+
+__host__ __device__ inline RbGeom rb_geom(const ResBlockTc &p)
+{
+    RbGeom g;
+    const int H = p.in.H, pitch = p.in.pitch, kg = p.in.C / 8;
+    g.nbands = (H + p.band_h - 1) / p.band_h;
+    g.S = (p.band_h + 4) * pitch + 2;
+    g.m_lo = pitch + 1;
+    g.NT1 = ((p.G - 1) * g.S + (p.band_h + 2) * pitch + 127) / 128;
+    g.NT2 = ((p.G - 1) * g.S + p.band_h * pitch + 127) / 128;
+    g.PR = p.G * g.S;
+    g.nchunk = (g.PR + 127) / 128;
+    g.plane = (size_t)g.PR * 16;
+    g.part = (size_t)kg * g.plane;
+    g.buf = (2 * g.part + 127) & ~(size_t)127;
+    g.tap_bytes = (size_t)2 * kg * p.in.C * 16;
+    g.smem = 2 * g.buf + p.stages * g.tap_bytes + 1024;
+    return g;
+}
+
+// Two 128-row tiles (the second only if `two`) of one conv: 9 taps x k-steps x passes of wgmma (ring slots n0 .. n0 + 8, released
+// as they are consumed).  The warpgroup's 64-row slabs of the two tiles accumulate into independent registers, interleaved per
+// k-step: one dependent accumulator chain per warpgroup leaves the tensor pipe waiting on wgmma latency (the fused kernel runs
+// one CTA per SM, so no second CTA fills those gaps).  Each row's sums keep the tap -> k-step -> pass order.
+template <int N>
+__device__ __forceinline__ void rb_tiles(float (&acc)[2][N / 2], bool two, uint64_t a_desc0, int row0, const ResBlockTc &p,
+                                         const RbGeom &g, uint64_t b_desc0, RbBars *bars, int n0, int lane)
+{
+    const uint32_t plane16 = (uint32_t)(g.plane >> 4), a_lo16 = (uint32_t)(g.part >> 4), b_lo16 = (uint32_t)N;
+    const int nstages = p.stages;
+#pragma unroll
+    for (int s = 0; s < 2; ++s)
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) acc[s][i] = 0.0f;
+    for (int tap = 0; tap < 9; ++tap) {
+        const int n = n0 + tap, st = n % nstages;
+        mbar_wait(&bars->full[st], (n / nstages) & 1);
+        const uint64_t b0 = b_desc0 + (uint64_t)((st * g.tap_bytes) >> 4);
+        const uint64_t a0 = a_desc0 + (uint64_t)(row0 + p.tap_shift[tap]);
+        wg_fence();
+        for (int ks = 0; ks < N / 16; ++ks) {
+#pragma unroll
+            for (int s = 0; s < 2; ++s) {
+                if (s == 1 && !two) break;
+                const uint64_t as = a0 + s * 128 + ks * 2 * plane16;
+                wgmma_f16<N>(acc[s], as, b0 + ks * 4 * N);
+                if (p.npass == 3) {
+                    wgmma_f16<N>(acc[s], as, b0 + b_lo16 + ks * 4 * N);
+                    wgmma_f16<N>(acc[s], as + a_lo16, b0 + ks * 4 * N);
+                }
+            }
+        }
+        wg_commit();
+        if (tap > 0) {
+            wg_wait<1>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&bars->empty[(n - 1) % nstages]);
+        }
+    }
+    wg_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars->empty[(n0 + 8) % nstages]);
+}
+
+template <int N>
+__global__ void __launch_bounds__(kCvThreads, 1) k_resblock_tc(ResBlockTc p)
+{
+    extern __shared__ __align__(1024) unsigned char smem[];
+    const RbGeom g = rb_geom(p);
+    unsigned char *in_s = smem, *mid_s = smem + g.buf, *ring = smem + 2 * g.buf;
+    RbBars *bars = reinterpret_cast<RbBars *>(ring + p.stages * g.tap_bytes);
+    const int nstages = p.stages;
+    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;   // warp-uniform value: uniform role branches
+    const int pitch = p.in.pitch, H = p.in.H, W = p.in.W, kg_in = N / 8;
+    const int group = blockIdx.x / g.nbands, band = blockIdx.x - group * g.nbands;
+    const int img0 = group * p.G, nimg = min(p.G, p.B - img0);
+    const int y0 = band * p.band_h;
+    const int np1 = (g.NT1 + 1) / 2, ntaps = 9 * (np1 + (g.NT2 + 1) / 2);   // the taps stream once per pair of tiles
+
+    if (tid == 0) {
+        for (int i = 0; i < kCvStages; ++i) { mbar_init(&bars->full[i], 1); mbar_init(&bars->empty[i], kCvConsumers / 32); }
+        for (int c = 0; c < g.nchunk; ++c) mbar_init(&bars->chunk[c], 1);
+        fence_mbar_init();
+    }
+    __syncthreads();
+
+    if (warp == kCvConsumers / 32) {
+        // ================= producer: the first ring fill, the input band chunk by chunk, then conv1's and conv2's taps =================
+        if (lane == 0) {
+            auto load_tap = [&](int n) {
+                const int st = n % nstages, tap = n % 9;
+                if (n >= nstages) mbar_wait(&bars->empty[st], ((n / nstages) - 1) & 1);
+                mbar_expect_tx(&bars->full[st], (uint32_t)g.tap_bytes);
+                bulk_g2s(ring + st * g.tap_bytes, p.w[n >= 9 * np1] + (size_t)tap * g.tap_bytes, (uint32_t)g.tap_bytes, &bars->full[st]);
+            };
+            for (int n = 0; n < nstages; ++n) load_tap(n);   // queued ahead of the band, so that conv1's first tile waits on its rows only
+            // rows outside the tensor (above the first band, below the last) are not copied: they only feed conv1 rows outside
+            // the image, which are stored as zeros whatever they hold
+            const int g0 = (y0 - 1) * pitch;
+            const int r0 = max(0, -g0), r1 = min(g.S, p.in.plane_rows - g0);
+            for (int c = 0; c < g.nchunk; ++c) {
+                uint32_t rows = 0;
+                for (int k = 0; k < nimg; ++k) rows += (uint32_t)max(0, min(k * g.S + r1, c * 128 + 128) - max(k * g.S + r0, c * 128));
+                mbar_expect_tx(&bars->chunk[c], rows * 16u * (uint32_t)(2 * kg_in));
+                for (int k = 0; k < nimg; ++k) {
+                    const int lo = max(k * g.S + r0, c * 128), hi = min(k * g.S + r1, c * 128 + 128);
+                    if (hi <= lo) continue;
+                    for (int part = 0; part < 2; ++part)
+                        for (int kg = 0; kg < kg_in; ++kg) {
+                            const unsigned char *src = p.in.base + (size_t)(img0 + k) * p.in.img_stride + part * p.in.part_stride +
+                                                       ((size_t)kg * p.in.plane_rows + g0 + lo - k * g.S) * 16;
+                            bulk_g2s(in_s + part * g.part + kg * g.plane + (size_t)lo * 16, src, (uint32_t)(hi - lo) * 16u, &bars->chunk[c]);
+                        }
+                }
+            }
+            for (int n = nstages; n < ntaps; ++n) load_tap(n);
+        }
+        return;
+    }
+
+    // ================= two warpgroups: rows [64 wg, 64 wg + 64) of every tile =================
+    const int wg = warp >> 2;
+    const uint32_t plane16 = (uint32_t)(g.plane >> 4);
+    const uint64_t in_desc = make_desc(smem_u32(in_s), plane16, 8), mid_desc = make_desc(smem_u32(mid_s), plane16, 8);
+    const uint64_t b_desc0 = make_desc(smem_u32(ring), 2 * N, 8);        // tap block [kg][N hi rows | N lo rows][16 B]: LBO = 2N rows
+    const int qc = 2 * (lane & 3);                                        // first of the thread's two columns in each 8-column group
+    // t1 row 0 (the pad column left of image 0's first halo row) is read by conv2 but is no conv1 output row
+    if (tid < 2 * kg_in) *reinterpret_cast<uint4 *>(mid_s + tid * g.plane) = make_uint4(0u, 0u, 0u, 0u);
+
+    // ================= conv1 -> BN -> ReLU -> t1 (shared memory) =================
+    int ready = 0;                                                        // input chunks known to have landed
+    for (int t = 0; t < g.NT1; t += 2) {
+        const bool two = t + 1 < g.NT1;
+        const int need = min(g.nchunk, (t * 128 + 256 + 2 * pitch + 1) / 128 + 1);   // rows [128 t, 128 t + 256 + 2 pitch + 2)
+        for (; ready < need; ++ready) mbar_wait(&bars->chunk[ready], 0);
+        float acc[2][N / 2];
+        rb_tiles<N>(acc, two, in_desc, g.m_lo + t * 128 + wg * 64, p, g, b_desc0, bars, t / 2 * 9, lane);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int s = e >> 1, hr = e & 1;
+            if (s == 1 && !two) break;
+            const int m = g.m_lo + (t + s) * 128 + wg * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
+            const int i = m - pitch;
+            const int k = m / g.S;
+            const int rho = (y0 - 1) * pitch - 1 + (m - k * g.S);
+            const int yy = rho / pitch - 1, xx = rho - (yy + 1) * pitch;
+            const bool valid = (k < nimg) && (rho >= pitch) && (yy >= y0 - 1) && (yy <= y0 + p.band_h) && (yy < H) && (xx < W);
+            if (i >= g.PR) continue;
+#pragma unroll
+            for (int j = 0; j < N / 8; ++j) {
+                const int col = 8 * j + qc;
+                float v0 = fmaf(acc[s][4 * j + 2 * hr], __ldg(p.scale[0] + col), __ldg(p.shift[0] + col));
+                float v1 = fmaf(acc[s][4 * j + 2 * hr + 1], __ldg(p.scale[0] + col + 1), __ldg(p.shift[0] + col + 1));
+                v0 = valid ? fmaxf(v0, 0.0f) : 0.0f;
+                v1 = valid ? fmaxf(v1, 0.0f) : 0.0f;
+                unsigned char *op = mid_s + (size_t)(col >> 3) * g.plane + (size_t)i * 16 + (col & 7) * 2;
+                store_split2(op, op + g.part, v0, v1);
+            }
+        }
+    }
+    for (; ready < g.nchunk; ++ready) mbar_wait(&bars->chunk[ready], 0);   // the residual reads every input row
+    fence_proxy_async();                                                  // t1's stores -> conv2's wgmma reads
+    asm volatile("bar.sync 1, %0;\n" ::"n"(kCvConsumers) : "memory");
+
+    // ================= conv2 -> BN -> + x -> ReLU -> output TCL =================
+    const int yend = min(y0 + p.band_h, H);
+    for (int t = 0; t < g.NT2; t += 2) {
+        const bool two = t + 1 < g.NT2;
+        float acc[2][N / 2];
+        rb_tiles<N>(acc, two, mid_desc, g.m_lo + t * 128 + wg * 64, p, g, b_desc0, bars, (np1 + t / 2) * 9, lane);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int s = e >> 1, hr = e & 1;
+            if (s == 1 && !two) break;
+            const int m = g.m_lo + (t + s) * 128 + wg * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
+            const int k = m / g.S;
+            const int rho = y0 * pitch - 1 + (m - k * g.S);
+            const int yy = rho / pitch - 1, xx = rho - (yy + 1) * pitch;
+            const bool in_band = (k < nimg) && (rho >= pitch) && (yy >= y0) && (yy < yend);
+            const bool valid = in_band && (xx < W);
+            const Tcl &o = p.out;
+            size_t obase = 0;
+            bool do_write = in_band;
+            if (in_band) {
+                if (o.nphase == 1) {
+                    obase = (size_t)(img0 + k) * o.img_stride + (size_t)(rho + 1) * 16;
+                } else if (valid) {                  // phase-split output for a stride-2 consumer
+                    const int ph = (yy & 1) * 2 + (xx & 1);
+                    const int rho2 = ((yy >> 1) + 1) * o.pitch + (xx >> 1);
+                    obase = (size_t)(img0 + k) * o.img_stride + ph * o.phase_stride + (size_t)(rho2 + 1) * 16;
+                } else {
+                    do_write = false;
+                }
+            }
+#pragma unroll
+            for (int j = 0; j < N / 8; ++j) {
+                const int col = 8 * j + qc;
+                float v0 = fmaf(acc[s][4 * j + 2 * hr], __ldg(p.scale[1] + col), __ldg(p.shift[1] + col));
+                float v1 = fmaf(acc[s][4 * j + 2 * hr + 1], __ldg(p.scale[1] + col + 1), __ldg(p.shift[1] + col + 1));
+                if (valid) {
+                    const unsigned char *rp = in_s + (size_t)(col >> 3) * g.plane + (size_t)(m + pitch) * 16 + (col & 7) * 2;
+                    const float2 a = __half22float2(*reinterpret_cast<const __half2 *>(rp));
+                    const float2 b = __half22float2(*reinterpret_cast<const __half2 *>(rp + g.part));
+                    v0 += a.x + b.x;
+                    v1 += a.y + b.y;
+                }
+                v0 = valid ? fmaxf(v0, 0.0f) : 0.0f;
+                v1 = valid ? fmaxf(v1, 0.0f) : 0.0f;
                 if (do_write) {
-                    unsigned char *op = o.base + obase + (size_t)(c >> 3) * o.plane_rows * 16 + (c & 7) * 2;
+                    unsigned char *op = o.base + obase + (size_t)(col >> 3) * o.plane_rows * 16 + (col & 7) * 2;
                     store_split2(op, op + o.part_stride, v0, v1);
                 }
             }
@@ -255,9 +484,10 @@ __global__ void k_pool_tcl(Tcl in, Tcl out, float *out_nchw, int B, int Hout)
 int conv_tc_prepare_launch()
 {
     const int big = 227 * 1024;
-    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
     LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
     LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
+    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_resblock_tc<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
+    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_resblock_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
     return LZ_OK;
 }
 
@@ -266,13 +496,49 @@ int conv_tc_launch(const ConvTc &p, cudaStream_t s)
     const CvGeom g = cv_geom(p);
     LZ_REQUIRE(g.smem <= 227 * 1024, LZ_EINVAL, "conv_tc: band needs %zu B shared memory", g.smem);
     LZ_REQUIRE(g.tap_bytes <= 16384 && (p.in.C % 16) == 0, LZ_EINVAL, "conv_tc: unsupported channel counts");
+    LZ_REQUIRE(p.out[0].nphase == 1 && (p.N < 128 || p.out[1].nphase == 1), LZ_EINVAL, "conv_tc: phase-split output is not supported");
     const int groups = (p.B + p.G - 1) / p.G;
     const int grid = groups * g.nbands;
     switch (p.N) {
-        case 32: k_conv_tc<32><<<grid, kCvThreads, g.smem, s>>>(p); break;
         case 64: k_conv_tc<64><<<grid, kCvThreads, g.smem, s>>>(p); break;
         case 128: k_conv_tc<128><<<grid, kCvThreads, g.smem, s>>>(p); break;
-        default: LZ_REQUIRE(false, LZ_EINVAL, "conv_tc: N must be 32, 64 or 128");
+        default: LZ_REQUIRE(false, LZ_EINVAL, "conv_tc: N must be 64 or 128");
+    }
+    LZ_KERNEL_CHECK();
+    return LZ_OK;
+}
+
+// Scores useful output rows (both convs) over issued MMA rows, which count conv1's halo recompute and the 128-row tile padding of
+// both convs.  A band of ~200 KB leaves room for one CTA per SM, so there is no co-residency term as in the plain conv's picker.
+int resblock_tc_plan(ResBlockTc &p)
+{
+    const int H = p.in.H, W = p.in.W;
+    ResBlockTc q = p;
+    double best = -1.0;
+    for (int G = 1; G <= 4; ++G)
+        for (int bh = (G > 1 ? H : 1); bh <= H; ++bh)
+            for (int st = 2; st <= 4; st += 2) {
+                q.G = G; q.band_h = bh; q.stages = st;
+                const RbGeom g = rb_geom(q);
+                if (g.smem > 227 * 1024 || g.nchunk > kRbChunks) continue;
+                double score = (double)(2 * G * H * W) / ((double)g.nbands * (g.NT1 + g.NT2) * 128);
+                score *= (st == 4) ? 1.0 : 0.97;
+                if (score > best + 1e-9) { best = score; p.G = G; p.band_h = bh; p.stages = st; }
+            }
+    LZ_REQUIRE(best > 0.0, LZ_EINVAL, "resblock_tc: no band of a %dx%d, %d-channel block fits shared memory", H, W, p.in.C);
+    return LZ_OK;
+}
+
+int resblock_tc_launch(const ResBlockTc &p, cudaStream_t s)
+{
+    const RbGeom g = rb_geom(p);
+    LZ_REQUIRE(g.smem <= 227 * 1024 && g.nchunk <= kRbChunks, LZ_EINVAL, "resblock_tc: band needs %zu B shared memory", g.smem);
+    LZ_REQUIRE(p.in.nphase == 1 && p.out.C == p.in.C, LZ_EINVAL, "resblock_tc: unsupported input / output layout");
+    const int grid = (p.B + p.G - 1) / p.G * g.nbands;
+    switch (p.in.C) {
+        case 32: k_resblock_tc<32><<<grid, kCvThreads, g.smem, s>>>(p); break;
+        case 64: k_resblock_tc<64><<<grid, kCvThreads, g.smem, s>>>(p); break;
+        default: LZ_REQUIRE(false, LZ_EINVAL, "resblock_tc: channels must be 32 or 64");
     }
     LZ_KERNEL_CHECK();
     return LZ_OK;

@@ -40,20 +40,36 @@ inline size_t tcl_bytes(int B, int C, int H, int W, int nphase)
 
 struct ConvTc {
     Tcl in;                       // input (nphase 1 or 4); its (H, W, pitch) is the output/row-space geometry
-    Tcl out[2];                   // column group 0 / 1 (group 1 only for N = 128); nphase 4 = write phase-split
+    Tcl out[2];                   // column group 0 / 1 (group 1 only for N = 128), nphase 1
     Tcl res;                      // residual added to group 0 (base == nullptr: none)
     const unsigned char *w;       // [9 taps][kg_in][N hi rows | N lo rows][8] fp16
     const float *scale, *shift;   // [N]
     int tap_phase[9], tap_shift[9];
     int relu[2];
-    int N;                        // 32, 64 or 128
+    int N;                        // 64 or 128
     int G, band_h;                // images per CTA (band_h == H when G > 1), image rows per band
     int stages;                   // weight ring depth (2..4)
     int B, npass;
 };
 
+// One plain ResBlock, relu(bn2(conv2(relu(bn1(conv1(x))))) + x), C -> C channels at stride 1, in one kernel: conv1's output
+// stays in shared memory (see k_resblock_tc)
+struct ResBlockTc {
+    Tcl in;                       // x (nphase 1); its (C, H, W, pitch) is the geometry of the whole block
+    Tcl out;                      // nphase 1, or 4 = written phase-split for a stride-2 consumer
+    const unsigned char *w[2];    // conv1 / conv2 tap blocks (conv_tc_pack with ncols = C)
+    const float *scale[2], *shift[2];
+    int tap_shift[9];
+    int G, band_h;                // images per CTA (band_h == H when G > 1), output rows per band
+    int stages;                   // weight ring depth (2 or 4)
+    int B, npass;
+};
+
 int conv_tc_prepare_launch();
 int conv_tc_launch(const ConvTc &p, cudaStream_t s);
+// picks G, band_h and stages of a ResBlockTc whose `in` geometry is set; returns LZ_EINVAL if no band fits
+int resblock_tc_plan(ResBlockTc &p);
+int resblock_tc_launch(const ResBlockTc &p, cudaStream_t s);
 // weights [cout][cin][3][3] -> tap blocks with `ncols` columns, this tensor occupying columns
 // [col0, col0+cout); returns the exact power-of-two scale applied
 float conv_tc_pack(const float *w_torch, int cin, int cout, int ncols, int col0, unsigned char *dst);

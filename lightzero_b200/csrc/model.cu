@@ -527,7 +527,7 @@ int model_reserve(lz_model *m, int B)
         const int h1 = m->tower[0].hout, h2 = m->tower[3].hout, h3 = (h2 - 1) / 2 + 1, c2 = kC / 2;
         const size_t bT = tcl_bytes(B, c2, h1, h1, 1), bT2 = tcl_bytes(B, c2, h1 / 2, h1 / 2, 4);
         const size_t bU = tcl_bytes(B, kC, h2, h2, 1), bV = tcl_bytes(B, kC, h3, h3, 1);
-        const size_t total = 2 * bT + bT2 + 3 * bU + 3 * bV;
+        const size_t total = bT + bT2 + 3 * bU + 2 * bV;
         if (m->tws) cudaFree(m->tws);
         m->tws = nullptr;
         int rc = dev_alloc(&m->tws, total);
@@ -536,14 +536,12 @@ int model_reserve(lz_model *m, int B)
         m->tws_bytes = total;
         unsigned char *q = m->tws;
         m->T0 = make_tcl(q, c2, h1, h1, 1); q += bT;
-        m->T1 = make_tcl(q, c2, h1, h1, 1); q += bT;
-        m->T2 = make_tcl(q, c2, h1 / 2, h1 / 2, 4); q += bT2;
+        m->T1 = make_tcl(q, c2, h1 / 2, h1 / 2, 4); q += bT2;
         m->U0 = make_tcl(q, kC, h2, h2, 1); q += bU;
         m->U1 = make_tcl(q, kC, h2, h2, 1); q += bU;
         m->U2 = make_tcl(q, kC, h2, h2, 1); q += bU;
         m->V0 = make_tcl(q, kC, h3, h3, 1); q += bV;
         m->V1 = make_tcl(q, kC, h3, h3, 1); q += bV;
-        m->V2 = make_tcl(q, kC, h3, h3, 1); q += bV;
     }
     return LZ_OK;
 }
@@ -598,16 +596,18 @@ static int tower_tc_run(lz_model *m, int B, const float *d_obs, float *pre_laten
         p.B = B; p.npass = npass;
         return conv_tc_launch(p, s);
     };
-    if ((rc = run(m->tower_tc[0], m->T0, m->T1, nullptr, nullptr))) return rc;        // resblocks1.0.conv1
-    if ((rc = run(m->tower_tc[1], m->T1, m->T2, nullptr, &m->T0))) return rc;         // resblocks1.0.conv2 (+x) -> phase-split
-    if ((rc = run(m->tower_tc[2], m->T2, m->U0, &m->U1, nullptr))) return rc;         // downsample conv1 | conv3 (stride 2)
-    if ((rc = run(m->tower_tc[3], m->U0, m->U2, nullptr, &m->U1))) return rc;         // downsample conv2 + identity
-    if ((rc = run(m->tower_tc[4], m->U2, m->U0, nullptr, nullptr))) return rc;        // resblocks2.0.conv1
-    if ((rc = run(m->tower_tc[5], m->U0, m->U1, nullptr, &m->U2))) return rc;         // resblocks2.0.conv2 (+x)
-    if ((rc = pool_tcl_launch(m->U1, m->V0, B, s))) return rc;                        // pooling1
-    if ((rc = run(m->tower_tc_rb3[0], m->V0, m->V1, nullptr, nullptr))) return rc;    // resblocks3.0.conv1
-    if ((rc = run(m->tower_tc_rb3[1], m->V1, m->V2, nullptr, &m->V0))) return rc;     // resblocks3.0.conv2 (+x)
-    return pool_tcl_to_nchw_launch(m->V2, pre_latent, B, kHW, s);                    // pooling2 -> [B][64][6][6]
+    auto rb = [&](ResBlockTc p, const Tcl &in, const Tcl &out) {
+        p.in = in; p.out = out;
+        p.B = B; p.npass = npass;
+        return resblock_tc_launch(p, s);
+    };
+    if ((rc = rb(m->tower_rb[0], m->T0, m->T1))) return rc;                           // resblocks1.0 -> phase-split
+    if ((rc = run(m->tower_tc[0], m->T1, m->U0, &m->U1, nullptr))) return rc;         // downsample conv1 | conv3 (stride 2)
+    if ((rc = run(m->tower_tc[1], m->U0, m->U2, nullptr, &m->U1))) return rc;         // downsample conv2 + identity
+    if ((rc = rb(m->tower_rb[1], m->U2, m->U0))) return rc;                           // resblocks2.0
+    if ((rc = pool_tcl_launch(m->U0, m->V0, B, s))) return rc;                        // pooling1
+    if ((rc = rb(m->tower_rb[2], m->V0, m->V1))) return rc;                           // resblocks3.0
+    return pool_tcl_to_nchw_launch(m->V1, pre_latent, B, kHW, s);                    // pooling2 -> [B][64][6][6]
 }
 
 // tensor-core path only: the DownSample tower alone (obs -> pre-latent [B][64][36]) ...
@@ -770,6 +770,7 @@ static int pack_tower_tc(lz_model *m)
     const int h1 = m->tower[0].hout, h2 = m->tower[3].hout, h3 = (h2 - 1) / 2 + 1;
     struct Item { std::string w, bn; int cin, cout; };
     // layer table: 0 rb1.c1, 1 rb1.c2, 2 ds.c1 | ds.c3 (merged N=128), 3 ds.c2, 4 rb2.c1, 5 rb2.c2, 6 rb3.c1, 7 rb3.c2
+    // (layers 0-1, 4-5 and 6-7 run as fused ResBlocks, 2 and 3 as single convs)
     const Item items[9] = {
         {R + "resblocks1.0.conv1.0.weight", R + "resblocks1.0.conv1.1", c2, c2},
         {R + "resblocks1.0.conv2.0.weight", R + "resblocks1.0.conv2.1", c2, c2},
@@ -833,14 +834,22 @@ static int pack_tower_tc(lz_model *m)
         pick_band(p);
         return p;
     };
-    m->tower_tc[0] = base(0, c2, h1, 1, c2);
-    m->tower_tc[1] = base(1, c2, h1, 1, c2);
-    m->tower_tc[2] = base(2, 2 * kC, h2, 4, c2);
-    m->tower_tc[3] = base(3, kC, h2, 1, kC);
-    m->tower_tc[4] = base(4, kC, h2, 1, kC);
-    m->tower_tc[5] = base(5, kC, h2, 1, kC);
-    m->tower_tc_rb3[0] = base(6, kC, h3, 1, kC);
-    m->tower_tc_rb3[1] = base(7, kC, h3, 1, kC);
+    m->tower_tc[0] = base(2, 2 * kC, h2, 4, c2);
+    m->tower_tc[1] = base(3, kC, h2, 1, kC);
+    // ResBlocks: layers (li, li + 1) are conv1 and conv2 of one block
+    auto block = [&](ResBlockTc &p, int li, int C, int H) {
+        memset(&p, 0, sizeof(p));
+        for (int c = 0; c < 2; ++c) {
+            p.w[c] = m->d_tower + woff[li + c];
+            p.scale[c] = dtab + (li + c) * 256; p.shift[c] = p.scale[c] + 128;
+        }
+        p.in = make_tcl(nullptr, C, H, H, 1);
+        for (int t = 0; t < 9; ++t) p.tap_shift[t] = (t / 3 - 1) * p.in.pitch + (t % 3 - 1);
+        return resblock_tc_plan(p);
+    };
+    if ((rc = block(m->tower_rb[0], 0, c2, h1))) return rc;
+    if ((rc = block(m->tower_rb[1], 4, kC, h2))) return rc;
+    if ((rc = block(m->tower_rb[2], 6, kC, h3))) return rc;
     return conv_tc_prepare_launch();
 }
 

@@ -101,11 +101,11 @@ struct lz_model {
     int tc_skip_B;
     // tensor-core DownSample tower: packed weights / folded BN per layer, TCL activation workspace
     unsigned char *d_tower;           // weights + scale/shift tables
-    lz::ConvTc tower_tc[7];           // rb1.c1, rb1.c2, ds(c1+c3), ds.c2, rb2.c1, rb2.c2, rb3.c1 / rb3.c2 share [6]: see model.cu
-    lz::ConvTc tower_tc_rb3[2];
+    lz::ConvTc tower_tc[2];           // downsample block: conv1 | conv3 (stride 2), conv2 (+ identity)
+    lz::ResBlockTc tower_rb[3];       // resblocks1, resblocks2, resblocks3
     unsigned char *tws;               // TCL workspace (one allocation)
     size_t tws_bytes;
-    lz::Tcl T0, T1, T2, U0, U1, U2, V0, V1, V2;
+    lz::Tcl T0, T1, U0, U1, U2, V0, V1;
     // workspace for initial inference (grown on demand, outside graph capture)
     float *ws[3];
     size_t ws_floats;
