@@ -186,6 +186,18 @@ int lz_model_debug_tc_program(lz_model *m, int which, int nlayers, const int *la
                               int has_reward);
 /* Test hook: 64 clock64 stamps of CTA 0 of the last tensor-core launch made with env LZ_TC_DEBUG=1. */
 int lz_debug_tc_stamps(unsigned long long *h_out);
+/* Test hook: runs the tensor-core DownSample tower on d_obs (f32) or d_obs_u8 (uint8; exactly one non-NULL) through
+ * stage `stage` and copies that stage's output tensor, byte for byte, to d_out (out_bytes must be large enough).
+ * Stages: 0 stem -> T0, 1 resblocks1 -> T1 (phase-split), 2 / 3 downsample conv1 / conv3 (one launch) -> U0 / U1,
+ * 4 downsample conv2 + identity -> U2, 5 resblocks2 -> U0, 6 pooling1 -> V0, 7 resblocks3 -> V1, 8 pooling2 -> the
+ * f32 NCHW pre-latent [B][64][6][6].  Stages 0-7 copy the tensor-core layout (conv_tc.cuh):
+ * [B][nphase][hi | lo][C / 8][plane_rows][8] fp16.
+ * h_info (int32[10]) receives the tensor geometry and the plan of the launch that wrote it:
+ * C, H, W, nphase, plane_rows (nphase = plane_rows = 0 for stage 8), then G (images per CTA), band_h (output rows per
+ * CTA; 0 where the launch has no bands), stages (weight ring depth; 0 off the wgmma kernels) and the CTA count of the
+ * launch, then npass (3 = tc3, 1 = tc1).  Needs a finalized conv model with math != 0 (LZ_ESTATE otherwise). */
+int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uint8_t *d_obs_u8, int stage,
+                               void *d_out, size_t out_bytes, int32_t *h_info, lz_stream s);
 int lz_model_latent_hw(const lz_model *m);   /* 6 for 84/96, 8 for 64 */
 int lz_model_support_size(const lz_model *m);
 

@@ -60,6 +60,8 @@ SIGNATURES = {
     "lz_model_set_math": (c_int, [c_void_p, c_int]),
     "lz_model_debug_tc_program": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int]),
     "lz_debug_tc_stamps": (c_int, [c_void_p]),
+    "lz_model_debug_tower_stage": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, ctypes.c_size_t,
+                                           c_void_p, c_void_p]),
     "lz_model_latent_hw": (c_int, [c_void_p]),
     "lz_model_support_size": (c_int, [c_void_p]),
     "lz_model_initial_inference": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

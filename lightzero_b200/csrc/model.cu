@@ -574,7 +574,10 @@ static void pick_band(ConvTc &p)
     p.stages = best_st;
 }
 
-static int tower_tc_run(lz_model *m, int B, const float *d_obs, float *pre_latent, cudaStream_t s, const uint8_t *d_obs_u8 = nullptr)
+// stop_after < 8 ends the tower after that stage's launch (stage numbers of lz_model_debug_tower_stage); pre_latent is then
+// not written
+static int tower_tc_run(lz_model *m, int B, const float *d_obs, float *pre_latent, cudaStream_t s, const uint8_t *d_obs_u8 = nullptr,
+                        int stop_after = 8)
 {
     int rc;
     const int npass = (m->math == 1) ? 3 : 1;
@@ -589,6 +592,7 @@ static int tower_tc_run(lz_model *m, int B, const float *d_obs, float *pre_laten
         else k_stem4_tcl<false><<<grid, 256, smem, s>>>(P, d_obs, nullptr, S0.hin, S0.win, S0.hout, S0.wout, rows_per_cta, m->T0);
         LZ_KERNEL_CHECK();
     } else if ((rc = launch_convg(S0, d_obs, nullptr, nullptr, 1, B, s, &m->T0, d_obs_u8))) return rc;
+    if (stop_after <= 0) return LZ_OK;
     auto run = [&](ConvTc p, const Tcl &in, const Tcl &o0, const Tcl *o1, const Tcl *res) {
         p.in = in; p.out[0] = o0;
         if (o1) p.out[1] = *o1;
@@ -602,11 +606,17 @@ static int tower_tc_run(lz_model *m, int B, const float *d_obs, float *pre_laten
         return resblock_tc_launch(p, s);
     };
     if ((rc = rb(m->tower_rb[0], m->T0, m->T1))) return rc;                           // resblocks1.0 -> phase-split
+    if (stop_after <= 1) return LZ_OK;
     if ((rc = run(m->tower_tc[0], m->T1, m->U0, &m->U1, nullptr))) return rc;         // downsample conv1 | conv3 (stride 2)
+    if (stop_after <= 3) return LZ_OK;
     if ((rc = run(m->tower_tc[1], m->U0, m->U2, nullptr, &m->U1))) return rc;         // downsample conv2 + identity
+    if (stop_after <= 4) return LZ_OK;
     if ((rc = rb(m->tower_rb[1], m->U2, m->U0))) return rc;                           // resblocks2.0
+    if (stop_after <= 5) return LZ_OK;
     if ((rc = pool_tcl_launch(m->U0, m->V0, B, s))) return rc;                        // pooling1
+    if (stop_after <= 6) return LZ_OK;
     if ((rc = rb(m->tower_rb[2], m->V0, m->V1))) return rc;                           // resblocks3.0
+    if (stop_after <= 7) return LZ_OK;
     return pool_tcl_to_nchw_launch(m->V1, pre_latent, B, kHW, s);                    // pooling2 -> [B][64][6][6]
 }
 
@@ -1280,6 +1290,71 @@ int lz_model_initial_inference(lz_model *m, int B, const float *d_obs, float *d_
     memset(&io, 0, sizeof(io));
     io.latent = d_latent; io.policy_logits = d_policy_logits; io.value_logits = d_value_logits; io.value = d_value;
     return model_initial(m, B, d_obs, io, (cudaStream_t)s);
+}
+
+int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uint8_t *d_obs_u8, int stage, void *d_out,
+                               size_t out_bytes, int32_t *h_info, lz_stream s)
+{
+    LZ_REQUIRE(m && B > 0 && (d_obs == nullptr) != (d_obs_u8 == nullptr) && d_out && h_info && stage >= 0 && stage <= 8, LZ_EINVAL,
+               "lz_model_debug_tower_stage: bad argument");
+    LZ_REQUIRE(m->finalized && m->kind == 0 && m->cfg.obs_h != 64, LZ_ESTATE, "lz_model_debug_tower_stage: not a finalized conv model with a tensor-core tower");
+    LZ_REQUIRE(m->math != 0, LZ_ESTATE, "lz_model_debug_tower_stage: math mode 0 does not run the tensor-core tower");
+    if (B > m->ws_B) {
+        int rc = model_reserve(m, B);
+        if (rc != LZ_OK) return rc;
+    }
+    LZ_REQUIRE(B <= m->ws_B, LZ_ESTATE, "lz_model_debug_tower_stage: workspace sized for %d roots, got %d", m->ws_B, B);
+    // stage -> the tensor it leaves and the launch that wrote it (tower_tc_run)
+    const Tcl *outs[8] = {&m->T0, &m->T1, &m->U0, &m->U1, &m->U2, &m->U0, &m->V0, &m->V1};
+    int32_t info[10] = {0};
+    size_t bytes;
+    if (stage < 8) {
+        const Tcl &t = *outs[stage];
+        info[0] = t.C; info[1] = t.H; info[2] = t.W; info[3] = t.nphase; info[4] = t.plane_rows;
+        bytes = (size_t)B * t.img_stride;
+    } else {
+        info[0] = kC; info[1] = kHW; info[2] = kHW;                    // fp32 NCHW: nphase = plane_rows = 0
+        bytes = (size_t)B * kC * kHW * kHW * sizeof(float);
+    }
+    LZ_REQUIRE(out_bytes >= bytes, LZ_EINVAL, "lz_model_debug_tower_stage: stage %d needs %zu bytes, got %zu", stage, bytes, out_bytes);
+    const ConvG &S0 = m->tower[0];
+    auto pool_ctas = [&](const Tcl &in, int hout) {
+        return (int)std::min<size_t>(((size_t)B * (in.C / 8) * hout * hout + 255) / 256, kNumSMs * 32);
+    };
+    auto rb_plan = [&](const ResBlockTc &p) {
+        info[5] = p.G; info[6] = p.band_h; info[7] = p.stages;
+        info[8] = (B + p.G - 1) / p.G * ((p.in.H + p.band_h - 1) / p.band_h);
+    };
+    auto cv_plan = [&](const ConvTc &p) {
+        info[5] = p.G; info[6] = p.band_h; info[7] = p.stages;
+        info[8] = (B + p.G - 1) / p.G * ((p.in.H + p.band_h - 1) / p.band_h);
+    };
+    switch (stage) {
+        case 0:
+            info[5] = 1;
+            if (m->stem_valid) {
+                const int rows_per_cta = std::max(1, 256 / S0.wout);
+                info[6] = rows_per_cta;
+                info[8] = ceil_div(S0.hout, rows_per_cta) * B;
+            } else {
+                info[8] = ceil_div(S0.hout * S0.wout, 128) * (S0.cout / 32) * B;
+            }
+            break;
+        case 1: rb_plan(m->tower_rb[0]); break;
+        case 2: case 3: cv_plan(m->tower_tc[0]); break;
+        case 4: cv_plan(m->tower_tc[1]); break;
+        case 5: rb_plan(m->tower_rb[1]); break;
+        case 6: info[5] = 1; info[8] = pool_ctas(m->U0, m->V0.H); break;
+        case 7: rb_plan(m->tower_rb[2]); break;
+        default: info[5] = 1; info[8] = pool_ctas(m->V1, kHW); break;
+    }
+    info[9] = (m->math == 1) ? 3 : 1;
+    const cudaStream_t st = (cudaStream_t)s;
+    int rc = tower_tc_run(m, B, d_obs, stage == 8 ? reinterpret_cast<float *>(d_out) : nullptr, st, d_obs_u8, stage);
+    if (rc != LZ_OK) return rc;
+    if (stage < 8) LZ_CUDA_CHECK(cudaMemcpyAsync(d_out, outs[stage]->base, bytes, cudaMemcpyDeviceToDevice, st));
+    memcpy(h_info, info, sizeof(info));
+    return LZ_OK;
 }
 
 int lz_model_recurrent_inference(lz_model *m, int B, const float *d_latent, const int32_t *d_action,
