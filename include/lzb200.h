@@ -198,6 +198,17 @@ int lz_debug_tc_stamps(unsigned long long *h_out);
  * launch, then npass (3 = tc3, 1 = tc1).  Needs a finalized conv model with math != 0 (LZ_ESTATE otherwise). */
 int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uint8_t *d_obs_u8, int stage,
                                void *d_out, size_t out_bytes, int32_t *h_info, lz_stream s);
+/* Test hook: runs a copy of the latent-grid tensor-core program (`which` 0: recurrent_inference on d_latent f32 [B,64,6,6]
+ * NCHW and d_action int32 [B]; 1: the tail of initial_inference on the pre-latent d_latent, d_action unused) cut off after
+ * layer `stage`, and writes that layer's f32 output [B,64,6,6] NCHW to d_out.  The model's own programs are not changed.
+ * stage == nlayers runs the whole program twice and writes, f32: reward logits [B,K], value logits [B,K], policy logits
+ * [B,A], reward [B], value [B] with the raw logits requested, then policy logits [B,A], reward [B], value [B] without raw
+ * reward / value logits (the joint categorical read-out of the search), then for EfficientZero (`which` 0) the reward-head
+ * features [B, reward_head_channels*36] the LSTM consumes.  Sections a program does not produce are zero.
+ * h_info (int32[8]) receives the launch plan: roots per CTA R, row tiles NT, CTA count, roots of the last CTA, layers of
+ * the launched program, MMA passes, 1 if the FC2 biases are staged in shared memory, FC2 tiles. */
+int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_latent, const int32_t *d_action, int stage,
+                             void *d_out, size_t out_bytes, int32_t *h_info, lz_stream s);
 int lz_model_latent_hw(const lz_model *m);   /* 6 for 84/96, 8 for 64 */
 int lz_model_support_size(const lz_model *m);
 

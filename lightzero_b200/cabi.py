@@ -62,6 +62,8 @@ SIGNATURES = {
     "lz_debug_tc_stamps": (c_int, [c_void_p]),
     "lz_model_debug_tower_stage": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, ctypes.c_size_t,
                                            c_void_p, c_void_p]),
+    "lz_model_debug_net_stage": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, ctypes.c_size_t,
+                                         c_void_p, c_void_p]),
     "lz_model_latent_hw": (c_int, [c_void_p]),
     "lz_model_support_size": (c_int, [c_void_p]),
     "lz_model_initial_inference": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

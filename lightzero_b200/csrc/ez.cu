@@ -306,6 +306,8 @@ __global__ void __launch_bounds__(kTThreads, 1) k_ez_lstm_tc(EzNet net, EzIO io)
     }
 }
 
+bool ez_tc_shape(int nin, int H) { return (nin % kTK) == 0 && (H % kTK) == 0; }
+
 size_t ez_wtc_bytes(int nin, int H) { return (size_t)(4 * H / kTN) * ((nin + H) / kTK) * (2 * kTWPart); }
 
 // W_ih [4H][nin], W_hh [4H][H] (torch gate order i, f, g, o along dim 0) -> per (n-tile, k-chunk) [hi | lo] blocks of
@@ -345,7 +347,7 @@ int ez_launch(const EzNet &net, const EzIO &io, cudaStream_t s, int math)
 {
     LZ_REQUIRE(net.H <= kHMaxH && net.hid <= kHMaxHid && net.K <= kHLd && (net.H % 8) == 0, LZ_EINVAL,
                "ez_launch: unsupported LSTM / head size (H=%d hid=%d K=%d)", net.H, net.hid, net.K);
-    const bool tc_ok = net.wtc && (net.nin % kTK) == 0 && (net.H % kTK) == 0;
+    const bool tc_ok = net.wtc && ez_tc_shape(net.nin, net.H);
     if (math != 0 && tc_ok) {
         dim3 grid(4 * net.H / kTN, (io.B + kTM - 1) / kTM);
         k_ez_lstm_tc<<<grid, kTThreads, kTSmem, s>>>(net, io);

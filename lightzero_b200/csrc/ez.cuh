@@ -34,6 +34,7 @@ struct EzIO {
 
 int ez_launch(const EzNet &net, const EzIO &io, cudaStream_t s, int math);   // math 0: fp32 FFMA GEMM, else tensor-core (wgmma) 3xFP16
 int ez_prepare_launch();
+bool ez_tc_shape(int nin, int H);   // k_ez_lstm_tc runs K = nin + H in whole chunks of 64 and N = 4H in tiles of 64
 // host: pack W ([4H][nin] and [4H][H], torch gate order) into the tensor-core layout; returns the scale applied
 size_t ez_wtc_bytes(int nin, int H);
 float ez_pack_wtc(const float *w_ih, const float *w_hh, int nin, int H, unsigned char *dst);

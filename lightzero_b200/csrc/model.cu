@@ -1162,11 +1162,12 @@ int lz_model_finalize(lz_model *m)
             for (int i = 0; i < H; ++i) fc1[(size_t)i * hid + j] = (*W0)[(size_t)j * H + i];
         for (int k = 0; k < K; ++k)
             for (int j = 0; j < hid; ++j) fc2[(size_t)j * K + k] = (*W3)[(size_t)k * hid + j];
-        {   // tensor-core copy of the LSTM weights (fp16 hi / lo, power-of-two scaled), own allocation
+        if (m->d_ez_wtc) cudaFree(m->d_ez_wtc);
+        m->d_ez_wtc = nullptr;
+        if (ez_tc_shape(nin, H)) {   // tensor-core copy of the LSTM weights (fp16 hi / lo, power-of-two scaled), own allocation;
+                                     // other shapes (e.g. 8 reward-head channels: nin = 288) run the fp32 k_ez_lstm
             std::vector<unsigned char> wtc(ez_wtc_bytes(nin, H));
             ez_scale = ez_pack_wtc(Wih->data(), Whh->data(), nin, H, wtc.data());
-            if (m->d_ez_wtc) cudaFree(m->d_ez_wtc);
-            m->d_ez_wtc = nullptr;
             int rc2 = dev_alloc(&m->d_ez_wtc, wtc.size());
             if (rc2 != LZ_OK) return rc2;
             LZ_CUDA_CHECK(cudaMemcpy(m->d_ez_wtc, wtc.data(), wtc.size(), cudaMemcpyHostToDevice));
@@ -1355,6 +1356,58 @@ int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uin
     if (stage < 8) LZ_CUDA_CHECK(cudaMemcpyAsync(d_out, outs[stage]->base, bytes, cudaMemcpyDeviceToDevice, st));
     memcpy(h_info, info, sizeof(info));
     return LZ_OK;
+}
+
+int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_latent, const int32_t *d_action, int stage, void *d_out,
+                             size_t out_bytes, int32_t *h_info, lz_stream s)
+{
+    LZ_REQUIRE(m && (which == 0 || which == 1) && B > 0 && d_latent && (which == 1 || d_action) && d_out && h_info && stage >= 0,
+               LZ_EINVAL, "lz_model_debug_net_stage: bad argument");
+    LZ_REQUIRE(m->finalized && m->kind == 0 && m->math != 0, LZ_ESTATE, "lz_model_debug_net_stage: not a finalized conv model on the tensor-core path");
+    TcNet net = which ? m->tc_tail : m->tc_rec;          // a copy: the model's programs stay as they are
+    const int nl = net.nlayers, K = m->K, A = m->cfg.action_space_size;
+    const bool ez = m->cfg.efficientzero != 0 && which == 0;
+    const int nfeat = ez ? m->cfg.reward_head_channels * kP : 0;
+    LZ_REQUIRE(stage <= nl, LZ_EINVAL, "lz_model_debug_net_stage: stage %d past the %d layers of the program", stage, nl);
+    {
+        int rc = model_reserve(m, B);
+        if (rc != LZ_OK) return rc;
+    }
+    const size_t nfl = stage < nl ? (size_t)B * kActFloats : (size_t)B * (2 * K + 2 * A + 4 + nfeat);
+    LZ_REQUIRE(out_bytes >= nfl * sizeof(float), LZ_EINVAL, "lz_model_debug_net_stage: stage %d needs %zu bytes, got %zu", stage,
+               nfl * sizeof(float), out_bytes);
+    const cudaStream_t st = (cudaStream_t)s;
+    float *o = reinterpret_cast<float *>(d_out);
+    TcIO t;
+    memset(&t, 0, sizeof(t));
+    t.B = B; t.npass = (m->math == 1) ? 3 : 1;
+    t.latent_base = d_latent; t.action = which ? nullptr : d_action;
+    t.skip_scratch = m->tc_skip;
+    t.ez_feat = ez ? m->ez_feat : nullptr;
+    int rc;
+    if (stage < nl) {
+        // the program cut after layer `stage`, whose output is the only latent written
+        net.nlayers = stage + 1;
+        for (int L = 0; L <= stage; ++L) net.layer_flags[L] &= ~LF_WRITE_LATENT;
+        net.layer_flags[stage] |= LF_WRITE_LATENT;
+        t.latent_out = o;
+        tc_describe(net, t, h_info);
+        return tc_launch(net, t, st);
+    }
+    // the whole program: [reward logits B x K | value logits B x K | policy logits B x A | reward B | value B] with the raw logits
+    // requested, then [policy logits B x A | reward B | value B] without them (the joint categorical read-out), then ez_feat
+    LZ_CUDA_CHECK(cudaMemsetAsync(d_out, 0, nfl * sizeof(float), st));
+    float *rl = o, *vl = rl + (size_t)B * K, *pl = vl + (size_t)B * K, *r = pl + (size_t)B * A, *v = r + B;
+    float *pl2 = v + B, *r2 = pl2 + (size_t)B * A, *v2 = r2 + B, *feat = v2 + B;
+    if (ez) t.ez_feat = feat;
+    const bool rew = net.has_reward && !ez;
+    t.policy_logits = pl; t.value_logits = vl; t.value = v;
+    t.reward_logits = rew ? rl : nullptr; t.reward = rew ? r : nullptr;
+    tc_describe(net, t, h_info);
+    if ((rc = tc_launch(net, t, st))) return rc;
+    t.policy_logits = pl2; t.value_logits = nullptr; t.value = v2;
+    t.reward_logits = nullptr; t.reward = rew ? r2 : nullptr;
+    return tc_launch(net, t, st);
 }
 
 int lz_model_recurrent_inference(lz_model *m, int B, const float *d_latent, const int32_t *d_action,

@@ -92,8 +92,11 @@ constexpr int kFrBytes = 72 * 8 * 16 * 2;                 // reward features par
 constexpr int kHbHeadBytes = 4 * 16 * 16;                 // FC2 B operand of one head: [4 k-groups][8 roots hi | 8 roots lo][16 B] = 1 KB
 constexpr int kFc1Stages = 18;                            // 576 inputs / 32 per stage (2 k-steps x (A_hi + A_lo))
 constexpr int kFc1StageBytes = 2 * 2 * 2 * 96 * 16;       // 12,288 B: only the 96 real rows (3 heads x 32 units) of the M = 128 operand are streamed
-constexpr int kF2MaxTiles = 15;                           // FC2 accumulators, hi + lo added: [tile][128 outputs][8 roots] fp32 (61,440 B, overlays the dead FC1 operand)
+// FC2 accumulators, hi + lo added: [tile][128 outputs][8 roots] fp32 over the dead FC1 operand: room for 18 tiles (73,728 B).
+// lz_model_finalize takes heads of up to 608 outputs on this path (support and action space alike): 3 x 5 = 15 tiles
+constexpr int kF2MaxTiles = 18;
 static_assert(kF2MaxTiles * 128 * 8 * 4 <= kFbBytes, "FC2 staging must fit under the FC1 operand");
+static_assert(3 * ((608 + 127) / 128) <= kF2MaxTiles, "FC2 staging must hold the largest heads");
 
 __device__ __forceinline__ void put_half(unsigned char *p, float v, float &rem)
 {
@@ -750,11 +753,25 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
             unsigned char *fb = act, *hb = act + kFbBytes;
             float *red = reinterpret_cast<float *>(hb + 3 * kHbHeadBytes);
             float *f2 = reinterpret_cast<float *>(act);           // FC2 accumulators [tile][128][8], over the dead FC1 operand
-            if (hmask_fc & 1) {      // the parked reward features become rows 0-7 (hi) / 32-39 (lo) of the B operand
+            // the parked reward features become rows 0-7 (hi) / 32-39 (lo) of the B operand.  FC1 multiplies all 576 inputs of
+            // every head: the host packs zero weights past hc * 36, but 0 x an Inf / NaN bit pattern that an earlier simulation
+            // (the FC2 staging overlays these rows) or kernel left there is NaN, so a head of hc < 16 channels gets zeros there
+            for (int h = 0; h < 3; ++h) {
+                const int nin = net.hc[h] * kP;
+                if (!((hmask_fc >> h) & 1) || (h > 0 && nin == 576)) continue;
                 for (int i = tid; i < 2 * 72 * 8; i += kEpiThreads) {
                     const int part = i / (72 * 8), rem = i - part * (72 * 8), kg = rem >> 3, r = rem & 7;
-                    *reinterpret_cast<uint4 *>(fb + kg * kFbKgBytes + (part * 32 + r) * 16) =
-                        *reinterpret_cast<const uint4 *>(fr + part * (kFrBytes / 2) + (kg * 8 + r) * 16);
+                    unsigned char *dst = fb + kg * kFbKgBytes + (part * 32 + h * 8 + r) * 16;
+                    const int keep = nin - kg * 8;                // inputs of this k-group that exist
+                    if (h > 0 && keep >= 8) continue;
+                    uint4 q = make_uint4(0, 0, 0, 0);
+                    if (keep > 0) {
+                        q = *reinterpret_cast<const uint4 *>(h == 0 ? fr + part * (kFrBytes / 2) + (kg * 8 + r) * 16 : dst);
+                        if (keep < 8) {                           // hc * 36 = 4 (mod 8) for odd hc: keep the first 4 halves
+                            q.z = 0; q.w = 0;
+                        }
+                    }
+                    *reinterpret_cast<uint4 *>(dst) = q;
                 }
             }
             fence_proxy_async();
@@ -915,6 +932,35 @@ int tc_pick_roots(int B)
     return std::min(std::max(r, 1), kMaxRoots);
 }
 
+// the heads k_net_tc evaluates (the hmask_fc of the kernel) and the FC2 tiles they stream
+static int tc_heads_mask(const TcNet &net, const TcIO &io) { return ((net.has_reward && !io.ez_feat) ? 1 : 0) | 6; }
+static int tc_fc2_tiles(const TcNet &net, int hmask)
+{
+    int tiles = 0;
+    for (int h = 0; h < 3; ++h)
+        if ((hmask >> h) & 1) tiles += (net.fc[h].K + 127) >> 7;
+    return tiles;
+}
+
+// The plan of a (non-persistent) tc_launch: R, NT, CTAs, roots of the last CTA, layers, passes, whether the FC2 biases are
+// staged in shared memory, FC2 tiles.  Mirrors the kernel's set-up code.
+void tc_describe(const TcNet &net, const TcIO &io, int32_t *info)
+{
+    const int R = tc_pick_roots(io.B), ctas = (io.B + R - 1) / R, hmask = tc_heads_mask(net, io);
+    int nb2 = 0;
+    for (int h = 0; h < 3; ++h)
+        if ((hmask >> h) & 1) nb2 += net.fc[h].K;
+    const int used = net.nlayers * 128;
+    info[0] = R;
+    info[1] = (R * kRowsPerRoot - 8 + 127) >> 7;
+    info[2] = ctas;
+    info[3] = io.B - (ctas - 1) * R;
+    info[4] = net.nlayers;
+    info[5] = io.npass;
+    info[6] = (used + nb2) * 4 <= kBnSmemBytes;
+    info[7] = tc_fc2_tiles(net, hmask);
+}
+
 int tc_launch(const TcNet &net, const TcIO &io_in, cudaStream_t s, const TreeParams *tp_in)
 {
     TcIO io = io_in;
@@ -924,6 +970,8 @@ int tc_launch(const TcNet &net, const TcIO &io_in, cudaStream_t s, const TreePar
     LZ_REQUIRE(!io.persistent || tp_in, LZ_EINVAL, "tc_launch: persistent search needs tree parameters");
     LZ_REQUIRE(net.A <= 1000, LZ_EINVAL, "tc_launch: action space %d too large for the head scratch of the tensor-core path", net.A);
     LZ_REQUIRE(io.skip_scratch, LZ_EINVAL, "tc_launch: no skip scratch");
+    LZ_REQUIRE(tc_fc2_tiles(net, tc_heads_mask(net, io)) <= kF2MaxTiles, LZ_EINVAL, "tc_launch: %d FC2 tiles exceed the %d of the head scratch",
+               tc_fc2_tiles(net, tc_heads_mask(net, io)), kF2MaxTiles);
     io.dbg = g_dbg;
     io.roots_per_cta = tc_pick_roots(io.B);
     LZ_REQUIRE(!io.persistent || tp.A <= 32, LZ_EINVAL, "tc_launch: the persistent search needs A <= 32 (got %d)", tp.A);
