@@ -115,6 +115,11 @@ int lz_tree_backpropagate_ez(lz_tree *t, int latent_index, const float *d_value_
  * d_traj int32 [B, max_sims+1] -1 padded.  Any pointer may be NULL. */
 int lz_tree_results(lz_tree *t, int32_t *d_visits, float *d_values, int32_t *d_nlegal,
                     int32_t *d_traj, lz_stream s);
+/* Test hook: the key of the tree's tie-break draws, hash(seed, epoch, tree, step, depth) (tree.cuh).  h_epoch is the
+ * epoch the next descent uses (every reset advances it; it lives in device memory, so this synchronises the device and
+ * copies it); h_step_counter is the step the next step-wise descent takes (each one consumes a step; a fused search
+ * uses steps 0 ... num_simulations - 1). */
+int lz_tree_debug_rng(lz_tree *t, uint64_t *h_seed, uint64_t *h_epoch, uint32_t *h_step_counter);
 
 /* ---- ReZero search_with_reuse (cnode.cpp:502-549, 597-652, 701-752, 828-932; SURVEY 8(f) row f-4); works on MuZero trees and,
  * with value-prefix semantics, on EfficientZero trees (ctree_efficientzero/lib/cnode.cpp:603-650, 699-754, 816-874, 960-1072) ----
@@ -290,6 +295,11 @@ int lz_search_collect_host_u8(lz_search *q, const uint8_t *h_obs_u8, const uint8
                               float *d_pred_value, float *d_policy_logits, lz_stream s);
 /* Number of kernel nodes of the search graph this search launched last (any lz_search_run* / lz_search_collect* call). */
 int lz_search_num_kernels(const lz_search *q);
+/* Test hook: the launch plan of lz_search_run, host only.  h_info int32[8]: 1 if the search is one persistent launch of the
+ * tensor-core kernel (else 0 and the next six entries are 0), roots per CTA R, CTAs, roots of the last CTA, 1 if the
+ * exploration-rate table pbc[] is staged in shared memory, 1 if the FC2 biases are, layers of the recurrent program, and the
+ * node slots N of the tree (max_sims + 1). */
+int lz_search_debug_plan(const lz_search *q, int32_t *h_info);
 /* Device pointer of the latent pool (NCHW per slot) for inspection in tests. */
 const float *lz_search_latent_pool(const lz_search *q);
 /* EfficientZero: device LSTM-state pool [(S+1)][B][H], which = 0 / 1 for tuple element 0 / 1 (NULL for MuZero). */

@@ -52,6 +52,7 @@ SIGNATURES = {
     "lz_tree_traverse_ez": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lz_tree_backpropagate_ez": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lz_tree_results": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "lz_tree_debug_rng": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "lz_model_create": (c_int, [ctypes.POINTER(ModelConfig), ctypes.POINTER(c_void_p)]),
     "lz_model_create_mlp": (c_int, [ctypes.POINTER(MlpConfig), ctypes.POINTER(c_void_p)]),
     "lz_model_destroy": (c_int, [c_void_p]),
@@ -84,6 +85,7 @@ SIGNATURES = {
     "lz_search_collect_host_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_int, c_int, c_void_p,
                                           c_void_p, c_void_p]),
     "lz_search_num_kernels": (c_int, [c_void_p]),
+    "lz_search_debug_plan": (c_int, [c_void_p, c_void_p]),
     "lz_search_latent_pool": (c_void_p, [c_void_p]),
     "lz_search_run_with_reuse": (c_int, [c_void_p] * 6),
     "lz_search_run_ez": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -961,6 +961,24 @@ void tc_describe(const TcNet &net, const TcIO &io, int32_t *info)
     info[7] = tc_fc2_tiles(net, hmask);
 }
 
+// The plan of a persistent search launch on a tree of N node slots: R, CTAs, roots of the last CTA, whether pbc[] and the FC2
+// biases are staged in shared memory, layers.  Mirrors the kernel's set-up code.
+void tc_describe_search(const TcNet &net, const TcIO &io, int N, int32_t *info)
+{
+    const int R = tc_pick_roots(io.B), ctas = (io.B + R - 1) / R, hmask = tc_heads_mask(net, io);
+    int nb2 = 0;
+    for (int h = 0; h < 3; ++h)
+        if ((hmask >> h) & 1) nb2 += net.fc[h].K;
+    const bool pbc_smem = (net.nlayers * 128 + N + 1) * 4 <= kBnSmemBytes;
+    const int used = net.nlayers * 128 + (pbc_smem ? N + 1 : 0);
+    info[0] = R;
+    info[1] = ctas;
+    info[2] = io.B - (ctas - 1) * R;
+    info[3] = pbc_smem;
+    info[4] = (used + nb2) * 4 <= kBnSmemBytes;
+    info[5] = net.nlayers;
+}
+
 int tc_launch(const TcNet &net, const TcIO &io_in, cudaStream_t s, const TreeParams *tp_in)
 {
     TcIO io = io_in;

@@ -64,6 +64,7 @@ int tc_conv_layout_bytes();
 int tc_prepare_launch();
 int tc_launch(const TcNet &net, const TcIO &io, cudaStream_t s, const TreeParams *tp = nullptr);
 void tc_describe(const TcNet &net, const TcIO &io, int32_t *info);   // info[8]: the plan of tc_launch(net, io) (net_tc.cu)
+void tc_describe_search(const TcNet &net, const TcIO &io, int N, int32_t *info);   // info[6]: the plan of a persistent search launch
 unsigned long long *tc_debug_buffer();   // device buffer [64] used when env LZ_TC_DEBUG=1
 
 }  // namespace lz

@@ -74,26 +74,34 @@ static RecIO rec_io(const lz_search *q, int sim)
 // (:370-468, :878-1003): [descent] + S x [recurrent_inference, back-up (+ next descent)].  Under reuse every tree goes through the
 // network every simulation (the reference compacts the batch on the host; here the rows of "no inference" trees are computed and
 // ignored, which keeps the loop one static CUDA graph).
+// Persistent search: roots never interact, so the CTA that owns up to 8 roots can run their whole search -- tree
+// back-up / descent and the network -- for all num_simulations inside ONE launch of the tensor-core kernel.
+// EfficientZero stays a multi-kernel graph: its LSTM step is a GEMM over all roots (several launches per simulation).
+static bool persistent_search(const lz_search *q, bool reuse)
+{
+    return !reuse && !q->hpool && q->model->kind == 0 && q->model->math != 0 && q->tree->p.A <= 32;   // tree_persist.cuh: one lane per child
+}
+
+static TcIO persistent_io(const lz_search *q, int deterministic)
+{
+    TcIO io;
+    memset(&io, 0, sizeof(io));
+    io.B = q->B; io.npass = (q->model->math == 1) ? 3 : 1;
+    io.latent_base = q->pool; io.latent_pool_rw = q->pool; io.slot_stride = q->slot_stride;
+    io.ix = q->d_ix; io.ix_rw = q->d_ix; io.action = q->d_action; io.action_rw = q->d_action;
+    io.reward = q->d_reward; io.value = q->d_value; io.policy_logits = q->d_policy;
+    io.persistent = 1; io.nsims = q->S; io.sim0 = 0; io.deterministic = deterministic;
+    io.skip_scratch = q->d_skip;
+    io.pool_cl = 1;      // slots >= 1 are written and read only by this kernel: channels-last (vector loads / stores); slot 0 stays NCHW
+    return io;
+}
+
 static int enqueue_search(lz_search *q, int deterministic, bool reuse, cudaStream_t s)
 {
     int rc;
     lz_tree *t = q->tree;
     t->step_counter = 0;
-    // Persistent search: roots never interact, so the CTA that owns up to 8 roots can run their whole search -- tree
-    // back-up / descent and the network -- for all num_simulations inside ONE launch of the tensor-core kernel.
-    // EfficientZero stays a multi-kernel graph: its LSTM step is a GEMM over all roots (several launches per simulation).
-    if (!reuse && !q->hpool && q->model->kind == 0 && q->model->math != 0 && t->p.A <= 32) {   // tree_persist.cuh: one lane per child
-        TcIO io;
-        memset(&io, 0, sizeof(io));
-        io.B = q->B; io.npass = (q->model->math == 1) ? 3 : 1;
-        io.latent_base = q->pool; io.latent_pool_rw = q->pool; io.slot_stride = q->slot_stride;
-        io.ix = q->d_ix; io.ix_rw = q->d_ix; io.action = q->d_action; io.action_rw = q->d_action;
-        io.reward = q->d_reward; io.value = q->d_value; io.policy_logits = q->d_policy;
-        io.persistent = 1; io.nsims = q->S; io.sim0 = 0; io.deterministic = deterministic;
-        io.skip_scratch = q->d_skip;
-        io.pool_cl = 1;      // slots >= 1 are written and read only by this kernel: channels-last (vector loads / stores); slot 0 stays NCHW
-        return tc_launch(q->model->tc_rec, io, s, &t->p);
-    }
+    if (persistent_search(q, reuse)) return tc_launch(q->model->tc_rec, persistent_io(q, deterministic), s, &t->p);
     TreeStep descent = {};
     descent.traverse = 1; descent.deterministic = deterministic;
     descent.act = q->d_action; descent.is_reset = q->d_is_reset;
@@ -427,6 +435,17 @@ int lz_search_collect_host_u8(lz_search *q, const uint8_t *h_obs_u8, const uint8
 }
 
 int lz_search_num_kernels(const lz_search *q) { return q ? q->num_kernels : 0; }
+
+int lz_search_debug_plan(const lz_search *q, int32_t *h_info)
+{
+    LZ_REQUIRE(q && h_info, LZ_EINVAL, "lz_search_debug_plan: null argument");
+    memset(h_info, 0, 8 * sizeof(int32_t));
+    h_info[7] = q->tree->p.N;
+    if (!persistent_search(q, false)) return LZ_OK;
+    h_info[0] = 1;
+    tc_describe_search(q->model->tc_rec, persistent_io(q, 1), q->tree->p.N, h_info + 1);
+    return LZ_OK;
+}
 const float *lz_search_latent_pool(const lz_search *q) { return q ? q->pool : nullptr; }
 const float *lz_search_hidden_pool(const lz_search *q, int which) { return q ? (which ? q->cpool : q->hpool) : nullptr; }
 

@@ -457,6 +457,18 @@ int lz_tree_select_action(lz_tree *t, float temperature, int deterministic, uint
     return LZ_OK;
 }
 
+int lz_tree_debug_rng(lz_tree *t, uint64_t *h_seed, uint64_t *h_epoch, uint32_t *h_step_counter)
+{
+    LZ_REQUIRE(t && h_seed && h_epoch && h_step_counter, LZ_EINVAL, "lz_tree_debug_rng: null argument");
+    LZ_CUDA_CHECK(cudaDeviceSynchronize());      // the epoch is bumped on the device by every reset
+    unsigned long long epoch = 0;
+    LZ_CUDA_CHECK(cudaMemcpy(&epoch, t->p.rng_epoch, sizeof(epoch), cudaMemcpyDeviceToHost));
+    *h_seed = t->p.rng_seed;
+    *h_epoch = epoch;
+    *h_step_counter = t->step_counter;
+    return LZ_OK;
+}
+
 int lz_tree_results(lz_tree *t, int32_t *d_visits, float *d_values, int32_t *d_nlegal, int32_t *d_traj, lz_stream s)
 {
     LZ_REQUIRE(t, LZ_EINVAL, "lz_tree_results: null tree");

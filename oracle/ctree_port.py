@@ -46,6 +46,11 @@ def lib():
         L.lzo_tree_seed.argtypes = [P, ctypes.c_uint]
         L.lzo_tree_traverse_with_reuse.argtypes = [P, I, F, F, P, P, P, P, P, P, P]
         L.lzo_tree_backpropagate_with_reuse.argtypes = [P, I, F, P, P, P, P, P, P, P]
+        L.lzo_tree_set_tie_hash.argtypes = [P, ctypes.c_uint64, ctypes.c_uint64]
+        L.lzo_tree_set_tie_step.argtypes = [P, ctypes.c_uint]
+        L.lzo_tree_set_tie_variant.argtypes = [P, I]
+        L.lzo_tree_tie_stats_reset.argtypes = [P]
+        L.lzo_tree_tie_stats.argtypes = [P, P]
         _lib = L
     return _lib
 
@@ -91,6 +96,7 @@ class Roots:
         A = action_space_size or (max(max(l) for l in legal_actions_list if len(l)) + 1)
         self.A = A
         self.max_sims = max_sims or 256
+        self.tie_hash = False
         self._h = lib().lzo_tree_create(root_num, A, self.max_sims)
         legal = np.full((root_num, A), -1, np.int32)
         nlegal = np.zeros(root_num, np.int32)
@@ -143,6 +149,25 @@ class Roots:
         ln = np.empty(self.root_num, np.int32)
         lib().lzo_tree_trajectories(self._h, _p(out), _p(ln))
         return [out[i, :ln[i]].tolist() for i in range(self.root_num)]
+
+    def set_tie_hash(self, seed, epoch, step=0, variant=0):
+        """Hash mode: non-deterministic descents draw from the tie list with the device trees' counter-based hash keyed by
+        (seed, epoch, tree, step, depth) instead of rand().  ``step`` is the step of the next traverse (each traverse
+        consumes one).  ``variant`` is for sensitivity tests: 1 always draws the first tie, 2 draws the tie after the hashed one.
+        Also clears the tie statistics."""
+        L = lib()
+        L.lzo_tree_set_tie_hash(self._h, int(seed) & (2 ** 64 - 1), int(epoch) & (2 ** 64 - 1))
+        L.lzo_tree_set_tie_step(self._h, int(step) & (2 ** 32 - 1))
+        L.lzo_tree_set_tie_variant(self._h, int(variant))
+        L.lzo_tree_tie_stats_reset(self._h)
+        self.tie_hash = True
+
+    def tie_stats(self):
+        """descents with more than one tie, hash draws other than the first tie, tie lists with unequal scores (near ties),
+        longest search path"""
+        out = np.zeros(4, np.int64)
+        lib().lzo_tree_tie_stats(self._h, _p(out))
+        return dict(ties=int(out[0]), draws=int(out[1]), near=int(out[2]), max_len=int(out[3]))
 
     def clear(self):
         pass

@@ -3,7 +3,8 @@
 ``batch_backpropagate`` takes ``is_reset_list``.
 
 Tie-breaking: the reference draws ``rand() % len(ties)``; the compiled reference under oracle/_ref is linked with
-oracle/rand_shim.c (rand() == 0), which is element 0 of the tie list = this port's deterministic rule.
+oracle/rand_shim.c (rand() == 0), which is element 0 of the tie list = this port's deterministic rule.  After
+``Roots.set_tie_hash`` the descents draw with the device trees' hash instead (``lz_tree_set_tiebreak(t, 0)``).
 
 TEST INFRASTRUCTURE ONLY -- never imported by the product package ``lightzero_b200``.
 """
@@ -35,9 +36,10 @@ class Roots(_mz.Roots):
 
 
 def batch_traverse(roots, pb_c_base, pb_c_init, discount_factor, min_max_stats_lst, results, virtual_to_play_batch):
-    """ez_tree.pyx batch_traverse (ctree_efficientzero/lib/cnode.cpp:876-958)"""
+    """ez_tree.pyx batch_traverse (ctree_efficientzero/lib/cnode.cpp:876-958): first maximum (rand() == 0), or the hashed
+    draw once ``roots.set_tie_hash`` was called"""
     return _mz.batch_traverse(roots, pb_c_base, pb_c_init, discount_factor, min_max_stats_lst, results,
-                              virtual_to_play_batch, True)
+                              virtual_to_play_batch, not roots.tie_hash)
 
 
 def batch_backpropagate(current_latent_state_index, discount_factor, value_prefixs, values, policies,
