@@ -157,11 +157,13 @@ typedef struct lz_model_config {
     int reward_hidden, value_hidden, policy_hidden;                         /* one hidden layer: 32 */
     float support_min, support_max, support_step;                           /* -300, 301, 1 (value == reward) */
     /* EfficientZeroModel (lzero/model/efficientzero_model.py:20-272): the reward head becomes conv1x1 -> BN -> ReLU ->
-     * LSTM(hc*36 -> lstm_hidden_size) -> BN1d -> ReLU -> MLP and predicts a VALUE PREFIX; 0 = MuZeroModel */
+     * LSTM(hc*h*w -> lstm_hidden_size) -> BN1d -> ReLU -> MLP and predicts a VALUE PREFIX; 0 = MuZeroModel */
     int efficientzero;
     int lstm_hidden_size;          /* 512 (must be a multiple of 16, <= 512) */
 } lz_model_config;
 
+/* Conv models (DownSample representation, common.py:334-366): 84x84 and 96x96 observations give a 6x6 latent grid; 64x64 (the
+ * shipped Atari configs) gives 8x8, with no pooling2 (common.py:357-359).  Other sizes: LZ_EINVAL. */
 int lz_model_create(const lz_model_config *cfg, lz_model **out);
 
 /* MuZeroModelMLP (lzero/model/muzero_model_mlp.py:21-295; vector observations, BASELINE config 1).  The
@@ -181,7 +183,8 @@ int lz_model_set_tensor(lz_model *m, const char *name, const float *h_data, int6
 /* Folds eval-mode BatchNorm into per-channel scale/shift, packs weights for the kernels, uploads. */
 int lz_model_finalize(lz_model *m);
 /* Arithmetic of the latent-grid networks (recurrent_inference and the tail of initial_inference):
- *   0 = fp32 FFMA on the CUDA cores;
+ *   0 = fp32 FFMA on the CUDA cores (6x6 latent grid, 84/96-pixel MuZero models, only: LZ_EINVAL for a 64-pixel or an
+ *       EfficientZero model);
  *   1 = wgmma tensor cores with fp16 hi/lo operand splitting (3 MMAs per product, fp32 accumulate in
  *       registers): fp32-accurate, the mode parity is stated for;
  *   2 = wgmma single fp16 pass (fp32 accumulate): ~3x fewer MMAs, logits accurate to ~1e-3. */
@@ -195,22 +198,23 @@ int lz_debug_tc_stamps(unsigned long long *h_out);
  * stage `stage` and copies that stage's output tensor, byte for byte, to d_out (out_bytes must be large enough).
  * Stages: 0 stem -> T0, 1 resblocks1 -> T1 (phase-split), 2 / 3 downsample conv1 / conv3 (one launch) -> U0 / U1,
  * 4 downsample conv2 + identity -> U2, 5 resblocks2 -> U0, 6 pooling1 -> V0, 7 resblocks3 -> V1, 8 pooling2 -> the
- * f32 NCHW pre-latent [B][64][6][6].  Stages 0-7 copy the tensor-core layout (conv_tc.cuh):
+ * f32 NCHW pre-latent [B][64][6][6] (84 / 96 px); at 64 px the tower has no pooling2 and stage 8 is the conversion of V1 to
+ * the f32 NCHW pre-latent [B][64][8][8] (each value hi + lo, summed in fp32).  Stages 0-7 copy the tensor-core layout (conv_tc.cuh):
  * [B][nphase][hi | lo][C / 8][plane_rows][8] fp16.
  * h_info (int32[10]) receives the tensor geometry and the plan of the launch that wrote it:
- * C, H, W, nphase, plane_rows (nphase = plane_rows = 0 for stage 8), then G (images per CTA), band_h (output rows per
- * CTA; 0 where the launch has no bands), stages (weight ring depth; 0 off the wgmma kernels) and the CTA count of the
+ * C, H, W, nphase, plane_rows (nphase = plane_rows = 0 for stage 8), then G (images per CTA; 1 for the pools and the
+ * conversion), band_h (output rows per CTA; 0 where the launch has no bands), stages (weight ring depth; 0 off the wgmma kernels) and the CTA count of the
  * launch, then npass (3 = tc3, 1 = tc1).  Needs a finalized conv model with math != 0 (LZ_ESTATE otherwise). */
 int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uint8_t *d_obs_u8, int stage,
                                void *d_out, size_t out_bytes, int32_t *h_info, lz_stream s);
-/* Test hook: runs a copy of the latent-grid tensor-core program (`which` 0: recurrent_inference on d_latent f32 [B,64,6,6]
+/* Test hook: runs a copy of the latent-grid tensor-core program (`which` 0: recurrent_inference on d_latent f32 [B,64,h,w]
  * NCHW and d_action int32 [B]; 1: the tail of initial_inference on the pre-latent d_latent, d_action unused) cut off after
- * layer `stage`, and writes that layer's f32 output [B,64,6,6] NCHW to d_out.  The model's own programs are not changed.
+ * layer `stage`, and writes that layer's f32 output [B,64,h,w] NCHW to d_out (h = w = lz_model_latent_hw: 6 or 8).  The model's own programs are not changed.
  * stage == nlayers runs the whole program twice and writes, f32: reward logits [B,K], value logits [B,K], policy logits
  * [B,A], reward [B], value [B] with the raw logits requested, then policy logits [B,A], reward [B], value [B] without raw
  * reward / value logits (the joint categorical read-out of the search), then for EfficientZero (`which` 0) the reward-head
- * features [B, reward_head_channels*36] the LSTM consumes.  Sections a program does not produce are zero.
- * h_info (int32[8]) receives the launch plan: roots per CTA R, row tiles NT, CTA count, roots of the last CTA, layers of
+ * features [B, reward_head_channels*h*w] the LSTM consumes (h*w = 36 or 64).  Sections a program does not produce are zero.
+ * h_info (int32[8]) receives the launch plan: roots per CTA R (<= 8 on the 6x6 grid, <= 4 on 8x8), row tiles NT (<= 3), CTA count, roots of the last CTA, layers of
  * the launched program, MMA passes, 1 if the FC2 biases are staged in shared memory, FC2 tiles. */
 int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_latent, const int32_t *d_action, int stage,
                              void *d_out, size_t out_bytes, int32_t *h_info, lz_stream s);
@@ -286,7 +290,7 @@ int lz_search_collect_host(lz_search *q, const float *h_obs, const uint8_t *h_ma
 /* The same two entry points for uint8 frames [B,obs_c,H,W] (Atari frames as the emulator delivers them; a quarter of the
  * bytes on the wire).  The [0, 1] scaling of the reference's env wrapper (ScaledFloatFrameWrapper: obs / 255 -> float32,
  * zoo/atari/envs/atari_wrappers.py:219-220, atari_lightzero_env.py:87-88) is applied inside the first conv kernel, bit-identical
- * to that host arithmetic.  tensor-core conv model with 84x84 / 96x96 frames only. */
+ * to that host arithmetic.  Tensor-core conv model (math mode 1 or 2) only; 64x64, 84x84 and 96x96 frames. */
 int lz_search_collect_u8(lz_search *q, const uint8_t *d_obs_u8, const uint8_t *d_mask, const float *d_noise,
                          float noise_weight, const int32_t *d_to_play, int deterministic,
                          float *d_pred_value, float *d_policy_logits, lz_stream s);

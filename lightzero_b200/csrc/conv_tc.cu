@@ -480,6 +480,22 @@ __global__ void k_pool_tcl(Tcl in, Tcl out, float *out_nchw, int B, int Hout)
     }
 }
 
+// TCL -> fp32 NCHW, no pooling (the 64-pixel tower ends on the 8x8 grid: DownSample has no pooling2 there, common.py:357-359).
+// Each value is hi + lo, the same sum tcl_load8 gives the pools.
+__global__ void k_tcl_to_nchw(Tcl in, float *out_nchw, int B)
+{
+    const int kgs = in.C / 8, H = in.H, W = in.W;
+    const size_t n = (size_t)B * kgs * H * W;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const int x = (int)(i % W), y = (int)((i / W) % H);
+        const int kg = (int)((i / ((size_t)W * H)) % kgs), img = (int)(i / ((size_t)W * H * kgs));
+        float v[8];
+        tcl_load8(in, img, kg, (y + 1) * in.pitch + x, v);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) out_nchw[((size_t)img * in.C + kg * 8 + j) * H * W + y * W + x] = v[j];
+    }
+}
+
 // ---------------------------------------------------------------------------------------------- host
 int conv_tc_prepare_launch()
 {
@@ -584,6 +600,19 @@ int pool_tcl_to_nchw_launch(const Tcl &in, float *out, int B, int Hout, cudaStre
     k_pool_tcl<<<(int)std::min<size_t>((n + 255) / 256, kNumSMs * 32), 256, 0, s>>>(in, dummy, out, B, Hout);
     LZ_KERNEL_CHECK();
     return LZ_OK;
+}
+
+int tcl_to_nchw_launch(const Tcl &in, float *out, int B, cudaStream_t s)
+{
+    k_tcl_to_nchw<<<tcl_to_nchw_ctas(in, B), 256, 0, s>>>(in, out, B);
+    LZ_KERNEL_CHECK();
+    return LZ_OK;
+}
+
+int tcl_to_nchw_ctas(const Tcl &in, int B)
+{
+    const size_t n = (size_t)B * (in.C / 8) * in.H * in.W;
+    return (int)std::min<size_t>((n + 255) / 256, kNumSMs * 32);
 }
 
 }  // namespace lz

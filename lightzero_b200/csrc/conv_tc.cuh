@@ -78,5 +78,8 @@ size_t conv_tc_packed_bytes(int cin, int ncols);
 // pooling on TCL tensors: AvgPool2d(3, stride 2, pad 1), count_include_pad -> /9
 int pool_tcl_launch(const Tcl &in, const Tcl &out, int B, cudaStream_t s);                 // TCL -> TCL
 int pool_tcl_to_nchw_launch(const Tcl &in, float *out, int B, int Hout, cudaStream_t s);   // TCL -> fp32 NCHW
+// TCL -> fp32 NCHW at the same size (hi + lo; the 64-pixel tower's last step), and the CTAs that launch uses
+int tcl_to_nchw_launch(const Tcl &in, float *out, int B, cudaStream_t s);
+int tcl_to_nchw_ctas(const Tcl &in, int B);
 
 }  // namespace lz

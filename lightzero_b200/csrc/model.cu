@@ -488,7 +488,7 @@ static int reserve_tc_skip(lz_model *m, int B)
     ++m->generation;
     cudaFree(m->tc_skip);
     m->tc_skip = nullptr; m->tc_skip_B = 0;
-    int rc = dev_alloc(&m->tc_skip, (size_t)kActFloats * B);
+    int rc = dev_alloc(&m->tc_skip, (size_t)m->latent_floats * B);
     if (rc != LZ_OK) return rc;
     m->tc_skip_B = B;
     return LZ_OK;
@@ -504,7 +504,7 @@ int model_reserve(lz_model *m, int B)
         ++m->generation;
         cudaFree(m->ez_feat); cudaFree(m->ez_htmp);
         m->ez_feat = m->ez_htmp = nullptr;
-        int rc = dev_alloc(&m->ez_feat, (size_t)B * m->cfg.reward_head_channels * kP);
+        int rc = dev_alloc(&m->ez_feat, (size_t)B * m->cfg.reward_head_channels * m->P);
         if (rc == LZ_OK) rc = dev_alloc(&m->ez_htmp, (size_t)B * m->cfg.lstm_hidden_size);
         if (rc != LZ_OK) return rc;
         m->ez_B = B;
@@ -513,7 +513,7 @@ int model_reserve(lz_model *m, int B)
     ++m->generation;
     size_t per_root = 0;
     for (const ConvG &L : m->tower) per_root = std::max(per_root, (size_t)L.cout * L.hout * L.wout);
-    per_root = std::max(per_root, (size_t)kActFloats);
+    per_root = std::max(per_root, (size_t)m->latent_floats);
     for (int i = 0; i < 3; ++i) {
         if (m->ws[i]) cudaFree(m->ws[i]);
         m->ws[i] = nullptr;
@@ -617,13 +617,14 @@ static int tower_tc_run(lz_model *m, int B, const float *d_obs, float *pre_laten
     if (stop_after <= 6) return LZ_OK;
     if ((rc = rb(m->tower_rb[2], m->V0, m->V1))) return rc;                           // resblocks3.0
     if (stop_after <= 7) return LZ_OK;
-    return pool_tcl_to_nchw_launch(m->V1, pre_latent, B, kHW, s);                    // pooling2 -> [B][64][6][6]
+    if (m->hw == 8) return tcl_to_nchw_launch(m->V1, pre_latent, B, s);             // 64 px: no pooling2 -> [B][64][8][8]
+    return pool_tcl_to_nchw_launch(m->V1, pre_latent, B, m->hw, s);                  // pooling2 -> [B][64][6][6]
 }
 
 // tensor-core path only: the DownSample tower alone (obs -> pre-latent [B][64][36]) ...
 int model_initial_tower(lz_model *m, int B, const float *d_obs, float *pre_latent, cudaStream_t s, const uint8_t *d_obs_u8)
 {
-    LZ_REQUIRE(m->kind == 0 && m->math != 0 && m->cfg.obs_h != 64, LZ_ESTATE, "model_initial_tower: tensor-core conv model only");
+    LZ_REQUIRE(m->kind == 0 && m->math != 0, LZ_ESTATE, "model_initial_tower: tensor-core conv model only");
     LZ_REQUIRE(B <= m->ws_B, LZ_ESTATE, "model_initial_tower: workspace sized for %d roots, got %d", m->ws_B, B);
     return tower_tc_run(m, B, d_obs, pre_latent, s, d_obs_u8);
 }
@@ -648,7 +649,7 @@ int model_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, c
     float *a = m->ws[0], *b = m->ws[1], *c = m->ws[2];
     const std::vector<ConvG> &T = m->tower;
     int rc;
-    if (m->math != 0 && m->cfg.obs_h != 64) {
+    if (m->math != 0) {
         if ((rc = tower_tc_run(m, B, d_obs, a, s))) return rc;
         return model_initial_tail(m, B, a, io_in, s);
     }
@@ -665,16 +666,11 @@ int model_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, c
     if ((rc = launch_pool(b, a, B * kC, h2, h3, s))) return rc;                    // pooling1
     if ((rc = launch_convg(T[8], a, b, nullptr, 1, B, s))) return rc;              // resblocks3.0
     if ((rc = launch_convg(T[9], b, c, a, 1, B, s))) return rc;
-    const float *pre = c;
-    if (m->cfg.obs_h != 64) {                                                      // pooling2 for 84 / 96
-        const int h4 = (h3 - 1) / 2 + 1;
-        if ((rc = launch_pool(c, a, B * kC, h3, h4, s))) return rc;
-        pre = a;
-    }
-    if (m->math != 0) return model_initial_tail(m, B, pre, io_in, s);
+    const int h4 = (h3 - 1) / 2 + 1;                                               // pooling2 (84 / 96 px: this path is 6x6 only)
+    if ((rc = launch_pool(c, a, B * kC, h3, h4, s))) return rc;
     TailIO io = io_in;
     io.B = B;
-    io.pre_latent = pre;
+    io.pre_latent = a;
     switch (pick_W(B)) {
         case 8: return launch_tail<8>(m->net, io, s);
         case 4: return launch_tail<4>(m->net, io, s);
@@ -868,6 +864,7 @@ static int pack_tc(lz_model *m, const NetDev &net)
 {
     const lz_model_config &c = m->cfg;
     const int A = c.action_space_size, n = c.num_res_blocks;
+    const int hw = m->hw, P = m->P, nfc1 = 16 * P / 32;      // latent grid, pixels, FC1 stages (16 P inputs at most)
     const int nconv = 1 + 6 * n;
     const size_t conv_bytes = (size_t)tc_conv_layout_bytes();
     const size_t off_convw = 0;
@@ -876,13 +873,13 @@ static int pack_tc(lz_model *m, const NetDev &net)
     const size_t off_headbn = off_bn + (size_t)nconv * 128 * 4;
     const size_t off_abias = off_headbn + 96 * 4;
     // FC weight stream of the heads (16 KB stages for the shared-memory ring of k_net_tc, fp16 hi / lo, the weights are the
-    // tensor cores' M operand): 18 FC1 stages covering all three heads, then one stage per 128-output tile of each head's FC2
+    // tensor cores' M operand): 16 P / 32 FC1 stages covering all three heads, then one stage per 128-output tile of each head's FC2
     const std::string fc_names[3] = {"dynamics_network.fc_reward_head", "prediction_network.fc_value", "prediction_network.fc_policy"};
     const Head *fc_heads[3] = {&net.reward, &net.value, &net.policy};
     size_t fc_off2[3];
-    size_t off_fc = (off_abias + (size_t)A * kC * kP * 4 + 127) & ~(size_t)127;
+    size_t off_fc = (off_abias + (size_t)A * kC * P * 4 + 127) & ~(size_t)127;
     const size_t off_fc0 = off_fc;
-    off_fc += (size_t)18 * 12288;
+    off_fc += (size_t)nfc1 * 12288;
     for (int h = 0; h < 3; ++h) {
         fc_off2[h] = off_fc - off_fc0;
         if (fc_heads[h]->hid > 0) off_fc += (size_t)((fc_heads[h]->K + 127) / 128) * 16384;      // EfficientZero: the reward head's FC part lives in ez.cu
@@ -912,16 +909,16 @@ static int pack_tc(lz_model *m, const NetDev &net)
         if (ci == 0) {   // one-hot action planes (muzero_model.py:341-369): border-aware tap sums, times the BN scale
             for (int a = 0; a < A; ++a)
                 for (int co = 0; co < kC; ++co)
-                    for (int y = 0; y < kHW; ++y)
-                        for (int x = 0; x < kHW; ++x) {
+                    for (int y = 0; y < hw; ++y)
+                        for (int x = 0; x < hw; ++x) {
                             float acc = 0.0f;
                             for (int ky = 0; ky < 3; ++ky)
                                 for (int kx = 0; kx < 3; ++kx) {
                                     const int yy = y + ky - 1, xx = x + kx - 1;
-                                    if (yy < 0 || yy >= kHW || xx < 0 || xx >= kHW) continue;
+                                    if (yy < 0 || yy >= hw || xx < 0 || xx >= hw) continue;
                                     acc += (*w)[((size_t)co * cin_total + kC + a) * 9 + ky * 3 + kx];
                                 }
-                            abias[(((size_t)a * 16 + co / 4) * kP + y * kHW + x) * 4 + co % 4] = acc * scale[co];   // k_net_tc's internal [c / 4][36][c % 4] layout
+                            abias[(((size_t)a * 16 + co / 4) * P + y * hw + x) * 4 + co % 4] = acc * scale[co];   // k_net_tc's internal [c / 4][P][c % 4] layout
                         }
         }
     }
@@ -946,8 +943,8 @@ static int pack_tc(lz_model *m, const NetDev &net)
     for (int h = 0; h < 3; ++h) {
         const Head &H = *fc_heads[h];
         if (H.hid <= 0) continue;
-        const int nin = H.hc * kP;
-        LZ_REQUIRE(H.hid <= 32 && H.K <= 608 && nin <= 576, LZ_EINVAL, "lz_model_finalize: tensor-core path needs head hidden <= 32, head channels <= 16 and support <= 608");
+        const int nin = H.hc * P;
+        LZ_REQUIRE(H.hid <= 32 && H.K <= 608 && nin <= 16 * P, LZ_EINVAL, "lz_model_finalize: tensor-core path needs head hidden <= 32, head channels <= 16 and support <= 608");
         auto W0 = find(m, fc_names[h] + ".0.weight", (size_t)H.hid * nin), W3 = find(m, fc_names[h] + ".3.weight", (size_t)H.K * H.hid);
         if (!W0 || !W3) return LZ_EINVAL;
         auto pow2_scale = [](const std::vector<float> &w) {
@@ -996,12 +993,13 @@ static int pack_tc(lz_model *m, const NetDev &net)
     base.fcw = m->d_tc + off_fc0;
     for (int h = 0; h < 3; ++h) {
         base.fc[h].fc2_off = (uint32_t)fc_off2[h];
-        base.fc[h].nin = fc_heads[h]->hid > 0 ? fc_heads[h]->hc * kP : 0;
+        base.fc[h].nin = fc_heads[h]->hid > 0 ? fc_heads[h]->hc * P : 0;
         base.fc[h].K = fc_heads[h]->hid > 0 ? fc_heads[h]->K : 0;
         base.fc[h].fc1_inv = fc1_inv[h]; base.fc[h].fc2_inv = fc2_inv[h];
     }
     base.hc[0] = c.reward_head_channels; base.hc[1] = c.value_head_channels; base.hc[2] = c.policy_head_channels;
     base.A = A; base.support_min = c.support_min; base.support_step = c.support_step;
+    base.hw = hw;
     // conv indices: 0 dyn conv | 1..2n dyn blocks | 2n+1..4n pred blocks | 4n+1..6n rep blocks
     TcNet rec = base, tail = base;
     int L = 0;
@@ -1039,8 +1037,8 @@ int lz_model_create(const lz_model_config *cfg, lz_model **out)
 {
     LZ_REQUIRE(cfg && out, LZ_EINVAL, "lz_model_create: null argument");
     LZ_REQUIRE(cfg->num_channels == kC, LZ_EINVAL, "lz_model_create: num_channels must be %d (got %d)", kC, cfg->num_channels);
-    LZ_REQUIRE(cfg->obs_h == cfg->obs_w && (cfg->obs_h == 84 || cfg->obs_h == 96), LZ_EINVAL,
-               "lz_model_create: observation %dx%d not supported (84x84 and 96x96 -> 6x6 latent)", cfg->obs_h, cfg->obs_w);
+    LZ_REQUIRE(cfg->obs_h == cfg->obs_w && (cfg->obs_h == 64 || cfg->obs_h == 84 || cfg->obs_h == 96), LZ_EINVAL,
+               "lz_model_create: observation %dx%d not supported (64x64 -> 8x8 latent, 84x84 and 96x96 -> 6x6 latent)", cfg->obs_h, cfg->obs_w);
     LZ_REQUIRE(cfg->num_res_blocks >= 1 && cfg->num_res_blocks <= kMaxResBlocks, LZ_EINVAL, "lz_model_create: num_res_blocks must be in [1,%d]", kMaxResBlocks);
     LZ_REQUIRE(cfg->reward_head_channels <= 16 && cfg->value_head_channels <= 16 && cfg->policy_head_channels <= 16, LZ_EINVAL, "lz_model_create: head channels must be <= 16");
     LZ_REQUIRE(cfg->reward_hidden <= 32 && cfg->value_hidden <= 32 && cfg->policy_hidden <= 32, LZ_EINVAL, "lz_model_create: head hidden sizes must be <= 32");
@@ -1056,11 +1054,13 @@ int lz_model_create(const lz_model_config *cfg, lz_model **out)
     m->cfg = *cfg;
     m->ez_feat = m->ez_htmp = nullptr; m->ez_B = 0; m->d_ez_wtc = nullptr;
     m->kind = 0;
-    m->latent_floats = kC * kP;
+    // DownSample (common.py:334-366): 64 px -> 8x8 (no pooling2), 84 / 96 px -> 6x6
+    const int hw = cfg->obs_h == 64 ? 8 : kHW;
+    m->latent_floats = kC * hw * hw;
     memset(&m->mcfg, 0, sizeof(m->mcfg));
     m->finalized = false;
     m->d_weights = nullptr;
-    m->hw = kHW; m->P = kP; m->K = K;
+    m->hw = hw; m->P = hw * hw; m->K = K;
     m->ws[0] = m->ws[1] = m->ws[2] = nullptr;
     m->ws_floats = 0; m->ws_B = 0;
     m->math = 1; m->d_tc = nullptr;   // default: tensor-core 3xFP16 (fp32-accurate)
@@ -1131,15 +1131,15 @@ int lz_model_finalize(lz_model *m)
              pack_conv3(m, P, "representation_network.resblocks." + si + ".conv2.0.weight", "representation_network.resblocks." + si + ".conv2.1", kC, kC, rep_res[2 * i + 1]);
     }
     if (!ok) return LZ_EINVAL;
-    ok = pack_head(m, P, D + "conv1x1_reward", D + "norm_reward", c.efficientzero ? std::string() : D + "fc_reward_head", c.reward_head_channels, c.reward_hidden, m->K, kP, hr) &&
-         pack_head(m, P, Q + "conv1x1_value", Q + "norm_value", Q + "fc_value", c.value_head_channels, c.value_hidden, m->K, kP, hv) &&
-         pack_head(m, P, Q + "conv1x1_policy", Q + "norm_policy", Q + "fc_policy", c.policy_head_channels, c.policy_hidden, A, kP, hp);
+    ok = pack_head(m, P, D + "conv1x1_reward", D + "norm_reward", c.efficientzero ? std::string() : D + "fc_reward_head", c.reward_head_channels, c.reward_hidden, m->K, m->P, hr) &&
+         pack_head(m, P, Q + "conv1x1_value", Q + "norm_value", Q + "fc_value", c.value_head_channels, c.value_hidden, m->K, m->P, hv) &&
+         pack_head(m, P, Q + "conv1x1_policy", Q + "norm_policy", Q + "fc_policy", c.policy_head_channels, c.policy_hidden, A, m->P, hp);
     if (!ok) return LZ_EINVAL;
     // ---- EfficientZero value-prefix head (efficientzero_model.py:511-525, 556-569)
     float ez_scale = 1.0f;
     size_t ez_wcat = 0, ez_bias = 0, ez_vps = 0, ez_vpt = 0, ez_fc1 = 0, ez_s2 = 0, ez_t2 = 0, ez_fc2 = 0, ez_b2 = 0;
     if (c.efficientzero) {
-        const int H = c.lstm_hidden_size, nin = c.reward_head_channels * kP, hid = c.reward_hidden, K = m->K;
+        const int H = c.lstm_hidden_size, nin = c.reward_head_channels * m->P, hid = c.reward_hidden, K = m->K;
         auto Wih = find(m, D + "lstm.weight_ih_l0", (size_t)4 * H * nin), Whh = find(m, D + "lstm.weight_hh_l0", (size_t)4 * H * H);
         auto bih = find(m, D + "lstm.bias_ih_l0", (size_t)4 * H), bhh = find(m, D + "lstm.bias_hh_l0", (size_t)4 * H);
         auto W0 = find(m, D + "fc_reward_head.0.weight", (size_t)hid * H), B0 = find(m, D + "fc_reward_head.0.bias", hid);
@@ -1200,7 +1200,7 @@ int lz_model_finalize(lz_model *m)
         EzNet &e = m->ez;
         e.wcat = base + ez_wcat; e.bias = base + ez_bias; e.vp_s = base + ez_vps; e.vp_t = base + ez_vpt;
         e.fc1 = base + ez_fc1; e.s2 = base + ez_s2; e.t2 = base + ez_t2; e.fc2 = base + ez_fc2; e.b2 = base + ez_b2;
-        e.nin = c.reward_head_channels * kP; e.H = c.lstm_hidden_size; e.hid = c.reward_hidden; e.K = m->K;
+        e.nin = c.reward_head_channels * m->P; e.H = c.lstm_hidden_size; e.hid = c.reward_hidden; e.K = m->K;
         e.support_min = c.support_min; e.support_step = c.support_step;
         e.wtc = m->d_ez_wtc; e.wtc_inv_scale = 1.0f / ez_scale;
         int rc3 = ez_prepare_launch();
@@ -1230,16 +1230,14 @@ int lz_model_finalize(lz_model *m)
         memcpy(SP.shift, P.host.data() + tower[0].shift, sizeof(SP.shift));
         m->stem_valid = 1;
     }
-    const int h4 = (h3 - 1) / 2 + 1;
-    LZ_REQUIRE(h4 == kHW, LZ_EINVAL, "lz_model_finalize: latent grid %d != %d", h4, kHW);
+    const int h4 = (h3 - 1) / 2 + 1, grid = h0 == 64 ? h3 : h4;      // 64 px: no pooling2
+    LZ_REQUIRE(grid == m->hw && (grid == 6 || grid == 8), LZ_EINVAL, "lz_model_finalize: latent grid %d is neither 6 nor 8", grid);
     rc = model_prepare_launch();
     if (rc != LZ_OK) return rc;
     rc = pack_tc(m, net);
     if (rc != LZ_OK) return rc;
-    if (c.obs_h != 64) {
-        rc = pack_tower_tc(m);
-        if (rc != LZ_OK) return rc;
-    }
+    rc = pack_tower_tc(m);
+    if (rc != LZ_OK) return rc;
     m->finalized = true;
     m->tensors.clear();
     return LZ_OK;
@@ -1250,6 +1248,9 @@ int lz_model_set_math(lz_model *m, int mode)
     LZ_REQUIRE(m && mode >= 0 && mode <= 2, LZ_EINVAL, "lz_model_set_math: mode must be 0 (fp32 FFMA), 1 (tensor-core 3xFP16) or 2 (tensor-core fp16)");
     LZ_REQUIRE(m->kind == 0 || mode == 0, LZ_EINVAL, "lz_model_set_math: the MLP model only has the fp32 path");
     LZ_REQUIRE(!(m->kind == 0 && m->cfg.efficientzero && mode == 0), LZ_EINVAL, "lz_model_set_math: the EfficientZero model runs its conv stack on the tensor-core path only (mode 1 or 2)");
+    LZ_REQUIRE(!(m->kind == 0 && m->hw != kHW && mode == 0), LZ_EINVAL,
+               "lz_model_set_math: the fp32 FFMA path runs the 6x6 latent grid only; this %dx%d-observation model (%dx%d latent) runs on the tensor-core path (mode 1 or 2)",
+               m->cfg.obs_h, m->cfg.obs_w, m->hw, m->hw);
     if (m->math != mode) ++m->generation;      // captured search graphs bake the path (and pass count) in
     m->math = mode;
     return LZ_OK;
@@ -1298,7 +1299,7 @@ int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uin
 {
     LZ_REQUIRE(m && B > 0 && (d_obs == nullptr) != (d_obs_u8 == nullptr) && d_out && h_info && stage >= 0 && stage <= 8, LZ_EINVAL,
                "lz_model_debug_tower_stage: bad argument");
-    LZ_REQUIRE(m->finalized && m->kind == 0 && m->cfg.obs_h != 64, LZ_ESTATE, "lz_model_debug_tower_stage: not a finalized conv model with a tensor-core tower");
+    LZ_REQUIRE(m->finalized && m->kind == 0, LZ_ESTATE, "lz_model_debug_tower_stage: not a finalized conv model with a tensor-core tower");
     LZ_REQUIRE(m->math != 0, LZ_ESTATE, "lz_model_debug_tower_stage: math mode 0 does not run the tensor-core tower");
     if (B > m->ws_B) {
         int rc = model_reserve(m, B);
@@ -1314,8 +1315,8 @@ int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uin
         info[0] = t.C; info[1] = t.H; info[2] = t.W; info[3] = t.nphase; info[4] = t.plane_rows;
         bytes = (size_t)B * t.img_stride;
     } else {
-        info[0] = kC; info[1] = kHW; info[2] = kHW;                    // fp32 NCHW: nphase = plane_rows = 0
-        bytes = (size_t)B * kC * kHW * kHW * sizeof(float);
+        info[0] = kC; info[1] = m->hw; info[2] = m->hw;                // fp32 NCHW: nphase = plane_rows = 0
+        bytes = (size_t)B * m->latent_floats * sizeof(float);
     }
     LZ_REQUIRE(out_bytes >= bytes, LZ_EINVAL, "lz_model_debug_tower_stage: stage %d needs %zu bytes, got %zu", stage, bytes, out_bytes);
     const ConvG &S0 = m->tower[0];
@@ -1347,7 +1348,7 @@ int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uin
         case 5: rb_plan(m->tower_rb[1]); break;
         case 6: info[5] = 1; info[8] = pool_ctas(m->U0, m->V0.H); break;
         case 7: rb_plan(m->tower_rb[2]); break;
-        default: info[5] = 1; info[8] = pool_ctas(m->V1, kHW); break;
+        default: info[5] = 1; info[8] = m->hw == 8 ? tcl_to_nchw_ctas(m->V1, B) : pool_ctas(m->V1, m->hw); break;
     }
     info[9] = (m->math == 1) ? 3 : 1;
     const cudaStream_t st = (cudaStream_t)s;
@@ -1367,13 +1368,13 @@ int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_laten
     TcNet net = which ? m->tc_tail : m->tc_rec;          // a copy: the model's programs stay as they are
     const int nl = net.nlayers, K = m->K, A = m->cfg.action_space_size;
     const bool ez = m->cfg.efficientzero != 0 && which == 0;
-    const int nfeat = ez ? m->cfg.reward_head_channels * kP : 0;
+    const int nfeat = ez ? m->cfg.reward_head_channels * m->P : 0;
     LZ_REQUIRE(stage <= nl, LZ_EINVAL, "lz_model_debug_net_stage: stage %d past the %d layers of the program", stage, nl);
     {
         int rc = model_reserve(m, B);
         if (rc != LZ_OK) return rc;
     }
-    const size_t nfl = stage < nl ? (size_t)B * kActFloats : (size_t)B * (2 * K + 2 * A + 4 + nfeat);
+    const size_t nfl = stage < nl ? (size_t)B * m->latent_floats : (size_t)B * (2 * K + 2 * A + 4 + nfeat);
     LZ_REQUIRE(out_bytes >= nfl * sizeof(float), LZ_EINVAL, "lz_model_debug_net_stage: stage %d needs %zu bytes, got %zu", stage,
                nfl * sizeof(float), out_bytes);
     const cudaStream_t st = (cudaStream_t)s;

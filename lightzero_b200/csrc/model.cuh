@@ -55,7 +55,7 @@ struct RecIO {
     float *reward, *value;            // [B] scalars or nullptr
     float *policy_logits;             // [B][A] or nullptr
     float *reward_logits, *value_logits;   // [B][K] or nullptr
-    float *skip_scratch;              // [B][2304] scratch of the tensor-core path (nullptr: the model's own, lz_model::tc_skip)
+    float *skip_scratch;              // [B][64 P] scratch of the tensor-core path (nullptr: the model's own, lz_model::tc_skip)
     // EfficientZero (reward == value prefix): LSTM state in / out, see ez.cuh
     const float *h_base, *c_base;     // base + ix[b]*hslot_stride + b*H
     size_t hslot_stride;
@@ -81,7 +81,7 @@ struct lz_model {
     float *ez_feat, *ez_htmp;         // [ws_B][hc*36], [ws_B][H] scratch between the conv kernel and the LSTM kernels
     int ez_B;
     unsigned char *d_ez_wtc;          // LSTM weights in the tensor-core layout (ez.cu)
-    int latent_floats;                // floats per root latent (64*36 or latent_dim)
+    int latent_floats;                // floats per root latent (64*36, 64*64 or latent_dim)
     lz_mlp_config mcfg;
     lz::MlpNet mlp;
     lz_model_config cfg;
@@ -97,7 +97,7 @@ struct lz_model {
     int math;                         // 0 = fp32 FFMA (net6.cuh), 1 = tensor-core 3xFP16 (fp32-accurate), 2 = tensor-core fp16 single pass
     unsigned char *d_tc;              // packed fp16 hi/lo weights + tables of the tensor-core path
     lz::TcNet tc_rec, tc_tail;
-    float *tc_skip;                   // [tc_skip_B][2304] ResBlock skip scratch of k_net_tc for launches outside a search (model_reserve)
+    float *tc_skip;                   // [tc_skip_B][64 P] ResBlock skip scratch of k_net_tc for launches outside a search (model_reserve)
     int tc_skip_B;
     // tensor-core DownSample tower: packed weights / folded BN per layer, TCL activation workspace
     unsigned char *d_tower;           // weights + scale/shift tables

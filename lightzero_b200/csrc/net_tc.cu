@@ -1,6 +1,7 @@
 // net_tc.cu -- tensor-core (wgmma) path of the MuZero latent-grid networks for sm_90a.
 //
-// One CTA runs the WHOLE recurrent_inference (or the latent-grid tail of initial_inference) for up to 8 roots -- and, in persistent
+// One CTA runs the WHOLE recurrent_inference (or the latent-grid tail of initial_inference) for up to 8 roots (6x6 grid; 4 on the
+// 8x8 grid of 64-pixel observations, see TcGeo) -- and, in persistent
 // mode, the whole num_simulations loop of their search (tree back-up + descent by one warp per tree, tree_persist.cuh): five 3x3
 // convolutions, three 1x1 head convolutions and the heads' fully connected layers as wgmma with fp32 accumulators in registers;
 // BatchNorm / residual / ReLU epilogues and the softmax expectation + inverse scalar transform on chip.  Activations never leave the SM.
@@ -13,8 +14,9 @@
 //
 // Implicit GEMM without im2col: activations live in shared memory as [k-group of 8 channels][row][8 halves] (the wgmma K-major
 // no-swizzle canonical layout with SBO = 128 B, so row r of the operand is at start + 16*r bytes).  Rows are the pixels of a 7-wide
-// padded grid (49 rows per root, column 6 and row 6 zero), so the input of output row m for tap (dy,dx) is row m + 7*dy + dx: each of
-// the 9 taps is the SAME buffer addressed through a descriptor whose start address is shifted by (7*dy+dx)*16 bytes.  The zero pad
+// padded grid (49 rows per root, column 6 and row 6 zero; 9-wide, 81 rows on the 8x8 grid), so the input of output row m for tap
+// (dy,dx) is row m + 7*dy + dx: each of the 9 taps is the SAME buffer addressed through a descriptor whose start address is shifted
+// by (7*dy+dx)*16 bytes.  The zero pad
 // rows double as the conv padding between rows and between consecutive roots.  The rows are cut into 128-row tiles; warpgroup g
 // computes rows [64 g, 64 g + 64) of every tile and keeps all of a layer's accumulators in registers (3 tiles x 32 per thread) until
 // every MMA of the layer has read the buffer; the epilogue then rewrites the buffer IN PLACE, one tile at a time through a 128-row
@@ -43,15 +45,7 @@ namespace lz {
 // ---------------------------------------------------------------------------------------------- geometry
 constexpr int kEpiWarps = 8, kEpiThreads = kEpiWarps * 32;   // two consumer warpgroups
 constexpr int kTcThreads = kEpiThreads + 32;                 // + the weight producer warp
-constexpr int kPitch = 7, kRowsPerRoot = 49;     // padded 7x7 grid per root
-// 8 roots = 392 grid rows, but the last 8 rows of a root (pixel (5, 6) and grid row 6) are padding: the output rows that hold
-// pixels end at 49 R - 8 = 384 = 3 tiles of 128, and the rows the taps read beyond them are the zeroed trailing margin
-constexpr int kMaxRoots = 8, kMaxTiles = 3;
-constexpr int kMargin = 8;                       // |7*dy+dx| <= 8
-constexpr int kRowsAlloc = kMargin + kMaxTiles * 128 + kMargin;   // 400
-constexpr int kPlaneBytes = kRowsAlloc * 16;     // one k-group (8 fp16 channels) of all rows: 6400 B
-constexpr int kPartBytes = 8 * kPlaneBytes;      // 64 channels: 51200 B
-constexpr int kActBytes = 2 * kPartBytes;        // hi + lo: 102400 B
+constexpr int kMaxTiles = 3;                     // 384 output rows: 3 tiles of 128 (the register accumulator budget)
 constexpr int kTapKgBytes = 128 * 16;            // one k-group (8 input channels) of a tap: 64 hi rows then 64 lo rows of 16 B
 constexpr int kTapBytes = 8 * kTapKgBytes;       // one 3x3 tap, [kg 8][co: 64 hi | 64 lo][ci % 8]: 16384 B
 constexpr int kStages = 3;                       // 16 KB ring stages: conv taps, then the heads' FC weight blocks
@@ -59,14 +53,55 @@ constexpr int kHeadWBytes = 3 * 2 * 16 * 64 * 2; // three 1x1 heads (hc <= 16), 
 constexpr int kBnSmemBytes = kTcMaxLayers * 128 * 4;   // folded BatchNorm tables of the program's layers
 constexpr int kStgLd = 68;                       // fp32 staging rows: 64 columns + 4 (conflict-free 16-byte row reads)
 constexpr int kStgBytes = 128 * kStgLd * 4;      // one 128-row tile of accumulators: 34,816 B
-constexpr int kSmemMain = kActBytes + kStages * kTapBytes + kHeadWBytes + 1024 + kBnSmemBytes + kStgBytes;
-constexpr int kHeadScratch = 72 * 8 * 16 * 2 + kEpiWarps * (16 + 3 * 32) * 4;   // kFrBytes (reward features parked from their hook to the heads' FC pass) + the parked trees (kTreeParkWords per warp)
 // tree <-> network hand-off of the persistent search, per root slot of the CTA: leaf slot, action | value, reward, policy logits
 // (the global copies are still written for the step-wise entry points; reading them back would cost an L2 round trip per use)
 constexpr int kHoWords = 4 + 32;
-constexpr int kHandoffBytes = 8 * kHoWords * 4;
-constexpr int kSmemBytes = kSmemMain + kHeadScratch + kHandoffBytes;
-static_assert(kSmemBytes <= 227 * 1024, "k_net_tc exceeds the 227 KB of shared memory of a block");
+// the tree of a warp (tree_persist.cuh) parked in shared memory while the warp does network work: 16 uniform words + 3 x 32
+// per-lane words
+constexpr int kTreeParkWords = 16 + 3 * 32;
+constexpr int kHbHeadBytes = 4 * 16 * 16;        // FC2 B operand of one head: [4 k-groups][8 roots hi | 8 roots lo][16 B] = 1 KB
+constexpr int kFc1StageBytes = 2 * 2 * 2 * 96 * 16;   // 12,288 B: only the 96 real rows (3 heads x 32 units) of the M = 128 operand are streamed
+
+// The latent grid HW x HW (6 for 84 / 96-pixel observations, 8 for 64) fixes everything that depends on the pixel count.  Rows
+// are the pixels of a padded (HW + 1)-wide grid, (HW + 1)^2 rows per root; the last HW + 2 rows of a root (pixel (HW - 1, HW) and
+// grid row HW) are padding, so the output rows that hold pixels end at R (HW + 1)^2 - (HW + 2):
+//   HW = 6: 8 roots -> 392 - 8 = 384 rows = 3 tiles; activation buffer (8 + 384 + 8) rows x 16 B x 16 planes = 102,400 B
+//   HW = 8: 4 roots -> 324 - 10 = 314 rows -> 3 tiles (5 roots would need 4); (10 + 384 + 10) rows -> 103,424 B
+// The taps read up to |pitch * dy + dx| <= HW + 2 rows beyond the tiles: the zeroed margins.
+template <int HW>
+struct TcGeo {
+    static constexpr int kPix = HW * HW;                          // pixels per root (the P of a [64][P] latent)
+    static constexpr int kPitch = HW + 1, kRowsPerRoot = kPitch * kPitch;
+    static constexpr int kMaxRoots = HW == 6 ? 8 : 4;
+    static constexpr int kRootsLog2 = HW == 6 ? 3 : 2;
+    static constexpr int kMargin = kPitch + 1;
+    static constexpr int kRowsAlloc = kMargin + kMaxTiles * 128 + kMargin;
+    static constexpr int kPlaneBytes = kRowsAlloc * 16;          // one k-group (8 fp16 channels) of all rows
+    static constexpr int kPartBytes = 8 * kPlaneBytes;           // 64 channels
+    static constexpr int kActBytes = 2 * kPartBytes;             // hi + lo
+    // heads (see the heads section): FC1 has 16 P inputs (head channels <= 16) = 2 P k-groups; its B operand holds, per k-group,
+    // 4 kMaxRoots hi rows (row head * kMaxRoots + root, 3 heads + padding) then as many lo rows, +16 B to spread the banks:
+    //   HW = 6: 72 k-groups x (64 rows + 1) x 16 B = 74,880 B, m64n64 MMAs
+    //   HW = 8: 128 k-groups x (32 rows + 1) x 16 B = 67,584 B, m64n32 MMAs (the 8-root layout would take 133 KB)
+    static constexpr int kFc1Kg = 2 * kPix;
+    static constexpr int kFbN = 8 * kMaxRoots;                   // B operand rows = MMA N: hi + lo
+    static constexpr int kFbKgBytes = kFbN * 16 + 16;
+    static constexpr int kFbBytes = kFc1Kg * kFbKgBytes;         // overlays the activation buffer
+    static constexpr int kFrBytes = 2 * kFc1Kg * kMaxRoots * 16; // reward features parked from their hook: [hi | lo][k-group][root][16 B]
+    static constexpr int kFc1Stages = 16 * kPix / 32;            // 32 inputs per 12 KB stage (2 k-steps x (A_hi + A_lo))
+    // FC2 accumulators, hi + lo added: [tile][128 outputs][8 root columns] fp32 over the dead FC1 operand (HW = 8 uses columns
+    // 0-3).  lz_model_finalize takes heads of up to 608 outputs on this path (support and action space alike): 3 x 5 = 15 tiles
+    static constexpr int kF2MaxTiles = HW == 6 ? 18 : 16;
+    static constexpr int kSmemMain = kActBytes + kStages * kTapBytes + kHeadWBytes + 1024 + kBnSmemBytes + kStgBytes;
+    static constexpr int kHeadScratch = kFrBytes + kEpiWarps * kTreeParkWords * 4;   // parked reward features + parked trees
+    static constexpr int kHandoffBytes = kMaxRoots * kHoWords * 4;
+    static constexpr int kSmemBytes = kSmemMain + kHeadScratch + kHandoffBytes;      // 231,552 B (HW = 6), 229,952 B (HW = 8)
+    static_assert(kSmemBytes <= 227 * 1024, "k_net_tc exceeds the 227 KB of shared memory of a block");
+    static_assert(kMaxRoots * kRowsPerRoot - (HW + 2) <= kMaxTiles * 128, "the roots of a CTA must fit the register tiles");
+    static_assert(kF2MaxTiles * 128 * 8 * 4 <= kFbBytes, "FC2 staging must fit under the FC1 operand");
+    static_assert(3 * ((608 + 127) / 128) <= kF2MaxTiles, "FC2 staging must hold the largest heads");
+    static_assert(kFbBytes + 3 * kHbHeadBytes + 2 * 2 * 4 * 4 * 3 * 4 <= kActBytes, "the head scratch must fit the activation buffer");
+};
 
 struct TcBars {
     uint64_t full[kStages], empty[kStages];     // producer -> consumers (complete_tx) / consumer warps -> producer (8 arrivals)
@@ -86,17 +121,7 @@ __device__ __forceinline__ void epi_sync() { asm volatile("bar.sync 1, %0;\n" ::
 //        (net6.cuh), so the softmax expectation runs straight out of the staged accumulators, the 601 logits are never stored.
 // Both products keep the fp32-accurate 3xFP16 scheme: A_hi x [B_hi | B_lo] and A_lo x [B_hi | B_lo] (the extra lo x lo term is
 // harmless), the two column halves are added at read-out.  Warpgroup g computes rows [64 g, 64 g + 64) of each product.
-constexpr int kFbKgBytes = 64 * 16 + 16;                  // FC1 B operand: per k-group 32 hi rows + 32 lo rows of 16 B (+16 B: bank spread)
-constexpr int kFbBytes = 72 * kFbKgBytes;                 // 576 inputs = 72 k-groups: 74,880 B (overlays the activation buffer)
-constexpr int kFrBytes = 72 * 8 * 16 * 2;                 // reward features parked from their hook: [hi | lo][72 k-groups][8 roots][16 B] = 18,432 B
-constexpr int kHbHeadBytes = 4 * 16 * 16;                 // FC2 B operand of one head: [4 k-groups][8 roots hi | 8 roots lo][16 B] = 1 KB
-constexpr int kFc1Stages = 18;                            // 576 inputs / 32 per stage (2 k-steps x (A_hi + A_lo))
-constexpr int kFc1StageBytes = 2 * 2 * 2 * 96 * 16;       // 12,288 B: only the 96 real rows (3 heads x 32 units) of the M = 128 operand are streamed
-// FC2 accumulators, hi + lo added: [tile][128 outputs][8 roots] fp32 over the dead FC1 operand: room for 18 tiles (73,728 B).
-// lz_model_finalize takes heads of up to 608 outputs on this path (support and action space alike): 3 x 5 = 15 tiles
-constexpr int kF2MaxTiles = 18;
-static_assert(kF2MaxTiles * 128 * 8 * 4 <= kFbBytes, "FC2 staging must fit under the FC1 operand");
-static_assert(3 * ((608 + 127) / 128) <= kF2MaxTiles, "FC2 staging must hold the largest heads");
+// On the 8x8 grid (1,024 FC1 inputs, 4 roots per CTA) the FC1 B operand has 16 + 16 rows and FC1 is m64n32 (TcGeo<8>).
 
 __device__ __forceinline__ void put_half(unsigned char *p, float v, float &rem)
 {
@@ -106,72 +131,81 @@ __device__ __forceinline__ void put_half(unsigned char *p, float v, float &rem)
 }
 
 // Row m of the CTA's padded pixel grid -> (root slot r in the CTA, pixel p); false for pad rows / absent roots.
+template <int HW>
 __device__ __forceinline__ bool row_decode(int R, int nvalid, int m, int &r, int &p)
 {
-    const int rr = m / kRowsPerRoot, q = m - rr * kRowsPerRoot, y = q / kPitch, x = q - y * kPitch;
+    using G = TcGeo<HW>;
+    const int rr = m / G::kRowsPerRoot, q = m - rr * G::kRowsPerRoot, y = q / G::kPitch, x = q - y * G::kPitch;
     r = rr;
-    p = y * 6 + x;
-    return (rr < R) && (r < nvalid) && (y < 6) && (x < 6);
+    p = y * HW + x;
+    return (rr < R) && (r < nvalid) && (y < HW) && (x < HW);
 }
 
 // Staged 1x1-conv accumulators of one tile (S columns [0,16) reward, [16,32) value, [32,48) policy) -> BatchNorm + ReLU -> fp16 hi/lo
 // features in FC1's B-operand layout, for the heads in hmask (bit 0 reward -> its parking buffer fr, bit 1 value / bit 2 policy ->
-// rows 8-15 / 16-23 of fb).  Feature k = c * 36 + p of root r sits at k-group k / 8, row (head * 8 + r), element k % 8.  No barrier inside.
+// rows kMaxRoots + r / 2 kMaxRoots + r of fb).  Feature k = c * P + p of root r sits at k-group k / 8, row (head * kMaxRoots + r),
+// element k % 8.  No barrier inside.
+template <int HW>
 __device__ __forceinline__ void head_scatter(const TcNet &net, int hmask, unsigned char *fr, unsigned char *fb, const float *S, int t,
                                              int R, int nvalid)
 {
+    using G = TcGeo<HW>;
+    constexpr int kP = G::kPix, kRt = G::kMaxRoots, kLo = 4 * kRt * 16;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int q4 = warp & 3, half = warp >> 2, rowid = q4 * 32 + lane;
     int r, p;
-    const bool valid = row_decode(R, nvalid, t * 128 + rowid, r, p);
+    const bool valid = row_decode<HW>(R, nvalid, t * 128 + rowid, r, p);
     if (!valid) return;
     const float *v = S + (size_t)rowid * kStgLd;
     // warps 0-3 scatter reward + value features, warps 4-7 policy features
     if (half == 0 && (hmask & 1)) {
         for (int c = 0; c < net.hc[0]; ++c) {
             const int k = c * kP + p;
-            unsigned char *d = fr + ((k >> 3) * 8 + r) * 16 + (k & 7) * 2;
+            unsigned char *d = fr + ((k >> 3) * kRt + r) * 16 + (k & 7) * 2;
             float rem;
             put_half(d, fmaxf(fmaf(v[c], __ldg(net.head_bn + c), __ldg(net.head_bn + 16 + c)), 0.0f), rem);
-            *reinterpret_cast<__half *>(d + kFrBytes / 2) = __float2half_rn(rem);
+            *reinterpret_cast<__half *>(d + G::kFrBytes / 2) = __float2half_rn(rem);
         }
     }
     if (half == 0 && (hmask & 2)) {
         for (int c = 0; c < net.hc[1]; ++c) {
             const int k = c * kP + p;
-            unsigned char *d = fb + (k >> 3) * kFbKgBytes + (8 + r) * 16 + (k & 7) * 2;
+            unsigned char *d = fb + (k >> 3) * G::kFbKgBytes + (kRt + r) * 16 + (k & 7) * 2;
             float rem;
             put_half(d, fmaxf(fmaf(v[16 + c], __ldg(net.head_bn + 32 + c), __ldg(net.head_bn + 48 + c)), 0.0f), rem);
-            *reinterpret_cast<__half *>(d + 32 * 16) = __float2half_rn(rem);
+            *reinterpret_cast<__half *>(d + kLo) = __float2half_rn(rem);
         }
     }
     if (half == 1 && (hmask & 4)) {
         for (int c = 0; c < net.hc[2]; ++c) {
             const int k = c * kP + p;
-            unsigned char *d = fb + (k >> 3) * kFbKgBytes + (16 + r) * 16 + (k & 7) * 2;
+            unsigned char *d = fb + (k >> 3) * G::kFbKgBytes + (2 * kRt + r) * 16 + (k & 7) * 2;
             float rem;
             put_half(d, fmaxf(fmaf(v[32 + c], __ldg(net.head_bn + 64 + c), __ldg(net.head_bn + 80 + c)), 0.0f), rem);
-            *reinterpret_cast<__half *>(d + 32 * 16) = __float2half_rn(rem);
+            *reinterpret_cast<__half *>(d + kLo) = __float2half_rn(rem);
         }
     }
 }
 
-// FC1 read-out (warps 0-2: staged rows 32 h + unit j of head h): BatchNorm + ReLU, then the hidden activations as FC2's B operand
-// hb[head][k-group j / 8][root | 8 + root (lo)][j % 8].
+// FC1 read-out (warps 0-2: staged rows 32 h + unit j of head h; columns h * kMaxRoots + root, lo parts 4 kMaxRoots further):
+// BatchNorm + ReLU, then the hidden activations as FC2's B operand hb[head][k-group j / 8][root | 8 + root (lo)][j % 8].  Root
+// columns past kMaxRoots (the 8x8 grid) get zeros.
+template <int HW>
 __device__ __forceinline__ void heads_hidden(const TcNet &net, int hmask, unsigned char *hb, const float *S)
 {
+    constexpr int kRt = TcGeo<HW>::kMaxRoots;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (warp >= 3 || !((hmask >> warp) & 1)) return;
     const int h = warp, j = lane;
     const Head &H = h == 0 ? net.reward : (h == 1 ? net.value : net.policy);
-    const float *a = S + (size_t)(warp * 32 + lane) * kStgLd + h * 8, *b = a + 32;
+    const float *a = S + (size_t)(warp * 32 + lane) * kStgLd + h * kRt, *b = a + 4 * kRt;
     const float inv = net.fc[h].fc1_inv;
     const float s2 = (j < H.hid) ? __ldg(H.s2 + j) : 0.0f, t2 = (j < H.hid) ? __ldg(H.t2 + j) : 0.0f;
     unsigned char *dst = hb + h * kHbHeadBytes + (j >> 3) * 256 + (j & 7) * 2;
 #pragma unroll
     for (int r = 0; r < 8; ++r) {
-        const float pre = (a[r] + b[r]) * inv;
-        const float hid = (j < H.hid) ? fmaxf(fmaf(pre, s2, t2), 0.0f) : 0.0f;
+        const float pre = r < kRt ? (a[r] + b[r]) * inv : 0.0f;
+        const float hid = (r < kRt && j < H.hid) ? fmaxf(fmaf(pre, s2, t2), 0.0f) : 0.0f;
         float rem;
         put_half(dst + r * 16, hid, rem);
         *reinterpret_cast<__half *>(dst + (8 + r) * 16) = __float2half_rn(rem);
@@ -315,11 +349,12 @@ __device__ __forceinline__ void heads_outputs(const TcNet &net, const TcIO &io, 
 }
 
 // ---------------------------------------------------------------------------------------------- kernel
-// 32 consecutive channels [32*half, 32*half+32) of pixel p of one root latent.  cl: the kernel-internal layout [c / 4][36][c % 4]
-// (the pool slots this kernel writes in persistent mode, the skip scratch, the action-bias table): a thread's float4 j is at
-// ((c0 / 4 + j) * 36 + p) * 4, so the lanes of a warp (consecutive pixels) touch consecutive 16-byte chunks -- coalesced 512-byte
-// warp accesses (a plain channels-last row per lane costs 32 separate sectors per warp instruction).  Else NCHW [64][36]
-// (every tensor that crosses the API).
+// 32 consecutive channels [32*half, 32*half+32) of pixel p of one root latent of kP pixels.  cl: the kernel-internal layout
+// [c / 4][kP][c % 4] (the pool slots this kernel writes in persistent mode, the skip scratch, the action-bias table): a thread's
+// float4 j is at ((c0 / 4 + j) * kP + p) * 4, so the lanes of a warp (consecutive pixels) touch consecutive 16-byte chunks --
+// coalesced 512-byte warp accesses (a plain channels-last row per lane costs 32 separate sectors per warp instruction).  Else NCHW
+// [64][kP] (every tensor that crosses the API).
+template <int kP>
 __device__ __forceinline__ void load_row32(const float *root, bool cl, int p, int half, float (&v)[32])
 {
     if (cl) {
@@ -339,6 +374,7 @@ __device__ __forceinline__ void load_row32(const float *root, bool cl, int p, in
 }
 
 // 16 consecutive channels [c0, c0 + 16) of pixel p of one root (same layouts)
+template <int kP>
 __device__ __forceinline__ void store_row16(float *root, bool cl, int p, int c0, const float (&v)[16])
 {
     if (cl) {
@@ -352,9 +388,7 @@ __device__ __forceinline__ void store_row16(float *root, bool cl, int p, int c0,
     }
 }
 
-// the tree of a warp (tree_persist.cuh) parked in shared memory while the warp does network work: 16 uniform words + 3 x 32
-// per-lane words
-constexpr int kTreeParkWords = 16 + 3 * 32;
+// park / unpark the tree of a warp (kTreeParkWords)
 __device__ __forceinline__ void ptree_park(const PTree &T, uint32_t *w, int lane)
 {
     if (lane == 0) {
@@ -373,10 +407,17 @@ __device__ __forceinline__ void ptree_unpark(PTree &T, const uint32_t *w, int la
     T.my_legal = (int)w[16 + lane]; T.my_pslot = (int)w[48 + lane]; T.my_pact = (int)w[80 + lane];
 }
 
-// One CTA per SM (222 KB of shared memory).  Its 9 warps spread over the SM's four register-file quarters of 16,384 registers, three
+// One CTA per SM (~225 KB of shared memory).  Its 9 warps spread over the SM's four register-file quarters of 16,384 registers, three
 // in one of them, which caps the kernel at 168 registers: ptxas spills some of the epilogue state (not the accumulators).
+// HW: the latent grid (TcGeo); one instantiation per grid, chosen by tc_launch from TcNet::hw.
+template <int HW>
 __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, TreeParams tp)
 {
+    using G = TcGeo<HW>;
+    constexpr int kP = G::kPix, kPitch = G::kPitch, kRowsPerRoot = G::kRowsPerRoot, kMargin = G::kMargin;
+    constexpr int kPlaneBytes = G::kPlaneBytes, kPartBytes = G::kPartBytes, kActBytes = G::kActBytes;
+    constexpr int kSmemMain = G::kSmemMain, kHeadScratch = G::kHeadScratch, kFrBytes = G::kFrBytes;
+    constexpr int kRt = G::kMaxRoots, kFbKgBytes = G::kFbKgBytes, kFbBytes = G::kFbBytes;
     extern __shared__ __align__(1024) unsigned char smem[];
     unsigned char *act = smem;                                   // [2 parts][8 planes][400 rows][16 B]
     unsigned char *ring = smem + kActBytes;                      // [kStages][8 k-groups][128 rows: 64 hi | 64 lo][16 B]
@@ -390,7 +431,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
     const int R = io.roots_per_cta;
     const int root0 = blockIdx.x * R;
     const int nvalid = min(R, io.B - root0);                     // roots of this CTA that exist
-    const int NT = (R * kRowsPerRoot - 8 + 127) >> 7;
+    const int NT = (R * kRowsPerRoot - (HW + 2) + 127) >> 7;
     const int npass = io.npass;
     const int nlayers = net.nlayers;
     const int nsims = io.nsims > 0 ? io.nsims : 1;     // > 1 (or persistent): the whole search loop runs inside this launch
@@ -402,8 +443,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
         fence_mbar_init();
     }
     // heads whose fully connected parts run in this kernel (EfficientZero: the reward features go to the LSTM kernels instead),
-    // streamed through the ring per simulation after the conv taps: FC1 of all heads as one [128 rows][576] operand (18 stages of
-    // 2 k-steps), then one stage per 128-output tile of each head's FC2
+    // streamed through the ring per simulation after the conv taps: FC1 of all heads as one [128 rows][16 P] operand (16 P / 32
+    // stages of 2 k-steps), then one stage per 128-output tile of each head's FC2
     const int hmask_fc = ((net.has_reward && !io.ez_feat) ? 1 : 0) | 6;
     // 1x1 head weights (12 KB) and the folded BatchNorm tables of this program's layers: plain copies
     for (int i = tid; i < kHeadWBytes / 16; i += kTcThreads)
@@ -457,8 +498,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
                     const unsigned char *src = net.convw + (size_t)net.layer_w[L] * (9 * kTapBytes);
                     for (int tap = 0; tap < 9; ++tap) stage_in(src + (size_t)tap * kTapBytes);
                 }
-                // the heads: FC1 weights of all heads (18 stages), then the FC2 tiles of every head this kernel evaluates
-                for (int i = 0; i < kFc1Stages; ++i) stage_in(net.fcw + (size_t)i * kFc1StageBytes, kFc1StageBytes);
+                // the heads: FC1 weights of all heads, then the FC2 tiles of every head this kernel evaluates
+                for (int i = 0; i < G::kFc1Stages; ++i) stage_in(net.fcw + (size_t)i * kFc1StageBytes, kFc1StageBytes);
                 for (int h = 0; h < 3; ++h) {
                     if (!((hmask_fc >> h) & 1)) continue;
                     const int nblk = (net.fc[h].K + 127) >> 7;
@@ -499,7 +540,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
 #pragma unroll
     for (int t = 0; t < kMaxTiles; ++t) {
         int r, p;
-        const bool valid = row_decode(R, nvalid, t * 128 + rowid, r, p) && (t < NT);
+        const bool valid = row_decode<HW>(R, nvalid, t * 128 + rowid, r, p) && (t < NT);
         rowc[t] = valid ? ((r << 8) | p) : -1;
     }
     for (int sim = 0; sim <= nsims; ++sim) {        // iteration nsims: only the back-up of the last simulation (mcts_ctree.py:365-368)
@@ -547,7 +588,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
         for (int t = 0; t < kMaxTiles; ++t) {
             if (t >= NT) continue;
             float va[32];
-            if (rowc[t] >= 0) load_row32(in_ptr(t), in_is_cl(t), rowc[t] & 255, half, va);
+            if (rowc[t] >= 0) load_row32<kP>(in_ptr(t), in_is_cl(t), rowc[t] & 255, half, va);
             else {
 #pragma unroll
                 for (int c = 0; c < 32; ++c) va[c] = 0.0f;
@@ -627,15 +668,15 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
                 // residual operand (skip + action bias, in that association): thread-private global rows (L2-resident)
                 float rs[32];
                 if (has_res && valid) {
-                    if (skip_in_scratch) load_row32(io.skip_scratch + (size_t)b * (kC * kP), true, p, half, rs);
-                    else load_row32(in_ptr(t), in_is_cl(t), p, half, rs);
+                    if (skip_in_scratch) load_row32<kP>(io.skip_scratch + (size_t)b * (kC * kP), true, p, half, rs);
+                    else load_row32<kP>(in_ptr(t), in_is_cl(t), p, half, rs);
                     if (has_ab) {
                         const int action_raw = persistent ? reinterpret_cast<const int *>(ho)[(rowc[t] >> 8) * kHoWords + 1] : io.action[b];
                         const int action = min(max(action_raw, 0), net.A - 1);
                         const float4 *ab = reinterpret_cast<const float4 *>(net.abias) + ((size_t)action * 16 + half * 8) * kP + p;
 #pragma unroll
                         for (int j = 0; j < 8; ++j) {
-                            const float4 q = __ldcg(ab + j * kP);      // 83 KB table, one row per (root, action): L2-only like the skip rows
+                            const float4 q = __ldcg(ab + j * kP);      // action-bias table (A x 9 KB on 6x6, A x 16 KB on 8x8), one row per (root, action): L2-only like the skip rows
                             rs[4 * j] += q.x; rs[4 * j + 1] += q.y; rs[4 * j + 2] += q.z; rs[4 * j + 3] += q.w;
                         }
                     }
@@ -663,10 +704,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
                         }
 #pragma unroll
                         for (int c = 0; c < 16; ++c) v[c] = fmaxf(v[c], 0.0f);       // every layer of these programs ends in ReLU
-                        if (park) store_row16(io.skip_scratch + (size_t)b * (kC * kP), true, p, half * 32 + hs * 16, v);
+                        if (park) store_row16<kP>(io.skip_scratch + (size_t)b * (kC * kP), true, p, half * 32 + hs * 16, v);
                         if (flags & LF_WRITE_LATENT) {
-                            if (latent_out) store_row16(latent_out + (size_t)b * (kC * kP), io.pool_cl != 0, p, half * 32 + hs * 16, v);
-                            if (io.latent_out2) store_row16(io.latent_out2 + (size_t)b * (kC * kP), false, p, half * 32 + hs * 16, v);
+                            if (latent_out) store_row16<kP>(latent_out + (size_t)b * (kC * kP), io.pool_cl != 0, p, half * 32 + hs * 16, v);
+                            if (io.latent_out2) store_row16<kP>(io.latent_out2 + (size_t)b * (kC * kP), false, p, half * 32 + hs * 16, v);
                         }
                     } else {
 #pragma unroll
@@ -737,9 +778,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
                                 io.ez_feat[(size_t)(root0 + (rowc[t] >> 8)) * nin + c * kP + (rowc[t] & 255)] =
                                     fmaxf(fmaf(v[c], __ldg(net.head_bn + c), __ldg(net.head_bn + 16 + c)), 0.0f);
                         }
-                        head_scatter(net, hm & 6, fr, act, stg, t, R, nvalid);
+                        head_scatter<HW>(net, hm & 6, fr, act, stg, t, R, nvalid);
                     } else {
-                        head_scatter(net, hm, fr, act, stg, t, R, nvalid);
+                        head_scatter<HW>(net, hm, fr, act, stg, t, R, nvalid);
                     }
                     epi_sync();
                 }
@@ -753,20 +794,20 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
             unsigned char *fb = act, *hb = act + kFbBytes;
             float *red = reinterpret_cast<float *>(hb + 3 * kHbHeadBytes);
             float *f2 = reinterpret_cast<float *>(act);           // FC2 accumulators [tile][128][8], over the dead FC1 operand
-            // the parked reward features become rows 0-7 (hi) / 32-39 (lo) of the B operand.  FC1 multiplies all 576 inputs of
-            // every head: the host packs zero weights past hc * 36, but 0 x an Inf / NaN bit pattern that an earlier simulation
-            // (the FC2 staging overlays these rows) or kernel left there is NaN, so a head of hc < 16 channels gets zeros there
+            // the parked reward features become rows 0..kMaxRoots-1 (hi) / 4 kMaxRoots.. (lo) of the B operand.  FC1 multiplies all
+            // 16 P inputs of every head: the host packs zero weights past hc * P, but 0 x an Inf / NaN bit pattern that an earlier
+            // simulation (the FC2 staging overlays these rows) or kernel left there is NaN, so a head of hc < 16 channels gets zeros there
             for (int h = 0; h < 3; ++h) {
                 const int nin = net.hc[h] * kP;
-                if (!((hmask_fc >> h) & 1) || (h > 0 && nin == 576)) continue;
-                for (int i = tid; i < 2 * 72 * 8; i += kEpiThreads) {
-                    const int part = i / (72 * 8), rem = i - part * (72 * 8), kg = rem >> 3, r = rem & 7;
-                    unsigned char *dst = fb + kg * kFbKgBytes + (part * 32 + h * 8 + r) * 16;
+                if (!((hmask_fc >> h) & 1) || (h > 0 && nin == 16 * kP)) continue;
+                for (int i = tid; i < 2 * G::kFc1Kg * kRt; i += kEpiThreads) {
+                    const int part = i / (G::kFc1Kg * kRt), rem = i - part * (G::kFc1Kg * kRt), kg = rem >> G::kRootsLog2, r = rem & (kRt - 1);
+                    unsigned char *dst = fb + kg * kFbKgBytes + (part * 4 * kRt + h * kRt + r) * 16;
                     const int keep = nin - kg * 8;                // inputs of this k-group that exist
                     if (h > 0 && keep >= 8) continue;
                     uint4 q = make_uint4(0, 0, 0, 0);
                     if (keep > 0) {
-                        q = *reinterpret_cast<const uint4 *>(h == 0 ? fr + part * (kFrBytes / 2) + (kg * 8 + r) * 16 : dst);
+                        q = *reinterpret_cast<const uint4 *>(h == 0 ? fr + part * (kFrBytes / 2) + (kg * kRt + r) * 16 : dst);
                         if (keep < 8) {                           // hc * 36 = 4 (mod 8) for odd hc: keep the first 4 halves
                             q.z = 0; q.w = 0;
                         }
@@ -779,11 +820,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
             if (dbg) dbg[44] = clock64();
             const uint32_t fb_s = act_s, hb_s = act_s + kFbBytes;
             {
-                float f1[32];
+                float f1[G::kFbN / 2];
 #pragma unroll
-                for (int i = 0; i < 32; ++i) f1[i] = 0.0f;
+                for (int i = 0; i < G::kFbN / 2; ++i) f1[i] = 0.0f;
                 wg_fence_acc(f1);
-                for (int i = 0; i < kFc1Stages; ++i) {
+                for (int i = 0; i < G::kFc1Stages; ++i) {
                     const uint32_t pos = n++;
                     ring_wait(pos);
                     const uint32_t st_s = ring_s + (pos % kStages) * kTapBytes;
@@ -795,8 +836,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
                         // in the slot (their accumulator rows are never read)
                         const uint64_t a_hi = make_desc(st_s + ksi * (kFc1StageBytes / 2) + wg * 64 * 16, 1536 >> 4, 8), a_lo = a_hi + (3072 >> 4);
                         const uint64_t b = make_desc(fb_s + kstep * 2 * kFbKgBytes, kFbKgBytes >> 4, 8);
-                        wgmma_n64(f1, a_hi, b);
-                        wgmma_n64(f1, a_lo, b);
+                        if constexpr (G::kFbN == 64) {
+                            wgmma_n64(f1, a_hi, b);
+                            wgmma_n64(f1, a_lo, b);
+                        } else {
+                            wgmma_n32(f1, a_hi, b);
+                            wgmma_n32(f1, a_lo, b);
+                        }
                     }
                     wg_commit();
                     if (i > 0) {
@@ -807,11 +853,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
                 wg_wait<0>();
                 wg_fence_acc(f1);
                 ring_release(n - 1);
-                wg_stage<64>(stg, kStgLd, wg * 64, 0, f1);
+                wg_stage<G::kFbN>(stg, kStgLd, wg * 64, 0, f1);
             }
             epi_sync();
             if (dbg) dbg[45] = clock64();
-            heads_hidden(net, hmask_fc, hb, stg);
+            heads_hidden<HW>(net, hmask_fc, hb, stg);
             fence_proxy_async();
             epi_sync();                                           // FC2 may start
             if (dbg) dbg[46] = clock64();
@@ -916,7 +962,8 @@ unsigned long long *tc_debug_buffer() { return g_dbg; }
 
 int tc_prepare_launch()
 {
-    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_net_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_net_tc<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcGeo<6>::kSmemBytes));
+    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_net_tc<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcGeo<8>::kSmemBytes));
     if (getenv("LZ_TC_DEBUG") && !g_dbg) {      // allocated here (model finalize), never inside a stream capture
         LZ_CUDA_CHECK(cudaMalloc(&g_dbg, 64 * 8));
         LZ_CUDA_CHECK(cudaMemset(g_dbg, 0, 64 * 8));
@@ -924,13 +971,15 @@ int tc_prepare_launch()
     return LZ_OK;
 }
 
-// roots per CTA: at most one wave of CTAs on the 132 SMs of an H100 SXM (one CTA per SM: 222 KB of shared memory), at most 8
-// roots (3 row tiles): B = 1024 -> 128 CTAs of 8
-int tc_pick_roots(int B)
+// roots per CTA: at most one wave of CTAs on the 132 SMs of an H100 SXM (one CTA per SM: ~225 KB of shared memory), at most the
+// roots of 3 row tiles: 8 on the 6x6 grid (B = 1024 -> 128 CTAs of 8), 4 on the 8x8 grid (B = 1024 -> 256 CTAs of 4)
+static int tc_pick_roots(int hw, int B)
 {
     int r = (B + kNumSMs - 1) / kNumSMs;
-    return std::min(std::max(r, 1), kMaxRoots);
+    return std::min(std::max(r, 1), hw == 8 ? TcGeo<8>::kMaxRoots : TcGeo<6>::kMaxRoots);
 }
+static int tc_rows_per_root(int hw) { return (hw + 1) * (hw + 1); }
+static int tc_f2_max_tiles(int hw) { return hw == 8 ? TcGeo<8>::kF2MaxTiles : TcGeo<6>::kF2MaxTiles; }
 
 // the heads k_net_tc evaluates (the hmask_fc of the kernel) and the FC2 tiles they stream
 static int tc_heads_mask(const TcNet &net, const TcIO &io) { return ((net.has_reward && !io.ez_feat) ? 1 : 0) | 6; }
@@ -946,13 +995,13 @@ static int tc_fc2_tiles(const TcNet &net, int hmask)
 // staged in shared memory, FC2 tiles.  Mirrors the kernel's set-up code.
 void tc_describe(const TcNet &net, const TcIO &io, int32_t *info)
 {
-    const int R = tc_pick_roots(io.B), ctas = (io.B + R - 1) / R, hmask = tc_heads_mask(net, io);
+    const int R = tc_pick_roots(net.hw, io.B), ctas = (io.B + R - 1) / R, hmask = tc_heads_mask(net, io);
     int nb2 = 0;
     for (int h = 0; h < 3; ++h)
         if ((hmask >> h) & 1) nb2 += net.fc[h].K;
     const int used = net.nlayers * 128;
     info[0] = R;
-    info[1] = (R * kRowsPerRoot - 8 + 127) >> 7;
+    info[1] = (R * tc_rows_per_root(net.hw) - (net.hw + 2) + 127) >> 7;
     info[2] = ctas;
     info[3] = io.B - (ctas - 1) * R;
     info[4] = net.nlayers;
@@ -965,7 +1014,7 @@ void tc_describe(const TcNet &net, const TcIO &io, int32_t *info)
 // biases are staged in shared memory, layers.  Mirrors the kernel's set-up code.
 void tc_describe_search(const TcNet &net, const TcIO &io, int N, int32_t *info)
 {
-    const int R = tc_pick_roots(io.B), ctas = (io.B + R - 1) / R, hmask = tc_heads_mask(net, io);
+    const int R = tc_pick_roots(net.hw, io.B), ctas = (io.B + R - 1) / R, hmask = tc_heads_mask(net, io);
     int nb2 = 0;
     for (int h = 0; h < 3; ++h)
         if ((hmask >> h) & 1) nb2 += net.fc[h].K;
@@ -988,13 +1037,15 @@ int tc_launch(const TcNet &net, const TcIO &io_in, cudaStream_t s, const TreePar
     LZ_REQUIRE(!io.persistent || tp_in, LZ_EINVAL, "tc_launch: persistent search needs tree parameters");
     LZ_REQUIRE(net.A <= 1000, LZ_EINVAL, "tc_launch: action space %d too large for the head scratch of the tensor-core path", net.A);
     LZ_REQUIRE(io.skip_scratch, LZ_EINVAL, "tc_launch: no skip scratch");
-    LZ_REQUIRE(tc_fc2_tiles(net, tc_heads_mask(net, io)) <= kF2MaxTiles, LZ_EINVAL, "tc_launch: %d FC2 tiles exceed the %d of the head scratch",
-               tc_fc2_tiles(net, tc_heads_mask(net, io)), kF2MaxTiles);
+    LZ_REQUIRE(net.hw == 6 || net.hw == 8, LZ_EINVAL, "tc_launch: latent grid %dx%d not supported (6x6 or 8x8)", net.hw, net.hw);
+    LZ_REQUIRE(tc_fc2_tiles(net, tc_heads_mask(net, io)) <= tc_f2_max_tiles(net.hw), LZ_EINVAL, "tc_launch: %d FC2 tiles exceed the %d of the head scratch",
+               tc_fc2_tiles(net, tc_heads_mask(net, io)), tc_f2_max_tiles(net.hw));
     io.dbg = g_dbg;
-    io.roots_per_cta = tc_pick_roots(io.B);
+    io.roots_per_cta = tc_pick_roots(net.hw, io.B);
     LZ_REQUIRE(!io.persistent || tp.A <= 32, LZ_EINVAL, "tc_launch: the persistent search needs A <= 32 (got %d)", tp.A);
     const int grid = (io.B + io.roots_per_cta - 1) / io.roots_per_cta;
-    k_net_tc<<<grid, kTcThreads, kSmemBytes, s>>>(net, io, tp);
+    if (net.hw == 8) k_net_tc<8><<<grid, kTcThreads, TcGeo<8>::kSmemBytes, s>>>(net, io, tp);
+    else k_net_tc<6><<<grid, kTcThreads, TcGeo<6>::kSmemBytes, s>>>(net, io, tp);
     LZ_KERNEL_CHECK();
     return LZ_OK;
 }

@@ -319,8 +319,7 @@ static int collect_device(lz_search *q, const float *d_obs, const uint8_t *d_obs
     io.value = d_pred_value ? d_pred_value : q->d_root_value;
     int rc;
     if (d_obs_u8) {
-        LZ_REQUIRE(q->model->kind == 0 && q->model->math != 0 && q->model->cfg.obs_h != 64, LZ_EINVAL,
-                   "lz_search_collect_u8: uint8 frames need the tensor-core conv model (84x84 / 96x96)");
+        LZ_REQUIRE(q->model->kind == 0 && q->model->math != 0, LZ_EINVAL, "lz_search_collect_u8: uint8 frames need the tensor-core conv model");
         if (!q->d_pre_stage && (rc = dev_alloc(&q->d_pre_stage, (size_t)q->B * q->model->latent_floats))) return rc;
         rc = model_initial_tower(q->model, q->B, nullptr, q->d_pre_stage, (cudaStream_t)s, d_obs_u8);
         if (rc == LZ_OK) rc = model_initial_tail(q->model, q->B, q->d_pre_stage, io, (cudaStream_t)s);
@@ -348,8 +347,8 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
                         float *d_policy_logits, lz_stream s_)
 {
     LZ_REQUIRE(q && h_obs, LZ_EINVAL, "lz_search_collect_host: bad argument");
-    LZ_REQUIRE(!obs_u8 || (q->model->kind == 0 && q->model->math != 0 && q->model->cfg.obs_h != 64), LZ_EINVAL,
-               "lz_search_collect_host_u8: uint8 frames need the tensor-core conv model (84x84 / 96x96)");
+    LZ_REQUIRE(!obs_u8 || (q->model->kind == 0 && q->model->math != 0), LZ_EINVAL,
+               "lz_search_collect_host_u8: uint8 frames need the tensor-core conv model");
     const size_t esz = obs_u8 ? 1 : sizeof(float);         // bytes per observation element on the wire and in the staging buffer
     cudaStream_t s = (cudaStream_t)s_;
     const lz_model_config &c = q->model->cfg;
@@ -388,7 +387,7 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
     if (h_to_play) LZ_CUDA_CHECK(cudaMemcpyAsync(q->d_tp_stage, h_to_play, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     float *logits = d_policy_logits ? d_policy_logits : q->d_root_logits;
     float *pred = d_pred_value ? d_pred_value : q->d_root_value;
-    const bool split = q->model->kind == 0 && q->model->math != 0 && c.obs_h != 64;   // tower per chunk, tail once
+    const bool split = q->model->kind == 0 && q->model->math != 0;   // tower per chunk, tail once
     for (int i = 0; i < nchunks; ++i) {
         const int b0 = i * per, bc = std::min(per, B - b0);
         LZ_CUDA_CHECK(cudaStreamWaitEvent(s, q->ev_chunk[i], 0));

@@ -25,7 +25,7 @@ class EZNetworkOutput:
 
 class EfficientZeroModel(MuZeroModel):
     def __init__(self, observation_shape: Sequence[int] = (4, 96, 96), action_space_size: int = 6,
-                 lstm_hidden_size: int = 512, downsample: bool = True, device: Optional[torch.device] = None, **kwargs):
+                 lstm_hidden_size: int = 512, downsample: Optional[bool] = None, device: Optional[torch.device] = None, **kwargs):
         kwargs.pop("_efficientzero", None)
         super().__init__(observation_shape=observation_shape, action_space_size=action_space_size, downsample=downsample,
                          device=device, _efficientzero=True, lstm_hidden_size=lstm_hidden_size, **kwargs)

@@ -33,10 +33,20 @@ class MuZeroModel:
                  policy_head_hidden_channels: Sequence[int] = (32,),
                  reward_support_range: Sequence[float] = (-300., 301., 1.),
                  value_support_range: Sequence[float] = (-300., 301., 1.),
-                 categorical_distribution: bool = True, downsample: bool = True, norm_type: str = "BN",
+                 categorical_distribution: bool = True, downsample: Optional[bool] = None, norm_type: str = "BN",
                  discrete_action_encoding_type: str = "one_hot", state_norm: bool = False,
                  device: Optional[torch.device] = None, **kwargs):
         # unknown kwargs are swallowed like muzero_model.py:49-50
+        if downsample is None:
+            # The reference's default is downsample=False (muzero_model.py:45, efficientzero_model.py:45): a full-resolution
+            # network this class does not implement.  84 / 96-pixel models default to the DownSample network here, as they
+            # always have.  A 64x64 model follows the reference default, so it must ask for DownSample as the shipped Atari
+            # configs do (zoo/atari/config/atari_muzero_config.py:56, atari_efficientzero_config.py:44).
+            downsample = tuple(observation_shape[1:]) != (64, 64)
+            if not downsample:
+                raise NotImplementedError(
+                    "a 64x64 observation_shape needs downsample=True (as in the reference's Atari configs): with the reference's "
+                    "default downsample=False the model is a full-resolution network, which this CUDA model does not implement")
         if not categorical_distribution or not downsample or norm_type != "BN" or \
                 discrete_action_encoding_type != "one_hot" or state_norm:
             raise NotImplementedError(
@@ -90,7 +100,8 @@ class MuZeroModel:
     MATH_MODES = {"fp32": 0, "tc3": 1, "tc1": 2}
 
     def set_math(self, mode):
-        """'fp32' = FFMA on CUDA cores, 'tc3' = wgmma 3xFP16 (fp32-accurate), 'tc1' = wgmma single fp16 pass."""
+        """'fp32' = FFMA on CUDA cores (6x6 latent grid only: 84/96-pixel observations), 'tc3' = wgmma 3xFP16
+        (fp32-accurate, the default), 'tc1' = wgmma single fp16 pass."""
         code = self.MATH_MODES[mode] if isinstance(mode, str) else int(mode)
         cabi.check(self._lib.lz_model_set_math(self._h, code), "lz_model_set_math")
         self.math = code
