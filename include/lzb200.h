@@ -146,6 +146,33 @@ int lz_tree_backpropagate_with_reuse(lz_tree *t, int latent_index, const float *
 int lz_tree_select_action(lz_tree *t, float temperature, int deterministic, uint64_t seed, int32_t *d_action,
                           int32_t *d_action_pos, float *d_entropy, lz_stream s);
 
+/* ---- Gumbel MuZero tree (lzero/mcts/ctree/ctree_gumbel_muzero/lib/cnode.cpp, gmz_tree.pyx) ----
+ * lz_tree_set_gumbel turns a MuZero tree into a Gumbel tree: sequential halving with Gumbel noise at the root
+ * (cselect_root_child, cnode.cpp:701-745) and completed-Q improved-policy selection below it (cselect_interior_child,
+ * :747-790); the back-up is the one-player recurrence for every to_play (:605-631).  It builds the root Gumbel vector
+ * (10 * Gumbel(0, 1) from std::mt19937(0), the first n draws for a root with n legal actions) and row min(m, S) of the
+ * considered-visit table on the host.  num_simulations == 0 turns the tree back into a MuZero tree.  Refused on an
+ * EfficientZero tree; on a Gumbel tree the MuZero / EfficientZero / reuse tree and search calls are refused.
+ * Descents use the discount of lz_tree_set_params. */
+int lz_tree_set_gumbel(lz_tree *t, int max_num_considered_actions, int num_simulations);
+/* CRoots::prepare / prepare_no_noise (cnode.cpp:418-455): lz_tree_prepare plus the roots' value estimates d_values f32 [B]. */
+int lz_tree_prepare_gumbel(lz_tree *t, const float *d_logits, const float *d_noise, float noise_weight,
+                           const float *d_rewards, const float *d_values, const int32_t *d_to_play, lz_stream s);
+/* cbatch_traverse (cnode.cpp:834-897): outputs as lz_tree_traverse; the virtual to_play is the root's, unchanged.  At most
+ * num_simulations descents per prepare (one more would index past the considered-visit table): LZ_ESTATE. */
+int lz_tree_traverse_gumbel(lz_tree *t, int32_t *d_ix, int32_t *d_iy, int32_t *d_last_action, int32_t *d_search_len,
+                            int32_t *d_virtual_to_play, lz_stream s);
+/* cbatch_back_propagate (cnode.cpp:633-652): arguments as lz_tree_backpropagate; d_value is also the new node's raw value. */
+int lz_tree_backpropagate_gumbel(lz_tree *t, int latent_index, const float *d_reward, const float *d_value,
+                                 const float *d_logits, const int32_t *d_to_play, lz_stream s);
+/* get_children_values / get_policies (cnode.cpp:309-385, 506-541) with the tree's discount: d_children_values f32 [B,A]
+ * completed Q by action id (-inf at illegal actions), d_improved_policy f32 [B,A] softmax(prior + completed Q) by action id.
+ * Either may be NULL.  Visit counts, values and trajectories: lz_tree_results. */
+int lz_tree_gumbel_policies(lz_tree *t, float *d_children_values, float *d_improved_policy, lz_stream s);
+/* Host only (no device needed): row min(m, S) of get_table_of_considered_visits(m, S) into h_seq int32 [S] and
+ * generate_gumbel(10, 0, A) into h_gumbel f32 [A] (cnode.cpp:1041-1094, 1133-1151).  Either may be NULL. */
+int lz_gumbel_tables(int max_num_considered_actions, int num_simulations, int A, int32_t *h_seq, float *h_gumbel);
+
 /* ------------------------------------------------------------------ model (muzero_model.py, efficientzero_model.py) */
 
 typedef struct lz_model_config {
@@ -272,6 +299,10 @@ int lz_search_run_ez(lz_search *q, const float *d_latent_roots, const float *d_h
  * tree at :1040-1046 / cnode.cpp:646, see DESIGN.md 4.6). */
 int lz_search_run_ez_with_reuse(lz_search *q, const float *d_latent_roots, const float *d_hidden0_roots, const float *d_hidden1_roots,
                                 const int32_t *d_true_action, const float *d_reuse_value, int32_t *d_infer_count, lz_stream s);
+/* GumbelMuZeroMCTSCtree.search (mcts_ctree.py:1076-1172) on a Gumbel tree prepared with lz_tree_prepare_gumbel and a MuZero
+ * conv or MLP model: one CUDA graph of [Gumbel descent] + num_simulations x [recurrent_inference, Gumbel back-up + next
+ * descent].  The search's num_simulations may not exceed the tree's Gumbel num_simulations. */
+int lz_search_run_gumbel(lz_search *q, const float *d_latent_roots, lz_stream s);
 /* The search-feeding part of _forward_collect (policy/muzero.py:749-779): initial_inference ->
  * reset(mask) -> prepare(noise) -> search.  d_obs f32 [B,obs_c,H,W]; d_mask uint8 [B,A] or NULL;
  * d_noise f32 [B,A] legal-order rows or NULL; d_to_play int32 [B] or NULL (-1).

@@ -8,6 +8,7 @@
 
 #include <algorithm>
 
+#include "gumbel.cuh"
 #include "model.cuh"
 #include "tree.cuh"
 
@@ -37,7 +38,7 @@ struct lz_search {
     // ReZero search_with_reuse: library-owned copies of the caller's per-root true action / reuse value (graph-stable addresses)
     int32_t *d_true_action;
     float *d_reuse_value;
-    SearchGraph graphs[3];       // plain search with deterministic 0 / 1, search with reuse
+    SearchGraph graphs[4];       // plain search with deterministic 0 / 1, search with reuse, Gumbel search
     cudaStream_t capture_stream; // library-owned: the caller's stream may be the legacy default stream,
                                  // which cannot be captured; the instantiated graph launches on the caller's
     int num_kernels;             // kernel nodes of the graph launched last
@@ -79,7 +80,7 @@ static RecIO rec_io(const lz_search *q, int sim)
 // EfficientZero stays a multi-kernel graph: its LSTM step is a GEMM over all roots (several launches per simulation).
 static bool persistent_search(const lz_search *q, bool reuse)
 {
-    return !reuse && !q->hpool && q->model->kind == 0 && q->model->math != 0 && q->tree->p.A <= 32;   // tree_persist.cuh: one lane per child
+    return !reuse && !q->tree->gumbel && !q->hpool && q->model->kind == 0 && q->model->math != 0 && q->tree->p.A <= 32;   // tree_persist.cuh: one lane per child
 }
 
 static TcIO persistent_io(const lz_search *q, int deterministic)
@@ -96,8 +97,30 @@ static TcIO persistent_io(const lz_search *q, int deterministic)
     return io;
 }
 
+// GumbelMuZeroMCTSCtree.search (mcts_ctree.py:1076-1172): [Gumbel descent] + S x [recurrent_inference, Gumbel back-up + next
+// descent] with the non-persistent network kernels.
+static int enqueue_gumbel(lz_search *q, cudaStream_t s)
+{
+    int rc;
+    lz_tree *t = q->tree;
+    TreeStep descent = {};
+    descent.traverse = 1;
+    descent.ix = q->d_ix; descent.act = q->d_action;
+    if ((rc = gumbel_launch_step(t, descent, s))) return rc;
+    for (int sim = 0; sim < q->S; ++sim) {
+        if ((rc = model_recurrent(q->model, rec_io(q, sim), s))) return rc;
+        TreeStep step = descent;
+        step.traverse = sim + 1 < q->S;
+        step.latent_index = sim + 1;
+        step.reward = q->d_reward; step.value = q->d_value; step.logits = q->d_policy;
+        if ((rc = gumbel_launch_step(t, step, s))) return rc;
+    }
+    return LZ_OK;
+}
+
 static int enqueue_search(lz_search *q, int deterministic, bool reuse, cudaStream_t s)
 {
+    if (q->tree->gumbel) return enqueue_gumbel(q, s);
     int rc;
     lz_tree *t = q->tree;
     t->step_counter = 0;
@@ -130,7 +153,7 @@ static int enqueue_search(lz_search *q, int deterministic, bool reuse, cudaStrea
 static int run_graph(lz_search *q, int deterministic, bool reuse, cudaStream_t s)
 {
     // an EfficientZero plain search breaks ties by p.tie_first (tracked by the tree generation), not by the flag: one graph
-    SearchGraph &g = q->graphs[reuse ? 2 : (deterministic || q->hpool) ? 1 : 0];
+    SearchGraph &g = q->graphs[q->tree->gumbel ? 3 : reuse ? 2 : (deterministic || q->hpool) ? 1 : 0];
     // a captured graph bakes in device pointers of the model's tables (passed by value in TcNet / NetDev / EzNet), the math mode
     // and the tree parameters (TreeParams by value): re-capture when any of them changed since (weight reload, set_math,
     // model_reserve growth, lz_tree_set_params / lz_tree_set_ez / lz_tree_set_tiebreak)
@@ -202,6 +225,7 @@ static int collect_search(lz_search *q, const uint8_t *d_mask, const float *d_lo
                           const int32_t *d_to_play, int deterministic, cudaStream_t s)
 {
     int rc;
+    LZ_REQUIRE(!q->tree->gumbel, LZ_ESTATE, "lz_search_collect: Gumbel tree (the collect entry points run MuZero / EfficientZero searches)");
     if ((rc = lz_tree_reset_mask(q->tree, d_mask, s))) return rc;                // policy/muzero.py:760,769
     if ((rc = lz_tree_prepare(q->tree, d_logits, d_noise, noise_weight, nullptr, d_to_play, s))) return rc;   // :774
     if (q->hpool) {      // EfficientZero: zero LSTM state at the roots; the tree has no deterministic argument, the collect call's flag selects its tie-breaking
@@ -270,6 +294,7 @@ int lz_search_destroy(lz_search *q)
 int lz_search_run_ez(lz_search *q, const float *d_latent_roots, const float *d_hidden0_roots, const float *d_hidden1_roots, lz_stream s)
 {
     LZ_REQUIRE(q && q->hpool, LZ_EINVAL, "lz_search_run_ez: not an EfficientZero search");
+    LZ_REQUIRE(!q->tree->gumbel, LZ_ESTATE, "lz_search_run_ez: Gumbel tree, use lz_search_run_gumbel");
     LZ_REQUIRE(q->tree->prepared, LZ_ESTATE, "lz_search_run_ez: roots not prepared (call lz_tree_prepare first)");
     int rc = copy_latent_roots(q, d_latent_roots, (cudaStream_t)s);
     if (rc == LZ_OK) rc = ez_root_hidden(q, d_hidden0_roots, d_hidden1_roots, (cudaStream_t)s);
@@ -283,6 +308,7 @@ int lz_search_run_with_reuse(lz_search *q, const float *d_latent_roots, const in
     LZ_REQUIRE(q && d_true_action && d_reuse_value, LZ_EINVAL, "lz_search_run_with_reuse: null argument");
     LZ_REQUIRE(!q->hpool, LZ_ESTATE, "lz_search_run_with_reuse: EfficientZero search, use lz_search_run_ez_with_reuse");
     LZ_REQUIRE(q->tree->prepared, LZ_ESTATE, "lz_search_run_with_reuse: roots not prepared (call lz_tree_prepare first)");
+    LZ_REQUIRE(!q->tree->gumbel, LZ_ESTATE, "lz_search_run_with_reuse: Gumbel tree, use lz_search_run_gumbel");
     return run_with_reuse(q, d_latent_roots, d_true_action, d_reuse_value, d_infer_count, (cudaStream_t)s_);
 }
 
@@ -292,6 +318,7 @@ int lz_search_run_ez_with_reuse(lz_search *q, const float *d_latent_roots, const
     LZ_REQUIRE(q && d_true_action && d_reuse_value, LZ_EINVAL, "lz_search_run_ez_with_reuse: null argument");
     LZ_REQUIRE(q->hpool, LZ_ESTATE, "lz_search_run_ez_with_reuse: not an EfficientZero search");
     LZ_REQUIRE(q->tree->prepared, LZ_ESTATE, "lz_search_run_ez_with_reuse: roots not prepared (call lz_tree_prepare first)");
+    LZ_REQUIRE(!q->tree->gumbel, LZ_ESTATE, "lz_search_run_ez_with_reuse: Gumbel tree, use lz_search_run_gumbel");
     int rc = ez_root_hidden(q, d_hidden0_roots, d_hidden1_roots, (cudaStream_t)s_);
     if (rc) return rc;
     return run_with_reuse(q, d_latent_roots, d_true_action, d_reuse_value, d_infer_count, (cudaStream_t)s_);
@@ -302,9 +329,28 @@ int lz_search_run(lz_search *q, const float *d_latent_roots, int deterministic, 
     LZ_REQUIRE(q, LZ_EINVAL, "lz_search_run: null search");
     LZ_REQUIRE(!q->hpool, LZ_ESTATE, "lz_search_run: EfficientZero search, use lz_search_run_ez");
     LZ_REQUIRE(q->tree->prepared, LZ_ESTATE, "lz_search_run: roots not prepared (call lz_tree_prepare first)");
+    LZ_REQUIRE(!q->tree->gumbel, LZ_ESTATE, "lz_search_run: Gumbel tree, use lz_search_run_gumbel");
     int rc = copy_latent_roots(q, d_latent_roots, (cudaStream_t)s);
     if (rc) return rc;
     return run_graph(q, deterministic, false, (cudaStream_t)s);
+}
+
+int lz_search_run_gumbel(lz_search *q, const float *d_latent_roots, lz_stream s)
+{
+    LZ_REQUIRE(q, LZ_EINVAL, "lz_search_run_gumbel: null search");
+    lz_gumbel *gs = q->tree->gumbel;
+    LZ_REQUIRE(gs, LZ_ESTATE, "lz_search_run_gumbel: not a Gumbel tree (lz_tree_set_gumbel)");
+    LZ_REQUIRE(!q->hpool && !q->tree->p.ez, LZ_ESTATE, "lz_search_run_gumbel: EfficientZero model or tree (the Gumbel search runs MuZero models)");
+    LZ_REQUIRE(gs->prepared && gs->traversals == 0, LZ_ESTATE,
+               "lz_search_run_gumbel: roots not freshly prepared (call lz_tree_prepare_gumbel first)");
+    LZ_REQUIRE(q->S <= gs->g.S, LZ_EINVAL, "lz_search_run_gumbel: %d simulations past the considered-visit table of num_simulations = %d",
+               q->S, gs->g.S);
+    int rc = copy_latent_roots(q, d_latent_roots, (cudaStream_t)s);
+    if (rc) return rc;
+    if ((rc = run_graph(q, 1, false, (cudaStream_t)s))) return rc;
+    gs->traversals = q->S;
+    gs->pending = false;
+    return LZ_OK;
 }
 
 static int collect_device(lz_search *q, const float *d_obs, const uint8_t *d_obs_u8, const uint8_t *d_mask, const float *d_noise,

@@ -8,6 +8,7 @@
 #include <vector>
 
 #include "lz_common.cuh"
+#include "gumbel.cuh"
 #include "tree.cuh"
 
 namespace lz {
@@ -291,6 +292,7 @@ int lz_tree_create(int B, int A, int max_sims, lz_tree **out)
 int lz_tree_destroy(lz_tree *t)
 {
     if (!t) return LZ_OK;
+    gumbel_free(t);
     cudaFree(t->alloc_base);
     delete t;
     return LZ_OK;
@@ -328,6 +330,7 @@ int lz_tree_reset(lz_tree *t, const int32_t *d_legal, const int32_t *d_nlegal, l
     k_tree_reset<<<tree_grid(t->p.B), kTreeBlock, 0, (cudaStream_t)s>>>(t->p, d_legal, d_nlegal, nullptr);
     LZ_KERNEL_CHECK();
     t->prepared = false;
+    if (t->gumbel) t->gumbel->prepared = false;
     return LZ_OK;
 }
 
@@ -337,6 +340,7 @@ int lz_tree_reset_mask(lz_tree *t, const uint8_t *d_mask, lz_stream s)
     k_tree_reset<<<tree_grid(t->p.B), kTreeBlock, 0, (cudaStream_t)s>>>(t->p, nullptr, nullptr, d_mask);
     LZ_KERNEL_CHECK();
     t->prepared = false;
+    if (t->gumbel) t->gumbel->prepared = false;
     return LZ_OK;
 }
 
@@ -348,6 +352,7 @@ int lz_tree_prepare(lz_tree *t, const float *d_logits, const float *d_noise, flo
                                                                          d_rewards, d_to_play);
     LZ_KERNEL_CHECK();
     t->prepared = true;
+    if (t->gumbel) t->gumbel->prepared = false;     // lz_tree_prepare_gumbel sets it after this call
     return LZ_OK;
 }
 
@@ -357,6 +362,7 @@ int lz_tree_traverse(lz_tree *t, int deterministic, int32_t *d_ix, int32_t *d_iy
     LZ_REQUIRE(t, LZ_EINVAL, "lz_tree_traverse: null tree");
     LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_traverse: roots not prepared (call lz_tree_prepare first)");
     LZ_REQUIRE(!t->p.ez, LZ_ESTATE, "lz_tree_traverse: tree is in EfficientZero mode, use lz_tree_traverse_ez");
+    LZ_REQUIRE(!t->gumbel, LZ_ESTATE, "lz_tree_traverse: Gumbel tree, use lz_tree_traverse_gumbel");
     TreeStep a = {};
     a.traverse = 1; a.deterministic = deterministic;
     a.ix = d_ix; a.iy = d_iy; a.act = d_last_action; a.len = d_search_len; a.vtp = d_virtual_to_play;
@@ -369,6 +375,7 @@ int lz_tree_backpropagate(lz_tree *t, int latent_index, const float *d_reward, c
     LZ_REQUIRE(t && d_reward && d_value && d_logits, LZ_EINVAL, "lz_tree_backpropagate: null argument");
     LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_backpropagate: roots not prepared");
     LZ_REQUIRE(!t->p.ez, LZ_ESTATE, "lz_tree_backpropagate: tree is in EfficientZero mode, use lz_tree_backpropagate_ez");
+    LZ_REQUIRE(!t->gumbel, LZ_ESTATE, "lz_tree_backpropagate: Gumbel tree, use lz_tree_backpropagate_gumbel");
     LZ_REQUIRE(latent_index >= 1 && latent_index <= t->max_sims, LZ_EINVAL,
                "lz_tree_backpropagate: latent_index %d outside [1, %d]", latent_index, t->max_sims);
     TreeStep a = {};
@@ -380,6 +387,7 @@ int lz_tree_set_ez(lz_tree *t, int efficientzero, int lstm_horizon_len)
 {
     LZ_REQUIRE(t, LZ_EINVAL, "lz_tree_set_ez: null tree");
     LZ_REQUIRE(!efficientzero || lstm_horizon_len > 0, LZ_EINVAL, "lz_tree_set_ez: lstm_horizon_len must be > 0 (mcts_ctree.py:857)");
+    LZ_REQUIRE(!efficientzero || !t->gumbel, LZ_ESTATE, "lz_tree_set_ez: Gumbel tree (lz_tree_set_gumbel(t, m, 0) turns it back into a MuZero tree)");
     const int ez = efficientzero ? 1 : 0, hor = efficientzero ? lstm_horizon_len : t->p.lstm_horizon;
     if (t->p.ez != ez || t->p.lstm_horizon != hor) ++t->generation;
     t->p.ez = ez;
@@ -426,6 +434,7 @@ int lz_tree_traverse_with_reuse(lz_tree *t, const int32_t *d_true_action, const 
 {
     LZ_REQUIRE(t && d_true_action && d_reuse_value, LZ_EINVAL, "lz_tree_traverse_with_reuse: null argument");
     LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_traverse_with_reuse: roots not prepared");
+    LZ_REQUIRE(!t->gumbel, LZ_ESTATE, "lz_tree_traverse_with_reuse: Gumbel tree, use lz_tree_traverse_gumbel");
     TreeStep a = {};
     a.traverse = 1; a.true_action = d_true_action; a.reuse_value = d_reuse_value;
     a.ix = d_ix; a.iy = d_iy; a.act = d_last_action; a.len = d_search_len; a.vtp = d_virtual_to_play;
@@ -438,6 +447,7 @@ int lz_tree_backpropagate_with_reuse(lz_tree *t, int latent_index, const float *
 {
     LZ_REQUIRE(t && d_reward && d_value && d_logits && d_reuse_value, LZ_EINVAL, "lz_tree_backpropagate_with_reuse: null argument");
     LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_backpropagate_with_reuse: roots not prepared");
+    LZ_REQUIRE(!t->gumbel, LZ_ESTATE, "lz_tree_backpropagate_with_reuse: Gumbel tree, use lz_tree_backpropagate_gumbel");
     LZ_REQUIRE(!t->p.ez || d_is_reset, LZ_EINVAL, "lz_tree_backpropagate_with_reuse: EfficientZero trees need d_is_reset");
     LZ_REQUIRE(latent_index >= 1 && latent_index <= t->max_sims, LZ_EINVAL,
                "lz_tree_backpropagate_with_reuse: latent_index %d outside [1, %d]", latent_index, t->max_sims);

@@ -20,7 +20,7 @@ from typing import Any, List, Optional, Union
 import numpy as np
 import torch
 
-from . import cabi, ez_tree, mz_tree
+from . import cabi, ez_tree, gmz_tree, mz_tree
 from .efficientzero_model import EfficientZeroModel
 from .muzero_model import MuZeroModel
 from .muzero_model_mlp import MuZeroModelMLP
@@ -363,3 +363,76 @@ class UniZeroMCTSCtree(MuZeroMCTSCtree):
                 cabi.check(t.lib.lz_tree_backpropagate(t.h, simulation_index + 1, reward.data_ptr(), value.data_ptr(),
                                                        pol.data_ptr(), None, cabi.stream_ptr()), "lz_tree_backpropagate")
         return first_action_latent_map
+
+
+class GumbelMuZeroMCTSCtree(MuZeroMCTSCtree):
+    """Mirror of ``lzero.mcts.tree_search.mcts_ctree.GumbelMuZeroMCTSCtree`` (mcts_ctree.py:1005-1172): same config keys
+    (+ ``max_num_considered_actions``, the policy config key read at :1124; default: every action), ``roots(n,
+    legal_actions)`` and ``search(roots, model, latent_state_roots, to_play_batch)``.  The roots are ``gmz_tree.Roots``
+    prepared with the 6-argument ``prepare`` (or ``prepare_no_noise``).
+
+    With a ``lightzero_b200`` ``MuZeroModel`` / ``MuZeroModelMLP`` the whole loop is one CUDA-graph launch
+    (``lz_search_run_gumbel``): Gumbel descent, recurrent_inference and back-up for every simulation.  Any other model object
+    is driven step-wise around the device trees.  The search is deterministic like the reference's (no rand() on its path)."""
+    config = dict(
+        num_simulations=50,
+        root_dirichlet_alpha=0.3,
+        root_noise_weight=0.25,
+        value_delta_max=0.01,
+    )
+
+    @classmethod
+    def roots(cls, active_collect_env_num: int, legal_actions: List[Any]) -> "gmz_tree.Roots":
+        """mcts_ctree.py:1062-1074"""
+        return gmz_tree.Roots(active_collect_env_num, legal_actions)
+
+    def _params(self):
+        c = self._cfg
+        return (19652, 1.25, c.discount_factor, c.value_delta_max)
+
+    def search(self, roots: "gmz_tree.Roots", model, latent_state_roots, to_play_batch: Union[int, List[Any]]) -> None:
+        """mcts_ctree.py:1076-1172.  ``latent_state_roots``: np.ndarray or CUDA tensor."""
+        if isinstance(model, EfficientZeroModel):
+            raise TypeError("GumbelMuZeroMCTSCtree.search: the Gumbel search runs MuZero models, not an EfficientZeroModel")
+        S = int(self._cfg.num_simulations)
+        if roots._pending is None:
+            raise RuntimeError("Roots: prepare()/prepare_no_noise() has not been called")
+        m = self._cfg.get("max_num_considered_actions", None)
+        m = roots._pending["A"] if m is None else int(m)
+        roots._materialize_gumbel((m, S), self._params())   # reset + prepare on device: a fresh search
+        t = roots._tree
+        dev = roots.device
+        if isinstance(latent_state_roots, torch.Tensor):
+            lat = latent_state_roots.to(dev, torch.float32, non_blocking=True).contiguous()
+        else:
+            lat = torch.from_numpy(np.ascontiguousarray(latent_state_roots, dtype=np.float32)).to(dev, non_blocking=True)
+        if isinstance(model, (MuZeroModel, MuZeroModelMLP)):
+            q = t.search_for(model, S, ("gumbel",))
+            with torch.cuda.device(dev):
+                cabi.check(t.lib.lz_search_run_gumbel(q, lat.data_ptr(), cabi.stream_ptr()), "lz_search_run_gumbel")
+            self.last_num_kernels = t.lib.lz_search_num_kernels(q)
+            return
+        self._search_stepwise_gumbel(roots, model, lat, S)
+
+    def _search_stepwise_gumbel(self, roots, model, lat, S):
+        t = roots._tree
+        dev = roots.device
+        self._make_inverse_transforms(dev)
+        B = roots.num
+        pool = torch.empty((S + 1,) + tuple(lat.shape), device=dev, dtype=torch.float32)
+        pool[0] = lat
+        rows = torch.arange(B, device=dev)
+        with torch.no_grad(), torch.cuda.device(dev):
+            if hasattr(model, "eval"):
+                model.eval()
+            for sim in range(S):
+                cabi.check(t.lib.lz_tree_traverse_gumbel(t.h, t.ix.data_ptr(), t.iy.data_ptr(), t.action.data_ptr(),
+                                                         t.search_len.data_ptr(), t.vtp.data_ptr(), cabi.stream_ptr()),
+                           "lz_tree_traverse_gumbel")
+                out = model.recurrent_inference(pool[t.ix.long(), rows], t.action.long())
+                pool[sim + 1] = out.latent_state
+                value = self._inv(out.value).reshape(-1).contiguous()
+                reward = self._inv_reward(out.reward).reshape(-1).contiguous()
+                pol = out.policy_logits.to(torch.float32).contiguous()
+                cabi.check(t.lib.lz_tree_backpropagate_gumbel(t.h, sim + 1, reward.data_ptr(), value.data_ptr(), pol.data_ptr(),
+                                                              None, cabi.stream_ptr()), "lz_tree_backpropagate_gumbel")

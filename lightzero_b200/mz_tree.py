@@ -267,6 +267,14 @@ class Roots:
         with torch.cuda.device(self.device):
             s = cabi.stream_ptr()
             cabi.check(t.lib.lz_tree_set_ez(t.h, int(self._ez), int(self._lstm_horizon)), "lz_tree_set_ez")
+            self._reset_tree(t, s)
+            cabi.check(t.lib.lz_tree_prepare(t.h, p["logits"].data_ptr(), cabi.ptr(p["noise"]), p["w"],
+                                             cabi.ptr(p["rewards"]), cabi.ptr(p["to_play"]), s), "lz_tree_prepare")
+
+    def _reset_tree(self, t, s):
+        """lz_tree_reset / lz_tree_reset_mask of tree t to these roots' legal actions, on stream s."""
+        A = self._pending["A"]
+        with torch.cuda.device(self.device):
             if self._mask is not None:
                 if self._mask_dev is None:      # uploaded once per Roots, not once per search
                     self._mask_dev = _to_dev(self._mask, torch.uint8, self.device, (self.root_num, A))
@@ -285,8 +293,6 @@ class Roots:
                     dn = torch.from_numpy(nl).to(self.device)
                     cabi.check(t.lib.lz_tree_reset(t.h, dl.data_ptr(), dn.data_ptr(), s), "lz_tree_reset")
                     self._keep = (dl, dn)
-            cabi.check(t.lib.lz_tree_prepare(t.h, p["logits"].data_ptr(), cabi.ptr(p["noise"]), p["w"],
-                                             cabi.ptr(p["rewards"]), cabi.ptr(p["to_play"]), s), "lz_tree_prepare")
 
 
 def batch_traverse(roots: Roots, pb_c_base: int, pb_c_init: float, discount_factor: float,
