@@ -209,12 +209,11 @@ int lz_model_destroy(lz_model *m);
 int lz_model_set_tensor(lz_model *m, const char *name, const float *h_data, int64_t numel);
 /* Folds eval-mode BatchNorm into per-channel scale/shift, packs weights for the kernels, uploads. */
 int lz_model_finalize(lz_model *m);
-/* Arithmetic of the latent-grid networks (recurrent_inference and the tail of initial_inference):
- *   0 = fp32 FFMA on the CUDA cores (6x6 latent grid, 84/96-pixel MuZero models, only: LZ_EINVAL for a 64-pixel or an
- *       EfficientZero model);
- *   1 = wgmma tensor cores with fp16 hi/lo operand splitting (3 MMAs per product, fp32 accumulate in
- *       registers): fp32-accurate, the mode parity is stated for;
- *   2 = wgmma single fp16 pass (fp32 accumulate): ~3x fewer MMAs, logits accurate to ~1e-3. */
+/* Arithmetic of the conv model's tensor-core kernels (the DownSample tower and the latent-grid networks):
+ *   1 = tc3: fp16 hi/lo operand splitting (3 MMAs per product, fp32 accumulate in registers): fp32-accurate, the default
+ *       and the mode parity is stated for;
+ *   2 = tc1: single fp16 pass (fp32 accumulate): ~3x fewer MMAs, logits accurate to ~1e-3.
+ * Any other mode, and any mode on the MLP model, is LZ_EINVAL. */
 int lz_model_set_math(lz_model *m, int mode);
 /* Test hook: overrides the layer program of the tensor-core kernels (see net_tc.cuh LF_* flags). */
 int lz_model_debug_tc_program(lz_model *m, int which, int nlayers, const int *layer_w, const int *layer_flags,
@@ -231,7 +230,7 @@ int lz_debug_tc_stamps(unsigned long long *h_out);
  * h_info (int32[10]) receives the tensor geometry and the plan of the launch that wrote it:
  * C, H, W, nphase, plane_rows (nphase = plane_rows = 0 for stage 8), then G (images per CTA; 1 for the pools and the
  * conversion), band_h (output rows per CTA; 0 where the launch has no bands), stages (weight ring depth; 0 off the wgmma kernels) and the CTA count of the
- * launch, then npass (3 = tc3, 1 = tc1).  Needs a finalized conv model with math != 0 (LZ_ESTATE otherwise). */
+ * launch, then npass (3 = tc3, 1 = tc1).  Needs a finalized conv model (LZ_ESTATE otherwise). */
 int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uint8_t *d_obs_u8, int stage,
                                void *d_out, size_t out_bytes, int32_t *h_info, lz_stream s);
 /* Test hook: runs a copy of the latent-grid tensor-core program (`which` 0: recurrent_inference on d_latent f32 [B,64,h,w]
@@ -321,7 +320,7 @@ int lz_search_collect_host(lz_search *q, const float *h_obs, const uint8_t *h_ma
 /* The same two entry points for uint8 frames [B,obs_c,H,W] (Atari frames as the emulator delivers them; a quarter of the
  * bytes on the wire).  The [0, 1] scaling of the reference's env wrapper (ScaledFloatFrameWrapper: obs / 255 -> float32,
  * zoo/atari/envs/atari_wrappers.py:219-220, atari_lightzero_env.py:87-88) is applied inside the first conv kernel, bit-identical
- * to that host arithmetic.  Tensor-core conv model (math mode 1 or 2) only; 64x64, 84x84 and 96x96 frames. */
+ * to that host arithmetic.  Conv model only; 64x64, 84x84 and 96x96 frames. */
 int lz_search_collect_u8(lz_search *q, const uint8_t *d_obs_u8, const uint8_t *d_mask, const float *d_noise,
                          float noise_weight, const int32_t *d_to_play, int deterministic,
                          float *d_pred_value, float *d_policy_logits, lz_stream s);

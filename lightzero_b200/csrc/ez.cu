@@ -343,12 +343,12 @@ int ez_prepare_launch()
     return LZ_OK;
 }
 
-int ez_launch(const EzNet &net, const EzIO &io, cudaStream_t s, int math)
+int ez_launch(const EzNet &net, const EzIO &io, cudaStream_t s)
 {
     LZ_REQUIRE(net.H <= kHMaxH && net.hid <= kHMaxHid && net.K <= kHLd && (net.H % 8) == 0, LZ_EINVAL,
                "ez_launch: unsupported LSTM / head size (H=%d hid=%d K=%d)", net.H, net.hid, net.K);
     const bool tc_ok = net.wtc && ez_tc_shape(net.nin, net.H);
-    if (math != 0 && tc_ok) {
+    if (tc_ok) {
         dim3 grid(4 * net.H / kTN, (io.B + kTM - 1) / kTM);
         k_ez_lstm_tc<<<grid, kTThreads, kTSmem, s>>>(net, io);
     } else {

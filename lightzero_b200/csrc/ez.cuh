@@ -32,7 +32,7 @@ struct EzIO {
     float *vp_logits;         // [B][K] or nullptr
 };
 
-int ez_launch(const EzNet &net, const EzIO &io, cudaStream_t s, int math);   // math 0: fp32 FFMA GEMM, else tensor-core (wgmma) 3xFP16
+int ez_launch(const EzNet &net, const EzIO &io, cudaStream_t s);   // LSTM GEMM on the tensor cores (wgmma 3xFP16) where ez_tc_shape, else fp32 FFMA
 int ez_prepare_launch();
 bool ez_tc_shape(int nin, int H);   // k_ez_lstm_tc runs K = nin + H in whole chunks of 64 and N = 4H in tiles of 64
 // host: pack W ([4H][nin] and [4H][H], torch gate order) into the tensor-core layout; returns the scale applied

@@ -313,9 +313,8 @@ extern "C" int lz_model_create_mlp(const lz_mlp_config *cfg, lz_model **out)
     m->latent_floats = cfg->latent_dim;
     m->finalized = false;
     m->d_weights = nullptr; m->d_tc = nullptr; m->d_tower = nullptr; m->tws = nullptr; m->tws_bytes = 0;
-    m->hw = 1; m->P = 1; m->K = K; m->math = 0;
-    m->ws[0] = m->ws[1] = m->ws[2] = nullptr;
-    m->ws_floats = 0; m->ws_B = 1 << 30;
+    m->hw = 1; m->P = 1; m->K = K;
+    m->pre_latent = nullptr; m->ws_B = 1 << 30;
     *out = m;
     return LZ_OK;
 }

@@ -1,5 +1,6 @@
-// model.cu -- MuZero conv model forward paths (initial_inference / recurrent_inference) as fused fp32
-// CUDA kernels, plus the host-side weight registry that ingests the reference state_dict.
+// model.cu -- MuZero conv model forward paths (initial_inference / recurrent_inference): the DownSample stem, the launches of
+// the tensor-core tower (conv_tc.cu) and latent-grid network (net_tc.cu), and the host-side weight registry that ingests the
+// reference state_dict.
 //
 // Replaces the forward paths of lzero/model/muzero_model.py:210-272 (MuZeroModel), :309-374 (_dynamics
 // one-hot encoding), :505-538 (DynamicsNetwork.forward), lzero/model/common.py:334-366 (DownSample),
@@ -15,173 +16,16 @@
 
 namespace lz {
 
-// ------------------------------------------------------------------------------------------------
-// Fused recurrent inference: gather latent -> dynamics -> reward head -> prediction -> heads.
-// One warp per root, W roots per CTA (see net6.cuh).  Shared memory (floats):
-//   actA[W][2304] | actB[W][2304] | hrew[W][576] | wstage[2][4608]
-// ------------------------------------------------------------------------------------------------
-constexpr int kActFloats = kC * kP;          // 2304
-constexpr int kHFlatMax = 16 * kP;           // head channels <= 16
-constexpr int kKpad = 608;                   // support size 601 padded
-
-template <int W>
-__device__ __forceinline__ void heads_and_outputs(const NetDev &net, float *actA, float *actB, float *hrew,
-                                                  float *wstage, bool with_reward, int B, float *o_reward,
-                                                  float *o_value, float *o_policy, float *o_reward_logits,
-                                                  float *o_value_logits)
-{
-    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int A = net.A, Apad = (A + 31) & ~31;
-    // On entry: hrew[r][..] = reward-head features, actA[r][0..576) = value features,
-    // actA[r][576..1152) = policy features; actB and wstage are free.  CTA-wide sync done by caller.
-    float *lg_rew = actB;                          // [W][kKpad]
-    float *lg_val = actB + W * kKpad;              // [W][kKpad]
-    float *lg_pol = actB + 2 * W * kKpad;          // [W][Apad]
-    float *hidden = wstage;                        // [3][W][32]
-    for (int h = w; h < 3; h += W) {
-        if (h == 0) {
-            if (with_reward) head_fc<W>(net.reward, hrew, kHFlatMax, hidden, lg_rew, kKpad, lane);
-        } else if (h == 1) {
-            head_fc<W>(net.value, actA, kActFloats, hidden + W * 32, lg_val, kKpad, lane);
-        } else {
-            head_fc<W>(net.policy, actA + kHFlatMax, kActFloats, hidden + 2 * W * 32, lg_pol, Apad, lane);
-        }
-    }
-    __syncthreads();
-    const int b = blockIdx.x * W + w;
-    if (b < B) {
-        const int K = net.value.K;
-        if (with_reward) {
-            float r = categorical_to_scalar(lg_rew + w * kKpad, net.reward.K, net.support_min, net.support_step, lane);
-            if (lane == 0 && o_reward) o_reward[b] = r;
-            if (o_reward_logits)
-                for (int k = lane; k < net.reward.K; k += 32) o_reward_logits[(size_t)b * net.reward.K + k] = lg_rew[w * kKpad + k];
-        }
-        float v = categorical_to_scalar(lg_val + w * kKpad, K, net.support_min, net.support_step, lane);
-        if (lane == 0 && o_value) o_value[b] = v;
-        if (o_value_logits)
-            for (int k = lane; k < K; k += 32) o_value_logits[(size_t)b * K + k] = lg_val[w * kKpad + k];
-        if (o_policy)
-            for (int a = lane; a < A; a += 32) o_policy[(size_t)b * A + a] = lg_pol[w * Apad + a];
-    }
-}
-
-template <int W>
-__global__ void __launch_bounds__(W * 32) k_recurrent(NetDev net, RecIO io)
-{
-    extern __shared__ __align__(16) float smem[];
-    float *actA_all = smem, *actB_all = smem + W * kActFloats;
-    float *hrew_all = actB_all + W * kActFloats;
-    float *wstage = hrew_all + W * kHFlatMax;
-    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int b = blockIdx.x * W + w;
-    const bool valid = b < io.B;
-    float *actA = actA_all + w * kActFloats, *actB = actB_all + w * kActFloats, *hrew = hrew_all + w * kHFlatMax;
-
-    // gather the parent latent (NCHW [64][36], contiguous 9216 B) selected by the tree
-    if (valid) {
-        const size_t slot = io.ix ? (size_t)io.ix[b] : 0;
-        const float *src = io.latent_base + slot * io.slot_stride + (size_t)b * kActFloats;
-        for (int i = lane * 4; i < kActFloats; i += 128) cp_async16(actA + i, src + i);
-    } else {
-        for (int i = lane; i < kActFloats; i += 32) actA[i] = 0.0f;
-    }
-    cp_async_commit();
-    cp_async_wait<0>();
-    __syncwarp();
-    int act = valid ? io.action[b] : 0;
-    act = min(max(act, 0), net.A - 1);
-
-    // dynamics: x = relu(bn(conv(cat(latent, onehot))) + latent)      muzero_model.py:518-524
-    conv3x3_layer(net.dyn_conv, actA, actB, actA, act, wstage, lane);
-    float *x = actB, *t = actA;
-    for (int i = 0; i < net.nres; ++i) {                            // muzero_model.py:526-527
-        conv3x3_layer(net.dyn_res[2 * i], x, t, nullptr, -1, wstage, lane);
-        conv3x3_layer(net.dyn_res[2 * i + 1], t, x, x, -1, wstage, lane);
-    }
-    // x == next_latent_state
-    if (valid && io.next_latent) {
-        float4 *dst = reinterpret_cast<float4 *>(io.next_latent + (size_t)b * kActFloats);
-        const float4 *srcv = reinterpret_cast<const float4 *>(x);
-        for (int i = lane; i < kActFloats / 4; i += 32) dst[i] = srcv[i];
-    }
-    head_conv1x1(net.reward, x, hrew, lane);                        // muzero_model.py:530-533
-    for (int i = 0; i < net.nres; ++i) {                            // common.py:1199-1200
-        conv3x3_layer(net.pred_res[2 * i], x, t, nullptr, -1, wstage, lane);
-        conv3x3_layer(net.pred_res[2 * i + 1], t, x, x, -1, wstage, lane);
-    }
-    head_conv1x1(net.value, x, t, lane);                            // common.py:1202-1208
-    head_conv1x1(net.policy, x, t + kHFlatMax, lane);
-    __syncthreads();
-    heads_and_outputs<W>(net, actA_all, actB_all, hrew_all, wstage, true, io.B, io.reward, io.value,
-                         io.policy_logits, io.reward_logits, io.value_logits);
-}
-
-// Tail of initial inference on the latent grid: representation resblocks -> latent -> prediction.
-template <int W>
-__global__ void __launch_bounds__(W * 32) k_initial_tail(NetDev net, TailIO io)
-{
-    extern __shared__ __align__(16) float smem[];
-    float *actA_all = smem, *actB_all = smem + W * kActFloats;
-    float *hrew_all = actB_all + W * kActFloats;
-    float *wstage = hrew_all + W * kHFlatMax;
-    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int b = blockIdx.x * W + w;
-    const bool valid = b < io.B;
-    float *actA = actA_all + w * kActFloats, *actB = actB_all + w * kActFloats;
-    if (valid) {
-        const float *src = io.pre_latent + (size_t)b * kActFloats;
-        for (int i = lane * 4; i < kActFloats; i += 128) cp_async16(actA + i, src + i);
-    } else {
-        for (int i = lane; i < kActFloats; i += 32) actA[i] = 0.0f;
-    }
-    cp_async_commit();
-    cp_async_wait<0>();
-    __syncwarp();
-    float *x = actA, *t = actB;
-    for (int i = 0; i < net.nres; ++i) {                            // common.py:774-775
-        conv3x3_layer(net.rep_res[2 * i], x, t, nullptr, -1, wstage, lane);
-        conv3x3_layer(net.rep_res[2 * i + 1], t, x, x, -1, wstage, lane);
-    }
-    if (valid) {
-        const float4 *srcv = reinterpret_cast<const float4 *>(x);
-        if (io.latent) {
-            float4 *dst = reinterpret_cast<float4 *>(io.latent + (size_t)b * kActFloats);
-            for (int i = lane; i < kActFloats / 4; i += 32) dst[i] = srcv[i];
-        }
-        if (io.latent2) {
-            float4 *dst = reinterpret_cast<float4 *>(io.latent2 + (size_t)b * kActFloats);
-            for (int i = lane; i < kActFloats / 4; i += 32) dst[i] = srcv[i];
-        }
-    }
-    for (int i = 0; i < net.nres; ++i) {
-        conv3x3_layer(net.pred_res[2 * i], x, t, nullptr, -1, wstage, lane);
-        conv3x3_layer(net.pred_res[2 * i + 1], t, x, x, -1, wstage, lane);
-    }
-    // x == actA here; the head features must land in actA for heads_and_outputs, so stage via t
-    head_conv1x1(net.value, x, t, lane);
-    head_conv1x1(net.policy, x, t + kHFlatMax, lane);
-    __syncwarp();
-    for (int i = lane; i < 2 * kHFlatMax; i += 32) x[i] = t[i];
-    __syncthreads();
-    heads_and_outputs<W>(net, actA_all, actB_all, hrew_all, wstage, false, io.B, nullptr, io.value,
-                         io.policy_logits, nullptr, io.value_logits);
-}
-
-static inline size_t fused_smem_bytes(int W)
-{
-    return (size_t)(2 * W * kActFloats + W * kHFlatMax + 2 * kStageFloats) * sizeof(float);
-}
+constexpr int kKpad = 608;                   // largest support size of the tensor-core heads (601 padded)
 
 // ------------------------------------------------------------------------------------------------
-// DownSample tower (common.py:334-366): generic direct 3x3 convolution, NCHW, stride 1 or 2, folded
-// BN + optional residual + optional ReLU.  One thread per output pixel (128 consecutive linear
-// pixels per CTA), 32 output channels per CTA.
+// The stem of the DownSample tower (conv1 + norm1 + ReLU, common.py:334-366) for the input channel counts k_stem4_tcl does not
+// take (e.g. 3- or 9-channel frames): direct 3x3 convolution of stride S = 2 from NCHW, written into the tensor-core layout of
+// the first wgmma layer.  One thread per output pixel (128 consecutive linear pixels per CTA), 32 output channels per CTA.
 // ------------------------------------------------------------------------------------------------
 template <int S>
 __global__ void __launch_bounds__(128)
-k_conv3x3_generic(ConvG L, const float *__restrict__ in, float *__restrict__ out, const float *__restrict__ res,
-                  int relu, int cic, int nrows_max, Tcl tcl, const uint8_t *__restrict__ in_u8 = nullptr)
+k_conv3x3_generic(ConvG L, const float *__restrict__ in, int cic, int nrows_max, Tcl tcl, const uint8_t *__restrict__ in_u8)
 {
     extern __shared__ __align__(16) float sm[];
     const int pitch = L.win + 2;
@@ -240,28 +84,16 @@ k_conv3x3_generic(ConvG L, const float *__restrict__ in, float *__restrict__ out
         }
         __syncthreads();
     }
-    if (valid && tcl.base) {
+    if (valid) {
         // write the tensor-core layout of conv_tc.cuh (fp16 hi/lo, k-group planes over the padded grid)
         float v[32];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-            v[j] = fmaf(acc[j], __ldg(L.scale + co0 + j), __ldg(L.shift + co0 + j));
-            if (relu) v[j] = fmaxf(v[j], 0.0f);
-        }
+        for (int j = 0; j < 32; ++j) v[j] = fmaxf(fmaf(acc[j], __ldg(L.scale + co0 + j), __ldg(L.shift + co0 + j)), 0.0f);
         const int rho = (y + 1) * tcl.pitch + x;
 #pragma unroll
         for (int g = 0; g < 4; ++g) {
             unsigned char *op = tcl.base + (size_t)b * tcl.img_stride + ((size_t)(co0 / 8 + g) * tcl.plane_rows + rho + 1) * 16;
             store_split8(op, op + tcl.part_stride, v + 8 * g);
-        }
-    } else if (valid) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-            const size_t o = (((size_t)b * L.cout + co0 + j) * L.hout + y) * L.wout + x;
-            float v = fmaf(acc[j], __ldg(L.scale + co0 + j), __ldg(L.shift + co0 + j));
-            if (res) v += res[o];
-            if (relu) v = fmaxf(v, 0.0f);
-            out[o] = v;
         }
     }
 }
@@ -331,31 +163,6 @@ k_stem4_tcl(const __grid_constant__ StemP P, const float *__restrict__ in, const
     }
 }
 
-// nn.AvgPool2d(kernel_size=3, stride=2, padding=1), count_include_pad=True (divisor 9)
-__global__ void k_avgpool3s2(const float *__restrict__ in, float *__restrict__ out, int planes, int hin, int win,
-                             int hout, int wout)
-{
-    const size_t n = (size_t)planes * hout * wout;
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        int xo = (int)(i % wout), yo = (int)((i / wout) % hout);
-        size_t pl = i / ((size_t)wout * hout);
-        const float *src = in + pl * hin * win;
-        float s = 0.0f;
-#pragma unroll
-        for (int ky = 0; ky < 3; ++ky) {
-            int yy = yo * 2 + ky - 1;
-            if (yy < 0 || yy >= hin) continue;
-#pragma unroll
-            for (int kx = 0; kx < 3; ++kx) {
-                int xx = xo * 2 + kx - 1;
-                if (xx < 0 || xx >= win) continue;
-                s += src[yy * win + xx];
-            }
-        }
-        out[i] = s / 9.0f;
-    }
-}
-
 __global__ void k_inverse_scalar(const float *logits, float *out, int B, int K, float smin, float sstep)
 {
     const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
@@ -367,116 +174,55 @@ __global__ void k_inverse_scalar(const float *logits, float *out, int B, int K, 
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-static int pick_W(int B)
-{
-    // largest roots-per-CTA that still yields ~one CTA per SM; small batches use small CTAs
-    if (B >= 8 * 120) return 8;
-    if (B >= 4 * 120) return 4;
-    if (B >= 2 * 120) return 2;
-    return 1;
-}
-
-template <int W>
-static int launch_recurrent(const NetDev &net, const RecIO &io, cudaStream_t s)
-{
-    const size_t smem = fused_smem_bytes(W);
-    k_recurrent<W><<<ceil_div(io.B, W), W * 32, smem, s>>>(net, io);
-    LZ_KERNEL_CHECK();
-    return LZ_OK;
-}
-
-template <int W>
-static int launch_tail(const NetDev &net, const TailIO &io, cudaStream_t s)
-{
-    const size_t smem = fused_smem_bytes(W);
-    k_initial_tail<W><<<ceil_div(io.B, W), W * 32, smem, s>>>(net, io);
-    LZ_KERNEL_CHECK();
-    return LZ_OK;
-}
-
-template <int W>
-static int set_fused_attrs()
-{
-    const int smem = (int)fused_smem_bytes(W);
-    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_recurrent<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_initial_tail<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    return LZ_OK;
-}
-
-// opt-in shared memory sizes are set once, outside any stream capture
+// opt-in shared memory size, set once outside any stream capture
 static int model_prepare_launch()
 {
-    int rc;
-    if ((rc = set_fused_attrs<8>()) || (rc = set_fused_attrs<4>()) || (rc = set_fused_attrs<2>()) || (rc = set_fused_attrs<1>())) return rc;
-    const int big = 200 * 1024;
-    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_generic<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
-    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_generic<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
+    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_generic<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     return LZ_OK;
 }
 
 int model_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
 {
     if (m->kind == 1) return mlp_recurrent(m, io, s);
-    if (m->math != 0) {
-        TcIO t;
-        memset(&t, 0, sizeof(t));
-        t.B = io.B; t.npass = (m->math == 1) ? 3 : 1;
-        t.latent_base = io.latent_base; t.ix = io.ix; t.slot_stride = io.slot_stride; t.action = io.action;
-        t.latent_out = io.next_latent; t.reward = io.reward; t.value = io.value; t.policy_logits = io.policy_logits;
-        t.reward_logits = io.reward_logits; t.value_logits = io.value_logits;
-        t.skip_scratch = io.skip_scratch;
-        if (!t.skip_scratch) {
-            LZ_REQUIRE(io.B <= m->tc_skip_B, LZ_ESTATE, "model_recurrent: scratch sized for %d roots, got %d (model_reserve)", m->tc_skip_B, io.B);
-            t.skip_scratch = m->tc_skip;
-        }
-        if (m->cfg.efficientzero) {
-            // conv trunk + prediction heads on the tensor cores; the reward features go through the LSTM head (ez.cu)
-            LZ_REQUIRE(io.B <= m->ez_B, LZ_ESTATE, "model_recurrent: EfficientZero scratch sized for %d roots, got %d (model_reserve)", m->ez_B, io.B);
-            LZ_REQUIRE(io.h_base && io.c_base, LZ_EINVAL, "model_recurrent: EfficientZero needs the reward hidden state");
-            t.reward = nullptr; t.reward_logits = nullptr; t.ez_feat = m->ez_feat;
-            int rc = tc_launch(m->tc_rec, t, s);
-            if (rc) return rc;
-            EzIO e;
-            memset(&e, 0, sizeof(e));
-            e.B = io.B; e.feat = m->ez_feat; e.h_base = io.h_base; e.c_base = io.c_base; e.ix = io.ix; e.slot_stride = io.hslot_stride;
-            e.h_out = io.h_out; e.c_out = io.c_out; e.is_reset = io.is_reset; e.h_tmp = m->ez_htmp;
-            e.value_prefix = io.reward; e.vp_logits = io.reward_logits;
-            return ez_launch(m->ez, e, s, m->math);
-        }
-        return tc_launch(m->tc_rec, t, s);
+    TcIO t;
+    memset(&t, 0, sizeof(t));
+    t.B = io.B; t.npass = m->npass;
+    t.latent_base = io.latent_base; t.ix = io.ix; t.slot_stride = io.slot_stride; t.action = io.action;
+    t.latent_out = io.next_latent; t.reward = io.reward; t.value = io.value; t.policy_logits = io.policy_logits;
+    t.reward_logits = io.reward_logits; t.value_logits = io.value_logits;
+    t.skip_scratch = io.skip_scratch;
+    if (!t.skip_scratch) {
+        LZ_REQUIRE(io.B <= m->tc_skip_B, LZ_ESTATE, "model_recurrent: scratch sized for %d roots, got %d (model_reserve)", m->tc_skip_B, io.B);
+        t.skip_scratch = m->tc_skip;
     }
-    switch (pick_W(io.B)) {
-        case 8: return launch_recurrent<8>(m->net, io, s);
-        case 4: return launch_recurrent<4>(m->net, io, s);
-        case 2: return launch_recurrent<2>(m->net, io, s);
-        default: return launch_recurrent<1>(m->net, io, s);
+    if (m->cfg.efficientzero) {
+        // conv trunk + prediction heads on the tensor cores; the reward features go through the LSTM head (ez.cu)
+        LZ_REQUIRE(io.B <= m->ez_B, LZ_ESTATE, "model_recurrent: EfficientZero scratch sized for %d roots, got %d (model_reserve)", m->ez_B, io.B);
+        LZ_REQUIRE(io.h_base && io.c_base, LZ_EINVAL, "model_recurrent: EfficientZero needs the reward hidden state");
+        t.reward = nullptr; t.reward_logits = nullptr; t.ez_feat = m->ez_feat;
+        int rc = tc_launch(m->tc_rec, t, s);
+        if (rc) return rc;
+        EzIO e;
+        memset(&e, 0, sizeof(e));
+        e.B = io.B; e.feat = m->ez_feat; e.h_base = io.h_base; e.c_base = io.c_base; e.ix = io.ix; e.slot_stride = io.hslot_stride;
+        e.h_out = io.h_out; e.c_out = io.c_out; e.is_reset = io.is_reset; e.h_tmp = m->ez_htmp;
+        e.value_prefix = io.reward; e.vp_logits = io.reward_logits;
+        return ez_launch(m->ez, e, s);
     }
+    return tc_launch(m->tc_rec, t, s);
 }
 
-static int launch_convg(const ConvG &L, const float *in, float *out, const float *res, int relu, int B, cudaStream_t s,
-                        const Tcl *tcl = nullptr, const uint8_t *in_u8 = nullptr)
+// the stem for input channel counts other than 4 (k_stem4_tcl), into the first TCL tensor
+static int launch_stem_generic(const ConvG &L, const float *in, const uint8_t *in_u8, int B, const Tcl &tcl, cudaStream_t s)
 {
-    Tcl t;
-    memset(&t, 0, sizeof(t));
-    if (tcl) t = *tcl;
     const int cic = std::min(8, L.cin);
     const int rows_out_max = std::min(L.hout, 127 / L.wout + 2);
-    const int nrows_max = (rows_out_max - 1) * L.stride + 3;
+    const int nrows_max = (rows_out_max - 1) * 2 + 3;
     const int pitch = L.win + 2;
     const size_t smem = ((((size_t)cic * nrows_max * pitch + 3) & ~(size_t)3) + (size_t)cic * 288) * sizeof(float);
     dim3 grid(ceil_div(L.hout * L.wout, 128), L.cout / 32, B);
-    LZ_REQUIRE(smem <= 200 * 1024, LZ_EINVAL, "conv tower stage needs %zu B shared memory", smem);
-    if (L.stride == 1) k_conv3x3_generic<1><<<grid, 128, smem, s>>>(L, in, out, res, relu, cic, nrows_max, t, in_u8);
-    else k_conv3x3_generic<2><<<grid, 128, smem, s>>>(L, in, out, res, relu, cic, nrows_max, t, in_u8);
-    LZ_KERNEL_CHECK();
-    return LZ_OK;
-}
-
-static int launch_pool(const float *in, float *out, int planes, int hin, int hout, cudaStream_t s)
-{
-    const size_t n = (size_t)planes * hout * hout;
-    int blocks = (int)std::min<size_t>((n + 255) / 256, kNumSMs * 16);
-    k_avgpool3s2<<<blocks, 256, 0, s>>>(in, out, planes, hin, hin, hout, hout);
+    LZ_REQUIRE(smem <= 200 * 1024, LZ_EINVAL, "DownSample stem needs %zu B shared memory", smem);
+    k_conv3x3_generic<2><<<grid, 128, smem, s>>>(L, in, cic, nrows_max, tcl, in_u8);
     LZ_KERNEL_CHECK();
     return LZ_OK;
 }
@@ -511,20 +257,16 @@ int model_reserve(lz_model *m, int B)
     }
     if (m->kind == 1 || B <= m->ws_B) return LZ_OK;
     ++m->generation;
-    size_t per_root = 0;
-    for (const ConvG &L : m->tower) per_root = std::max(per_root, (size_t)L.cout * L.hout * L.wout);
-    per_root = std::max(per_root, (size_t)m->latent_floats);
-    for (int i = 0; i < 3; ++i) {
-        if (m->ws[i]) cudaFree(m->ws[i]);
-        m->ws[i] = nullptr;
-        int rc = dev_alloc(&m->ws[i], per_root * B);
+    cudaFree(m->pre_latent);
+    m->pre_latent = nullptr;
+    {
+        int rc = dev_alloc(&m->pre_latent, (size_t)m->latent_floats * B);
         if (rc != LZ_OK) return rc;
     }
-    m->ws_floats = per_root * B;
     m->ws_B = B;
     // TCL activation workspace of the tensor-core tower (zeroed once: pad rows / columns are never written non-zero)
     {
-        const int h1 = m->tower[0].hout, h2 = m->tower[3].hout, h3 = (h2 - 1) / 2 + 1, c2 = kC / 2;
+        const int h1 = m->stem.hout, h2 = (h1 - 1) / 2 + 1, h3 = (h2 - 1) / 2 + 1, c2 = kC / 2;
         const size_t bT = tcl_bytes(B, c2, h1, h1, 1), bT2 = tcl_bytes(B, c2, h1 / 2, h1 / 2, 4);
         const size_t bU = tcl_bytes(B, kC, h2, h2, 1), bV = tcl_bytes(B, kC, h3, h3, 1);
         const size_t total = bT + bT2 + 3 * bU + 2 * bV;
@@ -580,9 +322,9 @@ static int tower_tc_run(lz_model *m, int B, const float *d_obs, float *pre_laten
                         int stop_after = 8)
 {
     int rc;
-    const int npass = (m->math == 1) ? 3 : 1;
-    // stem: conv1 (Cin = 4/12, stride 2) on the CUDA cores, written straight into TCL (uint8 frames are scaled to [0, 1] here)
-    const ConvG &S0 = m->tower[0];
+    const int npass = m->npass;
+    // stem: conv1 (stride 2) on the CUDA cores, written straight into TCL (uint8 frames are scaled to [0, 1] here)
+    const ConvG &S0 = m->stem;
     if (m->stem_valid) {
         const int rows_per_cta = std::max(1, 256 / S0.wout);
         const size_t smem = (size_t)4 * (2 * rows_per_cta + 1) * (S0.win + 4) * sizeof(float);
@@ -591,7 +333,7 @@ static int tower_tc_run(lz_model *m, int B, const float *d_obs, float *pre_laten
         if (d_obs_u8) k_stem4_tcl<true><<<grid, 256, smem, s>>>(P, nullptr, d_obs_u8, S0.hin, S0.win, S0.hout, S0.wout, rows_per_cta, m->T0);
         else k_stem4_tcl<false><<<grid, 256, smem, s>>>(P, d_obs, nullptr, S0.hin, S0.win, S0.hout, S0.wout, rows_per_cta, m->T0);
         LZ_KERNEL_CHECK();
-    } else if ((rc = launch_convg(S0, d_obs, nullptr, nullptr, 1, B, s, &m->T0, d_obs_u8))) return rc;
+    } else if ((rc = launch_stem_generic(S0, d_obs, d_obs_u8, B, m->T0, s))) return rc;
     if (stop_after <= 0) return LZ_OK;
     auto run = [&](ConvTc p, const Tcl &in, const Tcl &o0, const Tcl *o1, const Tcl *res) {
         p.in = in; p.out[0] = o0;
@@ -621,10 +363,10 @@ static int tower_tc_run(lz_model *m, int B, const float *d_obs, float *pre_laten
     return pool_tcl_to_nchw_launch(m->V1, pre_latent, B, m->hw, s);                  // pooling2 -> [B][64][6][6]
 }
 
-// tensor-core path only: the DownSample tower alone (obs -> pre-latent [B][64][36]) ...
+// conv model only: the DownSample tower alone (obs -> pre-latent [B][64][P]) ...
 int model_initial_tower(lz_model *m, int B, const float *d_obs, float *pre_latent, cudaStream_t s, const uint8_t *d_obs_u8)
 {
-    LZ_REQUIRE(m->kind == 0 && m->math != 0, LZ_ESTATE, "model_initial_tower: tensor-core conv model only");
+    LZ_REQUIRE(m->kind == 0, LZ_ESTATE, "model_initial_tower: conv model only");
     LZ_REQUIRE(B <= m->ws_B, LZ_ESTATE, "model_initial_tower: workspace sized for %d roots, got %d", m->ws_B, B);
     return tower_tc_run(m, B, d_obs, pre_latent, s, d_obs_u8);
 }
@@ -634,7 +376,7 @@ int model_initial_tail(lz_model *m, int B, const float *pre_latent, const TailIO
 {
     TcIO t;
     memset(&t, 0, sizeof(t));
-    t.B = B; t.npass = (m->math == 1) ? 3 : 1;
+    t.B = B; t.npass = m->npass;
     t.latent_base = pre_latent; t.latent_out = io_in.latent; t.latent_out2 = io_in.latent2;
     t.value = io_in.value; t.policy_logits = io_in.policy_logits; t.value_logits = io_in.value_logits;
     LZ_REQUIRE(B <= m->tc_skip_B, LZ_ESTATE, "model_initial_tail: scratch sized for %d roots, got %d (model_reserve)", m->tc_skip_B, B);
@@ -646,37 +388,9 @@ int model_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, c
 {
     if (m->kind == 1) return mlp_initial(m, B, d_obs, io_in, s);
     LZ_REQUIRE(B <= m->ws_B, LZ_ESTATE, "model_initial: workspace sized for %d roots, got %d (call model_reserve outside capture)", m->ws_B, B);
-    float *a = m->ws[0], *b = m->ws[1], *c = m->ws[2];
-    const std::vector<ConvG> &T = m->tower;
-    int rc;
-    if (m->math != 0) {
-        if ((rc = tower_tc_run(m, B, d_obs, a, s))) return rc;
-        return model_initial_tail(m, B, a, io_in, s);
-    }
-    // DownSample.forward, common.py:340-366
-    if ((rc = launch_convg(T[0], d_obs, a, nullptr, 1, B, s))) return rc;          // conv1 + norm1 + relu
-    if ((rc = launch_convg(T[1], a, b, nullptr, 1, B, s))) return rc;              // resblocks1.0
-    if ((rc = launch_convg(T[2], b, c, a, 1, B, s))) return rc;
-    if ((rc = launch_convg(T[3], c, a, nullptr, 0, B, s))) return rc;              // downsample_block.conv3 (identity path)
-    if ((rc = launch_convg(T[4], c, b, nullptr, 1, B, s))) return rc;              // downsample_block.conv1
-    if ((rc = launch_convg(T[5], b, c, a, 1, B, s))) return rc;                    // downsample_block.conv2 + identity
-    if ((rc = launch_convg(T[6], c, a, nullptr, 1, B, s))) return rc;              // resblocks2.0
-    if ((rc = launch_convg(T[7], a, b, c, 1, B, s))) return rc;
-    const int h2 = T[7].hout, h3 = (h2 - 1) / 2 + 1;
-    if ((rc = launch_pool(b, a, B * kC, h2, h3, s))) return rc;                    // pooling1
-    if ((rc = launch_convg(T[8], a, b, nullptr, 1, B, s))) return rc;              // resblocks3.0
-    if ((rc = launch_convg(T[9], b, c, a, 1, B, s))) return rc;
-    const int h4 = (h3 - 1) / 2 + 1;                                               // pooling2 (84 / 96 px: this path is 6x6 only)
-    if ((rc = launch_pool(c, a, B * kC, h3, h4, s))) return rc;
-    TailIO io = io_in;
-    io.B = B;
-    io.pre_latent = a;
-    switch (pick_W(B)) {
-        case 8: return launch_tail<8>(m->net, io, s);
-        case 4: return launch_tail<4>(m->net, io, s);
-        case 2: return launch_tail<2>(m->net, io, s);
-        default: return launch_tail<1>(m->net, io, s);
-    }
+    int rc = tower_tc_run(m, B, d_obs, m->pre_latent, s);
+    if (rc) return rc;
+    return model_initial_tail(m, B, m->pre_latent, io_in, s);
 }
 
 // ---- weight ingestion -------------------------------------------------------------------------
@@ -735,36 +449,21 @@ static bool pack_conv3(lz_model *m, Packer &P, const std::string &wname, const s
     return true;
 }
 
-struct HeadOff { size_t w1, s1, t1, fc1, s2, t2, fc2, b2; int hc, hid, K; };
+struct HeadOff { size_t s2, t2, b2; int hc, hid, K; };
 
-static bool pack_head(lz_model *m, Packer &P, const std::string &conv, const std::string &norm, const std::string &fc,
-                      int hc, int hid, int K, int Pix, HeadOff &o)
+// the fp32 tables of a head's FC part that k_net_tc reads (pack_tc packs the weights); fc empty: EfficientZero's reward head,
+// whose FC part follows the LSTM (ez.cu), is recorded with hid = 0
+static bool pack_head(lz_model *m, Packer &P, const std::string &fc, int hc, int hid, int K, HeadOff &o)
 {
-    auto w1 = find(m, conv + ".weight", (size_t)hc * kC), b1 = find(m, conv + ".bias", hc);
-    if (!w1 || !b1) return false;
-    std::vector<float> s1, t1, s2, t2;
-    if (!fold_bn(m, norm, hc, s1, t1)) return false;
-    for (int i = 0; i < hc; ++i) t1[i] += s1[i] * (*b1)[i];
-    if (fc.empty()) {               // EfficientZero reward head: only the 1x1 conv part lives here (the rest is ez.cu)
-        o.w1 = P.add(*w1); o.s1 = P.add(s1); o.t1 = P.add(t1);
-        o.fc1 = o.s2 = o.t2 = o.fc2 = o.b2 = o.w1;
-        o.hc = hc; o.hid = 0; o.K = K;
-        return true;
-    }
-    auto W0 = find(m, fc + ".0.weight", (size_t)hid * hc * Pix), B0 = find(m, fc + ".0.bias", hid);
-    auto W3 = find(m, fc + ".3.weight", (size_t)K * hid), B3 = find(m, fc + ".3.bias", K);
-    if (!W0 || !B0 || !W3 || !B3) return false;
-    if (!fold_bn(m, fc + ".1", hid, s2, t2)) return false;
+    o.s2 = o.t2 = o.b2 = 0;
+    o.hc = hc; o.hid = 0; o.K = K;
+    if (fc.empty()) return true;
+    auto B0 = find(m, fc + ".0.bias", hid), B3 = find(m, fc + ".3.bias", K);
+    std::vector<float> s2, t2;
+    if (!B0 || !B3 || !fold_bn(m, fc + ".1", hid, s2, t2)) return false;
     for (int j = 0; j < hid; ++j) t2[j] += s2[j] * (*B0)[j];
-    const int nin = hc * Pix;
-    std::vector<float> fc1((size_t)nin * hid), fc2((size_t)hid * K);
-    for (int j = 0; j < hid; ++j)
-        for (int i = 0; i < nin; ++i) fc1[(size_t)i * hid + j] = (*W0)[(size_t)j * nin + i];
-    for (int k = 0; k < K; ++k)
-        for (int j = 0; j < hid; ++j) fc2[(size_t)j * K + k] = (*W3)[(size_t)k * hid + j];
-    o.w1 = P.add(*w1); o.s1 = P.add(s1); o.t1 = P.add(t1); o.fc1 = P.add(fc1);
-    o.s2 = P.add(s2); o.t2 = P.add(t2); o.fc2 = P.add(fc2); o.b2 = P.add(*B3);
-    o.hc = hc; o.hid = hid; o.K = K;
+    o.s2 = P.add(s2); o.t2 = P.add(t2); o.b2 = P.add(*B3);
+    o.hid = hid;
     return true;
 }
 
@@ -773,7 +472,7 @@ static int pack_tower_tc(lz_model *m)
 {
     const std::string R = "representation_network.downsample_net.";
     const int c2 = kC / 2;
-    const int h1 = m->tower[0].hout, h2 = m->tower[3].hout, h3 = (h2 - 1) / 2 + 1;
+    const int h1 = m->stem.hout, h2 = (h1 - 1) / 2 + 1, h3 = (h2 - 1) / 2 + 1;
     struct Item { std::string w, bn; int cin, cout; };
     // layer table: 0 rb1.c1, 1 rb1.c2, 2 ds.c1 | ds.c3 (merged N=128), 3 ds.c2, 4 rb2.c1, 5 rb2.c2, 6 rb3.c1, 7 rb3.c2
     // (layers 0-1, 4-5 and 6-7 run as fused ResBlocks, 2 and 3 as single convs)
@@ -860,7 +559,7 @@ static int pack_tower_tc(lz_model *m)
 }
 
 // ---- tensor-core tables (net_tc.cu): fp16 hi/lo weights, folded BN, action-bias planes, layer programs ----
-static int pack_tc(lz_model *m, const NetDev &net)
+static int pack_tc(lz_model *m, const Head &reward, const Head &value, const Head &policy)
 {
     const lz_model_config &c = m->cfg;
     const int A = c.action_space_size, n = c.num_res_blocks;
@@ -875,7 +574,7 @@ static int pack_tc(lz_model *m, const NetDev &net)
     // FC weight stream of the heads (16 KB stages for the shared-memory ring of k_net_tc, fp16 hi / lo, the weights are the
     // tensor cores' M operand): 16 P / 32 FC1 stages covering all three heads, then one stage per 128-output tile of each head's FC2
     const std::string fc_names[3] = {"dynamics_network.fc_reward_head", "prediction_network.fc_value", "prediction_network.fc_policy"};
-    const Head *fc_heads[3] = {&net.reward, &net.value, &net.policy};
+    const Head *fc_heads[3] = {&reward, &value, &policy};
     size_t fc_off2[3];
     size_t off_fc = (off_abias + (size_t)A * kC * P * 4 + 127) & ~(size_t)127;
     const size_t off_fc0 = off_fc;
@@ -989,7 +688,7 @@ static int pack_tc(lz_model *m, const NetDev &net)
     base.bn = reinterpret_cast<const float *>(m->d_tc + off_bn);
     base.head_bn = reinterpret_cast<const float *>(m->d_tc + off_headbn);
     base.abias = reinterpret_cast<const float *>(m->d_tc + off_abias);
-    base.reward = net.reward; base.value = net.value; base.policy = net.policy;
+    base.reward = reward; base.value = value; base.policy = policy;
     base.fcw = m->d_tc + off_fc0;
     for (int h = 0; h < 3; ++h) {
         base.fc[h].fc2_off = (uint32_t)fc_off2[h];
@@ -1061,9 +760,8 @@ int lz_model_create(const lz_model_config *cfg, lz_model **out)
     m->finalized = false;
     m->d_weights = nullptr;
     m->hw = hw; m->P = hw * hw; m->K = K;
-    m->ws[0] = m->ws[1] = m->ws[2] = nullptr;
-    m->ws_floats = 0; m->ws_B = 0;
-    m->math = 1; m->d_tc = nullptr;   // default: tensor-core 3xFP16 (fp32-accurate)
+    m->pre_latent = nullptr; m->ws_B = 0;
+    m->npass = 3; m->d_tc = nullptr;   // default: tc3 (fp32-accurate)
     m->d_tower = nullptr; m->tws = nullptr; m->tws_bytes = 0; m->tc_skip = nullptr; m->tc_skip_B = 0;
     *out = m;
     return LZ_OK;
@@ -1078,7 +776,7 @@ int lz_model_destroy(lz_model *m)
     cudaFree(m->tws);
     cudaFree(m->tc_skip);
     cudaFree(m->ez_feat); cudaFree(m->ez_htmp); cudaFree(m->d_ez_wtc);
-    for (int i = 0; i < 3; ++i) cudaFree(m->ws[i]);
+    cudaFree(m->pre_latent);
     delete m;
     return LZ_OK;
 }
@@ -1102,38 +800,15 @@ int lz_model_finalize(lz_model *m)
     ++m->generation;          // every device table is re-allocated below: graphs captured against the old ones are stale
     if (m->kind == 1) return mlp_finalize(m);
     const lz_model_config &c = m->cfg;
-    const int A = c.action_space_size, n = c.num_res_blocks;
+    const int A = c.action_space_size;
     Packer P;
-    std::vector<ConvOff> tower(10);
-    ConvOff dyn_conv, dyn_res[2 * kMaxResBlocks], pred_res[2 * kMaxResBlocks], rep_res[2 * kMaxResBlocks];
+    ConvOff stem;
     HeadOff hr, hv, hp;
     const std::string R = "representation_network.downsample_net.", D = "dynamics_network.", Q = "prediction_network.";
-    const int c2 = kC / 2;
-    bool ok = pack_conv3(m, P, R + "conv1.weight", R + "norm1", c.obs_c, c2, tower[0]) &&
-              pack_conv3(m, P, R + "resblocks1.0.conv1.0.weight", R + "resblocks1.0.conv1.1", c2, c2, tower[1]) &&
-              pack_conv3(m, P, R + "resblocks1.0.conv2.0.weight", R + "resblocks1.0.conv2.1", c2, c2, tower[2]) &&
-              pack_conv3(m, P, R + "downsample_block.conv3.0.weight", "", c2, kC, tower[3]) &&
-              pack_conv3(m, P, R + "downsample_block.conv1.0.weight", R + "downsample_block.conv1.1", c2, kC, tower[4]) &&
-              pack_conv3(m, P, R + "downsample_block.conv2.0.weight", R + "downsample_block.conv2.1", kC, kC, tower[5]) &&
-              pack_conv3(m, P, R + "resblocks2.0.conv1.0.weight", R + "resblocks2.0.conv1.1", kC, kC, tower[6]) &&
-              pack_conv3(m, P, R + "resblocks2.0.conv2.0.weight", R + "resblocks2.0.conv2.1", kC, kC, tower[7]) &&
-              pack_conv3(m, P, R + "resblocks3.0.conv1.0.weight", R + "resblocks3.0.conv1.1", kC, kC, tower[8]) &&
-              pack_conv3(m, P, R + "resblocks3.0.conv2.0.weight", R + "resblocks3.0.conv2.1", kC, kC, tower[9]);
-    if (!ok) return LZ_EINVAL;
-    ok = pack_conv3(m, P, D + "conv.weight", D + "norm_common", kC + A, kC, dyn_conv);
-    for (int i = 0; ok && i < n; ++i) {
-        const std::string si = std::to_string(i);
-        ok = pack_conv3(m, P, D + "resblocks." + si + ".conv1.0.weight", D + "resblocks." + si + ".conv1.1", kC, kC, dyn_res[2 * i]) &&
-             pack_conv3(m, P, D + "resblocks." + si + ".conv2.0.weight", D + "resblocks." + si + ".conv2.1", kC, kC, dyn_res[2 * i + 1]) &&
-             pack_conv3(m, P, Q + "resblocks." + si + ".conv1.0.weight", Q + "resblocks." + si + ".conv1.1", kC, kC, pred_res[2 * i]) &&
-             pack_conv3(m, P, Q + "resblocks." + si + ".conv2.0.weight", Q + "resblocks." + si + ".conv2.1", kC, kC, pred_res[2 * i + 1]) &&
-             pack_conv3(m, P, "representation_network.resblocks." + si + ".conv1.0.weight", "representation_network.resblocks." + si + ".conv1.1", kC, kC, rep_res[2 * i]) &&
-             pack_conv3(m, P, "representation_network.resblocks." + si + ".conv2.0.weight", "representation_network.resblocks." + si + ".conv2.1", kC, kC, rep_res[2 * i + 1]);
-    }
-    if (!ok) return LZ_EINVAL;
-    ok = pack_head(m, P, D + "conv1x1_reward", D + "norm_reward", c.efficientzero ? std::string() : D + "fc_reward_head", c.reward_head_channels, c.reward_hidden, m->K, m->P, hr) &&
-         pack_head(m, P, Q + "conv1x1_value", Q + "norm_value", Q + "fc_value", c.value_head_channels, c.value_hidden, m->K, m->P, hv) &&
-         pack_head(m, P, Q + "conv1x1_policy", Q + "norm_policy", Q + "fc_policy", c.policy_head_channels, c.policy_hidden, A, m->P, hp);
+    bool ok = pack_conv3(m, P, R + "conv1.weight", R + "norm1", c.obs_c, kC / 2, stem) &&
+              pack_head(m, P, c.efficientzero ? std::string() : D + "fc_reward_head", c.reward_head_channels, c.reward_hidden, m->K, hr) &&
+              pack_head(m, P, Q + "fc_value", c.value_head_channels, c.value_hidden, m->K, hv) &&
+              pack_head(m, P, Q + "fc_policy", c.policy_head_channels, c.policy_hidden, A, hp);
     if (!ok) return LZ_EINVAL;
     // ---- EfficientZero value-prefix head (efficientzero_model.py:511-525, 556-569)
     float ez_scale = 1.0f;
@@ -1183,18 +858,12 @@ int lz_model_finalize(lz_model *m)
     LZ_CUDA_CHECK(cudaMemcpy(m->d_weights, P.host.data(), P.host.size() * sizeof(float), cudaMemcpyHostToDevice));
     m->n_weight_floats = P.host.size();
     const float *base = m->d_weights;
-    auto mk3 = [&](const ConvOff &o) { Conv3 L; L.w = base + o.w; L.scale = base + o.scale; L.shift = base + o.shift; L.cin = o.cin; return L; };
     auto mkh = [&](const HeadOff &o) {
-        Head H; H.w1 = base + o.w1; H.s1 = base + o.s1; H.t1 = base + o.t1; H.fc1 = base + o.fc1; H.s2 = base + o.s2;
-        H.t2 = base + o.t2; H.fc2 = base + o.fc2; H.b2 = base + o.b2; H.hc = o.hc; H.hid = o.hid; H.K = o.K; return H;
+        Head H;
+        H.s2 = o.hid ? base + o.s2 : nullptr; H.t2 = o.hid ? base + o.t2 : nullptr; H.b2 = o.hid ? base + o.b2 : nullptr;
+        H.hc = o.hc; H.hid = o.hid; H.K = o.K;
+        return H;
     };
-    NetDev &net = m->net;
-    memset(&net, 0, sizeof(net));
-    net.dyn_conv = mk3(dyn_conv);
-    for (int i = 0; i < 2 * n; ++i) { net.dyn_res[i] = mk3(dyn_res[i]); net.pred_res[i] = mk3(pred_res[i]); net.rep_res[i] = mk3(rep_res[i]); }
-    net.reward = mkh(hr); net.value = mkh(hv); net.policy = mkh(hp);
-    net.nres = n; net.A = A;
-    net.support_min = c.support_min; net.support_step = c.support_step;
     memset(&m->ez, 0, sizeof(m->ez));
     if (c.efficientzero) {
         EzNet &e = m->ez;
@@ -1209,32 +878,25 @@ int lz_model_finalize(lz_model *m)
 
     // DownSample geometry: conv s2 p1: h -> (h-1)/2+1
     const int h0 = c.obs_h, h1 = (h0 - 1) / 2 + 1, h2 = (h1 - 1) / 2 + 1, h3 = (h2 - 1) / 2 + 1;
-    struct G { int stride, hin, hout; };
-    const G geo[10] = {{2, h0, h1}, {1, h1, h1}, {1, h1, h1}, {2, h1, h2}, {2, h1, h2}, {1, h2, h2},
-                       {1, h2, h2}, {1, h2, h2}, {1, h3, h3}, {1, h3, h3}};
-    m->tower.clear();
-    for (int i = 0; i < 10; ++i) {
-        ConvG L;
-        L.w = base + tower[i].w; L.scale = base + tower[i].scale; L.shift = base + tower[i].shift;
-        L.cin = tower[i].cin; L.cout = tower[i].cout; L.stride = geo[i].stride;
-        L.hin = L.win = geo[i].hin; L.hout = L.wout = geo[i].hout;
-        m->tower.push_back(L);
-    }
+    ConvG &S0 = m->stem;
+    S0.w = base + stem.w; S0.scale = base + stem.scale; S0.shift = base + stem.shift;
+    S0.cin = stem.cin; S0.cout = stem.cout;
+    S0.hin = S0.win = h0; S0.hout = S0.wout = h1;
     // host copy of the stem's weights / folded BatchNorm for k_stem4_tcl (kernel-parameter operands)
     m->stem_valid = 0;
-    if (tower[0].cin == 4 && tower[0].cout == 32 && h0 % 4 == 0 && (h0 / 2) <= 256) {
+    if (stem.cin == 4 && stem.cout == 32 && h0 % 4 == 0 && (h0 / 2) <= 256) {
         m->stem_params.assign(sizeof(StemP) / sizeof(float), 0.0f);
         StemP &SP = *reinterpret_cast<StemP *>(m->stem_params.data());
-        memcpy(SP.w, P.host.data() + tower[0].w, sizeof(SP.w));
-        memcpy(SP.scale, P.host.data() + tower[0].scale, sizeof(SP.scale));
-        memcpy(SP.shift, P.host.data() + tower[0].shift, sizeof(SP.shift));
+        memcpy(SP.w, P.host.data() + stem.w, sizeof(SP.w));
+        memcpy(SP.scale, P.host.data() + stem.scale, sizeof(SP.scale));
+        memcpy(SP.shift, P.host.data() + stem.shift, sizeof(SP.shift));
         m->stem_valid = 1;
     }
     const int h4 = (h3 - 1) / 2 + 1, grid = h0 == 64 ? h3 : h4;      // 64 px: no pooling2
     LZ_REQUIRE(grid == m->hw && (grid == 6 || grid == 8), LZ_EINVAL, "lz_model_finalize: latent grid %d is neither 6 nor 8", grid);
     rc = model_prepare_launch();
     if (rc != LZ_OK) return rc;
-    rc = pack_tc(m, net);
+    rc = pack_tc(m, mkh(hr), mkh(hv), mkh(hp));
     if (rc != LZ_OK) return rc;
     rc = pack_tower_tc(m);
     if (rc != LZ_OK) return rc;
@@ -1245,14 +907,12 @@ int lz_model_finalize(lz_model *m)
 
 int lz_model_set_math(lz_model *m, int mode)
 {
-    LZ_REQUIRE(m && mode >= 0 && mode <= 2, LZ_EINVAL, "lz_model_set_math: mode must be 0 (fp32 FFMA), 1 (tensor-core 3xFP16) or 2 (tensor-core fp16)");
-    LZ_REQUIRE(m->kind == 0 || mode == 0, LZ_EINVAL, "lz_model_set_math: the MLP model only has the fp32 path");
-    LZ_REQUIRE(!(m->kind == 0 && m->cfg.efficientzero && mode == 0), LZ_EINVAL, "lz_model_set_math: the EfficientZero model runs its conv stack on the tensor-core path only (mode 1 or 2)");
-    LZ_REQUIRE(!(m->kind == 0 && m->hw != kHW && mode == 0), LZ_EINVAL,
-               "lz_model_set_math: the fp32 FFMA path runs the 6x6 latent grid only; this %dx%d-observation model (%dx%d latent) runs on the tensor-core path (mode 1 or 2)",
-               m->cfg.obs_h, m->cfg.obs_w, m->hw, m->hw);
-    if (m->math != mode) ++m->generation;      // captured search graphs bake the path (and pass count) in
-    m->math = mode;
+    LZ_REQUIRE(m && (mode == 1 || mode == 2), LZ_EINVAL,
+               "lz_model_set_math: mode must be 1 (tc3: tensor-core fp16 hi/lo, fp32-accurate) or 2 (tc1: tensor-core single fp16 pass)");
+    LZ_REQUIRE(m->kind == 0, LZ_EINVAL, "lz_model_set_math: the MLP model has no math mode");
+    const int npass = mode == 1 ? 3 : 1;
+    if (m->npass != npass) ++m->generation;      // captured search graphs bake the pass count in
+    m->npass = npass;
     return LZ_OK;
 }
 
@@ -1300,7 +960,6 @@ int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uin
     LZ_REQUIRE(m && B > 0 && (d_obs == nullptr) != (d_obs_u8 == nullptr) && d_out && h_info && stage >= 0 && stage <= 8, LZ_EINVAL,
                "lz_model_debug_tower_stage: bad argument");
     LZ_REQUIRE(m->finalized && m->kind == 0, LZ_ESTATE, "lz_model_debug_tower_stage: not a finalized conv model with a tensor-core tower");
-    LZ_REQUIRE(m->math != 0, LZ_ESTATE, "lz_model_debug_tower_stage: math mode 0 does not run the tensor-core tower");
     if (B > m->ws_B) {
         int rc = model_reserve(m, B);
         if (rc != LZ_OK) return rc;
@@ -1319,7 +978,7 @@ int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uin
         bytes = (size_t)B * m->latent_floats * sizeof(float);
     }
     LZ_REQUIRE(out_bytes >= bytes, LZ_EINVAL, "lz_model_debug_tower_stage: stage %d needs %zu bytes, got %zu", stage, bytes, out_bytes);
-    const ConvG &S0 = m->tower[0];
+    const ConvG &S0 = m->stem;
     auto pool_ctas = [&](const Tcl &in, int hout) {
         return (int)std::min<size_t>(((size_t)B * (in.C / 8) * hout * hout + 255) / 256, kNumSMs * 32);
     };
@@ -1350,7 +1009,7 @@ int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uin
         case 7: rb_plan(m->tower_rb[2]); break;
         default: info[5] = 1; info[8] = m->hw == 8 ? tcl_to_nchw_ctas(m->V1, B) : pool_ctas(m->V1, m->hw); break;
     }
-    info[9] = (m->math == 1) ? 3 : 1;
+    info[9] = m->npass;
     const cudaStream_t st = (cudaStream_t)s;
     int rc = tower_tc_run(m, B, d_obs, stage == 8 ? reinterpret_cast<float *>(d_out) : nullptr, st, d_obs_u8, stage);
     if (rc != LZ_OK) return rc;
@@ -1364,7 +1023,7 @@ int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_laten
 {
     LZ_REQUIRE(m && (which == 0 || which == 1) && B > 0 && d_latent && (which == 1 || d_action) && d_out && h_info && stage >= 0,
                LZ_EINVAL, "lz_model_debug_net_stage: bad argument");
-    LZ_REQUIRE(m->finalized && m->kind == 0 && m->math != 0, LZ_ESTATE, "lz_model_debug_net_stage: not a finalized conv model on the tensor-core path");
+    LZ_REQUIRE(m->finalized && m->kind == 0, LZ_ESTATE, "lz_model_debug_net_stage: not a finalized conv model");
     TcNet net = which ? m->tc_tail : m->tc_rec;          // a copy: the model's programs stay as they are
     const int nl = net.nlayers, K = m->K, A = m->cfg.action_space_size;
     const bool ez = m->cfg.efficientzero != 0 && which == 0;
@@ -1381,7 +1040,7 @@ int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_laten
     float *o = reinterpret_cast<float *>(d_out);
     TcIO t;
     memset(&t, 0, sizeof(t));
-    t.B = B; t.npass = (m->math == 1) ? 3 : 1;
+    t.B = B; t.npass = m->npass;
     t.latent_base = d_latent; t.action = which ? nullptr : d_action;
     t.skip_scratch = m->tc_skip;
     t.ez_feat = ez ? m->ez_feat : nullptr;

@@ -14,21 +14,10 @@ namespace lz {
 
 constexpr int kMaxResBlocks = 4;
 
-struct NetDev {                       // passed by value to kernels
-    Conv3 dyn_conv;                   // dynamics_network.conv (+ norm_common)
-    Conv3 dyn_res[2 * kMaxResBlocks]; // dynamics_network.resblocks
-    Conv3 pred_res[2 * kMaxResBlocks];
-    Conv3 rep_res[2 * kMaxResBlocks]; // representation_network.resblocks (on the latent grid)
-    Head reward, value, policy;
-    int nres;
-    int A;
-    float support_min, support_step;
-};
-
-struct ConvG {                        // generic 3x3 conv of the DownSample tower
+struct ConvG {                        // DownSample stem (conv1 + norm1 + ReLU, 3x3 stride 2) of any input channel count
     const float *w;                   // [cin][9][cout]
     const float *scale, *shift;       // [cout]
-    int cin, cout, stride, hin, win, hout, wout;
+    int cin, cout, hin, win, hout, wout;
 };
 
 struct Dense {                        // y = act(scale * (W x) + shift); wt is input-major [in][out]
@@ -89,12 +78,11 @@ struct lz_model {
     bool finalized;
     float *d_weights;                 // one packed device allocation
     size_t n_weight_floats;
-    lz::NetDev net;
-    std::vector<lz::ConvG> tower;     // DownSample convs in execution order
+    lz::ConvG stem;                   // DownSample conv1 + norm1 (fp32 tables in d_weights)
     std::vector<float> stem_params;   // host copy of the Cin = 4 stem's weights + folded BN (kernel-parameter operands of k_stem4_tcl, model.cu)
     int stem_valid;
     int hw, P, K;
-    int math;                         // 0 = fp32 FFMA (net6.cuh), 1 = tensor-core 3xFP16 (fp32-accurate), 2 = tensor-core fp16 single pass
+    int npass;                        // MMA passes per product of the tensor-core kernels: 3 = tc3 (fp16 hi/lo, fp32-accurate), 1 = tc1
     unsigned char *d_tc;              // packed fp16 hi/lo weights + tables of the tensor-core path
     lz::TcNet tc_rec, tc_tail;
     float *tc_skip;                   // [tc_skip_B][64 P] ResBlock skip scratch of k_net_tc for launches outside a search (model_reserve)
@@ -107,11 +95,10 @@ struct lz_model {
     size_t tws_bytes;
     lz::Tcl T0, T1, U0, U1, U2, V0, V1;
     // workspace for initial inference (grown on demand, outside graph capture)
-    float *ws[3];
-    size_t ws_floats;
+    float *pre_latent;                // [ws_B][latent_floats] DownSample output, input of the latent-grid tail
     int ws_B;
     unsigned long long generation;    // bumped when device tables / workspaces that captured search graphs point into are re-allocated
-                                      // or the math mode changes (finalize, set_math, model_reserve): lz_search re-captures
+                                      // or the pass count changes (finalize, set_math, model_reserve): lz_search re-captures
 };
 
 namespace lz {

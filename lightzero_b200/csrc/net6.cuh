@@ -1,20 +1,6 @@
-// net6.cuh -- fp32 SIMT building blocks for the MuZero networks on the small latent grid (6x6 for
-// 84/96-pixel observations): 3x3 convolution with folded eval-BatchNorm / residual / ReLU epilogue,
-// 1x1-conv heads, the two fully connected layers of each head, and the fused
-// softmax-expectation + inverse scalar transform.
-//
-// Replaces the eager PyTorch graph of lzero/model/muzero_model.py:505-538 (DynamicsNetwork.forward),
-// lzero/model/common.py:1189-1215 (PredictionNetwork.forward), DI-engine ResBlock (res_type basic)
-// and lzero/policy/scaling_transform.py:82-92.
-//
-// Mapping: ONE WARP OWNS ONE ROOT.  The root's activations [C=64][P=36] fp32 live in shared memory
-// for the whole network (two 9 KB ping-pong buffers per root); lane l computes output channels
-// {2l, 2l+1} for all 36 pixels (72 accumulators in registers).  Per input channel the warp
-// broadcast-loads the 36 inputs (9 x LDS.128) and each lane loads its 9x2 weights (9 x LDS.64,
-// conflict free) for 512 FFMA: the loop is FMA-issue bound, not shared-memory bound.  Image borders
-// are resolved at COMPILE time (the 6x6x3x3 tap loops are fully unrolled and out-of-range taps
-// vanish), so there is no padding and no bounds test in the inner loop.  Weights are streamed
-// through a double-buffered cp.async stage shared by all warps of the CTA (packed [cin][tap][cout]).
+// net6.cuh -- constants of the latent grid, the fp32 head tables the tensor-core kernels read, and the canonical fused
+// softmax-expectation + inverse scalar transform (lzero/policy/scaling_transform.py:82-92) shared by every kernel that turns
+// categorical logits into a scalar (k_net_tc, mlp.cu, ez.cu, k_inverse_scalar).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -24,154 +10,12 @@ namespace lz {
 constexpr int kC = 64;          // latent channels (num_channels)
 constexpr int kHW = 6;          // latent height == width
 constexpr int kP = kHW * kHW;   // 36 pixels
-constexpr int kCC = 8;          // input channels per weight stage
-constexpr int kStageFloats = kCC * 9 * kC;   // 4608 floats = 18 KB
 
-struct Conv3 {                  // 3x3, stride 1, pad 1, cout = 64
-    const float *w;             // [cin][9][64]
-    const float *scale, *shift; // folded BatchNorm, [64]
-    int cin;                    // 64 (+A action planes for the dynamics conv; handled as a bias)
+struct Head {                   // fp32 tables of conv1x1 -> BN -> ReLU -> Linear(hc*P->hid) -> BN1d -> ReLU -> Linear(hid->K)
+    const float *s2, *t2;       // [hid]  BN1d folded, Linear bias folded into t2
+    const float *b2;            // [K]    bias of the last Linear
+    int hc, hid, K;             // hid == 0: no FC part on the tensor cores (EfficientZero's reward head, ez.cu)
 };
-
-struct Head {                   // conv1x1(64->hc)+BN+ReLU -> flatten -> Linear(hc*P->hid)+BN1d+ReLU -> Linear(hid->K)
-    const float *w1;            // [hc][64]
-    const float *s1, *t1;       // [hc]   (conv bias folded into t1)
-    const float *fc1;           // [hc*P][hid]  (input-major, hid contiguous)
-    const float *s2, *t2;       // [hid]  (Linear bias folded into t2)
-    const float *fc2;           // [hid][K]     (K contiguous)
-    const float *b2;            // [K]
-    int hc, hid, K;
-};
-
-__device__ __forceinline__ void cp_async16(void *smem, const void *gmem)
-{
-    unsigned sa = (unsigned)__cvta_generic_to_shared(smem);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(sa), "l"(gmem));
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
-
-// CTA-cooperative copy of `nfloats` (multiple of 4, 16 B aligned) global -> shared with cp.async.
-__device__ __forceinline__ void stage_async(float *dst, const float *src, int nfloats)
-{
-    for (int i = threadIdx.x * 4; i < nfloats; i += blockDim.x * 4) cp_async16(dst + i, src + i);
-}
-
-// acc[p][j] += sum over taps of in[...] * w[tap][2*lane+j] for one input channel.
-__device__ __forceinline__ void conv_channel_fma(float (&acc)[kP][2], const float *in_c, const float *w_c, int lane)
-{
-    float in[kP];
-#pragma unroll
-    for (int i = 0; i < kP / 4; ++i) {
-        float4 v = reinterpret_cast<const float4 *>(in_c)[i];
-        in[4 * i + 0] = v.x; in[4 * i + 1] = v.y; in[4 * i + 2] = v.z; in[4 * i + 3] = v.w;
-    }
-#pragma unroll
-    for (int ky = 0; ky < 3; ++ky) {
-#pragma unroll
-        for (int kx = 0; kx < 3; ++kx) {
-            const float2 w = *reinterpret_cast<const float2 *>(w_c + (ky * 3 + kx) * kC + 2 * lane);
-#pragma unroll
-            for (int y = 0; y < kHW; ++y) {
-                const int yy = y + ky - 1;
-                if (yy < 0 || yy >= kHW) continue;
-#pragma unroll
-                for (int x = 0; x < kHW; ++x) {
-                    const int xx = x + kx - 1;
-                    if (xx < 0 || xx >= kHW) continue;
-                    acc[y * kHW + x][0] = fmaf(in[yy * kHW + xx], w.x, acc[y * kHW + x][0]);
-                    acc[y * kHW + x][1] = fmaf(in[yy * kHW + xx], w.y, acc[y * kHW + x][1]);
-                }
-            }
-        }
-    }
-}
-
-// The one-hot action planes of the dynamics conv (muzero_model.py:341-369) are constant-1 planes:
-// their contribution is the border-aware sum of the 9 taps of weight row (64 + action).
-__device__ __forceinline__ void conv_action_bias(float (&acc)[kP][2], const float *w_row /*[9][64] global*/, int lane)
-{
-#pragma unroll
-    for (int ky = 0; ky < 3; ++ky) {
-#pragma unroll
-        for (int kx = 0; kx < 3; ++kx) {
-            const float2 w = __ldg(reinterpret_cast<const float2 *>(w_row + (ky * 3 + kx) * kC + 2 * lane));
-#pragma unroll
-            for (int y = 0; y < kHW; ++y) {
-                const int yy = y + ky - 1;
-                if (yy < 0 || yy >= kHW) continue;
-#pragma unroll
-                for (int x = 0; x < kHW; ++x) {
-                    const int xx = x + kx - 1;
-                    if (xx < 0 || xx >= kHW) continue;
-                    acc[y * kHW + x][0] += w.x;
-                    acc[y * kHW + x][1] += w.y;
-                }
-            }
-        }
-    }
-}
-
-// Full 3x3 conv layer for the calling warp's root.  All warps of the CTA must call this together
-// (weight staging + __syncthreads).  in/out/res: this warp's [64][36] shared buffers.
-//   out = relu( scale * (conv(in) [+ action bias]) + shift [+ res] )
-// `out` may alias `res` (each lane only re-reads the elements it overwrites) but not `in`.
-__device__ __forceinline__ void conv3x3_layer(const Conv3 &L, const float *in, float *out, const float *res,
-                                              int action /* -1: none */, float *wstage /*[2][kStageFloats]*/,
-                                              int lane)
-{
-    float acc[kP][2];
-#pragma unroll
-    for (int p = 0; p < kP; ++p) { acc[p][0] = 0.0f; acc[p][1] = 0.0f; }
-
-    constexpr int nchunks = kC / kCC;
-    stage_async(wstage, L.w, kStageFloats);
-    cp_async_commit();
-    if (action >= 0) conv_action_bias(acc, L.w + (size_t)(kC + action) * 9 * kC, lane);
-    for (int ch = 0; ch < nchunks; ++ch) {
-        if (ch + 1 < nchunks) {
-            stage_async(wstage + ((ch + 1) & 1) * kStageFloats, L.w + (size_t)(ch + 1) * kStageFloats, kStageFloats);
-            cp_async_commit();
-            cp_async_wait<1>();
-        } else {
-            cp_async_wait<0>();
-        }
-        __syncthreads();
-        const float *ws = wstage + (ch & 1) * kStageFloats;
-#pragma unroll 1
-        for (int cl = 0; cl < kCC; ++cl)
-            conv_channel_fma(acc, in + (ch * kCC + cl) * kP, ws + cl * 9 * kC, lane);
-        __syncthreads();   // everyone done with this stage buffer before it is refilled
-    }
-    const float2 sc = __ldg(reinterpret_cast<const float2 *>(L.scale + 2 * lane));
-    const float2 sh = __ldg(reinterpret_cast<const float2 *>(L.shift + 2 * lane));
-    __syncwarp();
-#pragma unroll
-    for (int p = 0; p < kP; ++p) {
-        float v0 = fmaf(acc[p][0], sc.x, sh.x), v1 = fmaf(acc[p][1], sc.y, sh.y);
-        if (res) { v0 += res[(2 * lane) * kP + p]; v1 += res[(2 * lane + 1) * kP + p]; }
-        out[(2 * lane) * kP + p] = fmaxf(v0, 0.0f);
-        out[(2 * lane + 1) * kP + p] = fmaxf(v1, 0.0f);
-    }
-    __syncwarp();
-}
-
-// conv1x1(64->hc) + BN + ReLU, flattened NCHW (index = hc_i * 36 + p) into hflat[hc*36] (shared).
-__device__ __forceinline__ void head_conv1x1(const Head &H, const float *x /*[64][36] shared*/, float *hflat, int lane)
-{
-    const int total = H.hc * kP;
-    for (int o = lane; o < total; o += 32) {
-        const int hc_i = o / kP, p = o - hc_i * kP;
-        const float *w = H.w1 + hc_i * kC;
-        float a = 0.0f;
-#pragma unroll 8
-        for (int c = 0; c < kC; ++c) a = fmaf(x[c * kP + p], __ldg(w + c), a);
-        a = fmaf(a, __ldg(H.s1 + hc_i), __ldg(H.t1 + hc_i));
-        hflat[o] = fmaxf(a, 0.0f);
-    }
-    __syncwarp();
-}
 
 // torch.sign(v) * (((sqrt(1 + 4 eps (|v| + 1 + eps)) - 1) / (2 eps))^2 - 1), eps = 0.001, evaluated
 // in fp32 in the operation order of scaling_transform.py:89-91.
@@ -243,49 +87,6 @@ __device__ __forceinline__ float categorical_to_scalar(const float *logits /*sha
         W += warp_sum(w[j] * sc);
     }
     return inverse_scalar_transform(W / S);
-}
-
-// Fully connected part of one head for NR roots at once by the calling warp (weights are read once
-// per CTA instead of once per root).  hflat: [NR][stride_h] shared; hidden scratch: [NR][32] shared;
-// logits_out: [NR][K] shared scratch (or nullptr when K <= 32 and the caller wants registers).
-template <int NR>
-__device__ __forceinline__ void head_fc(const Head &H, const float *hflat, int stride_h, float *hidden /*[NR][32]*/,
-                                        float *logits /*[NR][Kpad]*/, int Kpad, int lane)
-{
-    // fc1: lane <-> hidden unit (hid <= 32)
-    float a[NR];
-#pragma unroll
-    for (int r = 0; r < NR; ++r) a[r] = 0.0f;
-    const int nin = H.hc * kP;
-    if (lane < H.hid) {
-        for (int i = 0; i < nin; ++i) {
-            const float w = __ldg(H.fc1 + (size_t)i * H.hid + lane);
-#pragma unroll
-            for (int r = 0; r < NR; ++r) a[r] = fmaf(hflat[r * stride_h + i], w, a[r]);
-        }
-        const float s = __ldg(H.s2 + lane), t = __ldg(H.t2 + lane);
-#pragma unroll
-        for (int r = 0; r < NR; ++r) hidden[r * 32 + lane] = fmaxf(fmaf(a[r], s, t), 0.0f);
-    }
-    __syncwarp();
-    // fc2: lanes stride over the K outputs
-    for (int k0 = 0; k0 < H.K; k0 += 32) {
-        const int k = k0 + lane;
-        float o[NR];
-        const float bias = k < H.K ? __ldg(H.b2 + k) : 0.0f;
-#pragma unroll
-        for (int r = 0; r < NR; ++r) o[r] = bias;
-        if (k < H.K) {
-            for (int j = 0; j < H.hid; ++j) {
-                const float w = __ldg(H.fc2 + (size_t)j * H.K + k);
-#pragma unroll
-                for (int r = 0; r < NR; ++r) o[r] = fmaf(hidden[r * 32 + j], w, o[r]);
-            }
-#pragma unroll
-            for (int r = 0; r < NR; ++r) logits[r * Kpad + k] = o[r];
-        }
-    }
-    __syncwarp();
 }
 
 }  // namespace lz

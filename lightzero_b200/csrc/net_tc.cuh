@@ -24,7 +24,7 @@ struct TcNet {
     const unsigned char *fcw;      // FC weight stream: 16 P / 32 FC1 stages of 12 KB ([2 k-steps][hi 3 KB | lo 3 KB], [kg 2][96 rows = 32 head + unit][8]) then the FC2 tiles
     TcFc fc[3];                    // reward, value, policy
     int hw;                        // latent grid hw x hw: 6 (84 / 96-pixel observations) or 8 (64): selects the k_net_tc instantiation
-    Head reward, value, policy;    // folded BN / bias tables of the FC parts (fp32, same tables as the SIMT path)
+    Head reward, value, policy;    // folded BN / bias tables of the FC parts (fp32, in lz_model::d_weights)
     int hc[3];
     int nlayers;
     int layer_w[kTcMaxLayers];     // conv index into convw / bn

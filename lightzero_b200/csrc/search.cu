@@ -80,14 +80,14 @@ static RecIO rec_io(const lz_search *q, int sim)
 // EfficientZero stays a multi-kernel graph: its LSTM step is a GEMM over all roots (several launches per simulation).
 static bool persistent_search(const lz_search *q, bool reuse)
 {
-    return !reuse && !q->tree->gumbel && !q->hpool && q->model->kind == 0 && q->model->math != 0 && q->tree->p.A <= 32;   // tree_persist.cuh: one lane per child
+    return !reuse && !q->tree->gumbel && !q->hpool && q->model->kind == 0 && q->tree->p.A <= 32;   // tree_persist.cuh: one lane per child
 }
 
 static TcIO persistent_io(const lz_search *q, int deterministic)
 {
     TcIO io;
     memset(&io, 0, sizeof(io));
-    io.B = q->B; io.npass = (q->model->math == 1) ? 3 : 1;
+    io.B = q->B; io.npass = q->model->npass;
     io.latent_base = q->pool; io.latent_pool_rw = q->pool; io.slot_stride = q->slot_stride;
     io.ix = q->d_ix; io.ix_rw = q->d_ix; io.action = q->d_action; io.action_rw = q->d_action;
     io.reward = q->d_reward; io.value = q->d_value; io.policy_logits = q->d_policy;
@@ -154,7 +154,7 @@ static int run_graph(lz_search *q, int deterministic, bool reuse, cudaStream_t s
 {
     // an EfficientZero plain search breaks ties by p.tie_first (tracked by the tree generation), not by the flag: one graph
     SearchGraph &g = q->graphs[q->tree->gumbel ? 3 : reuse ? 2 : (deterministic || q->hpool) ? 1 : 0];
-    // a captured graph bakes in device pointers of the model's tables (passed by value in TcNet / NetDev / EzNet), the math mode
+    // a captured graph bakes in device pointers of the model's tables (passed by value in TcNet / EzNet), the pass count
     // and the tree parameters (TreeParams by value): re-capture when any of them changed since (weight reload, set_math,
     // model_reserve growth, lz_tree_set_params / lz_tree_set_ez / lz_tree_set_tiebreak)
     if (g.exec && (g.gen_model != q->model->generation || g.gen_tree != q->tree->generation)) {
@@ -365,7 +365,7 @@ static int collect_device(lz_search *q, const float *d_obs, const uint8_t *d_obs
     io.value = d_pred_value ? d_pred_value : q->d_root_value;
     int rc;
     if (d_obs_u8) {
-        LZ_REQUIRE(q->model->kind == 0 && q->model->math != 0, LZ_EINVAL, "lz_search_collect_u8: uint8 frames need the tensor-core conv model");
+        LZ_REQUIRE(q->model->kind == 0, LZ_EINVAL, "lz_search_collect_u8: uint8 frames need the conv model");
         if (!q->d_pre_stage && (rc = dev_alloc(&q->d_pre_stage, (size_t)q->B * q->model->latent_floats))) return rc;
         rc = model_initial_tower(q->model, q->B, nullptr, q->d_pre_stage, (cudaStream_t)s, d_obs_u8);
         if (rc == LZ_OK) rc = model_initial_tail(q->model, q->B, q->d_pre_stage, io, (cudaStream_t)s);
@@ -393,8 +393,7 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
                         float *d_policy_logits, lz_stream s_)
 {
     LZ_REQUIRE(q && h_obs, LZ_EINVAL, "lz_search_collect_host: bad argument");
-    LZ_REQUIRE(!obs_u8 || (q->model->kind == 0 && q->model->math != 0), LZ_EINVAL,
-               "lz_search_collect_host_u8: uint8 frames need the tensor-core conv model");
+    LZ_REQUIRE(!obs_u8 || q->model->kind == 0, LZ_EINVAL, "lz_search_collect_host_u8: uint8 frames need the conv model");
     const size_t esz = obs_u8 ? 1 : sizeof(float);         // bytes per observation element on the wire and in the staging buffer
     cudaStream_t s = (cudaStream_t)s_;
     const lz_model_config &c = q->model->cfg;
@@ -433,7 +432,7 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
     if (h_to_play) LZ_CUDA_CHECK(cudaMemcpyAsync(q->d_tp_stage, h_to_play, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     float *logits = d_policy_logits ? d_policy_logits : q->d_root_logits;
     float *pred = d_pred_value ? d_pred_value : q->d_root_value;
-    const bool split = q->model->kind == 0 && q->model->math != 0;   // tower per chunk, tail once
+    const bool split = q->model->kind == 0;   // tower per chunk, tail once
     for (int i = 0; i < nchunks; ++i) {
         const int b0 = i * per, bc = std::min(per, B - b0);
         LZ_CUDA_CHECK(cudaStreamWaitEvent(s, q->ev_chunk[i], 0));

@@ -97,11 +97,12 @@ class MuZeroModel:
     def from_state_dict(cls, state_dict, **cfg):
         return cls(**cfg).load_state_dict(state_dict)
 
-    MATH_MODES = {"fp32": 0, "tc3": 1, "tc1": 2}
+    MATH_MODES = {"tc3": 1, "tc1": 2}
 
     def set_math(self, mode):
-        """'fp32' = FFMA on CUDA cores (6x6 latent grid only: 84/96-pixel observations), 'tc3' = wgmma 3xFP16
-        (fp32-accurate, the default), 'tc1' = wgmma single fp16 pass."""
+        """'tc3' = wgmma 3xFP16 (fp32-accurate, the default), 'tc1' = wgmma single fp16 pass."""
+        if isinstance(mode, str) and mode not in self.MATH_MODES:
+            raise ValueError(f"set_math: unknown mode {mode!r}: the conv models run tc3 or tc1")
         code = self.MATH_MODES[mode] if isinstance(mode, str) else int(mode)
         cabi.check(self._lib.lz_model_set_math(self._h, code), "lz_model_set_math")
         self.math = code

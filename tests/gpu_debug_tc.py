@@ -1,5 +1,5 @@
 """Bring-up diagnostics for the tensor-core (wgmma) path (run on the GPU box; not a pytest).  Single-layer
-programs first (localise descriptor / epilogue bugs), then the full network against fp32 FFMA and
+programs first (localise descriptor / epilogue bugs), then the full network in tc3 and tc1 against
 the PyTorch oracle."""
 import ctypes
 import os
@@ -67,7 +67,7 @@ def main():
     cu2 = lzb.MuZeroModel(observation_shape=(4, 84, 84), action_space_size=A).load_state_dict(ref.state_dict())
     with torch.no_grad():
         exp = ref.recurrent_inference(latent, action)
-    for mode in ("fp32", "tc3", "tc1"):
+    for mode in ("tc3", "tc1"):
         cu2.set_math(mode)
         out = cu2.recurrent_inference(latent.cuda(), action.cuda(), return_scalars=True)
         torch.cuda.synchronize()
@@ -79,7 +79,7 @@ def main():
     obs = torch.rand(B, 4, 84, 84, generator=g)
     with torch.no_grad():
         e0 = ref.initial_inference(obs)
-    for mode in ("fp32", "tc3"):
+    for mode in ("tc3", "tc1"):
         cu2.set_math(mode)
         o = cu2.initial_inference(obs.cuda())
         torch.cuda.synchronize()
@@ -91,7 +91,7 @@ def main():
     Bb = 1024
     lat = torch.rand(Bb, 64, 6, 6).cuda()
     act = torch.randint(0, A, (Bb,)).cuda()
-    for mode in ("fp32", "tc3", "tc1"):
+    for mode in ("tc3", "tc1"):
         cu2.set_math(mode)
         for _ in range(3):
             cu2.recurrent_inference(lat, act)

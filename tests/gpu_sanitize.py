@@ -12,7 +12,7 @@ from oracle.model_ref import MuZeroModelRef, emulate_trained_, MuZeroModelMLPRef
 torch.manual_seed(0)
 A, B, S = 6, 9, 6
 ref = emulate_trained_(MuZeroModelRef((4, 84, 84), A), 0)
-for math in ("tc3", "fp32"):
+for math in ("tc3", "tc1"):
     cu = lzb.MuZeroModel(observation_shape=(4, 84, 84), action_space_size=A).load_state_dict(ref.state_dict()).set_math(math)
     pol = MuZeroCollectPolicy(cu, dict(num_simulations=S, deterministic=True, discount_factor=0.997))
     obs = torch.rand(B, 4, 84, 84)

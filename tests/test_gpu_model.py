@@ -108,13 +108,19 @@ def test_model_rejects_unsupported_configs():
     m = lzb.MuZeroModel()
     with pytest.raises(RuntimeError):
         m.initial_inference(torch.zeros(1, 4, 84, 84).cuda())
+    # the conv models run on the tensor cores only: tc3 (mode 1) or tc1 (mode 2)
+    with pytest.raises(ValueError, match="tc3"):
+        m.set_math("fp32")
+    from lightzero_b200 import cabi
+    with pytest.raises(cabi.LzError, match="tc3"):
+        m.set_math(0)                                               # mode 0 passed straight to lz_model_set_math
 
 
 # ------------------------------------------------------------------ tensor-core path (lz_model_set_math)
 @pytest.mark.parametrize("B,A", [(7, 6), (50, 18), (1000, 6), (1024, 18)])
 def test_tensor_core_3xfp16_recurrent_matches_oracle(B, A):
     """math='tc3': wgmma MMAs on fp16 hi/lo splits (3 passes), fp32 accumulation in registers -- must meet the
-    same 1e-5 bar as the fp32 FFMA path."""
+    1e-5 bar against the fp32 restatement."""
     ref, cu = _models(A, seed=4)
     cu.set_math("tc3")
     g = torch.Generator().manual_seed(B)

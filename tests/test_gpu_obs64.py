@@ -482,7 +482,7 @@ def test_frame_stack_collect_equals_float_frames():
 def test_refusals():
     import lightzero_b200 as lzb
     _, _, cu = make_models(A=6, seed=1)
-    with pytest.raises(Exception, match="6x6"):
+    with pytest.raises(Exception, match="tc3"):
         cu.set_math("fp32")
     cu.set_math("tc1")
     cu.set_math("tc3")

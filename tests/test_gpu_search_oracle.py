@@ -175,7 +175,7 @@ CASES = {
     "nres3_k21_a9_b5_s600_sto": (9, 5, 600, False, "2p", dict(nres=3, support=SUPPORT_SMALL), {}, None, (0, 1)),
     "nres4_a6_b140_sto_mixed": (6, 140, 40, False, "mixed", dict(nres=4), dict(noise=False, tie_root=True), None, (0, 0)),
     "a33_b40_sto_2p": (33, 40, 20, False, "2p", {}, {}, None, None),
-    "fp32_a6_b64_sto": (6, 64, 20, False, "1p", dict(math="fp32"), {}, None, None),
+    "tc1_a40_b64_sto": (40, 64, 20, False, "1p", dict(math="tc1"), {}, None, None),
 }
 
 

@@ -414,16 +414,16 @@ class _Recorder:
         return out
 
 
-@pytest.mark.parametrize("math", ["tc3", "fp32"])
-def test_recurrent_on_search_latents(math):
+@pytest.mark.parametrize("math,px", [pytest.param("tc3", 84, id="tc3"), pytest.param("tc3", 96, id="tc3_96px")])
+def test_recurrent_on_search_latents(math, px):
     """recurrent_inference on what a search feeds it: sparse post-ReLU latents, chained up to S steps deep, against float64.
     Latents and logits at 1e-5, scalars at 2e-4 (DESIGN.md 4.4)."""
     import lightzero_b200 as lzb
     from oracle.model_ref import DiscreteSupport, InverseScalarTransform
     B, A, S = 300, 18, 50
-    _, ref64, cu = _models((4, 84, 84), A=A, seed=31, math=math)
+    _, ref64, cu = _models((4, px, px), A=A, seed=31, math=math)
     rng = np.random.default_rng(0)
-    obs = torch.rand(B, 4, 84, 84, generator=torch.Generator().manual_seed(5)).cuda()
+    obs = torch.rand(B, 4, px, px, generator=torch.Generator().manual_seed(5)).cuda()
     out = cu.initial_inference(obs)
     legal = [list(range(A))] * B
     noises = [rng.dirichlet([0.3] * A).astype(np.float32).tolist() for _ in range(B)]
