@@ -498,12 +498,13 @@ def test_persistent_search_with_narrow_heads(B):
 
 
 # ------------------------------------------------------------------------------------------------ EfficientZero
-def lstm_bound(lstm, feat, h0, c0):
-    """float64 (h1, c1) of one nn.LSTM step and their error bounds: TAU * M on the gate pre-activations, carried through
-    sigmoid / tanh (Lipschitz 1/4 and 1), plus the error of the fast sigmoid / tanh"""
+def lstm_bound(lstm, feat, h0, c0, tau=TAU["lstm"], weights=None):
+    """float64 (h1, c1) of one nn.LSTM step and their error bounds: tau * M on the gate pre-activations, carried through
+    sigmoid / tanh (Lipschitz 1/4 and 1), plus the error of the fast sigmoid / tanh.  `weights`: (W_ih, W_hh) to use
+    instead of the module's (the bound is always taken on the module's)"""
     Wi, Wh, b = lstm.weight_ih_l0, lstm.weight_hh_l0, lstm.bias_ih_l0 + lstm.bias_hh_l0
-    z = feat @ Wi.T + h0 @ Wh.T + b
-    E = TAU["lstm"] * (feat.abs() @ Wi.abs().T + h0.abs() @ Wh.abs().T + lstm.bias_ih_l0.abs() + lstm.bias_hh_l0.abs()) + ALPHA
+    z = feat @ (weights[0] if weights else Wi).T + h0 @ (weights[1] if weights else Wh).T + b
+    E = tau * (feat.abs() @ Wi.abs().T + h0.abs() @ Wh.abs().T + lstm.bias_ih_l0.abs() + lstm.bias_hh_l0.abs()) + ALPHA
     zi, zf, zg, zo = z.chunk(4, 1)
     Ei, Ef, Eg, Eo = E.chunk(4, 1)
     i, f, g, o = torch.sigmoid(zi), torch.sigmoid(zf), torch.tanh(zg), torch.sigmoid(zo)
