@@ -1,8 +1,8 @@
 // conv_tc.cu -- generic wgmma 3x3 convolution for the DownSample tower (see conv_tc.cuh for the layout).
 // One CTA = one band of image rows (or G small whole images): bulk-copies the band (+halo) of every k-group plane into shared
 // memory once, then for each 128-row tile runs 9 taps x (Cin/16) k-steps x 3 fp16 hi/lo passes of wgmma (two warpgroups, 64 rows
-// each, accumulators in registers) with row-shifted descriptors; the taps stream through a ring once per tile (L2-resident, 4-16 KB
-// each).  The epilogue applies BN / residual / ReLU straight from the accumulator fragments and writes the next layer's TCL tensor
+// each, accumulators in registers) with row-shifted descriptors; the taps stream through a ring once per tile group (L2-resident,
+// 4-16 KB each; see tc_group).  The epilogue applies BN / residual / ReLU straight from the accumulator fragments and writes the next layer's TCL tensor
 // (already split into fp16 hi/lo).  k_resblock_tc runs both convs of a plain ResBlock the same way, with conv1's output kept in
 // shared memory.
 #include <math.h>
@@ -59,9 +59,76 @@ __device__ __forceinline__ void store_split2(unsigned char *hi_ptr, unsigned cha
     *reinterpret_cast<__half2 *>(lo_ptr) = __halves2half2(__float2half_rn(a - __half2float(ha)), __float2half_rn(b - __half2float(hb)));
 }
 
+// A conv's NT tiles run in groups of at most MT tiles, split evenly (5 tiles with MT = 4: 3 + 2): ng groups of `per` tiles, the
+// last one possibly shorter
+__host__ __device__ inline void tile_groups(int NT, int MT, int &ng, int &per)
+{
+    ng = (NT + MT - 1) / MT;
+    per = (NT + ng - 1) / ng;
+}
+
+// The MMAs of one tile group, tap-major: for each of the 9 taps (ring slots n0 .. n0 + 8, each fetched once per group and released
+// as soon as its wgmmas are done), every k-step of every tile of the group.  The warpgroup's 64-row slabs of the nt <= MT tiles
+// are independent accumulator chains, so the tensor pipe has nt chains to interleave instead of waiting on one chain's wgmma
+// latency, and each tap crosses the ring once per group rather than once per tile.  Each row's sums keep the tap -> k-step ->
+// pass order.  tap_a(tap) is tile 0's A descriptor at that tap; tile_ready(s) runs before tile s's first wgmma.
+// KS > 0: KS k-steps, unrolled (the ResBlocks, Cin = N).  KS = 0: nks k-steps in a rolled loop (k_conv_tc: fewer live descriptor
+// registers, no spill at N = 128, and its 84-px launch ran 457 -> 406 us on an H100 80GB HBM3 at 700 W).
+template <int N, int MT, int KS, typename TapA, typename TileReady>
+__device__ __forceinline__ void tc_group(float (&acc)[MT][N / 2], int nt, TapA tap_a, TileReady tile_ready, int nks, int npass,
+                                         uint32_t plane16, uint32_t a_lo16, uint64_t b_desc0, size_t tap_bytes, int nstages,
+                                         uint64_t *full, uint64_t *empty, int n0, int lane)
+{
+    const uint32_t b_lo16 = (uint32_t)N;                                  // the lo rows of a k-group, in 16-byte units
+#pragma unroll
+    for (int s = 0; s < MT; ++s)
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) acc[s][i] = 0.0f;
+    for (int tap = 0; tap < 9; ++tap) {
+        const int n = n0 + tap, st = n % nstages;
+        mbar_wait(&full[st], (n / nstages) & 1);
+        const uint64_t b0 = b_desc0 + (uint64_t)((st * tap_bytes) >> 4);
+        const uint64_t a0 = tap_a(tap);
+        auto kstep = [&](int ks) {
+#pragma unroll
+            for (int s = 0; s < MT; ++s) {
+                if (s >= nt) break;
+                if (tap == 0 && ks == 0) tile_ready(s);
+                const uint64_t as = a0 + s * 128 + ks * 2 * plane16;
+                wgmma_f16<N>(acc[s], as, b0 + ks * 4 * N);
+                if (npass == 3) {
+                    wgmma_f16<N>(acc[s], as, b0 + b_lo16 + ks * 4 * N);
+                    wgmma_f16<N>(acc[s], as + a_lo16, b0 + ks * 4 * N);
+                }
+            }
+        };
+        wg_fence();
+        if constexpr (KS > 0) {
+#pragma unroll
+            for (int ks = 0; ks < KS; ++ks) kstep(ks);
+        } else {
+#pragma unroll 1
+            for (int ks = 0; ks < nks; ++ks) kstep(ks);
+        }
+        wg_commit();
+        if (tap > 0) {
+            wg_wait<1>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[(n - 1) % nstages]);
+        }
+    }
+    wg_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[(n0 + 8) % nstages]);
+}
+
+// Tiles in flight per warpgroup (accumulator slabs of N / 2 registers each): one.  N = 64 stays within 112 registers, so two CTAs
+// share an SM and one CTA's band load and epilogue overlap the other's MMAs.  N = 128 runs one CTA per SM at the 168-register cap
+// of 288 threads; two slabs (128 accumulators) spill in the epilogue (CUDA 12.9).
 template <int N>
-// N = 64: <= 112 registers (32 accumulators per thread), so two CTAs can share an SM and overlap one CTA's band load / epilogue
-// with the other's MMAs; N = 128 needs 64 accumulators per thread and runs one CTA per SM
+constexpr int kCvTiles = 1;
+
+template <int N>
 __global__ void __launch_bounds__(kCvThreads, N == 128 ? 1 : 2) k_conv_tc(ConvTc p)
 {
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -76,7 +143,9 @@ __global__ void __launch_bounds__(kCvThreads, N == 128 ? 1 : 2) k_conv_tc(ConvTc
     const int img0 = group * p.G, nimg = min(p.G, p.B - img0);
     const int y0 = band * p.band_h;
     const int rin0 = y0 * pitch - 1;
-    const int npass = p.npass;
+    constexpr int MT = kCvTiles<N>;
+    int ng, per;
+    tile_groups(g.NT, MT, ng, per);
 
     if (tid == 0) {
         for (int i = 0; i < kCvStages; ++i) { mbar_init(&bars->full[i], 1); mbar_init(&bars->empty[i], kCvConsumers / 32); }
@@ -86,7 +155,7 @@ __global__ void __launch_bounds__(kCvThreads, N == 128 ? 1 : 2) k_conv_tc(ConvTc
     __syncthreads();
 
     if (warp == kCvConsumers / 32) {
-        // ================= producer: input band, then the 9 weight taps once per tile =================
+        // ================= producer: input band, then the 9 weight taps once per tile group =================
         if (lane == 0) {
             const int grow0 = rin0 + 1;                                    // memory row of rho = rin0
             const int ncopy = min(g.rin, p.in.plane_rows - grow0);
@@ -101,7 +170,7 @@ __global__ void __launch_bounds__(kCvThreads, N == 128 ? 1 : 2) k_conv_tc(ConvTc
                             unsigned char *dst = in_s + f * g.phase + part * g.part + kg * g.plane + (size_t)k * g.rin * 16;
                             bulk_g2s(dst, src, bytes, &bars->in_full);
                         }
-            for (int n = 0; n < 9 * g.NT; ++n) {
+            for (int n = 0; n < 9 * ng; ++n) {
                 const int st = n % nstages, tap = n % 9;
                 if (n >= nstages) mbar_wait(&bars->empty[st], ((n / nstages) - 1) & 1);
                 mbar_expect_tx(&bars->full[st], (uint32_t)g.tap_bytes);
@@ -116,44 +185,25 @@ __global__ void __launch_bounds__(kCvThreads, N == 128 ? 1 : 2) k_conv_tc(ConvTc
     const uint32_t plane16 = (uint32_t)(g.plane >> 4);
     const uint64_t a_desc0 = make_desc(smem_u32(in_s), plane16, 8);
     const uint64_t b_desc0 = make_desc(smem_u32(ring), 2 * N, 8);        // tap block [kg][N hi rows | N lo rows][16 B]: LBO = 2N rows
-    const uint32_t b_lo16 = (uint32_t)N;                                  // the lo rows of a k-group, in 16-byte units
     const uint32_t a_lo16 = (uint32_t)(g.part >> 4);
-    const int nks = kg_in / 2;
     const int yend = min(y0 + p.band_h, H);
     const int qc = 2 * (lane & 3);                                        // first of the thread's two columns in each 8-column group
     mbar_wait(&bars->in_full, 0);
-    for (int t = 0; t < g.NT; ++t) {
-        float acc[N / 2];
-#pragma unroll
-        for (int i = 0; i < N / 2; ++i) acc[i] = 0.0f;
-        for (int tap = 0; tap < 9; ++tap) {
-            const int n = t * 9 + tap, st = n % nstages;
-            mbar_wait(&bars->full[st], (n / nstages) & 1);
-            const uint64_t b0 = b_desc0 + (uint64_t)((st * g.tap_bytes) >> 4);
-            const uint64_t a0 = a_desc0 + (uint64_t)((p.tap_phase[tap] * g.phase) >> 4) + (uint64_t)(g.m_lo + p.tap_shift[tap] + t * 128 + wg * 64);
-            wg_fence();
-            for (int ks = 0; ks < nks; ++ks) {
-                wgmma_f16<N>(acc, a0 + ks * 2 * plane16, b0 + ks * 4 * N);
-                if (npass == 3) {
-                    wgmma_f16<N>(acc, a0 + ks * 2 * plane16, b0 + b_lo16 + ks * 4 * N);
-                    wgmma_f16<N>(acc, a0 + a_lo16 + ks * 2 * plane16, b0 + ks * 4 * N);
-                }
-            }
-            wg_commit();
-            if (tap > 0) {
-                wg_wait<1>();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&bars->empty[(n - 1) % nstages]);
-            }
-        }
-        wg_wait<0>();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars->empty[(t * 9 + 8) % nstages]);
+    for (int gi = 0; gi < ng; ++gi) {
+        const int t0 = gi * per, nt = min(per, g.NT - t0);
+        float acc[MT][N / 2];
+        auto tap_a = [&](int tap) {
+            return a_desc0 + (uint64_t)((p.tap_phase[tap] * g.phase) >> 4) + (uint64_t)(g.m_lo + p.tap_shift[tap] + t0 * 128 + wg * 64);
+        };
+        tc_group<N, MT, 0>(acc, nt, tap_a, [](int) {}, kg_in / 2, p.npass, plane16, a_lo16, b_desc0, g.tap_bytes, nstages, bars->full,
+                           bars->empty, gi * 9, lane);
 
         // ================= epilogue from the fragment: BN (+residual) (+ReLU) -> fp16 hi/lo -> next layer's TCL =================
 #pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-            const int m = g.m_lo + t * 128 + wg * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
+        for (int e = 0; e < 2 * MT; ++e) {
+            const int s = e >> 1, hr = e & 1;
+            if (s >= nt) break;
+            const int m = g.m_lo + (t0 + s) * 128 + wg * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
             const int k = m / g.rin;
             const int rho = rin0 + (m - k * g.rin);
             const int yy = rho / pitch - 1, xx = rho - (yy + 1) * pitch;
@@ -166,8 +216,8 @@ __global__ void __launch_bounds__(kCvThreads, N == 128 ? 1 : 2) k_conv_tc(ConvTc
                 const int c = col - grp * 64;                     // channel within the output tensor
                 const Tcl &o = p.out[grp];
                 const bool relu = p.relu[grp] != 0;
-                float v0 = fmaf(acc[4 * j + 2 * hr], __ldg(p.scale + col), __ldg(p.shift + col));
-                float v1 = fmaf(acc[4 * j + 2 * hr + 1], __ldg(p.scale + col + 1), __ldg(p.shift + col + 1));
+                float v0 = fmaf(acc[s][4 * j + 2 * hr], __ldg(p.scale + col), __ldg(p.shift + col));
+                float v1 = fmaf(acc[s][4 * j + 2 * hr + 1], __ldg(p.scale + col + 1), __ldg(p.shift + col + 1));
                 if (p.res.base && grp == 0 && valid) {
                     const unsigned char *rp = p.res.base + (size_t)(img0 + k) * p.res.img_stride +
                                               ((size_t)(c >> 3) * p.res.plane_rows + rho + 1) * 16 + (c & 7) * 2;
@@ -231,49 +281,12 @@ __host__ __device__ inline RbGeom rb_geom(const ResBlockTc &p)
     return g;
 }
 
-// Two 128-row tiles (the second only if `two`) of one conv: 9 taps x k-steps x passes of wgmma (ring slots n0 .. n0 + 8, released
-// as they are consumed).  The warpgroup's 64-row slabs of the two tiles accumulate into independent registers, interleaved per
-// k-step: one dependent accumulator chain per warpgroup leaves the tensor pipe waiting on wgmma latency (the fused kernel runs
-// one CTA per SM, so no second CTA fills those gaps).  Each row's sums keep the tap -> k-step -> pass order.
+// Tiles in flight per warpgroup: the accumulator slabs (N / 2 registers each) of a whole conv at N = 32 (84-px resblocks1: NT1 = 6,
+// NT2 = 5; 96 registers, 151 in all), two slabs at N = 64 (three or four spill in the epilogue at the 168-register cap of 288
+// threads, CUDA 12.9).  The kernel runs one CTA per SM (~200 KB of shared memory), so only independent chains within the CTA hide
+// wgmma latency.
 template <int N>
-__device__ __forceinline__ void rb_tiles(float (&acc)[2][N / 2], bool two, uint64_t a_desc0, int row0, const ResBlockTc &p,
-                                         const RbGeom &g, uint64_t b_desc0, RbBars *bars, int n0, int lane)
-{
-    const uint32_t plane16 = (uint32_t)(g.plane >> 4), a_lo16 = (uint32_t)(g.part >> 4), b_lo16 = (uint32_t)N;
-    const int nstages = p.stages;
-#pragma unroll
-    for (int s = 0; s < 2; ++s)
-#pragma unroll
-        for (int i = 0; i < N / 2; ++i) acc[s][i] = 0.0f;
-    for (int tap = 0; tap < 9; ++tap) {
-        const int n = n0 + tap, st = n % nstages;
-        mbar_wait(&bars->full[st], (n / nstages) & 1);
-        const uint64_t b0 = b_desc0 + (uint64_t)((st * g.tap_bytes) >> 4);
-        const uint64_t a0 = a_desc0 + (uint64_t)(row0 + p.tap_shift[tap]);
-        wg_fence();
-        for (int ks = 0; ks < N / 16; ++ks) {
-#pragma unroll
-            for (int s = 0; s < 2; ++s) {
-                if (s == 1 && !two) break;
-                const uint64_t as = a0 + s * 128 + ks * 2 * plane16;
-                wgmma_f16<N>(acc[s], as, b0 + ks * 4 * N);
-                if (p.npass == 3) {
-                    wgmma_f16<N>(acc[s], as, b0 + b_lo16 + ks * 4 * N);
-                    wgmma_f16<N>(acc[s], as + a_lo16, b0 + ks * 4 * N);
-                }
-            }
-        }
-        wg_commit();
-        if (tap > 0) {
-            wg_wait<1>();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&bars->empty[(n - 1) % nstages]);
-        }
-    }
-    wg_wait<0>();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bars->empty[(n0 + 8) % nstages]);
-}
+constexpr int kRbTiles = N == 32 ? 6 : 2;
 
 template <int N>
 __global__ void __launch_bounds__(kCvThreads, 1) k_resblock_tc(ResBlockTc p)
@@ -288,7 +301,11 @@ __global__ void __launch_bounds__(kCvThreads, 1) k_resblock_tc(ResBlockTc p)
     const int group = blockIdx.x / g.nbands, band = blockIdx.x - group * g.nbands;
     const int img0 = group * p.G, nimg = min(p.G, p.B - img0);
     const int y0 = band * p.band_h;
-    const int np1 = (g.NT1 + 1) / 2, ntaps = 9 * (np1 + (g.NT2 + 1) / 2);   // the taps stream once per pair of tiles
+    constexpr int MT = kRbTiles<N>;
+    int ng1, per1, ng2, per2;
+    tile_groups(g.NT1, MT, ng1, per1);
+    tile_groups(g.NT2, MT, ng2, per2);
+    const int ntaps = 9 * (ng1 + ng2);                                    // the taps stream once per tile group
 
     if (tid == 0) {
         for (int i = 0; i < kCvStages; ++i) { mbar_init(&bars->full[i], 1); mbar_init(&bars->empty[i], kCvConsumers / 32); }
@@ -304,7 +321,7 @@ __global__ void __launch_bounds__(kCvThreads, 1) k_resblock_tc(ResBlockTc p)
                 const int st = n % nstages, tap = n % 9;
                 if (n >= nstages) mbar_wait(&bars->empty[st], ((n / nstages) - 1) & 1);
                 mbar_expect_tx(&bars->full[st], (uint32_t)g.tap_bytes);
-                bulk_g2s(ring + st * g.tap_bytes, p.w[n >= 9 * np1] + (size_t)tap * g.tap_bytes, (uint32_t)g.tap_bytes, &bars->full[st]);
+                bulk_g2s(ring + st * g.tap_bytes, p.w[n >= 9 * ng1] + (size_t)tap * g.tap_bytes, (uint32_t)g.tap_bytes, &bars->full[st]);
             };
             for (int n = 0; n < nstages; ++n) load_tap(n);   // queued ahead of the band, so that conv1's first tile waits on its rows only
             // rows outside the tensor (above the first band, below the last) are not copied: they only feed conv1 rows outside
@@ -336,23 +353,30 @@ __global__ void __launch_bounds__(kCvThreads, 1) k_resblock_tc(ResBlockTc p)
     const uint32_t plane16 = (uint32_t)(g.plane >> 4);
     const uint64_t in_desc = make_desc(smem_u32(in_s), plane16, 8), mid_desc = make_desc(smem_u32(mid_s), plane16, 8);
     const uint64_t b_desc0 = make_desc(smem_u32(ring), 2 * N, 8);        // tap block [kg][N hi rows | N lo rows][16 B]: LBO = 2N rows
+    const uint32_t a_lo16 = (uint32_t)(g.part >> 4);
     const int qc = 2 * (lane & 3);                                        // first of the thread's two columns in each 8-column group
     // t1 row 0 (the pad column left of image 0's first halo row) is read by conv2 but is no conv1 output row
     if (tid < 2 * kg_in) *reinterpret_cast<uint4 *>(mid_s + tid * g.plane) = make_uint4(0u, 0u, 0u, 0u);
 
     // ================= conv1 -> BN -> ReLU -> t1 (shared memory) =================
     int ready = 0;                                                        // input chunks known to have landed
-    for (int t = 0; t < g.NT1; t += 2) {
-        const bool two = t + 1 < g.NT1;
-        const int need = min(g.nchunk, (t * 128 + 256 + 2 * pitch + 1) / 128 + 1);   // rows [128 t, 128 t + 256 + 2 pitch + 2)
-        for (; ready < need; ++ready) mbar_wait(&bars->chunk[ready], 0);
-        float acc[2][N / 2];
-        rb_tiles<N>(acc, two, in_desc, g.m_lo + t * 128 + wg * 64, p, g, b_desc0, bars, t / 2 * 9, lane);
+    for (int gi = 0; gi < ng1; ++gi) {
+        const int t0 = gi * per1, nt = min(per1, g.NT1 - t0);
+        float acc[MT][N / 2];
+        auto tap_a = [&](int tap) { return in_desc + (uint64_t)(g.m_lo + t0 * 128 + wg * 64 + p.tap_shift[tap]); };
+        // tile t reads rows [128 t, 128 t + 128 + 2 pitch + 2) over its 9 taps: in the first tap it waits for their chunks only,
+        // so its MMAs start while the rest of the band is still landing
+        auto tile_ready = [&](int s) {
+            const int need = min(g.nchunk, ((t0 + s) * 128 + 128 + 2 * pitch + 1) / 128 + 1);
+            for (; ready < need; ++ready) mbar_wait(&bars->chunk[ready], 0);
+        };
+        tc_group<N, MT, N / 16>(acc, nt, tap_a, tile_ready, N / 16, p.npass, plane16, a_lo16, b_desc0, g.tap_bytes, nstages, bars->full,
+                                bars->empty, gi * 9, lane);
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
+        for (int e = 0; e < 2 * MT; ++e) {
             const int s = e >> 1, hr = e & 1;
-            if (s == 1 && !two) break;
-            const int m = g.m_lo + (t + s) * 128 + wg * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
+            if (s >= nt) break;
+            const int m = g.m_lo + (t0 + s) * 128 + wg * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
             const int i = m - pitch;
             const int k = m / g.S;
             const int rho = (y0 - 1) * pitch - 1 + (m - k * g.S);
@@ -377,15 +401,17 @@ __global__ void __launch_bounds__(kCvThreads, 1) k_resblock_tc(ResBlockTc p)
 
     // ================= conv2 -> BN -> + x -> ReLU -> output TCL =================
     const int yend = min(y0 + p.band_h, H);
-    for (int t = 0; t < g.NT2; t += 2) {
-        const bool two = t + 1 < g.NT2;
-        float acc[2][N / 2];
-        rb_tiles<N>(acc, two, mid_desc, g.m_lo + t * 128 + wg * 64, p, g, b_desc0, bars, (np1 + t / 2) * 9, lane);
+    for (int gi = 0; gi < ng2; ++gi) {
+        const int t0 = gi * per2, nt = min(per2, g.NT2 - t0);
+        float acc[MT][N / 2];
+        auto tap_a = [&](int tap) { return mid_desc + (uint64_t)(g.m_lo + t0 * 128 + wg * 64 + p.tap_shift[tap]); };
+        tc_group<N, MT, N / 16>(acc, nt, tap_a, [](int) {}, N / 16, p.npass, plane16, a_lo16, b_desc0, g.tap_bytes, nstages, bars->full,
+                                bars->empty, (ng1 + gi) * 9, lane);
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
+        for (int e = 0; e < 2 * MT; ++e) {
             const int s = e >> 1, hr = e & 1;
-            if (s == 1 && !two) break;
-            const int m = g.m_lo + (t + s) * 128 + wg * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
+            if (s >= nt) break;
+            const int m = g.m_lo + (t0 + s) * 128 + wg * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
             const int k = m / g.S;
             const int rho = y0 * pitch - 1 + (m - k * g.S);
             const int yy = rho / pitch - 1, xx = rho - (yy + 1) * pitch;
