@@ -64,7 +64,7 @@ class SearchRef:
                                    max_sims=self.num_simulations)
         return self.tree.Roots(n, legal_actions)
 
-    def search(self, roots, model, latent_state_roots, to_play_batch, recorder=None, replay=None):
+    def search(self, roots, model, latent_state_roots, to_play_batch, recorder=None):
         """mcts_ctree.py:281-368.  latent_state_roots: np.ndarray [B,C,H,W]."""
         tree = self.tree
         with torch.no_grad():
@@ -80,22 +80,18 @@ class SearchRef:
                 ix_l, iy_l, last_actions, virtual_to_play = tree.batch_traverse(
                     roots, self.pb_c_base, self.pb_c_init, self.discount_factor, mm, results,
                     list(tp_arg), self.deterministic)
-                if replay is not None:
-                    rec = replay[simulation_index]
-                    reward_batch, value_batch, policy_logits_batch = rec["reward"], rec["value"], rec["policy"]
-                else:
-                    latent_states = [latent_pool[ix][iy] for ix, iy in zip(ix_l, iy_l)]
-                    latent_states = torch.from_numpy(np.asarray(latent_states))
-                    actions = torch.from_numpy(np.asarray(last_actions)).long()
-                    if self.duplicate_inference:
-                        model.recurrent_inference(latent_states, actions)   # mcts_ctree.py:338 (discarded)
-                    out = model.recurrent_inference(latent_states, actions)
-                    latent_pool.append(out.latent_state.detach().cpu().numpy())
-                    value = self.value_inv(out.value).detach().cpu().numpy()
-                    reward = self.reward_inv(out.reward).detach().cpu().numpy()
-                    reward_batch = reward.reshape(-1).tolist()
-                    value_batch = value.reshape(-1).tolist()
-                    policy_logits_batch = out.policy_logits.detach().cpu().numpy().tolist()
+                latent_states = [latent_pool[ix][iy] for ix, iy in zip(ix_l, iy_l)]
+                latent_states = torch.from_numpy(np.asarray(latent_states))
+                actions = torch.from_numpy(np.asarray(last_actions)).long()
+                if self.duplicate_inference:
+                    model.recurrent_inference(latent_states, actions)   # mcts_ctree.py:338 (discarded)
+                out = model.recurrent_inference(latent_states, actions)
+                latent_pool.append(out.latent_state.detach().cpu().numpy())
+                value = self.value_inv(out.value).detach().cpu().numpy()
+                reward = self.reward_inv(out.reward).detach().cpu().numpy()
+                reward_batch = reward.reshape(-1).tolist()
+                value_batch = value.reshape(-1).tolist()
+                policy_logits_batch = out.policy_logits.detach().cpu().numpy().tolist()
                 if recorder is not None:
                     recorder.append(dict(ix=list(ix_l), iy=list(iy_l), last_action=list(last_actions),
                                          search_len=list(results.get_search_len()),
@@ -183,7 +179,7 @@ class SearchRefEZ(SearchRef):
         super().__init__(tree_module, **kw)
         self.lstm_horizon_len = lstm_horizon_len
 
-    def search(self, roots, model, latent_state_roots, reward_hidden_state_roots, to_play_batch, recorder=None, replay=None):
+    def search(self, roots, model, latent_state_roots, reward_hidden_state_roots, to_play_batch, recorder=None):
         tree = self.tree
         with torch.no_grad():
             if model is not None:
@@ -201,27 +197,23 @@ class SearchRefEZ(SearchRef):
                     roots, self.pb_c_base, self.pb_c_init, self.discount_factor, mm, results, list(tp_arg))
                 search_lens = results.get_search_len()
                 reset_idx = (np.array(search_lens) % self.lstm_horizon_len == 0)
-                if replay is not None:
-                    rec = replay[simulation_index]
-                    vp_batch, value_batch, policy_logits_batch = rec["reward"], rec["value"], rec["policy"]
-                else:
-                    latent_states = torch.from_numpy(np.asarray([latent_pool[ix][iy] for ix, iy in zip(ix_l, iy_l)]))
-                    s0 = torch.from_numpy(np.asarray([pool0[ix][0][iy] for ix, iy in zip(ix_l, iy_l)])).unsqueeze(0)
-                    s1 = torch.from_numpy(np.asarray([pool1[ix][0][iy] for ix, iy in zip(ix_l, iy_l)])).unsqueeze(0)
-                    actions = torch.from_numpy(np.asarray(last_actions)).long()
-                    out = model.recurrent_inference(latent_states, (s0, s1), actions)
-                    latent_pool.append(out.latent_state.detach().cpu().numpy())
-                    value = self.value_inv(out.value).detach().cpu().numpy()
-                    vp = self.value_inv(out.value_prefix).detach().cpu().numpy()      # :840-842 (value transform handle)
-                    n0 = out.reward_hidden_state[0].detach().cpu().numpy()
-                    n1 = out.reward_hidden_state[1].detach().cpu().numpy()
-                    n0[:, reset_idx, :] = 0
-                    n1[:, reset_idx, :] = 0
-                    pool0.append(n0)
-                    pool1.append(n1)
-                    vp_batch = vp.reshape(-1).tolist()
-                    value_batch = value.reshape(-1).tolist()
-                    policy_logits_batch = out.policy_logits.detach().cpu().numpy().tolist()
+                latent_states = torch.from_numpy(np.asarray([latent_pool[ix][iy] for ix, iy in zip(ix_l, iy_l)]))
+                s0 = torch.from_numpy(np.asarray([pool0[ix][0][iy] for ix, iy in zip(ix_l, iy_l)])).unsqueeze(0)
+                s1 = torch.from_numpy(np.asarray([pool1[ix][0][iy] for ix, iy in zip(ix_l, iy_l)])).unsqueeze(0)
+                actions = torch.from_numpy(np.asarray(last_actions)).long()
+                out = model.recurrent_inference(latent_states, (s0, s1), actions)
+                latent_pool.append(out.latent_state.detach().cpu().numpy())
+                value = self.value_inv(out.value).detach().cpu().numpy()
+                vp = self.value_inv(out.value_prefix).detach().cpu().numpy()      # :840-842 (value transform handle)
+                n0 = out.reward_hidden_state[0].detach().cpu().numpy()
+                n1 = out.reward_hidden_state[1].detach().cpu().numpy()
+                n0[:, reset_idx, :] = 0
+                n1[:, reset_idx, :] = 0
+                pool0.append(n0)
+                pool1.append(n1)
+                vp_batch = vp.reshape(-1).tolist()
+                value_batch = value.reshape(-1).tolist()
+                policy_logits_batch = out.policy_logits.detach().cpu().numpy().tolist()
                 is_reset_list = reset_idx.astype(np.int32).tolist()
                 if recorder is not None:
                     recorder.append(dict(ix=list(ix_l), iy=list(iy_l), last_action=list(last_actions),

@@ -3,8 +3,9 @@
 Each fixture holds the inputs of one search driven by synthetic network outputs (root logits / values / noise, legal
 lists, and per simulation the reward, value and policy logits fed to the back-up; values quantised so that scores tie
 exactly) and what the reference returned: per simulation the leaf choice (ix, iy, last action, search length, virtual
-to_play), and at the end visit counts, root values, trajectories, get_policies and get_children_values.  `replay` drives
-any module with the gmz_tree API (the compiled reference or lightzero_b200.gmz_tree) through the same loop.
+to_play), and at the end visit counts, root values, trajectories, get_policies and get_children_values.  A fixture is a
+tree_drive case: tree_drive.check_fixture replays it through any module with the gmz_tree API (the compiled reference
+or lightzero_b200.gmz_tree).
 
 usage: python tests/golden/make_gumbel_golden.py   (needs oracle/_ref/gmz_tree*.so, built by __graft_entry__.build())
 """
@@ -14,6 +15,8 @@ import sys
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
+from oracle.tree_drive import PER_SIM, drive, recorded  # noqa: E402
 
 # name -> (B, A, S, m, legal kind, noise, to_play, seed)
 CASES = {
@@ -47,54 +50,27 @@ def make_inputs(B, A, S, m, kind, noise, to_play, seed):
                 rewards=_q(rng, (S, B), 0.5), values=_q(rng, (S, B), 0.25), logits=_q(rng, (S, B, A), 1.0))
 
 
-def replay(mod, d):
-    """The reference search loop (mcts_ctree.py:1104-1172) on module `mod` with the fixture's inputs."""
-    B, A, S, m, tp = int(d["B"]), int(d["A"]), int(d["S"]), int(d["m"]), int(d["to_play"])
-    disc = float(d["discount"])
-    legal = [d["legal"][b, :d["nlegal"][b]].tolist() for b in range(B)]
-    roots = mod.Roots(B, legal)
-    if int(d["noise"]):
-        noises = [d["noises"][b, :d["nlegal"][b]].tolist() for b in range(B)]
-        roots.prepare(0.25, noises, [0.0] * B, d["root_values"].tolist(), d["root_logits"].tolist(), [tp] * B)
-    else:
-        roots.prepare_no_noise([0.0] * B, d["root_values"].tolist(), d["root_logits"].tolist(), [tp] * B)
-    mm = mod.MinMaxStatsList(B)
-    mm.set_delta(0.01)
-    rec = np.zeros((5, S, B), np.int32)
-    for sim in range(S):
-        res = mod.ResultsWrapper(B)
-        ix, iy, la, vtp = mod.batch_traverse(roots, S, m, disc, res, [tp] * B)
-        rec[:, sim] = [ix, iy, la, res.get_search_len(), vtp]
-        mod.batch_back_propagate(sim + 1, disc, d["rewards"][sim].tolist(), d["values"][sim].tolist(),
-                                 d["logits"][sim].tolist(), mm, res, list(vtp))
-    dist = np.full((B, A), -1, np.int32)
-    for b, v in enumerate(roots.get_distributions()):
-        dist[b, :len(v)] = v
-    traj = np.full((B, S + 1), -1, np.int32)
-    for b, v in enumerate(roots.get_trajectories()):
-        traj[b, :len(v)] = v
-    out = dict(rec=rec, dist=dist, root_value=np.asarray(roots.get_values(), np.float32), traj=traj,
-               policy=np.asarray(roots.get_policies(disc, A), np.float32),
-               children_values=np.asarray(roots.get_children_values(disc, A), np.float32))
-    if hasattr(roots, "clear") and mod.__name__.startswith("lightzero_b200"):
-        roots.clear()
-    return out
+def expected(trace):
+    """A tree_drive.drive trace under the fixtures' exp_* names (tree_drive.fixture_trace reads them back)."""
+    return dict(exp_rec=np.stack([trace[k] for k in PER_SIM[:5]]), exp_dist=trace["distributions"],
+                exp_root_value=trace["root_values_bits"].view(np.float32), exp_traj=trace["trajectories"],
+                exp_policy=trace["policies"], exp_children_values=trace["children_values"])
 
 
-EXPECTED = ("rec", "dist", "root_value", "traj", "policy", "children_values")
+def make_case(ref, *case):
+    d = make_inputs(*case)
+    trace, _ = drive(ref, d, "gumbel", recorded(d, "gumbel"))
+    return dict(d, **expected(trace))
 
 
 def main():
-    sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
     from oracle import build_gmz_ref
     ref = build_gmz_ref.load()
     if ref is None:
         raise SystemExit("oracle/_ref/gmz_tree*.so is missing: run __graft_entry__.build() with the reference sources present")
     for name, case in CASES.items():
-        d = make_inputs(*case)
-        out = replay(ref, d)
         path = os.path.join(HERE, name + ".npz")
-        np.savez_compressed(path, **d, **{"exp_" + k: v for k, v in out.items()})
+        np.savez_compressed(path, **make_case(ref, *case))
         print(path, os.path.getsize(path), "bytes")
 
 

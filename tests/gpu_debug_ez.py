@@ -4,7 +4,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import lightzero_b200 as lzb
-from lightzero_b200 import cabi, ez_tree, mz_tree
+from lightzero_b200 import cabi, ez_tree
 from oracle.model_ref import EfficientZeroModelRef, MuZeroModelRef, emulate_trained_
 
 B, A, S = int(os.environ.get("DBG_B", 256)), 6, 50
@@ -42,7 +42,6 @@ t_ez = timeit(lambda: lib.lz_model_recurrent_inference_ez(cez._h, B, lat.data_pt
 print(f"B={B}: MuZero recurrent (k_net_tc incl. reward FC) {t_mz:.1f} us | EfficientZero recurrent (k_net_tc + LSTM GEMM + head) {t_ez:.1f} us | LSTM+head ~ {t_ez - t_mz:.1f} us")
 # tree kernels: traverse + backprop on prepared EZ trees
 roots = ez_tree.Roots(B, [list(range(A))] * B)
-mz_tree.DEFAULT_MAX_SIMS = 64
 roots.prepare_no_noise([0.] * B, torch.randn(B, A).cuda(), [-1] * B)
 roots._materialize(S, (19652, 1.25, 0.997, 0.01))
 t = roots._tree

@@ -22,6 +22,7 @@ import lightzero_b200 as lzb
 from lightzero_b200 import mz_tree
 from oracle.model_ref import MuZeroModelRef, emulate_trained_
 from oracle.search_ref import SearchRef, collect_step_ref, load_tree_module
+from oracle.tree_drive import assert_same, drive, from_recorder, recorded
 
 
 class Recorder:
@@ -55,7 +56,6 @@ def run(B, A, S, seed):
     t0 = time.time()
     exp = collect_step_ref(SearchRef(tree, num_simulations=S), ref, obs, mask, [-1] * B, noises=noises, recorder=rec)
     t_ref = time.time() - t0
-    mz_tree.DEFAULT_MAX_SIMS = max(mz_tree.DEFAULT_MAX_SIMS, S)
     mcts = lzb.MuZeroMCTSCtree(dict(num_simulations=S, deterministic=True, discount_factor=0.997))
     out = cu.initial_inference(obs.cuda())
     # (1) the fused CUDA pipeline
@@ -67,18 +67,14 @@ def run(B, A, S, seed):
     exp_v = np.asarray(exp["values"], np.float64)
     same = np.array([g == e for g, e in zip(got_d, exp["distributions"])])
     # (2) replay of the oracle's network outputs through the CUDA trees
-    roots = mz_tree.Roots(B, legal)
-    roots.prepare(0.25, noises, [0.] * B, exp["policy_logits"].tolist(), [-1] * B)
-    mm = mz_tree.MinMaxStatsList(B)
-    mm.set_delta(0.01)
-    replay_ok = True
-    for s in range(S):
-        res = mz_tree.ResultsWrapper(B)
-        ix, iy, la, vtp = mz_tree.batch_traverse(roots, 19652, 1.25, 0.997, mm, res, [-1] * B, True)
-        replay_ok &= (ix == rec[s]["ix"] and la == rec[s]["last_action"] and res.get_search_len() == rec[s]["search_len"])
-        mz_tree.batch_backpropagate(s + 1, 0.997, rec[s]["reward"], rec[s]["value"], rec[s]["policy"], mm, res, vtp)
-    replay_ok &= roots.get_distributions() == exp["distributions"]
-    replay_ok &= bool(np.array_equal(np.asarray(roots.get_values(), np.float32).view(np.uint32), np.asarray(exp["values"], np.float32).view(np.uint32)))
+    c = dict(B=B, A=A, S=S, legal=legal, root_logits=exp["policy_logits"], noises=noises, to_play=[-1] * B, **from_recorder(rec))
+    trace, roots = drive(mz_tree, c, "mz", recorded(c))
+    try:
+        assert_same(trace, c)
+        replay_ok = roots.get_distributions() == exp["distributions"] and bool(np.array_equal(
+            np.asarray(roots.get_values(), np.float32).view(np.uint32), np.asarray(exp["values"], np.float32).view(np.uint32)))
+    except AssertionError:
+        replay_ok = False
     roots.clear()
     # (3) the same CUDA search step-wise with a recorder, to classify the diverging roots
     roots = mcts.roots(B, legal)

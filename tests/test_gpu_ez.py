@@ -135,23 +135,18 @@ def test_fused_ez_search_equals_stepwise_search(B, A, S, masks, horizon):
 def test_replay_of_reference_ez_pipeline_is_bit_exact():
     """Feed the CUDA value-prefix trees the network outputs recorded from the ORACLE pipeline (compiled
     ctree_efficientzero + PyTorch-CPU EfficientZero model): visit counts and root values must match bit for bit."""
-    from lightzero_b200 import ez_tree, mz_tree
+    from lightzero_b200 import ez_tree
     from oracle.search_ref import SearchRefEZ, collect_step_ref_ez, load_tree_module
+    from oracle.tree_drive import assert_same, drive, from_recorder, recorded
     B, A, S, H = 40, 18, 40, 3
     ref, cu, obs, mask, legal, noises, mcts = _setup(B, A, S, seed=5, masks=True, horizon=H)
     tree, kind = load_tree_module(name="ez_tree")
     rec = []
     exp = collect_step_ref_ez(SearchRefEZ(tree, lstm_horizon_len=H, num_simulations=S), ref, obs, mask, [-1] * B, noises=noises, recorder=rec)
-    mz_tree.DEFAULT_MAX_SIMS = max(mz_tree.DEFAULT_MAX_SIMS, S)
-    roots = ez_tree.Roots(B, legal)
-    roots.prepare(0.25, noises, [0.] * B, exp["policy_logits"].tolist(), [-1] * B)
-    mm = ez_tree.MinMaxStatsList(B)
-    mm.set_delta(0.01)
-    for s in range(S):
-        res = ez_tree.ResultsWrapper(B)
-        ix, iy, la, vtp = ez_tree.batch_traverse(roots, 19652, 1.25, 0.997, mm, res, [-1] * B)
-        assert ix == rec[s]["ix"] and la == rec[s]["last_action"] and res.get_search_len() == rec[s]["search_len"]
-        ez_tree.batch_backpropagate(s + 1, 0.997, rec[s]["reward"], rec[s]["value"], rec[s]["policy"], mm, res, rec[s]["is_reset"], vtp)
+    c = dict(B=B, A=A, S=S, legal=legal, root_logits=exp["policy_logits"], noises=noises, to_play=[-1] * B, lstm_horizon_len=H,
+             **from_recorder(rec))
+    trace, roots = drive(ez_tree, c, "ez", recorded(c))
+    assert_same(trace, c)
     assert roots.get_distributions() == exp["distributions"]
     assert np.array_equal(np.asarray(roots.get_values(), np.float32).view(np.uint32),
                           np.asarray(exp["values"], np.float32).view(np.uint32))

@@ -30,7 +30,9 @@ import torch
 from test_gpu_net_layers import ALPHA, _bn, inverse_h, lstm_bound, make_latents as latents6, net_stage as net_stage6, \
     pow2_hi, program, split_full, worst
 from test_gpu_obs64 import make_latents as latents8, net_stage as net_stage8
-from test_gpu_search_oracle import _inputs, _prepare, debug_rng, near_policy, peaked_zero_values, zero_policy
+from oracle.tree_drive import assert_same, drive, network, readout
+from test_gpu_search_oracle import _inputs, _prepare, debug_rng, differ, near_policy, peaked_zero_values, visits_sum_to, \
+    zero_policy
 
 pytestmark = pytest.mark.gpu
 
@@ -273,46 +275,20 @@ def fused_search_ez(cu, mcts, latent, h0, c0, legal, logits, noises, tp, cap=Non
     if cap is not None:
         roots._materialize(cap)
     mcts.search(roots, cu, latent, (h0[None], c0[None]), tp)
-    res = (roots.get_distributions(), np.asarray(roots.get_values(), np.float32).view(np.uint32).tolist(),
-           roots.get_trajectories())
-    return res, debug_rng(roots), roots
+    return readout(roots, logits.shape[1], int(mcts._cfg.num_simulations)), debug_rng(roots), roots
 
 
 def oracle_search_ez(cu, S, horizon, latent, h0, c0, legal, logits, noises, tp, det, key=None, step0=0, discount=0.997,
                      delta=0.01, zero_reset_state=True, reset_in_backup=True):
-    """The reference loop (mcts_ctree.py:729-876) on oracle.ctree_port_ez with the CUDA network evaluating the leaves.
-    Returns ((visit counts, root-value bits, trajectories), tie statistics, resets)."""
+    """The reference loop (mcts_ctree.py:729-876, oracle/tree_drive.py) on oracle.ctree_port_ez with the CUDA network
+    evaluating the leaves.  Returns (trace, tie statistics, resets)."""
     from oracle import ctree_port_ez as port
-    B, A, H = len(tp), logits.shape[1], h0.shape[1]
-    roots = port.Roots(B, legal, action_space_size=A, max_sims=S)
-    _prepare(roots, logits.tolist(), noises, tp)
-    if not det:
-        roots.set_tie_hash(key[0], key[1], step0)
-    mm = port.MinMaxStatsList(B)
-    mm.set_delta(delta)
-    pool = torch.empty((S + 1,) + tuple(latent.shape), device="cuda")
-    hpool, cpool = torch.empty(S + 1, B, H, device="cuda"), torch.empty(S + 1, B, H, device="cuda")
-    pool[0], hpool[0], cpool[0] = latent, h0, c0
-    resets = 0
-    with torch.no_grad():
-        for s in range(S):
-            res = port.ResultsWrapper(B)
-            ix, iy, la, vtp = port.batch_traverse(roots, 19652, 1.25, discount, mm, res, list(tp))
-            ixt, iyt = torch.tensor(ix, device="cuda"), torch.tensor(iy, device="cuda")
-            o = cu.recurrent_inference(pool[ixt, iyt], (hpool[ixt, iyt][None], cpool[ixt, iyt][None]),
-                                       torch.tensor(la, device="cuda"), return_scalars=True)
-            reset = np.asarray(res.get_search_len()) % horizon == 0
-            resets += int(reset.sum())
-            pool[s + 1] = o.latent_state
-            zero = torch.from_numpy(reset & zero_reset_state).cuda().view(B, 1)
-            hpool[s + 1] = torch.where(zero, 0.0, o.reward_hidden_state[0][0])
-            cpool[s + 1] = torch.where(zero, 0.0, o.reward_hidden_state[1][0])
-            port.batch_backpropagate(s + 1, discount, o.value_prefix_scalar.cpu().numpy(), o.value_scalar.cpu().numpy(),
-                                     o.policy_logits.cpu().numpy(), mm, res,
-                                     (reset if reset_in_backup else np.zeros(B, bool)).astype(np.int32), vtp)
-    out = (roots.get_distributions(), np.asarray(roots.get_values(), np.float32).view(np.uint32).tolist(),
-           roots.get_trajectories())
-    return out, roots.tie_stats(), resets
+    c = dict(B=len(tp), A=logits.shape[1], S=S, legal=legal, root_logits=logits, noises=noises, to_play=tp,
+             discount=discount, delta=delta, lstm_horizon_len=horizon)
+    setup = None if det else (lambda r: r.set_tie_hash(key[0], key[1], step0))
+    trace, roots = drive(port, c, "ez", network(cu, latent, (h0, c0), zero_reset_state), setup=setup,
+                         reset_in_backup=reset_in_backup)
+    return trace, roots.tie_stats(), int(trace["is_reset"].sum())
 
 
 def _setup(spec, A, B, seed, players, ikw, mutate=None, zero_hidden=False):
@@ -373,10 +349,8 @@ def test_fused_ez_search_equals_oracle_driving_the_same_network(name):
     roots.clear()
     kernel = lstm_kernel(spec[0], spec[1], spec[2])
     _report(name, st, resets, kernel, nk, time.time() - t0)
-    assert got[0] == exp[0], "visit counts"
-    assert got[1] == exp[1], "root value bits"
-    assert got[2] == exp[2], "trajectories"
-    assert all(sum(d) == S for d in got[0])
+    assert_same(got, exp)
+    assert visits_sum_to(got, S)
     assert nk == 1 + 4 * S
     # the branch the case is named for
     assert _kernels(lambda: cu.recurrent_inference(latent[:1], (h0[:1][None], c0[:1][None]), torch.zeros(1, dtype=torch.long).cuda())) \
@@ -417,7 +391,8 @@ def test_discount_and_value_delta_max():
     exp, st, resets = oracle_search_ez(cu, S, H, latent, h0, c0, legal, logits, noises, tp, False, key=key, discount=0.9, delta=0.05)
     default, _, _ = oracle_search_ez(cu, S, H, latent, h0, c0, legal, logits, noises, tp, False, key=key)
     _report("a9_b96_s40_h3_sto_2p_discount0.9_delta0.05", st, resets, lstm_kernel(96, 16, 512), mcts.last_num_kernels, 0.0)
-    assert got == exp and got[0] != default[0]
+    assert_same(got, exp)
+    assert not np.array_equal(got["distributions"], default["distributions"])
     assert st["draws"] > 0 and resets > 0
 
 
@@ -435,9 +410,9 @@ def test_repeated_stochastic_searches_on_one_pooled_tree():
     roots.clear()
     for got, key in ((first, key1), (second, key2)):
         exp, st, resets = oracle_search_ez(cu, S, H, latent, h0, c0, legal, logits, noises, tp, False, key=key)
-        assert got == exp
+        assert_same(got, exp)
     _report("a18_b200_s30_h4_sto_repeated", st, resets, lstm_kernel(96, 16, 512), mcts.last_num_kernels, 0.0)
-    assert first[0] != second[0] and st["draws"] > 0 and resets > 0
+    assert not np.array_equal(first["distributions"], second["distributions"]) and st["draws"] > 0 and resets > 0
 
 
 def test_sensitivity_of_the_comparison():
@@ -452,11 +427,11 @@ def test_sensitivity_of_the_comparison():
     run = lambda **kw: oracle_search_ez(cu, S, kw.pop("horizon", H), latent, h0, c0, legal, logits, noises, tp, False,
                                         **dict(dict(key=key), **kw))
     exp, st, resets = run()
-    assert got == exp
+    assert_same(got, exp)
     assert resets >= B * S // 4 and st["draws"] > 0
 
     def frac(o):
-        return float(np.mean([g != e or gv != ev for g, e, gv, ev in zip(got[0], o[0][0], got[1], o[0][1])]))
+        return float(differ(got, o[0]).mean())
     fr = {
         "horizon-1": frac(run(horizon=H - 1)),
         "horizon+1": frac(run(horizon=H + 1)),

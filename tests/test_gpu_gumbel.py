@@ -12,6 +12,8 @@ import numpy as np
 import pytest
 import torch
 
+from oracle.tree_drive import Sampled, assert_same, check_fixture, drive, network, readout
+
 pytestmark = pytest.mark.gpu
 
 
@@ -21,10 +23,6 @@ def _oracle():
     if mod is None:
         pytest.skip("compiled reference Gumbel tree not built (oracle/build_gmz_ref.py)")
     return mod
-
-
-def _bits(x):
-    return np.asarray(x, np.float32).view(np.uint32)
 
 
 def _legal(rng, B, A, kind):
@@ -44,44 +42,15 @@ def _q(rng, shape, step):
     return (np.round(rng.normal(size=shape) / step) * step).astype(np.float32)
 
 
-def _drive(mod, roots, B, A, S, m, legal, rng_seed, noise, to_play, discount=0.997):
-    """Runs the reference search loop (mcts_ctree.py:1104-1172) with synthetic network outputs on module `mod`
-    (the compiled reference or lightzero_b200.gmz_tree); returns the per-simulation records and the read-outs."""
-    rng = np.random.default_rng(rng_seed)
-    logits = _q(rng, (B, A), 0.5)
-    values = _q(rng, (B,), 0.25)
-    rewards = [0.0] * B
-    tp = [to_play] * B
+def _case(B, A, S, m, legal, seed, noise, to_play):
+    """Synthetic inputs and network outputs (quantised so that scores tie): root logits, values and noise, then per
+    simulation reward, value and policy logits drawn by the returned Sampled source."""
+    rng = np.random.default_rng(seed)
+    c = dict(B=B, A=A, S=S, m=m, legal=legal, to_play=to_play, noise=int(noise), root_logits=_q(rng, (B, A), 0.5),
+             root_values=_q(rng, (B,), 0.25))
     if noise:
-        noises = [rng.dirichlet([0.3] * len(l)).astype(np.float32).tolist() for l in legal]
-        roots.prepare(0.25, noises, rewards, values.tolist(), logits.tolist(), tp)
-    else:
-        roots.prepare_no_noise(rewards, values.tolist(), logits.tolist(), tp)
-    mm = mod.MinMaxStatsList(B)
-    mm.set_delta(0.01)
-    recs = []
-    for sim in range(S):
-        res = mod.ResultsWrapper(B)
-        ix, iy, la, vtp = mod.batch_traverse(roots, S, m, discount, res, list(tp))
-        recs.append((list(ix), list(iy), list(la), list(res.get_search_len()), list(vtp)))
-        r = _q(rng, (B,), 0.5)
-        v = _q(rng, (B,), 0.25)
-        pl = _q(rng, (B, A), 1.0)
-        mod.batch_back_propagate(sim + 1, discount, r.tolist(), v.tolist(), pl.tolist(), mm, res, list(vtp))
-    out = dict(dist=roots.get_distributions(), values=roots.get_values(), traj=roots.get_trajectories(),
-               pol=roots.get_policies(discount, A), cv=roots.get_children_values(discount, A))
-    return recs, out
-
-
-def _compare(exp, got):
-    (erec, eout), (grec, gout) = exp, got
-    for sim, (e, g) in enumerate(zip(erec, grec)):
-        assert e == g, f"simulation {sim}: reference {e} != device {g}"
-    assert eout["dist"] == gout["dist"]
-    assert np.array_equal(_bits(eout["values"]), _bits(gout["values"]))
-    assert eout["traj"] == gout["traj"]
-    assert np.array_equal(_bits(eout["pol"]), _bits(gout["pol"]))
-    assert np.array_equal(_bits(eout["cv"]), _bits(gout["cv"]))
+        c["noises"] = [rng.dirichlet([0.3] * len(l)).astype(np.float32).tolist() for l in legal]
+    return c, Sampled(lambda: (_q(rng, (B,), 0.5), _q(rng, (B,), 0.25), _q(rng, (B, A), 1.0)))
 
 
 CASES = [  # B, A, S, m, legal kind, noise, to_play
@@ -105,10 +74,11 @@ def test_stepwise_tree_matches_reference(B, A, S, m, kind, noise, to_play):
     from lightzero_b200 import gmz_tree
     legal = _legal(np.random.default_rng(B * 1000 + A), B, A, kind)
     seed = B + 7 * A + S + m
-    exp = _drive(ref, ref.Roots(B, legal), B, A, S, m, legal, seed, noise, to_play)
-    roots = gmz_tree.Roots(B, legal)
-    got = _drive(gmz_tree, roots, B, A, S, m, legal, seed, noise, to_play)
-    _compare(exp, got)
+    c, leaves = _case(B, A, S, m, legal, seed, noise, to_play)
+    exp, _ = drive(ref, c, "gumbel", leaves)
+    c, leaves = _case(B, A, S, m, legal, seed, noise, to_play)
+    got, roots = drive(gmz_tree, c, "gumbel", leaves)
+    assert_same(got, exp)
     roots.clear()
 
 
@@ -136,23 +106,11 @@ def _roots_inputs(model, B, A, obs, seed, masked):
     return out, legal, noises
 
 
-def _oracle_search(ref, model, out, legal, noises, B, A, S, m, discount=0.997):
+def _oracle_search(ref, model, out, legal, noises, B, A, S, m):
     """The reference tree picks every leaf, the CUDA network evaluates it (recurrent_inference(return_scalars=True))."""
-    roots = ref.Roots(B, legal)
-    roots.prepare(0.25, noises, [0.0] * B, out.value_scalar.cpu().tolist(), out.policy_logits.cpu().numpy().tolist(), [-1] * B)
-    mm = ref.MinMaxStatsList(B)
-    mm.set_delta(0.01)
-    pool = [out.latent_state]
-    for sim in range(S):
-        res = ref.ResultsWrapper(B)
-        ix, iy, la, vtp = ref.batch_traverse(roots, S, m, discount, res, [-1] * B)
-        lat = torch.stack([pool[i][j] for i, j in zip(ix, iy)])
-        o = model.recurrent_inference(lat, torch.tensor(la), return_scalars=True)
-        pool.append(o.latent_state)
-        ref.batch_back_propagate(sim + 1, discount, o.reward_scalar.cpu().tolist(), o.value_scalar.cpu().tolist(),
-                                 o.policy_logits.cpu().numpy().tolist(), mm, res, vtp)
-    return dict(dist=roots.get_distributions(), values=roots.get_values(), pol=roots.get_policies(discount, A),
-                cv=roots.get_children_values(discount, A), traj=roots.get_trajectories())
+    c = dict(B=B, A=A, S=S, m=m, legal=legal, to_play=-1, noises=noises, root_logits=out.policy_logits.cpu().numpy(),
+             root_values=out.value_scalar.cpu().numpy())
+    return drive(ref, c, "gumbel", network(model, out.latent_state))[0]
 
 
 def _fused_search(model, out, legal, noises, B, A, S, m):
@@ -161,17 +119,7 @@ def _fused_search(model, out, legal, noises, B, A, S, m):
     roots = mcts.roots(B, legal)
     roots.prepare(0.25, noises, [0.0] * B, out.value_scalar, out.policy_logits, [-1] * B)
     mcts.search(roots, model, out.latent_state, [-1] * B)
-    res = dict(dist=roots.get_distributions(), values=roots.get_values(), pol=roots.get_policies(0.997, A),
-               cv=roots.get_children_values(0.997, A), traj=roots.get_trajectories())
-    return res, mcts, roots
-
-
-def _same(e, g):
-    assert e["dist"] == g["dist"]
-    assert np.array_equal(_bits(e["values"]), _bits(g["values"]))
-    assert np.array_equal(_bits(e["pol"]), _bits(g["pol"]))
-    assert np.array_equal(_bits(e["cv"]), _bits(g["cv"]))
-    assert e["traj"] == g["traj"]
+    return readout(roots, A, S, 0.997), mcts, roots
 
 
 @pytest.mark.parametrize("obs,A,m,S,B,masked", [
@@ -188,7 +136,7 @@ def test_fused_search_matches_reference_driving_the_same_network(obs, A, m, S, B
     out, legal, noises = _roots_inputs(model, B, A, obs, 11, masked)
     got, mcts, roots = _fused_search(model, out, legal, noises, B, A, S, m)
     assert mcts.last_num_kernels >= 1 + 2 * S
-    _same(_oracle_search(ref, model, out, legal, noises, B, A, S, m), got)
+    assert_same(got, _oracle_search(ref, model, out, legal, noises, B, A, S, m))
     roots.clear()
 
 
@@ -205,8 +153,7 @@ def test_fused_equals_stepwise_and_recaptures():
     roots2 = mcts.roots(B, legal)
     roots2.prepare(0.25, noises, [0.0] * B, out.value_scalar, out.policy_logits, [-1] * B)
     mcts.search(roots2, Wrapped(), out.latent_state, [-1] * B)
-    _same(fused, dict(dist=roots2.get_distributions(), values=roots2.get_values(), pol=roots2.get_policies(0.997, A),
-                      cv=roots2.get_children_values(0.997, A), traj=roots2.get_trajectories()))
+    assert_same(fused, readout(roots2, A, S, 0.997))
     roots2.clear()
     # a weight reload and then a parameter change must re-capture the graph the first search captured on this pooled tree:
     # results follow the new weights / (m, S)
@@ -218,7 +165,7 @@ def test_fused_equals_stepwise_and_recaptures():
     for mm_ in (m, 4):
         got, _, r = _fused_search(model, out, legal, noises, B, A, S, mm_)
         assert r._tree is tree            # the same tree and search handle, whose graph was captured before
-        _same(_oracle_search(ref, model, out, legal, noises, B, A, S, mm_), got)
+        assert_same(got, _oracle_search(ref, model, out, legal, noises, B, A, S, mm_))
         r.clear()
 
 
@@ -238,13 +185,10 @@ def test_golden_fixtures_replay_on_device():
     """tests/golden/gumbel_*.npz (written from the compiled reference) replayed through lightzero_b200.gmz_tree, with no
     reference module involved: per-simulation leaf choices and virtual to_play, and the read-outs, bit for bit."""
     from lightzero_b200 import gmz_tree
-    gen, files = _golden()
+    _, files = _golden()
     for f in files:
-        d = dict(np.load(f))
-        got = gen.replay(gmz_tree, d)
-        for k in gen.EXPECTED:
-            assert np.array_equal(np.asarray(got[k]).view(np.uint32) if got[k].dtype == np.float32 else got[k],
-                                  d["exp_" + k].view(np.uint32) if d["exp_" + k].dtype == np.float32 else d["exp_" + k]), (f, k)
+        _, roots = check_fixture(gmz_tree, np.load(f))
+        roots.clear()
 
 
 def test_empty_legal_list_is_every_action():
@@ -253,27 +197,20 @@ def test_empty_legal_list_is_every_action():
     from lightzero_b200 import gmz_tree
     B, A, S, m = 3, 6, 16, 4
     rng = np.random.default_rng(5)
-    logits = _q(rng, (B, A), 0.5).tolist()
-    values = _q(rng, (B,), 0.25).tolist()
+    c = dict(B=B, A=A, S=S, m=m, to_play=-1, root_logits=_q(rng, (B, A), 0.5), root_values=_q(rng, (B,), 0.25))
     outs = []
     for legal in ([[], [0, 2], []], [list(range(A)), [0, 2], list(range(A))],
                   np.array([[0] * A, [1, 0, 1, 0, 0, 0], [0] * A], np.uint8)):
-        roots = gmz_tree.Roots(B, legal)
-        roots.prepare_no_noise([0.0] * B, values, logits, [-1] * B)
-        rec = []
-        for sim in range(S):
-            res = gmz_tree.ResultsWrapper(B)
-            ix, iy, la, vtp = gmz_tree.batch_traverse(roots, S, m, 0.997, res, [-1] * B)
-            assert min(la) >= 0
-            rec.append((ix, la, res.get_search_len()))
-            gmz_tree.batch_back_propagate(sim + 1, 0.997, _q(rng, (B,), 0.5).tolist(), _q(rng, (B,), 0.25).tolist(),
-                                          _q(rng, (B, A), 1.0).tolist(), None, res, vtp)
-        outs.append((rec, roots.get_distributions(), _bits(roots.get_policies(0.997, A)).tolist()))
-        roots.clear()
         rng = np.random.default_rng(5)
         rng.normal(size=B * A + B)       # same synthetic stream for each legal form
-    assert outs[0] == outs[1] == outs[2]
-    assert all(len(d) == A for d in (outs[0][1][0], outs[0][1][2]))
+        t, roots = drive(gmz_tree, dict(c, legal=legal), "gumbel",
+                         Sampled(lambda: (_q(rng, (B,), 0.5), _q(rng, (B,), 0.25), _q(rng, (B, A), 1.0))))
+        roots.clear()
+        assert (t["last_action"] >= 0).all()
+        outs.append({k: t[k] for k in ("ix", "last_action", "search_len", "distributions", "policies")})
+    assert_same(outs[1], outs[0])
+    assert_same(outs[2], outs[0])
+    assert (outs[0]["distributions"][[0, 2]] >= 0).all()
 
 
 def test_refusals():

@@ -21,6 +21,7 @@ import torch.nn.functional as F
 
 from test_gpu_net_layers import ALPHA, SUPPORT, TAU, check_scalars, head_features, head_reference, inverse_h, layer_reference, \
     lstm_bound, program, split_full, split_hi_lo, worst
+from oracle.tree_drive import assert_same
 from test_gpu_search_oracle import _inputs as search_inputs, fused_search, oracle_search
 from test_gpu_tower_layers import ALPHA as T_ALPHA, TAU as T_TAU, WGMMA_STAGES, _atari_frames, dump_stage, stage_reference, \
     stage_value, tcl_grid
@@ -317,9 +318,7 @@ def test_fused_search_equals_oracle_driving_the_same_network(name):
         assert mcts.last_num_kernels == 1
     else:
         assert plan["persistent"] == 0 and mcts.last_num_kernels == 2 * S + 1, plan
-    assert got[0] == exp[0], "visit counts"
-    assert got[1] == exp[1], "root value bits"
-    assert got[2] == exp[2], "trajectories"
+    assert_same(got, exp)
     if not det:
         assert st["draws"] > 0, st
 
@@ -342,6 +341,7 @@ def _search_setup(B, A, S, seed, ez=False):
 
 def test_search_with_reuse_equals_stepwise_drive():
     from lightzero_b200 import mz_tree
+    from oracle.tree_drive import drive, network, readout
     B, A, S = 96, 6, 30
     cu, obs, mask, legal, noises, mcts = _search_setup(B, A, S, seed=21)
     out = cu.initial_inference(obs.cuda())
@@ -351,36 +351,13 @@ def test_search_with_reuse_equals_stepwise_drive():
     roots = mcts.roots(B, legal)
     roots.prepare(0.25, noises, [0.] * B, out.policy_logits, [-1] * B)
     mcts.search_with_reuse(roots, cu, out.latent_state, [-1] * B, true_action, reuse_value)
-    fused = (roots.get_distributions(), np.asarray(roots.get_values(), np.float32).view(np.uint32).tolist())
+    fused = readout(roots, A, S)
     roots.clear()
-    mz_tree.DEFAULT_MAX_SIMS = max(mz_tree.DEFAULT_MAX_SIMS, S)
-    roots = mz_tree.Roots(B, legal)
-    roots.prepare(0.25, noises, [0.] * B, out.policy_logits, [-1] * B)
-    mm = mz_tree.MinMaxStatsList(B)
-    mm.set_delta(0.01)
-    pool, counts = [out.latent_state], []
-    for s in range(S):
-        res = mz_tree.ResultsWrapper(B)
-        ix, iy, la, vtp = mz_tree.batch_traverse_with_reuse(roots, 19652, 1.25, 0.997, mm, res, [-1] * B, true_action, reuse_value)
-        lat, acts, no_inf, reuse = [], [], [], []
-        for count, (x, y) in enumerate(zip(ix, iy)):
-            if x != -1:
-                lat.append(pool[x][y]); acts.append(la[count])
-            else:
-                no_inf.append(y)
-            if x == 0 and la[count] == true_action[count]:
-                reuse.append(count)
-        counts.append(len(acts))
-        if acts:
-            o = cu.recurrent_inference(torch.stack(lat), torch.tensor(acts), return_scalars=True)
-            pool.append(o.latent_state)
-            r, v, p = o.reward_scalar, o.value_scalar, o.policy_logits
-        else:
-            pool.append([]); r, v, p = [], [], []
-        no_inf.append(-1); reuse.append(-1)
-        mz_tree.batch_backpropagate_with_reuse(s + 1, 0.997, r, v, p, mm, res, vtp, no_inf, reuse, reuse_value)
-    step = (roots.get_distributions(), np.asarray(roots.get_values(), np.float32).view(np.uint32).tolist())
-    assert fused == step
+    c = dict(B=B, A=A, S=S, legal=legal, root_logits=out.policy_logits.cpu().numpy(), noises=noises, to_play=[-1] * B,
+             true_action=true_action, reuse_value=reuse_value)
+    step, _ = drive(mz_tree, c, "reuse", network(cu, out.latent_state))
+    assert_same(step, fused)
+    counts = step["n_inferred"].tolist()
     assert min(counts) < B
 
 

@@ -113,20 +113,14 @@ def test_replay_of_reference_pipeline_is_bit_exact(B, A, S):
     and root values bit for bit, on the same seeds -- also at BASELINE config 3's 200 simulations on a 128-root shard."""
     from lightzero_b200 import mz_tree
     from oracle.search_ref import SearchRef, collect_step_ref, load_tree_module
+    from oracle.tree_drive import assert_same, drive, from_recorder, recorded
     ref, cu, obs, mask, legal, noises, mcts = _setup(B, A, S, seed=5, masks=True)
     tree, kind = load_tree_module()
     rec = []
     exp = collect_step_ref(SearchRef(tree, num_simulations=S), ref, obs, mask, [-1] * B, noises=noises, recorder=rec)
-    mz_tree.DEFAULT_MAX_SIMS = max(mz_tree.DEFAULT_MAX_SIMS, S)
-    roots = mz_tree.Roots(B, legal)
-    roots.prepare(0.25, noises, [0.] * B, exp["policy_logits"].tolist(), [-1] * B)
-    mm = mz_tree.MinMaxStatsList(B)
-    mm.set_delta(0.01)
-    for s in range(S):
-        res = mz_tree.ResultsWrapper(B)
-        ix, iy, la, vtp = mz_tree.batch_traverse(roots, 19652, 1.25, 0.997, mm, res, [-1] * B, True)
-        assert ix == rec[s]["ix"] and la == rec[s]["last_action"] and res.get_search_len() == rec[s]["search_len"]
-        mz_tree.batch_backpropagate(s + 1, 0.997, rec[s]["reward"], rec[s]["value"], rec[s]["policy"], mm, res, vtp)
+    c = dict(B=B, A=A, S=S, legal=legal, root_logits=exp["policy_logits"], noises=noises, to_play=[-1] * B, **from_recorder(rec))
+    trace, roots = drive(mz_tree, c, "mz", recorded(c))
+    assert_same(trace, c)
     assert roots.get_distributions() == exp["distributions"]
     assert np.array_equal(np.asarray(roots.get_values(), np.float32).view(np.uint32),
                           np.asarray(exp["values"], np.float32).view(np.uint32))
@@ -238,10 +232,12 @@ def test_forward_collect_with_device_side_action_selection():
 
 
 def test_fused_search_with_reuse_equals_stepwise_drive():
-    """MuZeroMCTSCtree.search_with_reuse (mcts_ctree.py:370-468) as one CUDA graph vs the reference's driver loop restated over
-    the mirror's batch_traverse_with_reuse / batch_backpropagate_with_reuse and the same CUDA model (compacted inference
-    batch, no_inference_lst / reuse_lst built as the driver does): identical visit counts, value bits and inference counts."""
+    """MuZeroMCTSCtree.search_with_reuse (mcts_ctree.py:370-468) as one CUDA graph vs the reference's driver loop
+    (oracle/tree_drive.py) over the mirror's batch_traverse_with_reuse / batch_backpropagate_with_reuse and the same CUDA
+    model (compacted inference batch, no_inference_lst / reuse_lst built as the driver does): identical visit counts,
+    value bits, trajectories and inference counts."""
     from lightzero_b200 import mz_tree
+    from oracle.tree_drive import assert_same, drive, network, readout
     B, A, S = 96, 6, 30
     ref, cu, obs, mask, legal, noises, mcts = _setup(B, A, S, seed=21, masks=True)
     out = cu.initial_inference(obs.cuda())
@@ -251,37 +247,13 @@ def test_fused_search_with_reuse_equals_stepwise_drive():
     roots = mcts.roots(B, legal)
     roots.prepare(0.25, noises, [0.] * B, out.policy_logits, [-1] * B)
     length, avg = mcts.search_with_reuse(roots, cu, out.latent_state, [-1] * B, true_action, reuse_value)
-    fused = (roots.get_distributions(), np.asarray(roots.get_values(), np.float32).view(np.uint32).tolist())
+    fused = readout(roots, A, S)
     roots.clear()
-    # step-wise: the reference loop
-    mz_tree.DEFAULT_MAX_SIMS = max(mz_tree.DEFAULT_MAX_SIMS, S)
-    roots = mz_tree.Roots(B, legal)
-    roots.prepare(0.25, noises, [0.] * B, out.policy_logits, [-1] * B)
-    mm = mz_tree.MinMaxStatsList(B)
-    mm.set_delta(0.01)
-    pool, counts = [out.latent_state], []
-    for s in range(S):
-        res = mz_tree.ResultsWrapper(B)
-        ix, iy, la, vtp = mz_tree.batch_traverse_with_reuse(roots, 19652, 1.25, 0.997, mm, res, [-1] * B, true_action, reuse_value)
-        lat, acts, no_inf, reuse = [], [], [], []
-        for count, (x, y) in enumerate(zip(ix, iy)):
-            if x != -1:
-                lat.append(pool[x][y]); acts.append(la[count])
-            else:
-                no_inf.append(y)
-            if x == 0 and la[count] == true_action[count]:
-                reuse.append(count)
-        counts.append(len(acts))
-        if acts:
-            o = cu.recurrent_inference(torch.stack(lat), torch.tensor(acts), return_scalars=True)
-            pool.append(o.latent_state)
-            r, v, p = o.reward_scalar, o.value_scalar, o.policy_logits
-        else:
-            pool.append([]); r, v, p = [], [], []
-        no_inf.append(-1); reuse.append(-1)
-        mz_tree.batch_backpropagate_with_reuse(s + 1, 0.997, r, v, p, mm, res, vtp, no_inf, reuse, reuse_value)
-    step = (roots.get_distributions(), np.asarray(roots.get_values(), np.float32).view(np.uint32).tolist())
-    assert fused == step
+    c = dict(B=B, A=A, S=S, legal=legal, root_logits=out.policy_logits.cpu().numpy(), noises=noises, to_play=[-1] * B,
+             true_action=true_action, reuse_value=reuse_value)
+    step, _ = drive(mz_tree, c, "reuse", network(cu, out.latent_state))      # the reference loop, step-wise
+    assert_same(step, fused)
+    counts = step["n_inferred"].tolist()
     assert length == counts[-1] and abs(avg - sum(counts) / S) < 1e-9
     assert min(counts) < B       # some trees reused a value instead of calling the network
     assert mcts.last_num_kernels == 1 + 2 * S     # traverse + S x (network, back-up(+traverse))

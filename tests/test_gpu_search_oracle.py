@@ -18,6 +18,7 @@ import numpy as np
 import pytest
 import torch
 
+from oracle.tree_drive import assert_same, drive, network, readout
 from test_gpu_net_layers import make_latents, make_models
 
 pytestmark = pytest.mark.gpu
@@ -118,35 +119,27 @@ def fused_search(cu, mcts, S, latent, legal, logits, noises, tp, cap=None, roots
     if cap is not None:
         roots._materialize(cap)
     mcts.search(roots, cu, latent, tp)
-    res = (roots.get_distributions(), np.asarray(roots.get_values(), np.float32).view(np.uint32).tolist(),
-           roots.get_trajectories())
-    return res, debug_rng(roots), debug_plan(roots, cu, S), roots
+    return readout(roots, logits.shape[1], S), debug_rng(roots), debug_plan(roots, cu, S), roots
 
 
 def oracle_search(cu, S, latent, legal, logits, noises, tp, det, key=None, step0=0, variant=0, discount=0.997, delta=0.01):
-    """The reference loop (mcts_ctree.py:281-368) on the C oracle, with the CUDA network evaluating the leaves"""
+    """The reference loop (mcts_ctree.py:281-368, oracle/tree_drive.py) on the C oracle, with the CUDA network evaluating
+    the leaves; stochastic searches draw ties in hash mode with key = (seed, epoch) from step0"""
     from oracle import ctree_port as port
-    B, A = len(tp), logits.shape[1]
-    roots = port.Roots(B, legal, action_space_size=A, max_sims=S)
-    _prepare(roots, logits.tolist(), noises, tp)
-    if not det:
-        roots.set_tie_hash(key[0], key[1], step0, variant)
-    mm = port.MinMaxStatsList(B)
-    mm.set_delta(delta)
-    pool = torch.empty((S + 1,) + tuple(latent.shape), device="cuda")
-    pool[0] = latent
-    with torch.no_grad():
-        for s in range(S):
-            res = port.ResultsWrapper(B)
-            ix, iy, la, vtp = port.batch_traverse(roots, 19652, 1.25, discount, mm, res, list(tp), det)
-            o = cu.recurrent_inference(pool[torch.tensor(ix, device="cuda"), torch.tensor(iy, device="cuda")],
-                                       torch.tensor(la, device="cuda"), return_scalars=True)
-            pool[s + 1] = o.latent_state
-            port.batch_backpropagate(s + 1, discount, o.reward_scalar.cpu().numpy(), o.value_scalar.cpu().numpy(),
-                                     o.policy_logits.cpu().numpy(), mm, res, vtp)
-    out = (roots.get_distributions(), np.asarray(roots.get_values(), np.float32).view(np.uint32).tolist(),
-           roots.get_trajectories())
-    return out, roots.tie_stats()
+    c = dict(B=len(tp), A=logits.shape[1], S=S, legal=legal, root_logits=logits, noises=noises, to_play=tp,
+             discount=discount, delta=delta)
+    setup = None if det else (lambda r: r.set_tie_hash(key[0], key[1], step0, variant))
+    trace, roots = drive(port, c, "mz", network(cu, latent), det=det, setup=setup)
+    return trace, roots.tie_stats()
+
+
+def visits_sum_to(t, S):
+    return bool((np.maximum(t["distributions"], 0).sum(1) == S).all())
+
+
+def differ(a, b):
+    """per root: different visit counts or root value (the sensitivity tests' disagreement rule)"""
+    return (a["distributions"] != b["distributions"]).any(1) | (a["root_values_bits"] != b["root_values_bits"])
 
 
 def _report(name, st, plan, players, kernels, seconds):
@@ -194,10 +187,8 @@ def test_fused_search_equals_oracle_driving_the_same_network(name):
     kernels = mcts.last_num_kernels
     roots.clear()
     _report(name, st, plan, players, kernels, time.time() - t0)
-    assert got[0] == exp[0], "visit counts"
-    assert got[1] == exp[1], "root value bits"
-    assert got[2] == exp[2], "trajectories"
-    assert all(sum(d) == S for d in got[0])
+    assert_same(got, exp)
+    assert visits_sum_to(got, S)
     # the branch the case is named for
     assert plan["N"] == (cap or S) + 1
     if staging is None:
@@ -237,7 +228,7 @@ def test_mlp_model_multi_kernel_search_equals_oracle():
     kernels = mcts.last_num_kernels
     roots.clear()
     _report("mlp_a4_b96_sto_2p", st, plan, "2p", kernels, 0.0)
-    assert got == exp
+    assert_same(got, exp)
     assert not plan["persistent"] and kernels == 2 * S + 1 and st["draws"] > 0
 
 
@@ -254,7 +245,8 @@ def test_discount_and_value_delta_max():
     default, _ = oracle_search(cu, S, latent, legal, logits, noises, tp, False, key=key)
     roots.clear()
     _report("a9_b96_sto_2p_discount0.9_delta0.05", st, plan, "2p", mcts.last_num_kernels, 0.0)
-    assert got == exp and got[0] != default[0]
+    assert_same(got, exp)
+    assert not np.array_equal(got["distributions"], default["distributions"])
     assert plan["persistent"] and st["draws"] > 0
 
 
@@ -275,9 +267,9 @@ def test_repeated_stochastic_searches_on_one_pooled_tree():
     roots.clear()
     for got, key in ((first, key1), (second, key2)):
         exp, st = oracle_search(cu, S, latent, legal, logits, noises, tp, False, key=key)
-        assert got == exp
+        assert_same(got, exp)
     _report("a18_b200_sto_repeated", st, plan, "1p", mcts.last_num_kernels, 0.0)
-    assert first[0] != second[0]
+    assert not np.array_equal(first["distributions"], second["distributions"])
 
 
 def test_sensitivity_of_the_stochastic_comparison():
@@ -292,10 +284,10 @@ def test_sensitivity_of_the_stochastic_comparison():
     got, key, plan, roots = fused_search(cu, mcts, S, latent, legal, logits, noises, tp)
     roots.clear()
     exp, _ = oracle_search(cu, S, latent, legal, logits, noises, tp, False, key=key)
-    assert got == exp
+    assert_same(got, exp)
 
     def frac(o):
-        return np.mean([g != e or gv != ev for g, e, gv, ev in zip(got[0], o[0], got[1], o[1])])
+        return float(differ(got, o).mean())
     fr = {
         "epoch+1": frac(oracle_search(cu, S, latent, legal, logits, noises, tp, False, key=(key[0], key[1] + 1))[0]),
         "step+1": frac(oracle_search(cu, S, latent, legal, logits, noises, tp, False, key=key, step0=1)[0]),

@@ -71,16 +71,11 @@ def test_golden_fixtures_present():
 
 
 def test_golden_fixtures_reproduce_from_reference():
+    from oracle.tree_drive import check_fixture
     ref = _ref()
-    gen, files = _golden()
+    _, files = _golden()
     for f in files:
-        d = dict(np.load(f))
-        got = gen.replay(ref, d)
-        for k in gen.EXPECTED:
-            e = d["exp_" + k]
-            g = np.asarray(got[k], e.dtype)
-            assert np.array_equal(g.view(np.uint32) if e.dtype == np.float32 else g,
-                                  e.view(np.uint32) if e.dtype == np.float32 else e), (f, k)
+        check_fixture(ref, np.load(f))
 
 
 def test_logf_matches_libm(tmp_path):

@@ -4,13 +4,14 @@ In hash mode a non-deterministic descent draws from the reference's tie list (cn
 counter-based hash, r = mix64(seed ^ mix64(epoch) ^ mix64((b << 32) | step) ^ depth) % len(ties), instead of rand().
 Given the seed, epoch and step the device used, the oracle then judges the device's stochastic searches bit for bit.
 
-`tie_rich_case` / `tie_drive` are shared with the GPU tests (test_gpu_tree.py, test_gpu_search_oracle.py): quantized
-logits, rewards and values make exact and near ties common at every depth."""
+`tie_rich_case` is shared with the GPU tests (test_gpu_tree.py): quantized logits, rewards and values make exact and near
+ties common at every depth."""
 import numpy as np
 import pytest
 
 from oracle import ctree_port as port
 from oracle import ctree_port_ez as port_ez
+from oracle.tree_drive import assert_same, drive, recorded
 
 M64 = 2 ** 64 - 1
 
@@ -40,65 +41,15 @@ def tie_rich_case(B, A, S, seed, masks=True, two_p=False):
     def q(shape, lo, hi, step):
         return (rng.integers(lo, hi + 1, shape) * step).astype(np.float32)
     return dict(B=B, A=A, S=S, legal=legal, root_logits=q((B, A), -1, 1, 0.5), rewards=q((S, B), -1, 1, 0.25),
-                values=q((S, B), -2, 2, 0.25), policies=q((S, B, A), -1, 1, 0.5),
+                values_in=q((S, B), -2, 2, 0.25), policies=q((S, B, A), -1, 1, 0.5), lstm_horizon_len=3,
                 to_play=(rng.integers(1, 3, B) if two_p else np.full(B, -1)).astype(np.int32).tolist(),
                 true_action=[int(l[rng.integers(len(l))]) for l in legal], reuse_value=q((B,), -2, 2, 0.25).tolist())
 
 
-def tie_drive(mod, make_roots, c, kind="mz", det=False, setup=None, horizon=3):
-    """The reference driver loops (mcts_ctree.py:267-368, 370-468, 729-876, 878-1003) on tree module `mod` with the
-    recorded network outputs of case `c`.  kind: 'mz', 'ez', 'reuse' or 'ez_reuse'.  setup(roots) runs after prepare.
-    Returns the per-simulation (ix, iy, last_action, search_len, virtual_to_play), the visit counts, the root value bits,
-    the trajectories and the roots."""
-    B, A, S = c["B"], c["A"], c["S"]
-    ez, reuse = kind in ("ez", "ez_reuse"), kind in ("reuse", "ez_reuse")
-    roots = make_roots(B, c["legal"], A, S)
-    roots.prepare_no_noise([0.] * B, c["root_logits"].tolist(), c["to_play"])
-    if setup is not None:
-        setup(roots)
-    mm = mod.MinMaxStatsList(B)
-    mm.set_delta(0.01)
-    trace = []
-    for s in range(S):
-        res = mod.ResultsWrapper(B)
-        tp = list(c["to_play"])
-        if reuse:
-            ix, iy, la, vtp = mod.batch_traverse_with_reuse(roots, 19652, 1.25, 0.997, mm, res, tp, c["true_action"],
-                                                            c["reuse_value"])
-        elif ez:
-            ix, iy, la, vtp = mod.batch_traverse(roots, 19652, 1.25, 0.997, mm, res, tp)
-        else:
-            ix, iy, la, vtp = mod.batch_traverse(roots, 19652, 1.25, 0.997, mm, res, tp, det)
-        slen = list(res.get_search_len())
-        trace.append((list(ix), list(iy), list(la), slen, list(vtp)))
-        r, v, p = c["rewards"][s], c["values"][s], c["policies"][s]
-        reset = (np.asarray(slen) % horizon == 0).astype(np.int32).tolist()
-        if reuse:     # compacted inference batch, no_inference_lst / reuse_lst as the driver builds them
-            keep, no_inf, reuse_lst = [], [], []
-            for k, (x, y) in enumerate(zip(ix, iy)):
-                if x != -1:
-                    keep.append(k)
-                else:
-                    no_inf.append(y)
-                if x == 0 and la[k] == c["true_action"][k]:
-                    reuse_lst.append(k)
-            args = (s + 1, 0.997, r[keep].tolist(), v[keep].tolist(), p[keep].tolist(), mm, res)
-            tail = (vtp, no_inf + [-1], reuse_lst + [-1], c["reuse_value"])
-            if ez:
-                mod.batch_backpropagate_with_reuse(*args, reset, *tail)
-            else:
-                mod.batch_backpropagate_with_reuse(*args, *tail)
-        elif ez:
-            mod.batch_backpropagate(s + 1, 0.997, r.tolist(), v.tolist(), p.tolist(), mm, res, reset, vtp)
-        else:
-            mod.batch_backpropagate(s + 1, 0.997, r.tolist(), v.tolist(), p.tolist(), mm, res, vtp)
-    vals = np.asarray(roots.get_values(), np.float32).view(np.uint32).tolist()
-    return trace, roots.get_distributions(), vals, roots.get_trajectories(), roots
-
-
-def port_roots(kind):
+def port_drive(kind, c, **kw):
+    """tree_drive.drive on the port with the recorded outputs of case `c`"""
     mod = port_ez if kind in ("ez", "ez_reuse") else port
-    return mod, (lambda B, legal, A, S: mod.Roots(B, legal, action_space_size=A, max_sims=S))
+    return drive(mod, c, kind, recorded(c, kind), **kw)
 
 
 KINDS = ["mz", "ez", "reuse", "ez_reuse"]
@@ -109,16 +60,15 @@ KINDS = ["mz", "ez", "reuse", "ez_reuse"]
 def test_hash_that_draws_zero_equals_deterministic_mode(kind, two_p):
     """Hash mode with r forced to 0 takes the first tie like the deterministic rule: bit-identical traces and results.
     The unforced hash mode must leave the deterministic path on these tie-rich inputs."""
-    mod, mk = port_roots(kind)
     c = tie_rich_case(64, 7, 40, 11 + two_p, two_p=two_p)
-    det = tie_drive(mod, mk, c, kind, det=True)[:4]
-    zero = tie_drive(mod, mk, c, kind, setup=lambda r: r.set_tie_hash(0x5eed5eed, 3, 0, variant=1))
-    assert zero[:4] == det
-    st = zero[4].tie_stats()
+    det, _ = port_drive(kind, c, det=True)
+    zero, roots = port_drive(kind, c, det=False, setup=lambda r: r.set_tie_hash(0x5eed5eed, 3, 0, variant=1))
+    assert_same(zero, det)
+    st = roots.tie_stats()
     assert st["ties"] > 100 and st["draws"] == 0 and st["near"] == 0
-    drawn = tie_drive(mod, mk, c, kind, setup=lambda r: r.set_tie_hash(0x5eed5eed, 3, 0))
-    assert drawn[4].tie_stats()["draws"] > 50
-    assert drawn[1] != det[1]
+    drawn, roots = port_drive(kind, c, det=False, setup=lambda r: r.set_tie_hash(0x5eed5eed, 3, 0))
+    assert roots.tie_stats()["draws"] > 50
+    assert not np.array_equal(drawn["distributions"], det["distributions"])
 
 
 def test_hash_draw_is_the_device_formula():
