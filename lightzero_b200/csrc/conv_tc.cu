@@ -16,7 +16,15 @@
 
 namespace lz {
 
-constexpr int kCvConsumers = 256, kCvThreads = kCvConsumers + 32;   // two MMA / epilogue warpgroups + the producer warp
+// Two MMA / epilogue warpgroups + the producer, in one of two layouts (the kernels' Wide parameter):
+//   narrow: a single producer warp, 288 threads.  They are allocated registers as 12 warps, which caps every thread at 168.
+//   wide:   a whole producer warpgroup, 384 threads, that hands its registers to the MMA warpgroups (kProducerRegs /
+//           kConsumerRegs, tc_ptx.cuh), which then hold more accumulator slabs.
+// The wide layout only pays where a plan's tiles need more slabs than the narrow one holds: a launch whose tile groups would not
+// grow measured 1-4 % slower in it (H100 80GB HBM3, 700 W), so each launch picks the layout from its plan (conv_tc_launch, rb_wide).
+constexpr int kCvConsumers = 256;
+template <bool Wide>
+constexpr int kCvThreads = kCvConsumers + (Wide ? 128 : 32);
 constexpr int kCvStages = 4;          // ring slots reserved in the barrier block; p.stages (2..4) are used
 
 struct CvBars {
@@ -122,14 +130,14 @@ __device__ __forceinline__ void tc_group(float (&acc)[MT][N / 2], int nt, TapA t
     if (lane == 0) mbar_arrive(&empty[(n0 + 8) % nstages]);
 }
 
-// Tiles in flight per warpgroup (accumulator slabs of N / 2 registers each): one.  N = 64 stays within 112 registers, so two CTAs
-// share an SM and one CTA's band load and epilogue overlap the other's MMAs.  N = 128 runs one CTA per SM at the 168-register cap
-// of 288 threads; two slabs (128 accumulators) spill in the epilogue (CUDA 12.9).
-template <int N>
-constexpr int kCvTiles = 1;
+// Tiles in flight per warpgroup (accumulator slabs of N / 2 registers each).  Narrow: one.  N = 64 stays within 112 registers, so two
+// CTAs share an SM and one CTA's band load and epilogue overlap the other's MMAs; N = 128 runs one CTA per SM.  Wide (N = 128 only):
+// two slabs (128 accumulators, which spilled in the epilogue at 168 registers, CUDA 12.9), for bands of two or more tiles.
+template <bool Wide>
+constexpr int kCvTiles = Wide ? 2 : 1;
 
-template <int N>
-__global__ void __launch_bounds__(kCvThreads, N == 128 ? 1 : 2) k_conv_tc(ConvTc p)
+template <int N, bool Wide>
+__global__ void __launch_bounds__(kCvThreads<Wide>, N == 128 ? 1 : 2) k_conv_tc(ConvTc p)
 {
     extern __shared__ __align__(1024) unsigned char smem[];
     const CvGeom g = cv_geom(p);
@@ -143,7 +151,7 @@ __global__ void __launch_bounds__(kCvThreads, N == 128 ? 1 : 2) k_conv_tc(ConvTc
     const int img0 = group * p.G, nimg = min(p.G, p.B - img0);
     const int y0 = band * p.band_h;
     const int rin0 = y0 * pitch - 1;
-    constexpr int MT = kCvTiles<N>;
+    constexpr int MT = kCvTiles<Wide>;
     int ng, per;
     tile_groups(g.NT, MT, ng, per);
 
@@ -154,9 +162,10 @@ __global__ void __launch_bounds__(kCvThreads, N == 128 ? 1 : 2) k_conv_tc(ConvTc
     }
     __syncthreads();
 
-    if (warp == kCvConsumers / 32) {
+    if (warp >= kCvConsumers / 32) {
         // ================= producer: input band, then the 9 weight taps once per tile group =================
-        if (lane == 0) {
+        if constexpr (Wide) wg_reg_dealloc<kProducerRegs>();
+        if (warp == kCvConsumers / 32 && lane == 0) {
             const int grow0 = rin0 + 1;                                    // memory row of rho = rin0
             const int ncopy = min(g.rin, p.in.plane_rows - grow0);
             const uint32_t bytes = (uint32_t)ncopy * 16u;
@@ -181,6 +190,7 @@ __global__ void __launch_bounds__(kCvThreads, N == 128 ? 1 : 2) k_conv_tc(ConvTc
     }
 
     // ================= two warpgroups: rows [64 wg, 64 wg + 64) of every tile =================
+    if constexpr (Wide) wg_reg_alloc<kConsumerRegs>();
     const int wg = warp >> 2;
     const uint32_t plane16 = (uint32_t)(g.plane >> 4);
     const uint64_t a_desc0 = make_desc(smem_u32(in_s), plane16, 8);
@@ -282,14 +292,21 @@ __host__ __device__ inline RbGeom rb_geom(const ResBlockTc &p)
 }
 
 // Tiles in flight per warpgroup: the accumulator slabs (N / 2 registers each) of a whole conv at N = 32 (84-px resblocks1: NT1 = 6,
-// NT2 = 5; 96 registers, 151 in all), two slabs at N = 64 (three or four spill in the epilogue at the 168-register cap of 288
-// threads, CUDA 12.9).  The kernel runs one CTA per SM (~200 KB of shared memory), so only independent chains within the CTA hide
-// wgmma latency.
-template <int N>
-constexpr int kRbTiles = N == 32 ? 6 : 2;
+// NT2 = 5; 151 registers, narrow), two slabs at N = 64 narrow and four wide (128 accumulators; three or four spilled in the epilogue
+// at 168 registers, CUDA 12.9).  The kernel runs one CTA per SM (~200 KB of shared memory), so only independent chains within the
+// CTA hide wgmma latency.
+template <int N, bool Wide>
+constexpr int kRbTiles = N == 32 ? 6 : (Wide ? 4 : 2);
 
-template <int N>
-__global__ void __launch_bounds__(kCvThreads, 1) k_resblock_tc(ResBlockTc p)
+// The slabs a ResBlock plan runs with: the wide layout once a conv has more tiles than the narrow one holds (N = 64 only)
+__host__ __device__ inline bool rb_wide(int C, const RbGeom &g) { return C == 64 && (g.NT1 > kRbTiles<64, false> || g.NT2 > kRbTiles<64, false>); }
+__host__ __device__ inline int rb_tiles(int C, const RbGeom &g)
+{
+    return C == 32 ? kRbTiles<32, false> : (rb_wide(C, g) ? kRbTiles<64, true> : kRbTiles<64, false>);
+}
+
+template <int N, bool Wide>
+__global__ void __launch_bounds__(kCvThreads<Wide>, 1) k_resblock_tc(ResBlockTc p)
 {
     extern __shared__ __align__(1024) unsigned char smem[];
     const RbGeom g = rb_geom(p);
@@ -301,7 +318,7 @@ __global__ void __launch_bounds__(kCvThreads, 1) k_resblock_tc(ResBlockTc p)
     const int group = blockIdx.x / g.nbands, band = blockIdx.x - group * g.nbands;
     const int img0 = group * p.G, nimg = min(p.G, p.B - img0);
     const int y0 = band * p.band_h;
-    constexpr int MT = kRbTiles<N>;
+    constexpr int MT = kRbTiles<N, Wide>;
     int ng1, per1, ng2, per2;
     tile_groups(g.NT1, MT, ng1, per1);
     tile_groups(g.NT2, MT, ng2, per2);
@@ -314,9 +331,10 @@ __global__ void __launch_bounds__(kCvThreads, 1) k_resblock_tc(ResBlockTc p)
     }
     __syncthreads();
 
-    if (warp == kCvConsumers / 32) {
+    if (warp >= kCvConsumers / 32) {
         // ================= producer: the first ring fill, the input band chunk by chunk, then conv1's and conv2's taps =================
-        if (lane == 0) {
+        if constexpr (Wide) wg_reg_dealloc<kProducerRegs>();
+        if (warp == kCvConsumers / 32 && lane == 0) {
             auto load_tap = [&](int n) {
                 const int st = n % nstages, tap = n % 9;
                 if (n >= nstages) mbar_wait(&bars->empty[st], ((n / nstages) - 1) & 1);
@@ -349,6 +367,7 @@ __global__ void __launch_bounds__(kCvThreads, 1) k_resblock_tc(ResBlockTc p)
     }
 
     // ================= two warpgroups: rows [64 wg, 64 wg + 64) of every tile =================
+    if constexpr (Wide) wg_reg_alloc<kConsumerRegs>();
     const int wg = warp >> 2;
     const uint32_t plane16 = (uint32_t)(g.plane >> 4);
     const uint64_t in_desc = make_desc(smem_u32(in_s), plane16, 8), mid_desc = make_desc(smem_u32(mid_s), plane16, 8);
@@ -526,10 +545,12 @@ __global__ void k_tcl_to_nchw(Tcl in, float *out_nchw, int B)
 int conv_tc_prepare_launch()
 {
     const int big = 227 * 1024;
-    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
-    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
-    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_resblock_tc<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
-    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_resblock_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
+    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
+    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
+    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
+    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_resblock_tc<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
+    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_resblock_tc<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
+    LZ_CUDA_CHECK(cudaFuncSetAttribute(k_resblock_tc<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, big));
     return LZ_OK;
 }
 
@@ -541,9 +562,13 @@ int conv_tc_launch(const ConvTc &p, cudaStream_t s)
     LZ_REQUIRE(p.out[0].nphase == 1 && (p.N < 128 || p.out[1].nphase == 1), LZ_EINVAL, "conv_tc: phase-split output is not supported");
     const int groups = (p.B + p.G - 1) / p.G;
     const int grid = groups * g.nbands;
+    // N = 128: the wide layout for bands of two or more tiles (two slabs); a one-tile band gains nothing from it
     switch (p.N) {
-        case 64: k_conv_tc<64><<<grid, kCvThreads, g.smem, s>>>(p); break;
-        case 128: k_conv_tc<128><<<grid, kCvThreads, g.smem, s>>>(p); break;
+        case 64: k_conv_tc<64, false><<<grid, kCvThreads<false>, g.smem, s>>>(p); break;
+        case 128:
+            if (g.NT > kCvTiles<false>) k_conv_tc<128, true><<<grid, kCvThreads<true>, g.smem, s>>>(p);
+            else k_conv_tc<128, false><<<grid, kCvThreads<false>, g.smem, s>>>(p);
+            break;
         default: LZ_REQUIRE(false, LZ_EINVAL, "conv_tc: N must be 64 or 128");
     }
     LZ_KERNEL_CHECK();
@@ -551,10 +576,17 @@ int conv_tc_launch(const ConvTc &p, cudaStream_t s)
 }
 
 // Scores useful output rows (both convs) over issued MMA rows, which count conv1's halo recompute and the 128-row tile padding of
-// both convs.  A band of ~200 KB leaves room for one CTA per SM, so there is no co-residency term as in the plain conv's picker.
+// both convs.  A band of ~200 KB leaves room for one CTA per SM, so there is no co-residency term as in the plain conv's picker;
+// instead a conv of several tiles whose tile groups (rb_tiles) leave one tile on its own is marked down: that group runs its 9 taps
+// on a single accumulator chain per warpgroup.
 int resblock_tc_plan(ResBlockTc &p)
 {
     const int H = p.in.H, W = p.in.W;
+    auto lone_tile = [](int NT, int MT) {
+        int ng, per;
+        tile_groups(NT, MT, ng, per);
+        return NT > 1 && NT - (ng - 1) * per == 1;
+    };
     ResBlockTc q = p;
     double best = -1.0;
     for (int G = 1; G <= 4; ++G)
@@ -565,6 +597,9 @@ int resblock_tc_plan(ResBlockTc &p)
                 if (g.smem > 227 * 1024 || g.nchunk > kRbChunks) continue;
                 double score = (double)(2 * G * H * W) / ((double)g.nbands * (g.NT1 + g.NT2) * 128);
                 score *= (st == 4) ? 1.0 : 0.97;
+                const int MT = rb_tiles(p.in.C, g);
+                if (lone_tile(g.NT1, MT)) score *= 0.9;
+                if (lone_tile(g.NT2, MT)) score *= 0.9;
                 if (score > best + 1e-9) { best = score; p.G = G; p.band_h = bh; p.stages = st; }
             }
     LZ_REQUIRE(best > 0.0, LZ_EINVAL, "resblock_tc: no band of a %dx%d, %d-channel block fits shared memory", H, W, p.in.C);
@@ -578,8 +613,11 @@ int resblock_tc_launch(const ResBlockTc &p, cudaStream_t s)
     LZ_REQUIRE(p.in.nphase == 1 && p.out.C == p.in.C, LZ_EINVAL, "resblock_tc: unsupported input / output layout");
     const int grid = (p.B + p.G - 1) / p.G * g.nbands;
     switch (p.in.C) {
-        case 32: k_resblock_tc<32><<<grid, kCvThreads, g.smem, s>>>(p); break;
-        case 64: k_resblock_tc<64><<<grid, kCvThreads, g.smem, s>>>(p); break;
+        case 32: k_resblock_tc<32, false><<<grid, kCvThreads<false>, g.smem, s>>>(p); break;
+        case 64:
+            if (rb_wide(64, g)) k_resblock_tc<64, true><<<grid, kCvThreads<true>, g.smem, s>>>(p);
+            else k_resblock_tc<64, false><<<grid, kCvThreads<false>, g.smem, s>>>(p);
+            break;
         default: LZ_REQUIRE(false, LZ_EINVAL, "resblock_tc: channels must be 32 or 64");
     }
     LZ_KERNEL_CHECK();

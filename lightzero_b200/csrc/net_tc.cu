@@ -23,15 +23,17 @@
 // fp32 staging array (one row per thread, as the epilogue is written).  The ResBlock skip tensors are parked in an L2-resident
 // scratch (thread-private rows, .cg accesses).
 //
-// Warp roles (288 threads): warps 0-7 = two consumer warpgroups (MMA issue, epilogues, heads, trees; warp w's read-out rows are
-// 32*(w%4).. of a tile, its columns the 32-column half w/4), warp 8 lane 0 = weight producer (cp.async.bulk global->shared ring,
-// mbarrier complete_tx; every consumer warp releases a slot once its MMAs have read it).
+// Warp roles (384 threads): warps 0-7 = two consumer warpgroups (MMA issue, epilogues, heads, trees; warp w's read-out rows are
+// 32*(w%4).. of a tile, its columns the 32-column half w/4), warps 8-11 = the producer warpgroup, which gives its registers to the
+// consumers (setmaxnreg); warp 8 lane 0 is the weight producer (cp.async.bulk global->shared ring, mbarrier complete_tx; every
+// consumer warp releases a slot once its MMAs have read it).
 #include <cuda_fp16.h>
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "model.cuh"
 #include "net_tc.cuh"
@@ -44,7 +46,7 @@ namespace lz {
 
 // ---------------------------------------------------------------------------------------------- geometry
 constexpr int kEpiWarps = 8, kEpiThreads = kEpiWarps * 32;   // two consumer warpgroups
-constexpr int kTcThreads = kEpiThreads + 32;                 // + the weight producer warp
+constexpr int kTcThreads = kEpiThreads + 128;                // + the producer warpgroup (its warp 8 streams the weights)
 constexpr int kMaxTiles = 3;                     // 384 output rows: 3 tiles of 128 (the register accumulator budget)
 constexpr int kTapKgBytes = 128 * 16;            // one k-group (8 input channels) of a tap: 64 hi rows then 64 lo rows of 16 B
 constexpr int kTapBytes = 8 * kTapKgBytes;       // one 3x3 tap, [kg 8][co: 64 hi | 64 lo][ci % 8]: 16384 B
@@ -407,8 +409,9 @@ __device__ __forceinline__ void ptree_unpark(PTree &T, const uint32_t *w, int la
     T.my_legal = (int)w[16 + lane]; T.my_pslot = (int)w[48 + lane]; T.my_pact = (int)w[80 + lane];
 }
 
-// One CTA per SM (~225 KB of shared memory).  Its 9 warps spread over the SM's four register-file quarters of 16,384 registers, three
-// in one of them, which caps the kernel at 168 registers: ptxas spills some of the epilogue state (not the accumulators).
+// One CTA per SM (~225 KB of shared memory).  Its 12 warps are launched with 168 registers each (three per register-file quarter of
+// 16,384); the producer warpgroup drops to kProducerRegs and the consumer warpgroups rise to kConsumerRegs (tc_ptx.cuh), so the
+// tree, epilogue and head code keeps its state in registers (at 168 for every thread, ptxas spilled some of it).
 // HW: the latent grid (TcGeo); one instantiation per grid, chosen by tc_launch from TcNet::hw.
 template <int HW>
 __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, TreeParams tp)
@@ -427,7 +430,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
     float *stg = reinterpret_cast<float *>(headw + kHeadWBytes + 1024 + kBnSmemBytes);   // [128 rows][kStgLd] accumulator staging
 
     // warp index as a warp-UNIFORM value (shuffle broadcast): the role branches below become uniform branches
-    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
+    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
     const int R = io.roots_per_cta;
     const int root0 = blockIdx.x * R;
     const int nvalid = min(R, io.B - root0);                     // roots of this CTA that exist
@@ -482,9 +485,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
     fence_proxy_async();
     __syncthreads();
 
-    if (warp == kEpiWarps) {
+    if (warp >= kEpiWarps) {
         // ================= weight producer =================
-        if (lane == 0) {
+        wg_reg_dealloc<kProducerRegs>();
+        if (warp == kEpiWarps && (tid & 31) == 0) {
             uint32_t n = 0;
             auto stage_in = [&](const unsigned char *src, uint32_t bytes = kTapBytes) {      // every stage is released by all consumer warps
                 const int st = n % kStages;
@@ -512,6 +516,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
 
     // ================= consumer warpgroups: warpgroup wg issues the MMAs of rows [64 wg, 64 wg + 64) of every tile; for the
     // read-outs warp w owns staged rows 32*(w%4).. and the 32-column half w/4 =================
+    wg_reg_alloc<kConsumerRegs>();
+    const int lane = lane_id();          // read after the reallocation: a value live across it is kept in local memory by ptxas
     const int wg = warp >> 2;
     const int q4 = warp & 3, half = warp >> 2, rowid = q4 * 32 + lane;
     const uint32_t act_s = smem_u32(act), ring_s = smem_u32(ring), headw_s = smem_u32(headw);
@@ -739,23 +745,34 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
                     wg_fence_acc(hr[t]);
                     wg_fence_acc(hv[t]);
                 }
-                wg_fence();
+                // straight-line issue blocks, as in the 3x3 loop: all three tiles (rows past the loaded ones are never read back), the
+                // heads and the pass count hoisted out, so that no branch separates the wgmma of the commit group
+                auto hook_mma = [&](auto rew, auto vp, auto np) {
 #pragma unroll
-                for (int t = 0; t < kMaxTiles; ++t) {
-                    if (t >= NT) continue;
-                    const uint32_t arow = act_s + (uint32_t)(kMargin + t * 128 + wg * 64) * 16u;
-                    for (int ps = 0; ps < npass; ++ps) {
-                        const uint32_t apart = (ps == 2) ? kPartBytes : 0;
+                    for (int t = 0; t < kMaxTiles; ++t) {
+                        const uint32_t arow = act_s + (uint32_t)(kMargin + t * 128 + wg * 64) * 16u;
 #pragma unroll
-                        for (int ks = 0; ks < 4; ++ks) {
-                            const uint64_t ad = make_desc(arow + apart + ks * 2 * kPlaneBytes, a_lbo, 8);
-                            if (hook_rew)      // reward head: N = 16, [kg][16 co][8]
-                                wgmma_n16(hr[t], ad, make_desc(headw_s + ((ps == 1) ? 2048 : 0) + ks * 512, 16, 8));
-                            if (hook_vp)       // value + policy heads as one N = 32 matrix, [kg][32 co][8]
-                                wgmma_n32(hv[t], ad, make_desc(headw_s + 4096 + ((ps == 1) ? 4096 : 0) + ks * 1024, 32, 8));
+                        for (int ps = 0; ps < decltype(np)::value; ++ps) {
+                            const uint32_t apart = (ps == 2) ? kPartBytes : 0;
+#pragma unroll
+                            for (int ks = 0; ks < 4; ++ks) {
+                                const uint64_t ad = make_desc(arow + apart + ks * 2 * kPlaneBytes, a_lbo, 8);
+                                if constexpr (decltype(rew)::value)      // reward head: N = 16, [kg][16 co][8]
+                                    wgmma_n16(hr[t], ad, make_desc(headw_s + ((ps == 1) ? 2048 : 0) + ks * 512, 16, 8));
+                                if constexpr (decltype(vp)::value)       // value + policy heads as one N = 32 matrix, [kg][32 co][8]
+                                    wgmma_n32(hv[t], ad, make_desc(headw_s + 4096 + ((ps == 1) ? 4096 : 0) + ks * 1024, 32, 8));
+                            }
                         }
                     }
-                }
+                };
+                auto hook_heads = [&](auto np) {
+                    if (hook_rew && hook_vp) hook_mma(std::true_type(), std::true_type(), np);
+                    else if (hook_rew) hook_mma(std::true_type(), std::false_type(), np);
+                    else hook_mma(std::false_type(), std::true_type(), np);
+                };
+                wg_fence();
+                if (npass == 3) hook_heads(std::integral_constant<int, 3>());
+                else hook_heads(std::integral_constant<int, 1>());
                 wg_commit();
                 wg_wait<0>();
 #pragma unroll

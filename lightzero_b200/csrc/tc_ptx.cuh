@@ -44,6 +44,22 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t by
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory"); }
 
+// ---- register reallocation (sm_90a): a warpgroup lowers or raises its per-thread register count; all four of its warps execute
+// the same instruction (.sync.aligned).  A producer warpgroup that only issues bulk copies gives its registers to the MMA warpgroups:
+// per SM sub-partition (one warp of each of the three warpgroups) 40 + 2 x 232 = 504 <= 512 registers per lane, the 168 x 3 that a
+// 384-thread block is launched with.
+template <int R>
+__device__ __forceinline__ void wg_reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void wg_reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(R)); }
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+__device__ __forceinline__ int lane_id()
+{
+    int l;
+    asm volatile("mov.u32 %0, %%laneid;\n" : "=r"(l));
+    return l;
+}
+
 // ---- wgmma (sm_90a): D[64 x N] (+)= A[64 x 16] * B[16 x N], fp16 inputs from shared-memory descriptors, fp32 accumulators in the
 // registers of the issuing warpgroup.  Accumulator fragment of thread (warp w of the warpgroup, lane l): d[4 j + {0, 1}] = row
 // 16 w + l / 4, columns 8 j + 2 (l % 4) + {0, 1}; d[4 j + {2, 3}] = the same columns of row 16 w + l / 4 + 8.
