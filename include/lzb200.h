@@ -187,10 +187,16 @@ typedef struct lz_model_config {
      * LSTM(hc*h*w -> lstm_hidden_size) -> BN1d -> ReLU -> MLP and predicts a VALUE PREFIX; 0 = MuZeroModel */
     int efficientzero;
     int lstm_hidden_size;          /* 512 (must be a multiple of 16, <= 512) */
+    /* 1 = DownSample representation (the Atari network); 0 = the full-resolution board network of downsample=False
+     * (common.py:764-787; tictactoe, connect4, gomoku), every layer at the observation's H x W */
+    int downsample;
 } lz_model_config;
 
-/* Conv models (DownSample representation, common.py:334-366): 84x84 and 96x96 observations give a 6x6 latent grid; 64x64 (the
- * shipped Atari configs) gives 8x8, with no pooling2 (common.py:357-359).  Other sizes: LZ_EINVAL. */
+/* downsample = 1, conv models (DownSample representation, common.py:334-366): 84x84 and 96x96 observations give a 6x6 latent
+ * grid; 64x64 (the shipped Atari configs) gives 8x8, with no pooling2 (common.py:357-359).  Other sizes: LZ_EINVAL.
+ * downsample = 0, board models: latent [num_channels, obs_h, obs_w] with num_channels in {16, 32, 64}, 1 <= obs_h, obs_w <= 8,
+ * 1 <= obs_c <= 16, 1 <= action_space_size <= 64, MuZero only (efficientzero = 0); other configs: LZ_EINVAL.  Same head and
+ * support limits as the conv models.  The uint8 collect entry points take conv models only. */
 int lz_model_create(const lz_model_config *cfg, lz_model **out);
 
 /* MuZeroModelMLP (lzero/model/muzero_model_mlp.py:21-295; vector observations, BASELINE config 1).  The
@@ -241,10 +247,15 @@ int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uin
  * reward / value logits (the joint categorical read-out of the search), then for EfficientZero (`which` 0) the reward-head
  * features [B, reward_head_channels*h*w] the LSTM consumes (h*w = 36 or 64).  Sections a program does not produce are zero.
  * h_info (int32[8]) receives the launch plan: roots per CTA R (<= 8 on the 6x6 grid, <= 4 on 8x8), row tiles NT (<= 3), CTA count, roots of the last CTA, layers of
- * the launched program, MMA passes, 1 if the FC2 biases are staged in shared memory, FC2 tiles. */
+ * the launched program, MMA passes, 1 if the FC2 biases are staged in shared memory, FC2 tiles.
+ * Board models (downsample = 0): `which` 1 is the whole initial_inference program on the observations d_latent
+ * f32 [B,obs_c,H,W]; outputs as above without the EfficientZero section, latents [B,C,H,W]; h_info: roots per CTA R, 64-row tiles
+ * NT, CTA count, roots of the last CTA, layers, MMA passes, shared memory bytes, 0. */
 int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_latent, const int32_t *d_action, int stage,
                              void *d_out, size_t out_bytes, int32_t *h_info, lz_stream s);
-int lz_model_latent_hw(const lz_model *m);   /* 6 for 84/96, 8 for 64 */
+int lz_model_latent_hw(const lz_model *m);   /* 6 for 84/96, 8 for 64; a square board's side; 0 for a non-square board */
+/* Shape of one root's latent: channels, height, width (h_c / h_h / h_w may be NULL).  The MLP model reports (latent_dim, 1, 1). */
+int lz_model_latent_shape(const lz_model *m, int32_t *h_c, int32_t *h_h, int32_t *h_w);
 int lz_model_support_size(const lz_model *m);
 
 /* initial_inference (muzero_model.py:210-240).  d_obs f32 [B,obs_c,H,W].  Outputs (NULL to skip):

@@ -21,7 +21,8 @@ class ModelConfig(ctypes.Structure):
                 ("num_res_blocks", c_int), ("num_channels", c_int), ("reward_head_channels", c_int),
                 ("value_head_channels", c_int), ("policy_head_channels", c_int), ("reward_hidden", c_int),
                 ("value_hidden", c_int), ("policy_hidden", c_int), ("support_min", c_float),
-                ("support_max", c_float), ("support_step", c_float), ("efficientzero", c_int), ("lstm_hidden_size", c_int)]
+                ("support_max", c_float), ("support_step", c_float), ("efficientzero", c_int), ("lstm_hidden_size", c_int),
+                ("downsample", c_int)]
 
 
 class MlpConfig(ctypes.Structure):
@@ -72,6 +73,7 @@ SIGNATURES = {
     "lz_model_debug_net_stage": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, ctypes.c_size_t,
                                          c_void_p, c_void_p]),
     "lz_model_latent_hw": (c_int, [c_void_p]),
+    "lz_model_latent_shape": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "lz_model_support_size": (c_int, [c_void_p]),
     "lz_model_initial_inference": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lz_model_recurrent_inference": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,

@@ -181,9 +181,24 @@ static int model_prepare_launch()
     return LZ_OK;
 }
 
+static BoardIO board_io(const lz_model *m, int B)
+{
+    BoardIO b;
+    memset(&b, 0, sizeof(b));
+    b.B = B; b.npass = m->npass; b.obs_c = m->cfg.obs_c;
+    return b;
+}
+
 int model_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
 {
     if (m->kind == 1) return mlp_recurrent(m, io, s);
+    if (m->kind == 2) {
+        BoardIO b = board_io(m, io.B);
+        b.latent_base = io.latent_base; b.ix = io.ix; b.slot_stride = io.slot_stride; b.action = io.action;
+        b.latent_out = io.next_latent; b.reward = io.reward; b.value = io.value; b.policy_logits = io.policy_logits;
+        b.reward_logits = io.reward_logits; b.value_logits = io.value_logits;
+        return board_launch(m->board_rec, b, s);
+    }
     TcIO t;
     memset(&t, 0, sizeof(t));
     t.B = io.B; t.npass = m->npass;
@@ -255,7 +270,7 @@ int model_reserve(lz_model *m, int B)
         if (rc != LZ_OK) return rc;
         m->ez_B = B;
     }
-    if (m->kind == 1 || B <= m->ws_B) return LZ_OK;
+    if (m->kind != 0 || B <= m->ws_B) return LZ_OK;
     ++m->generation;
     cudaFree(m->pre_latent);
     m->pre_latent = nullptr;
@@ -387,6 +402,12 @@ int model_initial_tail(lz_model *m, int B, const float *pre_latent, const TailIO
 int model_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, cudaStream_t s)
 {
     if (m->kind == 1) return mlp_initial(m, B, d_obs, io_in, s);
+    if (m->kind == 2) {
+        BoardIO b = board_io(m, B);
+        b.obs = d_obs; b.latent_out = io_in.latent; b.latent_out2 = io_in.latent2;
+        b.value = io_in.value; b.policy_logits = io_in.policy_logits; b.value_logits = io_in.value_logits;
+        return board_launch(m->board_init, b, s);
+    }
     LZ_REQUIRE(B <= m->ws_B, LZ_ESTATE, "model_initial: workspace sized for %d roots, got %d (call model_reserve outside capture)", m->ws_B, B);
     int rc = tower_tc_run(m, B, d_obs, m->pre_latent, s);
     if (rc) return rc;
@@ -726,6 +747,116 @@ static int pack_tc(lz_model *m, const Head &reward, const Head &value, const Hea
     return tc_prepare_launch();
 }
 
+// ---- board network tables (board_tc.cu, downsample=False): fp16 hi/lo conv weights, folded BN, action planes, fp32 heads ----
+static int pack_board(lz_model *m)
+{
+    const lz_model_config &c = m->cfg;
+    const int C = c.num_channels, A = c.action_space_size, n = c.num_res_blocks, H = c.obs_h, W = c.obs_w, P = H * W;
+    const std::string D = "dynamics_network.", Q = "prediction_network.", R = "representation_network.";
+    struct Conv { std::string w, bn; int cin_total, cin_used, cin_pad; };
+    // conv indices: 0 dyn conv | 1..2n dyn blocks | 2n+1..4n pred blocks | 4n+1..6n rep blocks | 6n+1 rep conv
+    std::vector<Conv> convs;
+    convs.push_back({D + "conv.weight", D + "norm_common", C + A, C, C});
+    for (const std::string &pre : {D, Q, R})
+        for (int i = 0; i < n; ++i) {
+            const std::string b = pre + "resblocks." + std::to_string(i);
+            convs.push_back({b + ".conv1.0.weight", b + ".conv1.1", C, C, C});
+            convs.push_back({b + ".conv2.0.weight", b + ".conv2.1", C, C, C});
+        }
+    convs.push_back({R + "conv.weight", R + "norm", c.obs_c, c.obs_c, 16});   // observation planes padded to 16 with zero weights
+    const int nconv = (int)convs.size();
+    auto align = [](size_t v) { return (v + 127) & ~(size_t)127; };
+    std::vector<size_t> woff(nconv);
+    size_t off = 0;
+    for (int i = 0; i < nconv; ++i) { woff[i] = off; off += (size_t)9 * convs[i].cin_pad * C * 4; }
+    const size_t off_bn = align(off), off_ab = align(off_bn + (size_t)nconv * 2 * C * 4), off_heads = align(off_ab + (size_t)A * C * P * 4);
+    std::vector<unsigned char> host(off_heads, 0);
+    float *bn = reinterpret_cast<float *>(host.data() + off_bn), *ab = reinterpret_cast<float *>(host.data() + off_ab);
+    for (int ci = 0; ci < nconv; ++ci) {
+        const Conv &cv = convs[ci];
+        auto w = find(m, cv.w, (size_t)C * cv.cin_total * 9);
+        std::vector<float> scale, shift;
+        if (!w || !fold_bn(m, cv.bn, C, scale, shift)) return LZ_EINVAL;
+        const float ws = board_pack_conv3(w->data(), C, cv.cin_total, cv.cin_used, cv.cin_pad, host.data() + woff[ci]);
+        for (int k = 0; k < C; ++k) { bn[ci * 2 * C + k] = scale[k] / ws; bn[ci * 2 * C + C + k] = shift[k]; }
+        if (ci == 0)      // one-hot action planes (muzero_model.py:341-369): border-aware tap sums, times the BN scale
+            for (int a = 0; a < A; ++a)
+                for (int co = 0; co < C; ++co)
+                    for (int y = 0; y < H; ++y)
+                        for (int x = 0; x < W; ++x) {
+                            double acc = 0.0;
+                            for (int t = 0; t < 9; ++t) {
+                                const int yy = y + t / 3 - 1, xx = x + t % 3 - 1;
+                                if (yy >= 0 && yy < H && xx >= 0 && xx < W) acc += (*w)[((size_t)co * cv.cin_total + C + a) * 9 + t];
+                            }
+                            ab[((size_t)a * C + co) * P + y * W + x] = (float)acc * scale[co];
+                        }
+    }
+    // heads: fp32 tables (conv bias folded into the 1x1 BN shift, Linear bias into the BN1d shift)
+    struct HD { std::string conv, norm, fc; int hc, hid, K; };
+    const HD heads[3] = {{D + "conv1x1_reward", D + "norm_reward", D + "fc_reward_head", c.reward_head_channels, c.reward_hidden, m->K},
+                         {Q + "conv1x1_value", Q + "norm_value", Q + "fc_value", c.value_head_channels, c.value_hidden, m->K},
+                         {Q + "conv1x1_policy", Q + "norm_policy", Q + "fc_policy", c.policy_head_channels, c.policy_hidden, A}};
+    Packer hp;
+    size_t hoff[3][8];
+    for (int h = 0; h < 3; ++h) {
+        const HD &d = heads[h];
+        const int nin = d.hc * P;
+        auto w1 = find(m, d.conv + ".weight", (size_t)d.hc * C), b1 = find(m, d.conv + ".bias", d.hc);
+        auto W0 = find(m, d.fc + ".0.weight", (size_t)d.hid * nin), B0 = find(m, d.fc + ".0.bias", d.hid);
+        auto W3 = find(m, d.fc + ".3.weight", (size_t)d.K * d.hid), B3 = find(m, d.fc + ".3.bias", d.K);
+        std::vector<float> s1, t1, s2, t2;
+        if (!w1 || !b1 || !W0 || !B0 || !W3 || !B3 || !fold_bn(m, d.norm, d.hc, s1, t1) || !fold_bn(m, d.fc + ".1", d.hid, s2, t2))
+            return LZ_EINVAL;
+        for (int i = 0; i < d.hc; ++i) t1[i] += s1[i] * (*b1)[i];
+        for (int j = 0; j < d.hid; ++j) t2[j] += s2[j] * (*B0)[j];
+        const std::vector<float> *parts[8] = {w1, &s1, &t1, W0, &s2, &t2, W3, B3};
+        for (int k = 0; k < 8; ++k) hoff[h][k] = hp.add(*parts[k]);
+    }
+    host.resize(off_heads + hp.host.size() * sizeof(float));
+    memcpy(host.data() + off_heads, hp.host.data(), hp.host.size() * sizeof(float));
+    if (m->d_board) cudaFree(m->d_board);
+    m->d_board = nullptr;
+    int rc = dev_alloc(&m->d_board, host.size());
+    if (rc != LZ_OK) return rc;
+    LZ_CUDA_CHECK(cudaMemcpy(m->d_board, host.data(), host.size(), cudaMemcpyHostToDevice));
+    BoardNet base;
+    memset(&base, 0, sizeof(base));
+    base.convw = m->d_board;
+    base.bn = reinterpret_cast<const float *>(m->d_board + off_bn);
+    base.abias = reinterpret_cast<const float *>(m->d_board + off_ab);
+    const float *hb = reinterpret_cast<const float *>(m->d_board + off_heads);
+    for (int h = 0; h < 3; ++h) {
+        BoardHead &o = base.head[h];
+        o.w1 = hb + hoff[h][0]; o.s1 = hb + hoff[h][1]; o.t1 = hb + hoff[h][2];
+        o.fc1 = hb + hoff[h][3]; o.s2 = hb + hoff[h][4]; o.t2 = hb + hoff[h][5];
+        o.fc2 = hb + hoff[h][6]; o.b2 = hb + hoff[h][7];
+        o.hc = heads[h].hc; o.hid = heads[h].hid; o.K = heads[h].K;
+    }
+    base.C = C; base.H = H; base.W = W; base.A = A;
+    base.support_min = c.support_min; base.support_step = c.support_step;
+    BoardNet rec = base, init = base;
+    auto add = [&](BoardNet &net, int ci, int flags) {
+        net.layer_woff[net.nlayers] = (uint32_t)woff[ci];
+        net.layer_bn[net.nlayers] = ci * 2 * C;
+        net.layer_flags[net.nlayers++] = flags;
+    };
+    auto blocks = [&](BoardNet &net, int first, int last_flags) {
+        for (int i = 0; i < n; ++i) {
+            add(net, first + 2 * i, 0);
+            add(net, first + 2 * i + 1, BF_RES | BF_STORE_RES | (i == n - 1 ? last_flags : 0));
+        }
+    };
+    add(rec, 0, BF_RES | BF_STORE_RES | BF_ACT_BIAS);
+    blocks(rec, 1, BF_WRITE_LATENT | BF_HOOK_REWARD);
+    blocks(rec, 2 * n + 1, BF_HOOK_VALPOL);
+    add(init, 6 * n + 1, BF_OBS | BF_STORE_RES);
+    blocks(init, 4 * n + 1, BF_WRITE_LATENT);
+    blocks(init, 2 * n + 1, BF_HOOK_VALPOL);
+    m->board_rec = rec; m->board_init = init;
+    return board_prepare_launch();
+}
+
 }  // namespace lz
 
 using namespace lz;
@@ -735,9 +866,22 @@ extern "C" {
 int lz_model_create(const lz_model_config *cfg, lz_model **out)
 {
     LZ_REQUIRE(cfg && out, LZ_EINVAL, "lz_model_create: null argument");
-    LZ_REQUIRE(cfg->num_channels == kC, LZ_EINVAL, "lz_model_create: num_channels must be %d (got %d)", kC, cfg->num_channels);
-    LZ_REQUIRE(cfg->obs_h == cfg->obs_w && (cfg->obs_h == 64 || cfg->obs_h == 84 || cfg->obs_h == 96), LZ_EINVAL,
-               "lz_model_create: observation %dx%d not supported (64x64 -> 8x8 latent, 84x84 and 96x96 -> 6x6 latent)", cfg->obs_h, cfg->obs_w);
+    const bool board = cfg->downsample == 0;
+    if (board) {
+        LZ_REQUIRE(cfg->num_channels == 16 || cfg->num_channels == 32 || cfg->num_channels == 64, LZ_EINVAL,
+                   "lz_model_create: the board network (downsample=False) takes num_channels 16, 32 or 64 (got %d)", cfg->num_channels);
+        LZ_REQUIRE(cfg->obs_h >= 1 && cfg->obs_h <= kBoardMaxHW && cfg->obs_w >= 1 && cfg->obs_w <= kBoardMaxHW, LZ_EINVAL,
+                   "lz_model_create: observation %dx%d not supported by the board network (downsample=False): boards up to %dx%d",
+                   cfg->obs_h, cfg->obs_w, kBoardMaxHW, kBoardMaxHW);
+        LZ_REQUIRE(cfg->obs_c >= 1 && cfg->obs_c <= 16, LZ_EINVAL, "lz_model_create: the board network takes 1 to 16 observation planes (got %d)", cfg->obs_c);
+        LZ_REQUIRE(cfg->action_space_size >= 1 && cfg->action_space_size <= 64, LZ_EINVAL,
+                   "lz_model_create: the board network takes 1 to 64 actions (got %d)", cfg->action_space_size);
+        LZ_REQUIRE(!cfg->efficientzero, LZ_EINVAL, "lz_model_create: the board network (downsample=False) is MuZero only");
+    } else {
+        LZ_REQUIRE(cfg->num_channels == kC, LZ_EINVAL, "lz_model_create: num_channels must be %d (got %d)", kC, cfg->num_channels);
+        LZ_REQUIRE(cfg->obs_h == cfg->obs_w && (cfg->obs_h == 64 || cfg->obs_h == 84 || cfg->obs_h == 96), LZ_EINVAL,
+                   "lz_model_create: observation %dx%d not supported (64x64 -> 8x8 latent, 84x84 and 96x96 -> 6x6 latent)", cfg->obs_h, cfg->obs_w);
+    }
     LZ_REQUIRE(cfg->num_res_blocks >= 1 && cfg->num_res_blocks <= kMaxResBlocks, LZ_EINVAL, "lz_model_create: num_res_blocks must be in [1,%d]", kMaxResBlocks);
     LZ_REQUIRE(cfg->reward_head_channels <= 16 && cfg->value_head_channels <= 16 && cfg->policy_head_channels <= 16, LZ_EINVAL, "lz_model_create: head channels must be <= 16");
     LZ_REQUIRE(cfg->reward_hidden <= 32 && cfg->value_hidden <= 32 && cfg->policy_hidden <= 32, LZ_EINVAL, "lz_model_create: head hidden sizes must be <= 32");
@@ -752,14 +896,19 @@ int lz_model_create(const lz_model_config *cfg, lz_model **out)
     lz_model *m = new lz_model();
     m->cfg = *cfg;
     m->ez_feat = m->ez_htmp = nullptr; m->ez_B = 0; m->d_ez_wtc = nullptr;
-    m->kind = 0;
-    // DownSample (common.py:334-366): 64 px -> 8x8 (no pooling2), 84 / 96 px -> 6x6
+    m->kind = board ? 2 : 0;
+    // DownSample (common.py:334-366): 64 px -> 8x8 (no pooling2), 84 / 96 px -> 6x6; the board network keeps the board's H x W
     const int hw = cfg->obs_h == 64 ? 8 : kHW;
-    m->latent_floats = kC * hw * hw;
+    m->lat_c = board ? cfg->num_channels : kC;
+    m->lat_h = board ? cfg->obs_h : hw;
+    m->lat_w = board ? cfg->obs_w : hw;
+    m->latent_floats = m->lat_c * m->lat_h * m->lat_w;
     memset(&m->mcfg, 0, sizeof(m->mcfg));
     m->finalized = false;
     m->d_weights = nullptr;
-    m->hw = hw; m->P = hw * hw; m->K = K;
+    m->d_board = nullptr;
+    m->hw = board ? (cfg->obs_h == cfg->obs_w ? cfg->obs_h : 0) : hw;
+    m->P = m->lat_h * m->lat_w; m->K = K;
     m->pre_latent = nullptr; m->ws_B = 0;
     m->npass = 3; m->d_tc = nullptr;   // default: tc3 (fp32-accurate)
     m->d_tower = nullptr; m->tws = nullptr; m->tws_bytes = 0; m->tc_skip = nullptr; m->tc_skip_B = 0;
@@ -772,6 +921,7 @@ int lz_model_destroy(lz_model *m)
     if (!m) return LZ_OK;
     cudaFree(m->d_weights);
     cudaFree(m->d_tc);
+    cudaFree(m->d_board);
     cudaFree(m->d_tower);
     cudaFree(m->tws);
     cudaFree(m->tc_skip);
@@ -799,6 +949,13 @@ int lz_model_finalize(lz_model *m)
     LZ_REQUIRE(m, LZ_EINVAL, "lz_model_finalize: null model");
     ++m->generation;          // every device table is re-allocated below: graphs captured against the old ones are stale
     if (m->kind == 1) return mlp_finalize(m);
+    if (m->kind == 2) {
+        int rc = pack_board(m);
+        if (rc != LZ_OK) return rc;
+        m->finalized = true;
+        m->tensors.clear();
+        return LZ_OK;
+    }
     const lz_model_config &c = m->cfg;
     const int A = c.action_space_size;
     Packer P;
@@ -909,7 +1066,7 @@ int lz_model_set_math(lz_model *m, int mode)
 {
     LZ_REQUIRE(m && (mode == 1 || mode == 2), LZ_EINVAL,
                "lz_model_set_math: mode must be 1 (tc3: tensor-core fp16 hi/lo, fp32-accurate) or 2 (tc1: tensor-core single fp16 pass)");
-    LZ_REQUIRE(m->kind == 0, LZ_EINVAL, "lz_model_set_math: the MLP model has no math mode");
+    LZ_REQUIRE(m->kind != 1, LZ_EINVAL, "lz_model_set_math: the MLP model has no math mode");
     const int npass = mode == 1 ? 3 : 1;
     if (m->npass != npass) ++m->generation;      // captured search graphs bake the pass count in
     m->npass = npass;
@@ -919,7 +1076,7 @@ int lz_model_set_math(lz_model *m, int mode)
 /* debug: replace the layer program of the tensor-core recurrent kernel (which == 0) or tail kernel (which == 1) */
 int lz_model_debug_tc_program(lz_model *m, int which, int nlayers, const int *layer_w, const int *layer_flags, int has_reward)
 {
-    LZ_REQUIRE(m && m->finalized && nlayers >= 1 && nlayers <= kTcMaxLayers, LZ_EINVAL, "lz_model_debug_tc_program: bad argument");
+    LZ_REQUIRE(m && m->finalized && m->kind == 0 && nlayers >= 1 && nlayers <= kTcMaxLayers, LZ_EINVAL, "lz_model_debug_tc_program: bad argument");
     ++m->generation;
     TcNet &n = which ? m->tc_tail : m->tc_rec;
     n.nlayers = nlayers;
@@ -937,6 +1094,15 @@ int lz_debug_tc_stamps(unsigned long long *h_out)
 }
 
 int lz_model_latent_hw(const lz_model *m) { return m ? m->hw : 0; }
+int lz_model_latent_shape(const lz_model *m, int32_t *h_c, int32_t *h_h, int32_t *h_w)
+{
+    LZ_REQUIRE(m, LZ_EINVAL, "lz_model_latent_shape: null model");
+    const bool mlp = m->kind == 1;
+    if (h_c) *h_c = mlp ? m->latent_floats : m->lat_c;
+    if (h_h) *h_h = mlp ? 1 : m->lat_h;
+    if (h_w) *h_w = mlp ? 1 : m->lat_w;
+    return LZ_OK;
+}
 int lz_model_support_size(const lz_model *m) { return m ? m->K : 0; }
 
 int lz_model_initial_inference(lz_model *m, int B, const float *d_obs, float *d_latent, float *d_policy_logits,
@@ -1018,12 +1184,51 @@ int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uin
     return LZ_OK;
 }
 
+// lz_model_debug_net_stage of the board network: which 1 is the whole initial_inference program, d_latent the observations
+static int board_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out,
+                             size_t out_bytes, int32_t *h_info, cudaStream_t st)
+{
+    BoardNet net = which ? m->board_init : m->board_rec;      // a copy: the model's programs stay as they are
+    const int nl = net.nlayers, K = m->K, A = m->cfg.action_space_size;
+    LZ_REQUIRE(stage <= nl, LZ_EINVAL, "lz_model_debug_net_stage: stage %d past the %d layers of the program", stage, nl);
+    const size_t nfl = stage < nl ? (size_t)B * m->latent_floats : (size_t)B * (2 * K + 2 * A + 4);
+    LZ_REQUIRE(out_bytes >= nfl * sizeof(float), LZ_EINVAL, "lz_model_debug_net_stage: stage %d needs %zu bytes, got %zu", stage,
+               nfl * sizeof(float), out_bytes);
+    const BoardPlan p = board_plan(net, B);
+    const int32_t info[8] = {p.R, p.NT, p.ctas, p.last, stage < nl ? stage + 1 : nl, m->npass, p.smem, 0};
+    memcpy(h_info, info, sizeof(info));
+    float *o = reinterpret_cast<float *>(d_out);
+    BoardIO io = board_io(m, B);
+    if (which) io.obs = d_in;
+    else { io.latent_base = d_in; io.action = d_action; }
+    if (stage < nl) {
+        // the program cut after layer `stage`, whose output is the only latent written; no head runs
+        net.nlayers = stage + 1;
+        for (int L = 0; L <= stage; ++L) net.layer_flags[L] &= ~(BF_WRITE_LATENT | BF_HOOK_REWARD | BF_HOOK_VALPOL);
+        net.layer_flags[stage] |= BF_WRITE_LATENT;
+        io.latent_out = o;
+        return board_launch(net, io, st);
+    }
+    // the whole program with the raw logits, then without them (the scalars alone, as a search asks for them)
+    LZ_CUDA_CHECK(cudaMemsetAsync(d_out, 0, nfl * sizeof(float), st));
+    float *rl = o, *vl = rl + (size_t)B * K, *pl = vl + (size_t)B * K, *r = pl + (size_t)B * A, *v = r + B;
+    float *pl2 = v + B, *r2 = pl2 + (size_t)B * A, *v2 = r2 + B;
+    io.policy_logits = pl; io.value_logits = vl; io.value = v;
+    if (!which) { io.reward_logits = rl; io.reward = r; }
+    int rc = board_launch(net, io, st);
+    if (rc) return rc;
+    io.policy_logits = pl2; io.value_logits = nullptr; io.value = v2;
+    io.reward_logits = nullptr; io.reward = which ? nullptr : r2;
+    return board_launch(net, io, st);
+}
+
 int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_latent, const int32_t *d_action, int stage, void *d_out,
                              size_t out_bytes, int32_t *h_info, lz_stream s)
 {
     LZ_REQUIRE(m && (which == 0 || which == 1) && B > 0 && d_latent && (which == 1 || d_action) && d_out && h_info && stage >= 0,
                LZ_EINVAL, "lz_model_debug_net_stage: bad argument");
-    LZ_REQUIRE(m->finalized && m->kind == 0, LZ_ESTATE, "lz_model_debug_net_stage: not a finalized conv model");
+    LZ_REQUIRE(m->finalized && (m->kind == 0 || m->kind == 2), LZ_ESTATE, "lz_model_debug_net_stage: not a finalized conv model");
+    if (m->kind == 2) return board_debug_stage(m, which, B, d_latent, d_action, stage, d_out, out_bytes, h_info, (cudaStream_t)s);
     TcNet net = which ? m->tc_tail : m->tc_rec;          // a copy: the model's programs stay as they are
     const int nl = net.nlayers, K = m->K, A = m->cfg.action_space_size;
     const bool ez = m->cfg.efficientzero != 0 && which == 0;

@@ -9,6 +9,7 @@
 #include "net_tc.cuh"
 #include "conv_tc.cuh"
 #include "ez.cuh"
+#include "board_tc.cuh"
 
 namespace lz {
 
@@ -65,7 +66,11 @@ struct TailIO {
 }  // namespace lz
 
 struct lz_model {
-    int kind;                         // 0 = conv MuZeroModel / EfficientZeroModel (cfg.efficientzero), 1 = MuZeroModelMLP
+    int kind;                         // 0 = conv MuZeroModel / EfficientZeroModel (cfg.efficientzero), 1 = MuZeroModelMLP,
+                                      // 2 = board MuZeroModel (downsample=False, board_tc.cu)
+    unsigned char *d_board;           // kind 2: packed conv weights, BN / action-plane tables and fp32 head tables
+    lz::BoardNet board_rec, board_init;   // kind 2: recurrent_inference / initial_inference programs
+    int lat_c, lat_h, lat_w;          // latent shape of one root
     lz::EzNet ez;                     // EfficientZero value-prefix head tables (device pointers into d_weights)
     float *ez_feat, *ez_htmp;         // [ws_B][hc*36], [ws_B][H] scratch between the conv kernel and the LSTM kernels
     int ez_B;

@@ -37,21 +37,29 @@ class MuZeroModel:
                  discrete_action_encoding_type: str = "one_hot", state_norm: bool = False,
                  device: Optional[torch.device] = None, **kwargs):
         # unknown kwargs are swallowed like muzero_model.py:49-50
+        efficientzero = bool(kwargs.get("_efficientzero", False))
+        board = tuple(observation_shape[1:])
+        fits_board = len(board) == 2 and 1 <= board[0] <= 8 and 1 <= board[1] <= 8
         if downsample is None:
-            # The reference's default is downsample=False (muzero_model.py:45, efficientzero_model.py:45): a full-resolution
-            # network this class does not implement.  84 / 96-pixel models default to the DownSample network here, as they
-            # always have.  A 64x64 model follows the reference default, so it must ask for DownSample as the shipped Atari
-            # configs do (zoo/atari/config/atari_muzero_config.py:56, atari_efficientzero_config.py:44).
-            downsample = tuple(observation_shape[1:]) != (64, 64)
-            if not downsample:
+            # The reference's default is downsample=False (muzero_model.py:45, efficientzero_model.py:45): the full-resolution
+            # network of the board-game configs, which this class runs for MuZero boards up to 8x8.  84 / 96-pixel models
+            # default to the DownSample network here, as they always have.  A 64x64 model follows the reference default, so
+            # it must ask for DownSample as the shipped Atari configs do (zoo/atari/config/atari_muzero_config.py:56,
+            # atari_efficientzero_config.py:44).
+            downsample = not (fits_board and not efficientzero)
+            if board == (64, 64):
                 raise NotImplementedError(
                     "a 64x64 observation_shape needs downsample=True (as in the reference's Atari configs): with the reference's "
-                    "default downsample=False the model is a full-resolution network, which this CUDA model does not implement")
-        if not categorical_distribution or not downsample or norm_type != "BN" or \
-                discrete_action_encoding_type != "one_hot" or state_norm:
+                    "default downsample=False the model is a full-resolution network, which this CUDA model implements for "
+                    "boards up to 8x8 only")
+        if not downsample and (efficientzero or not fits_board):
             raise NotImplementedError(
-                "CUDA MuZeroModel implements the Atari configuration of the reference: categorical_distribution, "
-                "downsample, norm_type='BN', one_hot action encoding, state_norm=False")
+                "downsample=False (the full-resolution board network) is implemented for MuZeroModel on boards up to 8x8; "
+                f"got observation_shape {tuple(observation_shape)}" + (" for EfficientZeroModel" if efficientzero else ""))
+        if not categorical_distribution or norm_type != "BN" or discrete_action_encoding_type != "one_hot" or state_norm:
+            raise NotImplementedError(
+                "CUDA MuZeroModel implements the configurations of the reference's Atari and board-game configs: "
+                "categorical_distribution, norm_type='BN', one_hot action encoding, state_norm=False")
         if tuple(reward_support_range) != tuple(value_support_range):
             raise NotImplementedError("reward and value supports must be equal")
         if len(reward_head_hidden_channels) != 1 or len(value_head_hidden_channels) != 1 or len(policy_head_hidden_channels) != 1:
@@ -67,8 +75,8 @@ class MuZeroModel:
                                num_res_blocks, num_channels, reward_head_channels, value_head_channels,
                                policy_head_channels, reward_head_hidden_channels[0], value_head_hidden_channels[0],
                                policy_head_hidden_channels[0], value_support_range[0], value_support_range[1],
-                               value_support_range[2], int(bool(kwargs.get("_efficientzero", False))),
-                               int(kwargs.get("lstm_hidden_size", 0) if kwargs.get("_efficientzero", False) else 0))
+                               value_support_range[2], int(efficientzero),
+                               int(kwargs.get("lstm_hidden_size", 0) if efficientzero else 0), int(bool(downsample)))
         self._cfg = cfg
         h = cabi.c_void_p()
         with torch.cuda.device(self.device):
@@ -76,6 +84,11 @@ class MuZeroModel:
         self._h = h
         self._serial = next(_model_serial)
         self.latent_hw = self._lib.lz_model_latent_hw(self._h)
+        shape = (cabi.ctypes.c_int32 * 3)()
+        cabi.check(self._lib.lz_model_latent_shape(self._h, cabi.ctypes.byref(shape, 0), cabi.ctypes.byref(shape, 4),
+                                                   cabi.ctypes.byref(shape, 8)), "lz_model_latent_shape")
+        self.latent_shape = tuple(shape)          # (C, H, W) of one root's latent
+        self.downsample = bool(downsample)
         self.value_support_size = self.reward_support_size = self._lib.lz_model_support_size(self._h)
         self._loaded = False
 
@@ -123,8 +136,8 @@ class MuZeroModel:
         """muzero_model.py:210-240.  ``reward`` is the python list of zeros the reference returns."""
         self._check()
         obs = obs.to(self.device, torch.float32).contiguous()
-        B, hw, C = obs.shape[0], self.latent_hw, self.num_channels
-        latent = torch.empty(B, C, hw, hw, device=self.device)
+        B = obs.shape[0]
+        latent = torch.empty((B,) + self.latent_shape, device=self.device)
         policy = torch.empty(B, self.action_space_size, device=self.device)
         value = torch.empty(B, self.value_support_size, device=self.device)
         scalar = torch.empty(B, device=self.device) if return_scalar_value else None
@@ -143,8 +156,8 @@ class MuZeroModel:
         self._check()
         latent_state = latent_state.to(self.device, torch.float32).contiguous()
         action = action.to(self.device).reshape(-1).to(torch.int32).contiguous()
-        B, hw, C = latent_state.shape[0], self.latent_hw, self.num_channels
-        nxt = torch.empty(B, C, hw, hw, device=self.device)
+        B = latent_state.shape[0]
+        nxt = torch.empty((B,) + self.latent_shape, device=self.device)
         policy = torch.empty(B, self.action_space_size, device=self.device)
         value = torch.empty(B, self.value_support_size, device=self.device)
         reward = torch.empty(B, self.reward_support_size, device=self.device)

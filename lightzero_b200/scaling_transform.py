@@ -26,7 +26,7 @@ class InverseScalarTransform:
         self.support = scalar_support
         self._lib = cabi.load()
         cfg = cabi.ModelConfig(4, 84, 84, 1, 1, 64, 16, 16, 16, 32, 32, 32, scalar_support.start,
-                               scalar_support.stop, scalar_support.step)
+                               scalar_support.stop, scalar_support.step, downsample=1)
         h = cabi.c_void_p()
         cabi.check(self._lib.lz_model_create(cfg, h), "lz_model_create")
         self._h = h
