@@ -209,13 +209,29 @@ typedef struct lz_mlp_config {
     float support_min, support_max, support_step;
 } lz_mlp_config;
 int lz_model_create_mlp(const lz_mlp_config *cfg, lz_model **out);
+/* EfficientZeroModelMLP (lzero/model/efficientzero_model_mlp.py:150-300; vector observations): the MLP representation /
+ * prediction networks of MuZeroModelMLP, a dynamics MLP (fc_dynamics, or fc_dynamics_1 + latent -> fc_dynamics_2 with
+ * res_connection_in_dynamics) whose output feeds nn.LSTM(latent_dim -> lstm_hidden_size) and fc_reward_head (a VALUE PREFIX,
+ * no norm_value_prefix).  Same lz_model_* / lz_search_* calls as EfficientZeroModel: d_obs is f32 [B, obs_dim], latents
+ * f32 [B, latent_dim], the reward hidden state f32 [B, lstm_hidden_size] x 2.  Accepted: latent_dim a multiple of 32 in
+ * [32, 256], lstm_hidden_size a multiple of 16 in [16, 512], obs_dim 1-4096, action_space_size 1-608, head hidden sizes 1-32,
+ * support size <= 608; anything else is LZ_EINVAL.  Math modes tc3 / tc1 as the conv models (lz_model_set_math).  Latent
+ * buffers (in and out) must be 16-byte aligned: the kernel moves latent rows as vectors. */
+typedef struct lz_mlp_ez_config {
+    int obs_dim, action_space_size, latent_dim, lstm_hidden_size;
+    int reward_hidden, value_hidden, policy_hidden;     /* one hidden layer each: 32 */
+    int res_connection_in_dynamics;
+    float support_min, support_max, support_step;
+} lz_mlp_ez_config;
+int lz_model_create_mlp_ez(const lz_mlp_ez_config *cfg, lz_model **out);
 int lz_model_destroy(lz_model *m);
 /* Feed one tensor of the reference state_dict (names as produced by MuZeroModel.state_dict(),
  * SURVEY.md App. B.4; fp32, contiguous, HOST memory).  Unknown names are ignored (returns 1). */
 int lz_model_set_tensor(lz_model *m, const char *name, const float *h_data, int64_t numel);
 /* Folds eval-mode BatchNorm into per-channel scale/shift, packs weights for the kernels, uploads. */
 int lz_model_finalize(lz_model *m);
-/* Arithmetic of the conv model's tensor-core kernels (the DownSample tower and the latent-grid networks):
+/* Arithmetic of the conv model's tensor-core kernels (the DownSample tower and the latent-grid networks; the
+ * EfficientZeroModelMLP network and its LSTM likewise):
  *   1 = tc3: fp16 hi/lo operand splitting (3 MMAs per product, fp32 accumulate in registers): fp32-accurate, the default
  *       and the mode parity is stated for;
  *   2 = tc1: single fp16 pass (fp32 accumulate): ~3x fewer MMAs, logits accurate to ~1e-3.
@@ -250,7 +266,14 @@ int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uin
  * the launched program, MMA passes, 1 if the FC2 biases are staged in shared memory, FC2 tiles.
  * Board models (downsample = 0): `which` 1 is the whole initial_inference program on the observations d_latent
  * f32 [B,obs_c,H,W]; outputs as above without the EfficientZero section, latents [B,C,H,W]; h_info: roots per CTA R, 64-row tiles
- * NT, CTA count, roots of the last CTA, layers, MMA passes, shared memory bytes, 0. */
+ * NT, CTA count, roots of the last CTA, layers, MMA passes, shared memory bytes, 0.
+ * EfficientZeroModelMLP: `which` 0 is recurrent_inference's dense program on d_latent f32 [B, latent_dim] and d_action, `which` 1
+ * initial_inference's on the observations d_latent f32 [B, obs_dim].  stage < D (D = the L-wide layers before the heads: 4 for
+ * `which` 1, 4 or 6 for `which` 0) writes that layer's output f32 [B, latent_dim] (after the LayerNorm for the representation's
+ * second layer, after the residual for fc_dynamics_1); stage == D runs the whole program and writes latent [B, latent_dim], the
+ * LSTM input [B, latent_dim] (`which` 0; zeros for `which` 1; no LSTM runs), value logits [B,K], policy logits [B,A], value [B].
+ * h_info: roots per CTA, CTA count, roots of the last CTA, layers of the launched program, MMA passes, shared memory bytes, weight
+ * ring stages, D. */
 int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_latent, const int32_t *d_action, int stage,
                              void *d_out, size_t out_bytes, int32_t *h_info, lz_stream s);
 int lz_model_latent_hw(const lz_model *m);   /* 6 for 84/96, 8 for 64; a square board's side; 0 for a non-square board */

@@ -32,6 +32,14 @@ class MlpConfig(ctypes.Structure):
                 ("support_min", c_float), ("support_max", c_float), ("support_step", c_float)]
 
 
+class MlpEzConfig(ctypes.Structure):
+    """struct lz_mlp_ez_config (include/lzb200.h)"""
+    _fields_ = [("obs_dim", c_int), ("action_space_size", c_int), ("latent_dim", c_int), ("lstm_hidden_size", c_int),
+                ("reward_hidden", c_int), ("value_hidden", c_int), ("policy_hidden", c_int),
+                ("res_connection_in_dynamics", c_int), ("support_min", c_float), ("support_max", c_float),
+                ("support_step", c_float)]
+
+
 # name -> (restype, argtypes); every symbol include/lzb200.h declares
 SIGNATURES = {
     "lz_version": (c_int, []),
@@ -62,6 +70,7 @@ SIGNATURES = {
     "lz_gumbel_tables": (c_int, [c_int, c_int, c_int, c_void_p, c_void_p]),
     "lz_model_create": (c_int, [ctypes.POINTER(ModelConfig), ctypes.POINTER(c_void_p)]),
     "lz_model_create_mlp": (c_int, [ctypes.POINTER(MlpConfig), ctypes.POINTER(c_void_p)]),
+    "lz_model_create_mlp_ez": (c_int, [ctypes.POINTER(MlpEzConfig), ctypes.POINTER(c_void_p)]),
     "lz_model_destroy": (c_int, [c_void_p]),
     "lz_model_set_tensor": (c_int, [c_void_p, c_char_p, c_void_p, c_int64]),
     "lz_model_finalize": (c_int, [c_void_p]),

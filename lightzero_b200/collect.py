@@ -8,13 +8,14 @@ device, the representation+prediction networks, root preparation with Dirichlet 
 num_simulations search (one CUDA graph) and the result read-back are issued back to back on one
 stream; the only host synchronisation is the final read of the results.
 """
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Union
 
 import numpy as np
 import torch
 
 from . import cabi, mz_tree
 from .efficientzero_model import EfficientZeroModel
+from .efficientzero_model_mlp import EfficientZeroModelMLP
 from .mcts_ctree import EfficientZeroMCTSCtree, MuZeroMCTSCtree
 from .muzero_model import MuZeroModel
 
@@ -208,7 +209,7 @@ class EfficientZeroCollectPolicy(MuZeroCollectPolicy):
     690-760): value-prefix trees, the reward hidden state starts as zeros after ``initial_inference`` (:580-590) and is reset
     every ``lstm_horizon_len`` steps of search depth.  Same output dict."""
 
-    def __init__(self, model: EfficientZeroModel, cfg: Optional[dict] = None):
+    def __init__(self, model: Union[EfficientZeroModel, EfficientZeroModelMLP], cfg: Optional[dict] = None):
         super().__init__(model, cfg)
         self.mcts = EfficientZeroMCTSCtree(cfg or {})
         self.cfg = self.mcts._cfg

@@ -5,7 +5,7 @@
 // update fused into the epilogue: the weight columns are ordered unit-major / gate-minor so that the 4 x 4 register tile
 // of a thread holds (i, f, g, o) of one hidden unit for 4 roots.  torch.nn.LSTM gate order i, f, g, o; c' = sig(f) c +
 // sig(i) tanh(g); h' = sig(o) tanh(c').
-// k_ez_head: per root relu(bn(h')) -> Linear(H, hid) + BN + ReLU -> Linear(hid, K) -> softmax expectation -> h^-1.
+// k_ez_head: per root relu(bn(h')) (h' alone for EfficientZeroModelMLP) -> Linear(H, hid) + BN + ReLU -> Linear(hid, K) -> softmax expectation -> h^-1.
 #include <cuda_fp16.h>
 #include <math.h>
 #include <stdlib.h>
@@ -105,7 +105,12 @@ __global__ void __launch_bounds__(256) k_ez_head(EzNet net, EzIO io)
     const int H = net.H, hid = net.hid, K = net.K;
     for (int i = tid; i < kHR * H; i += 256) {                       // norm_value_prefix + ReLU (efficientzero_model.py:565-566)
         const int r = i / H, u = i - r * H;
-        x[r][u] = r < nr ? fmaxf(fmaf(io.h_tmp[(size_t)(r0 + r) * H + u], net.vp_s[u], net.vp_t[u]), 0.0f) : 0.0f;
+        float v = 0.0f;
+        if (r < nr) {
+            v = io.h_tmp[(size_t)(r0 + r) * H + u];
+            if (!net.no_vp_norm) v = fmaxf(fmaf(v, net.vp_s[u], net.vp_t[u]), 0.0f);
+        }
+        x[r][u] = v;
     }
     __syncthreads();
     {   // Linear(H -> hid): warp w sums its eighth of the inputs, lane = hidden unit; 16 weight rows in flight per batch

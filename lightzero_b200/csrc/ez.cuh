@@ -16,6 +16,7 @@ struct EzNet {
     const float *fc2;         // [hid][K]
     const float *b2;          // [K]
     int nin, H, hid, K;
+    int no_vp_norm;           // 1: the head reads h' directly (EfficientZeroModelMLP has no norm_value_prefix); vp_s / vp_t unused
     float support_min, support_step;
 };
 

@@ -1,0 +1,560 @@
+// mlp_tc.cu -- tensor-core (wgmma) network of EfficientZeroModelMLP (lzero/model/efficientzero_model_mlp.py:150-300):
+// representation Linear(obs -> L) + BN + GELU(tanh) + Linear(L -> L) + LayerNorm (common.py:790-850), the dynamics MLPs over
+// [latent | one-hot action] (fc_dynamics, or fc_dynamics_1 + latent -> fc_dynamics_2 with res_connection_in_dynamics,
+// efficientzero_model_mlp.py:440-468) and the prediction MLPs (common.py:1218-1292).  The LSTM value-prefix head that follows the
+// dynamics network runs in ez.cu on the LSTM input this kernel writes.
+//
+// One launch runs a whole layer program (initial_inference, or the dense part of recurrent_inference) for all roots; a CTA of one
+// warpgroup owns up to 64 roots, the rows of one m64 wgmma tile.  Arithmetic as net_tc.cu / board_tc.cu: 3xFP16 (A_hi B_hi +
+// A_hi B_lo + A_lo B_hi, fp32 accumulators in registers; one pass in tc1), weights pre-split on the host and pre-scaled by a power
+// of two that is folded into the BN scale.  Activations stay in shared memory in the wgmma K-major no-swizzle layout
+// [k-group of 8 features][64 rows][8 halves] (hi plane, then lo plane) in two L-wide slots and one 32-wide buffer (head hidden
+// layer, or the current 32-feature chunk of the observation, which is streamed from global memory).  Weights stream in chunks of
+// 32 inputs through a ring of stages (cp.async.bulk, mbarrier complete_tx), refilled by thread 0 as soon as the MMAs have read a
+// stage.  Every layer accumulates all of its outputs (N <= L <= 256: <= 128 fp32 registers per thread) before its epilogue runs
+// straight from the fragments: folded BN / bias, the one-hot action as a gathered fp32 weight row, ReLU or GELU, the residual
+// from the fp32 input latent, LayerNorm (a row lives in one lane quad: two quad-shuffle reductions), then the fp16 hi / lo
+// rewrite of the next layer's operand and the fp32 outputs.  The last Linear of each head is cut into pieces of <= L outputs
+// (K = 32 inputs) that run the same way; the value head's softmax expectation is folded online across its pieces.
+#include <cuda_fp16.h>
+#include <math.h>
+#include <string.h>
+
+#include <algorithm>
+#include <vector>
+
+#include "model.cuh"
+#include "tc_ptx.cuh"
+
+namespace lz {
+
+constexpr int kMezThreads = 128;
+constexpr int kMezKgBytes = kMezRows * 16;                 // one k-group plane of 64 rows: 1 KB
+constexpr int kMezHidBytes = 2 * 4 * kMezKgBytes;          // 32-wide buffer, hi | lo: 8 KB
+constexpr int kMezSmemMax = 227 * 1024;
+
+__host__ __device__ inline int mez_slot_part(int L) { return (L / 8) * kMezKgBytes; }    // hi (or lo) plane of an L-wide slot
+__host__ __device__ inline int mez_stage_bytes(int L) { return 128 * L; }               // 32 inputs x <= L outputs, hi | lo
+
+struct MezSmem {
+    int slot1, hid, ring, bars, total;
+};
+
+__host__ __device__ inline MezSmem mez_smem(int L, int stages)
+{
+    MezSmem s;
+    s.slot1 = 2 * mez_slot_part(L);
+    s.hid = 2 * s.slot1;
+    s.ring = s.hid + kMezHidBytes;
+    s.bars = s.ring + stages * mez_stage_bytes(L);
+    s.total = s.bars + stages * 8;
+    return s;
+}
+
+__device__ __forceinline__ float mez_gelu(float x)
+{
+    const float k0 = 0.7978845608028654f, k1 = 0.044715f;      // sqrt(2/pi), torch.nn.GELU(approximate='tanh')
+    return 0.5f * x * (1.0f + tanhf(k0 * (x + k1 * x * x * x)));
+}
+
+// The MMAs of one 32-input chunk: 2 k-steps, W n32 column blocks (as n64 pairs, an odd one as n32), NP passes; straight-line so
+// that no branch separates the wgmma of a commit group.  An n64 fragment is the two n32 fragments of its columns back to back.
+template <int NC, int W, int NP>
+__device__ __forceinline__ void mez_mma(float (&acc)[NC * 16], uint64_t a0, uint64_t b0, uint32_t a_kstep, uint32_t a_lo,
+                                        uint32_t b_kstep, uint32_t b_lo)
+{
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) {
+        const uint64_t a = a0 + ks * a_kstep, bk = b0 + ks * b_kstep;
+#pragma unroll
+        for (int p = 0; p < W / 2; ++p) {
+            float(&d)[32] = *reinterpret_cast<float(*)[32]>(&acc[32 * p]);
+            const uint64_t b = bk + 64 * p;                 // 64 weight rows of 16 B
+            wgmma_n64(d, a, b);
+            if constexpr (NP == 3) {
+                wgmma_n64(d, a, b + b_lo);
+                wgmma_n64(d, a + a_lo, b);
+            }
+        }
+        if constexpr (W % 2 == 1) {
+            float(&d)[16] = *reinterpret_cast<float(*)[16]>(&acc[16 * (W - 1)]);
+            const uint64_t b = bk + 32 * (W - 1);
+            wgmma_n32(d, a, b);
+            if constexpr (NP == 3) {
+                wgmma_n32(d, a, b + b_lo);
+                wgmma_n32(d, a + a_lo, b);
+            }
+        }
+    }
+}
+
+template <int NC>
+__global__ void __launch_bounds__(kMezThreads, 1) k_mez_tc(MezNet net, MezIO io, int R, int kS)
+{
+    extern __shared__ __align__(1024) unsigned char smem[];
+    constexpr int L = 32 * NC;
+    const MezSmem S = mez_smem(L, kS);
+    unsigned char *ring = smem + S.ring;
+    float *part = reinterpret_cast<float *>(smem + S.slot1);    // [NC * 16][128] fp32 partial sums of the observation layer
+    uint64_t *full = reinterpret_cast<uint64_t *>(smem + S.bars);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int root0 = blockIdx.x * R, nvalid = min(R, io.B - root0);
+    const int sbytes = mez_stage_bytes(L);
+
+    int il = 0, ic = 0, issued = 0;            // thread 0: the next weight chunk of the program to stream
+    auto issue_next = [&]() {
+        const uint32_t bytes = 128u * net.layer[il].N;
+        uint64_t *bar = &full[issued % kS];
+        mbar_expect_tx(bar, bytes);
+        bulk_g2s(ring + (issued % kS) * sbytes, net.w + net.layer[il].woff + (size_t)ic * bytes, bytes, bar);
+        ++issued;
+        if (++ic == net.layer[il].K / 32) { ic = 0; ++il; }
+    };
+    auto release = [&]() {                     // a stage has been read: it takes the next chunk in program order
+        if (tid == 0 && issued < net.nchunks) issue_next();
+    };
+    if (tid == 0) {
+        for (int i = 0; i < kS; ++i) mbar_init(&full[i], 1);
+        fence_mbar_init();
+        for (int i = 0; i < kS && issued < net.nchunks; ++i) issue_next();
+    }
+
+    // rows of this thread's accumulator fragments and their per-root operands
+    int brow[2];
+    bool on[2];
+    const float *zrow[2], *arow[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int m = 16 * warp + (lane >> 2) + 8 * h;
+        on[h] = m < nvalid;
+        brow[h] = root0 + (on[h] ? m : 0);
+        zrow[h] = io.latent_base ? io.latent_base + (io.ix ? (size_t)io.ix[brow[h]] * io.slot_stride : 0) + (size_t)brow[h] * L : nullptr;
+        arow[h] = io.action ? net.abias + (size_t)min(max(io.action[brow[h]], 0), net.A - 1) * L : nullptr;
+    }
+
+    // ---- input latents (recurrent programs) -> slot 0, fp16 hi / lo
+    if (net.layer[0].in == MB_SLOT0) {
+        for (int i = tid; i < kMezRows * (L / 8); i += kMezThreads) {
+            const int m = i % kMezRows, kg = i / kMezRows;
+            float v[8];
+            if (m < nvalid) {
+                const int b = root0 + m;
+                const float *src = io.latent_base + (io.ix ? (size_t)io.ix[b] * io.slot_stride : 0) + (size_t)b * L + 8 * kg;
+                const float4 x = *reinterpret_cast<const float4 *>(src), y = *reinterpret_cast<const float4 *>(src + 4);
+                v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w; v[4] = y.x; v[5] = y.y; v[6] = y.z; v[7] = y.w;
+            } else {
+#pragma unroll
+                for (int u = 0; u < 8; ++u) v[u] = 0.0f;
+            }
+            store_split8(smem + kg * kMezKgBytes + m * 16, smem + mez_slot_part(L) + kg * kMezKgBytes + m * 16, v);
+        }
+    }
+    fence_proxy_async();
+    __syncthreads();
+
+    float sm_m[2] = {-INFINITY, -INFINITY}, sm_s[2] = {0.0f, 0.0f}, sm_w[2] = {0.0f, 0.0f};   // value head: online softmax
+    int pos = 0;
+    for (int l = 0; l < net.nlayers; ++l) {
+        const int K = net.layer[l].K, N = net.layer[l].N, in = net.layer[l].in, out = net.layer[l].out;
+        const int f = net.layer[l].flags, nch = N / 32, nk = K / 32;
+        const bool obs = in == MB_OBS;
+        float acc[NC * 16];
+#pragma unroll
+        for (int i = 0; i < NC * 16; ++i) acc[i] = 0.0f;
+        wg_fence_acc(acc);
+        const bool narrow = obs || in == MB_HID;              // the 32-wide buffer
+        unsigned char *abuf = narrow ? smem + S.hid : smem + (in == MB_SLOT1 ? S.slot1 : 0);
+        const uint64_t a_base = make_desc(smem_u32(abuf), kMezKgBytes >> 4, 8);
+        const uint32_t a_kstep = (2 * kMezKgBytes) >> 4, a_lo = (narrow ? 4 * kMezKgBytes : mez_slot_part(L)) >> 4;
+        const uint32_t b_lo = N, b_kstep = 4 * N;             // 16-B units: N rows; two k-groups of [N hi | N lo] rows
+        for (int c = 0; c < nk; ++c, ++pos) {
+            uint64_t a0 = a_base;
+            if (obs) {      // observation features 32c .. 32c + 31 -> the 32-wide buffer (the previous chunk's MMAs are done)
+                const int m = tid % kMezRows, hf = tid / kMezRows;
+                float v[16];
+#pragma unroll
+                for (int u = 0; u < 16; ++u) {
+                    const int k = 32 * c + 16 * hf + u;
+                    v[u] = (m < nvalid && k < net.obs_dim) ? io.obs[(size_t)(root0 + m) * net.obs_dim + k] : 0.0f;
+                }
+#pragma unroll
+                for (int g = 0; g < 2; ++g) {
+                    unsigned char *d = smem + S.hid + (2 * hf + g) * kMezKgBytes + m * 16;
+                    store_split8(d, d + 4 * kMezKgBytes, v + 8 * g);
+                }
+                fence_proxy_async();
+                __syncthreads();
+            } else {
+                a0 += (uint64_t)((4 * c * kMezKgBytes) >> 4);
+            }
+            const int st = pos % kS;
+            mbar_wait(&full[st], (pos / kS) & 1);
+            const uint64_t b0 = make_desc(smem_u32(ring + st * sbytes), (2 * N * 16) >> 4, 8);
+            wg_fence();
+            if (io.npass == 3) {
+                if (nch == NC) mez_mma<NC, NC, 3>(acc, a0, b0, a_kstep, a_lo, b_kstep, b_lo);
+                else mez_mma<NC, 1, 3>(acc, a0, b0, a_kstep, a_lo, b_kstep, b_lo);
+            } else {
+                if (nch == NC) mez_mma<NC, NC, 1>(acc, a0, b0, a_kstep, a_lo, b_kstep, b_lo);
+                else mez_mma<NC, 1, 1>(acc, a0, b0, a_kstep, a_lo, b_kstep, b_lo);
+            }
+            wg_commit();
+            if (obs) {
+                // each chunk's sums are added into fp32 partials (round to nearest) in the free slot 1: the tensor cores'
+                // accumulation truncates, and over the ~270 accumulations of a 2835-wide observation that bias would grow
+                // linearly (2e-5 of the latent after the LayerNorm instead of 1e-6)
+                wg_wait<0>();
+                wg_fence_acc(acc);
+#pragma unroll
+                for (int i = 0; i < NC * 16; ++i) {
+                    const float p = c ? part[i * kMezThreads + tid] : 0.0f;
+                    part[i * kMezThreads + tid] = p + acc[i];
+                    acc[i] = 0.0f;
+                }
+                wg_fence_acc(acc);
+                __syncthreads();
+                release();
+            } else if (c > 0) {
+                wg_wait<1>();                                 // the previous chunk's MMAs have read their stage: refill it
+                __syncthreads();
+                release();
+            }
+        }
+        wg_wait<0>();
+        wg_fence_acc(acc);
+        if (obs) {
+#pragma unroll
+            for (int i = 0; i < NC * 16; ++i) acc[i] = part[i * kMezThreads + tid];
+        }
+        __syncthreads();                                      // every MMA of the layer has read its operand: it may be rewritten
+        if (!obs) release();
+
+        // ---- epilogue, pass 1 (in place): folded BN / bias, action row, activation, residual
+        const float *sc = net.tab + net.layer[l].bn, *sh = sc + N;
+#pragma unroll
+        for (int j = 0; j < NC; ++j) {
+            if (j >= nch) break;
+#pragma unroll
+            for (int q = 0; q < 4; ++q)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int col = 32 * j + 8 * q + 2 * (lane & 3) + e;
+                        float v = fmaf(acc[16 * j + 4 * q + 2 * h + e], __ldg(sc + col), __ldg(sh + col));
+                        if ((f & MF_ACT) && on[h]) v += __ldg(arow[h] + col);
+                        if (f & MF_RELU) v = fmaxf(v, 0.0f);
+                        else if (f & MF_GELU) v = mez_gelu(v);
+                        if ((f & MF_RES) && on[h]) v += zrow[h][col];
+                        acc[16 * j + 4 * q + 2 * h + e] = v;
+                    }
+        }
+        if (f & MF_LN) {     // nn.LayerNorm(L), eps 1e-5, biased variance: a row's L values live in one lane quad
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float s = 0.0f;
+#pragma unroll
+                for (int j = 0; j < NC; ++j)
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) s += acc[16 * j + 4 * q + 2 * h] + acc[16 * j + 4 * q + 2 * h + 1];
+                s += __shfl_xor_sync(0xffffffffu, s, 1);
+                s += __shfl_xor_sync(0xffffffffu, s, 2);
+                const float mean = s / (float)L;
+                float d2 = 0.0f;
+#pragma unroll
+                for (int j = 0; j < NC; ++j)
+#pragma unroll
+                    for (int q = 0; q < 4; ++q)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const float d = acc[16 * j + 4 * q + 2 * h + e] - mean;
+                            d2 += d * d;
+                        }
+                d2 += __shfl_xor_sync(0xffffffffu, d2, 1);
+                d2 += __shfl_xor_sync(0xffffffffu, d2, 2);
+                const float rstd = rsqrtf(d2 / (float)L + 1e-5f);
+#pragma unroll
+                for (int j = 0; j < NC; ++j)
+#pragma unroll
+                    for (int q = 0; q < 4; ++q)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int col = 32 * j + 8 * q + 2 * (lane & 3) + e;
+                            float &v = acc[16 * j + 4 * q + 2 * h + e];
+                            v = (v - mean) * rstd * __ldg(net.ln_w + col) + __ldg(net.ln_b + col);
+                        }
+            }
+        }
+        if (f & MF_CAT_BEGIN) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) { sm_m[h] = -INFINITY; sm_s[h] = 0.0f; sm_w[h] = 0.0f; }
+        }
+
+        // ---- pass 2: the fp32 outputs and the next layer's fp16 hi / lo operand
+        const bool val = (f & MF_VALUE) != 0, head = (f & (MF_VALUE | MF_POLICY)) != 0;
+        const int ncols = val ? net.K : net.A, col0 = net.layer[l].col0;
+        float *lg = val ? io.value_logits : io.policy_logits;
+        unsigned char *ob = out == MB_NONE ? nullptr : smem + (out == MB_HID ? S.hid : (out == MB_SLOT1 ? S.slot1 : 0));
+        const int opart = out == MB_HID ? 4 * kMezKgBytes : mez_slot_part(L);
+#pragma unroll
+        for (int j = 0; j < NC; ++j) {
+            if (j >= nch) break;
+#pragma unroll
+            for (int q = 0; q < 4; ++q)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int col = 32 * j + 8 * q + 2 * (lane & 3), m = 16 * warp + (lane >> 2) + 8 * h;
+                    float v0 = acc[16 * j + 4 * q + 2 * h], v1 = acc[16 * j + 4 * q + 2 * h + 1];
+                    if (on[h]) {
+                        const size_t o = (size_t)brow[h] * L + col;
+                        if ((f & MF_LATENT) && io.latent_out) *reinterpret_cast<float2 *>(io.latent_out + o) = make_float2(v0, v1);
+                        if ((f & MF_LATENT) && io.latent_out2) *reinterpret_cast<float2 *>(io.latent_out2 + o) = make_float2(v0, v1);
+                        if ((f & MF_FEAT) && io.feat) *reinterpret_cast<float2 *>(io.feat + o) = make_float2(v0, v1);
+                        if (head) {
+                            const int k = col0 + col;
+                            if (lg && k < ncols) lg[(size_t)brow[h] * ncols + k] = v0;
+                            if (lg && k + 1 < ncols) lg[(size_t)brow[h] * ncols + k + 1] = v1;
+                            if (val && k < ncols) softmax_push(sm_m[h], sm_s[h], sm_w[h], v0, support_at(net.support_min, net.support_step, k));
+                            if (val && k + 1 < ncols) softmax_push(sm_m[h], sm_s[h], sm_w[h], v1, support_at(net.support_min, net.support_step, k + 1));
+                        }
+                    } else {
+                        v0 = v1 = 0.0f;
+                    }
+                    if (ob) {
+                        const float c0 = fminf(fmaxf(v0, -65504.0f), 65504.0f), c1 = fminf(fmaxf(v1, -65504.0f), 65504.0f);
+                        const __half2 hi = __floats2half2_rn(c0, c1);
+                        const float2 back = __half22float2(hi);
+                        unsigned char *d = ob + (col >> 3) * kMezKgBytes + m * 16 + (col & 7) * 2;
+                        *reinterpret_cast<__half2 *>(d) = hi;
+                        *reinterpret_cast<__half2 *>(d + opart) = __floats2half2_rn(c0 - back.x, c1 - back.y);
+                    }
+                }
+        }
+        if (f & MF_CAT_END) {      // the quad's partial (max, sum, weighted sum) triples -> softmax . support -> h^-1
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float M = fmaxf(sm_m[h], __shfl_xor_sync(0xffffffffu, sm_m[h], 1));
+                M = fmaxf(M, __shfl_xor_sync(0xffffffffu, M, 2));
+                const float r = sm_m[h] == -INFINITY ? 0.0f : expf(sm_m[h] - M);
+                float s = sm_s[h] * r, w = sm_w[h] * r;
+                s += __shfl_xor_sync(0xffffffffu, s, 1);
+                w += __shfl_xor_sync(0xffffffffu, w, 1);
+                s += __shfl_xor_sync(0xffffffffu, s, 2);
+                w += __shfl_xor_sync(0xffffffffu, w, 2);
+                if (on[h] && (lane & 3) == 0 && io.value) io.value[brow[h]] = inverse_scalar_transform(w / s);
+            }
+        }
+        fence_proxy_async();
+        __syncthreads();                                      // the layer's output is visible to the next layer's MMAs
+    }
+}
+
+// ---------------------------------------------------------------------------------------------- host
+static int mez_stages(int L)
+{
+    const int fixed = mez_smem(L, 0).total;
+    return std::min(4, (kMezSmemMax - fixed) / (mez_stage_bytes(L) + 8));
+}
+
+// Roots per CTA: 64 (one full m64 tile) whenever the batch has them.  Every CTA streams the whole program's weights from L2
+// (0.3-2.4 MB in tc3), and that stream, not the MMAs, sets a CTA's time; splitting a batch into more, emptier CTAs would not
+// shorten any CTA and would multiply the L2 traffic.  Up to 64 x 132 roots run in one wave.
+MezPlan mez_plan(const MezNet &net, int B)
+{
+    MezPlan p;
+    p.R = std::min(kMezRows, std::max(1, B));
+    p.ctas = ceil_div(B, p.R);
+    p.last = B - (p.ctas - 1) * p.R;
+    p.stages = mez_stages(net.L);
+    p.smem = mez_smem(net.L, p.stages).total;
+    return p;
+}
+
+template <int NC = 1>
+static void mez_go(const MezNet &net, const MezIO &io, const MezPlan &p, cudaStream_t s)
+{
+    if constexpr (NC > kMezMaxL / 32) {
+        return;
+    } else {
+        if (net.L != 32 * NC) return mez_go<NC + 1>(net, io, p, s);
+        k_mez_tc<NC><<<p.ctas, kMezThreads, p.smem, s>>>(net, io, p.R, p.stages);
+    }
+}
+
+template <int NC = 1>
+static int mez_attr()
+{
+    if constexpr (NC > kMezMaxL / 32) {
+        return LZ_OK;
+    } else {
+        LZ_CUDA_CHECK(cudaFuncSetAttribute(k_mez_tc<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMezSmemMax));
+        return mez_attr<NC + 1>();
+    }
+}
+
+int mez_prepare_launch() { return mez_attr<1>(); }
+
+int mez_launch(const MezNet &net, const MezIO &io, cudaStream_t s)
+{
+    LZ_REQUIRE(io.B > 0 && (io.npass == 1 || io.npass == 3), LZ_EINVAL, "mez_launch: bad argument");
+    LZ_REQUIRE(net.L % 32 == 0 && net.L >= 32 && net.L <= kMezMaxL, LZ_EINVAL, "mez_launch: latent %d", net.L);
+    const MezPlan p = mez_plan(net, io.B);
+    LZ_REQUIRE(p.stages >= 2 && p.smem <= kMezSmemMax, LZ_EINVAL, "mez_launch: %d B of shared memory needed", p.smem);
+    mez_go(net, io, p, s);
+    LZ_KERNEL_CHECK();
+    return LZ_OK;
+}
+
+// ---- weights ----------------------------------------------------------------------------------
+namespace {
+
+struct MezPacker {
+    lz_model *m;
+    std::vector<unsigned char> w;
+    std::vector<float> tab;
+
+    const std::vector<float> *get(const std::string &name, size_t expect)
+    {
+        auto it = m->tensors.find(name);
+        if (it == m->tensors.end()) { set_error("lz_model_finalize: missing tensor '%s'", name.c_str()); return nullptr; }
+        if (it->second.size() != expect) {
+            set_error("lz_model_finalize: tensor '%s' has %zu elements, expected %zu", name.c_str(), it->second.size(), expect);
+            return nullptr;
+        }
+        return &it->second;
+    }
+    int add(const std::vector<float> &v)
+    {
+        while (tab.size() % 4) tab.push_back(0.0f);
+        const int off = (int)tab.size();
+        tab.insert(tab.end(), v.begin(), v.end());
+        return off;
+    }
+
+    // Linear `lin` (weight [out_total][in_total]) rows row0 .. row0 + N of inputs 0 .. in_used (+ eval BatchNorm1d `bn`) as one
+    // program layer of K (>= in_used, a multiple of 32) inputs; rows past out_total are zero.  Input columns in_used ..
+    // in_total (the one-hot action) become the [in_total - in_used][N] table `act` times the BN scale.
+    bool layer(MezNet &net, const std::string &lin, const std::string &bn, int in_total, int in_used, int out_total, int row0,
+               int N, int K, int in, int out, int flags, std::vector<float> *act = nullptr)
+    {
+        auto W = get(lin + ".weight", (size_t)out_total * in_total), b = get(lin + ".bias", out_total);
+        if (!W || !b) return false;
+        std::vector<float> s(N, 0.0f), t(N, 0.0f);
+        for (int n = 0; n < N; ++n) {
+            const int r = row0 + n;
+            if (r >= out_total) continue;
+            s[n] = 1.0f;
+            t[n] = (*b)[r];
+        }
+        if (!bn.empty()) {
+            auto g = get(bn + ".weight", out_total), be = get(bn + ".bias", out_total);
+            auto mu = get(bn + ".running_mean", out_total), var = get(bn + ".running_var", out_total);
+            if (!g || !be || !mu || !var) return false;
+            for (int n = 0; n < N && row0 + n < out_total; ++n) {
+                const int r = row0 + n;
+                const float sc = (*g)[r] / sqrtf((*var)[r] + 1e-5f);
+                s[n] = sc;
+                t[n] = (*be)[r] - (*mu)[r] * sc + sc * (*b)[r];
+            }
+        }
+        float mx = 0.0f;
+        for (int n = 0; n < N && row0 + n < out_total; ++n)
+            for (int k = 0; k < in_used; ++k) mx = std::max(mx, fabsf((*W)[(size_t)(row0 + n) * in_total + k]));
+        int e = 0;
+        if (mx > 0.0f) frexpf(mx, &e);
+        const float scale = ldexpf(1.0f, 13 - e);        // largest |w| lands in [4096, 8192): the lo parts stay in fp16's normal range
+        const size_t woff = w.size(), chunk = (size_t)128 * N;
+        w.resize(woff + chunk * (K / 32));
+        __half *hp = reinterpret_cast<__half *>(w.data() + woff);
+        for (int c = 0; c < K / 32; ++c)
+            for (int kg = 0; kg < 4; ++kg)
+                for (int n = 0; n < N; ++n)
+                    for (int u = 0; u < 8; ++u) {
+                        const int k = 32 * c + 8 * kg + u, r = row0 + n;
+                        const float v = (r < out_total && k < in_used) ? (*W)[(size_t)r * in_total + k] * scale : 0.0f;
+                        const __half hi = __float2half_rn(v), lo = __float2half_rn(v - __half2float(hi));
+                        const size_t off = c * chunk / 2 + ((size_t)kg * 2 * N + n) * 8 + u;
+                        hp[off] = hi;
+                        hp[off + (size_t)N * 8] = lo;
+                    }
+        if (act) {
+            const int na = in_total - in_used;
+            act->assign((size_t)na * N, 0.0f);
+            for (int a = 0; a < na; ++a)
+                for (int n = 0; n < N && row0 + n < out_total; ++n)
+                    (*act)[(size_t)a * N + n] = (*W)[(size_t)(row0 + n) * in_total + in_used + a] * s[n];
+        }
+        std::vector<float> st(2 * N);
+        for (int n = 0; n < N; ++n) { st[n] = s[n] / scale; st[N + n] = t[n]; }
+        LZ_REQUIRE(net.nlayers < kMezMaxLayers, false, "lz_model_finalize: more than %d layers", kMezMaxLayers);
+        MezLayer &ly = net.layer[net.nlayers++];
+        ly.woff = (uint32_t)woff; ly.K = K; ly.N = N; ly.in = in; ly.out = out; ly.flags = flags; ly.bn = add(st); ly.col0 = row0;
+        net.nchunks += K / 32;
+        return true;
+    }
+
+    // prediction network on the latent in `src` (common.py:1218-1292); the other slot is its work buffer
+    bool predict(MezNet &net, int src, int L, int A, int K, int vh, int ph)
+    {
+        const std::string Q = "prediction_network.";
+        const int wk = src == MB_SLOT0 ? MB_SLOT1 : MB_SLOT0;
+        bool ok = layer(net, Q + "fc_prediction_common.0", Q + "fc_prediction_common.1", L, L, L, 0, L, L, src, wk, MF_RELU) &&
+                  layer(net, Q + "fc_prediction_common.3", Q + "fc_prediction_common.4", L, L, L, 0, L, L, wk, wk, MF_RELU) &&
+                  layer(net, Q + "fc_value_head.0", Q + "fc_value_head.1", L, L, vh, 0, 32, L, wk, MB_HID, MF_RELU);
+        for (int r0 = 0; ok && r0 < K; r0 += L)
+            ok = layer(net, Q + "fc_value_head.3", "", vh, vh, K, r0, L, 32, MB_HID, MB_NONE,
+                       MF_VALUE | (r0 == 0 ? MF_CAT_BEGIN : 0) | (r0 + L >= K ? MF_CAT_END : 0));
+        ok = ok && layer(net, Q + "fc_policy_head.0", Q + "fc_policy_head.1", L, L, ph, 0, 32, L, wk, MB_HID, MF_RELU);
+        for (int r0 = 0; ok && r0 < A; r0 += L) ok = layer(net, Q + "fc_policy_head.3", "", ph, ph, A, r0, L, 32, MB_HID, MB_NONE, MF_POLICY);
+        return ok;
+    }
+};
+
+}  // namespace
+
+int mez_pack(lz_model *m)
+{
+    const lz_mlp_ez_config &c = m->ecfg;
+    const int L = c.latent_dim, A = c.action_space_size, K = m->K, kobs = (c.obs_dim + 31) / 32 * 32;
+    MezPacker P;
+    P.m = m;
+    MezNet init, rec;
+    memset(&init, 0, sizeof(init));
+    memset(&rec, 0, sizeof(rec));
+    const std::string R = "representation_network.", D = "dynamics_network.";
+    std::vector<float> act;
+    bool ok = P.layer(init, R + "fc_representation.0", R + "fc_representation.1", c.obs_dim, c.obs_dim, L, 0, L, kobs, MB_OBS, MB_SLOT0, MF_GELU) &&
+              P.layer(init, R + "fc_representation.3", "", L, L, L, 0, L, L, MB_SLOT0, MB_SLOT0, MF_LN | MF_LATENT) &&
+              P.predict(init, MB_SLOT0, L, A, K, c.value_hidden, c.policy_hidden);
+    if (ok && c.res_connection_in_dynamics)     // next = fc_dynamics_1([z | a]) + z; LSTM input = fc_dynamics_2(next)
+        ok = P.layer(rec, D + "fc_dynamics_1.0", D + "fc_dynamics_1.1", L + A, L, L, 0, L, L, MB_SLOT0, MB_SLOT1, MF_RELU | MF_ACT, &act) &&
+             P.layer(rec, D + "fc_dynamics_1.3", D + "fc_dynamics_1.4", L, L, L, 0, L, L, MB_SLOT1, MB_SLOT0, MF_RELU | MF_RES | MF_LATENT) &&
+             P.layer(rec, D + "fc_dynamics_2.0", D + "fc_dynamics_2.1", L, L, L, 0, L, L, MB_SLOT0, MB_SLOT1, MF_RELU) &&
+             P.layer(rec, D + "fc_dynamics_2.3", D + "fc_dynamics_2.4", L, L, L, 0, L, L, MB_SLOT1, MB_NONE, MF_RELU | MF_FEAT);
+    else if (ok)                                // next = LSTM input = fc_dynamics([z | a])
+        ok = P.layer(rec, D + "fc_dynamics.0", D + "fc_dynamics.1", L + A, L, L, 0, L, L, MB_SLOT0, MB_SLOT1, MF_RELU | MF_ACT, &act) &&
+             P.layer(rec, D + "fc_dynamics.3", D + "fc_dynamics.4", L, L, L, 0, L, L, MB_SLOT1, MB_SLOT0, MF_RELU | MF_LATENT | MF_FEAT);
+    ok = ok && P.predict(rec, MB_SLOT0, L, A, K, c.value_hidden, c.policy_hidden);
+    if (!ok) return LZ_EINVAL;
+    auto lw = P.get(R + "norm.weight", L), lb = P.get(R + "norm.bias", L);
+    if (!lw || !lb) return LZ_EINVAL;
+    const int o_lw = P.add(*lw), o_lb = P.add(*lb), o_act = P.add(act);
+    const size_t wbytes = (P.w.size() + 255) & ~(size_t)255;
+    if (m->d_mez) cudaFree(m->d_mez);
+    m->d_mez = nullptr;
+    int rc = dev_alloc(&m->d_mez, wbytes + P.tab.size() * sizeof(float));
+    if (rc != LZ_OK) return rc;
+    LZ_CUDA_CHECK(cudaMemcpy(m->d_mez, P.w.data(), P.w.size(), cudaMemcpyHostToDevice));
+    LZ_CUDA_CHECK(cudaMemcpy(m->d_mez + wbytes, P.tab.data(), P.tab.size() * sizeof(float), cudaMemcpyHostToDevice));
+    const float *tab = reinterpret_cast<const float *>(m->d_mez + wbytes);
+    for (MezNet *n : {&init, &rec}) {
+        n->w = m->d_mez; n->tab = tab; n->abias = tab + o_act; n->ln_w = tab + o_lw; n->ln_b = tab + o_lb;
+        n->L = L; n->A = A; n->K = K; n->obs_dim = c.obs_dim;
+        n->support_min = c.support_min; n->support_step = c.support_step;
+    }
+    m->mez_init = init;
+    m->mez_rec = rec;
+    return mez_prepare_launch();
+}
+
+}  // namespace lz

@@ -189,9 +189,42 @@ static BoardIO board_io(const lz_model *m, int B)
     return b;
 }
 
+bool model_is_ez(const lz_model *m) { return (m->kind == 0 && m->cfg.efficientzero) || m->kind == 3; }
+
+static MezIO mez_io(const lz_model *m, int B)
+{
+    MezIO e;
+    memset(&e, 0, sizeof(e));
+    e.B = B; e.npass = m->npass;
+    return e;
+}
+
+// the value-prefix head of the EfficientZero models on the LSTM input features in m->ez_feat (ez.cu)
+static int ez_tail(lz_model *m, const RecIO &io, cudaStream_t s)
+{
+    EzIO e;
+    memset(&e, 0, sizeof(e));
+    e.B = io.B; e.feat = m->ez_feat; e.h_base = io.h_base; e.c_base = io.c_base; e.ix = io.ix; e.slot_stride = io.hslot_stride;
+    e.h_out = io.h_out; e.c_out = io.c_out; e.is_reset = io.is_reset; e.h_tmp = m->ez_htmp;
+    e.value_prefix = io.reward; e.vp_logits = io.reward_logits;
+    return ez_launch(m->ez, e, s);
+}
+
 int model_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
 {
     if (m->kind == 1) return mlp_recurrent(m, io, s);
+    if (m->kind == 3) {
+        // the dense layers on the tensor cores (mlp_tc.cu), their LSTM input through the value-prefix head (ez.cu)
+        LZ_REQUIRE(io.B <= m->ez_B, LZ_ESTATE, "model_recurrent: EfficientZero scratch sized for %d roots, got %d (model_reserve)", m->ez_B, io.B);
+        LZ_REQUIRE(io.h_base && io.c_base, LZ_EINVAL, "model_recurrent: EfficientZero needs the reward hidden state");
+        MezIO e = mez_io(m, io.B);
+        e.latent_base = io.latent_base; e.ix = io.ix; e.slot_stride = io.slot_stride; e.action = io.action;
+        e.latent_out = io.next_latent; e.feat = m->ez_feat;
+        e.value = io.value; e.policy_logits = io.policy_logits; e.value_logits = io.value_logits;
+        int rc = mez_launch(m->mez_rec, e, s);
+        if (rc) return rc;
+        return ez_tail(m, io, s);
+    }
     if (m->kind == 2) {
         BoardIO b = board_io(m, io.B);
         b.latent_base = io.latent_base; b.ix = io.ix; b.slot_stride = io.slot_stride; b.action = io.action;
@@ -217,12 +250,7 @@ int model_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
         t.reward = nullptr; t.reward_logits = nullptr; t.ez_feat = m->ez_feat;
         int rc = tc_launch(m->tc_rec, t, s);
         if (rc) return rc;
-        EzIO e;
-        memset(&e, 0, sizeof(e));
-        e.B = io.B; e.feat = m->ez_feat; e.h_base = io.h_base; e.c_base = io.c_base; e.ix = io.ix; e.slot_stride = io.hslot_stride;
-        e.h_out = io.h_out; e.c_out = io.c_out; e.is_reset = io.is_reset; e.h_tmp = m->ez_htmp;
-        e.value_prefix = io.reward; e.vp_logits = io.reward_logits;
-        return ez_launch(m->ez, e, s);
+        return ez_tail(m, io, s);
     }
     return tc_launch(m->tc_rec, t, s);
 }
@@ -261,11 +289,11 @@ int model_reserve(lz_model *m, int B)
         int rc = reserve_tc_skip(m, B);
         if (rc != LZ_OK) return rc;
     }
-    if (m->kind == 0 && m->cfg.efficientzero && B > m->ez_B) {
+    if (model_is_ez(m) && B > m->ez_B) {
         ++m->generation;
         cudaFree(m->ez_feat); cudaFree(m->ez_htmp);
         m->ez_feat = m->ez_htmp = nullptr;
-        int rc = dev_alloc(&m->ez_feat, (size_t)B * m->cfg.reward_head_channels * m->P);
+        int rc = dev_alloc(&m->ez_feat, (size_t)B * m->ez.nin);
         if (rc == LZ_OK) rc = dev_alloc(&m->ez_htmp, (size_t)B * m->cfg.lstm_hidden_size);
         if (rc != LZ_OK) return rc;
         m->ez_B = B;
@@ -402,6 +430,12 @@ int model_initial_tail(lz_model *m, int B, const float *pre_latent, const TailIO
 int model_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, cudaStream_t s)
 {
     if (m->kind == 1) return mlp_initial(m, B, d_obs, io_in, s);
+    if (m->kind == 3) {
+        MezIO e = mez_io(m, B);
+        e.obs = d_obs; e.latent_out = io_in.latent; e.latent_out2 = io_in.latent2;
+        e.value = io_in.value; e.policy_logits = io_in.policy_logits; e.value_logits = io_in.value_logits;
+        return mez_launch(m->mez_init, e, s);
+    }
     if (m->kind == 2) {
         BoardIO b = board_io(m, B);
         b.obs = d_obs; b.latent_out = io_in.latent; b.latent_out2 = io_in.latent2;
@@ -489,6 +523,92 @@ static bool pack_head(lz_model *m, Packer &P, const std::string &fc, int hc, int
 }
 
 // ---- tensor-core tower tables (conv_tc.cu) ----
+// EfficientZero value-prefix head tables: nn.LSTM(nin -> H) (one step) and fc_reward_head (Linear(H -> hid) + BN1d + ReLU +
+// Linear(hid -> K)), preceded by norm_value_prefix (BN1d + ReLU) in the conv model (efficientzero_model.py:511-525, 556-569) and by
+// nothing in EfficientZeroModelMLP (efficientzero_model_mlp.py:416-429, 466-467).  fp32 tables into P; the tensor-core copy of
+// the LSTM weights into its own allocation m->d_ez_wtc.
+struct EzOff {
+    size_t wcat, bias, vps, vpt, fc1, s2, t2, fc2, b2;
+    float scale;
+    int nin, H, hid;
+    bool vp_norm;
+};
+
+static int pack_ez(lz_model *m, Packer &P, int nin, int H, int hid, bool vp_norm, EzOff &o)
+{
+    const std::string D = "dynamics_network.";
+    const int K = m->K;
+    o.scale = 1.0f; o.nin = nin; o.H = H; o.hid = hid; o.vp_norm = vp_norm;
+    auto Wih = find(m, D + "lstm.weight_ih_l0", (size_t)4 * H * nin), Whh = find(m, D + "lstm.weight_hh_l0", (size_t)4 * H * H);
+    auto bih = find(m, D + "lstm.bias_ih_l0", (size_t)4 * H), bhh = find(m, D + "lstm.bias_hh_l0", (size_t)4 * H);
+    auto W0 = find(m, D + "fc_reward_head.0.weight", (size_t)hid * H), B0 = find(m, D + "fc_reward_head.0.bias", hid);
+    auto W3 = find(m, D + "fc_reward_head.3.weight", (size_t)K * hid), B3 = find(m, D + "fc_reward_head.3.bias", K);
+    std::vector<float> vs, vt, s2, t2;
+    if (!Wih || !Whh || !bih || !bhh || !W0 || !B0 || !W3 || !B3 || (vp_norm && !fold_bn(m, D + "norm_value_prefix", H, vs, vt)) ||
+        !fold_bn(m, D + "fc_reward_head.1", hid, s2, t2))
+        return LZ_EINVAL;
+    for (int j = 0; j < hid; ++j) t2[j] += s2[j] * (*B0)[j];
+    // torch.nn.LSTM stacks the gates (i, f, g, o) along dim 0; column n = unit * 4 + gate
+    std::vector<float> wcat((size_t)(nin + H) * 4 * H), bias((size_t)4 * H), fc1((size_t)H * hid), fc2((size_t)hid * K);
+    for (int g = 0; g < 4; ++g)
+        for (int u = 0; u < H; ++u) {
+            const size_t row = (size_t)g * H + u, col = (size_t)u * 4 + g;
+            for (int k = 0; k < nin; ++k) wcat[(size_t)k * 4 * H + col] = (*Wih)[row * nin + k];
+            for (int k = 0; k < H; ++k) wcat[(size_t)(nin + k) * 4 * H + col] = (*Whh)[row * H + k];
+            bias[col] = (*bih)[row] + (*bhh)[row];
+        }
+    for (int j = 0; j < hid; ++j)
+        for (int i = 0; i < H; ++i) fc1[(size_t)i * hid + j] = (*W0)[(size_t)j * H + i];
+    for (int k = 0; k < K; ++k)
+        for (int j = 0; j < hid; ++j) fc2[(size_t)j * K + k] = (*W3)[(size_t)k * hid + j];
+    if (m->d_ez_wtc) cudaFree(m->d_ez_wtc);
+    m->d_ez_wtc = nullptr;
+    if (ez_tc_shape(nin, H)) {   // tensor-core copy of the LSTM weights (fp16 hi / lo, power-of-two scaled), own allocation;
+                                 // other shapes (e.g. 8 reward-head channels: nin = 288) run the fp32 k_ez_lstm
+        std::vector<unsigned char> wtc(ez_wtc_bytes(nin, H));
+        o.scale = ez_pack_wtc(Wih->data(), Whh->data(), nin, H, wtc.data());
+        int rc2 = dev_alloc(&m->d_ez_wtc, wtc.size());
+        if (rc2 != LZ_OK) return rc2;
+        LZ_CUDA_CHECK(cudaMemcpy(m->d_ez_wtc, wtc.data(), wtc.size(), cudaMemcpyHostToDevice));
+    }
+    o.wcat = P.add(wcat); o.bias = P.add(bias); o.vps = P.add(vs); o.vpt = P.add(vt); o.fc1 = P.add(fc1);
+    o.s2 = P.add(s2); o.t2 = P.add(t2); o.fc2 = P.add(fc2); o.b2 = P.add(*B3);
+    return LZ_OK;
+}
+
+// points m->ez at the tables pack_ez placed in the upload at `base`
+static int bind_ez(lz_model *m, const float *base, const EzOff &o)
+{
+    EzNet &e = m->ez;
+    e.wcat = base + o.wcat; e.bias = base + o.bias; e.vp_s = base + o.vps; e.vp_t = base + o.vpt;
+    e.fc1 = base + o.fc1; e.s2 = base + o.s2; e.t2 = base + o.t2; e.fc2 = base + o.fc2; e.b2 = base + o.b2;
+    e.nin = o.nin; e.H = o.H; e.hid = o.hid; e.K = m->K; e.no_vp_norm = o.vp_norm ? 0 : 1;
+    e.support_min = m->cfg.support_min; e.support_step = m->cfg.support_step;
+    e.wtc = m->d_ez_wtc; e.wtc_inv_scale = 1.0f / o.scale;
+    return ez_prepare_launch();
+}
+
+// EfficientZeroModelMLP: the dense layers (mlp_tc.cu) and the value-prefix head over the latent_dim-wide LSTM input
+static int finalize_mlp_ez(lz_model *m)
+{
+    const lz_mlp_ez_config &c = m->ecfg;
+    int rc = mez_pack(m);
+    if (rc != LZ_OK) return rc;
+    Packer P;
+    EzOff ez;
+    if ((rc = pack_ez(m, P, c.latent_dim, c.lstm_hidden_size, c.reward_hidden, false, ez)) != LZ_OK) return rc;
+    if (m->d_weights) cudaFree(m->d_weights);
+    m->d_weights = nullptr;
+    if ((rc = dev_alloc(&m->d_weights, P.host.size())) != LZ_OK) return rc;
+    LZ_CUDA_CHECK(cudaMemcpy(m->d_weights, P.host.data(), P.host.size() * sizeof(float), cudaMemcpyHostToDevice));
+    m->n_weight_floats = P.host.size();
+    memset(&m->ez, 0, sizeof(m->ez));
+    if ((rc = bind_ez(m, m->d_weights, ez)) != LZ_OK) return rc;
+    m->finalized = true;
+    m->tensors.clear();
+    return LZ_OK;
+}
+
 static int pack_tower_tc(lz_model *m)
 {
     const std::string R = "representation_network.downsample_net.";
@@ -916,12 +1036,50 @@ int lz_model_create(const lz_model_config *cfg, lz_model **out)
     return LZ_OK;
 }
 
+int lz_model_create_mlp_ez(const lz_mlp_ez_config *cfg, lz_model **out)
+{
+    LZ_REQUIRE(cfg && out, LZ_EINVAL, "lz_model_create_mlp_ez: null argument");
+    const lz_mlp_ez_config &c = *cfg;
+    LZ_REQUIRE(c.latent_dim >= 32 && c.latent_dim <= kMezMaxL && c.latent_dim % 32 == 0, LZ_EINVAL,
+               "lz_model_create_mlp_ez: latent_dim must be a multiple of 32 in [32, %d] (got %d)", kMezMaxL, c.latent_dim);
+    LZ_REQUIRE(c.lstm_hidden_size >= 16 && c.lstm_hidden_size <= 512 && c.lstm_hidden_size % 16 == 0, LZ_EINVAL,
+               "lz_model_create_mlp_ez: lstm_hidden_size must be a multiple of 16 in [16, 512] (got %d)", c.lstm_hidden_size);
+    LZ_REQUIRE(c.obs_dim >= 1 && c.obs_dim <= kMezMaxObs, LZ_EINVAL, "lz_model_create_mlp_ez: obs_dim must be in [1, %d] (got %d)",
+               kMezMaxObs, c.obs_dim);
+    LZ_REQUIRE(c.action_space_size >= 1 && c.action_space_size <= kMezMaxOut, LZ_EINVAL,
+               "lz_model_create_mlp_ez: action_space_size must be in [1, %d] (got %d)", kMezMaxOut, c.action_space_size);
+    LZ_REQUIRE(c.reward_hidden >= 1 && c.reward_hidden <= kMezMaxHid && c.value_hidden >= 1 && c.value_hidden <= kMezMaxHid &&
+                   c.policy_hidden >= 1 && c.policy_hidden <= kMezMaxHid, LZ_EINVAL,
+               "lz_model_create_mlp_ez: head hidden sizes must be in [1, %d] (got %d, %d, %d)", kMezMaxHid, c.reward_hidden,
+               c.value_hidden, c.policy_hidden);
+    const int K = (int)ceil((c.support_max - c.support_min) / c.support_step);      // len(torch.arange(min, max, step))
+    LZ_REQUIRE(K >= 2 && K <= kMezMaxOut, LZ_EINVAL, "lz_model_create_mlp_ez: support size %d not in [2, %d]", K, kMezMaxOut);
+    int ndev = 0;
+    LZ_CUDA_CHECK(cudaGetDeviceCount(&ndev));
+    LZ_REQUIRE(ndev > 0, LZ_ECUDA, "lz_model_create_mlp_ez: no CUDA device (this library has no CPU fallback)");
+    lz_model *m = new lz_model();
+    m->kind = 3;
+    m->ecfg = c;
+    m->cfg.action_space_size = c.action_space_size;
+    m->cfg.support_min = c.support_min; m->cfg.support_max = c.support_max; m->cfg.support_step = c.support_step;
+    m->cfg.lstm_hidden_size = c.lstm_hidden_size;
+    m->cfg.reward_hidden = c.reward_hidden; m->cfg.value_hidden = c.value_hidden; m->cfg.policy_hidden = c.policy_hidden;
+    m->latent_floats = c.latent_dim;
+    m->lat_c = c.latent_dim; m->lat_h = m->lat_w = 1;
+    m->hw = 1; m->P = 1; m->K = K;
+    m->npass = 3;                      // default: tc3 (fp32-accurate)
+    m->finalized = false;
+    *out = m;
+    return LZ_OK;
+}
+
 int lz_model_destroy(lz_model *m)
 {
     if (!m) return LZ_OK;
     cudaFree(m->d_weights);
     cudaFree(m->d_tc);
     cudaFree(m->d_board);
+    cudaFree(m->d_mez);
     cudaFree(m->d_tower);
     cudaFree(m->tws);
     cudaFree(m->tc_skip);
@@ -949,6 +1107,7 @@ int lz_model_finalize(lz_model *m)
     LZ_REQUIRE(m, LZ_EINVAL, "lz_model_finalize: null model");
     ++m->generation;          // every device table is re-allocated below: graphs captured against the old ones are stale
     if (m->kind == 1) return mlp_finalize(m);
+    if (m->kind == 3) return finalize_mlp_ez(m);
     if (m->kind == 2) {
         int rc = pack_board(m);
         if (rc != LZ_OK) return rc;
@@ -968,44 +1127,10 @@ int lz_model_finalize(lz_model *m)
               pack_head(m, P, Q + "fc_policy", c.policy_head_channels, c.policy_hidden, A, hp);
     if (!ok) return LZ_EINVAL;
     // ---- EfficientZero value-prefix head (efficientzero_model.py:511-525, 556-569)
-    float ez_scale = 1.0f;
-    size_t ez_wcat = 0, ez_bias = 0, ez_vps = 0, ez_vpt = 0, ez_fc1 = 0, ez_s2 = 0, ez_t2 = 0, ez_fc2 = 0, ez_b2 = 0;
+    EzOff ez;
     if (c.efficientzero) {
-        const int H = c.lstm_hidden_size, nin = c.reward_head_channels * m->P, hid = c.reward_hidden, K = m->K;
-        auto Wih = find(m, D + "lstm.weight_ih_l0", (size_t)4 * H * nin), Whh = find(m, D + "lstm.weight_hh_l0", (size_t)4 * H * H);
-        auto bih = find(m, D + "lstm.bias_ih_l0", (size_t)4 * H), bhh = find(m, D + "lstm.bias_hh_l0", (size_t)4 * H);
-        auto W0 = find(m, D + "fc_reward_head.0.weight", (size_t)hid * H), B0 = find(m, D + "fc_reward_head.0.bias", hid);
-        auto W3 = find(m, D + "fc_reward_head.3.weight", (size_t)K * hid), B3 = find(m, D + "fc_reward_head.3.bias", K);
-        std::vector<float> vs, vt, s2, t2;
-        if (!Wih || !Whh || !bih || !bhh || !W0 || !B0 || !W3 || !B3 || !fold_bn(m, D + "norm_value_prefix", H, vs, vt) ||
-            !fold_bn(m, D + "fc_reward_head.1", hid, s2, t2))
-            return LZ_EINVAL;
-        for (int j = 0; j < hid; ++j) t2[j] += s2[j] * (*B0)[j];
-        // torch.nn.LSTM stacks the gates (i, f, g, o) along dim 0; column n = unit * 4 + gate
-        std::vector<float> wcat((size_t)(nin + H) * 4 * H), bias((size_t)4 * H), fc1((size_t)H * hid), fc2((size_t)hid * K);
-        for (int g = 0; g < 4; ++g)
-            for (int u = 0; u < H; ++u) {
-                const size_t row = (size_t)g * H + u, col = (size_t)u * 4 + g;
-                for (int k = 0; k < nin; ++k) wcat[(size_t)k * 4 * H + col] = (*Wih)[row * nin + k];
-                for (int k = 0; k < H; ++k) wcat[(size_t)(nin + k) * 4 * H + col] = (*Whh)[row * H + k];
-                bias[col] = (*bih)[row] + (*bhh)[row];
-            }
-        for (int j = 0; j < hid; ++j)
-            for (int i = 0; i < H; ++i) fc1[(size_t)i * hid + j] = (*W0)[(size_t)j * H + i];
-        for (int k = 0; k < K; ++k)
-            for (int j = 0; j < hid; ++j) fc2[(size_t)j * K + k] = (*W3)[(size_t)k * hid + j];
-        if (m->d_ez_wtc) cudaFree(m->d_ez_wtc);
-        m->d_ez_wtc = nullptr;
-        if (ez_tc_shape(nin, H)) {   // tensor-core copy of the LSTM weights (fp16 hi / lo, power-of-two scaled), own allocation;
-                                     // other shapes (e.g. 8 reward-head channels: nin = 288) run the fp32 k_ez_lstm
-            std::vector<unsigned char> wtc(ez_wtc_bytes(nin, H));
-            ez_scale = ez_pack_wtc(Wih->data(), Whh->data(), nin, H, wtc.data());
-            int rc2 = dev_alloc(&m->d_ez_wtc, wtc.size());
-            if (rc2 != LZ_OK) return rc2;
-            LZ_CUDA_CHECK(cudaMemcpy(m->d_ez_wtc, wtc.data(), wtc.size(), cudaMemcpyHostToDevice));
-        }
-        ez_wcat = P.add(wcat); ez_bias = P.add(bias); ez_vps = P.add(vs); ez_vpt = P.add(vt); ez_fc1 = P.add(fc1);
-        ez_s2 = P.add(s2); ez_t2 = P.add(t2); ez_fc2 = P.add(fc2); ez_b2 = P.add(*B3);
+        const int rc0 = pack_ez(m, P, c.reward_head_channels * m->P, c.lstm_hidden_size, c.reward_hidden, true, ez);
+        if (rc0 != LZ_OK) return rc0;
     }
 
     if (m->d_weights) cudaFree(m->d_weights);
@@ -1023,13 +1148,7 @@ int lz_model_finalize(lz_model *m)
     };
     memset(&m->ez, 0, sizeof(m->ez));
     if (c.efficientzero) {
-        EzNet &e = m->ez;
-        e.wcat = base + ez_wcat; e.bias = base + ez_bias; e.vp_s = base + ez_vps; e.vp_t = base + ez_vpt;
-        e.fc1 = base + ez_fc1; e.s2 = base + ez_s2; e.t2 = base + ez_t2; e.fc2 = base + ez_fc2; e.b2 = base + ez_b2;
-        e.nin = c.reward_head_channels * m->P; e.H = c.lstm_hidden_size; e.hid = c.reward_hidden; e.K = m->K;
-        e.support_min = c.support_min; e.support_step = c.support_step;
-        e.wtc = m->d_ez_wtc; e.wtc_inv_scale = 1.0f / ez_scale;
-        int rc3 = ez_prepare_launch();
+        int rc3 = bind_ez(m, base, ez);
         if (rc3 != LZ_OK) return rc3;
     }
 
@@ -1097,7 +1216,7 @@ int lz_model_latent_hw(const lz_model *m) { return m ? m->hw : 0; }
 int lz_model_latent_shape(const lz_model *m, int32_t *h_c, int32_t *h_h, int32_t *h_w)
 {
     LZ_REQUIRE(m, LZ_EINVAL, "lz_model_latent_shape: null model");
-    const bool mlp = m->kind == 1;
+    const bool mlp = m->kind == 1 || m->kind == 3;
     if (h_c) *h_c = mlp ? m->latent_floats : m->lat_c;
     if (h_h) *h_h = mlp ? 1 : m->lat_h;
     if (h_w) *h_w = mlp ? 1 : m->lat_w;
@@ -1222,13 +1341,53 @@ static int board_debug_stage(lz_model *m, int which, int B, const float *d_in, c
     return board_launch(net, io, st);
 }
 
+// lz_model_debug_net_stage of EfficientZeroModelMLP: which 1 is initial_inference on the observations d_in
+static int mez_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out,
+                           size_t out_bytes, int32_t *h_info, cudaStream_t st)
+{
+    MezNet net = which ? m->mez_init : m->mez_rec;          // a copy: the model's programs stay as they are
+    const int L = net.L, K = net.K, A = net.A;
+    int D = 0;                                              // the L-wide layers before the heads
+    while (D < net.nlayers && net.layer[D].N == L && !(net.layer[D].flags & (MF_VALUE | MF_POLICY)) && net.layer[D].out != MB_HID) ++D;
+    LZ_REQUIRE(stage <= D, LZ_EINVAL, "lz_model_debug_net_stage: stage %d past the %d dense layers of the program", stage, D);
+    const size_t nfl = stage < D ? (size_t)B * L : (size_t)B * (K + A + 1 + 2 * L);
+    LZ_REQUIRE(out_bytes >= nfl * sizeof(float), LZ_EINVAL, "lz_model_debug_net_stage: stage %d needs %zu bytes, got %zu", stage,
+               nfl * sizeof(float), out_bytes);
+    MezIO io = mez_io(m, B);
+    if (which) io.obs = d_in;
+    else { io.latent_base = d_in; io.action = d_action; }
+    float *o = reinterpret_cast<float *>(d_out);
+    if (stage < D) {
+        // the program cut after layer `stage`, whose output is the only one written
+        net.nlayers = stage + 1;
+        net.nchunks = 0;
+        for (int l = 0; l <= stage; ++l) {
+            net.layer[l].flags &= ~(MF_LATENT | MF_FEAT);
+            net.nchunks += net.layer[l].K / 32;
+        }
+        net.layer[stage].flags |= MF_LATENT;
+        io.latent_out = o;
+    } else {
+        // the latent sections first: the kernel writes them as float2 pairs
+        LZ_CUDA_CHECK(cudaMemsetAsync(d_out, 0, nfl * sizeof(float), st));
+        io.latent_out = o;
+        if (!which) io.feat = o + (size_t)B * L;
+        io.value_logits = o + (size_t)2 * B * L; io.policy_logits = io.value_logits + (size_t)B * K; io.value = io.policy_logits + (size_t)B * A;
+    }
+    const MezPlan p = mez_plan(net, B);
+    const int32_t info[8] = {p.R, p.ctas, p.last, net.nlayers, m->npass, p.smem, p.stages, D};
+    memcpy(h_info, info, sizeof(info));
+    return mez_launch(net, io, st);
+}
+
 int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_latent, const int32_t *d_action, int stage, void *d_out,
                              size_t out_bytes, int32_t *h_info, lz_stream s)
 {
     LZ_REQUIRE(m && (which == 0 || which == 1) && B > 0 && d_latent && (which == 1 || d_action) && d_out && h_info && stage >= 0,
                LZ_EINVAL, "lz_model_debug_net_stage: bad argument");
-    LZ_REQUIRE(m->finalized && (m->kind == 0 || m->kind == 2), LZ_ESTATE, "lz_model_debug_net_stage: not a finalized conv model");
+    LZ_REQUIRE(m->finalized && m->kind != 1, LZ_ESTATE, "lz_model_debug_net_stage: not a finalized conv, board or EfficientZeroModelMLP model");
     if (m->kind == 2) return board_debug_stage(m, which, B, d_latent, d_action, stage, d_out, out_bytes, h_info, (cudaStream_t)s);
+    if (m->kind == 3) return mez_debug_stage(m, which, B, d_latent, d_action, stage, d_out, out_bytes, h_info, (cudaStream_t)s);
     TcNet net = which ? m->tc_tail : m->tc_rec;          // a copy: the model's programs stay as they are
     const int nl = net.nlayers, K = m->K, A = m->cfg.action_space_size;
     const bool ez = m->cfg.efficientzero != 0 && which == 0;
@@ -1299,7 +1458,7 @@ int lz_model_recurrent_inference_ez(lz_model *m, int B, const float *d_latent, c
                                     float *d_value_prefix, float *d_value, lz_stream s)
 {
     LZ_REQUIRE(m && d_latent && d_hidden0 && d_hidden1 && d_action && d_next_latent && B > 0, LZ_EINVAL, "lz_model_recurrent_inference_ez: bad argument");
-    LZ_REQUIRE(m->finalized && m->kind == 0 && m->cfg.efficientzero, LZ_ESTATE, "lz_model_recurrent_inference_ez: not a finalized EfficientZero model");
+    LZ_REQUIRE(m->finalized && model_is_ez(m), LZ_ESTATE, "lz_model_recurrent_inference_ez: not a finalized EfficientZero model");
     if (B > m->ez_B || B > m->tc_skip_B) {
         int rc = model_reserve(m, B);
         if (rc != LZ_OK) return rc;
@@ -1313,7 +1472,7 @@ int lz_model_recurrent_inference_ez(lz_model *m, int B, const float *d_latent, c
     return model_recurrent(m, io, (cudaStream_t)s);
 }
 
-int lz_model_lstm_hidden_size(const lz_model *m) { return (m && m->kind == 0 && m->cfg.efficientzero) ? m->cfg.lstm_hidden_size : 0; }
+int lz_model_lstm_hidden_size(const lz_model *m) { return (m && model_is_ez(m)) ? m->cfg.lstm_hidden_size : 0; }
 
 int lz_inverse_scalar_transform(lz_model *m, int B, const float *d_logits, float *d_out, lz_stream s)
 {

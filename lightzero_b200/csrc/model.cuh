@@ -10,6 +10,7 @@
 #include "conv_tc.cuh"
 #include "ez.cuh"
 #include "board_tc.cuh"
+#include "mlp_tc.cuh"
 
 namespace lz {
 
@@ -67,9 +68,12 @@ struct TailIO {
 
 struct lz_model {
     int kind;                         // 0 = conv MuZeroModel / EfficientZeroModel (cfg.efficientzero), 1 = MuZeroModelMLP,
-                                      // 2 = board MuZeroModel (downsample=False, board_tc.cu)
+                                      // 2 = board MuZeroModel (downsample=False, board_tc.cu), 3 = EfficientZeroModelMLP (mlp_tc.cu)
     unsigned char *d_board;           // kind 2: packed conv weights, BN / action-plane tables and fp32 head tables
     lz::BoardNet board_rec, board_init;   // kind 2: recurrent_inference / initial_inference programs
+    lz_mlp_ez_config ecfg;            // kind 3
+    unsigned char *d_mez;             // kind 3: packed fp16 hi / lo weights and fp32 tables of the dense layers
+    lz::MezNet mez_rec, mez_init;     // kind 3: recurrent_inference (dense part) / initial_inference programs
     int lat_c, lat_h, lat_w;          // latent shape of one root
     lz::EzNet ez;                     // EfficientZero value-prefix head tables (device pointers into d_weights)
     float *ez_feat, *ez_htmp;         // [ws_B][hc*36], [ws_B][H] scratch between the conv kernel and the LSTM kernels
@@ -115,4 +119,5 @@ int model_reserve(lz_model *m, int B);   // sizes the initial-inference workspac
 int mlp_recurrent(lz_model *m, const RecIO &io, cudaStream_t s);
 int mlp_initial(lz_model *m, int B, const float *d_obs, const TailIO &io, cudaStream_t s);
 int mlp_finalize(lz_model *m);
+bool model_is_ez(const lz_model *m);     // EfficientZero (value-prefix LSTM head): conv EfficientZeroModel or EfficientZeroModelMLP
 }  // namespace lz

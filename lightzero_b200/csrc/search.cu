@@ -243,7 +243,7 @@ int lz_search_create(lz_tree *t, lz_model *m, int num_simulations, lz_search **o
     LZ_REQUIRE(m->finalized, LZ_ESTATE, "lz_search_create: model not finalized");
     LZ_REQUIRE(num_simulations <= t->max_sims, LZ_EINVAL, "lz_search_create: num_simulations %d > tree capacity %d", num_simulations, t->max_sims);
     LZ_REQUIRE(t->p.A == m->cfg.action_space_size, LZ_EINVAL, "lz_search_create: tree has %d actions, model %d", t->p.A, m->cfg.action_space_size);
-    const bool ez = m->kind == 0 && m->cfg.efficientzero;
+    const bool ez = model_is_ez(m);
     LZ_REQUIRE(ez == (t->p.ez != 0), LZ_EINVAL, "lz_search_create: %s model needs a tree in %s mode (lz_tree_set_ez)",
                ez ? "an EfficientZero" : "a MuZero", ez ? "EfficientZero" : "MuZero");
     lz_search *q = new lz_search();
@@ -398,7 +398,8 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
     cudaStream_t s = (cudaStream_t)s_;
     const lz_model_config &c = q->model->cfg;
     const int B = q->B, A = q->A;
-    const size_t obs_elems = q->model->kind == 1 ? (size_t)q->model->mcfg.obs_dim : (size_t)c.obs_c * c.obs_h * c.obs_w;
+    const size_t obs_elems = q->model->kind == 1 ? (size_t)q->model->mcfg.obs_dim
+                             : q->model->kind == 3 ? (size_t)q->model->ecfg.obs_dim : (size_t)c.obs_c * c.obs_h * c.obs_w;
     nchunks = nchunks < 1 ? 1 : (nchunks > 8 ? 8 : nchunks);
     if (!q->copy_stream) {
         q->obs_elems = obs_elems;

@@ -22,6 +22,7 @@ import torch
 
 from . import cabi, ez_tree, gmz_tree, mz_tree
 from .efficientzero_model import EfficientZeroModel
+from .efficientzero_model_mlp import EfficientZeroModelMLP
 from .muzero_model import MuZeroModel
 from .muzero_model_mlp import MuZeroModelMLP
 from .scaling_transform import DiscreteSupport, InverseScalarTransform
@@ -103,8 +104,8 @@ class MuZeroMCTSCtree(object):
             lat = latent_state_roots.to(dev, torch.float32, non_blocking=True).contiguous()
         else:
             lat = torch.from_numpy(np.ascontiguousarray(latent_state_roots, dtype=np.float32)).to(dev, non_blocking=True)
-        if isinstance(model, EfficientZeroModel):
-            raise TypeError("MuZeroMCTSCtree.search: an EfficientZeroModel needs EfficientZeroMCTSCtree")
+        if isinstance(model, (EfficientZeroModel, EfficientZeroModelMLP)):
+            raise TypeError(f"MuZeroMCTSCtree.search: an {type(model).__name__} needs EfficientZeroMCTSCtree")
         if isinstance(model, (MuZeroModel, MuZeroModelMLP)):
             q = t.search_for(model, S)
             with torch.cuda.device(dev):
@@ -189,7 +190,7 @@ class EfficientZeroMCTSCtree(MuZeroMCTSCtree):
     (+ ``lstm_horizon_len``, read at :857), ``roots(n, legal_actions)`` and
     ``search(roots, model, latent_state_roots, reward_hidden_state_roots, to_play_batch)``.
 
-    With a ``lightzero_b200.EfficientZeroModel`` the whole loop is one CUDA-graph launch (``lz_search_run_ez``): per
+    With a ``lightzero_b200.EfficientZeroModel`` or ``EfficientZeroModelMLP`` the whole loop is one CUDA-graph launch (``lz_search_run_ez``): per
     simulation the descent (which also derives ``is_reset = search_len % lstm_horizon_len == 0``, :856-861), the conv
     trunk + prediction heads, the LSTM value-prefix head over all roots, and the back-up.  Any other model object is
     driven step-wise around the device trees.  Ties: first maximum (the reference's ``rand() % len(ties)`` with
@@ -225,7 +226,7 @@ class EfficientZeroMCTSCtree(MuZeroMCTSCtree):
         B = roots.num
         h0 = dev_f32(reward_hidden_state_roots[0]).reshape(B, -1)
         h1 = dev_f32(reward_hidden_state_roots[1]).reshape(B, -1)
-        if isinstance(model, EfficientZeroModel):
+        if isinstance(model, (EfficientZeroModel, EfficientZeroModelMLP)):
             q = t.search_for(model, S, (1, H))
             with torch.cuda.device(dev):
                 cabi.check(t.lib.lz_search_run_ez(q, lat.data_ptr(), h0.data_ptr(), h1.data_ptr(), cabi.stream_ptr()),
@@ -241,8 +242,9 @@ class EfficientZeroMCTSCtree(MuZeroMCTSCtree):
         ``ez_tree.batch_traverse_with_reuse`` / ``batch_backpropagate_with_reuse`` themselves."""
         S, H = int(self._cfg.num_simulations), int(self._cfg.lstm_horizon_len)
         assert H > 0
-        if not isinstance(model, EfficientZeroModel):
-            raise NotImplementedError("EfficientZeroMCTSCtree.search_with_reuse is fused only: pass a lightzero_b200 EfficientZeroModel")
+        if not isinstance(model, (EfficientZeroModel, EfficientZeroModelMLP)):
+            raise NotImplementedError("EfficientZeroMCTSCtree.search_with_reuse is fused only: pass a lightzero_b200 EfficientZeroModel "
+                                      "or EfficientZeroModelMLP")
         roots._ez, roots._lstm_horizon = True, H
         roots._materialize(S, self._params())
         t = roots._tree
@@ -392,8 +394,8 @@ class GumbelMuZeroMCTSCtree(MuZeroMCTSCtree):
 
     def search(self, roots: "gmz_tree.Roots", model, latent_state_roots, to_play_batch: Union[int, List[Any]]) -> None:
         """mcts_ctree.py:1076-1172.  ``latent_state_roots``: np.ndarray or CUDA tensor."""
-        if isinstance(model, EfficientZeroModel):
-            raise TypeError("GumbelMuZeroMCTSCtree.search: the Gumbel search runs MuZero models, not an EfficientZeroModel")
+        if isinstance(model, (EfficientZeroModel, EfficientZeroModelMLP)):
+            raise TypeError(f"GumbelMuZeroMCTSCtree.search: the Gumbel search runs MuZero models, not an {type(model).__name__}")
         S = int(self._cfg.num_simulations)
         if roots._pending is None:
             raise RuntimeError("Roots: prepare()/prepare_no_noise() has not been called")
