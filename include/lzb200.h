@@ -201,7 +201,14 @@ int lz_model_create(const lz_model_config *cfg, lz_model **out);
 
 /* MuZeroModelMLP (lzero/model/muzero_model_mlp.py:21-295; vector observations, BASELINE config 1).  The
  * handle is used with the same lz_model_* / lz_search_* calls: d_obs is f32 [B, obs_dim], latents are
- * f32 [B, latent_dim].  State-dict names follow muzero_model_mlp.py / common.py:790-850,1218-1292. */
+ * f32 [B, latent_dim].  State-dict names follow muzero_model_mlp.py / common.py:790-850,1218-1292.
+ * Two kernels run it, chosen from the config alone:
+ *   - the fp32 CUDA-core kernels take latent_dim 8-128, obs_dim 1-160, latent_dim + action_space_size <= 160 and head hidden
+ *     sizes <= 160 (no math mode: lz_model_set_math is LZ_EINVAL);
+ *   - every other config with latent_dim a multiple of 32 in [32, 256], obs_dim 1-4096, action_space_size 1-608 and head
+ *     hidden sizes 1-32 runs on the tensor-core kernel of EfficientZeroModelMLP (math modes tc3 / tc1; latent buffers in and
+ *     out 16-byte aligned).
+ * Support size <= 608; anything else is LZ_EINVAL. */
 typedef struct lz_mlp_config {
     int obs_dim, action_space_size, latent_dim;         /* 4, 2, 128 for CartPole */
     int reward_hidden, value_hidden, policy_hidden;     /* one hidden layer each: 32 */
@@ -235,7 +242,7 @@ int lz_model_finalize(lz_model *m);
  *   1 = tc3: fp16 hi/lo operand splitting (3 MMAs per product, fp32 accumulate in registers): fp32-accurate, the default
  *       and the mode parity is stated for;
  *   2 = tc1: single fp16 pass (fp32 accumulate): ~3x fewer MMAs, logits accurate to ~1e-3.
- * Any other mode, and any mode on the MLP model, is LZ_EINVAL. */
+ * Any other mode, and any mode on a MuZeroModelMLP that runs on the fp32 MLP kernels, is LZ_EINVAL. */
 int lz_model_set_math(lz_model *m, int mode);
 /* Test hook: overrides the layer program of the tensor-core kernels (see net_tc.cuh LF_* flags). */
 int lz_model_debug_tc_program(lz_model *m, int which, int nlayers, const int *layer_w, const int *layer_flags,

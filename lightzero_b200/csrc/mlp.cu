@@ -290,15 +290,36 @@ int mlp_finalize(lz_model *m)
 
 using namespace lz;
 
+// The fp32 kernels above take the configs they were sized for; every other config inside k_mez_tc's envelope (mlp_tc.cu) runs
+// there as model kind 4.  The choice follows from the config alone, and a config both take stays on these kernels, so its
+// outputs do not change.
+static bool mlp_fits(const lz_mlp_config &c)
+{
+    return c.latent_dim >= 8 && c.latent_dim <= 128 && c.obs_dim >= 1 && c.obs_dim <= kMlpWidth && c.action_space_size >= 1 &&
+           c.latent_dim + c.action_space_size <= kMlpWidth && c.reward_hidden <= kMlpWidth && c.value_hidden <= kMlpWidth &&
+           c.policy_hidden <= kMlpWidth;
+}
+
+static bool mez_fits(const lz_mlp_config &c)
+{
+    auto hid = [](int h) { return h >= 1 && h <= kMezMaxHid; };
+    return c.latent_dim >= 32 && c.latent_dim <= kMezMaxL && c.latent_dim % 32 == 0 && c.obs_dim >= 1 && c.obs_dim <= kMezMaxObs &&
+           c.action_space_size >= 1 && c.action_space_size <= kMezMaxOut && hid(c.reward_hidden) && hid(c.value_hidden) &&
+           hid(c.policy_hidden);
+}
+
 extern "C" int lz_model_create_mlp(const lz_mlp_config *cfg, lz_model **out)
 {
     LZ_REQUIRE(cfg && out, LZ_EINVAL, "lz_model_create_mlp: null argument");
-    LZ_REQUIRE(cfg->latent_dim >= 8 && cfg->latent_dim <= 128 && cfg->obs_dim >= 1 && cfg->obs_dim <= kMlpWidth, LZ_EINVAL,
-               "lz_model_create_mlp: latent_dim must be in [8,128], obs_dim in [1,%d]", kMlpWidth);
-    LZ_REQUIRE(cfg->action_space_size >= 1 && cfg->latent_dim + cfg->action_space_size <= kMlpWidth, LZ_EINVAL,
-               "lz_model_create_mlp: latent_dim + action_space_size must be <= %d", kMlpWidth);
-    LZ_REQUIRE(cfg->reward_hidden <= kMlpWidth && cfg->value_hidden <= kMlpWidth && cfg->policy_hidden <= kMlpWidth, LZ_EINVAL,
-               "lz_model_create_mlp: head hidden sizes must be <= %d", kMlpWidth);
+    const lz_mlp_config &c = *cfg;
+    const bool fp32 = mlp_fits(c);
+    LZ_REQUIRE(fp32 || mez_fits(c), LZ_EINVAL,
+               "lz_model_create_mlp: latent_dim %d, obs_dim %d, action_space_size %d, head hidden sizes %d / %d / %d fit neither the "
+               "fp32 MLP kernels (latent_dim in [8,128], obs_dim in [1,%d], latent_dim + action_space_size <= %d, head hidden sizes <= %d) "
+               "nor the tensor-core MLP kernel (latent_dim a multiple of 32 in [32,%d], obs_dim in [1,%d], action_space_size in [1,%d], "
+               "head hidden sizes in [1,%d])",
+               c.latent_dim, c.obs_dim, c.action_space_size, c.reward_hidden, c.value_hidden, c.policy_hidden, kMlpWidth, kMlpWidth,
+               kMlpWidth, kMezMaxL, kMezMaxObs, kMezMaxOut, kMezMaxHid);
     const int K = (int)ceil((cfg->support_max - cfg->support_min) / cfg->support_step);
     LZ_REQUIRE(K >= 2 && K <= kMlpK, LZ_EINVAL, "lz_model_create_mlp: support size %d not in [2, %d]", K, kMlpK);
     int ndev = 0;
@@ -309,12 +330,25 @@ extern "C" int lz_model_create_mlp(const lz_mlp_config *cfg, lz_model **out)
     m->cfg.action_space_size = cfg->action_space_size;
     m->cfg.support_min = cfg->support_min; m->cfg.support_max = cfg->support_max; m->cfg.support_step = cfg->support_step;
     m->mcfg = *cfg;
-    m->kind = 1;
     m->latent_floats = cfg->latent_dim;
     m->finalized = false;
     m->d_weights = nullptr; m->d_tc = nullptr; m->d_tower = nullptr; m->tws = nullptr; m->tws_bytes = 0;
     m->hw = 1; m->P = 1; m->K = K;
-    m->pre_latent = nullptr; m->ws_B = 1 << 30;
+    if (fp32) {
+        m->kind = 1;
+        m->pre_latent = nullptr; m->ws_B = 1 << 30;
+    } else {
+        m->kind = 4;
+        lz_mlp_ez_config &e = m->ecfg;       // the config mez_pack reads
+        memset(&e, 0, sizeof(e));
+        e.obs_dim = c.obs_dim; e.action_space_size = c.action_space_size; e.latent_dim = c.latent_dim;
+        e.reward_hidden = c.reward_hidden; e.value_hidden = c.value_hidden; e.policy_hidden = c.policy_hidden;
+        e.res_connection_in_dynamics = c.res_connection_in_dynamics;
+        e.support_min = c.support_min; e.support_max = c.support_max; e.support_step = c.support_step;
+        m->cfg.reward_hidden = c.reward_hidden; m->cfg.value_hidden = c.value_hidden; m->cfg.policy_hidden = c.policy_hidden;
+        m->lat_c = c.latent_dim; m->lat_h = m->lat_w = 1;
+        m->npass = 3;                      // default: tc3 (fp32-accurate)
+    }
     *out = m;
     return LZ_OK;
 }

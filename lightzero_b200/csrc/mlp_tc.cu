@@ -1,8 +1,10 @@
-// mlp_tc.cu -- tensor-core (wgmma) network of EfficientZeroModelMLP (lzero/model/efficientzero_model_mlp.py:150-300):
-// representation Linear(obs -> L) + BN + GELU(tanh) + Linear(L -> L) + LayerNorm (common.py:790-850), the dynamics MLPs over
-// [latent | one-hot action] (fc_dynamics, or fc_dynamics_1 + latent -> fc_dynamics_2 with res_connection_in_dynamics,
-// efficientzero_model_mlp.py:440-468) and the prediction MLPs (common.py:1218-1292).  The LSTM value-prefix head that follows the
-// dynamics network runs in ez.cu on the LSTM input this kernel writes.
+// mlp_tc.cu -- tensor-core (wgmma) network of EfficientZeroModelMLP (lzero/model/efficientzero_model_mlp.py:150-300) and
+// MuZeroModelMLP (lzero/model/muzero_model_mlp.py:21-442): representation Linear(obs -> L) + BN + GELU(tanh) + Linear(L -> L) +
+// LayerNorm (common.py:790-850), the dynamics MLPs over [latent | one-hot action] (fc_dynamics, or fc_dynamics_1 + latent ->
+// fc_dynamics_2 with res_connection_in_dynamics, efficientzero_model_mlp.py:440-468, muzero_model_mlp.py:428-438) and the
+// prediction MLPs (common.py:1218-1292).  EfficientZeroModelMLP's LSTM value-prefix head that follows the dynamics network runs
+// in ez.cu on the LSTM input this kernel writes; MuZeroModelMLP's categorical reward head (fc_reward_head, muzero_model_mlp.py:440)
+// runs in the recurrent program itself, the same way as the value head.
 //
 // One launch runs a whole layer program (initial_inference, or the dense part of recurrent_inference) for all roots; a CTA of one
 // warpgroup owns up to 64 roots, the rows of one m64 wgmma tile.  Arithmetic as net_tc.cu / board_tc.cu: 3xFP16 (A_hi B_hi +
@@ -15,7 +17,7 @@
 // straight from the fragments: folded BN / bias, the one-hot action as a gathered fp32 weight row, ReLU or GELU, the residual
 // from the fp32 input latent, LayerNorm (a row lives in one lane quad: two quad-shuffle reductions), then the fp16 hi / lo
 // rewrite of the next layer's operand and the fp32 outputs.  The last Linear of each head is cut into pieces of <= L outputs
-// (K = 32 inputs) that run the same way; the value head's softmax expectation is folded online across its pieces.
+// (K = 32 inputs) that run the same way; the value (and reward) head's softmax expectation is folded online across its pieces.
 #include <cuda_fp16.h>
 #include <math.h>
 #include <string.h>
@@ -152,7 +154,7 @@ __global__ void __launch_bounds__(kMezThreads, 1) k_mez_tc(MezNet net, MezIO io,
     fence_proxy_async();
     __syncthreads();
 
-    float sm_m[2] = {-INFINITY, -INFINITY}, sm_s[2] = {0.0f, 0.0f}, sm_w[2] = {0.0f, 0.0f};   // value head: online softmax
+    float sm_m[2] = {-INFINITY, -INFINITY}, sm_s[2] = {0.0f, 0.0f}, sm_w[2] = {0.0f, 0.0f};   // value / reward head: online softmax
     int pos = 0;
     for (int l = 0; l < net.nlayers; ++l) {
         const int K = net.layer[l].K, N = net.layer[l].N, in = net.layer[l].in, out = net.layer[l].out;
@@ -291,9 +293,10 @@ __global__ void __launch_bounds__(kMezThreads, 1) k_mez_tc(MezNet net, MezIO io,
         }
 
         // ---- pass 2: the fp32 outputs and the next layer's fp16 hi / lo operand
-        const bool val = (f & MF_VALUE) != 0, head = (f & (MF_VALUE | MF_POLICY)) != 0;
-        const int ncols = val ? net.K : net.A, col0 = net.layer[l].col0;
-        float *lg = val ? io.value_logits : io.policy_logits;
+        const bool rew = (f & MF_REWARD) != 0, cat = (f & (MF_VALUE | MF_REWARD)) != 0;   // cat: a categorical head's piece
+        const bool head = (f & (MF_VALUE | MF_REWARD | MF_POLICY)) != 0;
+        const int ncols = cat ? net.K : net.A, col0 = net.layer[l].col0;
+        float *lg = rew ? io.reward_logits : (cat ? io.value_logits : io.policy_logits);
         unsigned char *ob = out == MB_NONE ? nullptr : smem + (out == MB_HID ? S.hid : (out == MB_SLOT1 ? S.slot1 : 0));
         const int opart = out == MB_HID ? 4 * kMezKgBytes : mez_slot_part(L);
 #pragma unroll
@@ -314,8 +317,8 @@ __global__ void __launch_bounds__(kMezThreads, 1) k_mez_tc(MezNet net, MezIO io,
                             const int k = col0 + col;
                             if (lg && k < ncols) lg[(size_t)brow[h] * ncols + k] = v0;
                             if (lg && k + 1 < ncols) lg[(size_t)brow[h] * ncols + k + 1] = v1;
-                            if (val && k < ncols) softmax_push(sm_m[h], sm_s[h], sm_w[h], v0, support_at(net.support_min, net.support_step, k));
-                            if (val && k + 1 < ncols) softmax_push(sm_m[h], sm_s[h], sm_w[h], v1, support_at(net.support_min, net.support_step, k + 1));
+                            if (cat && k < ncols) softmax_push(sm_m[h], sm_s[h], sm_w[h], v0, support_at(net.support_min, net.support_step, k));
+                            if (cat && k + 1 < ncols) softmax_push(sm_m[h], sm_s[h], sm_w[h], v1, support_at(net.support_min, net.support_step, k + 1));
                         }
                     } else {
                         v0 = v1 = 0.0f;
@@ -331,6 +334,7 @@ __global__ void __launch_bounds__(kMezThreads, 1) k_mez_tc(MezNet net, MezIO io,
                 }
         }
         if (f & MF_CAT_END) {      // the quad's partial (max, sum, weighted sum) triples -> softmax . support -> h^-1
+            float *sc_out = rew ? io.reward : io.value;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 float M = fmaxf(sm_m[h], __shfl_xor_sync(0xffffffffu, sm_m[h], 1));
@@ -341,7 +345,7 @@ __global__ void __launch_bounds__(kMezThreads, 1) k_mez_tc(MezNet net, MezIO io,
                 w += __shfl_xor_sync(0xffffffffu, w, 1);
                 s += __shfl_xor_sync(0xffffffffu, s, 2);
                 w += __shfl_xor_sync(0xffffffffu, w, 2);
-                if (on[h] && (lane & 3) == 0 && io.value) io.value[brow[h]] = inverse_scalar_transform(w / s);
+                if (on[h] && (lane & 3) == 0 && sc_out) sc_out[brow[h]] = inverse_scalar_transform(w / s);
             }
         }
         fence_proxy_async();
@@ -493,6 +497,18 @@ struct MezPacker {
         return true;
     }
 
+    // a categorical head (MLP_V2: Linear(L -> hid) + BN1d + ReLU, Linear(hid -> K)) on the latent in `src`: the hidden layer
+    // into the 32-wide buffer, then the FC2 pieces flagged `flag` (MF_VALUE or MF_REWARD), the first and last closing the
+    // online softmax expectation
+    bool cat_head(MezNet &net, const std::string &mlp, int src, int L, int hid, int K, int flag)
+    {
+        bool ok = layer(net, mlp + ".0", mlp + ".1", L, L, hid, 0, 32, L, src, MB_HID, MF_RELU);
+        for (int r0 = 0; ok && r0 < K; r0 += L)
+            ok = layer(net, mlp + ".3", "", hid, hid, K, r0, L, 32, MB_HID, MB_NONE,
+                       flag | (r0 == 0 ? MF_CAT_BEGIN : 0) | (r0 + L >= K ? MF_CAT_END : 0));
+        return ok;
+    }
+
     // prediction network on the latent in `src` (common.py:1218-1292); the other slot is its work buffer
     bool predict(MezNet &net, int src, int L, int A, int K, int vh, int ph)
     {
@@ -500,10 +516,7 @@ struct MezPacker {
         const int wk = src == MB_SLOT0 ? MB_SLOT1 : MB_SLOT0;
         bool ok = layer(net, Q + "fc_prediction_common.0", Q + "fc_prediction_common.1", L, L, L, 0, L, L, src, wk, MF_RELU) &&
                   layer(net, Q + "fc_prediction_common.3", Q + "fc_prediction_common.4", L, L, L, 0, L, L, wk, wk, MF_RELU) &&
-                  layer(net, Q + "fc_value_head.0", Q + "fc_value_head.1", L, L, vh, 0, 32, L, wk, MB_HID, MF_RELU);
-        for (int r0 = 0; ok && r0 < K; r0 += L)
-            ok = layer(net, Q + "fc_value_head.3", "", vh, vh, K, r0, L, 32, MB_HID, MB_NONE,
-                       MF_VALUE | (r0 == 0 ? MF_CAT_BEGIN : 0) | (r0 + L >= K ? MF_CAT_END : 0));
+                  cat_head(net, Q + "fc_value_head", wk, L, vh, K, MF_VALUE);
         ok = ok && layer(net, Q + "fc_policy_head.0", Q + "fc_policy_head.1", L, L, ph, 0, 32, L, wk, MB_HID, MF_RELU);
         for (int r0 = 0; ok && r0 < A; r0 += L) ok = layer(net, Q + "fc_policy_head.3", "", ph, ph, A, r0, L, 32, MB_HID, MB_NONE, MF_POLICY);
         return ok;
@@ -512,9 +525,15 @@ struct MezPacker {
 
 }  // namespace
 
+// Kind 3 (EfficientZeroModelMLP) and kind 4 (MuZeroModelMLP) share the programs up to what follows the dynamics MLP: kind 3
+// writes its output as the LSTM input (MF_FEAT), kind 4 runs the reward head on it (muzero_model_mlp.py:428-440).  Slots of the
+// recurrent program: the input latent z in slot 0; fc_dynamics_1 (+ z) -> slot 0 = the next latent; fc_dynamics_2 -> slot 1,
+// which the reward head reads; the prediction network reads slot 0 and works in slot 1.  Without res_connection_in_dynamics
+// fc_dynamics -> slot 0 is both the next latent and the reward head's input.
 int mez_pack(lz_model *m)
 {
     const lz_mlp_ez_config &c = m->ecfg;
+    const bool mz = m->kind == 4;
     const int L = c.latent_dim, A = c.action_space_size, K = m->K, kobs = (c.obs_dim + 31) / 32 * 32;
     MezPacker P;
     P.m = m;
@@ -526,14 +545,17 @@ int mez_pack(lz_model *m)
     bool ok = P.layer(init, R + "fc_representation.0", R + "fc_representation.1", c.obs_dim, c.obs_dim, L, 0, L, kobs, MB_OBS, MB_SLOT0, MF_GELU) &&
               P.layer(init, R + "fc_representation.3", "", L, L, L, 0, L, L, MB_SLOT0, MB_SLOT0, MF_LN | MF_LATENT) &&
               P.predict(init, MB_SLOT0, L, A, K, c.value_hidden, c.policy_hidden);
-    if (ok && c.res_connection_in_dynamics)     // next = fc_dynamics_1([z | a]) + z; LSTM input = fc_dynamics_2(next)
+    if (ok && c.res_connection_in_dynamics)     // next = fc_dynamics_1([z | a]) + z; LSTM / reward head input = fc_dynamics_2(next)
         ok = P.layer(rec, D + "fc_dynamics_1.0", D + "fc_dynamics_1.1", L + A, L, L, 0, L, L, MB_SLOT0, MB_SLOT1, MF_RELU | MF_ACT, &act) &&
              P.layer(rec, D + "fc_dynamics_1.3", D + "fc_dynamics_1.4", L, L, L, 0, L, L, MB_SLOT1, MB_SLOT0, MF_RELU | MF_RES | MF_LATENT) &&
              P.layer(rec, D + "fc_dynamics_2.0", D + "fc_dynamics_2.1", L, L, L, 0, L, L, MB_SLOT0, MB_SLOT1, MF_RELU) &&
-             P.layer(rec, D + "fc_dynamics_2.3", D + "fc_dynamics_2.4", L, L, L, 0, L, L, MB_SLOT1, MB_NONE, MF_RELU | MF_FEAT);
-    else if (ok)                                // next = LSTM input = fc_dynamics([z | a])
+             P.layer(rec, D + "fc_dynamics_2.3", D + "fc_dynamics_2.4", L, L, L, 0, L, L, MB_SLOT1, mz ? MB_SLOT1 : MB_NONE,
+                     MF_RELU | (mz ? 0 : MF_FEAT)) &&
+             (!mz || P.cat_head(rec, D + "fc_reward_head", MB_SLOT1, L, c.reward_hidden, K, MF_REWARD));
+    else if (ok)                                // next = LSTM / reward head input = fc_dynamics([z | a])
         ok = P.layer(rec, D + "fc_dynamics.0", D + "fc_dynamics.1", L + A, L, L, 0, L, L, MB_SLOT0, MB_SLOT1, MF_RELU | MF_ACT, &act) &&
-             P.layer(rec, D + "fc_dynamics.3", D + "fc_dynamics.4", L, L, L, 0, L, L, MB_SLOT1, MB_SLOT0, MF_RELU | MF_LATENT | MF_FEAT);
+             P.layer(rec, D + "fc_dynamics.3", D + "fc_dynamics.4", L, L, L, 0, L, L, MB_SLOT1, MB_SLOT0, MF_RELU | MF_LATENT | (mz ? 0 : MF_FEAT)) &&
+             (!mz || P.cat_head(rec, D + "fc_reward_head", MB_SLOT0, L, c.reward_hidden, K, MF_REWARD));
     ok = ok && P.predict(rec, MB_SLOT0, L, A, K, c.value_hidden, c.policy_hidden);
     if (!ok) return LZ_EINVAL;
     auto lw = P.get(R + "norm.weight", L), lb = P.get(R + "norm.bias", L);

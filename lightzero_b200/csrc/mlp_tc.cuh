@@ -1,12 +1,14 @@
-// mlp_tc.cuh -- interface of the tensor-core (wgmma) network of EfficientZeroModelMLP (mlp_tc.cu): vector observations, a latent
-// of L = 32 .. 256 (a multiple of 32) features, the representation / dynamics / prediction MLPs as one layer program per launch.
-// The LSTM value-prefix head that follows the dynamics network is ez.cu's.
+// mlp_tc.cuh -- interface of the tensor-core (wgmma) network of EfficientZeroModelMLP and MuZeroModelMLP (mlp_tc.cu): vector
+// observations, a latent of L = 32 .. 256 (a multiple of 32) features, the representation / dynamics / prediction MLPs as one
+// layer program per launch.  EfficientZeroModelMLP's LSTM value-prefix head that follows the dynamics network is ez.cu's;
+// MuZeroModelMLP's categorical reward head is part of the recurrent program.
 #pragma once
 #include "lz_common.cuh"
 
 namespace lz {
 
-constexpr int kMezMaxLayers = 48;     // 6 dense layers + the value and policy FC2 cut into pieces of <= L outputs (K, A <= 608)
+constexpr int kMezMaxLayers = 66;     // 6 dense layers + 3 head hidden layers + the reward, value and policy FC2 cut into
+                                      // pieces of <= L outputs (K, A <= 608: 19 pieces each at L = 32)
 constexpr int kMezRows = 64;          // roots per CTA: one m64 wgmma tile
 constexpr int kMezMaxL = 256, kMezMaxObs = 4096, kMezMaxOut = 608, kMezMaxHid = 32;
 
@@ -19,7 +21,9 @@ enum : int {
     MF_LATENT = 32,                   // write the output as the latent
     MF_FEAT = 64,                     // write the output as the LSTM input (fp32 [B][L])
     MF_VALUE = 128, MF_POLICY = 256,  // an FC2 piece of the value / policy head: logits columns col0 .. col0 + N
-    MF_CAT_BEGIN = 512, MF_CAT_END = 1024   // first / last piece of the value head's softmax expectation
+    MF_CAT_BEGIN = 512, MF_CAT_END = 1024,  // first / last piece of a categorical head's softmax expectation (with MF_VALUE
+                                            // or MF_REWARD: the head whose scalar MF_CAT_END writes)
+    MF_REWARD = 2048                  // an FC2 piece of MuZeroModelMLP's reward head (fc_reward_head.3)
 };
 // operand buffers: the two L-wide activation slots, the 32-wide head hidden buffer, the observation (streamed from global)
 enum : int { MB_NONE = -1, MB_SLOT0 = 0, MB_SLOT1 = 1, MB_HID = 2, MB_OBS = 3 };
@@ -50,7 +54,9 @@ struct MezIO {
     size_t slot_stride;
     const int *action;                // [B]
     float *latent_out, *latent_out2;  // [B][L] or nullptr
-    float *feat;                      // [B][L] LSTM input or nullptr
+    float *feat;                      // [B][L] LSTM input (EfficientZeroModelMLP) or nullptr
+    float *reward;                    // [B] or nullptr (MuZeroModelMLP's reward head)
+    float *reward_logits;             // [B][K] or nullptr
     float *value;                     // [B] or nullptr
     float *policy_logits;             // [B][A] or nullptr
     float *value_logits;              // [B][K] or nullptr
@@ -62,6 +68,6 @@ struct MezPlan { int R, ctas, last, smem, stages; };
 MezPlan mez_plan(const MezNet &net, int B);
 int mez_launch(const MezNet &net, const MezIO &io, cudaStream_t s);
 int mez_prepare_launch();
-int mez_pack(lz_model *m);            // dense layers of kind 3 -> m->d_mez, m->mez_rec / m->mez_init
+int mez_pack(lz_model *m);            // dense layers of kinds 3 and 4 (+ kind 4's reward head) -> m->d_mez, m->mez_rec / m->mez_init
 
 }  // namespace lz

@@ -213,16 +213,22 @@ static int ez_tail(lz_model *m, const RecIO &io, cudaStream_t s)
 int model_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
 {
     if (m->kind == 1) return mlp_recurrent(m, io, s);
-    if (m->kind == 3) {
-        // the dense layers on the tensor cores (mlp_tc.cu), their LSTM input through the value-prefix head (ez.cu)
-        LZ_REQUIRE(io.B <= m->ez_B, LZ_ESTATE, "model_recurrent: EfficientZero scratch sized for %d roots, got %d (model_reserve)", m->ez_B, io.B);
-        LZ_REQUIRE(io.h_base && io.c_base, LZ_EINVAL, "model_recurrent: EfficientZero needs the reward hidden state");
+    if (m->kind == 3 || m->kind == 4) {
+        // the dense layers on the tensor cores (mlp_tc.cu); EfficientZeroModelMLP's LSTM input then goes through the value-prefix
+        // head (ez.cu), MuZeroModelMLP's reward head is part of the program
+        const bool ez = m->kind == 3;
+        if (ez) {
+            LZ_REQUIRE(io.B <= m->ez_B, LZ_ESTATE, "model_recurrent: EfficientZero scratch sized for %d roots, got %d (model_reserve)", m->ez_B, io.B);
+            LZ_REQUIRE(io.h_base && io.c_base, LZ_EINVAL, "model_recurrent: EfficientZero needs the reward hidden state");
+        }
         MezIO e = mez_io(m, io.B);
         e.latent_base = io.latent_base; e.ix = io.ix; e.slot_stride = io.slot_stride; e.action = io.action;
-        e.latent_out = io.next_latent; e.feat = m->ez_feat;
+        e.latent_out = io.next_latent;
+        if (ez) e.feat = m->ez_feat;
+        else { e.reward = io.reward; e.reward_logits = io.reward_logits; }
         e.value = io.value; e.policy_logits = io.policy_logits; e.value_logits = io.value_logits;
         int rc = mez_launch(m->mez_rec, e, s);
-        if (rc) return rc;
+        if (rc || !ez) return rc;
         return ez_tail(m, io, s);
     }
     if (m->kind == 2) {
@@ -283,6 +289,7 @@ static int reserve_tc_skip(lz_model *m, int B)
     return LZ_OK;
 }
 
+// kinds 1 and 4 (MuZeroModelMLP) have no workspace; kind 3 has the LSTM scratch only
 int model_reserve(lz_model *m, int B)
 {
     {
@@ -430,7 +437,7 @@ int model_initial_tail(lz_model *m, int B, const float *pre_latent, const TailIO
 int model_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, cudaStream_t s)
 {
     if (m->kind == 1) return mlp_initial(m, B, d_obs, io_in, s);
-    if (m->kind == 3) {
+    if (m->kind == 3 || m->kind == 4) {
         MezIO e = mez_io(m, B);
         e.obs = d_obs; e.latent_out = io_in.latent; e.latent_out2 = io_in.latent2;
         e.value = io_in.value; e.policy_logits = io_in.policy_logits; e.value_logits = io_in.value_logits;
@@ -1108,6 +1115,13 @@ int lz_model_finalize(lz_model *m)
     ++m->generation;          // every device table is re-allocated below: graphs captured against the old ones are stale
     if (m->kind == 1) return mlp_finalize(m);
     if (m->kind == 3) return finalize_mlp_ez(m);
+    if (m->kind == 4) {          // MuZeroModelMLP on the tensor cores: every layer, the reward head included, is in the programs
+        int rc = mez_pack(m);
+        if (rc != LZ_OK) return rc;
+        m->finalized = true;
+        m->tensors.clear();
+        return LZ_OK;
+    }
     if (m->kind == 2) {
         int rc = pack_board(m);
         if (rc != LZ_OK) return rc;
@@ -1216,7 +1230,7 @@ int lz_model_latent_hw(const lz_model *m) { return m ? m->hw : 0; }
 int lz_model_latent_shape(const lz_model *m, int32_t *h_c, int32_t *h_h, int32_t *h_w)
 {
     LZ_REQUIRE(m, LZ_EINVAL, "lz_model_latent_shape: null model");
-    const bool mlp = m->kind == 1 || m->kind == 3;
+    const bool mlp = m->kind == 1 || m->kind == 3 || m->kind == 4;
     if (h_c) *h_c = mlp ? m->latent_floats : m->lat_c;
     if (h_h) *h_h = mlp ? 1 : m->lat_h;
     if (h_w) *h_w = mlp ? 1 : m->lat_w;
@@ -1341,16 +1355,19 @@ static int board_debug_stage(lz_model *m, int which, int B, const float *d_in, c
     return board_launch(net, io, st);
 }
 
-// lz_model_debug_net_stage of EfficientZeroModelMLP: which 1 is initial_inference on the observations d_in
+// lz_model_debug_net_stage of EfficientZeroModelMLP and of MuZeroModelMLP on the tensor cores: which 1 is initial_inference on
+// the observations d_in
 static int mez_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out,
                            size_t out_bytes, int32_t *h_info, cudaStream_t st)
 {
     MezNet net = which ? m->mez_init : m->mez_rec;          // a copy: the model's programs stay as they are
     const int L = net.L, K = net.K, A = net.A;
-    int D = 0;                                              // the L-wide layers before the heads
-    while (D < net.nlayers && net.layer[D].N == L && !(net.layer[D].flags & (MF_VALUE | MF_POLICY)) && net.layer[D].out != MB_HID) ++D;
+    const bool rew = !which && m->kind == 4;               // MuZeroModelMLP's recurrent program has the reward head
+    int dense[kMezMaxLayers], D = 0;                        // the program indices of the L-wide layers outside the heads
+    for (int l = 0; l < net.nlayers; ++l)
+        if (net.layer[l].N == L && !(net.layer[l].flags & (MF_VALUE | MF_REWARD | MF_POLICY)) && net.layer[l].out != MB_HID) dense[D++] = l;
     LZ_REQUIRE(stage <= D, LZ_EINVAL, "lz_model_debug_net_stage: stage %d past the %d dense layers of the program", stage, D);
-    const size_t nfl = stage < D ? (size_t)B * L : (size_t)B * (K + A + 1 + 2 * L);
+    const size_t nfl = stage < D ? (size_t)B * L : (size_t)B * (K + A + 1 + 2 * L + (rew ? K + 1 : 0));
     LZ_REQUIRE(out_bytes >= nfl * sizeof(float), LZ_EINVAL, "lz_model_debug_net_stage: stage %d needs %zu bytes, got %zu", stage,
                nfl * sizeof(float), out_bytes);
     MezIO io = mez_io(m, B);
@@ -1358,21 +1375,25 @@ static int mez_debug_stage(lz_model *m, int which, int B, const float *d_in, con
     else { io.latent_base = d_in; io.action = d_action; }
     float *o = reinterpret_cast<float *>(d_out);
     if (stage < D) {
-        // the program cut after layer `stage`, whose output is the only one written
-        net.nlayers = stage + 1;
+        // the program cut after dense layer `stage`, whose output is the only one written (the reward head before it, in
+        // MuZeroModelMLP's recurrent program, runs with no output)
+        const int cut = dense[stage];
+        net.nlayers = cut + 1;
         net.nchunks = 0;
-        for (int l = 0; l <= stage; ++l) {
+        for (int l = 0; l <= cut; ++l) {
             net.layer[l].flags &= ~(MF_LATENT | MF_FEAT);
             net.nchunks += net.layer[l].K / 32;
         }
-        net.layer[stage].flags |= MF_LATENT;
+        net.layer[cut].flags |= MF_LATENT;
         io.latent_out = o;
     } else {
-        // the latent sections first: the kernel writes them as float2 pairs
+        // the latent sections first: the kernel writes them as float2 pairs; then value logits, policy logits, value, and for
+        // MuZeroModelMLP's recurrent program reward logits and reward (its LSTM-input section stays zero)
         LZ_CUDA_CHECK(cudaMemsetAsync(d_out, 0, nfl * sizeof(float), st));
         io.latent_out = o;
-        if (!which) io.feat = o + (size_t)B * L;
+        if (!which && m->kind == 3) io.feat = o + (size_t)B * L;
         io.value_logits = o + (size_t)2 * B * L; io.policy_logits = io.value_logits + (size_t)B * K; io.value = io.policy_logits + (size_t)B * A;
+        if (rew) { io.reward_logits = io.value + B; io.reward = io.reward_logits + (size_t)B * K; }
     }
     const MezPlan p = mez_plan(net, B);
     const int32_t info[8] = {p.R, p.ctas, p.last, net.nlayers, m->npass, p.smem, p.stages, D};
@@ -1385,9 +1406,10 @@ int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_laten
 {
     LZ_REQUIRE(m && (which == 0 || which == 1) && B > 0 && d_latent && (which == 1 || d_action) && d_out && h_info && stage >= 0,
                LZ_EINVAL, "lz_model_debug_net_stage: bad argument");
-    LZ_REQUIRE(m->finalized && m->kind != 1, LZ_ESTATE, "lz_model_debug_net_stage: not a finalized conv, board or EfficientZeroModelMLP model");
+    LZ_REQUIRE(m->finalized && m->kind != 1, LZ_ESTATE,
+               "lz_model_debug_net_stage: not a finalized conv, board, EfficientZeroModelMLP or tensor-core MuZeroModelMLP model");
     if (m->kind == 2) return board_debug_stage(m, which, B, d_latent, d_action, stage, d_out, out_bytes, h_info, (cudaStream_t)s);
-    if (m->kind == 3) return mez_debug_stage(m, which, B, d_latent, d_action, stage, d_out, out_bytes, h_info, (cudaStream_t)s);
+    if (m->kind == 3 || m->kind == 4) return mez_debug_stage(m, which, B, d_latent, d_action, stage, d_out, out_bytes, h_info, (cudaStream_t)s);
     TcNet net = which ? m->tc_tail : m->tc_rec;          // a copy: the model's programs stay as they are
     const int nl = net.nlayers, K = m->K, A = m->cfg.action_space_size;
     const bool ez = m->cfg.efficientzero != 0 && which == 0;

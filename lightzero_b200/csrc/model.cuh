@@ -67,20 +67,22 @@ struct TailIO {
 }  // namespace lz
 
 struct lz_model {
-    int kind;                         // 0 = conv MuZeroModel / EfficientZeroModel (cfg.efficientzero), 1 = MuZeroModelMLP,
-                                      // 2 = board MuZeroModel (downsample=False, board_tc.cu), 3 = EfficientZeroModelMLP (mlp_tc.cu)
+    int kind;                         // 0 = conv MuZeroModel / EfficientZeroModel (cfg.efficientzero), 1 = MuZeroModelMLP (mlp.cu),
+                                      // 2 = board MuZeroModel (downsample=False, board_tc.cu), 3 = EfficientZeroModelMLP (mlp_tc.cu),
+                                      // 4 = MuZeroModelMLP on the tensor cores (mlp_tc.cu): the configs mlp.cu does not take
+                                      // (lz_model_create_mlp picks 1 or 4)
     unsigned char *d_board;           // kind 2: packed conv weights, BN / action-plane tables and fp32 head tables
     lz::BoardNet board_rec, board_init;   // kind 2: recurrent_inference / initial_inference programs
-    lz_mlp_ez_config ecfg;            // kind 3
-    unsigned char *d_mez;             // kind 3: packed fp16 hi / lo weights and fp32 tables of the dense layers
-    lz::MezNet mez_rec, mez_init;     // kind 3: recurrent_inference (dense part) / initial_inference programs
+    lz_mlp_ez_config ecfg;            // kinds 3 and 4 (kind 4: the lz_mlp_config fields, lstm_hidden_size 0)
+    unsigned char *d_mez;             // kinds 3, 4: packed fp16 hi / lo weights and fp32 tables of the dense layers
+    lz::MezNet mez_rec, mez_init;     // kinds 3, 4: recurrent_inference (dense part) / initial_inference programs
     int lat_c, lat_h, lat_w;          // latent shape of one root
     lz::EzNet ez;                     // EfficientZero value-prefix head tables (device pointers into d_weights)
     float *ez_feat, *ez_htmp;         // [ws_B][hc*36], [ws_B][H] scratch between the conv kernel and the LSTM kernels
     int ez_B;
     unsigned char *d_ez_wtc;          // LSTM weights in the tensor-core layout (ez.cu)
     int latent_floats;                // floats per root latent (64*36, 64*64 or latent_dim)
-    lz_mlp_config mcfg;
+    lz_mlp_config mcfg;               // kinds 1 and 4
     lz::MlpNet mlp;
     lz_model_config cfg;
     std::map<std::string, std::vector<float>> tensors;   // raw reference state_dict (host)

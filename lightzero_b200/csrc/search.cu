@@ -398,7 +398,7 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
     cudaStream_t s = (cudaStream_t)s_;
     const lz_model_config &c = q->model->cfg;
     const int B = q->B, A = q->A;
-    const size_t obs_elems = q->model->kind == 1 ? (size_t)q->model->mcfg.obs_dim
+    const size_t obs_elems = (q->model->kind == 1 || q->model->kind == 4) ? (size_t)q->model->mcfg.obs_dim
                              : q->model->kind == 3 ? (size_t)q->model->ecfg.obs_dim : (size_t)c.obs_c * c.obs_h * c.obs_w;
     nchunks = nchunks < 1 ? 1 : (nchunks > 8 ? 8 : nchunks);
     if (!q->copy_stream) {

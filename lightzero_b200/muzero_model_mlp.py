@@ -1,8 +1,11 @@
 """Host-side mirror of ``lzero.model.muzero_model_mlp.MuZeroModelMLP`` (muzero_model_mlp.py:21-295):
-vector observations (BASELINE config 1: CartPole, obs 4, latent 128, A=2).  Same constructor keywords,
-``initial_inference`` / ``recurrent_inference`` and ``MZNetworkOutput``; weights from the reference
-``state_dict``.  Forward passes are the CUDA kernels of csrc/mlp.cu; the same object plugs into
-``MuZeroMCTSCtree.search`` (fused one-graph search) like the conv model."""
+vector observations (BASELINE config 1: CartPole, obs 4, latent 128, A=2; lunarlander and its ReZero variant, latent 256).
+Same constructor keywords, ``initial_inference`` / ``recurrent_inference`` and ``MZNetworkOutput``; weights from the
+reference ``state_dict``.  The library picks the kernels from the config: the fp32 kernels of csrc/mlp.cu take latents up to
+128 with obs_dim and latent + actions up to 160; every other config with a latent that is a multiple of 32 up to 256 runs on
+the tensor-core kernel of csrc/mlp_tc.cu (math modes tc3 / tc1, ``set_math``).  The same object plugs into
+``MuZeroMCTSCtree.search`` / ``search_with_reuse``, ``GumbelMuZeroMCTSCtree.search``, ``MuZeroCollectPolicy`` and reanalyze
+like the conv model."""
 from typing import Dict, Optional, Sequence
 
 import torch
@@ -12,6 +15,8 @@ from .muzero_model import MZNetworkOutput
 
 
 class MuZeroModelMLP:
+    MATH_MODES = {"tc3": 1, "tc1": 2}
+
     def __init__(self, observation_shape: int = 4, action_space_size: int = 2, latent_state_dim: int = 128,
                  reward_head_hidden_channels: Sequence[int] = (32,), value_head_hidden_channels: Sequence[int] = (32,),
                  policy_head_hidden_channels: Sequence[int] = (32,),
@@ -54,6 +59,16 @@ class MuZeroModelMLP:
         self._loaded = True
         return self
 
+    def set_math(self, mode):
+        """'tc3' = wgmma 3xFP16 (fp32-accurate, the default), 'tc1' = wgmma single fp16 pass.  Tensor-core configs only: a
+        model on the fp32 kernels has no math mode (LzError)."""
+        if isinstance(mode, str) and mode not in self.MATH_MODES:
+            raise ValueError(f"set_math: unknown mode {mode!r}: MuZeroModelMLP runs tc3 or tc1")
+        code = self.MATH_MODES[mode] if isinstance(mode, str) else int(mode)
+        cabi.check(self._lib.lz_model_set_math(self._h, code), "lz_model_set_math")
+        self.math = code
+        return self
+
     def eval(self):
         return self
 
@@ -84,6 +99,8 @@ class MuZeroModelMLP:
         if not self._loaded:
             raise RuntimeError("MuZeroModelMLP: load_state_dict() has not been called")
         latent_state = latent_state.to(self.device, torch.float32).contiguous()
+        if latent_state.data_ptr() % 16:      # the tensor-core kernel reads latent rows as 16-byte vectors
+            latent_state = latent_state.clone()
         action = action.to(self.device).reshape(-1).to(torch.int32).contiguous()
         B = latent_state.shape[0]
         nxt = torch.empty(B, self.latent_state_dim, device=self.device)
