@@ -280,7 +280,16 @@ int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uin
  * second layer, after the residual for fc_dynamics_1); stage == D runs the whole program and writes latent [B, latent_dim], the
  * LSTM input [B, latent_dim] (`which` 0; zeros for `which` 1; no LSTM runs), value logits [B,K], policy logits [B,A], value [B].
  * h_info: roots per CTA, CTA count, roots of the last CTA, layers of the launched program, MMA passes, shared memory bytes, weight
- * ring stages, D. */
+ * ring stages, D.
+ * MuZeroModelMLP on the fp32 kernels (latent_dim <= 128): `which` as for EfficientZeroModelMLP.  stage < D cuts the program after
+ * its dense layer `stage` and writes that layer's f32 output [B, width]: for `which` 1 (D = 9) fc_representation.0 with BN and
+ * GELU, fc_representation.3, the LayerNorm, then the prediction network; for `which` 0 fc_dynamics_1.0 (one-hot rows included),
+ * fc_dynamics_1.3, the residual add, fc_dynamics_2.0, fc_dynamics_2.3 (D = 13; without res_connection_in_dynamics fc_dynamics.0,
+ * fc_dynamics.3, D = 10), the reward head's two layers, then the prediction network.  The prediction network's stages are
+ * fc_prediction_common.0 and .3, the value head's two layers, the policy head's two layers; every layer with its BN and
+ * activation.  width is latent_dim, a head's hidden size, the support size or A.  stage == D runs the whole program and writes
+ * latent [B, latent_dim], value logits [B,K], policy logits [B,A], value [B], and for `which` 0 reward logits [B,K], reward [B].
+ * h_info: roots per CTA (4), CTA count, roots of the last CTA, D, width (0 for stage D), 0, 0, 0. */
 int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_latent, const int32_t *d_action, int stage,
                              void *d_out, size_t out_bytes, int32_t *h_info, lz_stream s);
 int lz_model_latent_hw(const lz_model *m);   /* 6 for 84/96, 8 for 64; a square board's side; 0 for a non-square board */

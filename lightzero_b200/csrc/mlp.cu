@@ -59,15 +59,45 @@ __device__ __forceinline__ void dense(const Dense &L, const float *x, float *y, 
     __syncthreads();
 }
 
-// prediction network + outputs for the latents in `lat` (shared, [RB][kMlpWidth])
+// Test hook of lz_model_debug_net_stage: the kTap instantiations of the kernels below stop after the layer numbered `cut` and
+// write its fp32 output rows [B][width] to `out`, and nothing else.  Inference and the searches launch the kTap = false
+// instantiations, in which every tap is a compile-time no-op.
+struct MlpTap {
+    float *out;
+    int cut;
+};
+
+// true when the program stops here: `stage` is the cut, whose rows y [RB][ldy] (width valid columns) are written
+template <bool kTap>
+__device__ __forceinline__ bool tap(const MlpTap &t, int stage, const float *y, int ldy, int width, int root0, int B)
+{
+    if constexpr (!kTap) {
+        return false;
+    } else {
+        if (stage != t.cut) return false;
+        for (int i = threadIdx.x; i < kMlpRoots * width; i += kMlpThreads) {
+            const int r = i / width, c = i - r * width, b = root0 + r;
+            if (b < B) t.out[(size_t)b * width + c] = y[r * ldy + c];
+        }
+        return true;
+    }
+}
+
+// prediction network + outputs for the latents in `lat` (shared, [RB][kMlpWidth]); its layers are tap stages s0 .. s0 + 5
+template <bool kTap>
 __device__ __forceinline__ void mlp_predict(const MlpNet &net, const float *lat, float *b0, float *b1, float *logits,
-                                            int root0, int B, float *o_value, float *o_policy, float *o_value_logits)
+                                            int root0, int B, float *o_value, float *o_policy, float *o_value_logits,
+                                            const MlpTap &tp, int s0)
 {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     dense(net.pc0, lat, b0, kMlpWidth, kMlpWidth, nullptr);
+    if (tap<kTap>(tp, s0, b0, kMlpWidth, net.pc0.out, root0, B)) return;
     dense(net.pc1, b0, b1, kMlpWidth, kMlpWidth, nullptr);
+    if (tap<kTap>(tp, s0 + 1, b1, kMlpWidth, net.pc1.out, root0, B)) return;
     dense(net.v0, b1, b0, kMlpWidth, kMlpWidth, nullptr);
+    if (tap<kTap>(tp, s0 + 2, b0, kMlpWidth, net.v0.out, root0, B)) return;
     dense(net.v1, b0, logits, kMlpWidth, kMlpK, nullptr);
+    if (tap<kTap>(tp, s0 + 3, logits, kMlpK, net.v1.out, root0, B)) return;
     if (root0 + warp < B) {
         const float v = categorical_to_scalar(logits + warp * kMlpK, net.v1.out, net.support_min, net.support_step, lane);
         if (lane == 0 && o_value) o_value[root0 + warp] = v;
@@ -76,13 +106,19 @@ __device__ __forceinline__ void mlp_predict(const MlpNet &net, const float *lat,
     }
     __syncthreads();
     dense(net.p0, b1, b0, kMlpWidth, kMlpWidth, nullptr);
+    if (tap<kTap>(tp, s0 + 4, b0, kMlpWidth, net.p0.out, root0, B)) return;
     dense(net.p1, b0, logits, kMlpWidth, kMlpK, nullptr);
+    if (tap<kTap>(tp, s0 + 5, logits, kMlpK, net.p1.out, root0, B)) return;
     if (root0 + warp < B && o_policy)
         for (int a = lane; a < net.A; a += 32) o_policy[(size_t)(root0 + warp) * net.A + a] = logits[warp * kMlpK + a];
     __syncthreads();
 }
 
-__global__ void __launch_bounds__(kMlpThreads) k_mlp_recurrent(MlpNet net, RecIO io)
+// tap stages: with res_connection_in_dynamics fc_dynamics_1.0 (with the one-hot rows) 0, fc_dynamics_1.3 1, + latent 2,
+// fc_dynamics_2.0 3, fc_dynamics_2.3 4, reward head 5 6, prediction 7 .. 12; without it fc_dynamics.0 0, fc_dynamics.3 1,
+// reward head 2 3, prediction 4 .. 9
+template <bool kTap>
+__global__ void __launch_bounds__(kMlpThreads) k_mlp_recurrent(MlpNet net, RecIO io, MlpTap tp)
 {
     __shared__ float xa[kMlpRoots * kMlpWidth], xb[kMlpRoots * kMlpWidth], xc[kMlpRoots * kMlpWidth], logits[kMlpRoots * kMlpK];
     __shared__ int act_row[kMlpRoots];
@@ -105,20 +141,28 @@ __global__ void __launch_bounds__(kMlpThreads) k_mlp_recurrent(MlpNet net, RecIO
     const float *nxt, *enc;
     if (net.res) {                                   // muzero_model_mlp.py:428-434
         dense(net.d1a, xa, xb, kMlpWidth, kMlpWidth, act_row);
+        if (tap<kTap>(tp, 0, xb, kMlpWidth, Ld, root0, io.B)) return;
         dense(net.d1b, xb, xc, kMlpWidth, kMlpWidth, nullptr);
+        if (tap<kTap>(tp, 1, xc, kMlpWidth, Ld, root0, io.B)) return;
         for (int i = threadIdx.x; i < kMlpRoots * Ld; i += kMlpThreads) {
             const int r = i / Ld, c = i - r * Ld;
             xc[r * kMlpWidth + c] += xa[r * kMlpWidth + c];
         }
         __syncthreads();
+        if (tap<kTap>(tp, 2, xc, kMlpWidth, Ld, root0, io.B)) return;
         dense(net.d2a, xc, xb, kMlpWidth, kMlpWidth, nullptr);
+        if (tap<kTap>(tp, 3, xb, kMlpWidth, Ld, root0, io.B)) return;
         dense(net.d2b, xb, xa, kMlpWidth, kMlpWidth, nullptr);
+        if (tap<kTap>(tp, 4, xa, kMlpWidth, Ld, root0, io.B)) return;
         nxt = xc; enc = xa;
     } else {                                         // :436-438
         dense(net.d1a, xa, xb, kMlpWidth, kMlpWidth, act_row);
+        if (tap<kTap>(tp, 0, xb, kMlpWidth, Ld, root0, io.B)) return;
         dense(net.d1b, xb, xc, kMlpWidth, kMlpWidth, nullptr);
+        if (tap<kTap>(tp, 1, xc, kMlpWidth, Ld, root0, io.B)) return;
         nxt = xc; enc = xc;
     }
+    const int sr = net.res ? 5 : 2;                  // tap stage of the reward head's first layer
     if (io.next_latent)
         for (int i = threadIdx.x; i < kMlpRoots * Ld; i += kMlpThreads) {
             const int r = i / Ld, c = i - r * Ld, b = root0 + r;
@@ -126,7 +170,9 @@ __global__ void __launch_bounds__(kMlpThreads) k_mlp_recurrent(MlpNet net, RecIO
         }
     // reward head (:440)
     dense(net.r0, enc, xb, kMlpWidth, kMlpWidth, nullptr);
+    if (tap<kTap>(tp, sr, xb, kMlpWidth, net.r0.out, root0, io.B)) return;
     dense(net.r1, xb, logits, kMlpWidth, kMlpK, nullptr);
+    if (tap<kTap>(tp, sr + 1, logits, kMlpK, net.r1.out, root0, io.B)) return;
     if (root0 + warp < io.B) {
         const float rv = categorical_to_scalar(logits + warp * kMlpK, net.r1.out, net.support_min, net.support_step, lane);
         if (lane == 0 && io.reward) io.reward[root0 + warp] = rv;
@@ -135,10 +181,12 @@ __global__ void __launch_bounds__(kMlpThreads) k_mlp_recurrent(MlpNet net, RecIO
     }
     __syncthreads();
     // prediction on the next latent: nxt lives in xc; xa / xb are scratch (enc no longer needed)
-    mlp_predict(net, nxt, xa, xb, logits, root0, io.B, io.value, io.policy_logits, io.value_logits);
+    mlp_predict<kTap>(net, nxt, xa, xb, logits, root0, io.B, io.value, io.policy_logits, io.value_logits, tp, sr + 2);
 }
 
-__global__ void __launch_bounds__(kMlpThreads) k_mlp_initial(MlpNet net, const float *obs, TailIO io)
+// tap stages: fc_representation.0 (+ BN + GELU) 0, fc_representation.3 1, LayerNorm 2, prediction 3 .. 8
+template <bool kTap>
+__global__ void __launch_bounds__(kMlpThreads) k_mlp_initial(MlpNet net, const float *obs, TailIO io, MlpTap tp)
 {
     __shared__ float xa[kMlpRoots * kMlpWidth], xb[kMlpRoots * kMlpWidth], xc[kMlpRoots * kMlpWidth], logits[kMlpRoots * kMlpK];
     const int root0 = blockIdx.x * kMlpRoots, Ld = net.latent;
@@ -149,7 +197,9 @@ __global__ void __launch_bounds__(kMlpThreads) k_mlp_initial(MlpNet net, const f
     }
     __syncthreads();
     dense(net.e0, xa, xb, kMlpWidth, kMlpWidth, nullptr);          // Linear + BN + GELU(tanh)
+    if (tap<kTap>(tp, 0, xb, kMlpWidth, Ld, root0, io.B)) return;
     dense(net.e1, xb, xc, kMlpWidth, kMlpWidth, nullptr);          // Linear
+    if (tap<kTap>(tp, 1, xc, kMlpWidth, Ld, root0, io.B)) return;
     {   // nn.LayerNorm(latent), eps 1e-5, biased variance: one warp per root
         float s = 0.0f;
         for (int c = lane; c < Ld; c += 32) s += xc[warp * kMlpWidth + c];
@@ -161,6 +211,7 @@ __global__ void __launch_bounds__(kMlpThreads) k_mlp_initial(MlpNet net, const f
             xc[warp * kMlpWidth + c] = (xc[warp * kMlpWidth + c] - mean) * rstd * __ldg(net.ln_w + c) + __ldg(net.ln_b + c);
     }
     __syncthreads();
+    if (tap<kTap>(tp, 2, xc, kMlpWidth, Ld, root0, io.B)) return;
     for (int i = threadIdx.x; i < kMlpRoots * Ld; i += kMlpThreads) {
         const int r = i / Ld, c = i - r * Ld, b = root0 + r;
         if (b < io.B) {
@@ -168,12 +219,12 @@ __global__ void __launch_bounds__(kMlpThreads) k_mlp_initial(MlpNet net, const f
             if (io.latent2) io.latent2[(size_t)b * Ld + c] = xc[r * kMlpWidth + c];
         }
     }
-    mlp_predict(net, xc, xa, xb, logits, root0, io.B, io.value, io.policy_logits, io.value_logits);
+    mlp_predict<kTap>(net, xc, xa, xb, logits, root0, io.B, io.value, io.policy_logits, io.value_logits, tp, 3);
 }
 
 int mlp_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
 {
-    k_mlp_recurrent<<<ceil_div(io.B, kMlpRoots), kMlpThreads, 0, s>>>(m->mlp, io);
+    k_mlp_recurrent<false><<<ceil_div(io.B, kMlpRoots), kMlpThreads, 0, s>>>(m->mlp, io, MlpTap{});
     LZ_KERNEL_CHECK();
     return LZ_OK;
 }
@@ -182,7 +233,59 @@ int mlp_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, cud
 {
     TailIO io = io_in;
     io.B = B;
-    k_mlp_initial<<<ceil_div(B, kMlpRoots), kMlpThreads, 0, s>>>(m->mlp, d_obs, io);
+    k_mlp_initial<false><<<ceil_div(B, kMlpRoots), kMlpThreads, 0, s>>>(m->mlp, d_obs, io, MlpTap{});
+    LZ_KERNEL_CHECK();
+    return LZ_OK;
+}
+
+// lz_model_debug_net_stage of the fp32 MLP kernels: the kTap instantiations cut after dense layer `stage`; stage == D (the
+// number of tap stages) launches the production kernel with every output in d_out
+int mlp_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out,
+                    size_t out_bytes, int32_t *h_info, cudaStream_t s)
+{
+    const MlpNet &n = m->mlp;
+    const int L = n.latent, K = m->K, A = n.A;
+    int w[16], D = 0;                                // output width of each tap stage, in program order
+    if (which) {
+        w[D++] = L; w[D++] = L; w[D++] = L;
+    } else {
+        w[D++] = L; w[D++] = L;
+        if (n.res) { w[D++] = L; w[D++] = L; w[D++] = L; }
+        w[D++] = n.r0.out; w[D++] = K;
+    }
+    w[D++] = L; w[D++] = L; w[D++] = n.v0.out; w[D++] = K; w[D++] = n.p0.out; w[D++] = A;
+    LZ_REQUIRE(stage <= D, LZ_EINVAL, "lz_model_debug_net_stage: stage %d past the %d dense layers of the program", stage, D);
+    const size_t nfl = stage < D ? (size_t)B * w[stage] : (size_t)B * (L + 2 * K + A + 2);
+    LZ_REQUIRE(out_bytes >= nfl * sizeof(float), LZ_EINVAL, "lz_model_debug_net_stage: stage %d needs %zu bytes, got %zu", stage,
+               nfl * sizeof(float), out_bytes);
+    const int ctas = ceil_div(B, kMlpRoots);
+    const int32_t info[8] = {kMlpRoots, ctas, B - (ctas - 1) * kMlpRoots, D, stage < D ? w[stage] : 0, 0, 0, 0};
+    memcpy(h_info, info, sizeof(info));
+    float *o = reinterpret_cast<float *>(d_out);
+    const MlpTap tp{o, stage};
+    if (which) {
+        TailIO io;
+        memset(&io, 0, sizeof(io));
+        io.B = B;
+        if (stage < D) {
+            k_mlp_initial<true><<<ctas, kMlpThreads, 0, s>>>(n, d_in, io, tp);
+        } else {                                     // [latent B x L | value logits B x K | policy logits B x A | value B]
+            io.latent = o; io.value_logits = o + (size_t)B * L; io.policy_logits = io.value_logits + (size_t)B * K;
+            io.value = io.policy_logits + (size_t)B * A;
+            k_mlp_initial<false><<<ctas, kMlpThreads, 0, s>>>(n, d_in, io, MlpTap{});
+        }
+    } else {
+        RecIO io;
+        memset(&io, 0, sizeof(io));
+        io.B = B; io.latent_base = d_in; io.action = d_action;
+        if (stage < D) {
+            k_mlp_recurrent<true><<<ctas, kMlpThreads, 0, s>>>(n, io, tp);
+        } else {                                     // the same, then [reward logits B x K | reward B]
+            io.next_latent = o; io.value_logits = o + (size_t)B * L; io.policy_logits = io.value_logits + (size_t)B * K;
+            io.value = io.policy_logits + (size_t)B * A; io.reward_logits = io.value + B; io.reward = io.reward_logits + (size_t)B * K;
+            k_mlp_recurrent<false><<<ctas, kMlpThreads, 0, s>>>(n, io, MlpTap{});
+        }
+    }
     LZ_KERNEL_CHECK();
     return LZ_OK;
 }

@@ -1406,8 +1406,8 @@ int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_laten
 {
     LZ_REQUIRE(m && (which == 0 || which == 1) && B > 0 && d_latent && (which == 1 || d_action) && d_out && h_info && stage >= 0,
                LZ_EINVAL, "lz_model_debug_net_stage: bad argument");
-    LZ_REQUIRE(m->finalized && m->kind != 1, LZ_ESTATE,
-               "lz_model_debug_net_stage: not a finalized conv, board, EfficientZeroModelMLP or tensor-core MuZeroModelMLP model");
+    LZ_REQUIRE(m->finalized, LZ_ESTATE, "lz_model_debug_net_stage: model not finalized");
+    if (m->kind == 1) return mlp_debug_stage(m, which, B, d_latent, d_action, stage, d_out, out_bytes, h_info, (cudaStream_t)s);
     if (m->kind == 2) return board_debug_stage(m, which, B, d_latent, d_action, stage, d_out, out_bytes, h_info, (cudaStream_t)s);
     if (m->kind == 3 || m->kind == 4) return mez_debug_stage(m, which, B, d_latent, d_action, stage, d_out, out_bytes, h_info, (cudaStream_t)s);
     TcNet net = which ? m->tc_tail : m->tc_rec;          // a copy: the model's programs stay as they are

@@ -121,5 +121,7 @@ int model_reserve(lz_model *m, int B);   // sizes the initial-inference workspac
 int mlp_recurrent(lz_model *m, const RecIO &io, cudaStream_t s);
 int mlp_initial(lz_model *m, int B, const float *d_obs, const TailIO &io, cudaStream_t s);
 int mlp_finalize(lz_model *m);
+int mlp_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out,
+                    size_t out_bytes, int32_t *h_info, cudaStream_t s);
 bool model_is_ez(const lz_model *m);     // EfficientZero (value-prefix LSTM head): conv EfficientZeroModel or EfficientZeroModelMLP
 }  // namespace lz
