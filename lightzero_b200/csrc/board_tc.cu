@@ -22,6 +22,7 @@
 #include <algorithm>
 
 #include "board_tc.cuh"
+#include "model.cuh"
 #include "net6.cuh"
 #include "tc_ptx.cuh"
 
@@ -378,21 +379,188 @@ float board_pack_conv3(const float *w, int C, int cin_total, int cin_used, int c
     for (int co = 0; co < C; ++co)
         for (int ci = 0; ci < cin_used; ++ci)
             for (int t = 0; t < 9; ++t) mx = std::max(mx, fabsf(w[((size_t)co * cin_total + ci) * 9 + t]));
-    int e = 0;
-    if (mx > 0.0f) frexpf(mx, &e);
-    const float scale = ldexpf(1.0f, 13 - e);       // largest |w| lands in [4096, 8192): the lo parts stay in fp16's normal range
+    const float scale = pow2_scale(mx);
     __half *h = reinterpret_cast<__half *>(dst);
     const size_t tap_halves = (size_t)cin_pad * C * 2;
     for (int t = 0; t < 9; ++t)
         for (int co = 0; co < C; ++co)
             for (int ci = 0; ci < cin_pad; ++ci) {
                 const float v = ci < cin_used ? w[((size_t)co * cin_total + ci) * 9 + t] * scale : 0.0f;
-                const __half hi = __float2half_rn(v), lo = __float2half_rn(v - __half2float(hi));
                 const size_t off = t * tap_halves + ((size_t)(ci / 8) * 2 * C + co) * 8 + ci % 8;
-                h[off] = hi;
-                h[off + (size_t)C * 8] = lo;
+                split_hi_lo(v, h[off], h[off + (size_t)C * 8]);
             }
     return scale;
+}
+
+// ---- the Board family (lz_model::board) ----------------------------------------------------------------------------------
+// tables of the board network: fp16 hi/lo conv weights, folded BN, action planes, fp32 heads ----
+int board_finalize(lz_model *m)
+{
+    const lz_model_config &c = m->board.cfg;
+    const int C = c.num_channels, A = c.action_space_size, n = c.num_res_blocks, H = c.obs_h, W = c.obs_w, P = H * W;
+    const std::string D = "dynamics_network.", Q = "prediction_network.", R = "representation_network.";
+    struct Conv { std::string w, bn; int cin_total, cin_used, cin_pad; };
+    // conv indices: 0 dyn conv | 1..2n dyn blocks | 2n+1..4n pred blocks | 4n+1..6n rep blocks | 6n+1 rep conv
+    std::vector<Conv> convs;
+    convs.push_back({D + "conv.weight", D + "norm_common", C + A, C, C});
+    for (const std::string &pre : {D, Q, R})
+        for (int i = 0; i < n; ++i) {
+            const std::string b = pre + "resblocks." + std::to_string(i);
+            convs.push_back({b + ".conv1.0.weight", b + ".conv1.1", C, C, C});
+            convs.push_back({b + ".conv2.0.weight", b + ".conv2.1", C, C, C});
+        }
+    convs.push_back({R + "conv.weight", R + "norm", c.obs_c, c.obs_c, 16});   // observation planes padded to 16 with zero weights
+    const int nconv = (int)convs.size();
+    auto align = [](size_t v) { return (v + 127) & ~(size_t)127; };
+    std::vector<size_t> woff(nconv);
+    size_t off = 0;
+    for (int i = 0; i < nconv; ++i) { woff[i] = off; off += (size_t)9 * convs[i].cin_pad * C * 4; }
+    const size_t off_bn = align(off), off_ab = align(off_bn + (size_t)nconv * 2 * C * 4), off_heads = align(off_ab + (size_t)A * C * P * 4);
+    std::vector<unsigned char> host(off_heads, 0);
+    float *bn = reinterpret_cast<float *>(host.data() + off_bn), *ab = reinterpret_cast<float *>(host.data() + off_ab);
+    for (int ci = 0; ci < nconv; ++ci) {
+        const Conv &cv = convs[ci];
+        auto w = find_tensor(m, cv.w, (size_t)C * cv.cin_total * 9);
+        std::vector<float> scale, shift;
+        if (!w || !fold_bn(m, cv.bn, C, scale, shift)) return LZ_EINVAL;
+        const float ws = board_pack_conv3(w->data(), C, cv.cin_total, cv.cin_used, cv.cin_pad, host.data() + woff[ci]);
+        for (int k = 0; k < C; ++k) { bn[ci * 2 * C + k] = scale[k] / ws; bn[ci * 2 * C + C + k] = shift[k]; }
+        if (ci == 0)      // one-hot action planes (muzero_model.py:341-369): border-aware tap sums, times the BN scale
+            for (int a = 0; a < A; ++a)
+                for (int co = 0; co < C; ++co)
+                    for (int y = 0; y < H; ++y)
+                        for (int x = 0; x < W; ++x) {
+                            double acc = 0.0;
+                            for (int t = 0; t < 9; ++t) {
+                                const int yy = y + t / 3 - 1, xx = x + t % 3 - 1;
+                                if (yy >= 0 && yy < H && xx >= 0 && xx < W) acc += (*w)[((size_t)co * cv.cin_total + C + a) * 9 + t];
+                            }
+                            ab[((size_t)a * C + co) * P + y * W + x] = (float)acc * scale[co];
+                        }
+    }
+    // heads: fp32 tables (conv bias folded into the 1x1 BN shift, Linear bias into the BN1d shift)
+    struct HD { std::string conv, norm, fc; int hc, hid, K; };
+    const HD heads[3] = {{D + "conv1x1_reward", D + "norm_reward", D + "fc_reward_head", c.reward_head_channels, c.reward_hidden, m->K},
+                         {Q + "conv1x1_value", Q + "norm_value", Q + "fc_value", c.value_head_channels, c.value_hidden, m->K},
+                         {Q + "conv1x1_policy", Q + "norm_policy", Q + "fc_policy", c.policy_head_channels, c.policy_hidden, A}};
+    TablePacker hp;
+    size_t hoff[3][8];
+    for (int h = 0; h < 3; ++h) {
+        const HD &d = heads[h];
+        const int nin = d.hc * P;
+        auto w1 = find_tensor(m, d.conv + ".weight", (size_t)d.hc * C), b1 = find_tensor(m, d.conv + ".bias", d.hc);
+        auto W0 = find_tensor(m, d.fc + ".0.weight", (size_t)d.hid * nin), B0 = find_tensor(m, d.fc + ".0.bias", d.hid);
+        auto W3 = find_tensor(m, d.fc + ".3.weight", (size_t)d.K * d.hid), B3 = find_tensor(m, d.fc + ".3.bias", d.K);
+        std::vector<float> s1, t1, s2, t2;
+        if (!w1 || !b1 || !W0 || !B0 || !W3 || !B3 || !fold_bn(m, d.norm, d.hc, s1, t1) || !fold_bn(m, d.fc + ".1", d.hid, s2, t2))
+            return LZ_EINVAL;
+        for (int i = 0; i < d.hc; ++i) t1[i] += s1[i] * (*b1)[i];
+        for (int j = 0; j < d.hid; ++j) t2[j] += s2[j] * (*B0)[j];
+        const std::vector<float> *parts[8] = {w1, &s1, &t1, W0, &s2, &t2, W3, B3};
+        for (int k = 0; k < 8; ++k) hoff[h][k] = hp.add(*parts[k]);
+    }
+    host.resize(off_heads + hp.host.size() * sizeof(float));
+    memcpy(host.data() + off_heads, hp.host.data(), hp.host.size() * sizeof(float));
+    int rc = upload(&m->board.d_board, host.data(), host.size());
+    if (rc != LZ_OK) return rc;
+    BoardNet base;
+    memset(&base, 0, sizeof(base));
+    base.convw = m->board.d_board;
+    base.bn = reinterpret_cast<const float *>(m->board.d_board + off_bn);
+    base.abias = reinterpret_cast<const float *>(m->board.d_board + off_ab);
+    const float *hb = reinterpret_cast<const float *>(m->board.d_board + off_heads);
+    for (int h = 0; h < 3; ++h) {
+        BoardHead &o = base.head[h];
+        o.w1 = hb + hoff[h][0]; o.s1 = hb + hoff[h][1]; o.t1 = hb + hoff[h][2];
+        o.fc1 = hb + hoff[h][3]; o.s2 = hb + hoff[h][4]; o.t2 = hb + hoff[h][5];
+        o.fc2 = hb + hoff[h][6]; o.b2 = hb + hoff[h][7];
+        o.hc = heads[h].hc; o.hid = heads[h].hid; o.K = heads[h].K;
+    }
+    base.C = C; base.H = H; base.W = W; base.A = A;
+    base.support_min = c.support_min; base.support_step = c.support_step;
+    BoardNet rec = base, init = base;
+    auto add = [&](BoardNet &net, int ci, int flags) {
+        net.layer_woff[net.nlayers] = (uint32_t)woff[ci];
+        net.layer_bn[net.nlayers] = ci * 2 * C;
+        net.layer_flags[net.nlayers++] = flags;
+    };
+    auto blocks = [&](BoardNet &net, int first, int last_flags) {
+        for (int i = 0; i < n; ++i) {
+            add(net, first + 2 * i, 0);
+            add(net, first + 2 * i + 1, BF_RES | BF_STORE_RES | (i == n - 1 ? last_flags : 0));
+        }
+    };
+    add(rec, 0, BF_RES | BF_STORE_RES | BF_ACT_BIAS);
+    blocks(rec, 1, BF_WRITE_LATENT | BF_HOOK_REWARD);
+    blocks(rec, 2 * n + 1, BF_HOOK_VALPOL);
+    add(init, 6 * n + 1, BF_OBS | BF_STORE_RES);
+    blocks(init, 4 * n + 1, BF_WRITE_LATENT);
+    blocks(init, 2 * n + 1, BF_HOOK_VALPOL);
+    m->board.rec = rec; m->board.init = init;
+    return board_prepare_launch();
+}
+
+static BoardIO board_io(const lz_model *m, int B)
+{
+    BoardIO b;
+    memset(&b, 0, sizeof(b));
+    b.B = B; b.npass = m->npass; b.obs_c = m->board.cfg.obs_c;
+    return b;
+}
+
+int board_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
+{
+    BoardIO b = board_io(m, io.B);
+    b.latent_base = io.latent_base; b.ix = io.ix; b.slot_stride = io.slot_stride; b.action = io.action;
+    b.latent_out = io.next_latent; b.reward = io.reward; b.value = io.value; b.policy_logits = io.policy_logits;
+    b.reward_logits = io.reward_logits; b.value_logits = io.value_logits;
+    return board_launch(m->board.rec, b, s);
+}
+
+int board_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, cudaStream_t s)
+{
+    BoardIO b = board_io(m, B);
+    b.obs = d_obs; b.latent_out = io_in.latent; b.latent_out2 = io_in.latent2;
+    b.value = io_in.value; b.policy_logits = io_in.policy_logits; b.value_logits = io_in.value_logits;
+    return board_launch(m->board.init, b, s);
+}
+
+// lz_model_debug_net_stage of the board network: which 1 is the whole initial_inference program, d_latent the observations
+int board_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out,
+                             size_t out_bytes, int32_t *h_info, cudaStream_t st)
+{
+    BoardNet net = which ? m->board.init : m->board.rec;      // a copy: the model's programs stay as they are
+    const int nl = net.nlayers, K = m->K, A = m->A;
+    LZ_REQUIRE(stage <= nl, LZ_EINVAL, "lz_model_debug_net_stage: stage %d past the %d layers of the program", stage, nl);
+    const size_t nfl = stage < nl ? (size_t)B * m->latent_floats : (size_t)B * (2 * K + 2 * A + 4);
+    LZ_REQUIRE(out_bytes >= nfl * sizeof(float), LZ_EINVAL, "lz_model_debug_net_stage: stage %d needs %zu bytes, got %zu", stage,
+               nfl * sizeof(float), out_bytes);
+    const BoardPlan p = board_plan(net, B);
+    const int32_t info[8] = {p.R, p.NT, p.ctas, p.last, stage < nl ? stage + 1 : nl, m->npass, p.smem, 0};
+    memcpy(h_info, info, sizeof(info));
+    float *o = reinterpret_cast<float *>(d_out);
+    BoardIO io = board_io(m, B);
+    if (which) io.obs = d_in;
+    else { io.latent_base = d_in; io.action = d_action; }
+    if (stage < nl) {
+        // the program cut after layer `stage`, whose output is the only latent written; no head runs
+        net.nlayers = stage + 1;
+        for (int L = 0; L <= stage; ++L) net.layer_flags[L] &= ~(BF_WRITE_LATENT | BF_HOOK_REWARD | BF_HOOK_VALPOL);
+        net.layer_flags[stage] |= BF_WRITE_LATENT;
+        io.latent_out = o;
+        return board_launch(net, io, st);
+    }
+    // the whole program with the raw logits, then without them (the scalars alone, as a search asks for them)
+    LZ_CUDA_CHECK(cudaMemsetAsync(d_out, 0, nfl * sizeof(float), st));
+    float *rl = o, *vl = rl + (size_t)B * K, *pl = vl + (size_t)B * K, *r = pl + (size_t)B * A, *v = r + B;
+    float *pl2 = v + B, *r2 = pl2 + (size_t)B * A, *v2 = r2 + B;
+    io.policy_logits = pl; io.value_logits = vl; io.value = v;
+    if (!which) { io.reward_logits = rl; io.reward = r; }
+    int rc = board_launch(net, io, st);
+    if (rc) return rc;
+    io.policy_logits = pl2; io.value_logits = nullptr; io.value = v2;
+    io.reward_logits = nullptr; io.reward = which ? nullptr : r2;
+    return board_launch(net, io, st);
 }
 
 }  // namespace lz

@@ -12,6 +12,7 @@
 #include <algorithm>
 
 #include "conv_tc.cuh"
+#include "model.cuh"
 #include "tc_ptx.cuh"
 
 namespace lz {
@@ -630,21 +631,15 @@ float conv_tc_pack(const float *w, int cin, int cout, int ncols, int col0, unsig
 {
     float mx = 0.0f;
     for (size_t i = 0; i < (size_t)cout * cin * 9; ++i) mx = std::max(mx, fabsf(w[i]));
-    int e = 0;
-    if (mx > 0.0f) frexpf(mx, &e);
-    const float scale = ldexpf(1.0f, 13 - e);
+    const float scale = pow2_scale(mx);
     // tap block: [k-group ci / 8][ncols hi rows | ncols lo rows][ci % 8]: [B_hi | B_lo] of a k-group is one contiguous 2 x ncols-row operand
     const size_t tap_halves = (size_t)2 * (cin / 8) * ncols * 8, part_halves = (size_t)ncols * 8;
     __half *h = reinterpret_cast<__half *>(dst);
     for (int t = 0; t < 9; ++t)
         for (int co = 0; co < cout; ++co)
             for (int ci = 0; ci < cin; ++ci) {
-                const float sv = w[((size_t)co * cin + ci) * 9 + t] * scale;
-                const __half hi = __float2half_rn(sv);
-                const __half lo = __float2half_rn(sv - __half2float(hi));
                 const size_t off = (size_t)t * tap_halves + ((size_t)(ci / 8) * 2 * ncols + col0 + co) * 8 + (ci % 8);
-                h[off] = hi;
-                h[off + part_halves] = lo;
+                split_hi_lo(w[((size_t)co * cin + ci) * 9 + t] * scale, h[off], h[off + part_halves]);
             }
     return scale;
 }

@@ -9,11 +9,12 @@
 #include <cuda_fp16.h>
 #include <math.h>
 #include <stdlib.h>
+#include <string.h>
 
 #include <algorithm>
 
 #include "ez.cuh"
-#include "lz_common.cuh"
+#include "model.cuh"
 #include "tc_ptx.cuh"
 
 namespace lz {
@@ -323,20 +324,16 @@ float ez_pack_wtc(const float *w_ih, const float *w_hh, int nin, int H, unsigned
     float mx = 0.0f;
     for (size_t i = 0; i < (size_t)N * nin; ++i) mx = std::max(mx, fabsf(w_ih[i]));
     for (size_t i = 0; i < (size_t)N * H; ++i) mx = std::max(mx, fabsf(w_hh[i]));
-    int e = 0;
-    if (mx > 0.0f) frexpf(mx, &e);
-    const float scale = ldexpf(1.0f, 13 - e);    // largest |w| lands in [4096, 8192): lo parts stay normal fp16
+    const float scale = pow2_scale(mx);
     __half *h = reinterpret_cast<__half *>(dst);
     for (int n = 0; n < N; ++n) {
         const int unit = n >> 2, gate = n & 3, row = gate * H + unit, nt = n / kTN, nn = n % kTN;
         for (int k = 0; k < KT; ++k) {
             const float w = (k < nin ? w_ih[(size_t)row * nin + k] : w_hh[(size_t)row * H + (k - nin)]) * scale;
-            const __half hi = __float2half_rn(w), lo = __float2half_rn(w - __half2float(hi));
             const int c = k / kTK, kk = k % kTK;
             const size_t blk = ((size_t)nt * nchunks + c) * (2 * kTWPart / 2);      // in halves
             const size_t off = blk + ((size_t)(kk / 8) * kTN + nn) * 8 + (kk % 8);
-            h[off] = hi;
-            h[off + kTWPart / 2] = lo;
+            split_hi_lo(w, h[off], h[off + kTWPart / 2]);
         }
     }
     return scale;
@@ -364,6 +361,90 @@ int ez_launch(const EzNet &net, const EzIO &io, cudaStream_t s)
     k_ez_head<<<(io.B + kHR - 1) / kHR, 256, 0, s>>>(net, io);
     LZ_KERNEL_CHECK();
     return LZ_OK;
+}
+
+// ---- the value-prefix head of a model (lz_model::ez) ------------------------------------------------------------------------
+// Tables of nn.LSTM(nin -> H) (one step) and fc_reward_head (Linear(H -> hid) + BN1d + ReLU + Linear(hid -> K)), preceded by
+// norm_value_prefix (BN1d + ReLU, vp_norm) in the conv model (efficientzero_model.py:511-525, 556-569) and by nothing in
+// EfficientZeroModelMLP (efficientzero_model_mlp.py:416-429, 466-467): fp32 tables in m->ez.d_tables, the tensor-core copy of
+// the LSTM weights in m->ez.d_wtc.
+int ez_finalize(lz_model *m, int nin, int hid, bool vp_norm)
+{
+    const std::string D = "dynamics_network.";
+    const int K = m->K, H = m->lstm_hidden;
+    auto Wih = find_tensor(m, D + "lstm.weight_ih_l0", (size_t)4 * H * nin), Whh = find_tensor(m, D + "lstm.weight_hh_l0", (size_t)4 * H * H);
+    auto bih = find_tensor(m, D + "lstm.bias_ih_l0", (size_t)4 * H), bhh = find_tensor(m, D + "lstm.bias_hh_l0", (size_t)4 * H);
+    auto W0 = find_tensor(m, D + "fc_reward_head.0.weight", (size_t)hid * H), B0 = find_tensor(m, D + "fc_reward_head.0.bias", hid);
+    auto W3 = find_tensor(m, D + "fc_reward_head.3.weight", (size_t)K * hid), B3 = find_tensor(m, D + "fc_reward_head.3.bias", K);
+    std::vector<float> vs, vt, s2, t2;
+    if (!Wih || !Whh || !bih || !bhh || !W0 || !B0 || !W3 || !B3 || (vp_norm && !fold_bn(m, D + "norm_value_prefix", H, vs, vt)) ||
+        !fold_bn(m, D + "fc_reward_head.1", hid, s2, t2))
+        return LZ_EINVAL;
+    for (int j = 0; j < hid; ++j) t2[j] += s2[j] * (*B0)[j];
+    // torch.nn.LSTM stacks the gates (i, f, g, o) along dim 0; column n = unit * 4 + gate
+    std::vector<float> wcat((size_t)(nin + H) * 4 * H), bias((size_t)4 * H), fc1((size_t)H * hid), fc2((size_t)hid * K);
+    for (int g = 0; g < 4; ++g)
+        for (int u = 0; u < H; ++u) {
+            const size_t row = (size_t)g * H + u, col = (size_t)u * 4 + g;
+            for (int k = 0; k < nin; ++k) wcat[(size_t)k * 4 * H + col] = (*Wih)[row * nin + k];
+            for (int k = 0; k < H; ++k) wcat[(size_t)(nin + k) * 4 * H + col] = (*Whh)[row * H + k];
+            bias[col] = (*bih)[row] + (*bhh)[row];
+        }
+    for (int j = 0; j < hid; ++j)
+        for (int i = 0; i < H; ++i) fc1[(size_t)i * hid + j] = (*W0)[(size_t)j * H + i];
+    for (int k = 0; k < K; ++k)
+        for (int j = 0; j < hid; ++j) fc2[(size_t)j * K + k] = (*W3)[(size_t)k * hid + j];
+    EzHead &z = m->ez;
+    float scale = 1.0f;
+    cudaFree(z.d_wtc);
+    z.d_wtc = nullptr;
+    if (ez_tc_shape(nin, H)) {   // tensor-core copy of the LSTM weights (fp16 hi / lo, power-of-two scaled); other shapes (e.g. 8
+                                 // reward-head channels: nin = 288) run the fp32 k_ez_lstm
+        std::vector<unsigned char> wtc(ez_wtc_bytes(nin, H));
+        scale = ez_pack_wtc(Wih->data(), Whh->data(), nin, H, wtc.data());
+        int rc = upload(&z.d_wtc, wtc.data(), wtc.size());
+        if (rc != LZ_OK) return rc;
+    }
+    TablePacker P;
+    const size_t o_wcat = P.add(wcat), o_bias = P.add(bias), o_vps = P.add(vs), o_vpt = P.add(vt), o_fc1 = P.add(fc1);
+    const size_t o_s2 = P.add(s2), o_t2 = P.add(t2), o_fc2 = P.add(fc2), o_b2 = P.add(*B3);
+    int rc = upload(&z.d_tables, P.host.data(), P.host.size() * sizeof(float));
+    if (rc != LZ_OK) return rc;
+    const float *base = z.d_tables;
+    EzNet &e = z.net;
+    memset(&e, 0, sizeof(e));
+    e.wcat = base + o_wcat; e.bias = base + o_bias; e.vp_s = base + o_vps; e.vp_t = base + o_vpt;
+    e.fc1 = base + o_fc1; e.s2 = base + o_s2; e.t2 = base + o_t2; e.fc2 = base + o_fc2; e.b2 = base + o_b2;
+    e.nin = nin; e.H = H; e.hid = hid; e.K = K; e.no_vp_norm = vp_norm ? 0 : 1;
+    e.support_min = m->support_min; e.support_step = m->support_step;
+    e.wtc = z.d_wtc; e.wtc_inv_scale = 1.0f / scale;
+    return ez_prepare_launch();
+}
+
+// the LSTM input and hidden-state scratch of B roots
+int ez_reserve(lz_model *m, int B)
+{
+    EzHead &z = m->ez;
+    if (B <= z.B) return LZ_OK;
+    ++m->generation;
+    cudaFree(z.feat); cudaFree(z.htmp);
+    z.feat = z.htmp = nullptr;
+    int rc = dev_alloc(&z.feat, (size_t)B * z.net.nin);
+    if (rc == LZ_OK) rc = dev_alloc(&z.htmp, (size_t)B * m->lstm_hidden);
+    if (rc != LZ_OK) return rc;
+    z.B = B;
+    return LZ_OK;
+}
+
+// the head on the LSTM input features in m->ez.feat
+int ez_tail(lz_model *m, const RecIO &io, cudaStream_t s)
+{
+    EzIO e;
+    memset(&e, 0, sizeof(e));
+    e.B = io.B; e.feat = m->ez.feat; e.h_base = io.h_base; e.c_base = io.c_base; e.ix = io.ix; e.slot_stride = io.hslot_stride;
+    e.h_out = io.h_out; e.c_out = io.c_out; e.is_reset = io.is_reset; e.h_tmp = m->ez.htmp;
+    e.value_prefix = io.reward; e.vp_logits = io.reward_logits;
+    return ez_launch(m->ez.net, e, s);
 }
 
 }  // namespace lz

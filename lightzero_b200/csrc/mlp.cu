@@ -224,7 +224,7 @@ __global__ void __launch_bounds__(kMlpThreads) k_mlp_initial(MlpNet net, const f
 
 int mlp_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
 {
-    k_mlp_recurrent<false><<<ceil_div(io.B, kMlpRoots), kMlpThreads, 0, s>>>(m->mlp, io, MlpTap{});
+    k_mlp_recurrent<false><<<ceil_div(io.B, kMlpRoots), kMlpThreads, 0, s>>>(m->mlp.net, io, MlpTap{});
     LZ_KERNEL_CHECK();
     return LZ_OK;
 }
@@ -233,7 +233,7 @@ int mlp_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, cud
 {
     TailIO io = io_in;
     io.B = B;
-    k_mlp_initial<false><<<ceil_div(B, kMlpRoots), kMlpThreads, 0, s>>>(m->mlp, d_obs, io, MlpTap{});
+    k_mlp_initial<false><<<ceil_div(B, kMlpRoots), kMlpThreads, 0, s>>>(m->mlp.net, d_obs, io, MlpTap{});
     LZ_KERNEL_CHECK();
     return LZ_OK;
 }
@@ -243,7 +243,7 @@ int mlp_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, cud
 int mlp_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out,
                     size_t out_bytes, int32_t *h_info, cudaStream_t s)
 {
-    const MlpNet &n = m->mlp;
+    const MlpNet &n = m->mlp.net;
     const int L = n.latent, K = m->K, A = n.A;
     int w[16], D = 0;                                // output width of each tap stage, in program order
     if (which) {
@@ -291,92 +291,59 @@ int mlp_debug_stage(lz_model *m, int which, int B, const float *d_in, const int3
 }
 
 // ---- weights ----------------------------------------------------------------------------------
-static const std::vector<float> *mfind(lz_model *m, const std::string &name, size_t expect)
-{
-    auto it = m->tensors.find(name);
-    if (it == m->tensors.end()) { set_error("lz_model_finalize: missing tensor '%s'", name.c_str()); return nullptr; }
-    if (expect && it->second.size() != expect) {
-        set_error("lz_model_finalize: tensor '%s' has %zu elements, expected %zu", name.c_str(), it->second.size(), expect);
-        return nullptr;
-    }
-    return &it->second;
-}
-
 struct DenseOff { size_t wt, scale, shift; int in, out, act, nact; };
 
 // Linear `lin` (weight [out][in], bias [out]) optionally followed by eval BatchNorm1d `bn`
-static bool pack_dense(lz_model *m, std::vector<float> &host, const std::string &lin, const std::string &bn, int in, int out,
-                       int act, int nact, DenseOff &o)
+static bool pack_dense(lz_model *m, TablePacker &P, const std::string &lin, const std::string &bn, int in, int out, int act,
+                       int nact, DenseOff &o)
 {
-    auto W = mfind(m, lin + ".weight", (size_t)out * in), b = mfind(m, lin + ".bias", out);
+    auto W = find_tensor(m, lin + ".weight", (size_t)out * in), b = find_tensor(m, lin + ".bias", out);
     if (!W || !b) return false;
     std::vector<float> scale(out, 1.0f), shift(*b);
-    if (!bn.empty()) {
-        auto g = mfind(m, bn + ".weight", out), be = mfind(m, bn + ".bias", out);
-        auto mu = mfind(m, bn + ".running_mean", out), var = mfind(m, bn + ".running_var", out);
-        if (!g || !be || !mu || !var) return false;
-        for (int j = 0; j < out; ++j) {
-            const float s = (*g)[j] / sqrtf((*var)[j] + 1e-5f);
-            scale[j] = s;
-            shift[j] = (*be)[j] - (*mu)[j] * s + s * (*b)[j];
-        }
-    }
-    auto add = [&](const std::vector<float> &v) {
-        while (host.size() % 4) host.push_back(0.0f);
-        size_t off = host.size();
-        host.insert(host.end(), v.begin(), v.end());
-        return off;
-    };
+    if (!bn.empty() && !fold_bn_linear(m, bn, *b, scale, shift)) return false;
     std::vector<float> wt((size_t)in * out);
     for (int j = 0; j < out; ++j)
         for (int i = 0; i < in; ++i) wt[(size_t)i * out + j] = (*W)[(size_t)j * in + i];
-    o.wt = add(wt); o.scale = add(scale); o.shift = add(shift);
+    o.wt = P.add(wt); o.scale = P.add(scale); o.shift = P.add(shift);
     o.in = in; o.out = out; o.act = act; o.nact = nact;
     return true;
 }
 
 int mlp_finalize(lz_model *m)
 {
-    const lz_mlp_config &c = m->mcfg;
+    const lz_mlp_config &c = m->mlp.cfg;
     const int L = c.latent_dim, A = c.action_space_size, K = m->K;
-    std::vector<float> host;
+    TablePacker P;
     DenseOff e0, e1, d1a, d1b, d2a, d2b, r0, r1, pc0, pc1, v0, v1, p0, p1;
     memset(&d2a, 0, sizeof(d2a)); memset(&d2b, 0, sizeof(d2b));
     const std::string R = "representation_network.", D = "dynamics_network.", Q = "prediction_network.";
-    bool ok = pack_dense(m, host, R + "fc_representation.0", R + "fc_representation.1", c.obs_dim, L, 2, 0, e0) &&
-              pack_dense(m, host, R + "fc_representation.3", "", L, L, 0, 0, e1);
+    bool ok = pack_dense(m, P, R + "fc_representation.0", R + "fc_representation.1", c.obs_dim, L, 2, 0, e0) &&
+              pack_dense(m, P, R + "fc_representation.3", "", L, L, 0, 0, e1);
     if (ok && c.res_connection_in_dynamics)
-        ok = pack_dense(m, host, D + "fc_dynamics_1.0", D + "fc_dynamics_1.1", L + A, L, 1, A, d1a) &&
-             pack_dense(m, host, D + "fc_dynamics_1.3", D + "fc_dynamics_1.4", L, L, 1, 0, d1b) &&
-             pack_dense(m, host, D + "fc_dynamics_2.0", D + "fc_dynamics_2.1", L, L, 1, 0, d2a) &&
-             pack_dense(m, host, D + "fc_dynamics_2.3", D + "fc_dynamics_2.4", L, L, 1, 0, d2b);
+        ok = pack_dense(m, P, D + "fc_dynamics_1.0", D + "fc_dynamics_1.1", L + A, L, 1, A, d1a) &&
+             pack_dense(m, P, D + "fc_dynamics_1.3", D + "fc_dynamics_1.4", L, L, 1, 0, d1b) &&
+             pack_dense(m, P, D + "fc_dynamics_2.0", D + "fc_dynamics_2.1", L, L, 1, 0, d2a) &&
+             pack_dense(m, P, D + "fc_dynamics_2.3", D + "fc_dynamics_2.4", L, L, 1, 0, d2b);
     else if (ok)
-        ok = pack_dense(m, host, D + "fc_dynamics.0", D + "fc_dynamics.1", L + A, L, 1, A, d1a) &&
-             pack_dense(m, host, D + "fc_dynamics.3", D + "fc_dynamics.4", L, L, 1, 0, d1b);
-    ok = ok && pack_dense(m, host, D + "fc_reward_head.0", D + "fc_reward_head.1", L, c.reward_hidden, 1, 0, r0) &&
-         pack_dense(m, host, D + "fc_reward_head.3", "", c.reward_hidden, K, 0, 0, r1) &&
-         pack_dense(m, host, Q + "fc_prediction_common.0", Q + "fc_prediction_common.1", L, L, 1, 0, pc0) &&
-         pack_dense(m, host, Q + "fc_prediction_common.3", Q + "fc_prediction_common.4", L, L, 1, 0, pc1) &&
-         pack_dense(m, host, Q + "fc_value_head.0", Q + "fc_value_head.1", L, c.value_hidden, 1, 0, v0) &&
-         pack_dense(m, host, Q + "fc_value_head.3", "", c.value_hidden, K, 0, 0, v1) &&
-         pack_dense(m, host, Q + "fc_policy_head.0", Q + "fc_policy_head.1", L, c.policy_hidden, 1, 0, p0) &&
-         pack_dense(m, host, Q + "fc_policy_head.3", "", c.policy_hidden, A, 0, 0, p1);
+        ok = pack_dense(m, P, D + "fc_dynamics.0", D + "fc_dynamics.1", L + A, L, 1, A, d1a) &&
+             pack_dense(m, P, D + "fc_dynamics.3", D + "fc_dynamics.4", L, L, 1, 0, d1b);
+    ok = ok && pack_dense(m, P, D + "fc_reward_head.0", D + "fc_reward_head.1", L, c.reward_hidden, 1, 0, r0) &&
+         pack_dense(m, P, D + "fc_reward_head.3", "", c.reward_hidden, K, 0, 0, r1) &&
+         pack_dense(m, P, Q + "fc_prediction_common.0", Q + "fc_prediction_common.1", L, L, 1, 0, pc0) &&
+         pack_dense(m, P, Q + "fc_prediction_common.3", Q + "fc_prediction_common.4", L, L, 1, 0, pc1) &&
+         pack_dense(m, P, Q + "fc_value_head.0", Q + "fc_value_head.1", L, c.value_hidden, 1, 0, v0) &&
+         pack_dense(m, P, Q + "fc_value_head.3", "", c.value_hidden, K, 0, 0, v1) &&
+         pack_dense(m, P, Q + "fc_policy_head.0", Q + "fc_policy_head.1", L, c.policy_hidden, 1, 0, p0) &&
+         pack_dense(m, P, Q + "fc_policy_head.3", "", c.policy_hidden, A, 0, 0, p1);
     if (!ok) return LZ_EINVAL;
-    auto lw = mfind(m, R + "norm.weight", L), lb = mfind(m, R + "norm.bias", L);
+    auto lw = find_tensor(m, R + "norm.weight", L), lb = find_tensor(m, R + "norm.bias", L);
     if (!lw || !lb) return LZ_EINVAL;
-    while (host.size() % 4) host.push_back(0.0f);
-    const size_t o_lw = host.size();
-    host.insert(host.end(), lw->begin(), lw->end());
-    const size_t o_lb = host.size();
-    host.insert(host.end(), lb->begin(), lb->end());
-    if (m->d_weights) cudaFree(m->d_weights);
-    m->d_weights = nullptr;
-    int rc = dev_alloc(&m->d_weights, host.size());
+    const size_t o_lw = P.add(*lw), o_lb = P.add(*lb);
+    int rc = upload(&m->mlp.d_weights, P.host.data(), P.host.size() * sizeof(float));
     if (rc != LZ_OK) return rc;
-    LZ_CUDA_CHECK(cudaMemcpy(m->d_weights, host.data(), host.size() * sizeof(float), cudaMemcpyHostToDevice));
-    const float *base = m->d_weights;
+    const float *base = m->mlp.d_weights;
     auto mk = [&](const DenseOff &o) { Dense d; d.wt = base + o.wt; d.scale = base + o.scale; d.shift = base + o.shift; d.in = o.in; d.out = o.out; d.act = o.act; d.nact = o.nact; return d; };
-    MlpNet &n = m->mlp;
+    MlpNet &n = m->mlp.net;
     memset(&n, 0, sizeof(n));
     n.e0 = mk(e0); n.e1 = mk(e1); n.d1a = mk(d1a); n.d1b = mk(d1b);
     if (c.res_connection_in_dynamics) { n.d2a = mk(d2a); n.d2b = mk(d2b); }
@@ -384,8 +351,6 @@ int mlp_finalize(lz_model *m)
     n.ln_w = base + o_lw; n.ln_b = base + o_lb;
     n.latent = L; n.obs_dim = c.obs_dim; n.A = A; n.res = c.res_connection_in_dynamics;
     n.support_min = c.support_min; n.support_step = c.support_step;
-    m->finalized = true;
-    m->tensors.clear();
     return LZ_OK;
 }
 
@@ -394,7 +359,7 @@ int mlp_finalize(lz_model *m)
 using namespace lz;
 
 // The fp32 kernels above take the configs they were sized for; every other config inside k_mez_tc's envelope (mlp_tc.cu) runs
-// there as model kind 4.  The choice follows from the config alone, and a config both take stays on these kernels, so its
+// there, as the MlpTc family.  The choice follows from the config alone, and a config both take stays on these kernels, so its
 // outputs do not change.
 static bool mlp_fits(const lz_mlp_config &c)
 {
@@ -423,35 +388,16 @@ extern "C" int lz_model_create_mlp(const lz_mlp_config *cfg, lz_model **out)
                "head hidden sizes in [1,%d])",
                c.latent_dim, c.obs_dim, c.action_space_size, c.reward_hidden, c.value_hidden, c.policy_hidden, kMlpWidth, kMlpWidth,
                kMlpWidth, kMezMaxL, kMezMaxObs, kMezMaxOut, kMezMaxHid);
-    const int K = (int)ceil((cfg->support_max - cfg->support_min) / cfg->support_step);
-    LZ_REQUIRE(K >= 2 && K <= kMlpK, LZ_EINVAL, "lz_model_create_mlp: support size %d not in [2, %d]", K, kMlpK);
-    int ndev = 0;
-    LZ_CUDA_CHECK(cudaGetDeviceCount(&ndev));
-    LZ_REQUIRE(ndev > 0, LZ_ECUDA, "lz_model_create_mlp: no CUDA device (this library has no CPU fallback)");
+    int K = 0;
+    int rc = check_create("lz_model_create_mlp", c.support_min, c.support_max, c.support_step, kMlpK, &K);
+    if (rc != LZ_OK) return rc;
     lz_model *m = new lz_model();
-    memset(&m->cfg, 0, sizeof(m->cfg));
-    m->cfg.action_space_size = cfg->action_space_size;
-    m->cfg.support_min = cfg->support_min; m->cfg.support_max = cfg->support_max; m->cfg.support_step = cfg->support_step;
-    m->mcfg = *cfg;
-    m->latent_floats = cfg->latent_dim;
-    m->finalized = false;
-    m->d_weights = nullptr; m->d_tc = nullptr; m->d_tower = nullptr; m->tws = nullptr; m->tws_bytes = 0;
-    m->hw = 1; m->P = 1; m->K = K;
-    if (fp32) {
-        m->kind = 1;
-        m->pre_latent = nullptr; m->ws_B = 1 << 30;
-    } else {
-        m->kind = 4;
-        lz_mlp_ez_config &e = m->ecfg;       // the config mez_pack reads
-        memset(&e, 0, sizeof(e));
-        e.obs_dim = c.obs_dim; e.action_space_size = c.action_space_size; e.latent_dim = c.latent_dim;
-        e.reward_hidden = c.reward_hidden; e.value_hidden = c.value_hidden; e.policy_hidden = c.policy_hidden;
-        e.res_connection_in_dynamics = c.res_connection_in_dynamics;
-        e.support_min = c.support_min; e.support_max = c.support_max; e.support_step = c.support_step;
-        m->cfg.reward_hidden = c.reward_hidden; m->cfg.value_hidden = c.value_hidden; m->cfg.policy_hidden = c.policy_hidden;
-        m->lat_c = c.latent_dim; m->lat_h = m->lat_w = 1;
-        m->npass = 3;                      // default: tc3 (fp32-accurate)
-    }
+    m->family = fp32 ? ModelFamily::MlpFp32 : ModelFamily::MlpTc;
+    m->A = c.action_space_size; m->K = K; m->support_min = c.support_min; m->support_step = c.support_step;
+    m->lat_c = m->latent_floats = c.latent_dim; m->lat_h = m->lat_w = 1;
+    m->obs_elems = c.obs_dim;
+    if (fp32) m->mlp.cfg = c;
+    else m->mez = MlpTcState{c.obs_dim, c.latent_dim, c.reward_hidden, c.value_hidden, c.policy_hidden, c.res_connection_in_dynamics};
     *out = m;
     return LZ_OK;
 }

@@ -415,25 +415,7 @@ namespace {
 struct MezPacker {
     lz_model *m;
     std::vector<unsigned char> w;
-    std::vector<float> tab;
-
-    const std::vector<float> *get(const std::string &name, size_t expect)
-    {
-        auto it = m->tensors.find(name);
-        if (it == m->tensors.end()) { set_error("lz_model_finalize: missing tensor '%s'", name.c_str()); return nullptr; }
-        if (it->second.size() != expect) {
-            set_error("lz_model_finalize: tensor '%s' has %zu elements, expected %zu", name.c_str(), it->second.size(), expect);
-            return nullptr;
-        }
-        return &it->second;
-    }
-    int add(const std::vector<float> &v)
-    {
-        while (tab.size() % 4) tab.push_back(0.0f);
-        const int off = (int)tab.size();
-        tab.insert(tab.end(), v.begin(), v.end());
-        return off;
-    }
+    TablePacker tab;
 
     // Linear `lin` (weight [out_total][in_total]) rows row0 .. row0 + N of inputs 0 .. in_used (+ eval BatchNorm1d `bn`) as one
     // program layer of K (>= in_used, a multiple of 32) inputs; rows past out_total are zero.  Input columns in_used ..
@@ -441,32 +423,17 @@ struct MezPacker {
     bool layer(MezNet &net, const std::string &lin, const std::string &bn, int in_total, int in_used, int out_total, int row0,
                int N, int K, int in, int out, int flags, std::vector<float> *act = nullptr)
     {
-        auto W = get(lin + ".weight", (size_t)out_total * in_total), b = get(lin + ".bias", out_total);
+        auto W = find_tensor(m, lin + ".weight", (size_t)out_total * in_total), b = find_tensor(m, lin + ".bias", out_total);
         if (!W || !b) return false;
-        std::vector<float> s(N, 0.0f), t(N, 0.0f);
-        for (int n = 0; n < N; ++n) {
-            const int r = row0 + n;
-            if (r >= out_total) continue;
-            s[n] = 1.0f;
-            t[n] = (*b)[r];
-        }
-        if (!bn.empty()) {
-            auto g = get(bn + ".weight", out_total), be = get(bn + ".bias", out_total);
-            auto mu = get(bn + ".running_mean", out_total), var = get(bn + ".running_var", out_total);
-            if (!g || !be || !mu || !var) return false;
-            for (int n = 0; n < N && row0 + n < out_total; ++n) {
-                const int r = row0 + n;
-                const float sc = (*g)[r] / sqrtf((*var)[r] + 1e-5f);
-                s[n] = sc;
-                t[n] = (*be)[r] - (*mu)[r] * sc + sc * (*b)[r];
-            }
-        }
+        std::vector<float> fs(out_total, 1.0f), ft(*b), s(N, 0.0f), t(N, 0.0f);
+        if (!bn.empty() && !fold_bn_linear(m, bn, *b, fs, ft)) return false;
         float mx = 0.0f;
-        for (int n = 0; n < N && row0 + n < out_total; ++n)
+        for (int n = 0; n < N && row0 + n < out_total; ++n) {
+            s[n] = fs[row0 + n];
+            t[n] = ft[row0 + n];
             for (int k = 0; k < in_used; ++k) mx = std::max(mx, fabsf((*W)[(size_t)(row0 + n) * in_total + k]));
-        int e = 0;
-        if (mx > 0.0f) frexpf(mx, &e);
-        const float scale = ldexpf(1.0f, 13 - e);        // largest |w| lands in [4096, 8192): the lo parts stay in fp16's normal range
+        }
+        const float scale = pow2_scale(mx);
         const size_t woff = w.size(), chunk = (size_t)128 * N;
         w.resize(woff + chunk * (K / 32));
         __half *hp = reinterpret_cast<__half *>(w.data() + woff);
@@ -476,10 +443,8 @@ struct MezPacker {
                     for (int u = 0; u < 8; ++u) {
                         const int k = 32 * c + 8 * kg + u, r = row0 + n;
                         const float v = (r < out_total && k < in_used) ? (*W)[(size_t)r * in_total + k] * scale : 0.0f;
-                        const __half hi = __float2half_rn(v), lo = __float2half_rn(v - __half2float(hi));
                         const size_t off = c * chunk / 2 + ((size_t)kg * 2 * N + n) * 8 + u;
-                        hp[off] = hi;
-                        hp[off + (size_t)N * 8] = lo;
+                        split_hi_lo(v, hp[off], hp[off + (size_t)N * 8]);
                     }
         if (act) {
             const int na = in_total - in_used;
@@ -492,7 +457,7 @@ struct MezPacker {
         for (int n = 0; n < N; ++n) { st[n] = s[n] / scale; st[N + n] = t[n]; }
         LZ_REQUIRE(net.nlayers < kMezMaxLayers, false, "lz_model_finalize: more than %d layers", kMezMaxLayers);
         MezLayer &ly = net.layer[net.nlayers++];
-        ly.woff = (uint32_t)woff; ly.K = K; ly.N = N; ly.in = in; ly.out = out; ly.flags = flags; ly.bn = add(st); ly.col0 = row0;
+        ly.woff = (uint32_t)woff; ly.K = K; ly.N = N; ly.in = in; ly.out = out; ly.flags = flags; ly.bn = (int)tab.add(st); ly.col0 = row0;
         net.nchunks += K / 32;
         return true;
     }
@@ -525,16 +490,17 @@ struct MezPacker {
 
 }  // namespace
 
-// Kind 3 (EfficientZeroModelMLP) and kind 4 (MuZeroModelMLP) share the programs up to what follows the dynamics MLP: kind 3
-// writes its output as the LSTM input (MF_FEAT), kind 4 runs the reward head on it (muzero_model_mlp.py:428-440).  Slots of the
+// EfficientZeroModelMLP and MuZeroModelMLP share the programs up to what follows the dynamics MLP: EfficientZeroModelMLP writes
+// its output as the LSTM input (MF_FEAT) of the value-prefix head (ez.cu), MuZeroModelMLP runs the reward head on it
+// (muzero_model_mlp.py:428-440).  Slots of the
 // recurrent program: the input latent z in slot 0; fc_dynamics_1 (+ z) -> slot 0 = the next latent; fc_dynamics_2 -> slot 1,
 // which the reward head reads; the prediction network reads slot 0 and works in slot 1.  Without res_connection_in_dynamics
 // fc_dynamics -> slot 0 is both the next latent and the reward head's input.
-int mez_pack(lz_model *m)
+int mez_finalize(lz_model *m)
 {
-    const lz_mlp_ez_config &c = m->ecfg;
-    const bool mz = m->kind == 4;
-    const int L = c.latent_dim, A = c.action_space_size, K = m->K, kobs = (c.obs_dim + 31) / 32 * 32;
+    const MlpTcState &c = m->mez;
+    const bool mz = !m->vp;
+    const int L = c.latent, A = m->A, K = m->K, kobs = (c.obs_dim + 31) / 32 * 32;
     MezPacker P;
     P.m = m;
     MezNet init, rec;
@@ -545,7 +511,7 @@ int mez_pack(lz_model *m)
     bool ok = P.layer(init, R + "fc_representation.0", R + "fc_representation.1", c.obs_dim, c.obs_dim, L, 0, L, kobs, MB_OBS, MB_SLOT0, MF_GELU) &&
               P.layer(init, R + "fc_representation.3", "", L, L, L, 0, L, L, MB_SLOT0, MB_SLOT0, MF_LN | MF_LATENT) &&
               P.predict(init, MB_SLOT0, L, A, K, c.value_hidden, c.policy_hidden);
-    if (ok && c.res_connection_in_dynamics)     // next = fc_dynamics_1([z | a]) + z; LSTM / reward head input = fc_dynamics_2(next)
+    if (ok && c.res)     // next = fc_dynamics_1([z | a]) + z; LSTM / reward head input = fc_dynamics_2(next)
         ok = P.layer(rec, D + "fc_dynamics_1.0", D + "fc_dynamics_1.1", L + A, L, L, 0, L, L, MB_SLOT0, MB_SLOT1, MF_RELU | MF_ACT, &act) &&
              P.layer(rec, D + "fc_dynamics_1.3", D + "fc_dynamics_1.4", L, L, L, 0, L, L, MB_SLOT1, MB_SLOT0, MF_RELU | MF_RES | MF_LATENT) &&
              P.layer(rec, D + "fc_dynamics_2.0", D + "fc_dynamics_2.1", L, L, L, 0, L, L, MB_SLOT0, MB_SLOT1, MF_RELU) &&
@@ -558,25 +524,108 @@ int mez_pack(lz_model *m)
              (!mz || P.cat_head(rec, D + "fc_reward_head", MB_SLOT0, L, c.reward_hidden, K, MF_REWARD));
     ok = ok && P.predict(rec, MB_SLOT0, L, A, K, c.value_hidden, c.policy_hidden);
     if (!ok) return LZ_EINVAL;
-    auto lw = P.get(R + "norm.weight", L), lb = P.get(R + "norm.bias", L);
+    auto lw = find_tensor(m, R + "norm.weight", L), lb = find_tensor(m, R + "norm.bias", L);
     if (!lw || !lb) return LZ_EINVAL;
-    const int o_lw = P.add(*lw), o_lb = P.add(*lb), o_act = P.add(act);
+    const size_t o_lw = P.tab.add(*lw), o_lb = P.tab.add(*lb), o_act = P.tab.add(act);
+    // one upload: the weight chunks, then the tables from the next 256-byte boundary
     const size_t wbytes = (P.w.size() + 255) & ~(size_t)255;
-    if (m->d_mez) cudaFree(m->d_mez);
-    m->d_mez = nullptr;
-    int rc = dev_alloc(&m->d_mez, wbytes + P.tab.size() * sizeof(float));
+    P.w.resize(wbytes, 0);
+    P.w.insert(P.w.end(), reinterpret_cast<const unsigned char *>(P.tab.host.data()),
+               reinterpret_cast<const unsigned char *>(P.tab.host.data() + P.tab.host.size()));
+    int rc = upload(&m->mez.d_mez, P.w.data(), P.w.size());
     if (rc != LZ_OK) return rc;
-    LZ_CUDA_CHECK(cudaMemcpy(m->d_mez, P.w.data(), P.w.size(), cudaMemcpyHostToDevice));
-    LZ_CUDA_CHECK(cudaMemcpy(m->d_mez + wbytes, P.tab.data(), P.tab.size() * sizeof(float), cudaMemcpyHostToDevice));
-    const float *tab = reinterpret_cast<const float *>(m->d_mez + wbytes);
+    const float *tab = reinterpret_cast<const float *>(m->mez.d_mez + wbytes);
     for (MezNet *n : {&init, &rec}) {
-        n->w = m->d_mez; n->tab = tab; n->abias = tab + o_act; n->ln_w = tab + o_lw; n->ln_b = tab + o_lb;
+        n->w = m->mez.d_mez; n->tab = tab; n->abias = tab + o_act; n->ln_w = tab + o_lw; n->ln_b = tab + o_lb;
         n->L = L; n->A = A; n->K = K; n->obs_dim = c.obs_dim;
-        n->support_min = c.support_min; n->support_step = c.support_step;
+        n->support_min = m->support_min; n->support_step = m->support_step;
     }
-    m->mez_init = init;
-    m->mez_rec = rec;
-    return mez_prepare_launch();
+    m->mez.init = init;
+    m->mez.rec = rec;
+    if ((rc = mez_prepare_launch()) != LZ_OK) return rc;
+    return m->vp ? ez_finalize(m, L, c.reward_hidden, false) : LZ_OK;
+}
+
+static MezIO mez_io(const lz_model *m, int B)
+{
+    MezIO e;
+    memset(&e, 0, sizeof(e));
+    e.B = B; e.npass = m->npass;
+    return e;
+}
+
+int mez_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
+{
+    // EfficientZeroModelMLP's LSTM input goes on through the value-prefix head (ez.cu), MuZeroModelMLP's reward head is part of
+    // the program
+    const bool ez = m->vp;
+    if (ez) {
+        LZ_REQUIRE(io.B <= m->ez.B, LZ_ESTATE, "model_recurrent: EfficientZero scratch sized for %d roots, got %d (model_reserve)", m->ez.B, io.B);
+        LZ_REQUIRE(io.h_base && io.c_base, LZ_EINVAL, "model_recurrent: EfficientZero needs the reward hidden state");
+    }
+    MezIO e = mez_io(m, io.B);
+    e.latent_base = io.latent_base; e.ix = io.ix; e.slot_stride = io.slot_stride; e.action = io.action;
+    e.latent_out = io.next_latent;
+    if (ez) e.feat = m->ez.feat;
+    else { e.reward = io.reward; e.reward_logits = io.reward_logits; }
+    e.value = io.value; e.policy_logits = io.policy_logits; e.value_logits = io.value_logits;
+    int rc = mez_launch(m->mez.rec, e, s);
+    if (rc || !ez) return rc;
+    return ez_tail(m, io, s);
+}
+
+int mez_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, cudaStream_t s)
+{
+    MezIO e = mez_io(m, B);
+    e.obs = d_obs; e.latent_out = io_in.latent; e.latent_out2 = io_in.latent2;
+    e.value = io_in.value; e.policy_logits = io_in.policy_logits; e.value_logits = io_in.value_logits;
+    return mez_launch(m->mez.init, e, s);
+}
+
+// lz_model_debug_net_stage of EfficientZeroModelMLP and of MuZeroModelMLP on the tensor cores: which 1 is initial_inference on
+// the observations d_in
+int mez_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out,
+                           size_t out_bytes, int32_t *h_info, cudaStream_t st)
+{
+    MezNet net = which ? m->mez.init : m->mez.rec;          // a copy: the model's programs stay as they are
+    const int L = net.L, K = net.K, A = net.A;
+    const bool rew = !which && !m->vp;               // MuZeroModelMLP's recurrent program has the reward head
+    int dense[kMezMaxLayers], D = 0;                        // the program indices of the L-wide layers outside the heads
+    for (int l = 0; l < net.nlayers; ++l)
+        if (net.layer[l].N == L && !(net.layer[l].flags & (MF_VALUE | MF_REWARD | MF_POLICY)) && net.layer[l].out != MB_HID) dense[D++] = l;
+    LZ_REQUIRE(stage <= D, LZ_EINVAL, "lz_model_debug_net_stage: stage %d past the %d dense layers of the program", stage, D);
+    const size_t nfl = stage < D ? (size_t)B * L : (size_t)B * (K + A + 1 + 2 * L + (rew ? K + 1 : 0));
+    LZ_REQUIRE(out_bytes >= nfl * sizeof(float), LZ_EINVAL, "lz_model_debug_net_stage: stage %d needs %zu bytes, got %zu", stage,
+               nfl * sizeof(float), out_bytes);
+    MezIO io = mez_io(m, B);
+    if (which) io.obs = d_in;
+    else { io.latent_base = d_in; io.action = d_action; }
+    float *o = reinterpret_cast<float *>(d_out);
+    if (stage < D) {
+        // the program cut after dense layer `stage`, whose output is the only one written (the reward head before it, in
+        // MuZeroModelMLP's recurrent program, runs with no output)
+        const int cut = dense[stage];
+        net.nlayers = cut + 1;
+        net.nchunks = 0;
+        for (int l = 0; l <= cut; ++l) {
+            net.layer[l].flags &= ~(MF_LATENT | MF_FEAT);
+            net.nchunks += net.layer[l].K / 32;
+        }
+        net.layer[cut].flags |= MF_LATENT;
+        io.latent_out = o;
+    } else {
+        // the latent sections first: the kernel writes them as float2 pairs; then value logits, policy logits, value, and for
+        // MuZeroModelMLP's recurrent program reward logits and reward (its LSTM-input section stays zero)
+        LZ_CUDA_CHECK(cudaMemsetAsync(d_out, 0, nfl * sizeof(float), st));
+        io.latent_out = o;
+        if (!which && m->vp) io.feat = o + (size_t)B * L;
+        io.value_logits = o + (size_t)2 * B * L; io.policy_logits = io.value_logits + (size_t)B * K; io.value = io.policy_logits + (size_t)B * A;
+        if (rew) { io.reward_logits = io.value + B; io.reward = io.reward_logits + (size_t)B * K; }
+    }
+    const MezPlan p = mez_plan(net, B);
+    const int32_t info[8] = {p.R, p.ctas, p.last, net.nlayers, m->npass, p.smem, p.stages, D};
+    memcpy(h_info, info, sizeof(info));
+    return mez_launch(net, io, st);
 }
 
 }  // namespace lz

@@ -68,6 +68,5 @@ struct MezPlan { int R, ctas, last, smem, stages; };
 MezPlan mez_plan(const MezNet &net, int B);
 int mez_launch(const MezNet &net, const MezIO &io, cudaStream_t s);
 int mez_prepare_launch();
-int mez_pack(lz_model *m);            // dense layers of kinds 3 and 4 (+ kind 4's reward head) -> m->d_mez, m->mez_rec / m->mez_init
 
 }  // namespace lz

@@ -1,5 +1,9 @@
-// model.cuh -- device-side weight tables of the MuZero conv model and the internal launch API.
+// model.cuh -- the model families' state, the common lz_model fields, the internal launch API and the state_dict reader /
+// weight-packing kit that every family's finalize uses (model.cu).
 #pragma once
+#include <cuda_fp16.h>
+#include <math.h>
+
 #include <map>
 #include <string>
 #include <vector>
@@ -46,7 +50,7 @@ struct RecIO {
     float *reward, *value;            // [B] scalars or nullptr
     float *policy_logits;             // [B][A] or nullptr
     float *reward_logits, *value_logits;   // [B][K] or nullptr
-    float *skip_scratch;              // [B][64 P] scratch of the tensor-core path (nullptr: the model's own, lz_model::tc_skip)
+    float *skip_scratch;              // [B][64 P] scratch of the tensor-core path (nullptr: the model's own, ConvState::tc_skip)
     // EfficientZero (reward == value prefix): LSTM state in / out, see ez.cuh
     const float *h_base, *c_base;     // base + ix[b]*hslot_stride + b*H
     size_t hslot_stride;
@@ -64,64 +68,167 @@ struct TailIO {
     float *value_logits;              // [B][K] or nullptr
 };
 
-}  // namespace lz
+// The model families: each has its own state below and its own module; model.cu switches on the family at every lz_model_*
+// entry point and calls the owning module's function.
+enum class ModelFamily {
+    Conv,                             // MuZeroModel / EfficientZeroModel with the DownSample tower (conv_model.cu)
+    Board,                            // MuZeroModel with downsample=False, the board games (board_tc.cu)
+    MlpFp32,                          // MuZeroModelMLP on the fp32 kernels (mlp.cu)
+    MlpTc,                            // EfficientZeroModelMLP, and the MuZeroModelMLP configs mlp.cu does not take (mlp_tc.cu)
+};
 
-struct lz_model {
-    int kind;                         // 0 = conv MuZeroModel / EfficientZeroModel (cfg.efficientzero), 1 = MuZeroModelMLP (mlp.cu),
-                                      // 2 = board MuZeroModel (downsample=False, board_tc.cu), 3 = EfficientZeroModelMLP (mlp_tc.cu),
-                                      // 4 = MuZeroModelMLP on the tensor cores (mlp_tc.cu): the configs mlp.cu does not take
-                                      // (lz_model_create_mlp picks 1 or 4)
-    unsigned char *d_board;           // kind 2: packed conv weights, BN / action-plane tables and fp32 head tables
-    lz::BoardNet board_rec, board_init;   // kind 2: recurrent_inference / initial_inference programs
-    lz_mlp_ez_config ecfg;            // kinds 3 and 4 (kind 4: the lz_mlp_config fields, lstm_hidden_size 0)
-    unsigned char *d_mez;             // kinds 3, 4: packed fp16 hi / lo weights and fp32 tables of the dense layers
-    lz::MezNet mez_rec, mez_init;     // kinds 3, 4: recurrent_inference (dense part) / initial_inference programs
-    int lat_c, lat_h, lat_w;          // latent shape of one root
-    lz::EzNet ez;                     // EfficientZero value-prefix head tables (device pointers into d_weights)
-    float *ez_feat, *ez_htmp;         // [ws_B][hc*36], [ws_B][H] scratch between the conv kernel and the LSTM kernels
-    int ez_B;
-    unsigned char *d_ez_wtc;          // LSTM weights in the tensor-core layout (ez.cu)
-    int latent_floats;                // floats per root latent (64*36, 64*64 or latent_dim)
-    lz_mlp_config mcfg;               // kinds 1 and 4
-    lz::MlpNet mlp;
+struct ConvState {
     lz_model_config cfg;
-    std::map<std::string, std::vector<float>> tensors;   // raw reference state_dict (host)
-    bool finalized;
-    float *d_weights;                 // one packed device allocation
-    size_t n_weight_floats;
-    lz::ConvG stem;                   // DownSample conv1 + norm1 (fp32 tables in d_weights)
-    std::vector<float> stem_params;   // host copy of the Cin = 4 stem's weights + folded BN (kernel-parameter operands of k_stem4_tcl, model.cu)
+    float *d_weights;                 // fp32 tables of the stem and of the heads' FC parts
+    ConvG stem;                       // DownSample conv1 + norm1 (fp32 tables in d_weights)
+    std::vector<float> stem_params;   // host copy of the Cin = 4 stem's weights + folded BN (kernel-parameter operands of k_stem4_tcl)
     int stem_valid;
-    int hw, P, K;
-    int npass;                        // MMA passes per product of the tensor-core kernels: 3 = tc3 (fp16 hi/lo, fp32-accurate), 1 = tc1
-    unsigned char *d_tc;              // packed fp16 hi/lo weights + tables of the tensor-core path
-    lz::TcNet tc_rec, tc_tail;
-    float *tc_skip;                   // [tc_skip_B][64 P] ResBlock skip scratch of k_net_tc for launches outside a search (model_reserve)
+    unsigned char *d_tc;              // packed fp16 hi/lo weights + tables of the latent-grid network (net_tc.cu)
+    TcNet tc_rec, tc_tail;
+    float *tc_skip;                   // [tc_skip_B][64 P] ResBlock skip scratch of k_net_tc for launches outside a search
     int tc_skip_B;
     // tensor-core DownSample tower: packed weights / folded BN per layer, TCL activation workspace
     unsigned char *d_tower;           // weights + scale/shift tables
-    lz::ConvTc tower_tc[2];           // downsample block: conv1 | conv3 (stride 2), conv2 (+ identity)
-    lz::ResBlockTc tower_rb[3];       // resblocks1, resblocks2, resblocks3
+    ConvTc tower_tc[2];               // downsample block: conv1 | conv3 (stride 2), conv2 (+ identity)
+    ResBlockTc tower_rb[3];           // resblocks1, resblocks2, resblocks3
     unsigned char *tws;               // TCL workspace (one allocation)
-    size_t tws_bytes;
-    lz::Tcl T0, T1, U0, U1, U2, V0, V1;
+    Tcl T0, T1, U0, U1, U2, V0, V1;
     // workspace for initial inference (grown on demand, outside graph capture)
     float *pre_latent;                // [ws_B][latent_floats] DownSample output, input of the latent-grid tail
     int ws_B;
+};
+
+struct BoardState {
+    lz_model_config cfg;
+    unsigned char *d_board;           // packed conv weights, BN / action-plane tables and fp32 head tables
+    BoardNet rec, init;               // recurrent_inference / initial_inference programs
+};
+
+struct MlpFp32State {
+    lz_mlp_config cfg;
+    float *d_weights;
+    MlpNet net;
+};
+
+struct MlpTcState {
+    int obs_dim, latent, reward_hidden, value_hidden, policy_hidden, res;   // res: res_connection_in_dynamics
+    unsigned char *d_mez;             // packed fp16 hi / lo weights and fp32 tables of the dense layers
+    MezNet rec, init;                 // recurrent_inference (dense part) / initial_inference programs
+};
+
+// EfficientZero's value-prefix head (ez.cu) on the LSTM input features that the Conv or the MlpTc network writes into `feat`
+struct EzHead {
+    EzNet net;
+    float *d_tables;                  // fp32 tables of the LSTM and of fc_reward_head
+    unsigned char *d_wtc;             // LSTM weights in the tensor-core layout
+    float *feat, *htmp;               // [B][nin], [B][H] scratch between the network kernel and the LSTM kernels
+    int B;
+};
+
+}  // namespace lz
+
+struct lz_model {
+    lz::ModelFamily family;
+    bool vp;                          // EfficientZero: the reward is a value prefix from the LSTM head in `ez`
+    int lstm_hidden;                  // its LSTM width (0 without the head)
+    int A, K;                         // actions, support size
+    float support_min, support_step;
+    int lat_c, lat_h, lat_w;          // latent shape of one root ([latent_dim][1][1] for the MLP families)
+    int latent_floats;                // lat_c * lat_h * lat_w
+    size_t obs_elems;                 // observation elements of one root
+    int npass = 3;                    // MMA passes per product of the tensor-core kernels: 3 = tc3 (fp16 hi/lo, fp32-accurate), 1 = tc1
     unsigned long long generation;    // bumped when device tables / workspaces that captured search graphs point into are re-allocated
                                       // or the pass count changes (finalize, set_math, model_reserve): lz_search re-captures
+    bool finalized;
+    std::map<std::string, std::vector<float>> tensors;   // raw reference state_dict (host)
+    lz::ConvState conv;
+    lz::BoardState board;
+    lz::MlpFp32State mlp;
+    lz::MlpTcState mez;
+    lz::EzHead ez;
 };
 
 namespace lz {
+// ---- the state_dict reader and weight-packing kit (model.cu) ----
+// the tensor `name` of the state_dict given to lz_model_set_tensor, with `expect` elements (0: any); nullptr and the error set
+// when it is missing or has another size
+const std::vector<float> *find_tensor(const lz_model *m, const std::string &name, size_t expect);
+
+// Eval-mode BatchNorm (eps = 1e-5) as y = x * scale + shift.  The two folds round differently and each family's tables were
+// fixed with its own: fold_bn computes g * (1 / sqrt(v + eps)) and leaves any preceding bias to the caller (the conv families);
+// fold_bn_linear computes g / sqrt(v + eps) and folds the Linear bias b into the shift as be - mu s + s b (the MLP families).
+bool fold_bn(const lz_model *m, const std::string &prefix, int n, std::vector<float> &scale, std::vector<float> &shift);
+bool fold_bn_linear(const lz_model *m, const std::string &prefix, const std::vector<float> &b, std::vector<float> &scale,
+                    std::vector<float> &shift);
+
+// fp32 tables appended at 16-byte aligned float offsets
+struct TablePacker {
+    std::vector<float> host;
+    size_t add(const std::vector<float> &v);
+};
+
+// the power-of-two scale that puts a weight matrix's largest |w| (`maxabs`) in [4096, 8192): the lo parts of the fp16 hi / lo
+// split stay in fp16's normal range.  The scale is exact; callers fold its inverse into the layer's fp32 scale.
+float pow2_scale(float maxabs);
+
+inline void split_hi_lo(float v, __half &hi, __half &lo)
+{
+    hi = __float2half_rn(v);
+    lo = __float2half_rn(v - __half2float(hi));
+}
+
+// replaces the device table *dst with a copy of `bytes` host bytes
+template <typename T>
+int upload(T **dst, const void *src, size_t bytes)
+{
+    cudaFree(*dst);
+    *dst = nullptr;
+    int rc = dev_alloc(reinterpret_cast<unsigned char **>(dst), bytes);
+    if (rc != LZ_OK) return rc;
+    LZ_CUDA_CHECK(cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice));
+    return LZ_OK;
+}
+
+// the create functions' common checks: the support size K = len(torch.arange(min, max, step)) in [2, kmax], and a CUDA device
+int check_create(const char *fn, float support_min, float support_max, float support_step, int kmax, int *K);
+
+// ---- the families behind the entry points ----
 int model_recurrent(lz_model *m, const RecIO &io, cudaStream_t s);
 int model_initial(lz_model *m, int B, const float *d_obs, const TailIO &io, cudaStream_t s);
-int model_initial_tower(lz_model *m, int B, const float *d_obs, float *pre_latent, cudaStream_t s, const uint8_t *d_obs_u8 = nullptr);   // exactly one of d_obs / d_obs_u8
-int model_initial_tail(lz_model *m, int B, const float *pre_latent, const TailIO &io, cudaStream_t s);
-int model_reserve(lz_model *m, int B);   // sizes the initial-inference workspace (synchronous)
+int model_reserve(lz_model *m, int B);   // sizes the scratch of launches outside a search (synchronous, outside capture)
+// lz_model_debug_net_stage of each family: `which` 0 is the recurrent program on the latents d_in and actions d_action, 1 the
+// initial_inference program on the observations d_in
+
+// Conv (conv_model.cu)
+int conv_finalize(lz_model *m);
+int conv_reserve(lz_model *m, int B);
+int conv_reserve_skip(lz_model *m, int B);   // the skip scratch alone (lz_model_recurrent_inference)
+int conv_recurrent(lz_model *m, const RecIO &io, cudaStream_t s);
+int conv_initial(lz_model *m, int B, const float *d_obs, const TailIO &io, cudaStream_t s);
+int conv_initial_tower(lz_model *m, int B, const float *d_obs, float *pre_latent, cudaStream_t s, const uint8_t *d_obs_u8 = nullptr);   // exactly one of d_obs / d_obs_u8
+int conv_initial_tail(lz_model *m, int B, const float *pre_latent, const TailIO &io, cudaStream_t s);
+int conv_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out, size_t out_bytes,
+                     int32_t *h_info, cudaStream_t s);
+// Board (board_tc.cu)
+int board_finalize(lz_model *m);
+int board_recurrent(lz_model *m, const RecIO &io, cudaStream_t s);
+int board_initial(lz_model *m, int B, const float *d_obs, const TailIO &io, cudaStream_t s);
+int board_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out, size_t out_bytes,
+                      int32_t *h_info, cudaStream_t s);
+// MlpFp32 (mlp.cu)
+int mlp_finalize(lz_model *m);
 int mlp_recurrent(lz_model *m, const RecIO &io, cudaStream_t s);
 int mlp_initial(lz_model *m, int B, const float *d_obs, const TailIO &io, cudaStream_t s);
-int mlp_finalize(lz_model *m);
-int mlp_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out,
-                    size_t out_bytes, int32_t *h_info, cudaStream_t s);
-bool model_is_ez(const lz_model *m);     // EfficientZero (value-prefix LSTM head): conv EfficientZeroModel or EfficientZeroModelMLP
+int mlp_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out, size_t out_bytes,
+                    int32_t *h_info, cudaStream_t s);
+// MlpTc (mlp_tc.cu)
+int mez_finalize(lz_model *m);
+int mez_recurrent(lz_model *m, const RecIO &io, cudaStream_t s);
+int mez_initial(lz_model *m, int B, const float *d_obs, const TailIO &io, cudaStream_t s);
+int mez_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out, size_t out_bytes,
+                    int32_t *h_info, cudaStream_t s);
+// the value-prefix head (ez.cu)
+int ez_finalize(lz_model *m, int nin, int hid, bool vp_norm);
+int ez_reserve(lz_model *m, int B);
+int ez_tail(lz_model *m, const RecIO &io, cudaStream_t s);
 }  // namespace lz

@@ -920,13 +920,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_net_tc(TcNet net, TcIO io, Tr
 }
 
 // ---------------------------------------------------------------------------------------------- host
-static void split_half(float v, float scale, __half &hi, __half &lo)
-{
-    float s = v * scale;
-    hi = __float2half_rn(s);
-    lo = __float2half_rn(s - __half2float(hi));
-}
-
 // One 3x3 conv -> 9 tap blocks, each [kg = ci/8][co: 64 hi rows | 64 lo rows][ci % 8] fp16.  Returns the power-of-two
 // scale applied to the weights (exact), which the caller folds into the BatchNorm scale.
 float tc_pack_conv3(const float *w_torch /*[64][cin][3][3]*/, int cin_total, int cin_used, unsigned char *dst)
@@ -935,18 +928,14 @@ float tc_pack_conv3(const float *w_torch /*[64][cin][3][3]*/, int cin_total, int
     for (int co = 0; co < 64; ++co)
         for (int ci = 0; ci < cin_used; ++ci)
             for (int t = 0; t < 9; ++t) mx = std::max(mx, fabsf(w_torch[((size_t)co * cin_total + ci) * 9 + t]));
-    int e = 0;
-    if (mx > 0.0f) frexpf(mx, &e);               // mx = f * 2^e, f in [0.5, 1)
-    const float scale = ldexpf(1.0f, 13 - e);    // largest |w| lands in [4096, 8192)
+    const float scale = pow2_scale(mx);
     __half *h = reinterpret_cast<__half *>(dst);
     for (int t = 0; t < 9; ++t)
         for (int co = 0; co < 64; ++co)
             for (int ci = 0; ci < 64; ++ci) {
-                __half hi, lo;
-                split_half(w_torch[((size_t)co * cin_total + ci) * 9 + t], scale, hi, lo);
                 const size_t off = (size_t)t * (kTapBytes / 2) + ((size_t)(ci / 8) * 128 + co) * 8 + (ci % 8);
-                h[off] = hi;
-                h[off + 64 * 8] = lo;             // rows 64-127 of the k-group: the lo parts ([B_hi | B_lo] is one N = 128 operand)
+                // rows 64-127 of the k-group: the lo parts ([B_hi | B_lo] is one N = 128 operand)
+                split_hi_lo(w_torch[((size_t)co * cin_total + ci) * 9 + t] * scale, h[off], h[off + 64 * 8]);
             }
     return scale;
 }
@@ -956,17 +945,12 @@ float tc_pack_conv1(const float *w /*[hc][64]*/, int hc, int nco, int co_offset,
 {
     float mx = 0.0f;
     for (int i = 0; i < hc * 64; ++i) mx = std::max(mx, fabsf(w[i]));
-    int e = 0;
-    if (mx > 0.0f) frexpf(mx, &e);
-    const float scale = ldexpf(1.0f, 13 - e);
+    const float scale = pow2_scale(mx);
     __half *hh = reinterpret_cast<__half *>(dst_hi), *hl = reinterpret_cast<__half *>(dst_lo);
     for (int co = 0; co < hc; ++co)
         for (int ci = 0; ci < 64; ++ci) {
-            __half hi, lo;
-            split_half(w[co * 64 + ci], scale, hi, lo);
             const size_t off = ((size_t)(ci / 8) * nco + co + co_offset) * 8 + (ci % 8);
-            hh[off] = hi;
-            hl[off] = lo;
+            split_hi_lo(w[co * 64 + ci] * scale, hh[off], hl[off]);
         }
     return scale;
 }

@@ -80,7 +80,7 @@ static RecIO rec_io(const lz_search *q, int sim)
 // EfficientZero stays a multi-kernel graph: its LSTM step is a GEMM over all roots (several launches per simulation).
 static bool persistent_search(const lz_search *q, bool reuse)
 {
-    return !reuse && !q->tree->gumbel && !q->hpool && q->model->kind == 0 && q->tree->p.A <= 32;   // tree_persist.cuh: one lane per child
+    return !reuse && !q->tree->gumbel && !q->hpool && q->model->family == ModelFamily::Conv && q->tree->p.A <= 32;   // tree_persist.cuh: one lane per child
 }
 
 static TcIO persistent_io(const lz_search *q, int deterministic)
@@ -124,7 +124,7 @@ static int enqueue_search(lz_search *q, int deterministic, bool reuse, cudaStrea
     int rc;
     lz_tree *t = q->tree;
     t->step_counter = 0;
-    if (persistent_search(q, reuse)) return tc_launch(q->model->tc_rec, persistent_io(q, deterministic), s, &t->p);
+    if (persistent_search(q, reuse)) return tc_launch(q->model->conv.tc_rec, persistent_io(q, deterministic), s, &t->p);
     TreeStep descent = {};
     descent.traverse = 1; descent.deterministic = deterministic;
     descent.act = q->d_action; descent.is_reset = q->d_is_reset;
@@ -242,8 +242,8 @@ int lz_search_create(lz_tree *t, lz_model *m, int num_simulations, lz_search **o
     LZ_REQUIRE(t && m && out && num_simulations > 0, LZ_EINVAL, "lz_search_create: bad argument");
     LZ_REQUIRE(m->finalized, LZ_ESTATE, "lz_search_create: model not finalized");
     LZ_REQUIRE(num_simulations <= t->max_sims, LZ_EINVAL, "lz_search_create: num_simulations %d > tree capacity %d", num_simulations, t->max_sims);
-    LZ_REQUIRE(t->p.A == m->cfg.action_space_size, LZ_EINVAL, "lz_search_create: tree has %d actions, model %d", t->p.A, m->cfg.action_space_size);
-    const bool ez = model_is_ez(m);
+    LZ_REQUIRE(t->p.A == m->A, LZ_EINVAL, "lz_search_create: tree has %d actions, model %d", t->p.A, m->A);
+    const bool ez = m->vp;
     LZ_REQUIRE(ez == (t->p.ez != 0), LZ_EINVAL, "lz_search_create: %s model needs a tree in %s mode (lz_tree_set_ez)",
                ez ? "an EfficientZero" : "a MuZero", ez ? "EfficientZero" : "MuZero");
     lz_search *q = new lz_search();
@@ -260,7 +260,7 @@ int lz_search_create(lz_tree *t, lz_model *m, int num_simulations, lz_search **o
     if (rc == LZ_OK) rc = dev_alloc(&q->d_root_value, (size_t)q->B);
     if (rc == LZ_OK) rc = dev_alloc(&q->d_skip, q->slot_stride);
     if (rc == LZ_OK && ez) {
-        q->hslot_stride = (size_t)q->B * m->cfg.lstm_hidden_size;
+        q->hslot_stride = (size_t)q->B * m->lstm_hidden;
         rc = dev_alloc(&q->hpool, q->hslot_stride * (size_t)(q->S + 1));
         if (rc == LZ_OK) rc = dev_alloc(&q->cpool, q->hslot_stride * (size_t)(q->S + 1));
         if (rc == LZ_OK) rc = dev_alloc(&q->d_is_reset, (size_t)q->B);
@@ -365,10 +365,10 @@ static int collect_device(lz_search *q, const float *d_obs, const uint8_t *d_obs
     io.value = d_pred_value ? d_pred_value : q->d_root_value;
     int rc;
     if (d_obs_u8) {
-        LZ_REQUIRE(q->model->kind == 0, LZ_EINVAL, "lz_search_collect_u8: uint8 frames need the conv model");
+        LZ_REQUIRE(q->model->family == ModelFamily::Conv, LZ_EINVAL, "lz_search_collect_u8: uint8 frames need the conv model");
         if (!q->d_pre_stage && (rc = dev_alloc(&q->d_pre_stage, (size_t)q->B * q->model->latent_floats))) return rc;
-        rc = model_initial_tower(q->model, q->B, nullptr, q->d_pre_stage, (cudaStream_t)s, d_obs_u8);
-        if (rc == LZ_OK) rc = model_initial_tail(q->model, q->B, q->d_pre_stage, io, (cudaStream_t)s);
+        rc = conv_initial_tower(q->model, q->B, nullptr, q->d_pre_stage, (cudaStream_t)s, d_obs_u8);
+        if (rc == LZ_OK) rc = conv_initial_tail(q->model, q->B, q->d_pre_stage, io, (cudaStream_t)s);
     } else {
         rc = model_initial(q->model, q->B, d_obs, io, (cudaStream_t)s);          // policy/muzero.py:749
     }
@@ -393,16 +393,13 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
                         float *d_policy_logits, lz_stream s_)
 {
     LZ_REQUIRE(q && h_obs, LZ_EINVAL, "lz_search_collect_host: bad argument");
-    LZ_REQUIRE(!obs_u8 || q->model->kind == 0, LZ_EINVAL, "lz_search_collect_host_u8: uint8 frames need the conv model");
+    LZ_REQUIRE(!obs_u8 || q->model->family == ModelFamily::Conv, LZ_EINVAL, "lz_search_collect_host_u8: uint8 frames need the conv model");
     const size_t esz = obs_u8 ? 1 : sizeof(float);         // bytes per observation element on the wire and in the staging buffer
     cudaStream_t s = (cudaStream_t)s_;
-    const lz_model_config &c = q->model->cfg;
     const int B = q->B, A = q->A;
-    const size_t obs_elems = (q->model->kind == 1 || q->model->kind == 4) ? (size_t)q->model->mcfg.obs_dim
-                             : q->model->kind == 3 ? (size_t)q->model->ecfg.obs_dim : (size_t)c.obs_c * c.obs_h * c.obs_w;
     nchunks = nchunks < 1 ? 1 : (nchunks > 8 ? 8 : nchunks);
     if (!q->copy_stream) {
-        q->obs_elems = obs_elems;
+        q->obs_elems = q->model->obs_elems;
         LZ_CUDA_CHECK(cudaStreamCreateWithFlags(&q->copy_stream, cudaStreamNonBlocking));
         LZ_CUDA_CHECK(cudaStreamCreateWithFlags(&q->copy_stream2, cudaStreamNonBlocking));
         for (int i = 0; i < 8; ++i) LZ_CUDA_CHECK(cudaEventCreateWithFlags(&q->ev_chunk[i], cudaEventDisableTiming));
@@ -433,15 +430,15 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
     if (h_to_play) LZ_CUDA_CHECK(cudaMemcpyAsync(q->d_tp_stage, h_to_play, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     float *logits = d_policy_logits ? d_policy_logits : q->d_root_logits;
     float *pred = d_pred_value ? d_pred_value : q->d_root_value;
-    const bool split = q->model->kind == 0;   // tower per chunk, tail once
+    const bool split = q->model->family == ModelFamily::Conv;   // tower per chunk, tail once
     for (int i = 0; i < nchunks; ++i) {
         const int b0 = i * per, bc = std::min(per, B - b0);
         LZ_CUDA_CHECK(cudaStreamWaitEvent(s, q->ev_chunk[i], 0));
         int rc;
         if (split) {
             const unsigned char *stage = reinterpret_cast<const unsigned char *>(q->d_obs_stage) + (size_t)b0 * q->obs_elems * esz;
-            rc = model_initial_tower(q->model, bc, obs_u8 ? nullptr : reinterpret_cast<const float *>(stage),
-                                     q->d_pre_stage + (size_t)b0 * q->model->latent_floats, s, obs_u8 ? stage : nullptr);
+            rc = conv_initial_tower(q->model, bc, obs_u8 ? nullptr : reinterpret_cast<const float *>(stage),
+                                    q->d_pre_stage + (size_t)b0 * q->model->latent_floats, s, obs_u8 ? stage : nullptr);
         } else {
             TailIO io;
             memset(&io, 0, sizeof(io));
@@ -458,7 +455,7 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
         io.latent2 = q->pool;
         io.policy_logits = logits;
         io.value = pred;
-        int rc = model_initial_tail(q->model, B, q->d_pre_stage, io, s);
+        int rc = conv_initial_tail(q->model, B, q->d_pre_stage, io, s);
         if (rc) return rc;
     }
     return collect_search(q, h_mask ? q->d_mask_stage : nullptr, logits, h_noise ? q->d_noise_stage : nullptr, noise_weight,
@@ -488,7 +485,7 @@ int lz_search_debug_plan(const lz_search *q, int32_t *h_info)
     h_info[7] = q->tree->p.N;
     if (!persistent_search(q, false)) return LZ_OK;
     h_info[0] = 1;
-    tc_describe_search(q->model->tc_rec, persistent_io(q, 1), q->tree->p.N, h_info + 1);
+    tc_describe_search(q->model->conv.tc_rec, persistent_io(q, 1), q->tree->p.N, h_info + 1);
     return LZ_OK;
 }
 const float *lz_search_latent_pool(const lz_search *q) { return q ? q->pool : nullptr; }
