@@ -169,6 +169,14 @@ int lz_tree_backpropagate_gumbel(lz_tree *t, int latent_index, const float *d_re
  * completed Q by action id (-inf at illegal actions), d_improved_policy f32 [B,A] softmax(prior + completed Q) by action id.
  * Either may be NULL.  Visit counts, values and trajectories: lz_tree_results. */
 int lz_tree_gumbel_policies(lz_tree *t, float *d_children_values, float *d_improved_policy, lz_stream s);
+/* What GumbelMuZeroPolicy._forward_collect / _forward_eval (lzero/policy/gumbel_muzero.py:573-605, 685-700) take from the
+ * searched roots, in the one pass of lz_tree_gumbel_policies: d_action int32 [B] = np.argmax(np.where(action_mask,
+ * improved_policy, 0)) (the first maximum; the same in collect and eval), d_entropy f32 [B] = select_action's visit-count
+ * entropy at this temperature (the arithmetic of lz_tree_select_action; it does not depend on the draw), d_children_values
+ * f32 [B,A] = np.where(action_mask, completed Q, 0) (roots_completed_value), d_improved_policy f32 [B,A] as
+ * lz_tree_gumbel_policies.  Any output may be NULL. */
+int lz_tree_gumbel_select_action(lz_tree *t, float temperature, int32_t *d_action, float *d_entropy, float *d_children_values,
+                                 float *d_improved_policy, lz_stream s);
 /* Host only (no device needed): row min(m, S) of get_table_of_considered_visits(m, S) into h_seq int32 [S] and
  * generate_gumbel(10, 0, A) into h_gumbel f32 [A] (cnode.cpp:1041-1094, 1133-1151).  Either may be NULL. */
 int lz_gumbel_tables(int max_num_considered_actions, int num_simulations, int A, int32_t *h_seq, float *h_gumbel);
@@ -355,7 +363,11 @@ int lz_search_run_gumbel(lz_search *q, const float *d_latent_roots, lz_stream s)
 /* The search-feeding part of _forward_collect (policy/muzero.py:749-779): initial_inference ->
  * reset(mask) -> prepare(noise) -> search.  d_obs f32 [B,obs_c,H,W]; d_mask uint8 [B,A] or NULL;
  * d_noise f32 [B,A] legal-order rows or NULL; d_to_play int32 [B] or NULL (-1).
- * Optional outputs: d_pred_value f32 [B] (root value prediction), d_policy_logits f32 [B,A]. */
+ * Optional outputs: d_pred_value f32 [B] (root value prediction), d_policy_logits f32 [B,A].
+ * On a Gumbel tree (lz_tree_set_gumbel) lz_tree_prepare_gumbel prepares the roots with the root value prediction as their values
+ * (GumbelMuZeroPolicy._forward_collect, gumbel_muzero.py:560-571) and the search is the graph of lz_search_run_gumbel; the
+ * search's num_simulations may not exceed the tree's Gumbel num_simulations (LZ_EINVAL).  The same holds for the three
+ * entry points below.  Read the results with lz_tree_results and lz_tree_gumbel_select_action. */
 int lz_search_collect(lz_search *q, const float *d_obs, const uint8_t *d_mask, const float *d_noise,
                       float noise_weight, const int32_t *d_to_play, int deterministic,
                       float *d_pred_value, float *d_policy_logits, lz_stream s);
@@ -417,6 +429,13 @@ int lz_segments_store_search_stats(lz_segments *g, const int32_t *d_visits, cons
 int lz_segments_reset(lz_segments *g, const uint8_t *d_done, lz_stream s);
 /* Device pointers: child_visits f32 [B,T,A], root_values f32 [B,T], len int32 [B] (any may be NULL). */
 int lz_segments_data(lz_segments *g, float **d_child_visits, float **d_root_values, int32_t **d_len);
+/* The improved_policy argument of store_search_stats (Gumbel MuZero, game_segment.py:258-259): d_improved_policy f32 [B,A] by
+ * action id is stored at position len[b], the one the NEXT lz_segments_store_search_stats fills, with the same d_active and
+ * full-segment rule: call it first for the step.  The f32 [B,T,A] array is allocated (zeroed) by the first call; lz_segments_reset
+ * zeroes the rows of the segments it resets. */
+int lz_segments_store_improved_policy(lz_segments *g, const float *d_improved_policy, const uint8_t *d_active, lz_stream s);
+/* Device pointer of the improved-policy array f32 [B,T,A]; NULL before the first lz_segments_store_improved_policy. */
+int lz_segments_improved_policy(lz_segments *g, float **d_improved_policy);
 
 #ifdef __cplusplus
 }

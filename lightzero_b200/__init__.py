@@ -9,6 +9,8 @@ from .muzero_model import MuZeroModel, MZNetworkOutput  # noqa: F401
 from .muzero_model_mlp import MuZeroModelMLP  # noqa: F401
 from .scaling_transform import DiscreteSupport, InverseScalarTransform  # noqa: F401
 from . import ez_tree, gmz_tree, mz_tree  # noqa: F401
+from .collect import EfficientZeroCollectPolicy, GumbelMuZeroCollectPolicy, MuZeroCollectPolicy  # noqa: F401
 
 __all__ = ["MuZeroMCTSCtree", "EfficientZeroMCTSCtree", "GumbelMuZeroMCTSCtree", "gmz_tree", "UniZeroMCTSCtree", "EfficientZeroModel", "EfficientZeroModelMLP", "EZNetworkOutput", "ez_tree", "MuZeroModel", "MuZeroModelMLP", "MZNetworkOutput", "DiscreteSupport",
-           "InverseScalarTransform", "mz_tree"]
+           "InverseScalarTransform", "mz_tree", "MuZeroCollectPolicy", "EfficientZeroCollectPolicy",
+           "GumbelMuZeroCollectPolicy"]

@@ -67,6 +67,7 @@ SIGNATURES = {
     "lz_tree_traverse_gumbel": (c_int, [c_void_p] * 7),
     "lz_tree_backpropagate_gumbel": (c_int, [c_void_p, c_int] + [c_void_p] * 5),
     "lz_tree_gumbel_policies": (c_int, [c_void_p] * 4),
+    "lz_tree_gumbel_select_action": (c_int, [c_void_p, c_float] + [c_void_p] * 5),
     "lz_gumbel_tables": (c_int, [c_int, c_int, c_int, c_void_p, c_void_p]),
     "lz_model_create": (c_int, [ctypes.POINTER(ModelConfig), ctypes.POINTER(c_void_p)]),
     "lz_model_create_mlp": (c_int, [ctypes.POINTER(MlpConfig), ctypes.POINTER(c_void_p)]),
@@ -118,6 +119,8 @@ SIGNATURES = {
     "lz_segments_store_search_stats": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lz_segments_reset": (c_int, [c_void_p, c_void_p, c_void_p]),
     "lz_segments_data": (c_int, [c_void_p, ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p)]),
+    "lz_segments_store_improved_policy": (c_int, [c_void_p] * 4),
+    "lz_segments_improved_policy": (c_int, [c_void_p, ctypes.POINTER(c_void_p)]),
     "lz_search_hidden_pool": (c_void_p, [c_void_p, c_int]),
 }
 

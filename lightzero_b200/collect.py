@@ -16,8 +16,9 @@ import torch
 from . import cabi, mz_tree
 from .efficientzero_model import EfficientZeroModel
 from .efficientzero_model_mlp import EfficientZeroModelMLP
-from .mcts_ctree import EfficientZeroMCTSCtree, MuZeroMCTSCtree
+from .mcts_ctree import EfficientZeroMCTSCtree, GumbelMuZeroMCTSCtree, MuZeroMCTSCtree
 from .muzero_model import MuZeroModel
+from .muzero_model_mlp import MuZeroModelMLP
 
 
 def select_action(visit_counts: np.ndarray, temperature: float = 1, deterministic: bool = True):
@@ -66,7 +67,8 @@ class MuZeroCollectPolicy:
         """obs [B,C,H,W] (host or device), action_mask [B,A] 0/1, noises [B,A] rows in legal order or None
         (eval).  Returns dict of tensors; with read_back=True they are pinned host tensors and the call
         ends with the single stream synchronisation of the step.  select=(temperature, deterministic_action, seed) also
-        runs select_action (policy/utils.py:637-661) on the device and returns 'action' / 'entropy'."""
+        runs select_action (policy/utils.py:637-661) on the device and returns 'action' / 'entropy' (GumbelMuZeroCollectPolicy: the
+        Gumbel read-out, which adds 'improved_policy' / 'completed_values' [B, A])."""
         B = obs.shape[0]
         A = self.model.action_space_size
         S = int(self.cfg.num_simulations)
@@ -106,8 +108,7 @@ class MuZeroCollectPolicy:
             tree = mz_tree.acquire_tree(dev, B, A, S)
             try:
                 tree.set_params(*self.mcts._params())
-                cabi.check(tree.lib.lz_tree_set_ez(tree.h, *self._tree_mode), "lz_tree_set_ez")
-                q = tree.search_for(self.model, S, self._tree_mode if self._tree_mode[0] else ())
+                q = self._search_for(tree, S)
                 s = cabi.stream_ptr()
                 if host_path:
                     fn = tree.lib.lz_search_collect_host_u8 if u8 else tree.lib.lz_search_collect_host
@@ -124,32 +125,40 @@ class MuZeroCollectPolicy:
                 cabi.check(tree.lib.lz_tree_results(tree.h, tree.visits.data_ptr(), tree.values.data_ptr(),
                                                     tree.nlegal.data_ptr(), None, s), "lz_tree_results")
                 self.last_num_kernels = tree.lib.lz_search_num_kernels(q)
-                if select is not None:
-                    cabi.check(tree.lib.lz_tree_select_action(tree.h, float(select[0]), int(bool(select[1])), int(select[2]) & (2 ** 64 - 1),
-                                                              bufs["action"].data_ptr(), bufs["action_pos"].data_ptr(),
-                                                              bufs["entropy"].data_ptr(), s), "lz_tree_select_action")
+                selected = self._select(tree, bufs, select, s) if select is not None else ()
                 if not read_back:
                     dev_out = dict(visits=tree.visits.clone(), values=tree.values.clone(), nlegal=tree.nlegal.clone(),
                                    pred_value=bufs["pred_value"], policy_logits=bufs["logits"])
-                    if select is not None:      # the device-side select_action results stay on the device too
-                        dev_out.update(action=bufs["action"].clone(), entropy=bufs["entropy"].clone())
+                    # the device-side select_action results stay on the device too
+                    dev_out.update({k: bufs[k].clone() for k in selected})
                     return dev_out
                 bufs["h_visits"].copy_(tree.visits, non_blocking=True)
                 bufs["h_values"].copy_(tree.values, non_blocking=True)
                 bufs["h_nlegal"].copy_(tree.nlegal, non_blocking=True)
                 bufs["h_pred"].copy_(bufs["pred_value"], non_blocking=True)
                 bufs["h_logits"].copy_(bufs["logits"], non_blocking=True)
-                if select is not None:
-                    bufs["h_action"].copy_(bufs["action"], non_blocking=True)
-                    bufs["h_entropy"].copy_(bufs["entropy"], non_blocking=True)
+                for k in selected:
+                    bufs["h_" + k].copy_(bufs[k], non_blocking=True)
                 torch.cuda.current_stream().synchronize()
             finally:
                 tree.busy = False
         out = dict(visits=bufs["h_visits"], values=bufs["h_values"], nlegal=bufs["h_nlegal"],
                    pred_value=bufs["h_pred"], policy_logits=bufs["h_logits"])
-        if select is not None:
-            out.update(action=bufs["h_action"], entropy=bufs["h_entropy"])
+        out.update({k: bufs["h_" + k] for k in selected})
         return out
+
+    def _search_for(self, tree, S):
+        """Puts the pooled tree in this policy's mode and returns its lz_search for the model."""
+        cabi.check(tree.lib.lz_tree_set_gumbel(tree.h, 0, 0), "lz_tree_set_gumbel")    # a tree a Gumbel collect left behind
+        cabi.check(tree.lib.lz_tree_set_ez(tree.h, *self._tree_mode), "lz_tree_set_ez")
+        return tree.search_for(self.model, S, self._tree_mode if self._tree_mode[0] else ())
+
+    def _select(self, tree, bufs, select, s):
+        """select_action on the device into bufs; returns the names of the tensors it wrote."""
+        cabi.check(tree.lib.lz_tree_select_action(tree.h, float(select[0]), int(bool(select[1])), int(select[2]) & (2 ** 64 - 1),
+                                                  bufs["action"].data_ptr(), bufs["action_pos"].data_ptr(),
+                                                  bufs["entropy"].data_ptr(), s), "lz_tree_select_action")
+        return ("action", "entropy")
 
     # ---- reference-shaped API --------------------------------------------------------------------
     def forward_collect(self, data: torch.Tensor, action_mask, temperature: float = 1, to_play=(-1,),
@@ -214,3 +223,86 @@ class EfficientZeroCollectPolicy(MuZeroCollectPolicy):
         self.mcts = EfficientZeroMCTSCtree(cfg or {})
         self.cfg = self.mcts._cfg
         self._tree_mode = (1, int(self.cfg.lstm_horizon_len))
+
+
+class GumbelMuZeroCollectPolicy(MuZeroCollectPolicy):
+    """The same for ``GumbelMuZeroPolicy._forward_collect`` / ``_forward_eval`` (lzero/policy/gumbel_muzero.py:498-720) with a
+    ``MuZeroModel`` (conv or board) or ``MuZeroModelMLP``: the pooled tree is a Gumbel tree (``max_num_considered_actions``,
+    default 4 as the reference policy's config, and ``num_simulations``), the roots are prepared with the initial inference's
+    value, and one device read-out gives per root the improved policy, the masked completed Q, the action (the first maximum
+    of the improved policy over the legal actions, in collect and eval alike) and select_action's visit-count entropy.  Output
+    dicts have the reference's keys."""
+
+    def __init__(self, model: Union[MuZeroModel, MuZeroModelMLP], cfg: Optional[dict] = None):
+        if isinstance(model, (EfficientZeroModel, EfficientZeroModelMLP)):
+            raise TypeError(f"GumbelMuZeroCollectPolicy: the Gumbel search runs MuZero models, not an {type(model).__name__}")
+        super().__init__(model, cfg)
+        self.mcts = GumbelMuZeroMCTSCtree(cfg or {})
+        self.cfg = self.mcts._cfg
+        self.cfg.setdefault("max_num_considered_actions", 4)
+
+    def _bufs(self, B, A):
+        bufs = super()._bufs(B, A)
+        if "improved_policy" not in bufs:
+            for k in ("improved_policy", "completed_values"):
+                bufs[k] = torch.empty(B, A, device=self.device)
+                bufs["h_" + k] = torch.empty(B, A).pin_memory()
+        return bufs
+
+    def _search_for(self, tree, S):
+        cabi.check(tree.lib.lz_tree_set_ez(tree.h, 0, 5), "lz_tree_set_ez")
+        cabi.check(tree.lib.lz_tree_set_gumbel(tree.h, int(self.cfg.max_num_considered_actions), S), "lz_tree_set_gumbel")
+        return tree.search_for(self.model, S, ("gumbel",))
+
+    def _select(self, tree, bufs, select, s):
+        """lz_tree_gumbel_select_action at temperature select[0]: the action never depends on a draw."""
+        cabi.check(tree.lib.lz_tree_gumbel_select_action(tree.h, float(select[0]), bufs["action"].data_ptr(), bufs["entropy"].data_ptr(),
+                                                         bufs["completed_values"].data_ptr(), bufs["improved_policy"].data_ptr(), s),
+                   "lz_tree_gumbel_select_action")
+        return ("action", "entropy", "improved_policy", "completed_values")
+
+    def forward_collect(self, data: torch.Tensor, action_mask, temperature: float = 1, to_play=(-1,),
+                        epsilon: float = 0.25, ready_env_id=None, **kwargs) -> Dict[int, dict]:
+        """gumbel_muzero.py:498-607: Dirichlet noise in legal order drawn with np.random as the reference does."""
+        B = data.shape[0]
+        action_mask = np.asarray(action_mask)
+        alpha = float(self.cfg.root_dirichlet_alpha)
+        noises = np.zeros((B, action_mask.shape[1]), np.float32)
+        for j in range(B):                                   # gumbel_muzero.py:555-558
+            n = int(action_mask[j].sum())
+            noises[j, :n] = np.random.dirichlet([alpha] * n).astype(np.float32)
+        r = self.search_batch(data, action_mask, noises, self._to_play(to_play, B), select=(temperature, False, 0))
+        return self._format_gumbel(r, B, ready_env_id, collect=True)
+
+    def forward_eval(self, data: torch.Tensor, action_mask, to_play=(-1,), ready_env_id=None, **kwargs) -> Dict[int, dict]:
+        """gumbel_muzero.py:619-720: no noise, entropy at temperature 1."""
+        B = data.shape[0]
+        r = self.search_batch(data, np.asarray(action_mask), None, self._to_play(to_play, B), select=(1.0, True, 0))
+        return self._format_gumbel(r, B, ready_env_id, collect=False)
+
+    @staticmethod
+    def _to_play(to_play, B):
+        return np.broadcast_to(np.asarray(to_play, np.int32).reshape(-1), (B,)) if np.size(to_play) in (1, B) else to_play
+
+    def _format_gumbel(self, r, B, ready_env_id, collect) -> Dict[int, dict]:
+        if ready_env_id is None:
+            ready_env_id = np.arange(B)
+        visits, nl = r["visits"].numpy(), r["nlegal"].numpy()
+        values, pred, logits = r["values"].numpy(), r["pred_value"].numpy(), r["policy_logits"].numpy()
+        action, ent = r["action"].numpy(), r["entropy"].numpy()
+        improved, completed = r["improved_policy"].numpy(), r["completed_values"].numpy()
+        output = {}
+        for i, env_id in enumerate(ready_env_id):
+            out = {
+                'action': np.int64(action[i]),
+                'visit_count_distributions': visits[i, :nl[i]].tolist(),
+                'visit_count_distribution_entropy': float(ent[i]),
+                'searched_value': float(values[i]),
+            }
+            if collect:
+                out['roots_completed_value'] = completed[i].astype(np.float64)
+                out['improved_policy_probs'] = improved[i].astype(np.float64)
+            out['predicted_value'] = float(pred[i])
+            out['predicted_policy_logits'] = logits[i].tolist()
+            output[env_id] = out
+        return output

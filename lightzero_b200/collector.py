@@ -5,7 +5,7 @@ environment over PCIe and nothing comes back except the chosen actions.
 * ``FrameStack``     -- ``GameSegment.get_obs()`` / ``append()`` / the ``frame_stack_num`` seeding (game_segment.py:140-181,
                         muzero_collector.py:451-457): [B, stack, H, W] uint8 on the device, oldest frame first;
 * ``SegmentStats``   -- ``GameSegment.store_search_stats`` / ``reset`` (game_segment.py:241-263, 340-362): child-visit distributions
-                        and root values appended per step for B segments of capacity T;
+                        and root values (and Gumbel MuZero's improved policies) appended per step for B segments of capacity T;
 * ``gather_segments``-- the all-gather of finished segments across ranks (one NCCL ``all_gather_into_tensor`` of a packed buffer).
 
 All compute is in ``csrc/collector.cu`` behind the C ABI (include/lzb200.h); there is no CPU fallback.
@@ -94,13 +94,18 @@ class SegmentStats:
             cabi.check(self._lib.lz_segments_create(self.B, self.T, self.A, ctypes.byref(h)), "lz_segments_create")
         self._h = h
 
-    def store_search_stats(self, visit_counts: torch.Tensor, root_values: torch.Tensor, active=None) -> None:
+    def store_search_stats(self, visit_counts: torch.Tensor, root_values: torch.Tensor, active=None, improved_policy=None) -> None:
         """game_segment.py:241-263 for every (active) environment: ``visit_counts`` int32 [B, A] (-1 beyond the legal list, as
-        ``lz_tree_results`` / ``Roots`` deliver them on the device), ``root_values`` f32 [B]."""
+        ``lz_tree_results`` / ``Roots`` deliver them on the device), ``root_values`` f32 [B], and for Gumbel MuZero
+        ``improved_policy`` f32 [B, A] by action id (``GumbelMuZeroCollectPolicy.search_batch``'s ``improved_policy``)."""
         v = visit_counts.to(self.device, torch.int32).contiguous()
         r = root_values.to(self.device, torch.float32).contiguous()
         a = None if active is None else torch.as_tensor(active).to(self.device, torch.uint8).contiguous()
         with torch.cuda.device(self.device):
+            if improved_policy is not None:      # stored at the position store_search_stats is about to fill
+                ip = improved_policy.to(self.device, torch.float32).contiguous()
+                cabi.check(self._lib.lz_segments_store_improved_policy(self._h, ip.data_ptr(), cabi.ptr(a), cabi.stream_ptr()),
+                           "lz_segments_store_improved_policy")
             cabi.check(self._lib.lz_segments_store_search_stats(self._h, v.data_ptr(), r.data_ptr(), cabi.ptr(a), cabi.stream_ptr()),
                        "lz_segments_store_search_stats")
 
@@ -117,6 +122,15 @@ class SegmentStats:
         with torch.cuda.device(self.device):
             outs = [_view(ptr.value, shape, ts, self.device).clone() for ptr, (shape, ts) in zip(p, shapes)]
         return tuple(outs)
+
+    def improved_policy(self):
+        """A copy of the improved policies f32 [B, T, A] stored so far (0 where none was), or None before the first one."""
+        p = ctypes.c_void_p()
+        cabi.check(self._lib.lz_segments_improved_policy(self._h, ctypes.byref(p)), "lz_segments_improved_policy")
+        if not p.value:
+            return None
+        with torch.cuda.device(self.device):
+            return _view(p.value, (self.B, self.T, self.A), "<f4", self.device).clone()
 
     def __del__(self):
         try:

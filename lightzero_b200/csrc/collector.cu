@@ -5,6 +5,8 @@
 // HBM-bound byte moves: each kernel touches every byte once with 16-byte accesses.
 #include <string.h>
 
+#include <algorithm>
+
 #include "lz_common.cuh"
 
 struct lz_frames {
@@ -20,6 +22,7 @@ struct lz_segments {
     float *child_visits;            // [B][T][A]  visit_count / sum(visit_counts) per position of the root's legal list, 0 beyond it
     float *root_values;             // [B][T]
     int32_t *len;                   // [B] entries stored so far (<= T)
+    float *improved_policy;         // [B][T][A] Gumbel MuZero improved policy by action id; allocated by the first store
 };
 
 namespace lz {
@@ -61,6 +64,26 @@ __global__ void __launch_bounds__(128) k_segments_store(const int32_t *__restric
         root_values[(size_t)b * T + t] = values[b];
         len[b] = t + 1;
     }
+}
+
+// GameSegment.store_search_stats(..., improved_policy=...) (game_segment.py:258-259): the improved policy goes in at the position
+// len that k_segments_store then fills and advances past, under the same full-segment rule
+__global__ void __launch_bounds__(128) k_segments_store_policy(const float *__restrict__ policy, const uint8_t *__restrict__ active,
+                                                               float *improved_policy, const int32_t *len, int B, int T, int A)
+{
+    const int b = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (b >= B || (active && !active[b])) return;
+    const int t = len[b];
+    if (t >= T) return;
+    for (int a = lane; a < A; a += 32) improved_policy[((size_t)b * T + t) * A + a] = policy[(size_t)b * A + a];
+}
+
+// zeroes the `row` floats of every done segment b (all of them when done is null)
+__global__ void k_segments_clear_rows(float *x, const uint8_t *__restrict__ done, int B, size_t row)
+{
+    const size_t n = (size_t)B * row;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        if (!done || done[i / row]) x[i] = 0.0f;
 }
 
 __global__ void k_segments_reset(int32_t *len, const uint8_t *__restrict__ done, int B)
@@ -144,7 +167,7 @@ int lz_segments_create(int B, int T, int A, lz_segments **out)
 int lz_segments_destroy(lz_segments *g)
 {
     if (!g) return LZ_OK;
-    cudaFree(g->child_visits); cudaFree(g->root_values); cudaFree(g->len);
+    cudaFree(g->child_visits); cudaFree(g->root_values); cudaFree(g->len); cudaFree(g->improved_policy);
     delete g;
     return LZ_OK;
 }
@@ -163,6 +186,27 @@ int lz_segments_reset(lz_segments *g, const uint8_t *d_done, lz_stream s)
     LZ_REQUIRE(g, LZ_EINVAL, "lz_segments_reset: null argument");
     k_segments_reset<<<ceil_div(g->B, 256), 256, 0, (cudaStream_t)s>>>(g->len, d_done, g->B);
     LZ_KERNEL_CHECK();
+    if (g->improved_policy) {
+        const size_t n = (size_t)g->B * g->T * g->A;
+        const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)kNumSMs * 8);
+        k_segments_clear_rows<<<blocks, 256, 0, (cudaStream_t)s>>>(g->improved_policy, d_done, g->B, (size_t)g->T * g->A);
+        LZ_KERNEL_CHECK();
+    }
+    return LZ_OK;
+}
+
+int lz_segments_store_improved_policy(lz_segments *g, const float *d_improved_policy, const uint8_t *d_active, lz_stream s)
+{
+    LZ_REQUIRE(g && d_improved_policy, LZ_EINVAL, "lz_segments_store_improved_policy: null argument");
+    if (!g->improved_policy) {
+        const size_t n = (size_t)g->B * g->T * g->A;
+        int rc = dev_alloc(&g->improved_policy, n);
+        if (rc != LZ_OK) return rc;
+        LZ_CUDA_CHECK(cudaMemsetAsync(g->improved_policy, 0, n * sizeof(float), (cudaStream_t)s));
+    }
+    k_segments_store_policy<<<ceil_div(g->B, 4), 128, 0, (cudaStream_t)s>>>(d_improved_policy, d_active, g->improved_policy, g->len,
+                                                                           g->B, g->T, g->A);
+    LZ_KERNEL_CHECK();
     return LZ_OK;
 }
 
@@ -172,6 +216,13 @@ int lz_segments_data(lz_segments *g, float **d_child_visits, float **d_root_valu
     if (d_child_visits) *d_child_visits = g->child_visits;
     if (d_root_values) *d_root_values = g->root_values;
     if (d_len) *d_len = g->len;
+    return LZ_OK;
+}
+
+int lz_segments_improved_policy(lz_segments *g, float **d_improved_policy)
+{
+    LZ_REQUIRE(g && d_improved_policy, LZ_EINVAL, "lz_segments_improved_policy: null argument");
+    *d_improved_policy = g->improved_policy;
     return LZ_OK;
 }
 

@@ -294,10 +294,23 @@ k_gumbel_step(TreeParams p, GumbelParams g, TreeStep a)
     }
 }
 
-// get_children_values / get_policies (cnode.cpp:309-385, 506-541): completed Q at the legal positions (-inf elsewhere) and
-// csoftmax over all A entries of prior + completed Q (-inf at illegal positions, which come out as 0).
+// Outputs of one read-out of the roots; every pointer may be null.
+struct GumbelReadout {
+    float *children_values;   // [B][A] completed Q by action id, cv_fill at illegal actions
+    float cv_fill;            // -inf for get_children_values, 0 for the policy's np.where(action_mask, completed_q, 0)
+    float *policy;            // [B][A] improved policy by action id
+    int32_t *action;          // [B] np.argmax(np.where(action_mask, improved_policy, 0)): the first maximum
+    float *entropy;           // [B] select_action's visit-count entropy in bits
+    double inv_temperature;   // of the entropy
+};
+
+// get_children_values / get_policies (cnode.cpp:309-385, 506-541): completed Q at the legal positions (cv_fill elsewhere) and
+// csoftmax over all A entries of prior + completed Q (-inf at illegal positions, which come out as 0); then what
+// GumbelMuZeroPolicy._forward_collect / _forward_eval (lzero/policy/gumbel_muzero.py:573-605, 685-700) derive from them: the
+// action of the largest improved-policy entry over the legal actions (the illegal entries are 0, as np.where makes them) and
+// select_action's entropy of the visit counts.
 __global__ void __launch_bounds__(kGumbelBlock)
-k_gumbel_policies(TreeParams p, GumbelParams g, float *children_values, float *policy)
+k_gumbel_readout(TreeParams p, GumbelParams g, GumbelReadout o)
 {
     const int b = blockIdx.x * (kGumbelBlock / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (b >= p.B) return;
@@ -306,17 +319,22 @@ k_gumbel_policies(TreeParams p, GumbelParams g, float *children_values, float *p
     const int *lg = p.legal + (size_t)b * A;
     const int n = p.nlegal[b];
     const NodeQ s = node_q(nb, A, n, lg, g.raw_value[(size_t)b * N], p.discount, lane);
-    float *cv = children_values ? children_values + (size_t)b * A : nullptr;
-    float *pol = policy ? policy + (size_t)b * A : nullptr;
+    float *cv = o.children_values ? o.children_values + (size_t)b * A : nullptr;
+    float *pol = o.policy ? o.policy + (size_t)b * A : nullptr;
     if (cv) {
-        for (int a = lane; a < A; a += 32) cv[a] = -INFINITY;
+        for (int a = lane; a < A; a += 32) cv[a] = o.cv_fill;
         __syncwarp();
         for (int k = lane; k < n; k += 32) {
             const int a = lg[k], vis = (int)nb[F_VISIT * A + a];
             cv[a] = completed_q(vis, vis > 0 ? child_q(nb, A, a, p.discount) : 0.0f, s);
         }
     }
-    if (!pol) return;
+    if (o.entropy) {
+        double total;
+        const double ent = root_visit_entropy(nb, lg, A, n, o.inv_temperature, lane, &total);
+        if (lane == 0) o.entropy[b] = (float)(ent / 0.69314718055994530942);    // as k_tree_select_action
+    }
+    if (!pol && !o.action) return;
     // probs[a] by action id: the legal position of a is found by a scan of the legal list (lane-parallel, A <= a few hundred)
     auto logit = [&](int a) -> float {
         for (int k = 0; k < n; ++k)
@@ -338,7 +356,26 @@ k_gumbel_policies(TreeParams p, GumbelParams g, float *children_values, float *p
         seq_sum(a < A ? lz_expf_exact(__fsub_rn(logit(a), m)) : 0.0f, a < A, sum);
     }
     const float lsum = lz_logf_exact(sum);
-    for (int a = lane; a < A; a += 32) pol[a] = lz_expf_exact(__fsub_rn(__fsub_rn(logit(a), m), lsum));
+    float best = -1.0f;
+    int best_a = 0;
+    for (int c0 = 0; c0 < A; c0 += 32) {
+        const int a = c0 + lane;
+        const float pr = a < A ? lz_expf_exact(__fsub_rn(__fsub_rn(logit(a), m), lsum)) : -1.0f;
+        if (pol && a < A) pol[a] = pr;
+        const float cmax = warp_max_exact(pr);
+        if (cmax > best) {
+            best = cmax;
+            best_a = c0 + __ffs(__ballot_sync(0xffffffffu, a < A && pr == cmax)) - 1;
+        }
+    }
+    if (o.action && lane == 0) o.action[b] = best_a;
+}
+
+static int gumbel_readout(lz_tree *t, const GumbelReadout &o, cudaStream_t s)
+{
+    k_gumbel_readout<<<gumbel_grid(t->p.B), kGumbelBlock, 0, s>>>(t->p, t->gumbel->g, o);
+    LZ_KERNEL_CHECK();
+    return LZ_OK;
 }
 
 int gumbel_launch_step(lz_tree *t, const TreeStep &a, cudaStream_t s)
@@ -494,9 +531,21 @@ int lz_tree_gumbel_policies(lz_tree *t, float *d_children_values, float *d_impro
 {
     LZ_REQUIRE(t && t->gumbel, LZ_ESTATE, "lz_tree_gumbel_policies: not a Gumbel tree (lz_tree_set_gumbel)");
     LZ_REQUIRE(t->gumbel->prepared, LZ_ESTATE, "lz_tree_gumbel_policies: roots not prepared (call lz_tree_prepare_gumbel first)");
-    k_gumbel_policies<<<gumbel_grid(t->p.B), kGumbelBlock, 0, (cudaStream_t)s>>>(t->p, t->gumbel->g, d_children_values, d_improved_policy);
-    LZ_KERNEL_CHECK();
-    return LZ_OK;
+    GumbelReadout o = {};
+    o.children_values = d_children_values; o.cv_fill = -INFINITY; o.policy = d_improved_policy;
+    return gumbel_readout(t, o, (cudaStream_t)s);
+}
+
+int lz_tree_gumbel_select_action(lz_tree *t, float temperature, int32_t *d_action, float *d_entropy, float *d_children_values,
+                                 float *d_improved_policy, lz_stream s)
+{
+    LZ_REQUIRE(t && t->gumbel, LZ_ESTATE, "lz_tree_gumbel_select_action: not a Gumbel tree (lz_tree_set_gumbel)");
+    LZ_REQUIRE(t->gumbel->prepared, LZ_ESTATE, "lz_tree_gumbel_select_action: roots not prepared (call lz_tree_prepare_gumbel first)");
+    LZ_REQUIRE(temperature > 0.0f, LZ_EINVAL, "lz_tree_gumbel_select_action: temperature must be > 0");
+    GumbelReadout o = {};
+    o.children_values = d_children_values; o.cv_fill = 0.0f; o.policy = d_improved_policy;
+    o.action = d_action; o.entropy = d_entropy; o.inv_temperature = 1.0 / (double)temperature;
+    return gumbel_readout(t, o, (cudaStream_t)s);
 }
 
 }  // extern "C"

@@ -220,13 +220,31 @@ static int run_with_reuse(lz_search *q, const float *d_latent_roots, const int32
     return LZ_OK;
 }
 
-// lz_search_collect*: reset the roots to the legal mask, prepare them from the initial inference's logits (+ noise), then search
-static int collect_search(lz_search *q, const uint8_t *d_mask, const float *d_logits, const float *d_noise, float noise_weight,
-                          const int32_t *d_to_play, int deterministic, cudaStream_t s)
+// Checked before the initial inference: a Gumbel search may not take more simulations than its considered-visit table has
+static int collect_check(const lz_search *q)
+{
+    const lz_gumbel *gs = q->tree->gumbel;
+    LZ_REQUIRE(!gs || q->S <= gs->g.S, LZ_EINVAL,
+               "lz_search_collect: %d simulations past the considered-visit table of the Gumbel tree's num_simulations = %d",
+               q->S, gs ? gs->g.S : 0);
+    return LZ_OK;
+}
+
+// lz_search_collect*: reset the roots to the legal mask, prepare them from the initial inference's logits (+ noise), then search.
+// A Gumbel tree also takes the initial inference's root values d_values (GumbelMuZeroPolicy._forward_collect,
+// lzero/policy/gumbel_muzero.py:560-571) and runs the Gumbel search graph.
+static int collect_search(lz_search *q, const uint8_t *d_mask, const float *d_logits, const float *d_values, const float *d_noise,
+                          float noise_weight, const int32_t *d_to_play, int deterministic, cudaStream_t s)
 {
     int rc;
-    LZ_REQUIRE(!q->tree->gumbel, LZ_ESTATE, "lz_search_collect: Gumbel tree (the collect entry points run MuZero / EfficientZero searches)");
     if ((rc = lz_tree_reset_mask(q->tree, d_mask, s))) return rc;                // policy/muzero.py:760,769
+    if (lz_gumbel *gs = q->tree->gumbel) {
+        if ((rc = lz_tree_prepare_gumbel(q->tree, d_logits, d_noise, noise_weight, nullptr, d_values, d_to_play, s))) return rc;
+        if ((rc = run_graph(q, 1, false, s))) return rc;
+        gs->traversals = q->S;
+        gs->pending = false;
+        return LZ_OK;
+    }
     if ((rc = lz_tree_prepare(q->tree, d_logits, d_noise, noise_weight, nullptr, d_to_play, s))) return rc;   // :774
     if (q->hpool) {      // EfficientZero: zero LSTM state at the roots; the tree has no deterministic argument, the collect call's flag selects its tie-breaking
         if ((rc = ez_root_hidden(q, nullptr, nullptr, s))) return rc;
@@ -358,12 +376,13 @@ static int collect_device(lz_search *q, const float *d_obs, const uint8_t *d_obs
                           float *d_policy_logits, lz_stream s)
 {
     LZ_REQUIRE(q && (d_obs || d_obs_u8), LZ_EINVAL, "lz_search_collect: bad argument");
+    int rc = collect_check(q);
+    if (rc) return rc;
     TailIO io;
     memset(&io, 0, sizeof(io));
     io.latent2 = q->pool;                                   // latent roots go straight into pool slot 0
     io.policy_logits = d_policy_logits ? d_policy_logits : q->d_root_logits;
     io.value = d_pred_value ? d_pred_value : q->d_root_value;
-    int rc;
     if (d_obs_u8) {
         LZ_REQUIRE(q->model->family == ModelFamily::Conv, LZ_EINVAL, "lz_search_collect_u8: uint8 frames need the conv model");
         if (!q->d_pre_stage && (rc = dev_alloc(&q->d_pre_stage, (size_t)q->B * q->model->latent_floats))) return rc;
@@ -373,7 +392,7 @@ static int collect_device(lz_search *q, const float *d_obs, const uint8_t *d_obs
         rc = model_initial(q->model, q->B, d_obs, io, (cudaStream_t)s);          // policy/muzero.py:749
     }
     if (rc) return rc;
-    return collect_search(q, d_mask, io.policy_logits, d_noise, noise_weight, d_to_play, deterministic, (cudaStream_t)s);
+    return collect_search(q, d_mask, io.policy_logits, io.value, d_noise, noise_weight, d_to_play, deterministic, (cudaStream_t)s);
 }
 
 int lz_search_collect(lz_search *q, const float *d_obs, const uint8_t *d_mask, const float *d_noise, float noise_weight,
@@ -394,6 +413,7 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
 {
     LZ_REQUIRE(q && h_obs, LZ_EINVAL, "lz_search_collect_host: bad argument");
     LZ_REQUIRE(!obs_u8 || q->model->family == ModelFamily::Conv, LZ_EINVAL, "lz_search_collect_host_u8: uint8 frames need the conv model");
+    if (int rc = collect_check(q)) return rc;
     const size_t esz = obs_u8 ? 1 : sizeof(float);         // bytes per observation element on the wire and in the staging buffer
     cudaStream_t s = (cudaStream_t)s_;
     const int B = q->B, A = q->A;
@@ -458,7 +478,7 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
         int rc = conv_initial_tail(q->model, B, q->d_pre_stage, io, s);
         if (rc) return rc;
     }
-    return collect_search(q, h_mask ? q->d_mask_stage : nullptr, logits, h_noise ? q->d_noise_stage : nullptr, noise_weight,
+    return collect_search(q, h_mask ? q->d_mask_stage : nullptr, logits, pred, h_noise ? q->d_noise_stage : nullptr, noise_weight,
                           h_to_play ? q->d_tp_stage : nullptr, deterministic, s);
 }
 

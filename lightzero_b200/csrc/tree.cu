@@ -180,17 +180,8 @@ k_tree_select_action(TreeParams p, double inv_temperature, int deterministic, un
     const int A = p.A, n = p.nlegal[b];
     const uint32_t *nb = p.edges + (size_t)b * p.N * kEdgeFields * A;      // root block
     const int *lg = p.legal + (size_t)b * A;
-    double total = 0.0;
-    for (int k = lane; k < n; k += 32) total += pow((double)(int)nb[F_VISIT * A + lg[k]], inv_temperature);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
-    double ent = 0.0;
-    for (int k = lane; k < n; k += 32) {
-        const double pr = pow((double)(int)nb[F_VISIT * A + lg[k]], inv_temperature) / total;
-        if (pr > 0.0) ent -= pr * log(pr);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) ent += __shfl_xor_sync(0xffffffffu, ent, o);
+    double total;
+    const double ent = root_visit_entropy(nb, lg, A, n, inv_temperature, lane, &total);
     if (lane == 0) {
         int pos = 0;
         if (deterministic) {

@@ -66,6 +66,27 @@ __device__ __forceinline__ float warp_max_exact(float v)
     return v;
 }
 
+// select_action's fp64 arithmetic (lzero/policy/utils.py:637-661) on the n root visit counts of node block nb, legal list lg:
+// returns the natural-log entropy -sum p ln p of p = visit ** inv_temperature / total on every lane, and total in *total.
+// Shared by lz_tree_select_action and the Gumbel read-out, both compiled with -fmad=false, so the two give the same bits.
+__device__ __forceinline__ double root_visit_entropy(const uint32_t *nb, const int *lg, int A, int n, double inv_temperature,
+                                                     int lane, double *total_out)
+{
+    double total = 0.0;
+    for (int k = lane; k < n; k += 32) total += pow((double)(int)nb[F_VISIT * A + lg[k]], inv_temperature);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
+    double ent = 0.0;
+    for (int k = lane; k < n; k += 32) {
+        const double pr = pow((double)(int)nb[F_VISIT * A + lg[k]], inv_temperature) / total;
+        if (pr > 0.0) ent -= pr * log(pr);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) ent += __shfl_xor_sync(0xffffffffu, ent, o);
+    *total_out = total;
+    return ent;
+}
+
 __device__ __forceinline__ unsigned long long mix64(unsigned long long z)
 {
     z += 0x9e3779b97f4a7c15ull;

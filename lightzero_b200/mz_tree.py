@@ -266,6 +266,7 @@ class Roots:
         s = None
         with torch.cuda.device(self.device):
             s = cabi.stream_ptr()
+            cabi.check(t.lib.lz_tree_set_gumbel(t.h, 0, 0), "lz_tree_set_gumbel")    # a pooled tree a Gumbel collect left behind
             cabi.check(t.lib.lz_tree_set_ez(t.h, int(self._ez), int(self._lstm_horizon)), "lz_tree_set_ez")
             self._reset_tree(t, s)
             cabi.check(t.lib.lz_tree_prepare(t.h, p["logits"].data_ptr(), cabi.ptr(p["noise"]), p["w"],
