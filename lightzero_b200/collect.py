@@ -141,7 +141,7 @@ class MuZeroCollectPolicy:
                     bufs["h_" + k].copy_(bufs[k], non_blocking=True)
                 torch.cuda.current_stream().synchronize()
             finally:
-                tree.busy = False
+                tree.release()         # the search and the clones above may still be queued: the next holder waits for them
         out = dict(visits=bufs["h_visits"], values=bufs["h_values"], nlegal=bufs["h_nlegal"],
                    pred_value=bufs["h_pred"], policy_logits=bufs["h_logits"])
         out.update({k: bufs["h_" + k] for k in selected})

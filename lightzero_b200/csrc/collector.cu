@@ -110,8 +110,8 @@ int lz_frames_create(int B, int stack, int H, int W, lz_frames **out)
     if (rc == LZ_OK) rc = dev_alloc(&f->buf[1], n);
     if (rc == LZ_OK) rc = dev_alloc(&f->d_new, (size_t)B * f->frame_bytes);
     if (rc == LZ_OK) rc = dev_alloc(&f->d_reset, (size_t)B);
+    if (rc == LZ_OK) rc = setup_memset(f->buf[0], n);
     if (rc != LZ_OK) { lz_frames_destroy(f); return rc; }
-    cudaMemset(f->buf[0], 0, n);
     *out = f;
     return LZ_OK;
 }
@@ -156,10 +156,10 @@ int lz_segments_create(int B, int T, int A, lz_segments **out)
     int rc = dev_alloc(&g->child_visits, (size_t)B * T * A);
     if (rc == LZ_OK) rc = dev_alloc(&g->root_values, (size_t)B * T);
     if (rc == LZ_OK) rc = dev_alloc(&g->len, (size_t)B);
+    if (rc == LZ_OK) rc = setup_memset(g->child_visits, (size_t)B * T * A * sizeof(float));
+    if (rc == LZ_OK) rc = setup_memset(g->root_values, (size_t)B * T * sizeof(float));
+    if (rc == LZ_OK) rc = setup_memset(g->len, (size_t)B * sizeof(int32_t));
     if (rc != LZ_OK) { lz_segments_destroy(g); return rc; }
-    cudaMemset(g->child_visits, 0, (size_t)B * T * A * sizeof(float));
-    cudaMemset(g->root_values, 0, (size_t)B * T * sizeof(float));
-    cudaMemset(g->len, 0, (size_t)B * sizeof(int32_t));
     *out = g;
     return LZ_OK;
 }

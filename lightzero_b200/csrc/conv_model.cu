@@ -208,7 +208,7 @@ int conv_reserve_skip(lz_model *m, int B)
 {
     if (B <= m->conv.tc_skip_B) return LZ_OK;
     ++m->generation;
-    cudaFree(m->conv.tc_skip);
+    dev_free(m->conv.tc_skip);
     m->conv.tc_skip = nullptr; m->conv.tc_skip_B = 0;
     int rc = dev_alloc(&m->conv.tc_skip, (size_t)m->latent_floats * B);
     if (rc != LZ_OK) return rc;
@@ -216,8 +216,8 @@ int conv_reserve_skip(lz_model *m, int B)
     return LZ_OK;
 }
 
-// the skip scratch, and the DownSample tower's workspace of initial inference
-int conv_reserve(lz_model *m, int B)
+// the skip scratch, and the DownSample tower's workspace of initial inference (zeroed on s)
+int conv_reserve(lz_model *m, int B, cudaStream_t s)
 {
     {
         int rc = conv_reserve_skip(m, B);
@@ -225,7 +225,7 @@ int conv_reserve(lz_model *m, int B)
     }
     if (B <= m->conv.ws_B) return LZ_OK;
     ++m->generation;
-    cudaFree(m->conv.pre_latent);
+    dev_free(m->conv.pre_latent);
     m->conv.pre_latent = nullptr;
     {
         int rc = dev_alloc(&m->conv.pre_latent, (size_t)m->latent_floats * B);
@@ -238,11 +238,11 @@ int conv_reserve(lz_model *m, int B)
         const size_t bT = tcl_bytes(B, c2, h1, h1, 1), bT2 = tcl_bytes(B, c2, h1 / 2, h1 / 2, 4);
         const size_t bU = tcl_bytes(B, kC, h2, h2, 1), bV = tcl_bytes(B, kC, h3, h3, 1);
         const size_t total = bT + bT2 + 3 * bU + 2 * bV;
-        cudaFree(m->conv.tws);
+        dev_free(m->conv.tws);
         m->conv.tws = nullptr;
         int rc = dev_alloc(&m->conv.tws, total);
         if (rc != LZ_OK) return rc;
-        LZ_CUDA_CHECK(cudaMemset(m->conv.tws, 0, total));
+        LZ_CUDA_CHECK(cudaMemsetAsync(m->conv.tws, 0, total, s));
         unsigned char *q = m->conv.tws;
         m->conv.T0 = make_tcl(q, c2, h1, h1, 1); q += bT;
         m->conv.T1 = make_tcl(q, c2, h1 / 2, h1 / 2, 4); q += bT2;
@@ -707,7 +707,7 @@ int conv_debug_stage(lz_model *m, int which, int B, const float *d_latent, const
     const int nfeat = ez ? m->ez.net.nin : 0;
     LZ_REQUIRE(stage <= nl, LZ_EINVAL, "lz_model_debug_net_stage: stage %d past the %d layers of the program", stage, nl);
     {
-        int rc = model_reserve(m, B);
+        int rc = model_reserve(m, B, st);
         if (rc != LZ_OK) return rc;
     }
     const size_t nfl = stage < nl ? (size_t)B * m->latent_floats : (size_t)B * (2 * K + 2 * A + 4 + nfeat);
@@ -771,7 +771,7 @@ int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uin
                "lz_model_debug_tower_stage: bad argument");
     LZ_REQUIRE(m->finalized && m->family == ModelFamily::Conv, LZ_ESTATE, "lz_model_debug_tower_stage: not a finalized conv model with a tensor-core tower");
     if (B > m->conv.ws_B) {
-        int rc = model_reserve(m, B);
+        int rc = model_reserve(m, B, (cudaStream_t)s);
         if (rc != LZ_OK) return rc;
     }
     LZ_REQUIRE(B <= m->conv.ws_B, LZ_ESTATE, "lz_model_debug_tower_stage: workspace sized for %d roots, got %d", m->conv.ws_B, B);

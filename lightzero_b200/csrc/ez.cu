@@ -396,7 +396,7 @@ int ez_finalize(lz_model *m, int nin, int hid, bool vp_norm)
         for (int j = 0; j < hid; ++j) fc2[(size_t)j * K + k] = (*W3)[(size_t)k * hid + j];
     EzHead &z = m->ez;
     float scale = 1.0f;
-    cudaFree(z.d_wtc);
+    dev_free(z.d_wtc);
     z.d_wtc = nullptr;
     if (ez_tc_shape(nin, H)) {   // tensor-core copy of the LSTM weights (fp16 hi / lo, power-of-two scaled); other shapes (e.g. 8
                                  // reward-head channels: nin = 288) run the fp32 k_ez_lstm
@@ -427,7 +427,7 @@ int ez_reserve(lz_model *m, int B)
     EzHead &z = m->ez;
     if (B <= z.B) return LZ_OK;
     ++m->generation;
-    cudaFree(z.feat); cudaFree(z.htmp);
+    dev_free(z.feat); dev_free(z.htmp);
     z.feat = z.htmp = nullptr;
     int rc = dev_alloc(&z.feat, (size_t)B * z.net.nin);
     if (rc == LZ_OK) rc = dev_alloc(&z.htmp, (size_t)B * m->lstm_hidden);

@@ -385,12 +385,16 @@ int gumbel_launch_step(lz_tree *t, const TreeStep &a, cudaStream_t s)
     return LZ_OK;
 }
 
+// frees the Gumbel state, attached and idle (cudaFree: waits for all work on the device)
 void gumbel_free(lz_tree *t)
 {
-    if (!t || !t->gumbel) return;
-    cudaFree(t->gumbel->alloc);
-    delete t->gumbel;
-    t->gumbel = nullptr;
+    if (!t) return;
+    for (lz_gumbel **g : {&t->gumbel, &t->gumbel_idle}) {
+        if (!*g) continue;
+        cudaFree((*g)->alloc);
+        delete *g;
+        *g = nullptr;
+    }
 }
 
 // get_sequence_of_considered_visits (cnode.cpp:1041-1076) for row min(m, S) of get_table_of_considered_visits, and
@@ -442,8 +446,12 @@ int lz_gumbel_tables(int max_num_considered_actions, int num_simulations, int A,
 int lz_tree_set_gumbel(lz_tree *t, int max_num_considered_actions, int num_simulations)
 {
     LZ_REQUIRE(t, LZ_EINVAL, "lz_tree_set_gumbel: null tree");
-    if (num_simulations == 0) {                 // back to a MuZero tree
-        if (t->gumbel) { gumbel_free(t); ++t->generation; }
+    if (num_simulations == 0) {                 // back to a MuZero tree: the Gumbel state stays allocated, idle, so that switching
+        if (t->gumbel) {                        // a pooled tree back and forth frees nothing (a cudaFree waits for the whole device)
+            t->gumbel_idle = t->gumbel;
+            t->gumbel = nullptr;
+            ++t->generation;
+        }
         return LZ_OK;
     }
     LZ_REQUIRE(!t->p.ez, LZ_ESTATE, "lz_tree_set_gumbel: tree is in EfficientZero mode (the Gumbel tree is a MuZero tree)");
@@ -451,6 +459,16 @@ int lz_tree_set_gumbel(lz_tree *t, int max_num_considered_actions, int num_simul
                "lz_tree_set_gumbel: bad arguments max_num_considered_actions=%d num_simulations=%d",
                max_num_considered_actions, num_simulations);
     if (t->gumbel && t->gumbel->g.m == max_num_considered_actions && t->gumbel->g.S == num_simulations) return LZ_OK;
+    if (lz_gumbel *idle = t->gumbel_idle) {     // the same tables as when it was detached: attach it again, nothing to write
+        if (!t->gumbel && idle->g.m == max_num_considered_actions && idle->g.S == num_simulations) {
+            t->gumbel = idle;
+            t->gumbel_idle = nullptr;
+            idle->prepared = idle->pending = false;
+            idle->traversals = 0;
+            ++t->generation;
+            return LZ_OK;
+        }
+    }
     const int A = t->p.A, S = num_simulations;
     std::vector<int> seq(S);
     std::vector<float> gum(A);
@@ -470,9 +488,9 @@ int lz_tree_set_gumbel(lz_tree *t, int max_num_considered_actions, int num_simul
     gs->g.gumbel = (const float *)(base + o_gum);
     gs->g.considered = (const int *)(base + o_seq);
     gs->g.raw_value = (float *)(base + o_raw);
-    LZ_CUDA_CHECK(cudaMemset(base, 0, words * 4));
-    LZ_CUDA_CHECK(cudaMemcpy(base + o_gum, gum.data(), A * sizeof(float), cudaMemcpyHostToDevice));
-    LZ_CUDA_CHECK(cudaMemcpy(base + o_seq, seq.data(), S * sizeof(int), cudaMemcpyHostToDevice));
+    if ((rc = setup_memset(base, words * 4)) != LZ_OK) return rc;
+    if ((rc = setup_upload(base + o_gum, gum.data(), A * sizeof(float))) != LZ_OK) return rc;
+    if ((rc = setup_upload(base + o_seq, seq.data(), S * sizeof(int))) != LZ_OK) return rc;
     ++t->generation;                             // captured search graphs bake GumbelParams in
     return LZ_OK;
 }

@@ -47,6 +47,20 @@ inline int dev_alloc(T **p, size_t n)
     return LZ_OK;
 }
 
+// cudaFree of a live buffer waits for all work on the device; a null pointer skips the call
+inline void dev_free(void *p)
+{
+    if (p) cudaFree(p);
+}
+
+// Device writes of the setup entry points (create, set_params, set_gumbel, finalize): they go on a library-owned non-blocking
+// stream of the current device and are complete when the call returns, so they never queue behind work on the legacy default
+// stream (a learner's backward pass, say) and a caller's stream may use what they wrote right away.  Defined in tree.cu.
+int setup_memset(void *d, size_t bytes);                    // zeroes d[0, bytes)
+int setup_upload(void *d, const void *h, size_t bytes);     // copies host bytes to the device
+int setup_stream(cudaStream_t *s);                          // the stream itself: enqueue on it, then setup_sync
+int setup_sync();
+
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
 constexpr int kNumSMs = 132;       // streaming multiprocessors of the H100 SXM the grid sizes are tuned for

@@ -112,9 +112,9 @@ int model_initial(lz_model *m, int B, const float *d_obs, const TailIO &io, cuda
 }
 
 // the Board and MLP networks have no workspace; the value-prefix head has its LSTM scratch
-int model_reserve(lz_model *m, int B)
+int model_reserve(lz_model *m, int B, cudaStream_t s)
 {
-    int rc = m->family == ModelFamily::Conv ? conv_reserve(m, B) : LZ_OK;
+    int rc = m->family == ModelFamily::Conv ? conv_reserve(m, B, s) : LZ_OK;
     if (rc == LZ_OK && m->vp) rc = ez_reserve(m, B);
     return rc;
 }
@@ -280,7 +280,7 @@ int lz_model_initial_inference(lz_model *m, int B, const float *d_obs, float *d_
 {
     LZ_REQUIRE(m && d_obs && B > 0, LZ_EINVAL, "lz_model_initial_inference: bad argument");
     LZ_REQUIRE(m->finalized, LZ_ESTATE, "lz_model_initial_inference: model not finalized");
-    int rc = model_reserve(m, B);
+    int rc = model_reserve(m, B, (cudaStream_t)s);
     if (rc != LZ_OK) return rc;
     TailIO io;
     memset(&io, 0, sizeof(io));
@@ -329,7 +329,7 @@ int lz_model_recurrent_inference_ez(lz_model *m, int B, const float *d_latent, c
 {
     LZ_REQUIRE(m && d_latent && d_hidden0 && d_hidden1 && d_action && d_next_latent && B > 0, LZ_EINVAL, "lz_model_recurrent_inference_ez: bad argument");
     LZ_REQUIRE(m->finalized && m->vp, LZ_ESTATE, "lz_model_recurrent_inference_ez: not a finalized EfficientZero model");
-    int rc = model_reserve(m, B);
+    int rc = model_reserve(m, B, (cudaStream_t)s);
     if (rc != LZ_OK) return rc;
     RecIO io;
     memset(&io, 0, sizeof(io));

@@ -177,16 +177,16 @@ inline void split_hi_lo(float v, __half &hi, __half &lo)
     lo = __float2half_rn(v - __half2float(hi));
 }
 
-// replaces the device table *dst with a copy of `bytes` host bytes
+// replaces the device table *dst with a copy of `bytes` host bytes, complete on return (setup_upload).  Freeing a table that
+// already exists (a weight reload) waits for all work on the device, so no search in flight still reads it.
 template <typename T>
 int upload(T **dst, const void *src, size_t bytes)
 {
-    cudaFree(*dst);
+    dev_free(*dst);
     *dst = nullptr;
     int rc = dev_alloc(reinterpret_cast<unsigned char **>(dst), bytes);
     if (rc != LZ_OK) return rc;
-    LZ_CUDA_CHECK(cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice));
-    return LZ_OK;
+    return setup_upload(*dst, src, bytes);
 }
 
 // the create functions' common checks: the support size K = len(torch.arange(min, max, step)) in [2, kmax], and a CUDA device
@@ -195,13 +195,15 @@ int check_create(const char *fn, float support_min, float support_max, float sup
 // ---- the families behind the entry points ----
 int model_recurrent(lz_model *m, const RecIO &io, cudaStream_t s);
 int model_initial(lz_model *m, int B, const float *d_obs, const TailIO &io, cudaStream_t s);
-int model_reserve(lz_model *m, int B);   // sizes the scratch of launches outside a search (synchronous, outside capture)
+// sizes the scratch of launches outside a search, outside capture; a growth frees the old scratch (waits for the whole device)
+// and zeroes what must start zeroed on `s`
+int model_reserve(lz_model *m, int B, cudaStream_t s);
 // lz_model_debug_net_stage of each family: `which` 0 is the recurrent program on the latents d_in and actions d_action, 1 the
 // initial_inference program on the observations d_in
 
 // Conv (conv_model.cu)
 int conv_finalize(lz_model *m);
-int conv_reserve(lz_model *m, int B);
+int conv_reserve(lz_model *m, int B, cudaStream_t s);
 int conv_reserve_skip(lz_model *m, int B);   // the skip scratch alone (lz_model_recurrent_inference)
 int conv_recurrent(lz_model *m, const RecIO &io, cudaStream_t s);
 int conv_initial(lz_model *m, int B, const float *d_obs, const TailIO &io, cudaStream_t s);

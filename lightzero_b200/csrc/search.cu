@@ -283,7 +283,12 @@ int lz_search_create(lz_tree *t, lz_model *m, int num_simulations, lz_search **o
         if (rc == LZ_OK) rc = dev_alloc(&q->cpool, q->hslot_stride * (size_t)(q->S + 1));
         if (rc == LZ_OK) rc = dev_alloc(&q->d_is_reset, (size_t)q->B);
     }
-    if (rc == LZ_OK) rc = model_reserve(m, q->B);
+    if (rc == LZ_OK) {      // no stream here: the model's scratch is grown on the setup stream and complete on return
+        cudaStream_t ss;
+        rc = setup_stream(&ss);
+        if (rc == LZ_OK) rc = model_reserve(m, q->B, ss);
+        if (rc == LZ_OK) rc = setup_sync();
+    }
     if (rc != LZ_OK) { lz_search_destroy(q); return rc; }
     *out = q;
     return LZ_OK;

@@ -5,6 +5,7 @@
 
 #include <atomic>
 #include <limits.h>
+#include <mutex>
 #include <vector>
 
 #include "lz_common.cuh"
@@ -23,6 +24,46 @@ void set_error(const char *fmt, ...)
     va_start(ap, fmt);
     vsnprintf(g_err, sizeof(g_err), fmt, ap);
     va_end(ap);
+}
+
+// the setup stream of each device (lz_common.cuh), created on first use and kept for the life of the process
+int setup_stream(cudaStream_t *s)
+{
+    static std::mutex mu;
+    static cudaStream_t streams[64];
+    int dev = 0;
+    LZ_CUDA_CHECK(cudaGetDevice(&dev));
+    LZ_REQUIRE(dev >= 0 && dev < 64, LZ_ECUDA, "setup stream: device ordinal %d out of range", dev);
+    std::lock_guard<std::mutex> lock(mu);
+    if (!streams[dev]) LZ_CUDA_CHECK(cudaStreamCreateWithFlags(&streams[dev], cudaStreamNonBlocking));
+    *s = streams[dev];
+    return LZ_OK;
+}
+
+int setup_sync()
+{
+    cudaStream_t s;
+    if (int rc = setup_stream(&s)) return rc;
+    LZ_CUDA_CHECK(cudaStreamSynchronize(s));
+    return LZ_OK;
+}
+
+int setup_memset(void *d, size_t bytes)
+{
+    cudaStream_t s;
+    if (int rc = setup_stream(&s)) return rc;
+    LZ_CUDA_CHECK(cudaMemsetAsync(d, 0, bytes, s));
+    LZ_CUDA_CHECK(cudaStreamSynchronize(s));
+    return LZ_OK;
+}
+
+int setup_upload(void *d, const void *h, size_t bytes)
+{
+    cudaStream_t s;
+    if (int rc = setup_stream(&s)) return rc;
+    LZ_CUDA_CHECK(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, s));
+    LZ_CUDA_CHECK(cudaStreamSynchronize(s));
+    return LZ_OK;
 }
 
 constexpr int kTreeBlock = 64;   // 2 warps = 2 trees per CTA: latency-bound work, spread over all SMs
@@ -260,8 +301,7 @@ int lz_tree_create(int B, int A, int max_sims, lz_tree **out)
     uint32_t *base = nullptr;
     int rc = dev_alloc(&base, words);
     if (rc != LZ_OK) { delete t; return rc; }
-    cudaError_t e = cudaMemset(base, 0, words * 4);
-    if (e != cudaSuccess) { set_error("cudaMemset failed: %s", cudaGetErrorString(e)); cudaFree(base); delete t; return LZ_ECUDA; }
+    if ((rc = setup_memset(base, words * 4)) != LZ_OK) { cudaFree(base); delete t; return rc; }
     t->alloc_base = base;
     p.edges = base + o_edges;
     p.n_to_play = (int *)(base + o_ntp); p.n_best = (int *)(base + o_nbest); p.n_reset = (int *)(base + o_nreset);
@@ -306,7 +346,7 @@ int lz_tree_set_params(lz_tree *t, int pb_c_base, float pb_c_init, float discoun
         volatile float lg = logf(arg);
         tab[i] = lg + pb_c_init;
     }
-    LZ_CUDA_CHECK(cudaMemcpy(t->d_pbc, tab.data(), n * sizeof(float), cudaMemcpyHostToDevice));
+    if (int rc = setup_upload(t->d_pbc, tab.data(), n * sizeof(float))) return rc;
     if (t->p.discount != discount || t->p.delta != value_delta_max) ++t->generation;   // passed BY VALUE into captured search graphs
     t->p.discount = discount;
     t->p.delta = value_delta_max;

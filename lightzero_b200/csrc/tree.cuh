@@ -463,6 +463,7 @@ struct lz_tree {
     unsigned long long generation;   // bumped whenever TreeParams values that captured graphs bake in change (set_params / set_ez)
     void *alloc_base;
     struct lz_gumbel *gumbel;        // Gumbel MuZero mode (gumbel.cu; nullptr: MuZero / EfficientZero)
+    struct lz_gumbel *gumbel_idle;   // the Gumbel state of a tree switched back to MuZero, kept until destroy or the next switch
 };
 
 namespace lz {

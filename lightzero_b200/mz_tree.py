@@ -35,6 +35,7 @@ class TreeHandle:
         self.h = h
         self.busy = False
         self.params = None
+        self._released = None  # CUDA event recorded where the last holder let go: its searches / read-outs may still be queued
         i32 = dict(dtype=torch.int32, device=device)
         self.ix, self.iy, self.action = (torch.empty(B, **i32) for _ in range(3))
         self.search_len, self.vtp = torch.empty(B, **i32), torch.empty(B, **i32)
@@ -47,9 +48,25 @@ class TreeHandle:
     def set_params(self, pb_c_base, pb_c_init, discount, delta):
         p = (int(pb_c_base), float(pb_c_init), float(discount), float(delta))
         if p != self.params:
+            # lz_tree_set_params rewrites the pb_c table on the library's setup stream, which no caller stream is ordered
+            # against: first wait, on the host, for every search that may still read it -- the earlier holders' (the release
+            # event) and this holder's own queued work (the current stream)
             with torch.cuda.device(self.device):
+                if self._released is not None:
+                    self._released.synchronize()
+                torch.cuda.current_stream(self.device).synchronize()
                 cabi.check(self.lib.lz_tree_set_params(self.h, *p), "lz_tree_set_params")
             self.params = p
+
+    def release(self):
+        """Hands the tree back to the pool.  The holder's work on it may still be queued on the current stream (a
+        search_batch(read_back=False), Roots.clear() before the read-outs ran): the event recorded here orders the next
+        holder after it (acquire_tree, set_params)."""
+        with torch.cuda.device(self.device):
+            if self._released is None:
+                self._released = torch.cuda.Event()
+            self._released.record(torch.cuda.current_stream(self.device))
+        self.busy = False
 
     def search_for(self, model, num_simulations, mode=()):
         # keyed by the model's serial (unique for the life of the process; id() is recycled after garbage collection).  The
@@ -73,11 +90,15 @@ class TreeHandle:
 
 
 def acquire_tree(device, B, A, max_sims) -> TreeHandle:
+    """A free pooled tree of this shape, or a new one.  The current stream waits for the work the last holder queued on it
+    (TreeHandle.release), so two holders on two streams never use one tree, its searches or its scratch at the same time."""
     key = (device.index, B, A, max_sims)
     with _pool_lock:
         for h in _tree_pool.setdefault(key, []):
             if not h.busy:
                 h.busy = True
+                if h._released is not None:
+                    torch.cuda.current_stream(device).wait_event(h._released)
                 return h
         h = TreeHandle(device, B, A, max_sims)
         h.busy = True
@@ -183,7 +204,7 @@ class Roots:
 
     def clear(self):
         if self._tree is not None:
-            self._tree.busy = False
+            self._tree.release()
             self._tree = None
 
     @property

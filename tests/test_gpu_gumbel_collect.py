@@ -348,7 +348,7 @@ def test_refusals():
         assert rc == -1 and b"considered-visit table" in lib.lz_last_error()
         cabi.check(lib.lz_tree_set_gumbel(tree.h, 0, 0), "lz_tree_set_gumbel off")
     finally:
-        tree.busy = False
+        tree.release()
     # uint8 frames stay the conv model's: board and MLP models refuse them on Gumbel trees too
     for name in ("tictactoe", "cartpole"):
         cu, shape = _model(name, 1)
