@@ -389,6 +389,37 @@ int lz_search_collect_u8(lz_search *q, const uint8_t *d_obs_u8, const uint8_t *d
 int lz_search_collect_host_u8(lz_search *q, const uint8_t *h_obs_u8, const uint8_t *h_mask, const float *h_noise,
                               float noise_weight, const int32_t *h_to_play, int deterministic, int nchunks,
                               float *d_pred_value, float *d_policy_logits, lz_stream s);
+/* ---- ReZero policy reanalyze (ReZeroMZGameBuffer._compute_target_policy_reanalyzed, lzero/mcts/buffer/game_buffer_rezero_mz.py:194-404;
+ * ReZeroEZGameBuffer, game_buffer_rezero_ez.py:126-330; SURVEY 8(f) row f-4) ----
+ * The whole sweep over N sampled segments of L positions, for a search q created for N roots (B = N).  Every [N*L] input is in the
+ * reference's flat order, row i = segment * L + position:
+ *   d_obs f32 [N*L, obs...] (initial_inference runs over all rows in mini_infer_size slices), or instead d_latent f32 [N*L, latent]
+ *   and d_logits f32 [N*L, A] of a prior initial_inference (d_obs NULL);
+ *   d_mask uint8 [N*L, A] (legal actions; an all-zero row is every action), d_to_play int32 [N*L] or NULL (-1),
+ *   d_true_action int32 [N*L] (the reference's -2 for a segment's last step and for padding), d_policy_mask uint8 [N*L],
+ *   d_noise f32 [N*L, A] in legal order or NULL (reanalyze_noise = False), noise_weight.
+ * The searches run backward from position L - 1: a plain search (MuZero: ties by `deterministic`; EfficientZero: first maximum),
+ * then, with reuse_search, L - 1 search_with_reuse calls each reusing the root values of the position searched before it (ties:
+ * first maximum, the reference's rand() == 0); without reuse_search L plain searches.  Outputs:
+ *   d_targets f64 [N, L, A]: visit / sum(visits) by legal position (scatter_legal = 0, fixed_action_space) or by action id
+ *   (scatter_legal != 0), zeros where policy_mask == 0; d_root_values f32 [N, L]; d_child_visits f64 [N, L, A]: visit / sum in
+ *   legal order, zero padded (what the buffer stores back); d_infer_count int32 [L - 1, S] (reuse_search, L > 1; else may be NULL):
+ *   per reuse search and simulation, how many trees needed the network.
+ * Everything is enqueued on s with no host synchronisation: initial_inference, then L x [handoff kernel, the search's captured
+ * graph, targets kernel].  The graphs are those of lz_search_run / *_with_reuse, captured once and replayed along the sweep.
+ * Sets the tree's tie-break rule to first maximum (lz_tree_set_tiebreak). */
+int lz_rezero_reanalyze(lz_search *q, int L, int reuse_search, int mini_infer_size, const float *d_obs, const float *d_latent,
+                        const float *d_logits, const uint8_t *d_mask, const int32_t *d_to_play, const int32_t *d_true_action,
+                        const uint8_t *d_policy_mask, const float *d_noise, float noise_weight, int deterministic, int scatter_legal,
+                        double *d_targets, float *d_root_values, double *d_child_visits, int32_t *d_infer_count, lz_stream s);
+/* The same for an EfficientZero search (the LSTM state at every root is zero, as initial_inference returns it). */
+int lz_rezero_reanalyze_ez(lz_search *q, int L, int reuse_search, int mini_infer_size, const float *d_obs, const float *d_latent,
+                           const float *d_logits, const uint8_t *d_mask, const int32_t *d_to_play, const int32_t *d_true_action,
+                           const uint8_t *d_policy_mask, const float *d_noise, float noise_weight, int scatter_legal,
+                           double *d_targets, float *d_root_values, double *d_child_visits, int32_t *d_infer_count, lz_stream s);
+/* Test hook: search graphs this library has captured since load (a capture happens on a search's first run and after a change of
+ * the model, the tree parameters or the tie rule). */
+unsigned long long lz_debug_graph_captures(void);
 /* Number of kernel nodes of the search graph this search launched last (any lz_search_run* / lz_search_collect* call). */
 int lz_search_num_kernels(const lz_search *q);
 /* Test hook: the launch plan of lz_search_run, host only.  h_info int32[8]: 1 if the search is one persistent launch of the

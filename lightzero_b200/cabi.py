@@ -122,6 +122,9 @@ SIGNATURES = {
     "lz_segments_store_improved_policy": (c_int, [c_void_p] * 4),
     "lz_segments_improved_policy": (c_int, [c_void_p, ctypes.POINTER(c_void_p)]),
     "lz_search_hidden_pool": (c_void_p, [c_void_p, c_int]),
+    "lz_rezero_reanalyze": (c_int, [c_void_p, c_int, c_int, c_int] + [c_void_p] * 8 + [c_float, c_int, c_int] + [c_void_p] * 5),
+    "lz_rezero_reanalyze_ez": (c_int, [c_void_p, c_int, c_int, c_int] + [c_void_p] * 8 + [c_float, c_int] + [c_void_p] * 5),
+    "lz_debug_graph_captures": (ctypes.c_uint64, []),
 }
 
 

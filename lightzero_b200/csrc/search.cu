@@ -7,49 +7,10 @@
 #include <string.h>
 
 #include <algorithm>
+#include <atomic>
 
 #include "gumbel.cuh"
-#include "model.cuh"
-#include "tree.cuh"
-
-struct SearchGraph {              // one instantiated search graph and what it baked in
-    cudaGraphExec_t exec;
-    unsigned long long gen_model, gen_tree;   // model / tree generation at capture
-    int num_kernels;              // kernel nodes
-};
-
-struct lz_search {
-    lz_tree *tree;
-    lz_model *model;
-    int S, B, A;
-    float *pool;                 // [(S+1)][B][C*P] latent pool, slot-major, NCHW per root
-    size_t slot_stride;          // B*C*P floats
-    int32_t *d_ix, *d_action;    // [B]
-    float *d_reward, *d_value;   // [B]
-    float *d_policy;             // [B][A]
-    float *d_root_logits;        // [B][A]
-    float *d_root_value;         // [B]
-    float *d_skip;               // [B][C*P] ResBlock skip scratch of the tensor-core network kernel (per search: searches may overlap on streams)
-    // EfficientZero: LSTM state pools [(S+1)][B][H] (tuple element 0 / 1 of reward_hidden_state, mcts_ctree.py:775-776)
-    // and the per-leaf is_reset flags handed from the traverse to the LSTM kernel and the back-up (:856-861)
-    float *hpool, *cpool;
-    size_t hslot_stride;
-    int32_t *d_is_reset;
-    // ReZero search_with_reuse: library-owned copies of the caller's per-root true action / reuse value (graph-stable addresses)
-    int32_t *d_true_action;
-    float *d_reuse_value;
-    SearchGraph graphs[4];       // plain search with deterministic 0 / 1, search with reuse, Gumbel search
-    cudaStream_t capture_stream; // library-owned: the caller's stream may be the legacy default stream,
-                                 // which cannot be captured; the instantiated graph launches on the caller's
-    int num_kernels;             // kernel nodes of the graph launched last
-    // host-buffer collect: staging + copy stream so the H2D of chunk i+1 overlaps the tower of chunk i
-    cudaStream_t copy_stream, copy_stream2;   // chunks alternate between two copy streams (two DMA engines)
-    cudaEvent_t ev_chunk[8], ev_start;
-    float *d_obs_stage, *d_noise_stage, *d_pre_stage;
-    uint8_t *d_mask_stage;
-    int32_t *d_tp_stage;
-    size_t obs_elems;            // floats per observation
-};
+#include "search.cuh"
 
 using namespace lz;
 
@@ -150,7 +111,9 @@ static int enqueue_search(lz_search *q, int deterministic, bool reuse, cudaStrea
     return LZ_OK;
 }
 
-static int run_graph(lz_search *q, int deterministic, bool reuse, cudaStream_t s)
+static std::atomic<unsigned long long> g_captures{0};   // lz_debug_graph_captures
+
+int lz::search_run_graph(lz_search *q, int deterministic, bool reuse, cudaStream_t s)
 {
     // an EfficientZero plain search breaks ties by p.tie_first (tracked by the tree generation), not by the flag: one graph
     SearchGraph &g = q->graphs[q->tree->gumbel ? 3 : reuse ? 2 : (deterministic || q->hpool) ? 1 : 0];
@@ -162,6 +125,7 @@ static int run_graph(lz_search *q, int deterministic, bool reuse, cudaStream_t s
         g.exec = nullptr;
     }
     if (!g.exec) {
+        g_captures.fetch_add(1, std::memory_order_relaxed);
         g.gen_model = q->model->generation;
         g.gen_tree = q->tree->generation;
         cudaGraph_t graph = nullptr;
@@ -201,20 +165,24 @@ static int ez_root_hidden(lz_search *q, const float *d_hidden0, const float *d_h
     return LZ_OK;
 }
 
+int lz::search_reuse_buffers(lz_search *q)
+{
+    if (q->d_true_action) return LZ_OK;
+    int rc = dev_alloc(&q->d_true_action, (size_t)q->B);
+    if (rc == LZ_OK) rc = dev_alloc(&q->d_reuse_value, (size_t)q->B);
+    return rc;
+}
+
 static int run_with_reuse(lz_search *q, const float *d_latent_roots, const int32_t *d_true_action, const float *d_reuse_value,
                           int32_t *d_infer_count, cudaStream_t s)
 {
-    if (!q->d_true_action) {
-        int rc = dev_alloc(&q->d_true_action, (size_t)q->B);
-        if (rc == LZ_OK) rc = dev_alloc(&q->d_reuse_value, (size_t)q->B);
-        if (rc != LZ_OK) return rc;
-    }
-    int rc = copy_latent_roots(q, d_latent_roots, s);
+    int rc = search_reuse_buffers(q);
+    if (rc == LZ_OK) rc = copy_latent_roots(q, d_latent_roots, s);
     if (rc) return rc;
     LZ_CUDA_CHECK(cudaMemcpyAsync(q->d_true_action, d_true_action, (size_t)q->B * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
     LZ_CUDA_CHECK(cudaMemcpyAsync(q->d_reuse_value, d_reuse_value, (size_t)q->B * sizeof(float), cudaMemcpyDeviceToDevice, s));
     LZ_CUDA_CHECK(cudaMemsetAsync(q->tree->p.infer_count, 0, (size_t)q->tree->p.N * sizeof(int), s));
-    if ((rc = run_graph(q, 0, true, s))) return rc;
+    if ((rc = search_run_graph(q, 0, true, s))) return rc;
     if (d_infer_count)      // per simulation: how many trees needed the network (mcts_ctree.py:433,466-467)
         LZ_CUDA_CHECK(cudaMemcpyAsync(d_infer_count, q->tree->p.infer_count, (size_t)q->S * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
     return LZ_OK;
@@ -240,7 +208,7 @@ static int collect_search(lz_search *q, const uint8_t *d_mask, const float *d_lo
     if ((rc = lz_tree_reset_mask(q->tree, d_mask, s))) return rc;                // policy/muzero.py:760,769
     if (lz_gumbel *gs = q->tree->gumbel) {
         if ((rc = lz_tree_prepare_gumbel(q->tree, d_logits, d_noise, noise_weight, nullptr, d_values, d_to_play, s))) return rc;
-        if ((rc = run_graph(q, 1, false, s))) return rc;
+        if ((rc = search_run_graph(q, 1, false, s))) return rc;
         gs->traversals = q->S;
         gs->pending = false;
         return LZ_OK;
@@ -250,7 +218,7 @@ static int collect_search(lz_search *q, const uint8_t *d_mask, const float *d_lo
         if ((rc = ez_root_hidden(q, nullptr, nullptr, s))) return rc;
         if ((rc = lz_tree_set_tiebreak(q->tree, deterministic))) return rc;
     }
-    return run_graph(q, deterministic, false, s);                                // :775
+    return search_run_graph(q, deterministic, false, s);                                // :775
 }
 
 extern "C" {
@@ -310,6 +278,7 @@ int lz_search_destroy(lz_search *q)
     cudaFree(q->d_policy); cudaFree(q->d_root_logits); cudaFree(q->d_root_value); cudaFree(q->d_skip);
     cudaFree(q->hpool); cudaFree(q->cpool); cudaFree(q->d_is_reset);
     cudaFree(q->d_true_action); cudaFree(q->d_reuse_value);
+    cudaFree(q->rz_latent); cudaFree(q->rz_logits);
     delete q;
     return LZ_OK;
 }
@@ -322,7 +291,7 @@ int lz_search_run_ez(lz_search *q, const float *d_latent_roots, const float *d_h
     int rc = copy_latent_roots(q, d_latent_roots, (cudaStream_t)s);
     if (rc == LZ_OK) rc = ez_root_hidden(q, d_hidden0_roots, d_hidden1_roots, (cudaStream_t)s);
     if (rc) return rc;
-    return run_graph(q, 1, false, (cudaStream_t)s);
+    return search_run_graph(q, 1, false, (cudaStream_t)s);
 }
 
 int lz_search_run_with_reuse(lz_search *q, const float *d_latent_roots, const int32_t *d_true_action, const float *d_reuse_value,
@@ -355,7 +324,7 @@ int lz_search_run(lz_search *q, const float *d_latent_roots, int deterministic, 
     LZ_REQUIRE(!q->tree->gumbel, LZ_ESTATE, "lz_search_run: Gumbel tree, use lz_search_run_gumbel");
     int rc = copy_latent_roots(q, d_latent_roots, (cudaStream_t)s);
     if (rc) return rc;
-    return run_graph(q, deterministic, false, (cudaStream_t)s);
+    return search_run_graph(q, deterministic, false, (cudaStream_t)s);
 }
 
 int lz_search_run_gumbel(lz_search *q, const float *d_latent_roots, lz_stream s)
@@ -370,7 +339,7 @@ int lz_search_run_gumbel(lz_search *q, const float *d_latent_roots, lz_stream s)
                q->S, gs->g.S);
     int rc = copy_latent_roots(q, d_latent_roots, (cudaStream_t)s);
     if (rc) return rc;
-    if ((rc = run_graph(q, 1, false, (cudaStream_t)s))) return rc;
+    if ((rc = search_run_graph(q, 1, false, (cudaStream_t)s))) return rc;
     gs->traversals = q->S;
     gs->pending = false;
     return LZ_OK;
@@ -502,6 +471,7 @@ int lz_search_collect_host_u8(lz_search *q, const uint8_t *h_obs_u8, const uint8
 }
 
 int lz_search_num_kernels(const lz_search *q) { return q ? q->num_kernels : 0; }
+unsigned long long lz_debug_graph_captures(void) { return g_captures.load(std::memory_order_relaxed); }
 
 int lz_search_debug_plan(const lz_search *q, int32_t *h_info)
 {

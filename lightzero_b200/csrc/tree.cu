@@ -77,39 +77,9 @@ k_tree_reset(TreeParams p, const int32_t *legal, const int32_t *nlegal, const ui
         *p.rng_epoch += 1ull;
     }
     if (b >= p.B) return;
-    const int A = p.A;
-    int *lg = p.legal + (size_t)b * A;
-    int n = 0;
-    if (mask) {                              // ascending ids == np.nonzero order (policy/muzero.py:760)
-        for (int c0 = 0; c0 < A; c0 += 32) {
-            int a = c0 + lane;
-            bool on = a < A && mask[(size_t)b * A + a] != 0;
-            unsigned m = __ballot_sync(0xffffffffu, on);
-            if (on) lg[n + __popc(m & ((1u << lane) - 1u))] = a;
-            n += __popc(m);
-        }
-    } else if (legal && nlegal) {
-        n = nlegal[b];
-        for (int k = lane; k < n; k += 32) lg[k] = legal[(size_t)b * A + k];
-    }
-    if (n == 0) {                            // cnode.cpp:101-107: empty list == every action
-        n = A;
-        for (int k = lane; k < A; k += 32) lg[k] = k;
-    }
-    for (int k = n + lane; k < A; k += 32) lg[k] = -1;
-    if (lane == 0) {
-        p.nlegal[b] = n;
-        p.root_visit[b] = 0;
-        p.root_vsum[b] = 0.0f;
-        p.root_reward[b] = 0.0f;
-        p.mm_max[b] = kFloatMin;             // cminimax.cpp:7-11
-        p.mm_min[b] = kFloatMax;
-        p.path_len[b] = 0;
-        p.search_len[b] = 0;
-        p.n_reset[(size_t)b * p.N] = 0;      // the root is never reset (ctree_efficientzero cnode.cpp:54,75)
-        p.n_batch[(size_t)b * p.N] = b;      // root.expand(to_play, 0, i, ...)
-        p.reuse_state[b] = 0;
-    }
+    const size_t row = (size_t)b * p.A;
+    tree_reset_root(p, b, lane, mask ? mask + row : nullptr, (legal && nlegal) ? legal + row : nullptr,
+                    (legal && nlegal) ? nlegal[b] : 0);
 }
 
 // CRoots::prepare / prepare_no_noise (cnode.cpp:321-358)
@@ -119,31 +89,10 @@ k_tree_prepare(TreeParams p, const float *logits, const float *noise, float nois
 {
     const int b = blockIdx.x * (kTreeBlock / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (b >= p.B) return;
-    const int A = p.A, N = p.N;
-    uint32_t *nb = p.edges + (size_t)b * N * kEdgeFields * A;   // slot 0
-    const int *lg = p.legal + (size_t)b * A;
-    const int n = p.nlegal[b];
-    expand_block(nb, A, logits + (size_t)b * A, lg, n, lane);
-    __syncwarp();
-    if (noise) {                             // add_exploration_noise (cnode.cpp:149-167)
-        const float keep = __fsub_rn(1.0f, noise_w);
-        for (int k = lane; k < n; k += 32) {
-            int a = lg[k];
-            float prior = u2f(nb[F_PRIOR * A + a]);
-            float nz = noise[(size_t)b * A + k];
-            nb[F_PRIOR * A + a] = f2u(__fadd_rn(__fmul_rn(prior, keep), __fmul_rn(nz, noise_w)));
-        }
-    }
-    if (lane == 0) {
-        const int tp = to_play ? to_play[b] : -1;
-        p.to_play[b] = tp;
-        p.n_to_play[(size_t)b * N] = tp;
-        p.n_best[(size_t)b * N] = -1;
-        p.root_reward[b] = rewards ? rewards[b] : 0.0f;
-        p.root_visit[b] += 1;                // cnode.cpp:338,356
-        p.vtp[b] = tp;
-        atomicMax(p.players_max, tp);
-    }
+    const int tp = to_play ? to_play[b] : -1;
+    tree_prepare_root(p, b, lane, logits + (size_t)b * p.A, noise ? noise + (size_t)b * p.A : nullptr, noise_w,
+                      rewards ? rewards[b] : 0.0f, tp);
+    if (lane == 0) atomicMax(p.players_max, tp);
 }
 
 // One simulation boundary of every tree: the back-up of the last expansion, then the next descent (see TreeStep).  Fusing
@@ -188,10 +137,7 @@ k_tree_results(TreeParams p, int32_t *visits, float *values, int32_t *nlegal, in
             visits[(size_t)b * A + k] = k < n ? (int)tree_edges[F_VISIT * A + p.legal[(size_t)b * A + k]] : -1;
     }
     if (lane == 0) {
-        if (values) {
-            int vc = p.root_visit[b];
-            values[b] = vc == 0 ? 0.0f : __fdiv_rn(p.root_vsum[b], (float)vc);
-        }
+        if (values) values[b] = tree_root_value(p, b);
         if (nlegal) nlegal[b] = n;
     }
     if (traj) {

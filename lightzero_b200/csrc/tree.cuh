@@ -328,6 +328,83 @@ __device__ __forceinline__ void expand_block(uint32_t *nb, int A, const float *l
     }
 }
 
+// CRoots::CRoots (cnode.cpp:301-317) and a fresh MinMaxStats (cminimax.cpp:7-11) of tree b by the calling warp.  The root's legal
+// list comes from mask (uint8 [A], ascending ids == np.nonzero order, policy/muzero.py:760), else from legal[0, nlegal), else is
+// every action (as is an empty list, cnode.cpp:101-107).  The tree-wide words (players_max, rng_epoch) are the launch's job.
+__device__ __forceinline__ void tree_reset_root(const TreeParams &p, int b, int lane, const uint8_t *mask, const int32_t *legal,
+                                                int nlegal)
+{
+    const int A = p.A;
+    int *lg = p.legal + (size_t)b * A;
+    int n = 0;
+    if (mask) {
+        for (int c0 = 0; c0 < A; c0 += 32) {
+            int a = c0 + lane;
+            bool on = a < A && mask[a] != 0;
+            unsigned m = __ballot_sync(0xffffffffu, on);
+            if (on) lg[n + __popc(m & ((1u << lane) - 1u))] = a;
+            n += __popc(m);
+        }
+    } else if (legal) {
+        n = nlegal;
+        for (int k = lane; k < n; k += 32) lg[k] = legal[k];
+    }
+    if (n == 0) {
+        n = A;
+        for (int k = lane; k < A; k += 32) lg[k] = k;
+    }
+    for (int k = n + lane; k < A; k += 32) lg[k] = -1;
+    if (lane == 0) {
+        p.nlegal[b] = n;
+        p.root_visit[b] = 0;
+        p.root_vsum[b] = 0.0f;
+        p.root_reward[b] = 0.0f;
+        p.mm_max[b] = kFloatMin;
+        p.mm_min[b] = kFloatMax;
+        p.path_len[b] = 0;
+        p.search_len[b] = 0;
+        p.n_reset[(size_t)b * p.N] = 0;      // the root is never reset (ctree_efficientzero cnode.cpp:54,75)
+        p.n_batch[(size_t)b * p.N] = b;      // root.expand(to_play, 0, i, ...)
+        p.reuse_state[b] = 0;
+    }
+}
+
+// CRoots::prepare / prepare_no_noise (cnode.cpp:321-358) of tree b, reset before by this warp: logits f32 [A] by action id,
+// noise f32 [A] in legal order or nullptr.  players_max is the launch's job.
+__device__ __forceinline__ void tree_prepare_root(const TreeParams &p, int b, int lane, const float *logits, const float *noise,
+                                                  float noise_w, float reward, int tp)
+{
+    const int A = p.A, N = p.N;
+    uint32_t *nb = p.edges + (size_t)b * N * kEdgeFields * A;   // slot 0
+    const int *lg = p.legal + (size_t)b * A;
+    const int n = p.nlegal[b];
+    expand_block(nb, A, logits, lg, n, lane);
+    __syncwarp();
+    if (noise) {                             // add_exploration_noise (cnode.cpp:149-167)
+        const float keep = __fsub_rn(1.0f, noise_w);
+        for (int k = lane; k < n; k += 32) {
+            int a = lg[k];
+            float prior = u2f(nb[F_PRIOR * A + a]);
+            nb[F_PRIOR * A + a] = f2u(__fadd_rn(__fmul_rn(prior, keep), __fmul_rn(noise[k], noise_w)));
+        }
+    }
+    if (lane == 0) {
+        p.to_play[b] = tp;
+        p.n_to_play[(size_t)b * N] = tp;
+        p.n_best[(size_t)b * N] = -1;
+        p.root_reward[b] = reward;
+        p.root_visit[b] += 1;                // cnode.cpp:338,356
+        p.vtp[b] = tp;
+    }
+}
+
+// get_values (cnode.cpp:369-380) of tree b
+__device__ __forceinline__ float tree_root_value(const TreeParams &p, int b)
+{
+    const int vc = p.root_visit[b];
+    return vc == 0 ? 0.0f : __fdiv_rn(p.root_vsum[b], (float)vc);
+}
+
 // cbatch_backpropagate body for tree b (cnode.cpp:495-499): expand the leaf reached by the last
 // traverse into slot `latent_index`, then cbackpropagate (cnode.cpp:419-478) along the recorded path.
 // EZ = true: ctree_efficientzero/lib/cnode.cpp:577-601 + 482-575; `reward` is the value prefix, `leaf_reset` the leaf's is_reset.

@@ -89,3 +89,128 @@ def compute_target_policy_reanalyzed(
         return out, roots_values, roots
     roots.clear()
     return out
+
+
+def rezero_write_back(child_visits, root_values, pos_in_game_segment_list, length, policy_mask, action_mask, visits, values):
+    """The buffer-side write-back of the sweep (game_buffer_rezero_mz.py:378-392): where policy_mask is 1, segment n's
+    ``child_visits[n][pos + p]`` becomes the legal-order distribution visits[n, p, :nlegal] and ``root_values[n][pos + p]`` the
+    searched value (a Python float of the fp32 value, as get_values() returns it).  Either list may be None."""
+    action_mask = np.asarray(action_mask)
+    nlegal = np.count_nonzero(action_mask, axis=1)
+    nlegal[nlegal == 0] = action_mask.shape[1]          # an empty legal list is every action (cnode.cpp:101-107)
+    pm = np.asarray(policy_mask)
+    for n, state_index in enumerate(pos_in_game_segment_list):
+        for p in range(length):
+            i = n * length + p
+            if pm[i] == 0:
+                continue
+            if child_visits is not None:
+                child_visits[n][state_index + p] = visits[n, p, :nlegal[i]].tolist()
+            if root_values is not None:
+                root_values[n][state_index + p] = float(values[n, p])
+
+
+def rezero_reuse_stats(infer_count: np.ndarray, num_simulations: int):
+    """What ReZeroMZGameBuffer adds to ``active_root_num`` / ``average_infer`` (game_buffer_rezero_mz.py:352-359) from the
+    per-simulation inference counts [L - 1, S] of the reuse searches: the mean over them of the last count and of
+    ``sum / num_simulations`` (mcts_ctree.py:464-467); (0, 0.0) without reuse searches."""
+    if len(infer_count) == 0:
+        return 0, 0.0
+    temp_length, temp_infer = 0, 0
+    for c in infer_count:
+        temp_length += int(c[-1])
+        temp_infer += int(c.sum()) / num_simulations
+    return temp_length / len(infer_count), temp_infer / len(infer_count)
+
+
+def compute_target_policy_reanalyzed_rezero(
+        model, mcts: MuZeroMCTSCtree, policy_obs, action_mask, to_play, true_action, policy_mask,
+        pos_in_game_segment_list: Sequence[int], length: int, child_visits: Optional[List[list]] = None,
+        root_values: Optional[List[list]] = None, action_space_size: Optional[int] = None,
+        action_type: str = "fixed_action_space", reanalyze_noise: bool = True, reuse_search: bool = True,
+        mini_infer_size: int = 10240, noises: Optional[np.ndarray] = None):
+    """Mirror of ``ReZeroMZGameBuffer._compute_target_policy_reanalyzed`` (lzero/mcts/buffer/game_buffer_rezero_mz.py:194-404;
+    with an ``EfficientZeroMCTSCtree``, ``ReZeroEZGameBuffer``'s, game_buffer_rezero_ez.py:126-330) as one device call
+    (``lz_rezero_reanalyze`` / ``_ez``): initial_inference over every row, the plain search of the last position, then
+    ``length - 1`` search_with_reuse calls walking backward, each reusing the previous search's root values, and the targets.
+
+    policy_obs [N * length, ...] (row = segment * length + position), action_mask [N * length, A] 0/1, to_play, true_action
+    (-2 past a segment's end) and policy_mask [N * length]; pos_in_game_segment_list [N].  ``child_visits`` / ``root_values``:
+    per segment, the lists the reference rewrites in place at ``pos + position`` where policy_mask is 1.
+    Returns ``(targets, (active_root_num, average_infer))``: the np.ndarray [N, length, A] the reference returns and what it adds
+    to those two statistics.  Ties: the first search by the config's ``deterministic`` (MuZero), the reuse searches and every
+    EfficientZero search by the first maximum (the reference's rand() % len(ties) with rand() == 0).  ``noises`` [N * length, A]
+    (legal order) are drawn with np.random.dirichlet like the reference only when None."""
+    from . import mz_tree
+    from .efficientzero_model import EfficientZeroModel
+    from .efficientzero_model_mlp import EfficientZeroModelMLP
+    from .mcts_ctree import GumbelMuZeroMCTSCtree, UniZeroMCTSCtree
+    from .muzero_model import MuZeroModel
+    from .muzero_model_mlp import MuZeroModelMLP
+    from . import cabi
+
+    L = int(length)
+    if L < 1:
+        raise ValueError(f"compute_target_policy_reanalyzed_rezero: length must be >= 1 (got {length}); the reference builds no "
+                         "rows for length < 1")
+    if isinstance(mcts, (GumbelMuZeroMCTSCtree, UniZeroMCTSCtree)) or not isinstance(mcts, MuZeroMCTSCtree):
+        raise TypeError(f"compute_target_policy_reanalyzed_rezero: {type(mcts).__name__} has no ReZero sweep "
+                        "(MuZeroMCTSCtree or EfficientZeroMCTSCtree)")
+    ez = isinstance(mcts, EfficientZeroMCTSCtree)
+    ez_model = isinstance(model, (EfficientZeroModel, EfficientZeroModelMLP))
+    if ez and not ez_model:
+        raise TypeError(f"EfficientZeroMCTSCtree: the ReZero sweep needs an EfficientZeroModel or EfficientZeroModelMLP, "
+                        f"not a {type(model).__name__}")
+    if not ez and (ez_model or not isinstance(model, (MuZeroModel, MuZeroModelMLP))):
+        raise TypeError(f"MuZeroMCTSCtree: the ReZero sweep needs a MuZeroModel or MuZeroModelMLP, not a {type(model).__name__}")
+    if ez and not mcts.deterministic:
+        raise ValueError("EfficientZeroMCTSCtree: the ReZero sweep breaks every tie by the first maximum (the reference's "
+                         "EfficientZero tree has no other rule); deterministic=False is not available")
+    cfg = mcts._cfg
+    S = int(cfg.num_simulations)
+    N = len(pos_in_game_segment_list)
+    rows = N * L
+    action_mask = np.asarray(action_mask)
+    A = int(action_space_size or action_mask.shape[1])
+    if policy_obs.shape[0] != rows or action_mask.shape != (rows, A):
+        raise ValueError(f"compute_target_policy_reanalyzed_rezero: {N} segments x length {L} = {rows} rows, got policy_obs "
+                         f"{tuple(policy_obs.shape)} and action_mask {action_mask.shape}")
+    if noises is None:        # game_buffer_rezero_mz.py:266-270 (drawn whether or not reanalyze_noise uses them)
+        noises = np.stack([np.random.dirichlet([cfg.root_dirichlet_alpha] * A).astype(np.float32) for _ in range(rows)])
+    dev = model.device
+    H = int(cfg.lstm_horizon_len) if ez else 5
+    t = mz_tree.acquire_tree(dev, N, A, S)
+    try:
+        t.set_params(*mcts._params())
+        cabi.check(t.lib.lz_tree_set_gumbel(t.h, 0, 0), "lz_tree_set_gumbel")     # a pooled tree a Gumbel collect left behind
+        cabi.check(t.lib.lz_tree_set_ez(t.h, int(ez), H), "lz_tree_set_ez")
+        q = t.search_for(model, S, (1, H) if ez else ())
+        with torch.cuda.device(dev):
+            s = cabi.stream_ptr()
+            obs = mz_tree._to_dev(policy_obs, torch.float32, dev)
+            mask = mz_tree._to_dev(action_mask, torch.uint8, dev, (rows, A))
+            tp = mz_tree._to_dev(np.asarray(to_play, np.int32), torch.int32, dev, (rows,))
+            ta = mz_tree._to_dev(np.asarray(true_action, np.int32), torch.int32, dev, (rows,))
+            pm = mz_tree._to_dev(np.asarray(policy_mask, np.uint8), torch.uint8, dev, (rows,))
+            nz = mz_tree._to_dev(noises, torch.float32, dev, (rows, A)) if reanalyze_noise else None
+            targets = torch.empty((N, L, A), dtype=torch.float64, device=dev)
+            visits = torch.empty((N, L, A), dtype=torch.float64, device=dev)
+            values = torch.empty((N, L), dtype=torch.float32, device=dev)
+            nreuse = L - 1 if reuse_search else 0
+            counts = torch.empty((nreuse, S), dtype=torch.int32, device=dev)
+            head = (q, L, int(bool(reuse_search)), int(mini_infer_size), obs.data_ptr(), None, None, mask.data_ptr(),
+                    tp.data_ptr(), ta.data_ptr(), pm.data_ptr(), cabi.ptr(nz), float(cfg.root_noise_weight))
+            tail = (int(action_type != "fixed_action_space"), targets.data_ptr(), values.data_ptr(), visits.data_ptr(),
+                    counts.data_ptr() if nreuse else None, s)
+            if ez:
+                cabi.check(t.lib.lz_rezero_reanalyze_ez(*head, *tail), "lz_rezero_reanalyze_ez")
+            else:
+                cabi.check(t.lib.lz_rezero_reanalyze(*head, int(mcts.deterministic), *tail), "lz_rezero_reanalyze")
+            mcts.last_num_kernels = t.lib.lz_search_num_kernels(q)
+            out, vis, val, cnt = targets.cpu().numpy(), visits.cpu().numpy(), values.cpu().numpy(), counts.cpu().numpy()
+    finally:
+        t.release()
+
+    mcts.last_infer_count = cnt       # [L - 1, S] per reuse search and simulation: trees that needed the network
+    rezero_write_back(child_visits, root_values, pos_in_game_segment_list, L, policy_mask, action_mask, vis, val)
+    return out, rezero_reuse_stats(cnt, S)
