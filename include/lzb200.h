@@ -417,6 +417,43 @@ int lz_rezero_reanalyze_ez(lz_search *q, int L, int reuse_search, int mini_infer
                            const float *d_logits, const uint8_t *d_mask, const int32_t *d_to_play, const int32_t *d_true_action,
                            const uint8_t *d_policy_mask, const float *d_noise, float noise_weight, int scatter_legal,
                            double *d_targets, float *d_root_values, double *d_child_visits, int32_t *d_infer_count, lz_stream s);
+/* ---- Replay-buffer reward and value targets (MuZeroGameBuffer._compute_target_reward_value,
+ * lzero/mcts/buffer/game_buffer_muzero.py:467-575; EfficientZeroGameBuffer, game_buffer_efficientzero.py:167-323) ----
+ * N sampled segments of K1 = num_unroll_steps + 1 rows, T = N * K1 rows, row = segment * K1 + position (the reference's
+ * value_obs_list order).  The host packs the ragged reward and to_play windows and the discount powers into the device tables
+ * below (lightzero_b200.reanalyze.compute_target_reward_value); every power is computed on the host with the reference's own
+ * expression, the device only multiplies and adds. */
+typedef struct lz_value_tables {
+    int N, K1;                     /* segments, rows per segment */
+    int W, P;                      /* reward window width (K1 - 1 + P), power-table length (the largest td) */
+    int value_prefix;              /* 1: EfficientZero value prefixes and targets; 0: MuZero rewards and targets */
+    int fp32;                      /* 1: float32 rewards (float32 products, float32 sums after the first add); 0: float64 */
+    int two_player;                /* env_type == 'board_games' and to_play_segment[0][0] in [1, 2] */
+    int horizon;                   /* lstm_horizon_len (value_prefix) */
+    int alias_prefix;              /* value_prefix with (n, 1) rewards: the reference appends one array per horizon chunk, added
+                                      to in place, so every row of a chunk reads the chunk's last prefix */
+    const double *rewards;         /* [N][W]: reward_list[pos + w] (exact float64 of the float32 rewards), 0 past rlen */
+    const int32_t *rlen;           /* [N]: clip(len(reward_list) - pos, 0, W) */
+    const int32_t *seglen;         /* [N]: clip(game_segment_len - pos, 0, K1) (value_prefix) */
+    const int32_t *td;             /* [T]: td_steps_list */
+    const double *bootstrap;       /* [T]: discount ** td, negated for odd td in two_player mode */
+    const double *value_mask;      /* [T] */
+    const double *powers;          /* [P]: discount ** i */
+    const int32_t *to_play;        /* two_player: [N][P + K1], to_play_list[i] for i < P then to_play_list[pos + k]; else NULL */
+} lz_value_tables;
+/* initial_inference over the T observations d_obs f32 [T, obs...] in mini_infer_size slices (value scalars only, into d_values
+ * f32 [T]), then one thread per segment writes d_reward_out f64 [N, K1] (rewards, or value prefixes) and d_value_out f64 [N, K1]
+ * (value targets).  The model must be an EfficientZero model exactly when tab->value_prefix.  Enqueued on s, no host sync. */
+int lz_value_targets(lz_model *m, const lz_value_tables *tab, int mini_infer_size, const float *d_obs, float *d_values,
+                     double *d_reward_out, double *d_value_out, lz_stream s);
+/* EfficientZero with use_root_value: for an EfficientZero search q of B = T roots, initial_inference in mini_infer_size slices
+ * (latents into the search's pool, policy logits), the roots reset to d_mask uint8 [T, A] and prepared with zero value prefixes,
+ * d_noise f32 [T, A] in legal order (NULL: prepare_no_noise), noise_weight and d_to_play int32 [T] (NULL: -1), the search's
+ * captured graph on zero LSTM state (ties: first maximum when first_maximum, lz_tree_set_tiebreak), its root values into
+ * d_values f32 [T], then the targets as lz_value_targets.  A repeated call of the same shapes captures no graph. */
+int lz_value_targets_root(lz_search *q, const lz_value_tables *tab, int mini_infer_size, const float *d_obs, const uint8_t *d_mask,
+                          const int32_t *d_to_play, const float *d_noise, float noise_weight, int first_maximum, float *d_values,
+                          double *d_reward_out, double *d_value_out, lz_stream s);
 /* Test hook: search graphs this library has captured since load (a capture happens on a search's first run and after a change of
  * the model, the tree parameters or the tie rule). */
 unsigned long long lz_debug_graph_captures(void);

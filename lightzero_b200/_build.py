@@ -2,7 +2,8 @@
 
 In-tree build: the .so is git-ignored and rebuilt when a source or header is newer.
 tree.cu, gumbel.cu and rezero.cu are compiled with -fmad=false (the reference tree is built for baseline x86-64 and never
-contracts a*b+c; bit-exact visit counts depend on it); the network kernels want FMA.
+contracts a*b+c; bit-exact visit counts depend on it), and so is targets.cu (the buffer's NumPy target arithmetic never fuses
+either); the network kernels want FMA.
 """
 import os
 import subprocess
@@ -16,7 +17,7 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fno-fast-math"]
 # Experiment builds: `python -m lightzero_b200._build --tag NAME -DFOO ...` writes _lib/NAME/liblzb200.so with the extra
 # defines; LZ_LIB_TAG=NAME makes cabi.load() pick it (one GPU session can then compare several kernel variants).
-UNITS = [("tree.cu", ["-fmad=false"]), ("gumbel.cu", ["-fmad=false"]), ("model.cu", []), ("conv_model.cu", []), ("net_tc.cu", []), ("board_tc.cu", []), ("conv_tc.cu", []), ("mlp.cu", []), ("mlp_tc.cu", []), ("ez.cu", []), ("search.cu", []), ("rezero.cu", ["-fmad=false"]), ("collector.cu", [])]
+UNITS = [("tree.cu", ["-fmad=false"]), ("gumbel.cu", ["-fmad=false"]), ("model.cu", []), ("conv_model.cu", []), ("net_tc.cu", []), ("board_tc.cu", []), ("conv_tc.cu", []), ("mlp.cu", []), ("mlp_tc.cu", []), ("ez.cu", []), ("search.cu", []), ("rezero.cu", ["-fmad=false"]), ("targets.cu", ["-fmad=false"]), ("collector.cu", [])]
 
 
 def _stale(target, deps):

@@ -40,6 +40,14 @@ class MlpEzConfig(ctypes.Structure):
                 ("support_step", c_float)]
 
 
+class ValueTables(ctypes.Structure):
+    """struct lz_value_tables (include/lzb200.h): host struct of device table pointers"""
+    _fields_ = [("N", c_int), ("K1", c_int), ("W", c_int), ("P", c_int), ("value_prefix", c_int), ("fp32", c_int),
+                ("two_player", c_int), ("horizon", c_int), ("alias_prefix", c_int), ("rewards", c_void_p), ("rlen", c_void_p),
+                ("seglen", c_void_p), ("td", c_void_p), ("bootstrap", c_void_p), ("value_mask", c_void_p), ("powers", c_void_p),
+                ("to_play", c_void_p)]
+
+
 # name -> (restype, argtypes); every symbol include/lzb200.h declares
 SIGNATURES = {
     "lz_version": (c_int, []),
@@ -124,6 +132,9 @@ SIGNATURES = {
     "lz_search_hidden_pool": (c_void_p, [c_void_p, c_int]),
     "lz_rezero_reanalyze": (c_int, [c_void_p, c_int, c_int, c_int] + [c_void_p] * 8 + [c_float, c_int, c_int] + [c_void_p] * 5),
     "lz_rezero_reanalyze_ez": (c_int, [c_void_p, c_int, c_int, c_int] + [c_void_p] * 8 + [c_float, c_int] + [c_void_p] * 5),
+    "lz_value_targets": (c_int, [c_void_p, ctypes.POINTER(ValueTables), c_int] + [c_void_p] * 5),
+    "lz_value_targets_root": (c_int, [c_void_p, ctypes.POINTER(ValueTables), c_int] + [c_void_p] * 4 + [c_float, c_int] +
+                              [c_void_p] * 4),
     "lz_debug_graph_captures": (ctypes.c_uint64, []),
 }
 
