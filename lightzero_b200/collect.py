@@ -17,8 +17,11 @@ from . import cabi, mz_tree
 from .efficientzero_model import EfficientZeroModel
 from .efficientzero_model_mlp import EfficientZeroModelMLP
 from .mcts_ctree import EfficientZeroMCTSCtree, GumbelMuZeroMCTSCtree, MuZeroMCTSCtree
+from .model_base import LzModel
 from .muzero_model import MuZeroModel
 from .muzero_model_mlp import MuZeroModelMLP
+
+_NP = {torch.uint8: np.uint8, torch.float32: np.float32, torch.int32: np.int32}
 
 
 def select_action(visit_counts: np.ndarray, temperature: float = 1, deterministic: bool = True):
@@ -35,6 +38,29 @@ def select_action(visit_counts: np.ndarray, temperature: float = 1, deterministi
     return action_pos, entropy
 
 
+def _as_tensor(x, dtype):
+    """A mask, noise or to_play argument (tensor, array or list) as a tensor of dtype where it already lives: arrays and
+    lists on the host."""
+    if isinstance(x, torch.Tensor):
+        return x.to(dtype)
+    return torch.from_numpy(np.require(x, _NP[dtype], ["C", "W"]))     # copies read-only views (np.broadcast_to)
+
+
+def _broadcast_to_play(to_play, B):
+    return np.broadcast_to(np.asarray(to_play, np.int32).reshape(-1), (B,)) if np.size(to_play) in (1, B) else to_play
+
+
+def _legal_dirichlet(action_mask, alpha):
+    """Root noise drawn with np.random as the reference policies do (policy/muzero.py:763-766, gumbel_muzero.py:555-558):
+    per root, Dirichlet(alpha) over its legal actions, in legal order, zero padded to [B, A]."""
+    B, A = action_mask.shape
+    noises = np.zeros((B, A), np.float32)
+    for j in range(B):
+        n = int(action_mask[j].sum())
+        noises[j, :n] = np.random.dirichlet([alpha] * n).astype(np.float32)
+    return noises
+
+
 class MuZeroCollectPolicy:
     def __init__(self, model: MuZeroModel, cfg: Optional[dict] = None):
         self.model = model
@@ -43,7 +69,7 @@ class MuZeroCollectPolicy:
         self.device = model.device
         self._buf = {}
         self.h2d_chunks = 2      # host observation batches are copied in this many overlapped pieces
-        self._tree_mode = (0, 5)   # (EfficientZero value-prefix trees?, lstm_horizon_len)
+        self._tree_mode = ()     # the search_for / TreeHandle.set_mode mode: MuZero trees
 
     # ---- device-resident fast path ---------------------------------------------------------------
     def _bufs(self, B, A):
@@ -80,46 +106,29 @@ class MuZeroCollectPolicy:
             # uint8 frames (what the Atari emulator delivers) stay uint8 on the wire: a quarter of the bytes; the [0, 1] scaling
             # of the reference's ScaledFloatFrameWrapper happens inside the first conv kernel (lz_search_collect*_u8)
             u8 = obs.dtype == torch.uint8
+            obs = obs.contiguous() if u8 else obs.to(torch.float32).contiguous()
+            args = ((action_mask, "mask"), (noises, "noise"), (to_play, "to_play"))
             if host_path:
-                h_obs = obs.contiguous() if u8 else obs.to(torch.float32).contiguous()
-                h_mask = (action_mask if isinstance(action_mask, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(action_mask))).to(torch.uint8).contiguous()
-                h_noise = None
-                if noises is not None:
-                    h_noise = (noises if isinstance(noises, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(noises, dtype=np.float32))).to(torch.float32).contiguous()
-                h_tp = None
-                if to_play is not None:
-                    h_tp = (to_play if isinstance(to_play, torch.Tensor) else torch.from_numpy(np.array(to_play, np.int32).reshape(-1))).to(torch.int32).contiguous()
-                assert not h_mask.is_cuda and (h_noise is None or not h_noise.is_cuda), "host observation batch needs host mask / noise"
-                self._keep_host = (h_obs, h_mask, h_noise, h_tp)
+                mask, noise, tp = (None if x is None else _as_tensor(x, bufs[k].dtype).contiguous() for x, k in args)
+                assert not mask.is_cuda and (noise is None or not noise.is_cuda), "host observation batch needs host mask / noise"
+                self._keep_host = (obs, mask, noise, tp)
             else:
-                d_obs = obs.contiguous() if u8 else obs.to(torch.float32).contiguous()
-                mask_t = action_mask if isinstance(action_mask, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(action_mask))
-                bufs["mask"].copy_(mask_t.to(torch.uint8), non_blocking=True)
-                d_noise = None
-                if noises is not None:
-                    nz = noises if isinstance(noises, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(noises, dtype=np.float32))
-                    bufs["noise"].copy_(nz, non_blocking=True)
-                    d_noise = bufs["noise"]
-                d_tp = None
-                if to_play is not None:
-                    tp = to_play if isinstance(to_play, torch.Tensor) else torch.from_numpy(np.array(to_play, np.int32).reshape(-1))
-                    bufs["to_play"].copy_(tp.to(torch.int32), non_blocking=True)
-                    d_tp = bufs["to_play"]
-            tree = mz_tree.acquire_tree(dev, B, A, S)
-            try:
-                tree.set_params(*self.mcts._params())
-                q = self._search_for(tree, S)
+                mask, noise, tp = (None if x is None else bufs[k].copy_(_as_tensor(x, bufs[k].dtype), non_blocking=True)
+                                   for x, k in args)
+            # the search and the clones below may still be queued when the tree is released: the next holder waits for them
+            with self._held_tree(B, A, S, det) as tree:
+                q = tree.search_for(self.model, S, self._tree_mode)
                 s = cabi.stream_ptr()
                 if host_path:
                     fn = tree.lib.lz_search_collect_host_u8 if u8 else tree.lib.lz_search_collect_host
-                    cabi.check(fn(q, h_obs.data_ptr(), h_mask.data_ptr(), cabi.ptr(h_noise),
-                                  float(self.cfg.root_noise_weight), cabi.ptr(h_tp), int(det),
+                    cabi.check(fn(q, obs.data_ptr(), mask.data_ptr(), cabi.ptr(noise),
+                                  float(self.cfg.root_noise_weight), cabi.ptr(tp), int(det),
                                   int(self.h2d_chunks), bufs["pred_value"].data_ptr(),
                                   bufs["logits"].data_ptr(), s), "lz_search_collect_host")
                 else:
                     fn = tree.lib.lz_search_collect_u8 if u8 else tree.lib.lz_search_collect
-                    cabi.check(fn(q, d_obs.data_ptr(), bufs["mask"].data_ptr(), cabi.ptr(d_noise),
-                                  float(self.cfg.root_noise_weight), cabi.ptr(d_tp), int(det),
+                    cabi.check(fn(q, obs.data_ptr(), mask.data_ptr(), cabi.ptr(noise),
+                                  float(self.cfg.root_noise_weight), cabi.ptr(tp), int(det),
                                   bufs["pred_value"].data_ptr(), bufs["logits"].data_ptr(), s),
                                "lz_search_collect")
                 cabi.check(tree.lib.lz_tree_results(tree.h, tree.visits.data_ptr(), tree.values.data_ptr(),
@@ -140,18 +149,15 @@ class MuZeroCollectPolicy:
                 for k in selected:
                     bufs["h_" + k].copy_(bufs[k], non_blocking=True)
                 torch.cuda.current_stream().synchronize()
-            finally:
-                tree.release()         # the search and the clones above may still be queued: the next holder waits for them
         out = dict(visits=bufs["h_visits"], values=bufs["h_values"], nlegal=bufs["h_nlegal"],
                    pred_value=bufs["h_pred"], policy_logits=bufs["h_logits"])
         out.update({k: bufs["h_" + k] for k in selected})
         return out
 
-    def _search_for(self, tree, S):
-        """Puts the pooled tree in this policy's mode and returns its lz_search for the model."""
-        cabi.check(tree.lib.lz_tree_set_gumbel(tree.h, 0, 0), "lz_tree_set_gumbel")    # a tree a Gumbel collect left behind
-        cabi.check(tree.lib.lz_tree_set_ez(tree.h, *self._tree_mode), "lz_tree_set_ez")
-        return tree.search_for(self.model, S, self._tree_mode if self._tree_mode[0] else ())
+    def _held_tree(self, B, A, S, det):
+        """A pooled tree in this policy's mode for one search_batch: the collect's tie rule is its ``deterministic``, which
+        lz_search_collect also applies to EfficientZero trees."""
+        return mz_tree.held_tree(self.device, B, A, S, self.mcts._params(), self._tree_mode, det)
 
     def _select(self, tree, bufs, select, s):
         """select_action on the device into bufs; returns the names of the tensors it wrote."""
@@ -170,14 +176,8 @@ class MuZeroCollectPolicy:
         if ready_env_id is None:
             ready_env_id = np.arange(B)
         action_mask = np.asarray(action_mask)
-        A = action_mask.shape[1]
-        alpha = float(self.cfg.root_dirichlet_alpha)
-        noises = np.zeros((B, A), np.float32)
-        for j in range(B):                                   # policy/muzero.py:763-766
-            n = int(action_mask[j].sum())
-            noises[j, :n] = np.random.dirichlet([alpha] * n).astype(np.float32)
-        tp = np.broadcast_to(np.asarray(to_play, np.int32).reshape(-1), (B,)) if np.size(to_play) in (1, B) else to_play
-        r = self.search_batch(data, action_mask, noises, tp, deterministic=self.mcts.deterministic,
+        noises = _legal_dirichlet(action_mask, float(self.cfg.root_dirichlet_alpha))
+        r = self.search_batch(data, action_mask, noises, _broadcast_to_play(to_play, B), deterministic=self.mcts.deterministic,
                               select=(temperature, False, seed) if device_select_action else None)
         return self._format(r, action_mask, ready_env_id, temperature, deterministic_action=False)
 
@@ -187,8 +187,7 @@ class MuZeroCollectPolicy:
         if ready_env_id is None:
             ready_env_id = np.arange(B)
         action_mask = np.asarray(action_mask)
-        tp = np.broadcast_to(np.asarray(to_play, np.int32).reshape(-1), (B,)) if np.size(to_play) in (1, B) else to_play
-        r = self.search_batch(data, action_mask, None, tp, deterministic=self.mcts.deterministic)
+        r = self.search_batch(data, action_mask, None, _broadcast_to_play(to_play, B), deterministic=self.mcts.deterministic)
         return self._format(r, action_mask, ready_env_id, 1, deterministic_action=True)
 
     def _format(self, r, action_mask, ready_env_id, temperature, deterministic_action) -> Dict[int, dict]:
@@ -222,7 +221,7 @@ class EfficientZeroCollectPolicy(MuZeroCollectPolicy):
         super().__init__(model, cfg)
         self.mcts = EfficientZeroMCTSCtree(cfg or {})
         self.cfg = self.mcts._cfg
-        self._tree_mode = (1, int(self.cfg.lstm_horizon_len))
+        self._tree_mode = (1, int(self.cfg.lstm_horizon_len))     # value-prefix trees
 
 
 class GumbelMuZeroCollectPolicy(MuZeroCollectPolicy):
@@ -234,12 +233,13 @@ class GumbelMuZeroCollectPolicy(MuZeroCollectPolicy):
     dicts have the reference's keys."""
 
     def __init__(self, model: Union[MuZeroModel, MuZeroModelMLP], cfg: Optional[dict] = None):
-        if isinstance(model, (EfficientZeroModel, EfficientZeroModelMLP)):
+        if isinstance(model, LzModel) and model.value_prefix:
             raise TypeError(f"GumbelMuZeroCollectPolicy: the Gumbel search runs MuZero models, not an {type(model).__name__}")
         super().__init__(model, cfg)
         self.mcts = GumbelMuZeroMCTSCtree(cfg or {})
         self.cfg = self.mcts._cfg
         self.cfg.setdefault("max_num_considered_actions", 4)
+        self._tree_mode = ("gumbel",)
 
     def _bufs(self, B, A):
         bufs = super()._bufs(B, A)
@@ -249,10 +249,10 @@ class GumbelMuZeroCollectPolicy(MuZeroCollectPolicy):
                 bufs["h_" + k] = torch.empty(B, A).pin_memory()
         return bufs
 
-    def _search_for(self, tree, S):
-        cabi.check(tree.lib.lz_tree_set_ez(tree.h, 0, 5), "lz_tree_set_ez")
-        cabi.check(tree.lib.lz_tree_set_gumbel(tree.h, int(self.cfg.max_num_considered_actions), S), "lz_tree_set_gumbel")
-        return tree.search_for(self.model, S, ("gumbel",))
+    def _held_tree(self, B, A, S, det):
+        """A Gumbel tree: its descents never read the tie rule."""
+        return mz_tree.held_tree(self.device, B, A, S, self.mcts._params(),
+                                 gumbel=(int(self.cfg.max_num_considered_actions), S))
 
     def _select(self, tree, bufs, select, s):
         """lz_tree_gumbel_select_action at temperature select[0]: the action never depends on a draw."""
@@ -266,23 +266,15 @@ class GumbelMuZeroCollectPolicy(MuZeroCollectPolicy):
         """gumbel_muzero.py:498-607: Dirichlet noise in legal order drawn with np.random as the reference does."""
         B = data.shape[0]
         action_mask = np.asarray(action_mask)
-        alpha = float(self.cfg.root_dirichlet_alpha)
-        noises = np.zeros((B, action_mask.shape[1]), np.float32)
-        for j in range(B):                                   # gumbel_muzero.py:555-558
-            n = int(action_mask[j].sum())
-            noises[j, :n] = np.random.dirichlet([alpha] * n).astype(np.float32)
-        r = self.search_batch(data, action_mask, noises, self._to_play(to_play, B), select=(temperature, False, 0))
+        noises = _legal_dirichlet(action_mask, float(self.cfg.root_dirichlet_alpha))
+        r = self.search_batch(data, action_mask, noises, _broadcast_to_play(to_play, B), select=(temperature, False, 0))
         return self._format_gumbel(r, B, ready_env_id, collect=True)
 
     def forward_eval(self, data: torch.Tensor, action_mask, to_play=(-1,), ready_env_id=None, **kwargs) -> Dict[int, dict]:
         """gumbel_muzero.py:619-720: no noise, entropy at temperature 1."""
         B = data.shape[0]
-        r = self.search_batch(data, np.asarray(action_mask), None, self._to_play(to_play, B), select=(1.0, True, 0))
+        r = self.search_batch(data, np.asarray(action_mask), None, _broadcast_to_play(to_play, B), select=(1.0, True, 0))
         return self._format_gumbel(r, B, ready_env_id, collect=False)
-
-    @staticmethod
-    def _to_play(to_play, B):
-        return np.broadcast_to(np.asarray(to_play, np.int32).reshape(-1), (B,)) if np.size(to_play) in (1, B) else to_play
 
     def _format_gumbel(self, r, B, ready_env_id, collect) -> Dict[int, dict]:
         if ready_env_id is None:

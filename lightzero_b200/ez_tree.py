@@ -31,34 +31,21 @@ def batch_traverse(roots: Roots, pb_c_base: int, pb_c_init: float, discount_fact
                    return_tensors: bool = False):
     """ez_tree.pyx batch_traverse -> (latent_state_index_in_search_path, latent_state_index_in_batch, last_actions,
     virtual_to_play_batch)."""
-    if roots._tree is None:
-        roots._materialize(_mz.DEFAULT_MAX_SIMS)
-    t = roots._tree
+    t = roots._need_tree()
     t.set_params(pb_c_base, pb_c_init, discount_factor, min_max_stats_lst.value_delta_max)
     with torch.cuda.device(roots.device):
         cabi.check(t.lib.lz_tree_traverse_ez(t.h, t.ix.data_ptr(), t.iy.data_ptr(), t.action.data_ptr(),
                                              t.search_len.data_ptr(), t.vtp.data_ptr(), None, cabi.stream_ptr()),
                    "lz_tree_traverse_ez")
-    results._roots = roots
-    if return_tensors:
-        return t.ix, t.iy, t.action, t.vtp
-    packed = torch.stack((t.ix, t.iy, t.action, t.vtp)).cpu().numpy()
-    return packed[0].tolist(), packed[1].tolist(), packed[2].tolist(), packed[3].tolist()
+    return _mz._traversed(roots, results, return_tensors)
 
 
 def batch_backpropagate(current_latent_state_index: int, discount_factor: float, value_prefixs, values, policies,
                         min_max_stats_lst: MinMaxStatsList, results: ResultsWrapper, is_reset_list, to_play_batch):
     """ez_tree.pyx batch_backpropagate"""
-    roots = results._roots
-    t = roots._tree
-    B, A = roots.root_num, t.A
-    dev = roots.device
-    vp = _to_dev(value_prefixs, torch.float32, dev, (B,))
-    val = _to_dev(values, torch.float32, dev, (B,))
-    pol = _to_dev(policies, torch.float32, dev, (B, A))
-    rs = _to_dev(is_reset_list, torch.int32, dev, (B,))
-    tp = _to_dev(to_play_batch, torch.int32, dev, (B,)) if to_play_batch is not None else None
-    with torch.cuda.device(dev):
+    roots, t, vp, val, pol, tp = _mz._backup_inputs(results, value_prefixs, values, policies, to_play_batch)
+    rs = _to_dev(is_reset_list, torch.int32, roots.device, (roots.root_num,))
+    with torch.cuda.device(roots.device):
         cabi.check(t.lib.lz_tree_backpropagate_ez(t.h, int(current_latent_state_index), vp.data_ptr(), val.data_ptr(),
                                                   pol.data_ptr(), rs.data_ptr(), cabi.ptr(tp), cabi.stream_ptr()),
                    "lz_tree_backpropagate_ez")

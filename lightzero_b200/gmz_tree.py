@@ -42,13 +42,6 @@ class Roots(mz_tree.Roots):
     def get_policies(self, discount: float, action_space_size: int) -> List[List[float]]:
         return self.get_policies_tensor(discount, action_space_size).cpu().tolist()
 
-    def clear(self):
-        if self._tree is not None:      # hand the pooled tree back as a MuZero tree
-            with torch.cuda.device(self.device):
-                cabi.check(self._tree.lib.lz_tree_set_gumbel(self._tree.h, 0, 0), "lz_tree_set_gumbel")
-            self._gumbel = None
-        super().clear()
-
     # ---- device-side extras ----------------------------------------------------------------------
     def get_children_values_tensor(self, discount: float, action_space_size: int):
         return self._policies(discount, action_space_size)[0]
@@ -90,20 +83,7 @@ class Roots(mz_tree.Roots):
         return self._tree
 
     def _materialize_gumbel(self, g, params=None):
-        m, S = g
-        if self._pending is None:
-            raise RuntimeError("Roots: prepare()/prepare_no_noise() has not been called")
-        A = self._pending["A"]
-        if self._tree is not None and (self._tree.max_sims < S or self._tree.A != A):
-            self.clear()
-        if self._tree is None:
-            self._tree = mz_tree.acquire_tree(self.device, self.root_num, A, S)
-        t = self._tree
-        if params is not None:
-            t.set_params(*params)
-        with torch.cuda.device(self.device):
-            cabi.check(t.lib.lz_tree_set_ez(t.h, 0, 5), "lz_tree_set_ez")
-            cabi.check(t.lib.lz_tree_set_gumbel(t.h, m, S), "lz_tree_set_gumbel")
+        self._acquire(g[1], params, True, gumbel=g)     # the Gumbel descents never read the tie rule
         self._gumbel = g
         self._reset_and_prepare()
 
@@ -117,7 +97,7 @@ class Roots(mz_tree.Roots):
                                                     cabi.ptr(p["rewards"]), self._values.data_ptr(), cabi.ptr(p["to_play"]), s),
                        "lz_tree_prepare_gumbel")
 
-    def _materialize(self, max_sims, params=None):
+    def _materialize(self, max_sims, params=None, deterministic=None):
         # a re-prepare of a materialised tree (mz_tree.Roots._stage) starts a fresh Gumbel search
         if self._gumbel is None:
             self._gumbel = (max_sims, max_sims)
@@ -133,25 +113,15 @@ def batch_traverse(roots: Roots, num_simulations: int, max_num_considered_action
         cabi.check(t.lib.lz_tree_traverse_gumbel(t.h, t.ix.data_ptr(), t.iy.data_ptr(), t.action.data_ptr(),
                                                  t.search_len.data_ptr(), t.vtp.data_ptr(), cabi.stream_ptr()),
                    "lz_tree_traverse_gumbel")
-    results._roots = roots
-    if return_tensors:
-        return t.ix, t.iy, t.action, t.vtp
-    packed = torch.stack((t.ix, t.iy, t.action, t.vtp)).cpu().numpy()
-    return packed[0].tolist(), packed[1].tolist(), packed[2].tolist(), packed[3].tolist()
+    return mz_tree._traversed(roots, results, return_tensors)
 
 
 def batch_back_propagate(current_latent_state_index: int, discount: float, value_prefixs, values, policies,
                          min_max_stats_lst: MinMaxStatsList, results: ResultsWrapper, to_play_batch):
     """gmz_tree.pyx:81-88"""
-    roots = results._roots
-    t = roots._tree
-    roots._set_discount(float(discount))
-    B, A, dev = roots.root_num, t.A, roots.device
-    rew = _to_dev(value_prefixs, torch.float32, dev, (B,))
-    val = _to_dev(values, torch.float32, dev, (B,))
-    pol = _to_dev(policies, torch.float32, dev, (B, A))
-    tp = _to_dev(to_play_batch, torch.int32, dev, (B,)) if to_play_batch is not None else None
-    with torch.cuda.device(dev):
+    results._roots._set_discount(float(discount))
+    roots, t, rew, val, pol, tp = mz_tree._backup_inputs(results, value_prefixs, values, policies, to_play_batch)
+    with torch.cuda.device(roots.device):
         cabi.check(t.lib.lz_tree_backpropagate_gumbel(t.h, int(current_latent_state_index), rew.data_ptr(), val.data_ptr(),
                                                       pol.data_ptr(), cabi.ptr(tp), cabi.stream_ptr()),
                    "lz_tree_backpropagate_gumbel")

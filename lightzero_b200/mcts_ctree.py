@@ -21,11 +21,20 @@ import numpy as np
 import torch
 
 from . import cabi, ez_tree, gmz_tree, mz_tree
-from .efficientzero_model import EfficientZeroModel
-from .efficientzero_model_mlp import EfficientZeroModelMLP
-from .muzero_model import MuZeroModel
-from .muzero_model_mlp import MuZeroModelMLP
+from .model_base import LzModel
 from .scaling_transform import DiscreteSupport, InverseScalarTransform
+
+
+def _dev_f32(x, dev):
+    """A latent or hidden-state batch (np.ndarray or tensor) as a contiguous float32 tensor on dev."""
+    if isinstance(x, torch.Tensor):
+        return x.to(dev, torch.float32, non_blocking=True).contiguous()
+    return torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32)).to(dev, non_blocking=True)
+
+
+def _value_prefix_model(model):
+    """True for a lightzero_b200 EfficientZero model, False for a MuZero one, None for any other object (step-wise)."""
+    return model.value_prefix if isinstance(model, LzModel) else None
 
 
 class ConfigDict(dict):
@@ -96,50 +105,46 @@ class MuZeroMCTSCtree(object):
     def search(self, roots: "mz_tree.Roots", model, latent_state_roots, to_play_batch: Union[int, List[Any]],
                task_id: Optional[int] = None) -> None:
         """mcts_ctree.py:267-368.  ``latent_state_roots``: np.ndarray or CUDA tensor [B,C,H,W]."""
-        S = int(self._cfg.num_simulations)
-        roots._materialize(S, self._params())     # reset + prepare on device, MinMax stats fresh (:291-292)
-        t = roots._tree
-        dev = roots.device
-        if isinstance(latent_state_roots, torch.Tensor):
-            lat = latent_state_roots.to(dev, torch.float32, non_blocking=True).contiguous()
-        else:
-            lat = torch.from_numpy(np.ascontiguousarray(latent_state_roots, dtype=np.float32)).to(dev, non_blocking=True)
-        if isinstance(model, (EfficientZeroModel, EfficientZeroModelMLP)):
+        family = _value_prefix_model(model)
+        if family:
             raise TypeError(f"MuZeroMCTSCtree.search: an {type(model).__name__} needs EfficientZeroMCTSCtree")
-        if isinstance(model, (MuZeroModel, MuZeroModelMLP)):
-            q = t.search_for(model, S)
-            with torch.cuda.device(dev):
-                cabi.check(t.lib.lz_search_run(q, lat.data_ptr(), int(self.deterministic), cabi.stream_ptr()),
-                           "lz_search_run")
-            self.last_num_kernels = t.lib.lz_search_num_kernels(q)
+        S = int(self._cfg.num_simulations)
+        roots._materialize(S, self._params(), self.deterministic)     # reset + prepare on device, MinMax stats fresh (:291-292)
+        t = roots._tree
+        lat = _dev_f32(latent_state_roots, roots.device)
+        if family is None:
+            self._search_stepwise(roots, model, lat, S)
             return
-        self._search_stepwise(roots, model, lat, S)
+        q = t.search_for(model, S)
+        with torch.cuda.device(roots.device):
+            cabi.check(t.lib.lz_search_run(q, lat.data_ptr(), int(self.deterministic), cabi.stream_ptr()), "lz_search_run")
+        self.last_num_kernels = t.lib.lz_search_num_kernels(q)
 
     def search_with_reuse(self, roots: "mz_tree.Roots", model, latent_state_roots, to_play_batch: Union[int, List[Any]],
                           true_action_list=None, reuse_value_list=None):
         """mcts_ctree.py:370-468 (ReZero): the root child of ``true_action`` is scored with the stored ``reuse_value`` and the
         descent stops there.  Returns ``(length, average_infer)`` like the reference: how many trees needed the network in
         the last simulation and on average.  One CUDA graph with a ``lightzero_b200`` model."""
-        S = int(self._cfg.num_simulations)
-        roots._materialize(S, self._params())
-        t = roots._tree
-        dev = roots.device
-        if not isinstance(model, (MuZeroModel, MuZeroModelMLP)) or isinstance(model, EfficientZeroModel):
+        if _value_prefix_model(model) is not False:
             raise NotImplementedError("search_with_reuse is fused only: pass a lightzero_b200 MuZeroModel / MuZeroModelMLP "
                                       "(or drive mz_tree.batch_traverse_with_reuse / batch_backpropagate_with_reuse yourself)")
-        if isinstance(latent_state_roots, torch.Tensor):
-            lat = latent_state_roots.to(dev, torch.float32, non_blocking=True).contiguous()
-        else:
-            lat = torch.from_numpy(np.ascontiguousarray(latent_state_roots, dtype=np.float32)).to(dev, non_blocking=True)
-        B = roots.num
+        S = int(self._cfg.num_simulations)
+        lat = _dev_f32(latent_state_roots, roots.device)
+        return self._run_with_reuse(roots, model, S, (), true_action_list, reuse_value_list,
+                                    lambda lib, q, ta, rv, counts, s: cabi.check(
+                                        lib.lz_search_run_with_reuse(q, lat.data_ptr(), ta, rv, counts, s), "lz_search_run_with_reuse"))
+
+    def _run_with_reuse(self, roots, model, S, mode, true_action_list, reuse_value_list, run):
+        """The fused search_with_reuse of either tree family: ``run(lib, q, true_action, reuse_value, counts, stream)`` runs
+        the search on the staged device pointers; returns the reference's ``(length, average_infer)``."""
+        roots._materialize(S, self._params(), self.deterministic)     # the reference draws rand() % len(ties) (cnode.cpp:610-640)
+        t, dev, B = roots._tree, roots.device, roots.num
         ta = mz_tree._to_dev(true_action_list, torch.int32, dev, (B,))
         rv = mz_tree._to_dev(reuse_value_list, torch.float32, dev, (B,))
         counts = torch.empty(S, dtype=torch.int32, device=dev)
-        cabi.check(t.lib.lz_tree_set_tiebreak(t.h, int(self.deterministic)), "lz_tree_set_tiebreak")   # the reference draws rand() % len(ties) (cnode.cpp:610-640)
-        q = t.search_for(model, S)
+        q = t.search_for(model, S, mode)
         with torch.cuda.device(dev):
-            cabi.check(t.lib.lz_search_run_with_reuse(q, lat.data_ptr(), ta.data_ptr(), rv.data_ptr(), counts.data_ptr(),
-                                                      cabi.stream_ptr()), "lz_search_run_with_reuse")
+            run(t.lib, q, ta.data_ptr(), rv.data_ptr(), counts.data_ptr(), cabi.stream_ptr())
         self.last_num_kernels = t.lib.lz_search_num_kernels(q)
         c = counts.cpu().numpy()
         return int(c[-1]), float(c.sum()) / S
@@ -159,7 +164,8 @@ class MuZeroMCTSCtree(object):
         vr, rr = rng("value_support_range"), rng("reward_support_range")
         self._inv_reward = self._inv if vr == rr else InverseScalarTransform(DiscreteSupport(*rr, device=dev))
 
-    def _search_stepwise(self, roots, model, lat, S):
+    def _search_stepwise(self, roots, model, lat, S, gumbel=False):
+        """The search driven one simulation at a time around any model object (gumbel: on Gumbel trees)."""
         t = roots._tree
         dev = roots.device
         self._make_inverse_transforms(dev)
@@ -167,22 +173,25 @@ class MuZeroMCTSCtree(object):
         pool = torch.empty((S + 1,) + tuple(lat.shape), device=dev, dtype=torch.float32)
         pool[0] = lat
         rows = torch.arange(B, device=dev)
+        backprop = "lz_tree_backpropagate_gumbel" if gumbel else "lz_tree_backpropagate"
         with torch.no_grad(), torch.cuda.device(dev):
             if hasattr(model, "eval"):
                 model.eval()
             for sim in range(S):
-                cabi.check(t.lib.lz_tree_traverse(t.h, int(self.deterministic), t.ix.data_ptr(), t.iy.data_ptr(),
-                                                  t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(),
-                                                  cabi.stream_ptr()), "lz_tree_traverse")
+                leaves = (t.ix.data_ptr(), t.iy.data_ptr(), t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(),
+                          cabi.stream_ptr())
+                if gumbel:
+                    cabi.check(t.lib.lz_tree_traverse_gumbel(t.h, *leaves), "lz_tree_traverse_gumbel")
+                else:
+                    cabi.check(t.lib.lz_tree_traverse(t.h, int(self.deterministic), *leaves), "lz_tree_traverse")
                 latent_states = pool[t.ix.long(), rows]                       # mcts_ctree.py:323-324 on device
                 out = model.recurrent_inference(latent_states, t.action.long())
                 pool[sim + 1] = out.latent_state
                 value = self._inv(out.value).reshape(-1).contiguous()        # :349 (value support)
                 reward = self._inv_reward(out.reward).reshape(-1).contiguous()      # :350 (reward support)
                 pol = out.policy_logits.to(torch.float32).contiguous()
-                cabi.check(t.lib.lz_tree_backpropagate(t.h, sim + 1, reward.data_ptr(), value.data_ptr(),
-                                                       pol.data_ptr(), None, cabi.stream_ptr()),
-                           "lz_tree_backpropagate")
+                cabi.check(getattr(t.lib, backprop)(t.h, sim + 1, reward.data_ptr(), value.data_ptr(), pol.data_ptr(), None,
+                                                    cabi.stream_ptr()), backprop)
 
 
 class EfficientZeroMCTSCtree(MuZeroMCTSCtree):
@@ -213,27 +222,16 @@ class EfficientZeroMCTSCtree(MuZeroMCTSCtree):
         S, H = int(self._cfg.num_simulations), int(self._cfg.lstm_horizon_len)
         assert H > 0                                   # mcts_ctree.py:857
         roots._ez, roots._lstm_horizon = True, H
-        roots._materialize(S, self._params())
+        roots._materialize(S, self._params(), self.deterministic)
         t = roots._tree
-        dev = roots.device
-        cabi.check(t.lib.lz_tree_set_tiebreak(t.h, int(self.deterministic)), "lz_tree_set_tiebreak")
-
-        def dev_f32(x):
-            if isinstance(x, torch.Tensor):
-                return x.to(dev, torch.float32, non_blocking=True).contiguous()
-            return torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32)).to(dev, non_blocking=True)
-        lat = dev_f32(latent_state_roots)
-        B = roots.num
-        h0 = dev_f32(reward_hidden_state_roots[0]).reshape(B, -1)
-        h1 = dev_f32(reward_hidden_state_roots[1]).reshape(B, -1)
-        if isinstance(model, (EfficientZeroModel, EfficientZeroModelMLP)):
-            q = t.search_for(model, S, (1, H))
-            with torch.cuda.device(dev):
-                cabi.check(t.lib.lz_search_run_ez(q, lat.data_ptr(), h0.data_ptr(), h1.data_ptr(), cabi.stream_ptr()),
-                           "lz_search_run_ez")
-            self.last_num_kernels = t.lib.lz_search_num_kernels(q)
+        lat, h0, h1 = self._ez_inputs(roots, latent_state_roots, reward_hidden_state_roots)
+        if not _value_prefix_model(model):
+            self._search_stepwise_ez(roots, model, lat, h0, h1, S, H)
             return
-        self._search_stepwise_ez(roots, model, lat, h0, h1, S, H)
+        q = t.search_for(model, S, (1, H))
+        with torch.cuda.device(roots.device):
+            cabi.check(t.lib.lz_search_run_ez(q, lat.data_ptr(), h0.data_ptr(), h1.data_ptr(), cabi.stream_ptr()), "lz_search_run_ez")
+        self.last_num_kernels = t.lib.lz_search_num_kernels(q)
 
     def search_with_reuse(self, roots: "ez_tree.Roots", model, latent_state_roots, reward_hidden_state_roots,
                           to_play_batch: Union[int, List[Any]], true_action_list=None, reuse_value_list=None):
@@ -242,33 +240,21 @@ class EfficientZeroMCTSCtree(MuZeroMCTSCtree):
         ``ez_tree.batch_traverse_with_reuse`` / ``batch_backpropagate_with_reuse`` themselves."""
         S, H = int(self._cfg.num_simulations), int(self._cfg.lstm_horizon_len)
         assert H > 0
-        if not isinstance(model, (EfficientZeroModel, EfficientZeroModelMLP)):
+        if not _value_prefix_model(model):
             raise NotImplementedError("EfficientZeroMCTSCtree.search_with_reuse is fused only: pass a lightzero_b200 EfficientZeroModel "
                                       "or EfficientZeroModelMLP")
         roots._ez, roots._lstm_horizon = True, H
-        roots._materialize(S, self._params())
-        t = roots._tree
-        dev = roots.device
-        cabi.check(t.lib.lz_tree_set_tiebreak(t.h, int(self.deterministic)), "lz_tree_set_tiebreak")
+        lat, h0, h1 = self._ez_inputs(roots, latent_state_roots, reward_hidden_state_roots)
+        return self._run_with_reuse(roots, model, S, (1, H), true_action_list, reuse_value_list,
+                                    lambda lib, q, ta, rv, counts, s: cabi.check(lib.lz_search_run_ez_with_reuse(
+                                        q, lat.data_ptr(), h0.data_ptr(), h1.data_ptr(), ta, rv, counts, s), "lz_search_run_ez_with_reuse"))
 
-        def dev_f32(x):
-            if isinstance(x, torch.Tensor):
-                return x.to(dev, torch.float32, non_blocking=True).contiguous()
-            return torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32)).to(dev, non_blocking=True)
-        lat = dev_f32(latent_state_roots)
-        B = roots.num
-        h0 = dev_f32(reward_hidden_state_roots[0]).reshape(B, -1)
-        h1 = dev_f32(reward_hidden_state_roots[1]).reshape(B, -1)
-        ta = mz_tree._to_dev(true_action_list, torch.int32, dev, (B,))
-        rv = mz_tree._to_dev(reuse_value_list, torch.float32, dev, (B,))
-        counts = torch.empty(S, dtype=torch.int32, device=dev)
-        q = t.search_for(model, S, (1, H))
-        with torch.cuda.device(dev):
-            cabi.check(t.lib.lz_search_run_ez_with_reuse(q, lat.data_ptr(), h0.data_ptr(), h1.data_ptr(), ta.data_ptr(), rv.data_ptr(),
-                                                         counts.data_ptr(), cabi.stream_ptr()), "lz_search_run_ez_with_reuse")
-        self.last_num_kernels = t.lib.lz_search_num_kernels(q)
-        c = counts.cpu().numpy()
-        return int(c[-1]), float(c.sum()) / S
+    @staticmethod
+    def _ez_inputs(roots, latent_state_roots, reward_hidden_state_roots):
+        """The roots' latents and LSTM state (h, c) as float32 on the device, the state as [B, lstm_hidden_size]."""
+        dev, B = roots.device, roots.num
+        return (_dev_f32(latent_state_roots, dev), _dev_f32(reward_hidden_state_roots[0], dev).reshape(B, -1),
+                _dev_f32(reward_hidden_state_roots[1], dev).reshape(B, -1))
 
     def _search_stepwise_ez(self, roots, model, lat, h0, h1, S, H):
         t = roots._tree
@@ -322,7 +308,7 @@ class UniZeroMCTSCtree(MuZeroMCTSCtree):
     def search(self, roots: "mz_tree.Roots", model, latent_state_roots, to_play_batch: Union[int, List[Any]],
                timestep: Union[int, List[Any]] = None, task_id: Optional[int] = None) -> dict:
         S = int(self._cfg.num_simulations)
-        roots._materialize(S, self._params())
+        roots._materialize(S, self._params(), self.deterministic)
         t = roots._tree
         dev = roots.device
         self._make_inverse_transforms(dev)
@@ -394,7 +380,8 @@ class GumbelMuZeroMCTSCtree(MuZeroMCTSCtree):
 
     def search(self, roots: "gmz_tree.Roots", model, latent_state_roots, to_play_batch: Union[int, List[Any]]) -> None:
         """mcts_ctree.py:1076-1172.  ``latent_state_roots``: np.ndarray or CUDA tensor."""
-        if isinstance(model, (EfficientZeroModel, EfficientZeroModelMLP)):
+        family = _value_prefix_model(model)
+        if family:
             raise TypeError(f"GumbelMuZeroMCTSCtree.search: the Gumbel search runs MuZero models, not an {type(model).__name__}")
         S = int(self._cfg.num_simulations)
         if roots._pending is None:
@@ -403,38 +390,11 @@ class GumbelMuZeroMCTSCtree(MuZeroMCTSCtree):
         m = roots._pending["A"] if m is None else int(m)
         roots._materialize_gumbel((m, S), self._params())   # reset + prepare on device: a fresh search
         t = roots._tree
-        dev = roots.device
-        if isinstance(latent_state_roots, torch.Tensor):
-            lat = latent_state_roots.to(dev, torch.float32, non_blocking=True).contiguous()
-        else:
-            lat = torch.from_numpy(np.ascontiguousarray(latent_state_roots, dtype=np.float32)).to(dev, non_blocking=True)
-        if isinstance(model, (MuZeroModel, MuZeroModelMLP)):
-            q = t.search_for(model, S, ("gumbel",))
-            with torch.cuda.device(dev):
-                cabi.check(t.lib.lz_search_run_gumbel(q, lat.data_ptr(), cabi.stream_ptr()), "lz_search_run_gumbel")
-            self.last_num_kernels = t.lib.lz_search_num_kernels(q)
+        lat = _dev_f32(latent_state_roots, roots.device)
+        if family is None:
+            self._search_stepwise(roots, model, lat, S, gumbel=True)
             return
-        self._search_stepwise_gumbel(roots, model, lat, S)
-
-    def _search_stepwise_gumbel(self, roots, model, lat, S):
-        t = roots._tree
-        dev = roots.device
-        self._make_inverse_transforms(dev)
-        B = roots.num
-        pool = torch.empty((S + 1,) + tuple(lat.shape), device=dev, dtype=torch.float32)
-        pool[0] = lat
-        rows = torch.arange(B, device=dev)
-        with torch.no_grad(), torch.cuda.device(dev):
-            if hasattr(model, "eval"):
-                model.eval()
-            for sim in range(S):
-                cabi.check(t.lib.lz_tree_traverse_gumbel(t.h, t.ix.data_ptr(), t.iy.data_ptr(), t.action.data_ptr(),
-                                                         t.search_len.data_ptr(), t.vtp.data_ptr(), cabi.stream_ptr()),
-                           "lz_tree_traverse_gumbel")
-                out = model.recurrent_inference(pool[t.ix.long(), rows], t.action.long())
-                pool[sim + 1] = out.latent_state
-                value = self._inv(out.value).reshape(-1).contiguous()
-                reward = self._inv_reward(out.reward).reshape(-1).contiguous()
-                pol = out.policy_logits.to(torch.float32).contiguous()
-                cabi.check(t.lib.lz_tree_backpropagate_gumbel(t.h, sim + 1, reward.data_ptr(), value.data_ptr(), pol.data_ptr(),
-                                                              None, cabi.stream_ptr()), "lz_tree_backpropagate_gumbel")
+        q = t.search_for(model, S, ("gumbel",))
+        with torch.cuda.device(roots.device):
+            cabi.check(t.lib.lz_search_run_gumbel(q, lat.data_ptr(), cabi.stream_ptr()), "lz_search_run_gumbel")
+        self.last_num_kernels = t.lib.lz_search_num_kernels(q)

@@ -10,6 +10,7 @@ Differences a caller can observe:
   * ``MinMaxStatsList`` is bookkeeping only -- min/max live inside the tree and are reset when the
     Roots are (re)prepared, i.e. once per search like mcts_ctree.py:291-292.
 """
+import contextlib
 import threading
 from typing import List, Optional
 
@@ -58,6 +59,20 @@ class TreeHandle:
                 cabi.check(self.lib.lz_tree_set_params(self.h, *p), "lz_tree_set_params")
             self.params = p
 
+    def set_mode(self, mode=(), deterministic: bool = True, gumbel=(0, 0)):
+        """Puts the tree in one holder's whole mode: ``mode`` () for MuZero or (1, lstm_horizon_len) for EfficientZero
+        value-prefix trees (the ``search_for`` mode), ``gumbel`` (max_num_considered_actions, num_simulations) for a Gumbel
+        tree, and the tie rule of the EfficientZero and *_with_reuse descents (``deterministic``: the first maximum, else the
+        uniform draw).  The mode is C state that outlives its holder, so every acquirer sets all of it, once: a change bumps
+        the tree's generation and re-captures its search graphs (csrc/search.cu)."""
+        if gumbel[1]:       # a Gumbel tree is a MuZero tree
+            cabi.check(self.lib.lz_tree_set_ez(self.h, 0, 5), "lz_tree_set_ez")
+            cabi.check(self.lib.lz_tree_set_gumbel(self.h, int(gumbel[0]), int(gumbel[1])), "lz_tree_set_gumbel")
+        else:
+            cabi.check(self.lib.lz_tree_set_gumbel(self.h, 0, 0), "lz_tree_set_gumbel")
+            cabi.check(self.lib.lz_tree_set_ez(self.h, *(mode or (0, 5))), "lz_tree_set_ez")
+        cabi.check(self.lib.lz_tree_set_tiebreak(self.h, int(bool(deterministic))), "lz_tree_set_tiebreak")
+
     def release(self):
         """Hands the tree back to the pool.  The holder's work on it may still be queued on the current stream (a
         search_batch(read_back=False), Roots.clear() before the read-outs ran): the event recorded here orders the next
@@ -104,6 +119,19 @@ def acquire_tree(device, B, A, max_sims) -> TreeHandle:
         h.busy = True
         _tree_pool[key].append(h)
         return h
+
+
+@contextlib.contextmanager
+def held_tree(device, B, A, max_sims, params, mode=(), deterministic: bool = True, gumbel=(0, 0)):
+    """A pooled tree with these parameters and this whole mode (TreeHandle.set_mode) for the length of one call, released
+    at its end even when the call raises."""
+    t = acquire_tree(device, B, A, max_sims)
+    try:
+        t.set_params(*params)
+        t.set_mode(mode, deterministic, gumbel)
+        yield t
+    finally:
+        t.release()
 
 
 def drop_model_searches(serial: int):
@@ -177,6 +205,7 @@ class Roots:
             assert len(self._legal_lists) == root_num
         self._pending = None      # prepare() arguments until the tree is materialised
         self._ez, self._lstm_horizon = False, 5     # EfficientZero value-prefix semantics (set by ez_tree.Roots)
+        self._deterministic = True     # tie rule of the EfficientZero / *_with_reuse descents (the mirrors: first maximum)
         self._tree: Optional[TreeHandle] = None
         self._delta_reset = None
 
@@ -272,26 +301,34 @@ class Roots:
             self._materialize(DEFAULT_MAX_SIMS)
         return self._tree
 
-    def _materialize(self, max_sims: int, params=None):
+    def _materialize(self, max_sims: int, params=None, deterministic=None):
+        """Reset + prepare on device in a pooled tree of at least max_sims simulations.  ``deterministic``: the tie rule the
+        holder searches with (MCTS searches pass their own); None keeps these roots' rule."""
+        t = self._acquire(max_sims, params, deterministic)
+        p = self._pending
+        with torch.cuda.device(self.device):
+            s = cabi.stream_ptr()
+            self._reset_tree(t, s)
+            cabi.check(t.lib.lz_tree_prepare(t.h, p["logits"].data_ptr(), cabi.ptr(p["noise"]), p["w"],
+                                             cabi.ptr(p["rewards"]), cabi.ptr(p["to_play"]), s), "lz_tree_prepare")
+
+    def _acquire(self, max_sims, params, deterministic, gumbel=(0, 0)) -> TreeHandle:
+        """This Roots' pooled tree, at least max_sims deep and in its whole mode (TreeHandle.set_mode)."""
         if self._pending is None:
             raise RuntimeError("Roots: prepare()/prepare_no_noise() has not been called")
-        p = self._pending
-        A = p["A"]
+        A = self._pending["A"]
         if self._tree is not None and (self._tree.max_sims < max_sims or self._tree.A != A):
             self.clear()
         if self._tree is None:
             self._tree = acquire_tree(self.device, self.root_num, A, max_sims)
+        if deterministic is not None:
+            self._deterministic = bool(deterministic)
         t = self._tree
         if params is not None:
             t.set_params(*params)
-        s = None
         with torch.cuda.device(self.device):
-            s = cabi.stream_ptr()
-            cabi.check(t.lib.lz_tree_set_gumbel(t.h, 0, 0), "lz_tree_set_gumbel")    # a pooled tree a Gumbel collect left behind
-            cabi.check(t.lib.lz_tree_set_ez(t.h, int(self._ez), int(self._lstm_horizon)), "lz_tree_set_ez")
-            self._reset_tree(t, s)
-            cabi.check(t.lib.lz_tree_prepare(t.h, p["logits"].data_ptr(), cabi.ptr(p["noise"]), p["w"],
-                                             cabi.ptr(p["rewards"]), cabi.ptr(p["to_play"]), s), "lz_tree_prepare")
+            t.set_mode((1, int(self._lstm_horizon)) if self._ez else (), self._deterministic, gumbel)
+        return t
 
     def _reset_tree(self, t, s):
         """lz_tree_reset / lz_tree_reset_mask of tree t to these roots' legal actions, on stream s."""
@@ -317,38 +354,44 @@ class Roots:
                     self._keep = (dl, dn)
 
 
+def _traversed(roots: Roots, results: ResultsWrapper, return_tensors: bool):
+    """What every batch_traverse returns once its descent is queued: (latent_state_index_in_search_path,
+    latent_state_index_in_batch, last_actions, virtual_to_play_batch) as lists, or the device tensors."""
+    results._roots = roots
+    t = roots._tree
+    if return_tensors:
+        return t.ix, t.iy, t.action, t.vtp
+    return tuple(x.tolist() for x in torch.stack((t.ix, t.iy, t.action, t.vtp)).cpu().numpy())
+
+
+def _backup_inputs(results: ResultsWrapper, value_prefixs, values, policies, to_play_batch):
+    """The inputs every batch_backpropagate stages on the device -> (roots, tree, rewards or value prefixes, values,
+    policy logits, to_play or None)."""
+    roots = results._roots
+    B, A, dev = roots.root_num, roots._tree.A, roots.device
+    return (roots, roots._tree, _to_dev(value_prefixs, torch.float32, dev, (B,)), _to_dev(values, torch.float32, dev, (B,)),
+            _to_dev(policies, torch.float32, dev, (B, A)), _to_dev(to_play_batch, torch.int32, dev, (B,)))
+
+
 def batch_traverse(roots: Roots, pb_c_base: int, pb_c_init: float, discount_factor: float,
                    min_max_stats_lst: MinMaxStatsList, results: ResultsWrapper, virtual_to_play_batch,
                    deterministic: bool = False, return_tensors: bool = False):
     """mz_tree.pyx:94-99 -> (latent_state_index_in_search_path, latent_state_index_in_batch, last_actions,
     virtual_to_play_batch)."""
-    if roots._tree is None:
-        roots._materialize(DEFAULT_MAX_SIMS)
-    t = roots._tree
+    t = roots._need_tree()
     t.set_params(pb_c_base, pb_c_init, discount_factor, min_max_stats_lst.value_delta_max)
     with torch.cuda.device(roots.device):
         cabi.check(t.lib.lz_tree_traverse(t.h, int(bool(deterministic)), t.ix.data_ptr(), t.iy.data_ptr(),
                                           t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(),
                                           cabi.stream_ptr()), "lz_tree_traverse")
-    results._roots = roots
-    if return_tensors:
-        return t.ix, t.iy, t.action, t.vtp
-    packed = torch.stack((t.ix, t.iy, t.action, t.vtp)).cpu().numpy()
-    return packed[0].tolist(), packed[1].tolist(), packed[2].tolist(), packed[3].tolist()
+    return _traversed(roots, results, return_tensors)
 
 
 def batch_backpropagate(current_latent_state_index: int, discount_factor: float, value_prefixs, values, policies,
                         min_max_stats_lst: MinMaxStatsList, results: ResultsWrapper, to_play_batch):
     """mz_tree.pyx:73-82"""
-    roots = results._roots
-    t = roots._tree
-    B, A = roots.root_num, t.A
-    dev = roots.device
-    rew = _to_dev(value_prefixs, torch.float32, dev, (B,))
-    val = _to_dev(values, torch.float32, dev, (B,))
-    pol = _to_dev(policies, torch.float32, dev, (B, A))
-    tp = _to_dev(to_play_batch, torch.int32, dev, (B,)) if to_play_batch is not None else None
-    with torch.cuda.device(dev):
+    roots, t, rew, val, pol, tp = _backup_inputs(results, value_prefixs, values, policies, to_play_batch)
+    with torch.cuda.device(roots.device):
         cabi.check(t.lib.lz_tree_backpropagate(t.h, int(current_latent_state_index), rew.data_ptr(), val.data_ptr(),
                                                pol.data_ptr(), cabi.ptr(tp), cabi.stream_ptr()),
                    "lz_tree_backpropagate")
@@ -360,9 +403,7 @@ def batch_traverse_with_reuse(roots: Roots, pb_c_base: int, pb_c_init: float, di
                               true_action, reuse_value, return_tensors: bool = False):
     """mz_tree.pyx batch_traverse_with_reuse (cnode.cpp:828-932): ``latent_state_index_in_search_path`` is -1 for trees
     that stopped on an already expanded child of the root (no inference needed)."""
-    if roots._tree is None:
-        roots._materialize(DEFAULT_MAX_SIMS)
-    t = roots._tree
+    t = roots._need_tree()
     t.set_params(pb_c_base, pb_c_init, discount_factor, min_max_stats_lst.value_delta_max)
     dev = roots.device
     ta = _to_dev(true_action, torch.int32, dev, (roots.root_num,))
@@ -371,12 +412,8 @@ def batch_traverse_with_reuse(roots: Roots, pb_c_base: int, pb_c_init: float, di
         cabi.check(t.lib.lz_tree_traverse_with_reuse(t.h, ta.data_ptr(), rv.data_ptr(), t.ix.data_ptr(), t.iy.data_ptr(),
                                                      t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(),
                                                      cabi.stream_ptr()), "lz_tree_traverse_with_reuse")
-    results._roots = roots
     t._keep = (ta, rv)
-    if return_tensors:
-        return t.ix, t.iy, t.action, t.vtp
-    packed = torch.stack((t.ix, t.iy, t.action, t.vtp)).cpu().numpy()
-    return packed[0].tolist(), packed[1].tolist(), packed[2].tolist(), packed[3].tolist()
+    return _traversed(roots, results, return_tensors)
 
 
 def batch_backpropagate_with_reuse(current_latent_state_index: int, discount_factor: float, value_prefixs, values, policies,
@@ -404,8 +441,8 @@ def batch_backpropagate_with_reuse(current_latent_state_index: int, discount_fac
     rew, val, pol = scatter(value_prefixs, ()), scatter(values, ()), scatter(policies, (A,))
     rv = _to_dev(reuse_value_lst, torch.float32, dev, (B,))
     rk = torch.from_numpy(rank.astype(np.int32)).to(dev)
-    tp = _to_dev(to_play_batch, torch.int32, dev, (B,)) if to_play_batch is not None else None
-    rs = _to_dev(_is_reset_list, torch.int32, dev, (B,)) if _is_reset_list is not None else None
+    tp = _to_dev(to_play_batch, torch.int32, dev, (B,))
+    rs = _to_dev(_is_reset_list, torch.int32, dev, (B,))
     with torch.cuda.device(dev):
         cabi.check(t.lib.lz_tree_backpropagate_with_reuse(t.h, int(current_latent_state_index), rew.data_ptr(), val.data_ptr(),
                                                           pol.data_ptr(), rv.data_ptr(), rk.data_ptr(), cabi.ptr(rs), cabi.ptr(tp),

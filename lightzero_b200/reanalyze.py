@@ -19,7 +19,9 @@ from typing import List, Optional, Sequence
 import numpy as np
 import torch
 
-from .mcts_ctree import EfficientZeroMCTSCtree, MuZeroMCTSCtree
+from . import cabi, mz_tree
+from .mcts_ctree import EfficientZeroMCTSCtree, GumbelMuZeroMCTSCtree, MuZeroMCTSCtree, UniZeroMCTSCtree
+from .model_base import LzModel
 
 
 def compute_target_policy_reanalyzed(
@@ -144,14 +146,6 @@ def compute_target_policy_reanalyzed_rezero(
     to those two statistics.  Ties: the first search by the config's ``deterministic`` (MuZero), the reuse searches and every
     EfficientZero search by the first maximum (the reference's rand() % len(ties) with rand() == 0).  ``noises`` [N * length, A]
     (legal order) are drawn with np.random.dirichlet like the reference only when None."""
-    from . import mz_tree
-    from .efficientzero_model import EfficientZeroModel
-    from .efficientzero_model_mlp import EfficientZeroModelMLP
-    from .mcts_ctree import GumbelMuZeroMCTSCtree, UniZeroMCTSCtree
-    from .muzero_model import MuZeroModel
-    from .muzero_model_mlp import MuZeroModelMLP
-    from . import cabi
-
     L = int(length)
     if L < 1:
         raise ValueError(f"compute_target_policy_reanalyzed_rezero: length must be >= 1 (got {length}); the reference builds no "
@@ -160,12 +154,10 @@ def compute_target_policy_reanalyzed_rezero(
         raise TypeError(f"compute_target_policy_reanalyzed_rezero: {type(mcts).__name__} has no ReZero sweep "
                         "(MuZeroMCTSCtree or EfficientZeroMCTSCtree)")
     ez = isinstance(mcts, EfficientZeroMCTSCtree)
-    ez_model = isinstance(model, (EfficientZeroModel, EfficientZeroModelMLP))
-    if ez and not ez_model:
-        raise TypeError(f"EfficientZeroMCTSCtree: the ReZero sweep needs an EfficientZeroModel or EfficientZeroModelMLP, "
-                        f"not a {type(model).__name__}")
-    if not ez and (ez_model or not isinstance(model, (MuZeroModel, MuZeroModelMLP))):
-        raise TypeError(f"MuZeroMCTSCtree: the ReZero sweep needs a MuZeroModel or MuZeroModelMLP, not a {type(model).__name__}")
+    if not isinstance(model, LzModel) or model.value_prefix != ez:
+        need = "EfficientZeroMCTSCtree: the ReZero sweep needs an EfficientZeroModel or EfficientZeroModelMLP" if ez else \
+            "MuZeroMCTSCtree: the ReZero sweep needs a MuZeroModel or MuZeroModelMLP"
+        raise TypeError(f"{need}, not a {type(model).__name__}")
     if ez and not mcts.deterministic:
         raise ValueError("EfficientZeroMCTSCtree: the ReZero sweep breaks every tie by the first maximum (the reference's "
                          "EfficientZero tree has no other rule); deterministic=False is not available")
@@ -182,37 +174,32 @@ def compute_target_policy_reanalyzed_rezero(
         noises = np.stack([np.random.dirichlet([cfg.root_dirichlet_alpha] * A).astype(np.float32) for _ in range(rows)])
     dev = model.device
     H = int(cfg.lstm_horizon_len) if ez else 5
-    t = mz_tree.acquire_tree(dev, N, A, S)
-    try:
-        t.set_params(*mcts._params())
-        cabi.check(t.lib.lz_tree_set_gumbel(t.h, 0, 0), "lz_tree_set_gumbel")     # a pooled tree a Gumbel collect left behind
-        cabi.check(t.lib.lz_tree_set_ez(t.h, int(ez), H), "lz_tree_set_ez")
-        q = t.search_for(model, S, (1, H) if ez else ())
-        with torch.cuda.device(dev):
-            s = cabi.stream_ptr()
-            obs = mz_tree._to_dev(policy_obs, torch.float32, dev)
-            mask = mz_tree._to_dev(action_mask, torch.uint8, dev, (rows, A))
-            tp = mz_tree._to_dev(np.asarray(to_play, np.int32), torch.int32, dev, (rows,))
-            ta = mz_tree._to_dev(np.asarray(true_action, np.int32), torch.int32, dev, (rows,))
-            pm = mz_tree._to_dev(np.asarray(policy_mask, np.uint8), torch.uint8, dev, (rows,))
-            nz = mz_tree._to_dev(noises, torch.float32, dev, (rows, A)) if reanalyze_noise else None
-            targets = torch.empty((N, L, A), dtype=torch.float64, device=dev)
-            visits = torch.empty((N, L, A), dtype=torch.float64, device=dev)
-            values = torch.empty((N, L), dtype=torch.float32, device=dev)
-            nreuse = L - 1 if reuse_search else 0
-            counts = torch.empty((nreuse, S), dtype=torch.int32, device=dev)
-            head = (q, L, int(bool(reuse_search)), int(mini_infer_size), obs.data_ptr(), None, None, mask.data_ptr(),
-                    tp.data_ptr(), ta.data_ptr(), pm.data_ptr(), cabi.ptr(nz), float(cfg.root_noise_weight))
-            tail = (int(action_type != "fixed_action_space"), targets.data_ptr(), values.data_ptr(), visits.data_ptr(),
-                    counts.data_ptr() if nreuse else None, s)
-            if ez:
-                cabi.check(t.lib.lz_rezero_reanalyze_ez(*head, *tail), "lz_rezero_reanalyze_ez")
-            else:
-                cabi.check(t.lib.lz_rezero_reanalyze(*head, int(mcts.deterministic), *tail), "lz_rezero_reanalyze")
-            mcts.last_num_kernels = t.lib.lz_search_num_kernels(q)
-            out, vis, val, cnt = targets.cpu().numpy(), visits.cpu().numpy(), values.cpu().numpy(), counts.cpu().numpy()
-    finally:
-        t.release()
+    mode = (1, H) if ez else ()
+    # the sweep's tie rule is the one lz_rezero_reanalyze* sets: the first maximum
+    with torch.cuda.device(dev), mz_tree.held_tree(dev, N, A, S, mcts._params(), mode) as t:
+        q = t.search_for(model, S, mode)
+        s = cabi.stream_ptr()
+        obs = mz_tree._to_dev(policy_obs, torch.float32, dev)
+        mask = mz_tree._to_dev(action_mask, torch.uint8, dev, (rows, A))
+        tp = mz_tree._to_dev(np.asarray(to_play, np.int32), torch.int32, dev, (rows,))
+        ta = mz_tree._to_dev(np.asarray(true_action, np.int32), torch.int32, dev, (rows,))
+        pm = mz_tree._to_dev(np.asarray(policy_mask, np.uint8), torch.uint8, dev, (rows,))
+        nz = mz_tree._to_dev(noises, torch.float32, dev, (rows, A)) if reanalyze_noise else None
+        targets = torch.empty((N, L, A), dtype=torch.float64, device=dev)
+        visits = torch.empty((N, L, A), dtype=torch.float64, device=dev)
+        values = torch.empty((N, L), dtype=torch.float32, device=dev)
+        nreuse = L - 1 if reuse_search else 0
+        counts = torch.empty((nreuse, S), dtype=torch.int32, device=dev)
+        head = (q, L, int(bool(reuse_search)), int(mini_infer_size), obs.data_ptr(), None, None, mask.data_ptr(),
+                tp.data_ptr(), ta.data_ptr(), pm.data_ptr(), cabi.ptr(nz), float(cfg.root_noise_weight))
+        tail = (int(action_type != "fixed_action_space"), targets.data_ptr(), values.data_ptr(), visits.data_ptr(),
+                counts.data_ptr() if nreuse else None, s)
+        if ez:
+            cabi.check(t.lib.lz_rezero_reanalyze_ez(*head, *tail), "lz_rezero_reanalyze_ez")
+        else:
+            cabi.check(t.lib.lz_rezero_reanalyze(*head, int(mcts.deterministic), *tail), "lz_rezero_reanalyze")
+        mcts.last_num_kernels = t.lib.lz_search_num_kernels(q)
+        out, vis, val, cnt = targets.cpu().numpy(), visits.cpu().numpy(), values.cpu().numpy(), counts.cpu().numpy()
 
     mcts.last_infer_count = cnt       # [L - 1, S] per reuse search and simulation: trees that needed the network
     rezero_write_back(child_visits, root_values, pos_in_game_segment_list, L, policy_mask, action_mask, vis, val)
@@ -343,13 +330,6 @@ def compute_target_reward_value(
     EfficientZero, whose object arrays hold the same numbers), bit for bit the reference's given the same fp32 values.  With
     ``device=True`` they are CUDA float64 tensors and nothing waits for the device.  ``return_values=True`` appends the fp32
     bootstrap values [N * (K + 1)] (initial_inference's value scalars, or the searched root values)."""
-    from . import cabi, mz_tree
-    from .efficientzero_model import EfficientZeroModel
-    from .efficientzero_model_mlp import EfficientZeroModelMLP
-    from .mcts_ctree import EfficientZeroMCTSCtree
-    from .muzero_model import MuZeroModel
-    from .muzero_model_mlp import MuZeroModelMLP
-
     if use_root_value and not efficientzero:
         raise ValueError("compute_target_reward_value: use_root_value=True is not available for the MuZero buffer: the reference "
                          "reads np.array(root_values) from a list _prepare_reward_value_context never fills, and the product with "
@@ -361,11 +341,10 @@ def compute_target_reward_value(
     T = N * K1
     if value_obs.shape[0] != T:
         raise ValueError(f"compute_target_reward_value: {T} rows, got value_obs {tuple(value_obs.shape)}")
-    ez_model = isinstance(model, (EfficientZeroModel, EfficientZeroModelMLP))
-    if not isinstance(model, (MuZeroModel, MuZeroModelMLP, EfficientZeroModelMLP)):
+    if not isinstance(model, LzModel):
         raise TypeError(f"compute_target_reward_value: {type(model).__name__} has no CUDA initial_inference (MuZeroModel, "
                         "MuZeroModelMLP, EfficientZeroModel or EfficientZeroModelMLP)")
-    if bool(efficientzero) != ez_model:
+    if bool(efficientzero) != model.value_prefix:
         raise TypeError(f"compute_target_reward_value: the {'EfficientZero' if efficientzero else 'MuZero'} buffer's targets need "
                         f"{'an EfficientZero' if efficientzero else 'a MuZero'} model, not a {type(model).__name__}")
     sections = [tables[k] for k in _TABLE_ORDER if tables[k] is not None]
@@ -407,18 +386,12 @@ def compute_target_reward_value(
             mask_p, tp_p = rest[0], rest[1]
             nz_p = rest[2] if reanalyze_noise else None
             w = float(cfg.root_noise_weight if root_noise_weight is None else root_noise_weight)
-            t = mz_tree.acquire_tree(dev, T, A, S)
-            try:
-                t.set_params(*mcts._params())
-                cabi.check(t.lib.lz_tree_set_gumbel(t.h, 0, 0), "lz_tree_set_gumbel")     # a pooled tree a Gumbel collect left behind
-                cabi.check(t.lib.lz_tree_set_ez(t.h, 1, H), "lz_tree_set_ez")
+            with mz_tree.held_tree(dev, T, A, S, mcts._params(), (1, H), mcts.deterministic) as t:     # the search's tie rule
                 q = t.search_for(model, S, (1, H))
                 cabi.check(t.lib.lz_value_targets_root(q, tab, int(mini_infer_size), obs.data_ptr(), mask_p, tp_p, nz_p, w,
                                                        int(mcts.deterministic), values.data_ptr(), out[0].data_ptr(),
                                                        out[1].data_ptr(), s), "lz_value_targets_root")
                 mcts.last_num_kernels = t.lib.lz_search_num_kernels(q)
-            finally:
-                t.release()
         if device:
             res = (out[0], out[1])
         else:

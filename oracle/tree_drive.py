@@ -188,12 +188,7 @@ def drive(mod, c, kind, leaves, det=True, setup=None, reset_in_backup=True):
     else:
         roots.prepare(float(c.get("noise_w", 0.25)), noises, [0.] * B, *pre, logits, tp)
     if mod.__name__ in ("lightzero_b200.mz_tree", "lightzero_b200.ez_tree"):
-        from lightzero_b200 import cabi
         roots._materialize(S)          # node pool sized to this search (gmz_tree sizes its trees at the first descent)
-        # the EfficientZero and *_with_reuse descents take the first maximum, as the mirrors document; a pooled tree of
-        # this size may come from a stochastic fused search, which leaves it drawing ties
-        t = roots._tree
-        cabi.check(t.lib.lz_tree_set_tiebreak(t.h, 1), "lz_tree_set_tiebreak")
     if setup is not None:
         setup(roots)
     mm = mod.MinMaxStatsList(B)
