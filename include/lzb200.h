@@ -72,44 +72,62 @@ int lz_tree_reset_mask(lz_tree *t, const uint8_t *d_mask, lz_stream s);
 
 /* CRoots::prepare / prepare_no_noise (cnode.cpp:321-358).  d_logits f32 [B,A] by action id;
  * d_noise f32 [B,A] rows in LEGAL ORDER (first nlegal[b] used) or NULL for prepare_no_noise;
- * d_rewards f32 [B] or NULL (zeros); d_to_play int32 [B] (-1 == single player). */
+ * d_rewards f32 [B] or NULL (zeros); d_to_play int32 [B] (-1 == single player).
+ * d_values f32 [B]: the roots' value estimates, required on a Gumbel tree (ctree_gumbel_muzero cnode.cpp:418-455; it also
+ * starts a fresh round of at most num_simulations descents) and NULL on any other tree (LZ_EINVAL otherwise). */
 int lz_tree_prepare(lz_tree *t, const float *d_logits, const float *d_noise, float noise_weight,
-                    const float *d_rewards, const int32_t *d_to_play, lz_stream s);
+                    const float *d_rewards, const float *d_values, const int32_t *d_to_play, lz_stream s);
 
-/* cbatch_traverse (cnode.cpp:754-825): one PUCT descent per tree.  Outputs (each int32 [B], may be
- * NULL): latent-pool slot of the leaf's parent (== its current_latent_state_index), batch index
- * (== tree index), last action, search length, virtual to_play after the descent. */
-int lz_tree_traverse(lz_tree *t, int deterministic, int32_t *d_ix, int32_t *d_iy,
-                     int32_t *d_last_action, int32_t *d_search_len, int32_t *d_virtual_to_play,
+/* cbatch_traverse: one descent per tree, the one of the tree's mode.  Outputs (each int32 [B], may be NULL): latent-pool slot
+ * of the leaf's parent (== its current_latent_state_index), batch index (== tree index), last action, search length, virtual
+ * to_play after the descent.
+ *   MuZero tree (cnode.cpp:754-825): PUCT; ties by `deterministic`.
+ *   EfficientZero tree (ctree_efficientzero cnode.cpp:876-958): ties by lz_tree_set_tiebreak; d_is_reset int32 [B] out (may be
+ *     NULL; only EfficientZero trees take it, LZ_EINVAL otherwise) = (search_len % lstm_horizon_len == 0).
+ *   Reuse descent (ReZero search_with_reuse, cnode.cpp:597-652, 701-752, 828-932; EfficientZero :699-754, 960-1072), selected
+ *     by a non-NULL d_true_action int32 [B] / d_reuse_value f32 [B] pair (both or neither, LZ_EINVAL otherwise): the action
+ *     taken in the stored trajectory and the value to reuse for it.  The root scores that child with carm_score and the
+ *     descent stops right after the root when it is selected.  d_ix reports -1 for trees that stopped on an already expanded
+ *     child ("no inference"); d_iy is the batch_index recorded when the parent was expanded (the compact inference row).  Ties
+ *     by lz_tree_set_tiebreak.
+ *   Gumbel tree (ctree_gumbel_muzero cnode.cpp:834-897): sequential halving at the root; `deterministic` is ignored, the virtual
+ *     to_play is the root's, unchanged.  No reuse descent (LZ_ESTATE); at most num_simulations descents per prepare (one more
+ *     would index past the considered-visit table): LZ_ESTATE. */
+int lz_tree_traverse(lz_tree *t, int deterministic, const int32_t *d_true_action, const float *d_reuse_value, int32_t *d_ix,
+                     int32_t *d_iy, int32_t *d_last_action, int32_t *d_search_len, int32_t *d_virtual_to_play, int32_t *d_is_reset,
                      lz_stream s);
 
-/* cbatch_backpropagate (cnode.cpp:480-500): expand the leaves found by the last traverse into slot
- * `latent_index` (simulation_index + 1) and back up.  d_reward/d_value f32 [B] (scalars, after the
- * inverse transform), d_logits f32 [B,A]; d_to_play int32 [B] or NULL (use the virtual to_play the
- * last traverse produced, which is what mcts_ctree.py:365-368 passes). */
-int lz_tree_backpropagate(lz_tree *t, int latent_index, const float *d_reward, const float *d_value,
-                          const float *d_logits, const int32_t *d_to_play, lz_stream s);
+/* cbatch_backpropagate: expand the leaves found by the last traverse into slot `latent_index` (simulation_index + 1) and back
+ * up, the back-up of the tree's mode.  d_reward/d_value f32 [B] (scalars, after the inverse transform), d_logits f32 [B,A];
+ * d_to_play int32 [B] or NULL (use the virtual to_play the last traverse produced, which is what mcts_ctree.py:365-368 passes).
+ *   MuZero tree (cnode.cpp:480-500).
+ *   EfficientZero tree (ctree_efficientzero cnode.cpp:577-601): d_reward carries the value prefixes; d_is_reset int32 [B]
+ *     (is_reset_list) is required.  Any other tree takes d_is_reset == NULL (LZ_EINVAL otherwise).
+ *   Reuse back-up (cbatch_backpropagate_with_reuse, cnode.cpp:502-549; EfficientZero :603-650), selected by a non-NULL
+ *     d_reuse_value f32 [B]: rows are indexed BY TREE (not compacted; rows of "no inference" trees are ignored).  d_batch_rank
+ *     int32 [B] or NULL, only with d_reuse_value (LZ_EINVAL otherwise): compact row of each tree in the caller's inference
+ *     batch, stored as the batch_index of the node it expands.  Which trees skip the expansion / back up the reuse value is
+ *     the state the last traverse left.
+ *   Gumbel tree (ctree_gumbel_muzero cnode.cpp:633-652): the one-player back-up for every to_play; d_value is also the new
+ *     node's raw value.  It must follow a descent, and there is no reuse back-up (LZ_ESTATE). */
+int lz_tree_backpropagate(lz_tree *t, int latent_index, const float *d_reward, const float *d_value, const float *d_logits,
+                          const float *d_reuse_value, const int32_t *d_batch_rank, const int32_t *d_is_reset,
+                          const int32_t *d_to_play, lz_stream s);
 
 /* ---- EfficientZero tree (lzero/mcts/ctree/ctree_efficientzero/lib/cnode.cpp, ez_tree.pyx) ----
  * lz_tree_set_ez switches a tree to value-prefix semantics before lz_tree_prepare: the reward slot carries the child's
  * value prefix, every expanded node carries is_reset, the reward of a step is the prefix difference unless the parent
  * was reset (cnode.cpp:185-195, 496-573, 786-790).  lstm_horizon_len (mcts_ctree.py:857) is used by the fused search
- * and by lz_tree_traverse_ez to derive is_reset = (search_len % lstm_horizon_len == 0).
- * The reference tie-break is rand() % len(ties) with no deterministic switch (cnode.cpp:691); these entry points use
- * the first-maximum rule, which is that draw with rand() == 0 (how the parity oracle builds the reference). */
+ * and by lz_tree_traverse to derive is_reset = (search_len % lstm_horizon_len == 0).
+ * The reference tie-break is rand() % len(ties) with no deterministic switch (cnode.cpp:691); these trees use the rule of
+ * lz_tree_set_tiebreak, by default the first maximum, which is that draw with rand() == 0 (how the parity oracle builds the
+ * reference). */
 int lz_tree_set_ez(lz_tree *t, int efficientzero, int lstm_horizon_len);
-/* Tie-breaking of the EfficientZero and *_with_reuse descents, which have no deterministic switch in the reference (they draw
+/* Tie-breaking of the EfficientZero and reuse descents, which have no deterministic switch in the reference (they draw
  * rand() % len(ties) after reseeding from the wall clock, ctree_efficientzero/lib/cnode.cpp:691, ctree_muzero cnode.cpp:610-640):
  * first_maximum = 1 (default; the reference's draw with rand() == 0, what the parity tests pin) or 0 = a uniform draw from the same tie
- * list with the counter-based device RNG of lz_tree_traverse(deterministic = 0). */
+ * list with the counter-based device RNG of the MuZero lz_tree_traverse(deterministic = 0). */
 int lz_tree_set_tiebreak(lz_tree *t, int first_maximum);
-/* cbatch_traverse (ctree_efficientzero cnode.cpp:876-958); d_is_reset int32 [B] out (may be NULL). */
-int lz_tree_traverse_ez(lz_tree *t, int32_t *d_ix, int32_t *d_iy, int32_t *d_last_action, int32_t *d_search_len,
-                        int32_t *d_virtual_to_play, int32_t *d_is_reset, lz_stream s);
-/* cbatch_backpropagate (ctree_efficientzero cnode.cpp:577-601): value prefixes instead of rewards + is_reset_list. */
-int lz_tree_backpropagate_ez(lz_tree *t, int latent_index, const float *d_value_prefix, const float *d_value,
-                             const float *d_logits, const int32_t *d_is_reset, const int32_t *d_to_play, lz_stream s);
-
 /* get_distributions / get_values / get_trajectories (cnode.cpp:237-277,369-417).
  * d_visits int32 [B,A] in legal order, -1 padded; d_values f32 [B]; d_nlegal int32 [B];
  * d_traj int32 [B, max_sims+1] -1 padded.  Any pointer may be NULL. */
@@ -120,23 +138,6 @@ int lz_tree_results(lz_tree *t, int32_t *d_visits, float *d_values, int32_t *d_n
  * copies it); h_step_counter is the step the next step-wise descent takes (each one consumes a step; a fused search
  * uses steps 0 ... num_simulations - 1). */
 int lz_tree_debug_rng(lz_tree *t, uint64_t *h_seed, uint64_t *h_epoch, uint32_t *h_step_counter);
-
-/* ---- ReZero search_with_reuse (cnode.cpp:502-549, 597-652, 701-752, 828-932; SURVEY 8(f) row f-4); works on MuZero trees and,
- * with value-prefix semantics, on EfficientZero trees (ctree_efficientzero/lib/cnode.cpp:603-650, 699-754, 816-874, 960-1072) ----
- * d_true_action int32 [B] / d_reuse_value f32 [B]: the action taken in the stored trajectory and the value to reuse for it.
- * The root scores that child with carm_score and the descent stops right after the root when it is selected.  d_ix reports -1
- * for trees that stopped on an already expanded child ("no inference"); d_iy is the batch_index recorded when the parent was
- * expanded (the compact inference row under reuse).  Ties: first maximum (= the reference's rand() % len(ties) with rand()
- * == 0; these reference routines have no deterministic switch). */
-int lz_tree_traverse_with_reuse(lz_tree *t, const int32_t *d_true_action, const float *d_reuse_value, int32_t *d_ix, int32_t *d_iy,
-                                int32_t *d_last_action, int32_t *d_search_len, int32_t *d_virtual_to_play, lz_stream s);
-/* cbatch_backpropagate_with_reuse: rows are indexed BY TREE (not compacted; rows of "no inference" trees are ignored).
- * d_batch_rank int32 [B] or NULL: compact row of each tree in the caller's inference batch, stored as the batch_index of the
- * node it expands.  d_is_reset int32 [B]: EfficientZero trees only (NULL otherwise).  Which trees skip the expansion / back up
- * the reuse value is the state the last traverse left. */
-int lz_tree_backpropagate_with_reuse(lz_tree *t, int latent_index, const float *d_reward, const float *d_value, const float *d_logits,
-                                     const float *d_reuse_value, const int32_t *d_batch_rank, const int32_t *d_is_reset,
-                                     const int32_t *d_to_play, lz_stream s);
 
 /* select_action (lzero/policy/utils.py:637-661) on the device, from the root visit counts of the finished search:
  * p = visit ** (1 / temperature) / sum (fp64), d_entropy = -sum p log2 p (scipy.stats.entropy(p, base=2)), d_action_pos = arg-max (deterministic != 0; the
@@ -152,19 +153,10 @@ int lz_tree_select_action(lz_tree *t, float temperature, int deterministic, uint
  * :747-790); the back-up is the one-player recurrence for every to_play (:605-631).  It builds the root Gumbel vector
  * (10 * Gumbel(0, 1) from std::mt19937(0), the first n draws for a root with n legal actions) and row min(m, S) of the
  * considered-visit table on the host.  num_simulations == 0 turns the tree back into a MuZero tree.  Refused on an
- * EfficientZero tree; on a Gumbel tree the MuZero / EfficientZero / reuse tree and search calls are refused.
+ * EfficientZero tree.  On a Gumbel tree lz_tree_prepare, lz_tree_traverse, lz_tree_backpropagate and lz_search_run run the
+ * Gumbel prepare, descent, back-up and search; the reuse descent and search are refused.
  * Descents use the discount of lz_tree_set_params. */
 int lz_tree_set_gumbel(lz_tree *t, int max_num_considered_actions, int num_simulations);
-/* CRoots::prepare / prepare_no_noise (cnode.cpp:418-455): lz_tree_prepare plus the roots' value estimates d_values f32 [B]. */
-int lz_tree_prepare_gumbel(lz_tree *t, const float *d_logits, const float *d_noise, float noise_weight,
-                           const float *d_rewards, const float *d_values, const int32_t *d_to_play, lz_stream s);
-/* cbatch_traverse (cnode.cpp:834-897): outputs as lz_tree_traverse; the virtual to_play is the root's, unchanged.  At most
- * num_simulations descents per prepare (one more would index past the considered-visit table): LZ_ESTATE. */
-int lz_tree_traverse_gumbel(lz_tree *t, int32_t *d_ix, int32_t *d_iy, int32_t *d_last_action, int32_t *d_search_len,
-                            int32_t *d_virtual_to_play, lz_stream s);
-/* cbatch_back_propagate (cnode.cpp:633-652): arguments as lz_tree_backpropagate; d_value is also the new node's raw value. */
-int lz_tree_backpropagate_gumbel(lz_tree *t, int latent_index, const float *d_reward, const float *d_value,
-                                 const float *d_logits, const int32_t *d_to_play, lz_stream s);
 /* get_children_values / get_policies (cnode.cpp:309-385, 506-541) with the tree's discount: d_children_values f32 [B,A]
  * completed Q by action id (-inf at illegal actions), d_improved_policy f32 [B,A] softmax(prior + completed Q) by action id.
  * Either may be NULL.  Visit counts, values and trajectories: lz_tree_results. */
@@ -338,34 +330,32 @@ int lz_inverse_scalar_transform(lz_model *m, int B, const float *d_logits, float
 int lz_search_create(lz_tree *t, lz_model *m, int num_simulations, lz_search **out);
 int lz_search_destroy(lz_search *q);
 /* MuZeroMCTSCtree.search (mcts_ctree.py:267-368) on roots already prepared with lz_tree_prepare.
- * d_latent_roots f32 [B,C,h,w].  One graph launch, zero host syncs. */
+ * d_latent_roots f32 [B,C,h,w].  One graph launch, zero host syncs.  An EfficientZero search runs with lz_search_run_ez.
+ * On a Gumbel tree (lz_tree_set_gumbel) with a MuZero conv or MLP model: GumbelMuZeroMCTSCtree.search (mcts_ctree.py:1076-1172),
+ * one CUDA graph of [Gumbel descent] + num_simulations x [recurrent_inference, Gumbel back-up + next descent]; `deterministic`
+ * is ignored, the roots must be freshly prepared (no descent since lz_tree_prepare; LZ_ESTATE) and the search's
+ * num_simulations may not exceed the tree's Gumbel num_simulations (LZ_EINVAL). */
 int lz_search_run(lz_search *q, const float *d_latent_roots, int deterministic, lz_stream s);
-/* MuZeroMCTSCtree.search_with_reuse (mcts_ctree.py:370-468; ReZero).  d_true_action int32 [B], d_reuse_value f32 [B] as for
- * lz_tree_traverse_with_reuse; d_infer_count int32 [num_simulations] or NULL receives, per simulation, how many trees needed
- * the network (the reference returns the last count and the mean).  One CUDA graph; "no inference" rows are computed and
- * ignored instead of compacted on the host. */
-int lz_search_run_with_reuse(lz_search *q, const float *d_latent_roots, const int32_t *d_true_action, const float *d_reuse_value,
-                             int32_t *d_infer_count, lz_stream s);
+/* MuZeroMCTSCtree.search_with_reuse (mcts_ctree.py:370-468; ReZero) and EfficientZeroMCTSCtree.search_with_reuse (:878-1003).
+ * d_true_action int32 [B], d_reuse_value f32 [B] as for the reuse lz_tree_traverse; d_infer_count int32 [num_simulations] or
+ * NULL receives, per simulation, how many trees needed the network (the reference returns the last count and the mean).  One
+ * CUDA graph; "no inference" rows are computed and ignored instead of compacted on the host.  Ties by lz_tree_set_tiebreak.
+ * An EfficientZero search takes the roots' LSTM state d_hidden{0,1}_roots as lz_search_run_ez (NULL = zeros); its graph has
+ * 5 x num_simulations kernels and is_reset is taken per TREE from the descent (search_len % lstm_horizon_len; the
+ * reference indexes a compacted list by tree at :1040-1046 / cnode.cpp:646, see DESIGN.md 4.6).  A MuZero search takes
+ * NULL hidden pointers (LZ_EINVAL otherwise).  Refused on a Gumbel tree (LZ_ESTATE). */
+int lz_search_run_with_reuse(lz_search *q, const float *d_latent_roots, const float *d_hidden0_roots, const float *d_hidden1_roots,
+                             const int32_t *d_true_action, const float *d_reuse_value, int32_t *d_infer_count, lz_stream s);
 /* EfficientZeroMCTSCtree.search (mcts_ctree.py:671-876) for a search created from an EfficientZero model and a tree in
  * EfficientZero mode.  d_hidden{0,1}_roots: f32 [B, lstm_hidden_size] = reward_hidden_state_roots[0] / [1] (NULL = zeros,
  * what initial_inference returns).  The LSTM state of a leaf is zeroed every lstm_horizon_len steps of depth (:856-861). */
 int lz_search_run_ez(lz_search *q, const float *d_latent_roots, const float *d_hidden0_roots, const float *d_hidden1_roots, lz_stream s);
-/* EfficientZeroMCTSCtree.search_with_reuse (mcts_ctree.py:878-1003; ReZero on the value-prefix trees): arguments of lz_search_run_ez
- * plus d_true_action / d_reuse_value / d_infer_count of lz_search_run_with_reuse.  One CUDA graph (1 + 5 x num_simulations
- * kernels); is_reset is taken per TREE from the descent (search_len % lstm_horizon_len; the reference indexes a compacted list by
- * tree at :1040-1046 / cnode.cpp:646, see DESIGN.md 4.6). */
-int lz_search_run_ez_with_reuse(lz_search *q, const float *d_latent_roots, const float *d_hidden0_roots, const float *d_hidden1_roots,
-                                const int32_t *d_true_action, const float *d_reuse_value, int32_t *d_infer_count, lz_stream s);
-/* GumbelMuZeroMCTSCtree.search (mcts_ctree.py:1076-1172) on a Gumbel tree prepared with lz_tree_prepare_gumbel and a MuZero
- * conv or MLP model: one CUDA graph of [Gumbel descent] + num_simulations x [recurrent_inference, Gumbel back-up + next
- * descent].  The search's num_simulations may not exceed the tree's Gumbel num_simulations. */
-int lz_search_run_gumbel(lz_search *q, const float *d_latent_roots, lz_stream s);
 /* The search-feeding part of _forward_collect (policy/muzero.py:749-779): initial_inference ->
  * reset(mask) -> prepare(noise) -> search.  d_obs f32 [B,obs_c,H,W]; d_mask uint8 [B,A] or NULL;
  * d_noise f32 [B,A] legal-order rows or NULL; d_to_play int32 [B] or NULL (-1).
  * Optional outputs: d_pred_value f32 [B] (root value prediction), d_policy_logits f32 [B,A].
- * On a Gumbel tree (lz_tree_set_gumbel) lz_tree_prepare_gumbel prepares the roots with the root value prediction as their values
- * (GumbelMuZeroPolicy._forward_collect, gumbel_muzero.py:560-571) and the search is the graph of lz_search_run_gumbel; the
+ * On a Gumbel tree (lz_tree_set_gumbel) lz_tree_prepare takes the root value prediction as the roots' values
+ * (GumbelMuZeroPolicy._forward_collect, gumbel_muzero.py:560-571) and the search is the Gumbel graph of lz_search_run; the
  * search's num_simulations may not exceed the tree's Gumbel num_simulations (LZ_EINVAL).  The same holds for the three
  * entry points below.  Read the results with lz_tree_results and lz_tree_gumbel_select_action. */
 int lz_search_collect(lz_search *q, const float *d_obs, const uint8_t *d_mask, const float *d_noise,
@@ -398,7 +388,9 @@ int lz_search_collect_host_u8(lz_search *q, const uint8_t *h_obs_u8, const uint8
  *   d_mask uint8 [N*L, A] (legal actions; an all-zero row is every action), d_to_play int32 [N*L] or NULL (-1),
  *   d_true_action int32 [N*L] (the reference's -2 for a segment's last step and for padding), d_policy_mask uint8 [N*L],
  *   d_noise f32 [N*L, A] in legal order or NULL (reanalyze_noise = False), noise_weight.
- * The searches run backward from position L - 1: a plain search (MuZero: ties by `deterministic`; EfficientZero: first maximum),
+ * q may be a MuZero or an EfficientZero search (the LSTM state at every root is zero, as initial_inference returns it).
+ * The searches run backward from position L - 1: a plain search (MuZero: ties by `deterministic`; EfficientZero: first maximum,
+ * `deterministic` is ignored),
  * then, with reuse_search, L - 1 search_with_reuse calls each reusing the root values of the position searched before it (ties:
  * first maximum, the reference's rand() == 0); without reuse_search L plain searches.  Outputs:
  *   d_targets f64 [N, L, A]: visit / sum(visits) by legal position (scatter_legal = 0, fixed_action_space) or by action id
@@ -406,17 +398,13 @@ int lz_search_collect_host_u8(lz_search *q, const uint8_t *h_obs_u8, const uint8
  *   legal order, zero padded (what the buffer stores back); d_infer_count int32 [L - 1, S] (reuse_search, L > 1; else may be NULL):
  *   per reuse search and simulation, how many trees needed the network.
  * Everything is enqueued on s with no host synchronisation: initial_inference, then L x [handoff kernel, the search's captured
- * graph, targets kernel].  The graphs are those of lz_search_run / *_with_reuse, captured once and replayed along the sweep.
+ * graph, targets kernel].  The graphs are those of lz_search_run(_ez) / lz_search_run_with_reuse, captured once and replayed
+ * along the sweep.
  * Sets the tree's tie-break rule to first maximum (lz_tree_set_tiebreak). */
 int lz_rezero_reanalyze(lz_search *q, int L, int reuse_search, int mini_infer_size, const float *d_obs, const float *d_latent,
                         const float *d_logits, const uint8_t *d_mask, const int32_t *d_to_play, const int32_t *d_true_action,
                         const uint8_t *d_policy_mask, const float *d_noise, float noise_weight, int deterministic, int scatter_legal,
                         double *d_targets, float *d_root_values, double *d_child_visits, int32_t *d_infer_count, lz_stream s);
-/* The same for an EfficientZero search (the LSTM state at every root is zero, as initial_inference returns it). */
-int lz_rezero_reanalyze_ez(lz_search *q, int L, int reuse_search, int mini_infer_size, const float *d_obs, const float *d_latent,
-                           const float *d_logits, const uint8_t *d_mask, const int32_t *d_to_play, const int32_t *d_true_action,
-                           const uint8_t *d_policy_mask, const float *d_noise, float noise_weight, int scatter_legal,
-                           double *d_targets, float *d_root_values, double *d_child_visits, int32_t *d_infer_count, lz_stream s);
 /* ---- Replay-buffer reward and value targets (MuZeroGameBuffer._compute_target_reward_value,
  * lzero/mcts/buffer/game_buffer_muzero.py:467-575; EfficientZeroGameBuffer, game_buffer_efficientzero.py:167-323) ----
  * N sampled segments of K1 = num_unroll_steps + 1 rows, T = N * K1 rows, row = segment * K1 + position (the reference's

@@ -58,22 +58,15 @@ SIGNATURES = {
     "lz_tree_set_params": (c_int, [c_void_p, c_int, c_float, c_float, c_float]),
     "lz_tree_reset": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "lz_tree_reset_mask": (c_int, [c_void_p, c_void_p, c_void_p]),
-    "lz_tree_prepare": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p]),
-    "lz_tree_traverse": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "lz_tree_backpropagate": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "lz_tree_traverse_with_reuse": (c_int, [c_void_p] * 9),
-    "lz_tree_backpropagate_with_reuse": (c_int, [c_void_p, c_int] + [c_void_p] * 8),
+    "lz_tree_prepare": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "lz_tree_traverse": (c_int, [c_void_p, c_int] + [c_void_p] * 9),
+    "lz_tree_backpropagate": (c_int, [c_void_p, c_int] + [c_void_p] * 8),
     "lz_tree_select_action": (c_int, [c_void_p, c_float, c_int, ctypes.c_uint64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lz_tree_set_ez": (c_int, [c_void_p, c_int, c_int]),
     "lz_tree_set_tiebreak": (c_int, [c_void_p, c_int]),
-    "lz_tree_traverse_ez": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "lz_tree_backpropagate_ez": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lz_tree_results": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lz_tree_debug_rng": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "lz_tree_set_gumbel": (c_int, [c_void_p, c_int, c_int]),
-    "lz_tree_prepare_gumbel": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "lz_tree_traverse_gumbel": (c_int, [c_void_p] * 7),
-    "lz_tree_backpropagate_gumbel": (c_int, [c_void_p, c_int] + [c_void_p] * 5),
     "lz_tree_gumbel_policies": (c_int, [c_void_p] * 4),
     "lz_tree_gumbel_select_action": (c_int, [c_void_p, c_float] + [c_void_p] * 5),
     "lz_gumbel_tables": (c_int, [c_int, c_int, c_int, c_void_p, c_void_p]),
@@ -113,10 +106,8 @@ SIGNATURES = {
     "lz_search_num_kernels": (c_int, [c_void_p]),
     "lz_search_debug_plan": (c_int, [c_void_p, c_void_p]),
     "lz_search_latent_pool": (c_void_p, [c_void_p]),
-    "lz_search_run_with_reuse": (c_int, [c_void_p] * 6),
-    "lz_search_run_gumbel": (c_int, [c_void_p] * 3),
+    "lz_search_run_with_reuse": (c_int, [c_void_p] * 8),
     "lz_search_run_ez": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "lz_search_run_ez_with_reuse": (c_int, [c_void_p] * 8),
     "lz_frames_create": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(c_void_p)]),
     "lz_frames_destroy": (c_int, [c_void_p]),
     "lz_frames_push": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -131,7 +122,6 @@ SIGNATURES = {
     "lz_segments_improved_policy": (c_int, [c_void_p, ctypes.POINTER(c_void_p)]),
     "lz_search_hidden_pool": (c_void_p, [c_void_p, c_int]),
     "lz_rezero_reanalyze": (c_int, [c_void_p, c_int, c_int, c_int] + [c_void_p] * 8 + [c_float, c_int, c_int] + [c_void_p] * 5),
-    "lz_rezero_reanalyze_ez": (c_int, [c_void_p, c_int, c_int, c_int] + [c_void_p] * 8 + [c_float, c_int] + [c_void_p] * 5),
     "lz_value_targets": (c_int, [c_void_p, ctypes.POINTER(ValueTables), c_int] + [c_void_p] * 5),
     "lz_value_targets_root": (c_int, [c_void_p, ctypes.POINTER(ValueTables), c_int] + [c_void_p] * 4 + [c_float, c_int] +
                               [c_void_p] * 4),

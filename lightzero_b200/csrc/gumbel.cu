@@ -385,6 +385,35 @@ int gumbel_launch_step(lz_tree *t, const TreeStep &a, cudaStream_t s)
     return LZ_OK;
 }
 
+int gumbel_prepare(lz_tree *t, const float *d_values, cudaStream_t s)
+{
+    lz_gumbel *gs = t->gumbel;
+    k_gumbel_root_values<<<ceil_div(t->p.B, kGumbelBlock), kGumbelBlock, 0, s>>>(t->p, gs->g, d_values);
+    LZ_KERNEL_CHECK();
+    gs->prepared = true;
+    gs->pending = false;
+    gs->traversals = 0;
+    return LZ_OK;
+}
+
+int gumbel_step(lz_tree *t, const TreeStep &a, cudaStream_t s)
+{
+    lz_gumbel *gs = t->gumbel;
+    if (a.traverse) {
+        LZ_REQUIRE(gs->prepared, LZ_ESTATE, "lz_tree_traverse: Gumbel roots not prepared (call lz_tree_prepare first)");
+        LZ_REQUIRE(gs->traversals < gs->g.S, LZ_ESTATE,
+                   "lz_tree_traverse: %d descents after one prepare would index past the considered-visit table of "
+                   "num_simulations = %d", gs->traversals + 1, gs->g.S);
+    } else {
+        LZ_REQUIRE(gs->pending, LZ_ESTATE, "lz_tree_backpropagate: no Gumbel descent to back up (call lz_tree_traverse first)");
+    }
+    int rc = gumbel_launch_step(t, a, s);
+    if (rc != LZ_OK) return rc;
+    if (a.traverse) ++gs->traversals;
+    gs->pending = a.traverse != 0;
+    return LZ_OK;
+}
+
 // frees the Gumbel state, attached and idle (cudaFree: waits for all work on the device)
 void gumbel_free(lz_tree *t)
 {
@@ -495,60 +524,10 @@ int lz_tree_set_gumbel(lz_tree *t, int max_num_considered_actions, int num_simul
     return LZ_OK;
 }
 
-int lz_tree_prepare_gumbel(lz_tree *t, const float *d_logits, const float *d_noise, float noise_weight, const float *d_rewards,
-                           const float *d_values, const int32_t *d_to_play, lz_stream s)
-{
-    LZ_REQUIRE(t && d_logits && d_values, LZ_EINVAL, "lz_tree_prepare_gumbel: null argument");
-    LZ_REQUIRE(t->gumbel, LZ_ESTATE, "lz_tree_prepare_gumbel: not a Gumbel tree (lz_tree_set_gumbel)");
-    int rc = lz_tree_prepare(t, d_logits, d_noise, noise_weight, d_rewards, d_to_play, s);
-    if (rc != LZ_OK) return rc;
-    k_gumbel_root_values<<<ceil_div(t->p.B, kGumbelBlock), kGumbelBlock, 0, (cudaStream_t)s>>>(t->p, t->gumbel->g, d_values);
-    LZ_KERNEL_CHECK();
-    t->gumbel->prepared = true;
-    t->gumbel->pending = false;
-    t->gumbel->traversals = 0;
-    return LZ_OK;
-}
-
-int lz_tree_traverse_gumbel(lz_tree *t, int32_t *d_ix, int32_t *d_iy, int32_t *d_last_action, int32_t *d_search_len,
-                            int32_t *d_virtual_to_play, lz_stream s)
-{
-    LZ_REQUIRE(t && t->gumbel, LZ_ESTATE, "lz_tree_traverse_gumbel: not a Gumbel tree (lz_tree_set_gumbel)");
-    lz_gumbel *gs = t->gumbel;
-    LZ_REQUIRE(gs->prepared, LZ_ESTATE, "lz_tree_traverse_gumbel: roots not prepared (call lz_tree_prepare_gumbel first)");
-    LZ_REQUIRE(gs->traversals < gs->g.S, LZ_ESTATE,
-               "lz_tree_traverse_gumbel: %d descents after one prepare would index past the considered-visit table of "
-               "num_simulations = %d", gs->traversals + 1, gs->g.S);
-    TreeStep a = {};
-    a.traverse = 1;
-    a.ix = d_ix; a.iy = d_iy; a.act = d_last_action; a.len = d_search_len; a.vtp = d_virtual_to_play;
-    int rc = gumbel_launch_step(t, a, (cudaStream_t)s);
-    if (rc != LZ_OK) return rc;
-    ++gs->traversals;
-    gs->pending = true;
-    return LZ_OK;
-}
-
-int lz_tree_backpropagate_gumbel(lz_tree *t, int latent_index, const float *d_reward, const float *d_value, const float *d_logits,
-                                 const int32_t *d_to_play, lz_stream s)
-{
-    LZ_REQUIRE(t && d_reward && d_value && d_logits, LZ_EINVAL, "lz_tree_backpropagate_gumbel: null argument");
-    LZ_REQUIRE(t->gumbel, LZ_ESTATE, "lz_tree_backpropagate_gumbel: not a Gumbel tree (lz_tree_set_gumbel)");
-    LZ_REQUIRE(t->gumbel->pending, LZ_ESTATE, "lz_tree_backpropagate_gumbel: no descent to back up (call lz_tree_traverse_gumbel first)");
-    LZ_REQUIRE(latent_index >= 1 && latent_index <= t->max_sims, LZ_EINVAL,
-               "lz_tree_backpropagate_gumbel: latent_index %d outside [1, %d]", latent_index, t->max_sims);
-    TreeStep a = {};
-    a.latent_index = latent_index; a.reward = d_reward; a.value = d_value; a.logits = d_logits; a.to_play = d_to_play;
-    int rc = gumbel_launch_step(t, a, (cudaStream_t)s);
-    if (rc != LZ_OK) return rc;
-    t->gumbel->pending = false;
-    return LZ_OK;
-}
-
 int lz_tree_gumbel_policies(lz_tree *t, float *d_children_values, float *d_improved_policy, lz_stream s)
 {
     LZ_REQUIRE(t && t->gumbel, LZ_ESTATE, "lz_tree_gumbel_policies: not a Gumbel tree (lz_tree_set_gumbel)");
-    LZ_REQUIRE(t->gumbel->prepared, LZ_ESTATE, "lz_tree_gumbel_policies: roots not prepared (call lz_tree_prepare_gumbel first)");
+    LZ_REQUIRE(t->gumbel->prepared, LZ_ESTATE, "lz_tree_gumbel_policies: roots not prepared (call lz_tree_prepare first)");
     GumbelReadout o = {};
     o.children_values = d_children_values; o.cv_fill = -INFINITY; o.policy = d_improved_policy;
     return gumbel_readout(t, o, (cudaStream_t)s);
@@ -558,7 +537,7 @@ int lz_tree_gumbel_select_action(lz_tree *t, float temperature, int32_t *d_actio
                                  float *d_improved_policy, lz_stream s)
 {
     LZ_REQUIRE(t && t->gumbel, LZ_ESTATE, "lz_tree_gumbel_select_action: not a Gumbel tree (lz_tree_set_gumbel)");
-    LZ_REQUIRE(t->gumbel->prepared, LZ_ESTATE, "lz_tree_gumbel_select_action: roots not prepared (call lz_tree_prepare_gumbel first)");
+    LZ_REQUIRE(t->gumbel->prepared, LZ_ESTATE, "lz_tree_gumbel_select_action: roots not prepared (call lz_tree_prepare first)");
     LZ_REQUIRE(temperature > 0.0f, LZ_EINVAL, "lz_tree_gumbel_select_action: temperature must be > 0");
     GumbelReadout o = {};
     o.children_values = d_children_values; o.cv_fill = 0.0f; o.policy = d_improved_policy;

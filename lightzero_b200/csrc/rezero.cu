@@ -8,7 +8,7 @@
 //   initial_inference in mini_infer_size slices -> L x [k_rezero_handoff, captured search graph, k_rezero_targets].
 // k_rezero_handoff gathers the next group's latents, true actions and (zero) LSTM state into the search's fixed buffers, copies
 // the finished group's root values into the reuse-value buffer and resets + prepares the trees from the group's mask, logits,
-// noise and to_play; so the captured graphs of lz_search_run / *_with_reuse are replayed, never re-captured, along the sweep.
+// noise and to_play; so the captured graphs of lz_search_run / lz_search_run_with_reuse are replayed, never re-captured, along the sweep.
 // Compiled with -fmad=false like tree.cu: the reset / prepare arithmetic is the tree's.
 #include <limits.h>
 #include <string.h>
@@ -208,20 +208,7 @@ int lz_rezero_reanalyze(lz_search *q, int L, int reuse_search, int mini_infer_si
                         double *d_targets, float *d_root_values, double *d_child_visits, int32_t *d_infer_count, lz_stream s)
 {
     LZ_REQUIRE(q, LZ_EINVAL, "lz_rezero_reanalyze: null search");
-    LZ_REQUIRE(!q->hpool, LZ_ESTATE, "lz_rezero_reanalyze: EfficientZero search, use lz_rezero_reanalyze_ez");
     SweepArgs a = {L, reuse_search, mini_infer_size, deterministic, scatter_legal, d_obs, d_latent, d_logits, d_mask, d_policy_mask,
-                   d_to_play, d_true_action, d_noise, noise_weight, d_targets, d_child_visits, d_root_values, d_infer_count};
-    return sweep(q, a, (cudaStream_t)s);
-}
-
-int lz_rezero_reanalyze_ez(lz_search *q, int L, int reuse_search, int mini_infer_size, const float *d_obs, const float *d_latent,
-                           const float *d_logits, const uint8_t *d_mask, const int32_t *d_to_play, const int32_t *d_true_action,
-                           const uint8_t *d_policy_mask, const float *d_noise, float noise_weight, int scatter_legal,
-                           double *d_targets, float *d_root_values, double *d_child_visits, int32_t *d_infer_count, lz_stream s)
-{
-    LZ_REQUIRE(q, LZ_EINVAL, "lz_rezero_reanalyze_ez: null search");
-    LZ_REQUIRE(q->hpool, LZ_ESTATE, "lz_rezero_reanalyze_ez: not an EfficientZero search, use lz_rezero_reanalyze");
-    SweepArgs a = {L, reuse_search, mini_infer_size, 1, scatter_legal, d_obs, d_latent, d_logits, d_mask, d_policy_mask,
                    d_to_play, d_true_action, d_noise, noise_weight, d_targets, d_child_visits, d_root_values, d_infer_count};
     return sweep(q, a, (cudaStream_t)s);
 }

@@ -145,6 +145,10 @@ int lz::search_run_graph(lz_search *q, int deterministic, bool reuse, cudaStream
     LZ_CUDA_CHECK(cudaGraphLaunch(g.exec, s));
     q->num_kernels = g.num_kernels;
     count_launch(g.num_kernels);       // the graph's kernel nodes
+    if (lz_gumbel *gs = q->tree->gumbel) {      // the Gumbel graph makes all S descents of the prepared roots and backs each up
+        gs->traversals = q->S;
+        gs->pending = false;
+    }
     return LZ_OK;
 }
 
@@ -173,28 +177,13 @@ int lz::search_reuse_buffers(lz_search *q)
     return rc;
 }
 
-static int run_with_reuse(lz_search *q, const float *d_latent_roots, const int32_t *d_true_action, const float *d_reuse_value,
-                          int32_t *d_infer_count, cudaStream_t s)
-{
-    int rc = search_reuse_buffers(q);
-    if (rc == LZ_OK) rc = copy_latent_roots(q, d_latent_roots, s);
-    if (rc) return rc;
-    LZ_CUDA_CHECK(cudaMemcpyAsync(q->d_true_action, d_true_action, (size_t)q->B * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
-    LZ_CUDA_CHECK(cudaMemcpyAsync(q->d_reuse_value, d_reuse_value, (size_t)q->B * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    LZ_CUDA_CHECK(cudaMemsetAsync(q->tree->p.infer_count, 0, (size_t)q->tree->p.N * sizeof(int), s));
-    if ((rc = search_run_graph(q, 0, true, s))) return rc;
-    if (d_infer_count)      // per simulation: how many trees needed the network (mcts_ctree.py:433,466-467)
-        LZ_CUDA_CHECK(cudaMemcpyAsync(d_infer_count, q->tree->p.infer_count, (size_t)q->S * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
-    return LZ_OK;
-}
-
-// Checked before the initial inference: a Gumbel search may not take more simulations than its considered-visit table has
-static int collect_check(const lz_search *q)
+// A Gumbel search may not take more simulations than its considered-visit table has (checked before any work is enqueued)
+static int gumbel_sims_check(const lz_search *q, const char *fn)
 {
     const lz_gumbel *gs = q->tree->gumbel;
     LZ_REQUIRE(!gs || q->S <= gs->g.S, LZ_EINVAL,
-               "lz_search_collect: %d simulations past the considered-visit table of the Gumbel tree's num_simulations = %d",
-               q->S, gs ? gs->g.S : 0);
+               "%s: %d simulations past the considered-visit table of the Gumbel tree's num_simulations = %d", fn, q->S,
+               gs ? gs->g.S : 0);
     return LZ_OK;
 }
 
@@ -205,18 +194,13 @@ static int collect_search(lz_search *q, const uint8_t *d_mask, const float *d_lo
                           float noise_weight, const int32_t *d_to_play, int deterministic, cudaStream_t s)
 {
     int rc;
-    if ((rc = lz_tree_reset_mask(q->tree, d_mask, s))) return rc;                // policy/muzero.py:760,769
-    if (lz_gumbel *gs = q->tree->gumbel) {
-        if ((rc = lz_tree_prepare_gumbel(q->tree, d_logits, d_noise, noise_weight, nullptr, d_values, d_to_play, s))) return rc;
-        if ((rc = search_run_graph(q, 1, false, s))) return rc;
-        gs->traversals = q->S;
-        gs->pending = false;
-        return LZ_OK;
-    }
-    if ((rc = lz_tree_prepare(q->tree, d_logits, d_noise, noise_weight, nullptr, d_to_play, s))) return rc;   // :774
+    lz_tree *t = q->tree;
+    if ((rc = lz_tree_reset_mask(t, d_mask, s))) return rc;                        // policy/muzero.py:760,769
+    const float *values = t->gumbel ? d_values : nullptr;
+    if ((rc = lz_tree_prepare(t, d_logits, d_noise, noise_weight, nullptr, values, d_to_play, s))) return rc;   // :774
     if (q->hpool) {      // EfficientZero: zero LSTM state at the roots; the tree has no deterministic argument, the collect call's flag selects its tie-breaking
         if ((rc = ez_root_hidden(q, nullptr, nullptr, s))) return rc;
-        if ((rc = lz_tree_set_tiebreak(q->tree, deterministic))) return rc;
+        if ((rc = lz_tree_set_tiebreak(t, deterministic))) return rc;
     }
     return search_run_graph(q, deterministic, false, s);                                // :775
 }
@@ -286,7 +270,7 @@ int lz_search_destroy(lz_search *q)
 int lz_search_run_ez(lz_search *q, const float *d_latent_roots, const float *d_hidden0_roots, const float *d_hidden1_roots, lz_stream s)
 {
     LZ_REQUIRE(q && q->hpool, LZ_EINVAL, "lz_search_run_ez: not an EfficientZero search");
-    LZ_REQUIRE(!q->tree->gumbel, LZ_ESTATE, "lz_search_run_ez: Gumbel tree, use lz_search_run_gumbel");
+    LZ_REQUIRE(!q->tree->gumbel, LZ_ESTATE, "lz_search_run_ez: Gumbel tree, use lz_search_run");
     LZ_REQUIRE(q->tree->prepared, LZ_ESTATE, "lz_search_run_ez: roots not prepared (call lz_tree_prepare first)");
     int rc = copy_latent_roots(q, d_latent_roots, (cudaStream_t)s);
     if (rc == LZ_OK) rc = ez_root_hidden(q, d_hidden0_roots, d_hidden1_roots, (cudaStream_t)s);
@@ -294,26 +278,26 @@ int lz_search_run_ez(lz_search *q, const float *d_latent_roots, const float *d_h
     return search_run_graph(q, 1, false, (cudaStream_t)s);
 }
 
-int lz_search_run_with_reuse(lz_search *q, const float *d_latent_roots, const int32_t *d_true_action, const float *d_reuse_value,
-                             int32_t *d_infer_count, lz_stream s_)
+int lz_search_run_with_reuse(lz_search *q, const float *d_latent_roots, const float *d_hidden0_roots, const float *d_hidden1_roots,
+                             const int32_t *d_true_action, const float *d_reuse_value, int32_t *d_infer_count, lz_stream s_)
 {
     LZ_REQUIRE(q && d_true_action && d_reuse_value, LZ_EINVAL, "lz_search_run_with_reuse: null argument");
-    LZ_REQUIRE(!q->hpool, LZ_ESTATE, "lz_search_run_with_reuse: EfficientZero search, use lz_search_run_ez_with_reuse");
+    LZ_REQUIRE(q->hpool || (!d_hidden0_roots && !d_hidden1_roots), LZ_EINVAL,
+               "lz_search_run_with_reuse: LSTM state passed to a MuZero search");
     LZ_REQUIRE(q->tree->prepared, LZ_ESTATE, "lz_search_run_with_reuse: roots not prepared (call lz_tree_prepare first)");
-    LZ_REQUIRE(!q->tree->gumbel, LZ_ESTATE, "lz_search_run_with_reuse: Gumbel tree, use lz_search_run_gumbel");
-    return run_with_reuse(q, d_latent_roots, d_true_action, d_reuse_value, d_infer_count, (cudaStream_t)s_);
-}
-
-int lz_search_run_ez_with_reuse(lz_search *q, const float *d_latent_roots, const float *d_hidden0_roots, const float *d_hidden1_roots,
-                                const int32_t *d_true_action, const float *d_reuse_value, int32_t *d_infer_count, lz_stream s_)
-{
-    LZ_REQUIRE(q && d_true_action && d_reuse_value, LZ_EINVAL, "lz_search_run_ez_with_reuse: null argument");
-    LZ_REQUIRE(q->hpool, LZ_ESTATE, "lz_search_run_ez_with_reuse: not an EfficientZero search");
-    LZ_REQUIRE(q->tree->prepared, LZ_ESTATE, "lz_search_run_ez_with_reuse: roots not prepared (call lz_tree_prepare first)");
-    LZ_REQUIRE(!q->tree->gumbel, LZ_ESTATE, "lz_search_run_ez_with_reuse: Gumbel tree, use lz_search_run_gumbel");
-    int rc = ez_root_hidden(q, d_hidden0_roots, d_hidden1_roots, (cudaStream_t)s_);
+    LZ_REQUIRE(!q->tree->gumbel, LZ_ESTATE, "lz_search_run_with_reuse: Gumbel tree (it has no reuse search)");
+    const cudaStream_t s = (cudaStream_t)s_;
+    int rc = search_reuse_buffers(q);
+    if (rc == LZ_OK) rc = copy_latent_roots(q, d_latent_roots, s);
+    if (rc == LZ_OK && q->hpool) rc = ez_root_hidden(q, d_hidden0_roots, d_hidden1_roots, s);
     if (rc) return rc;
-    return run_with_reuse(q, d_latent_roots, d_true_action, d_reuse_value, d_infer_count, (cudaStream_t)s_);
+    LZ_CUDA_CHECK(cudaMemcpyAsync(q->d_true_action, d_true_action, (size_t)q->B * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+    LZ_CUDA_CHECK(cudaMemcpyAsync(q->d_reuse_value, d_reuse_value, (size_t)q->B * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    LZ_CUDA_CHECK(cudaMemsetAsync(q->tree->p.infer_count, 0, (size_t)q->tree->p.N * sizeof(int), s));
+    if ((rc = search_run_graph(q, 0, true, s))) return rc;
+    if (d_infer_count)      // per simulation: how many trees needed the network (mcts_ctree.py:433,466-467)
+        LZ_CUDA_CHECK(cudaMemcpyAsync(d_infer_count, q->tree->p.infer_count, (size_t)q->S * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+    return LZ_OK;
 }
 
 int lz_search_run(lz_search *q, const float *d_latent_roots, int deterministic, lz_stream s)
@@ -321,28 +305,14 @@ int lz_search_run(lz_search *q, const float *d_latent_roots, int deterministic, 
     LZ_REQUIRE(q, LZ_EINVAL, "lz_search_run: null search");
     LZ_REQUIRE(!q->hpool, LZ_ESTATE, "lz_search_run: EfficientZero search, use lz_search_run_ez");
     LZ_REQUIRE(q->tree->prepared, LZ_ESTATE, "lz_search_run: roots not prepared (call lz_tree_prepare first)");
-    LZ_REQUIRE(!q->tree->gumbel, LZ_ESTATE, "lz_search_run: Gumbel tree, use lz_search_run_gumbel");
+    if (const lz_gumbel *gs = q->tree->gumbel) {
+        LZ_REQUIRE(gs->prepared && gs->traversals == 0, LZ_ESTATE,
+                   "lz_search_run: Gumbel roots not freshly prepared (call lz_tree_prepare first)");
+        if (int rc = gumbel_sims_check(q, "lz_search_run")) return rc;
+    }
     int rc = copy_latent_roots(q, d_latent_roots, (cudaStream_t)s);
     if (rc) return rc;
     return search_run_graph(q, deterministic, false, (cudaStream_t)s);
-}
-
-int lz_search_run_gumbel(lz_search *q, const float *d_latent_roots, lz_stream s)
-{
-    LZ_REQUIRE(q, LZ_EINVAL, "lz_search_run_gumbel: null search");
-    lz_gumbel *gs = q->tree->gumbel;
-    LZ_REQUIRE(gs, LZ_ESTATE, "lz_search_run_gumbel: not a Gumbel tree (lz_tree_set_gumbel)");
-    LZ_REQUIRE(!q->hpool && !q->tree->p.ez, LZ_ESTATE, "lz_search_run_gumbel: EfficientZero model or tree (the Gumbel search runs MuZero models)");
-    LZ_REQUIRE(gs->prepared && gs->traversals == 0, LZ_ESTATE,
-               "lz_search_run_gumbel: roots not freshly prepared (call lz_tree_prepare_gumbel first)");
-    LZ_REQUIRE(q->S <= gs->g.S, LZ_EINVAL, "lz_search_run_gumbel: %d simulations past the considered-visit table of num_simulations = %d",
-               q->S, gs->g.S);
-    int rc = copy_latent_roots(q, d_latent_roots, (cudaStream_t)s);
-    if (rc) return rc;
-    if ((rc = search_run_graph(q, 1, false, (cudaStream_t)s))) return rc;
-    gs->traversals = q->S;
-    gs->pending = false;
-    return LZ_OK;
 }
 
 static int collect_device(lz_search *q, const float *d_obs, const uint8_t *d_obs_u8, const uint8_t *d_mask, const float *d_noise,
@@ -350,7 +320,7 @@ static int collect_device(lz_search *q, const float *d_obs, const uint8_t *d_obs
                           float *d_policy_logits, lz_stream s)
 {
     LZ_REQUIRE(q && (d_obs || d_obs_u8), LZ_EINVAL, "lz_search_collect: bad argument");
-    int rc = collect_check(q);
+    int rc = gumbel_sims_check(q, "lz_search_collect");
     if (rc) return rc;
     TailIO io;
     memset(&io, 0, sizeof(io));
@@ -387,7 +357,7 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
 {
     LZ_REQUIRE(q && h_obs, LZ_EINVAL, "lz_search_collect_host: bad argument");
     LZ_REQUIRE(!obs_u8 || q->model->family == ModelFamily::Conv, LZ_EINVAL, "lz_search_collect_host_u8: uint8 frames need the conv model");
-    if (int rc = collect_check(q)) return rc;
+    if (int rc = gumbel_sims_check(q, "lz_search_collect_host")) return rc;
     const size_t esz = obs_u8 ? 1 : sizeof(float);         // bytes per observation element on the wire and in the staging buffer
     cudaStream_t s = (cudaStream_t)s_;
     const int B = q->B, A = q->A;

@@ -165,7 +165,7 @@ int lz_value_targets_root(lz_search *q, const lz_value_tables *tab, int mini_inf
     }
     // :220-239: roots from the legal actions, zero value prefixes, the logits, noise and to_play; the search on zero LSTM state
     if ((rc = lz_tree_reset_mask(t, d_mask, s_))) return rc;
-    if ((rc = lz_tree_prepare(t, q->d_root_logits, d_noise, noise_weight, nullptr, d_to_play, s_))) return rc;
+    if ((rc = lz_tree_prepare(t, q->d_root_logits, d_noise, noise_weight, nullptr, nullptr, d_to_play, s_))) return rc;
     LZ_CUDA_CHECK(cudaMemsetAsync(q->hpool, 0, q->hslot_stride * sizeof(float), s));
     LZ_CUDA_CHECK(cudaMemsetAsync(q->cpool, 0, q->hslot_stride * sizeof(float), s));
     if ((rc = lz_tree_set_tiebreak(t, first_maximum))) return rc;

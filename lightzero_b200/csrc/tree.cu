@@ -321,43 +321,50 @@ int lz_tree_reset_mask(lz_tree *t, const uint8_t *d_mask, lz_stream s)
     return LZ_OK;
 }
 
-int lz_tree_prepare(lz_tree *t, const float *d_logits, const float *d_noise, float noise_weight,
-                    const float *d_rewards, const int32_t *d_to_play, lz_stream s)
+int lz_tree_prepare(lz_tree *t, const float *d_logits, const float *d_noise, float noise_weight, const float *d_rewards,
+                    const float *d_values, const int32_t *d_to_play, lz_stream s)
 {
     LZ_REQUIRE(t && d_logits, LZ_EINVAL, "lz_tree_prepare: null argument");
+    LZ_REQUIRE(!t->gumbel == !d_values, LZ_EINVAL, t->gumbel ? "lz_tree_prepare: a Gumbel tree needs the root values d_values"
+                                                             : "lz_tree_prepare: d_values is for Gumbel trees only (lz_tree_set_gumbel)");
     k_tree_prepare<<<tree_grid(t->p.B), kTreeBlock, 0, (cudaStream_t)s>>>(t->p, d_logits, d_noise, noise_weight,
                                                                          d_rewards, d_to_play);
     LZ_KERNEL_CHECK();
     t->prepared = true;
-    if (t->gumbel) t->gumbel->prepared = false;     // lz_tree_prepare_gumbel sets it after this call
-    return LZ_OK;
+    return t->gumbel ? gumbel_prepare(t, d_values, (cudaStream_t)s) : LZ_OK;
 }
 
-int lz_tree_traverse(lz_tree *t, int deterministic, int32_t *d_ix, int32_t *d_iy, int32_t *d_last_action,
-                     int32_t *d_search_len, int32_t *d_virtual_to_play, lz_stream s)
+int lz_tree_traverse(lz_tree *t, int deterministic, const int32_t *d_true_action, const float *d_reuse_value, int32_t *d_ix,
+                     int32_t *d_iy, int32_t *d_last_action, int32_t *d_search_len, int32_t *d_virtual_to_play, int32_t *d_is_reset,
+                     lz_stream s)
 {
     LZ_REQUIRE(t, LZ_EINVAL, "lz_tree_traverse: null tree");
+    LZ_REQUIRE(!d_true_action == !d_reuse_value, LZ_EINVAL, "lz_tree_traverse: pass both d_true_action and d_reuse_value or neither");
+    LZ_REQUIRE(!d_is_reset || t->p.ez, LZ_EINVAL, "lz_tree_traverse: d_is_reset is an output of EfficientZero trees only");
     LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_traverse: roots not prepared (call lz_tree_prepare first)");
-    LZ_REQUIRE(!t->p.ez, LZ_ESTATE, "lz_tree_traverse: tree is in EfficientZero mode, use lz_tree_traverse_ez");
-    LZ_REQUIRE(!t->gumbel, LZ_ESTATE, "lz_tree_traverse: Gumbel tree, use lz_tree_traverse_gumbel");
+    LZ_REQUIRE(!t->gumbel || !d_reuse_value, LZ_ESTATE, "lz_tree_traverse: Gumbel tree (it has no reuse descent)");
     TreeStep a = {};
-    a.traverse = 1; a.deterministic = deterministic;
-    a.ix = d_ix; a.iy = d_iy; a.act = d_last_action; a.len = d_search_len; a.vtp = d_virtual_to_play;
-    return tree_launch_step(t, a, (cudaStream_t)s);
+    a.traverse = 1; a.deterministic = deterministic; a.true_action = d_true_action; a.reuse_value = d_reuse_value;
+    a.ix = d_ix; a.iy = d_iy; a.act = d_last_action; a.len = d_search_len; a.vtp = d_virtual_to_play; a.is_reset = d_is_reset;
+    return t->gumbel ? gumbel_step(t, a, (cudaStream_t)s) : tree_launch_step(t, a, (cudaStream_t)s);
 }
 
-int lz_tree_backpropagate(lz_tree *t, int latent_index, const float *d_reward, const float *d_value,
-                          const float *d_logits, const int32_t *d_to_play, lz_stream s)
+int lz_tree_backpropagate(lz_tree *t, int latent_index, const float *d_reward, const float *d_value, const float *d_logits,
+                          const float *d_reuse_value, const int32_t *d_batch_rank, const int32_t *d_is_reset,
+                          const int32_t *d_to_play, lz_stream s)
 {
     LZ_REQUIRE(t && d_reward && d_value && d_logits, LZ_EINVAL, "lz_tree_backpropagate: null argument");
+    LZ_REQUIRE(!d_batch_rank || d_reuse_value, LZ_EINVAL, "lz_tree_backpropagate: d_batch_rank needs d_reuse_value");
+    LZ_REQUIRE(!t->p.ez == !d_is_reset, LZ_EINVAL, t->p.ez ? "lz_tree_backpropagate: EfficientZero trees need d_is_reset"
+                                                          : "lz_tree_backpropagate: d_is_reset is for EfficientZero trees only");
     LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_backpropagate: roots not prepared");
-    LZ_REQUIRE(!t->p.ez, LZ_ESTATE, "lz_tree_backpropagate: tree is in EfficientZero mode, use lz_tree_backpropagate_ez");
-    LZ_REQUIRE(!t->gumbel, LZ_ESTATE, "lz_tree_backpropagate: Gumbel tree, use lz_tree_backpropagate_gumbel");
+    LZ_REQUIRE(!t->gumbel || !d_reuse_value, LZ_ESTATE, "lz_tree_backpropagate: Gumbel tree (it has no reuse back-up)");
     LZ_REQUIRE(latent_index >= 1 && latent_index <= t->max_sims, LZ_EINVAL,
                "lz_tree_backpropagate: latent_index %d outside [1, %d]", latent_index, t->max_sims);
     TreeStep a = {};
     a.latent_index = latent_index; a.reward = d_reward; a.value = d_value; a.logits = d_logits; a.to_play = d_to_play;
-    return tree_launch_step(t, a, (cudaStream_t)s);
+    a.leaf_reset = d_is_reset; a.batch_rank = d_batch_rank; a.reuse_value = d_reuse_value;
+    return t->gumbel ? gumbel_step(t, a, (cudaStream_t)s) : tree_launch_step(t, a, (cudaStream_t)s);
 }
 
 int lz_tree_set_ez(lz_tree *t, int efficientzero, int lstm_horizon_len)
@@ -379,59 +386,6 @@ int lz_tree_set_tiebreak(lz_tree *t, int first_maximum)
     if (t->p.tie_first != v) ++t->generation;       // captured graphs bake TreeParams in
     t->p.tie_first = v;
     return LZ_OK;
-}
-
-int lz_tree_traverse_ez(lz_tree *t, int32_t *d_ix, int32_t *d_iy, int32_t *d_last_action, int32_t *d_search_len,
-                        int32_t *d_virtual_to_play, int32_t *d_is_reset, lz_stream s)
-{
-    LZ_REQUIRE(t && t->p.ez, LZ_ESTATE, "lz_tree_traverse_ez: tree is not in EfficientZero mode (lz_tree_set_ez)");
-    LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_traverse_ez: roots not prepared (call lz_tree_prepare first)");
-    TreeStep a = {};
-    a.traverse = 1;
-    a.ix = d_ix; a.iy = d_iy; a.act = d_last_action; a.len = d_search_len; a.vtp = d_virtual_to_play; a.is_reset = d_is_reset;
-    return tree_launch_step(t, a, (cudaStream_t)s);
-}
-
-int lz_tree_backpropagate_ez(lz_tree *t, int latent_index, const float *d_value_prefix, const float *d_value,
-                             const float *d_logits, const int32_t *d_is_reset, const int32_t *d_to_play, lz_stream s)
-{
-    LZ_REQUIRE(t && d_value_prefix && d_value && d_logits && d_is_reset, LZ_EINVAL, "lz_tree_backpropagate_ez: null argument");
-    LZ_REQUIRE(t->p.ez, LZ_ESTATE, "lz_tree_backpropagate_ez: tree is not in EfficientZero mode (lz_tree_set_ez)");
-    LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_backpropagate_ez: roots not prepared");
-    LZ_REQUIRE(latent_index >= 1 && latent_index <= t->max_sims, LZ_EINVAL,
-               "lz_tree_backpropagate_ez: latent_index %d outside [1, %d]", latent_index, t->max_sims);
-    TreeStep a = {};
-    a.latent_index = latent_index; a.reward = d_value_prefix; a.value = d_value; a.logits = d_logits; a.to_play = d_to_play;
-    a.leaf_reset = d_is_reset;
-    return tree_launch_step(t, a, (cudaStream_t)s);
-}
-
-int lz_tree_traverse_with_reuse(lz_tree *t, const int32_t *d_true_action, const float *d_reuse_value, int32_t *d_ix, int32_t *d_iy,
-                                int32_t *d_last_action, int32_t *d_search_len, int32_t *d_virtual_to_play, lz_stream s)
-{
-    LZ_REQUIRE(t && d_true_action && d_reuse_value, LZ_EINVAL, "lz_tree_traverse_with_reuse: null argument");
-    LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_traverse_with_reuse: roots not prepared");
-    LZ_REQUIRE(!t->gumbel, LZ_ESTATE, "lz_tree_traverse_with_reuse: Gumbel tree, use lz_tree_traverse_gumbel");
-    TreeStep a = {};
-    a.traverse = 1; a.true_action = d_true_action; a.reuse_value = d_reuse_value;
-    a.ix = d_ix; a.iy = d_iy; a.act = d_last_action; a.len = d_search_len; a.vtp = d_virtual_to_play;
-    return tree_launch_step(t, a, (cudaStream_t)s);
-}
-
-int lz_tree_backpropagate_with_reuse(lz_tree *t, int latent_index, const float *d_reward, const float *d_value, const float *d_logits,
-                                     const float *d_reuse_value, const int32_t *d_batch_rank, const int32_t *d_is_reset,
-                                     const int32_t *d_to_play, lz_stream s)
-{
-    LZ_REQUIRE(t && d_reward && d_value && d_logits && d_reuse_value, LZ_EINVAL, "lz_tree_backpropagate_with_reuse: null argument");
-    LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_backpropagate_with_reuse: roots not prepared");
-    LZ_REQUIRE(!t->gumbel, LZ_ESTATE, "lz_tree_backpropagate_with_reuse: Gumbel tree, use lz_tree_backpropagate_gumbel");
-    LZ_REQUIRE(!t->p.ez || d_is_reset, LZ_EINVAL, "lz_tree_backpropagate_with_reuse: EfficientZero trees need d_is_reset");
-    LZ_REQUIRE(latent_index >= 1 && latent_index <= t->max_sims, LZ_EINVAL,
-               "lz_tree_backpropagate_with_reuse: latent_index %d outside [1, %d]", latent_index, t->max_sims);
-    TreeStep a = {};
-    a.latent_index = latent_index; a.reward = d_reward; a.value = d_value; a.logits = d_logits; a.to_play = d_to_play;
-    a.leaf_reset = d_is_reset; a.batch_rank = d_batch_rank; a.reuse_value = d_reuse_value;
-    return tree_launch_step(t, a, (cudaStream_t)s);
 }
 
 int lz_tree_select_action(lz_tree *t, float temperature, int deterministic, uint64_t seed, int32_t *d_action,

@@ -11,9 +11,6 @@ Tie-breaking: the reference draws ``rand() % len(ties)`` reseeded from the wall 
 deterministic switch; this module always takes the first maximum, which is that draw with ``rand() == 0`` (the
 configuration in which the parity tests build the unmodified reference, see DESIGN.md).
 """
-import torch
-
-from . import cabi
 from . import mz_tree as _mz
 from .mz_tree import MinMaxStatsList, ResultsWrapper, _to_dev  # noqa: F401  (identical classes)
 
@@ -31,25 +28,14 @@ def batch_traverse(roots: Roots, pb_c_base: int, pb_c_init: float, discount_fact
                    return_tensors: bool = False):
     """ez_tree.pyx batch_traverse -> (latent_state_index_in_search_path, latent_state_index_in_batch, last_actions,
     virtual_to_play_batch)."""
-    t = roots._need_tree()
-    t.set_params(pb_c_base, pb_c_init, discount_factor, min_max_stats_lst.value_delta_max)
-    with torch.cuda.device(roots.device):
-        cabi.check(t.lib.lz_tree_traverse_ez(t.h, t.ix.data_ptr(), t.iy.data_ptr(), t.action.data_ptr(),
-                                             t.search_len.data_ptr(), t.vtp.data_ptr(), None, cabi.stream_ptr()),
-                   "lz_tree_traverse_ez")
-    return _mz._traversed(roots, results, return_tensors)
+    roots._need_tree().set_params(pb_c_base, pb_c_init, discount_factor, min_max_stats_lst.value_delta_max)
+    return _mz._traverse(roots, results, return_tensors)
 
 
 def batch_backpropagate(current_latent_state_index: int, discount_factor: float, value_prefixs, values, policies,
                         min_max_stats_lst: MinMaxStatsList, results: ResultsWrapper, is_reset_list, to_play_batch):
     """ez_tree.pyx batch_backpropagate"""
-    roots, t, vp, val, pol, tp = _mz._backup_inputs(results, value_prefixs, values, policies, to_play_batch)
-    rs = _to_dev(is_reset_list, torch.int32, roots.device, (roots.root_num,))
-    with torch.cuda.device(roots.device):
-        cabi.check(t.lib.lz_tree_backpropagate_ez(t.h, int(current_latent_state_index), vp.data_ptr(), val.data_ptr(),
-                                                  pol.data_ptr(), rs.data_ptr(), cabi.ptr(tp), cabi.stream_ptr()),
-                   "lz_tree_backpropagate_ez")
-    t._keep = (vp, val, pol, rs, tp)
+    _mz._backpropagate(results, current_latent_state_index, value_prefixs, values, policies, to_play_batch, is_reset_list)
 
 
 def batch_traverse_with_reuse(roots: Roots, pb_c_base: int, pb_c_init: float, discount_factor: float,

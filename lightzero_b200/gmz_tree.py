@@ -3,7 +3,7 @@
 ``get_policies`` and the read-outs), ``MinMaxStatsList``, ``ResultsWrapper``, ``batch_traverse`` and
 ``batch_back_propagate`` with the same names, argument order and meaning, so the reference search loop
 (mcts_ctree.py:1104-1172) runs unchanged on it.  Every list argument may also be a numpy array or a CUDA tensor.  State
-lives in the CUDA trees behind ``lz_tree_*_gumbel`` (include/lzb200.h); nothing here computes on the CPU.
+lives in the CUDA Gumbel trees behind ``lz_tree_*`` (include/lzb200.h); nothing here computes on the CPU.
 
 Differences a caller can observe: ``batch_traverse`` returns the device tree's virtual to_play, which is the roots'
 to_play given at prepare (the reference returns the ``virtual_to_play_batch`` argument unchanged, and its search loop
@@ -83,19 +83,9 @@ class Roots(mz_tree.Roots):
         return self._tree
 
     def _materialize_gumbel(self, g, params=None):
-        self._acquire(g[1], params, True, gumbel=g)     # the Gumbel descents never read the tie rule
+        t = self._acquire(g[1], params, True, gumbel=g)     # the Gumbel descents never read the tie rule
         self._gumbel = g
-        self._reset_and_prepare()
-
-    def _reset_and_prepare(self):
-        """Reset to the legal lists and lz_tree_prepare_gumbel: a fresh search on these roots."""
-        t, p = self._tree, self._pending
-        with torch.cuda.device(self.device):
-            s = cabi.stream_ptr()
-            self._reset_tree(t, s)
-            cabi.check(t.lib.lz_tree_prepare_gumbel(t.h, p["logits"].data_ptr(), cabi.ptr(p["noise"]), p["w"],
-                                                    cabi.ptr(p["rewards"]), self._values.data_ptr(), cabi.ptr(p["to_play"]), s),
-                       "lz_tree_prepare_gumbel")
+        self._reset_and_prepare(t)
 
     def _materialize(self, max_sims, params=None, deterministic=None):
         # a re-prepare of a materialised tree (mz_tree.Roots._stage) starts a fresh Gumbel search
@@ -108,21 +98,12 @@ def batch_traverse(roots: Roots, num_simulations: int, max_num_considered_action
                    results: ResultsWrapper, virtual_to_play_batch, return_tensors: bool = False):
     """gmz_tree.pyx:91-95 -> (latent_state_index_in_search_path, latent_state_index_in_batch, last_actions,
     virtual_to_play_batch)."""
-    t = roots._setup(max_num_considered_actions, num_simulations, discount)
-    with torch.cuda.device(roots.device):
-        cabi.check(t.lib.lz_tree_traverse_gumbel(t.h, t.ix.data_ptr(), t.iy.data_ptr(), t.action.data_ptr(),
-                                                 t.search_len.data_ptr(), t.vtp.data_ptr(), cabi.stream_ptr()),
-                   "lz_tree_traverse_gumbel")
-    return mz_tree._traversed(roots, results, return_tensors)
+    roots._setup(max_num_considered_actions, num_simulations, discount)
+    return mz_tree._traverse(roots, results, return_tensors)
 
 
 def batch_back_propagate(current_latent_state_index: int, discount: float, value_prefixs, values, policies,
                          min_max_stats_lst: MinMaxStatsList, results: ResultsWrapper, to_play_batch):
     """gmz_tree.pyx:81-88"""
     results._roots._set_discount(float(discount))
-    roots, t, rew, val, pol, tp = mz_tree._backup_inputs(results, value_prefixs, values, policies, to_play_batch)
-    with torch.cuda.device(roots.device):
-        cabi.check(t.lib.lz_tree_backpropagate_gumbel(t.h, int(current_latent_state_index), rew.data_ptr(), val.data_ptr(),
-                                                      pol.data_ptr(), cabi.ptr(tp), cabi.stream_ptr()),
-                   "lz_tree_backpropagate_gumbel")
-    t._keep = (rew, val, pol, tp)
+    mz_tree._backpropagate(results, current_latent_state_index, value_prefixs, values, policies, to_play_batch)

@@ -129,14 +129,12 @@ class MuZeroMCTSCtree(object):
             raise NotImplementedError("search_with_reuse is fused only: pass a lightzero_b200 MuZeroModel / MuZeroModelMLP "
                                       "(or drive mz_tree.batch_traverse_with_reuse / batch_backpropagate_with_reuse yourself)")
         S = int(self._cfg.num_simulations)
-        lat = _dev_f32(latent_state_roots, roots.device)
-        return self._run_with_reuse(roots, model, S, (), true_action_list, reuse_value_list,
-                                    lambda lib, q, ta, rv, counts, s: cabi.check(
-                                        lib.lz_search_run_with_reuse(q, lat.data_ptr(), ta, rv, counts, s), "lz_search_run_with_reuse"))
+        return self._run_with_reuse(roots, model, S, (), (_dev_f32(latent_state_roots, roots.device), None, None),
+                                    true_action_list, reuse_value_list)
 
-    def _run_with_reuse(self, roots, model, S, mode, true_action_list, reuse_value_list, run):
-        """The fused search_with_reuse of either tree family: ``run(lib, q, true_action, reuse_value, counts, stream)`` runs
-        the search on the staged device pointers; returns the reference's ``(length, average_infer)``."""
+    def _run_with_reuse(self, roots, model, S, mode, roots_state, true_action_list, reuse_value_list):
+        """The fused search_with_reuse (lz_search_run_with_reuse) of either tree family from ``roots_state`` = (latents, LSTM
+        h, LSTM c; None for MuZero); returns the reference's ``(length, average_infer)``."""
         roots._materialize(S, self._params(), self.deterministic)     # the reference draws rand() % len(ties) (cnode.cpp:610-640)
         t, dev, B = roots._tree, roots.device, roots.num
         ta = mz_tree._to_dev(true_action_list, torch.int32, dev, (B,))
@@ -144,7 +142,8 @@ class MuZeroMCTSCtree(object):
         counts = torch.empty(S, dtype=torch.int32, device=dev)
         q = t.search_for(model, S, mode)
         with torch.cuda.device(dev):
-            run(t.lib, q, ta.data_ptr(), rv.data_ptr(), counts.data_ptr(), cabi.stream_ptr())
+            cabi.check(t.lib.lz_search_run_with_reuse(q, *(cabi.ptr(x) for x in roots_state), ta.data_ptr(), rv.data_ptr(),
+                                                      counts.data_ptr(), cabi.stream_ptr()), "lz_search_run_with_reuse")
         self.last_num_kernels = t.lib.lz_search_num_kernels(q)
         c = counts.cpu().numpy()
         return int(c[-1]), float(c.sum()) / S
@@ -164,8 +163,9 @@ class MuZeroMCTSCtree(object):
         vr, rr = rng("value_support_range"), rng("reward_support_range")
         self._inv_reward = self._inv if vr == rr else InverseScalarTransform(DiscreteSupport(*rr, device=dev))
 
-    def _search_stepwise(self, roots, model, lat, S, gumbel=False):
-        """The search driven one simulation at a time around any model object (gumbel: on Gumbel trees)."""
+    def _search_stepwise(self, roots, model, lat, S):
+        """The search driven one simulation at a time around any model object, on the descent and back-up of the tree's mode
+        (MuZero or Gumbel)."""
         t = roots._tree
         dev = roots.device
         self._make_inverse_transforms(dev)
@@ -173,25 +173,21 @@ class MuZeroMCTSCtree(object):
         pool = torch.empty((S + 1,) + tuple(lat.shape), device=dev, dtype=torch.float32)
         pool[0] = lat
         rows = torch.arange(B, device=dev)
-        backprop = "lz_tree_backpropagate_gumbel" if gumbel else "lz_tree_backpropagate"
         with torch.no_grad(), torch.cuda.device(dev):
             if hasattr(model, "eval"):
                 model.eval()
             for sim in range(S):
-                leaves = (t.ix.data_ptr(), t.iy.data_ptr(), t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(),
-                          cabi.stream_ptr())
-                if gumbel:
-                    cabi.check(t.lib.lz_tree_traverse_gumbel(t.h, *leaves), "lz_tree_traverse_gumbel")
-                else:
-                    cabi.check(t.lib.lz_tree_traverse(t.h, int(self.deterministic), *leaves), "lz_tree_traverse")
+                cabi.check(t.lib.lz_tree_traverse(t.h, int(self.deterministic), None, None, t.ix.data_ptr(), t.iy.data_ptr(),
+                                                  t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(), None,
+                                                  cabi.stream_ptr()), "lz_tree_traverse")
                 latent_states = pool[t.ix.long(), rows]                       # mcts_ctree.py:323-324 on device
                 out = model.recurrent_inference(latent_states, t.action.long())
                 pool[sim + 1] = out.latent_state
                 value = self._inv(out.value).reshape(-1).contiguous()        # :349 (value support)
                 reward = self._inv_reward(out.reward).reshape(-1).contiguous()      # :350 (reward support)
                 pol = out.policy_logits.to(torch.float32).contiguous()
-                cabi.check(getattr(t.lib, backprop)(t.h, sim + 1, reward.data_ptr(), value.data_ptr(), pol.data_ptr(), None,
-                                                    cabi.stream_ptr()), backprop)
+                cabi.check(t.lib.lz_tree_backpropagate(t.h, sim + 1, reward.data_ptr(), value.data_ptr(), pol.data_ptr(), None,
+                                                       None, None, None, cabi.stream_ptr()), "lz_tree_backpropagate")
 
 
 class EfficientZeroMCTSCtree(MuZeroMCTSCtree):
@@ -235,7 +231,7 @@ class EfficientZeroMCTSCtree(MuZeroMCTSCtree):
 
     def search_with_reuse(self, roots: "ez_tree.Roots", model, latent_state_roots, reward_hidden_state_roots,
                           to_play_batch: Union[int, List[Any]], true_action_list=None, reuse_value_list=None):
-        """mcts_ctree.py:878-1003 (ReZero on the EfficientZero trees) as one CUDA graph (``lz_search_run_ez_with_reuse``); returns
+        """mcts_ctree.py:878-1003 (ReZero on the EfficientZero trees) as one CUDA graph (``lz_search_run_with_reuse``); returns
         ``(length, average_infer)`` like the reference.  Fused only: other model objects drive
         ``ez_tree.batch_traverse_with_reuse`` / ``batch_backpropagate_with_reuse`` themselves."""
         S, H = int(self._cfg.num_simulations), int(self._cfg.lstm_horizon_len)
@@ -244,10 +240,8 @@ class EfficientZeroMCTSCtree(MuZeroMCTSCtree):
             raise NotImplementedError("EfficientZeroMCTSCtree.search_with_reuse is fused only: pass a lightzero_b200 EfficientZeroModel "
                                       "or EfficientZeroModelMLP")
         roots._ez, roots._lstm_horizon = True, H
-        lat, h0, h1 = self._ez_inputs(roots, latent_state_roots, reward_hidden_state_roots)
-        return self._run_with_reuse(roots, model, S, (1, H), true_action_list, reuse_value_list,
-                                    lambda lib, q, ta, rv, counts, s: cabi.check(lib.lz_search_run_ez_with_reuse(
-                                        q, lat.data_ptr(), h0.data_ptr(), h1.data_ptr(), ta, rv, counts, s), "lz_search_run_ez_with_reuse"))
+        return self._run_with_reuse(roots, model, S, (1, H), self._ez_inputs(roots, latent_state_roots, reward_hidden_state_roots),
+                                    true_action_list, reuse_value_list)
 
     @staticmethod
     def _ez_inputs(roots, latent_state_roots, reward_hidden_state_roots):
@@ -271,9 +265,9 @@ class EfficientZeroMCTSCtree(MuZeroMCTSCtree):
             if hasattr(model, "eval"):
                 model.eval()
             for sim in range(S):
-                cabi.check(t.lib.lz_tree_traverse_ez(t.h, t.ix.data_ptr(), t.iy.data_ptr(), t.action.data_ptr(),
-                                                     t.search_len.data_ptr(), t.vtp.data_ptr(), reset.data_ptr(),
-                                                     cabi.stream_ptr()), "lz_tree_traverse_ez")
+                cabi.check(t.lib.lz_tree_traverse(t.h, 0, None, None, t.ix.data_ptr(), t.iy.data_ptr(), t.action.data_ptr(),
+                                                  t.search_len.data_ptr(), t.vtp.data_ptr(), reset.data_ptr(),
+                                                  cabi.stream_ptr()), "lz_tree_traverse")
                 ix = t.ix.long()
                 hidden = (hp0[ix, rows].unsqueeze(0), hp1[ix, rows].unsqueeze(0))          # mcts_ctree.py:819-831
                 out = model.recurrent_inference(pool[ix, rows], hidden, t.action.long())
@@ -284,9 +278,8 @@ class EfficientZeroMCTSCtree(MuZeroMCTSCtree):
                 value = self._inv(out.value).reshape(-1).contiguous()
                 vprefix = self._inv_reward(out.value_prefix).reshape(-1).contiguous()
                 pol = out.policy_logits.to(torch.float32).contiguous()
-                cabi.check(t.lib.lz_tree_backpropagate_ez(t.h, sim + 1, vprefix.data_ptr(), value.data_ptr(), pol.data_ptr(),
-                                                          reset.data_ptr(), None, cabi.stream_ptr()),
-                           "lz_tree_backpropagate_ez")
+                cabi.check(t.lib.lz_tree_backpropagate(t.h, sim + 1, vprefix.data_ptr(), value.data_ptr(), pol.data_ptr(), None,
+                                                       None, reset.data_ptr(), None, cabi.stream_ptr()), "lz_tree_backpropagate")
 
 
 class UniZeroMCTSCtree(MuZeroMCTSCtree):
@@ -321,8 +314,8 @@ class UniZeroMCTSCtree(MuZeroMCTSCtree):
             if hasattr(model, "eval"):
                 model.eval()
             for simulation_index in range(S):
-                cabi.check(t.lib.lz_tree_traverse(t.h, int(self.deterministic), t.ix.data_ptr(), t.iy.data_ptr(),
-                                                  t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(),
+                cabi.check(t.lib.lz_tree_traverse(t.h, int(self.deterministic), None, None, t.ix.data_ptr(), t.iy.data_ptr(),
+                                                  t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(), None,
                                                   cabi.stream_ptr()), "lz_tree_traverse")
                 ix, iy = t.ix.cpu().numpy(), t.iy.cpu().numpy()
                 last_actions = t.action.cpu().long()
@@ -349,7 +342,8 @@ class UniZeroMCTSCtree(MuZeroMCTSCtree):
                         first_action_latent_map[env_id][a] = latent[env_id]
                 latent_pool.append(latent)
                 cabi.check(t.lib.lz_tree_backpropagate(t.h, simulation_index + 1, reward.data_ptr(), value.data_ptr(),
-                                                       pol.data_ptr(), None, cabi.stream_ptr()), "lz_tree_backpropagate")
+                                                       pol.data_ptr(), None, None, None, None, cabi.stream_ptr()),
+                           "lz_tree_backpropagate")
         return first_action_latent_map
 
 
@@ -359,9 +353,9 @@ class GumbelMuZeroMCTSCtree(MuZeroMCTSCtree):
     legal_actions)`` and ``search(roots, model, latent_state_roots, to_play_batch)``.  The roots are ``gmz_tree.Roots``
     prepared with the 6-argument ``prepare`` (or ``prepare_no_noise``).
 
-    With a ``lightzero_b200`` ``MuZeroModel`` / ``MuZeroModelMLP`` the whole loop is one CUDA-graph launch
-    (``lz_search_run_gumbel``): Gumbel descent, recurrent_inference and back-up for every simulation.  Any other model object
-    is driven step-wise around the device trees.  The search is deterministic like the reference's (no rand() on its path)."""
+    With a ``lightzero_b200`` ``MuZeroModel`` / ``MuZeroModelMLP`` the whole loop is one CUDA-graph launch (``lz_search_run``
+    on the Gumbel tree): Gumbel descent, recurrent_inference and back-up for every simulation.  Any other model object is
+    driven step-wise around the device trees.  The search is deterministic like the reference's (no rand() on its path)."""
     config = dict(
         num_simulations=50,
         root_dirichlet_alpha=0.3,
@@ -392,9 +386,9 @@ class GumbelMuZeroMCTSCtree(MuZeroMCTSCtree):
         t = roots._tree
         lat = _dev_f32(latent_state_roots, roots.device)
         if family is None:
-            self._search_stepwise(roots, model, lat, S, gumbel=True)
+            self._search_stepwise(roots, model, lat, S)
             return
         q = t.search_for(model, S, ("gumbel",))
         with torch.cuda.device(roots.device):
-            cabi.check(t.lib.lz_search_run_gumbel(q, lat.data_ptr(), cabi.stream_ptr()), "lz_search_run_gumbel")
+            cabi.check(t.lib.lz_search_run(q, lat.data_ptr(), 1, cabi.stream_ptr()), "lz_search_run")
         self.last_num_kernels = t.lib.lz_search_num_kernels(q)

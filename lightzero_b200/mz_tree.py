@@ -204,6 +204,7 @@ class Roots:
             self._legal_lists = [list(l) for l in legal_actions_list]
             assert len(self._legal_lists) == root_num
         self._pending = None      # prepare() arguments until the tree is materialised
+        self._values = None       # root value estimates of a Gumbel tree's prepare (set by gmz_tree.Roots)
         self._ez, self._lstm_horizon = False, 5     # EfficientZero value-prefix semantics (set by ez_tree.Roots)
         self._deterministic = True     # tie rule of the EfficientZero / *_with_reuse descents (the mirrors: first maximum)
         self._tree: Optional[TreeHandle] = None
@@ -304,13 +305,16 @@ class Roots:
     def _materialize(self, max_sims: int, params=None, deterministic=None):
         """Reset + prepare on device in a pooled tree of at least max_sims simulations.  ``deterministic``: the tie rule the
         holder searches with (MCTS searches pass their own); None keeps these roots' rule."""
-        t = self._acquire(max_sims, params, deterministic)
+        self._reset_and_prepare(self._acquire(max_sims, params, deterministic))
+
+    def _reset_and_prepare(self, t):
+        """Reset tree t to the legal lists and lz_tree_prepare it: a fresh search on these roots."""
         p = self._pending
         with torch.cuda.device(self.device):
             s = cabi.stream_ptr()
             self._reset_tree(t, s)
-            cabi.check(t.lib.lz_tree_prepare(t.h, p["logits"].data_ptr(), cabi.ptr(p["noise"]), p["w"],
-                                             cabi.ptr(p["rewards"]), cabi.ptr(p["to_play"]), s), "lz_tree_prepare")
+            cabi.check(t.lib.lz_tree_prepare(t.h, p["logits"].data_ptr(), cabi.ptr(p["noise"]), p["w"], cabi.ptr(p["rewards"]),
+                                             cabi.ptr(self._values), cabi.ptr(p["to_play"]), s), "lz_tree_prepare")
 
     def _acquire(self, max_sims, params, deterministic, gumbel=(0, 0)) -> TreeHandle:
         """This Roots' pooled tree, at least max_sims deep and in its whole mode (TreeHandle.set_mode)."""
@@ -354,23 +358,43 @@ class Roots:
                     self._keep = (dl, dn)
 
 
-def _traversed(roots: Roots, results: ResultsWrapper, return_tensors: bool):
-    """What every batch_traverse returns once its descent is queued: (latent_state_index_in_search_path,
-    latent_state_index_in_batch, last_actions, virtual_to_play_batch) as lists, or the device tensors."""
-    results._roots = roots
+def _traverse(roots: Roots, results: ResultsWrapper, return_tensors: bool, deterministic=False, true_action=None,
+              reuse_value=None):
+    """lz_tree_traverse of the roots' tree, the descent of its mode (reuse with true_action / reuse_value), and what every
+    batch_traverse returns: (latent_state_index_in_search_path, latent_state_index_in_batch, last_actions,
+    virtual_to_play_batch) as lists, or the device tensors."""
     t = roots._tree
+    dev = roots.device
+    ta = _to_dev(true_action, torch.int32, dev, (roots.root_num,))
+    rv = _to_dev(reuse_value, torch.float32, dev, (roots.root_num,))
+    with torch.cuda.device(dev):
+        cabi.check(t.lib.lz_tree_traverse(t.h, int(bool(deterministic)), cabi.ptr(ta), cabi.ptr(rv), t.ix.data_ptr(),
+                                          t.iy.data_ptr(), t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(),
+                                          None, cabi.stream_ptr()), "lz_tree_traverse")
+    if rv is not None:
+        t._keep = (ta, rv)
+    results._roots = roots
     if return_tensors:
         return t.ix, t.iy, t.action, t.vtp
     return tuple(x.tolist() for x in torch.stack((t.ix, t.iy, t.action, t.vtp)).cpu().numpy())
 
 
-def _backup_inputs(results: ResultsWrapper, value_prefixs, values, policies, to_play_batch):
-    """The inputs every batch_backpropagate stages on the device -> (roots, tree, rewards or value prefixes, values,
-    policy logits, to_play or None)."""
+def _backpropagate(results: ResultsWrapper, current_latent_state_index: int, value_prefixs, values, policies, to_play_batch,
+                   is_reset_list=None):
+    """lz_tree_backpropagate of the tree the last batch_traverse descended, the back-up of its mode, on the inputs every
+    batch_backpropagate stages on the device: rewards (value prefixes on an EfficientZero tree, with is_reset_list), values,
+    policy logits, to_play or None."""
     roots = results._roots
-    B, A, dev = roots.root_num, roots._tree.A, roots.device
-    return (roots, roots._tree, _to_dev(value_prefixs, torch.float32, dev, (B,)), _to_dev(values, torch.float32, dev, (B,)),
-            _to_dev(policies, torch.float32, dev, (B, A)), _to_dev(to_play_batch, torch.int32, dev, (B,)))
+    t = roots._tree
+    B, A, dev = roots.root_num, t.A, roots.device
+    rew, val = _to_dev(value_prefixs, torch.float32, dev, (B,)), _to_dev(values, torch.float32, dev, (B,))
+    pol, tp = _to_dev(policies, torch.float32, dev, (B, A)), _to_dev(to_play_batch, torch.int32, dev, (B,))
+    rs = _to_dev(is_reset_list, torch.int32, dev, (B,))
+    with torch.cuda.device(dev):
+        cabi.check(t.lib.lz_tree_backpropagate(t.h, int(current_latent_state_index), rew.data_ptr(), val.data_ptr(),
+                                               pol.data_ptr(), None, None, cabi.ptr(rs), cabi.ptr(tp), cabi.stream_ptr()),
+                   "lz_tree_backpropagate")
+    t._keep = (rew, val, pol, rs, tp)
 
 
 def batch_traverse(roots: Roots, pb_c_base: int, pb_c_init: float, discount_factor: float,
@@ -378,24 +402,14 @@ def batch_traverse(roots: Roots, pb_c_base: int, pb_c_init: float, discount_fact
                    deterministic: bool = False, return_tensors: bool = False):
     """mz_tree.pyx:94-99 -> (latent_state_index_in_search_path, latent_state_index_in_batch, last_actions,
     virtual_to_play_batch)."""
-    t = roots._need_tree()
-    t.set_params(pb_c_base, pb_c_init, discount_factor, min_max_stats_lst.value_delta_max)
-    with torch.cuda.device(roots.device):
-        cabi.check(t.lib.lz_tree_traverse(t.h, int(bool(deterministic)), t.ix.data_ptr(), t.iy.data_ptr(),
-                                          t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(),
-                                          cabi.stream_ptr()), "lz_tree_traverse")
-    return _traversed(roots, results, return_tensors)
+    roots._need_tree().set_params(pb_c_base, pb_c_init, discount_factor, min_max_stats_lst.value_delta_max)
+    return _traverse(roots, results, return_tensors, deterministic)
 
 
 def batch_backpropagate(current_latent_state_index: int, discount_factor: float, value_prefixs, values, policies,
                         min_max_stats_lst: MinMaxStatsList, results: ResultsWrapper, to_play_batch):
     """mz_tree.pyx:73-82"""
-    roots, t, rew, val, pol, tp = _backup_inputs(results, value_prefixs, values, policies, to_play_batch)
-    with torch.cuda.device(roots.device):
-        cabi.check(t.lib.lz_tree_backpropagate(t.h, int(current_latent_state_index), rew.data_ptr(), val.data_ptr(),
-                                               pol.data_ptr(), cabi.ptr(tp), cabi.stream_ptr()),
-                   "lz_tree_backpropagate")
-    t._keep = (rew, val, pol, tp)
+    _backpropagate(results, current_latent_state_index, value_prefixs, values, policies, to_play_batch)
 
 
 def batch_traverse_with_reuse(roots: Roots, pb_c_base: int, pb_c_init: float, discount_factor: float,
@@ -403,17 +417,8 @@ def batch_traverse_with_reuse(roots: Roots, pb_c_base: int, pb_c_init: float, di
                               true_action, reuse_value, return_tensors: bool = False):
     """mz_tree.pyx batch_traverse_with_reuse (cnode.cpp:828-932): ``latent_state_index_in_search_path`` is -1 for trees
     that stopped on an already expanded child of the root (no inference needed)."""
-    t = roots._need_tree()
-    t.set_params(pb_c_base, pb_c_init, discount_factor, min_max_stats_lst.value_delta_max)
-    dev = roots.device
-    ta = _to_dev(true_action, torch.int32, dev, (roots.root_num,))
-    rv = _to_dev(reuse_value, torch.float32, dev, (roots.root_num,))
-    with torch.cuda.device(dev):
-        cabi.check(t.lib.lz_tree_traverse_with_reuse(t.h, ta.data_ptr(), rv.data_ptr(), t.ix.data_ptr(), t.iy.data_ptr(),
-                                                     t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(),
-                                                     cabi.stream_ptr()), "lz_tree_traverse_with_reuse")
-    t._keep = (ta, rv)
-    return _traversed(roots, results, return_tensors)
+    roots._need_tree().set_params(pb_c_base, pb_c_init, discount_factor, min_max_stats_lst.value_delta_max)
+    return _traverse(roots, results, return_tensors, true_action=true_action, reuse_value=reuse_value)
 
 
 def batch_backpropagate_with_reuse(current_latent_state_index: int, discount_factor: float, value_prefixs, values, policies,
@@ -444,7 +449,7 @@ def batch_backpropagate_with_reuse(current_latent_state_index: int, discount_fac
     tp = _to_dev(to_play_batch, torch.int32, dev, (B,))
     rs = _to_dev(_is_reset_list, torch.int32, dev, (B,))
     with torch.cuda.device(dev):
-        cabi.check(t.lib.lz_tree_backpropagate_with_reuse(t.h, int(current_latent_state_index), rew.data_ptr(), val.data_ptr(),
-                                                          pol.data_ptr(), rv.data_ptr(), rk.data_ptr(), cabi.ptr(rs), cabi.ptr(tp),
-                                                          cabi.stream_ptr()), "lz_tree_backpropagate_with_reuse")
+        cabi.check(t.lib.lz_tree_backpropagate(t.h, int(current_latent_state_index), rew.data_ptr(), val.data_ptr(),
+                                               pol.data_ptr(), rv.data_ptr(), rk.data_ptr(), cabi.ptr(rs), cabi.ptr(tp),
+                                               cabi.stream_ptr()), "lz_tree_backpropagate")
     t._keep = (rew, val, pol, rv, rk, rs, tp)

@@ -136,7 +136,7 @@ def compute_target_policy_reanalyzed_rezero(
         mini_infer_size: int = 10240, noises: Optional[np.ndarray] = None):
     """Mirror of ``ReZeroMZGameBuffer._compute_target_policy_reanalyzed`` (lzero/mcts/buffer/game_buffer_rezero_mz.py:194-404;
     with an ``EfficientZeroMCTSCtree``, ``ReZeroEZGameBuffer``'s, game_buffer_rezero_ez.py:126-330) as one device call
-    (``lz_rezero_reanalyze`` / ``_ez``): initial_inference over every row, the plain search of the last position, then
+    (``lz_rezero_reanalyze``): initial_inference over every row, the plain search of the last position, then
     ``length - 1`` search_with_reuse calls walking backward, each reusing the previous search's root values, and the targets.
 
     policy_obs [N * length, ...] (row = segment * length + position), action_mask [N * length, A] 0/1, to_play, true_action
@@ -175,7 +175,7 @@ def compute_target_policy_reanalyzed_rezero(
     dev = model.device
     H = int(cfg.lstm_horizon_len) if ez else 5
     mode = (1, H) if ez else ()
-    # the sweep's tie rule is the one lz_rezero_reanalyze* sets: the first maximum
+    # the sweep's tie rule is the one lz_rezero_reanalyze sets: the first maximum
     with torch.cuda.device(dev), mz_tree.held_tree(dev, N, A, S, mcts._params(), mode) as t:
         q = t.search_for(model, S, mode)
         s = cabi.stream_ptr()
@@ -190,14 +190,11 @@ def compute_target_policy_reanalyzed_rezero(
         values = torch.empty((N, L), dtype=torch.float32, device=dev)
         nreuse = L - 1 if reuse_search else 0
         counts = torch.empty((nreuse, S), dtype=torch.int32, device=dev)
-        head = (q, L, int(bool(reuse_search)), int(mini_infer_size), obs.data_ptr(), None, None, mask.data_ptr(),
-                tp.data_ptr(), ta.data_ptr(), pm.data_ptr(), cabi.ptr(nz), float(cfg.root_noise_weight))
-        tail = (int(action_type != "fixed_action_space"), targets.data_ptr(), values.data_ptr(), visits.data_ptr(),
-                counts.data_ptr() if nreuse else None, s)
-        if ez:
-            cabi.check(t.lib.lz_rezero_reanalyze_ez(*head, *tail), "lz_rezero_reanalyze_ez")
-        else:
-            cabi.check(t.lib.lz_rezero_reanalyze(*head, int(mcts.deterministic), *tail), "lz_rezero_reanalyze")
+        cabi.check(t.lib.lz_rezero_reanalyze(q, L, int(bool(reuse_search)), int(mini_infer_size), obs.data_ptr(), None, None,
+                                             mask.data_ptr(), tp.data_ptr(), ta.data_ptr(), pm.data_ptr(), cabi.ptr(nz),
+                                             float(cfg.root_noise_weight), int(mcts.deterministic),
+                                             int(action_type != "fixed_action_space"), targets.data_ptr(), values.data_ptr(),
+                                             visits.data_ptr(), counts.data_ptr() if nreuse else None, s), "lz_rezero_reanalyze")
         mcts.last_num_kernels = t.lib.lz_search_num_kernels(q)
         out, vis, val, cnt = targets.cpu().numpy(), visits.cpu().numpy(), values.cpu().numpy(), counts.cpu().numpy()
 

@@ -47,5 +47,5 @@ roots._materialize(S, (19652, 1.25, 0.997, 0.01))
 t = roots._tree
 rs = torch.zeros(B, dtype=torch.int32, device="cuda")
 def tree_step():
-    lib.lz_tree_traverse_ez(t.h, t.ix.data_ptr(), t.iy.data_ptr(), t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(), rs.data_ptr(), s)
+    lib.lz_tree_traverse(t.h, 0, None, None, t.ix.data_ptr(), t.iy.data_ptr(), t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(), rs.data_ptr(), s)
 print(f"tree traverse (EZ, shallow trees): {timeit(tree_step):.1f} us")

@@ -117,7 +117,8 @@ class _Proxy:
 @pytest.mark.parametrize("B,A,S,masks,horizon", [(16, 6, 20, False, 5), (256, 6, 50, False, 5), (130, 18, 40, True, 2)])
 def test_fused_ez_search_equals_stepwise_search(B, A, S, masks, horizon):
     """One CUDA graph for the whole search vs the step-wise drive of the same kernels through the public pieces
-    (lz_tree_traverse_ez / recurrent_inference / lz_tree_backpropagate_ez): identical visit counts and root value bits."""
+    (lz_tree_traverse / recurrent_inference / lz_tree_backpropagate on the EfficientZero tree): identical visit counts and root
+    value bits."""
     ref, cu, obs, mask, legal, noises, mcts = _setup(B, A, S, masks=masks, horizon=horizon)
     out = cu.initial_inference(obs.cuda())
     results = []
@@ -187,10 +188,10 @@ def test_ez_search_rejects_mismatched_model_and_tree():
         mz.search(roots, cu, out.latent_state, [-1] * 8)
 
 
-def test_fused_ez_search_with_reuse_equals_piecewise_drive():
+def test_fused_ez_search_with_reuse_equals_stepwise_reuse_drive():
     """EfficientZeroMCTSCtree.search_with_reuse (mcts_ctree.py:878-1003) as one CUDA graph vs the same steps driven one at a time
-    through the public pieces (lz_tree_traverse_with_reuse, EfficientZeroModel.recurrent_inference on every row,
-    lz_tree_backpropagate_with_reuse with the per-tree is_reset): identical visit counts, value bits and inference counts.
+    through the public pieces (the reuse lz_tree_traverse, EfficientZeroModel.recurrent_inference on every row, the reuse
+    lz_tree_backpropagate with the per-tree is_reset): identical visit counts, value bits and inference counts.
     (The tree entry points themselves are pinned to the shimmed reference ez_tree in test_gpu_tree.py.)"""
     from lightzero_b200 import cabi
     B, A, S, H = 64, 6, 25, 3
@@ -220,8 +221,8 @@ def test_fused_ez_search_with_reuse_equals_piecewise_drive():
     rows = torch.arange(B, device=dev)
     counts = []
     for sim in range(S):
-        cabi.check(t.lib.lz_tree_traverse_with_reuse(t.h, ta.data_ptr(), rv.data_ptr(), t.ix.data_ptr(), t.iy.data_ptr(), t.action.data_ptr(),
-                                                     t.search_len.data_ptr(), t.vtp.data_ptr(), cabi.stream_ptr()), "traverse")
+        cabi.check(t.lib.lz_tree_traverse(t.h, 0, ta.data_ptr(), rv.data_ptr(), t.ix.data_ptr(), t.iy.data_ptr(), t.action.data_ptr(),
+                                          t.search_len.data_ptr(), t.vtp.data_ptr(), None, cabi.stream_ptr()), "traverse")
         counts.append(int((t.ix >= 0).sum().item()))
         ix = t.ix.clamp(min=0).long()
         reset = (t.search_len % H == 0).to(torch.int32)
@@ -231,9 +232,9 @@ def test_fused_ez_search_with_reuse_equals_piecewise_drive():
         keep = (reset == 0).float().unsqueeze(1)
         hp0[sim + 1] = o.reward_hidden_state[0].reshape(B, -1) * keep
         hp1[sim + 1] = o.reward_hidden_state[1].reshape(B, -1) * keep
-        cabi.check(t.lib.lz_tree_backpropagate_with_reuse(t.h, sim + 1, o.value_prefix_scalar.data_ptr(), o.value_scalar.data_ptr(),
-                                                          o.policy_logits.data_ptr(), rv.data_ptr(), None, reset.data_ptr(), None,
-                                                          cabi.stream_ptr()), "backprop")
+        cabi.check(t.lib.lz_tree_backpropagate(t.h, sim + 1, o.value_prefix_scalar.data_ptr(), o.value_scalar.data_ptr(),
+                                               o.policy_logits.data_ptr(), rv.data_ptr(), None, reset.data_ptr(), None,
+                                               cabi.stream_ptr()), "backprop")
     step = (roots.get_distributions(), np.asarray(roots.get_values(), np.float32).view(np.uint32).tolist())
     assert fused == step
     assert length == counts[-1] and abs(avg - sum(counts) / S) < 1e-9

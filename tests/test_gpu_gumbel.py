@@ -213,7 +213,7 @@ def test_empty_legal_list_is_every_action():
     assert (outs[0]["distributions"][[0, 2]] >= 0).all()
 
 
-def test_refusals():
+def test_tree_entry_point_refusals():
     from lightzero_b200 import cabi
     lib = cabi.load()
     B, A, S = 4, 6, 3
@@ -224,23 +224,35 @@ def test_refusals():
         logits = torch.zeros(B, A, device=dev)
         vals = torch.zeros(B, device=dev)
         i32 = [torch.zeros(B, dtype=torch.int32, device=dev) for _ in range(5)]
+        leaves = [t.data_ptr() for t in i32] + [None]       # ix, iy, last action, search length, virtual to_play; no is_reset
         s = cabi.stream_ptr()
         cabi.check(lib.lz_tree_set_gumbel(h, A, S), "lz_tree_set_gumbel")
         assert lib.lz_tree_set_ez(h, 1, 5) < 0
         cabi.check(lib.lz_tree_reset(h, None, None, s), "lz_tree_reset")
-        assert lib.lz_tree_traverse_gumbel(h, *[t.data_ptr() for t in i32], s) < 0      # not prepared
-        cabi.check(lib.lz_tree_prepare_gumbel(h, logits.data_ptr(), None, 0.0, None, vals.data_ptr(), None, s), "prepare")
-        assert lib.lz_tree_traverse(h, 1, *[t.data_ptr() for t in i32], s) < 0           # MuZero call on a Gumbel tree
-        assert lib.lz_tree_backpropagate_gumbel(h, 1, vals.data_ptr(), vals.data_ptr(), logits.data_ptr(), None, s) < 0
+        assert lib.lz_tree_traverse(h, 1, None, None, *leaves, s) < 0                       # not prepared
+        assert lib.lz_tree_prepare(h, logits.data_ptr(), None, 0.0, None, None, None, s) < 0   # Gumbel roots need their values
+        cabi.check(lib.lz_tree_prepare(h, logits.data_ptr(), None, 0.0, None, vals.data_ptr(), None, s), "prepare")
+        ta = torch.zeros(B, dtype=torch.int32, device=dev)
+        assert lib.lz_tree_traverse(h, 1, ta.data_ptr(), vals.data_ptr(), *leaves, s) < 0   # reuse descent on a Gumbel tree
+        no_bp = lib.lz_tree_backpropagate(h, 1, vals.data_ptr(), vals.data_ptr(), logits.data_ptr(), None, None, None, None, s)
+        assert no_bp < 0                                                                  # back-up before any descent
         for sim in range(S):
-            cabi.check(lib.lz_tree_traverse_gumbel(h, *[t.data_ptr() for t in i32], s), "traverse")
-            cabi.check(lib.lz_tree_backpropagate_gumbel(h, sim + 1, vals.data_ptr(), vals.data_ptr(), logits.data_ptr(), None, s), "bp")
-        rc = lib.lz_tree_traverse_gumbel(h, *[t.data_ptr() for t in i32], s)                # one past num_simulations
+            cabi.check(lib.lz_tree_traverse(h, 1, None, None, *leaves, s), "traverse")
+            cabi.check(lib.lz_tree_backpropagate(h, sim + 1, vals.data_ptr(), vals.data_ptr(), logits.data_ptr(), None, None, None,
+                                                 None, s), "bp")
+        rc = lib.lz_tree_traverse(h, 1, None, None, *leaves, s)                             # one past num_simulations
         assert rc < 0 and b"considered-visit table" in lib.lz_last_error()
         torch.cuda.synchronize()
         cabi.check(lib.lz_tree_set_gumbel(h, 0, 0), "lz_tree_set_gumbel off")
+        assert lib.lz_tree_prepare(h, logits.data_ptr(), None, 0.0, None, vals.data_ptr(), None, s) == -1   # values: Gumbel only
+        assert lib.lz_tree_traverse(h, 1, None, None, *leaves[:5], i32[0].data_ptr(), s) == -1    # is_reset: EfficientZero only
+        assert lib.lz_tree_traverse(h, 1, ta.data_ptr(), None, *leaves, s) == -1                # half a reuse pair
+        assert lib.lz_tree_backpropagate(h, 1, vals.data_ptr(), vals.data_ptr(), logits.data_ptr(), None, ta.data_ptr(), None,
+                                         None, s) == -1                                         # batch rank without reuse
         cabi.check(lib.lz_tree_set_ez(h, 1, 5), "lz_tree_set_ez")
         assert lib.lz_tree_set_gumbel(h, A, S) < 0                                        # EfficientZero tree
+        assert lib.lz_tree_backpropagate(h, 1, vals.data_ptr(), vals.data_ptr(), logits.data_ptr(), None, None, None, None,
+                                         s) == -1                                               # EfficientZero needs is_reset
     finally:
         lib.lz_tree_destroy(h)
     import lightzero_b200 as lzb

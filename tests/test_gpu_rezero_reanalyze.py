@@ -1,4 +1,4 @@
-"""The ReZero reanalyze sweep (``compute_target_policy_reanalyzed_rezero``, ``lz_rezero_reanalyze`` / ``_ez``) against the
+"""The ReZero reanalyze sweep (``compute_target_policy_reanalyzed_rezero``, ``lz_rezero_reanalyze``) against the
 reference's own loop, bit for bit.
 
 The oracle restates ``ReZeroMZGameBuffer._compute_target_policy_reanalyzed`` (lzero/mcts/buffer/game_buffer_rezero_mz.py:194-404;

@@ -102,16 +102,16 @@ def test_gumbel_unit_has_no_fp32_contraction(tmp_path):
     assert ("gumbel.cu", ["-fmad=false"]) in _build.UNITS
 
 
-def test_gumbel_symbols_exported_and_no_device_is_loud():
+def test_gumbel_entry_points_exported_and_no_device_is_loud():
     from lightzero_b200 import _build, cabi
     lib = ctypes.CDLL(_build.build())
-    for name in ("lz_tree_set_gumbel", "lz_tree_prepare_gumbel", "lz_tree_traverse_gumbel", "lz_tree_backpropagate_gumbel",
-                 "lz_tree_gumbel_policies", "lz_search_run_gumbel", "lz_gumbel_tables"):
+    for name in ("lz_tree_set_gumbel", "lz_tree_prepare", "lz_tree_traverse", "lz_tree_backpropagate",
+                 "lz_tree_gumbel_policies", "lz_search_run", "lz_gumbel_tables"):
         assert hasattr(lib, name) and name in cabi.SIGNATURES, name
     lib = cabi.load()
     assert lib.lz_gumbel_tables(4, 0, 6, None, None) < 0 and b"bad arguments" in lib.lz_last_error()
     assert lib.lz_tree_set_gumbel(None, 4, 50) < 0
-    assert lib.lz_search_run_gumbel(None, None, None) < 0
+    assert lib.lz_search_run(None, None, 1, None) < 0
     import torch
     if torch.cuda.is_available():
         return
