@@ -54,8 +54,9 @@ __device__ __forceinline__ float warp_max(float v)
 __device__ __forceinline__ void softmax_push(float &m, float &s, float &w, float x, float sup)
 {
     // one exponential per logit, no divergent branch: t = exp(-|x - m|) is the rescale factor of the old sums when x is the new
-    // maximum and the new term otherwise (exp(-inf) = 0 for the first logit)
-    const float t = __expf(-fabsf(x - m));      // ex2.approx: ~2 ulp; the terms that matter have |x - m| of a few units
+    // maximum and the new term otherwise (exp(-inf) = 0 for the first logit).  A -inf logit adds nothing: while m is still
+    // -inf, x - m would be NaN, so it is selected away (finite x take the same exponential as before).
+    const float t = x == -INFINITY ? 0.0f : __expf(-fabsf(x - m));   // ex2.approx: ~2 ulp; the terms that matter have |x - m| of a few units
     const bool gt = x > m;
     s = gt ? fmaf(s, t, 1.0f) : s + t;
     w = gt ? fmaf(w, t, sup) : fmaf(t, sup, w);

@@ -45,7 +45,7 @@ class EfficientZeroModelMLP(LzModel):
                                reward_head_hidden_channels[0], value_head_hidden_channels[0], policy_head_hidden_channels[0],
                                int(bool(res_connection_in_dynamics)), value_support_range[0], value_support_range[1],
                                value_support_range[2])
-        self._create(device, "lz_model_create_mlp_ez", cfg)
+        self._create(device, "lz_model_create_mlp_ez", cfg, value_support_range)
 
     def recurrent_inference(self, latent_state: torch.Tensor, reward_hidden_state, action: torch.Tensor,
                             return_scalars: bool = False) -> EZNetworkOutput:

@@ -10,6 +10,7 @@ from typing import Dict, Tuple
 import torch
 
 from . import cabi, mz_tree
+from .scaling_transform import check_support
 
 _model_serial = itertools.count(1)      # never reused (unlike id()): keys of the per-tree lz_search caches in mz_tree
 
@@ -40,7 +41,8 @@ class LzModel:
     _align_latents = False      # the MLP kernels read latent rows as 16-byte vectors
     MATH_MODES = {"tc3": 1, "tc1": 2}
 
-    def _create(self, device, create: str, cfg):
+    def _create(self, device, create: str, cfg, support_range):
+        check_support(support_range)
         if not torch.cuda.is_available():
             raise RuntimeError(f"lightzero_b200.{type(self).__name__} needs a CUDA device; there is no CPU fallback")
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())

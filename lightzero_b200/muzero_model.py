@@ -61,7 +61,7 @@ class MuZeroModel(LzModel):
                                value_support_range[2], int(efficientzero),
                                int(kwargs.get("lstm_hidden_size", 0) if efficientzero else 0), int(bool(downsample)))
         self._cfg = cfg
-        self._create(device, "lz_model_create", cfg)
+        self._create(device, "lz_model_create", cfg, value_support_range)
         self.latent_hw = self._lib.lz_model_latent_hw(self._h)
         shape = (cabi.ctypes.c_int32 * 3)()
         cabi.check(self._lib.lz_model_latent_shape(self._h, cabi.ctypes.byref(shape, 0), cabi.ctypes.byref(shape, 4),

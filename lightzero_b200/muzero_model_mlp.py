@@ -36,4 +36,4 @@ class MuZeroModelMLP(LzModel):
         cfg = cabi.MlpConfig(self.observation_shape, action_space_size, latent_state_dim, reward_head_hidden_channels[0],
                              value_head_hidden_channels[0], policy_head_hidden_channels[0], int(bool(res_connection_in_dynamics)),
                              value_support_range[0], value_support_range[1], value_support_range[2])
-        self._create(device, "lz_model_create_mlp", cfg)
+        self._create(device, "lz_model_create_mlp", cfg, value_support_range)
