@@ -145,8 +145,14 @@ int lz_model_create(const lz_model_config *cfg, lz_model **out)
                    "lz_model_create: observation %dx%d not supported (64x64 -> 8x8 latent, 84x84 and 96x96 -> 6x6 latent)", cfg->obs_h, cfg->obs_w);
     }
     LZ_REQUIRE(cfg->num_res_blocks >= 1 && cfg->num_res_blocks <= kMaxResBlocks, LZ_EINVAL, "lz_model_create: num_res_blocks must be in [1,%d]", kMaxResBlocks);
-    LZ_REQUIRE(cfg->reward_head_channels <= 16 && cfg->value_head_channels <= 16 && cfg->policy_head_channels <= 16, LZ_EINVAL, "lz_model_create: head channels must be <= 16");
-    LZ_REQUIRE(cfg->reward_hidden <= 32 && cfg->value_hidden <= 32 && cfg->policy_hidden <= 32, LZ_EINVAL, "lz_model_create: head hidden sizes must be <= 32");
+    LZ_REQUIRE(cfg->reward_head_channels >= 1 && cfg->reward_head_channels <= 16 && cfg->value_head_channels >= 1 &&
+                   cfg->value_head_channels <= 16 && cfg->policy_head_channels >= 1 && cfg->policy_head_channels <= 16,
+               LZ_EINVAL, "lz_model_create: head channels must be in [1, 16] (got %d, %d, %d)", cfg->reward_head_channels,
+               cfg->value_head_channels, cfg->policy_head_channels);
+    LZ_REQUIRE(cfg->reward_hidden >= 1 && cfg->reward_hidden <= 32 && cfg->value_hidden >= 1 && cfg->value_hidden <= 32 &&
+                   cfg->policy_hidden >= 1 && cfg->policy_hidden <= 32,
+               LZ_EINVAL, "lz_model_create: head hidden sizes must be in [1, 32] (got %d, %d, %d)", cfg->reward_hidden,
+               cfg->value_hidden, cfg->policy_hidden);
     LZ_REQUIRE(cfg->action_space_size >= 1 && cfg->action_space_size <= 1024, LZ_EINVAL, "lz_model_create: action_space_size out of range");
     int K = 0;
     int rc = check_create("lz_model_create", cfg->support_min, cfg->support_max, cfg->support_step, kKpad, &K);

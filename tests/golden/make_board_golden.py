@@ -1,5 +1,6 @@
 """Pin the board-network restatement (tests/board_model_ref.py) to the REFERENCE'S OWN MuZeroModel with downsample=False and
-generate tests/golden/board_{tictactoe,gomoku,connect4,board8x8_r3}.npz.
+generate tests/golden/board_<name>.npz for every config of tests/board_model_ref.BOARD_CONFIGS: the shipped boards and the
+corners (1x8 and 8x1 boards, 1 and 16 planes, 1 and 64 actions, 4 blocks, 1 and 16 head channels, 608 support bins).
 
 Run where the reference sources are (LZ_REFERENCE, default /root/reference):   python tests/golden/make_board_golden.py
 

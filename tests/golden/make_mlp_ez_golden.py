@@ -1,5 +1,5 @@
 """Pin the EfficientZeroModelMLP restatement (tests/mlp_ez_model_ref.py) to the REFERENCE'S OWN EfficientZeroModelMLP and generate
-tests/golden/mlp_ez_{cartpole,lunarlander,minigrid,bipedalwalker,defaults,l96_h48}.npz.
+tests/golden/mlp_ez_<name>.npz for every config of tests/mlp_ez_model_ref.CONFIGS.
 
 Run where the reference sources are (LZ_REFERENCE, default /root/reference):   python tests/golden/make_mlp_ez_golden.py
 

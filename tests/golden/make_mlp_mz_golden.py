@@ -1,6 +1,6 @@
 """Pin the MuZeroModelMLP restatement (oracle.model_ref.MuZeroModelMLPRef, configs of tests/mlp_mz_model_ref.py) to the
-REFERENCE'S OWN MuZeroModelMLP and generate tests/golden/mlp_mz_{lunarlander,l160_a18,l224_wide}.npz: the configs that run on
-the tensor-core MLP kernel.
+REFERENCE'S OWN MuZeroModelMLP and generate tests/golden/mlp_mz_<name>.npz for every config of tests/mlp_mz_model_ref.CONFIGS:
+the configs that run on the tensor-core MLP kernel.
 
 Run where the reference sources are (LZ_REFERENCE, default /root/reference):   python tests/golden/make_mlp_mz_golden.py
 

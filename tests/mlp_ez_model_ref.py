@@ -25,6 +25,12 @@ CONFIGS = {
     "bipedalwalker": (24, 256, 256, 256, True),     # zoo/box2d/bipedalwalker/config/bipedalwalker_cont_disc_efficientzero_config.py
     "defaults": (2, 6, 256, 512, False),            # the class defaults (efficientzero_model_mlp.py:16-40)
     "l96_h48": (5, 3, 96, 48, False),               # a shape of the fp32 LSTM kernel (k_ez_lstm: L, H not multiples of 64)
+    # the narrowest latent (k_mez_tc<1>) on a one-feature observation
+    "l32_o1": (1, 5, 32, 32, False),
+    # k_mez_tc<2> on the widest observation: 128 streamed 32-feature chunks
+    "l64_o4096": (4096, 3, 64, 64, True),
+    # k_mez_tc<6>
+    "l192": (40, 9, 192, 96, False),
 }
 
 

@@ -21,6 +21,11 @@ CONFIGS = {
     "l160_a18": (200, 18, 160, False, 32, (-300., 301., 1.)),
     # a wide observation, narrow head hidden layers and a small support
     "l224_wide": (1000, 64, 224, True, 16, (-10., 11., 1.)),
+    # the longest recurrent program: 4 dense dynamics layers, the reward head, 2 prediction layers and the value and policy heads,
+    # with 608 support bins and 608 actions cut into 19 FC2 pieces each at L = 32: 66 layers, the kernel's limit
+    "l32_a608": (8, 608, 32, True, 32, (-304., 304., 1.)),
+    # the widest observation and head hidden layers of a single unit
+    "l96_o4096_h1": (4096, 6, 96, False, 1, (-300., 301., 1.)),
 }
 
 

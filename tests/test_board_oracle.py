@@ -36,6 +36,9 @@ def test_restatement_reproduces_the_fixture(name):
         assert torch.equal(getattr(o0, f), torch.from_numpy(d["init_" + f])), f
     for f in ("value", "reward", "policy_logits", "latent_state"):
         assert torch.equal(getattr(o1, f), torch.from_numpy(d["rec_" + f])), f
+    for f in ("init_value", "init_policy_logits", "rec_reward", "rec_value", "rec_policy_logits"):
+        x = d[f]
+        assert (x != x[:1]).any(), f        # every head depends on its root: none is a dead ReLU that outputs its bias
 
 
 @pytest.mark.parametrize("name", NAMES)

@@ -111,10 +111,11 @@ def test_model_against_restatement_at_every_packing(name):
         for which, x, act in ((0, lat, a), (1, obs.cuda().contiguous(), None)):
             p = plan(cu, which, B, x, act)
             assert p["ctas"] * p["R"] >= B > (p["ctas"] - 1) * p["R"] and p["last"] == B - (p["ctas"] - 1) * p["R"]
+            assert (p["R"], p["NT"], p["ctas"], p["last"]) == BR.board_plan(BR.BOARD_CONFIGS[name][2], *obs_shape[1:], B), (B, p)
             plans.append((B, which, p["R"], p["NT"], p["ctas"], p["last"]))
     print(f"\n[board] {name} plans (B, program, R, NT, ctas, last): {plans}")
     assert any(p[5] != p[2] for p in plans)               # some launch ends in a partial CTA
-    if name in ("connect4", "board8x8_r3"):
+    if name in ("connect4", "board8x8_r3", "board8x8_hc16"):
         assert any(p[4] > 132 for p in plans)              # and, with few roots per CTA, some runs a second wave
 
 
@@ -143,7 +144,12 @@ SEARCHES = {
     "gomoku_b32_s50_sto_2p": ("gomoku", 32, 50, False, "2p", None, 1.0),
     "connect4_b8_s50_det_mixed": ("connect4", 8, 50, True, "mixed", None, 1.0),
     "board8x8_b40_s20_sto_mixed": ("board8x8_r3", 40, 20, False, "mixed", None, 1.0),
+    # each channel width at its largest tile count, where the leaves' latents are gathered for many roots per CTA
+    "board8x8_hc16_b661_s6_det_mixed": ("board8x8_hc16", 661, 6, True, "mixed", None, 0.997),     # C16 NT8: 6 roots per CTA
+    "gomoku_b1201_s6_det_2p": ("gomoku", 1201, 6, True, "2p", None, 1.0),                          # C32 NT8: 10 roots per CTA
+    "board8x8_b300_s6_det_2p": ("board8x8_r3", 300, 6, True, "2p", None, 1.0),                      # C64 NT4: 3 roots per CTA
 }
+WIDEST = {"board8x8_hc16_b661_s6_det_mixed": 8, "gomoku_b1201_s6_det_2p": 8, "board8x8_b300_s6_det_2p": 4}
 
 
 @pytest.mark.parametrize("case", list(SEARCHES))
@@ -163,7 +169,9 @@ def test_fused_search_equals_oracle_driving_the_same_network(case):
     exp, st = oracle_search(cu, S, latent, legal, logits, noises, tp, det, key=key, discount=disc)
     kernels = mcts.last_num_kernels
     roots.clear()
-    print(f"\n[board-search] {case}: ties={st['ties']} draws={st['draws']} kernels={kernels}")
+    R, NT = BR.board_plan(BR.BOARD_CONFIGS[name][2], *BR.BOARD_CONFIGS[name][0][1:], B)[:2]
+    print(f"\n[board-search] {case}: ties={st['ties']} draws={st['draws']} kernels={kernels} R={R} NT={NT}")
+    assert NT == WIDEST.get(case, NT)
     assert_same(got, exp)
     assert visits_sum_to(got, S)
     assert not plan_["persistent"] and kernels == 2 * S + 1    # the multi-kernel search graph
@@ -267,6 +275,13 @@ def test_refusals():
         lzb.MuZeroModel(observation_shape=(17, 6, 6), action_space_size=36, num_channels=32)
     with pytest.raises(NotImplementedError, match="downsample"):
         lzb.EfficientZeroModel(observation_shape=(3, 3, 3), action_space_size=9, downsample=False)
+    # one step outside each corner of row1x8_r4, col8x1 and board8x8_hc16
+    for kw, msg in ((dict(action_space_size=65), "1 to 64 actions"), (dict(num_res_blocks=5), "num_res_blocks"),
+                    (dict(reward_head_channels=17), "head channels"), (dict(policy_head_channels=0), "head channels"),
+                    (dict(value_head_channels=0), "head channels"), (dict(value_head_hidden_channels=[33]), "hidden sizes"),
+                    (dict(reward_head_hidden_channels=[0]), "hidden sizes"), (dict(policy_head_hidden_channels=[0]), "hidden sizes")):
+        with pytest.raises(cabi.LzError, match=msg):
+            lzb.MuZeroModel(**dict(BR.model_kwargs("board8x8_hc16"), **kw))
     # uint8 frames are the Atari path: a board model refuses them
     _, cu = make("tictactoe", 1)
     mcts = lzb.MuZeroMCTSCtree(dict(num_simulations=4))

@@ -104,7 +104,7 @@ def run_program(cu, ref64, which, x0, action):
 
 def inputs(cu, name, B, seed):
     """(observations, latents from the model's own initial_inference, actions)"""
-    obs_shape, A = BR.BOARD_CONFIGS[name][0], BR.BOARD_CONFIGS[name][1]
+    obs_shape, A = BR.config(name)[0], BR.config(name)[1]
     g = torch.Generator().manual_seed(seed)
     obs = torch.rand((B,) + tuple(obs_shape), generator=g).cuda()
     action = torch.randint(0, A, (B,), generator=g).cuda()
@@ -121,6 +121,7 @@ def test_layers_match_float64(name, B):
         print(f"\n[board-layers] {name} B={B} program {which}: " + " ".join(f"{k}={v:.3g}" for k, v in ratios.items()))
         bad = {k: r for k, r in ratios.items() if not r <= (0.25 if k.startswith("L") else 1.0)}
         assert not bad, f"{name} B={B} program {which}: over the bound {bad}"
+        assert all(r > 0 for k, r in ratios.items() if k.endswith("head")), ratios   # an exact head is a dead one: bias only
         check_scalars(out, which, False, BR.BOARD_CONFIGS[name][6])
         nl = len(infos) - 1
         for L, info in enumerate(infos):
@@ -140,3 +141,56 @@ def test_bound_detects_single_pass(name):
         assert all(info[5] == 1 for info in infos)
         weak = {k: r for k, r in ratios.items() if k.startswith("L") and not r >= 8.0}
         assert not weak, f"{name} program {which}: tc1 within 8x of the bound on {weak}"
+
+
+# Every instantiation k_board_tc<C, NT> (C = 16, 32: NT = 1 .. 8; C = 64: NT = 1 .. 4) is its own straight-line code (its
+# acc[NT][C / 2] accumulators, its fragment-row map, its ring waits): each runs both programs under the float64 check at a
+# (board, B) whose launch plan has NT tiles.  NT -> (board, B): 1x1 boards pack up to 16 roots in one tile, so B = 1201 (10
+# roots per CTA) stays at NT = 1; an 8x8 root takes 71 rows (NT = 2) and 132 of them fill one wave of one root each.
+TILES = {1: ((1, 1), 1201), 2: ((8, 8), 132), 3: ((7, 8), 133), 4: ((7, 8), 265), 5: ((7, 8), 397), 6: ((7, 8), 529),
+         7: ((8, 8), 529), 8: ((8, 8), 661)}
+PAIRS = [(C, NT) for C in (16, 32, 64) for NT in range(1, (4 if C == 64 else 8) + 1)]
+
+
+def tile_config(C, H, W):
+    """a BOARD_CONFIGS-style config of C channels on an H x W board, one action per square"""
+    return ((3, H, W), H * W, C, 1, 4, 16, (-10., 11., 1.))
+
+
+@pytest.mark.parametrize("C,NT", PAIRS, ids=[f"C{C}_NT{NT}" for C, NT in PAIRS])
+def test_every_tile_count_matches_float64(C, NT):
+    """k_board_tc<C, NT> against float64 within the bounds of test_layers_match_float64 (tc3) and test_bound_detects_single_pass
+    (tc1), and the public initial_inference / recurrent_inference outputs are the bits of the checked whole program"""
+    (H, W), B = TILES[NT]
+    cfg = tile_config(C, H, W)
+    plan = BR.board_plan(C, H, W, B)
+    assert plan[1] == NT, plan
+    ref64, cu = make(cfg, "tc3")
+    obs, latent, action = inputs(cu, cfg, B, 500 + NT)
+    nres = cfg[3]
+    for math in ("tc3", "tc1"):
+        cu.set_math(math)
+        for which, x0 in ((0, latent), (1, obs)):
+            ratios, out, infos = run_program(cu, ref64, which, x0, action)
+            print(f"\n[board-tiles] C={C} NT={NT} {H}x{W} B={B} plan={plan} {math} program {which}: "
+                  + " ".join(f"{k}={v:.3g}" for k, v in ratios.items()))
+            assert all(tuple(info[:4]) == plan and info[5] == (3 if math == "tc3" else 1) for info in infos), infos
+            if math == "tc1":
+                weak = {k: r for k, r in ratios.items() if k.startswith("L") and not r >= 8.0}
+                assert not weak, f"C={C} NT={NT} program {which}: tc1 within 8x of the bound on {weak}"
+                continue
+            bad = {k: r for k, r in ratios.items() if not r <= (0.25 if k.startswith("L") else 1.0)}
+            assert not bad, f"C={C} NT={NT} program {which}: over the bound {bad}"
+            check_scalars(out, which, False, cfg[6])
+            # the program the hook checked is the one the public entry points launch: the same bits
+            lat, _ = board_stage(cu, which, x0, action, 2 * nres, len(infos) - 1)
+            if which:
+                o = cu.initial_inference(obs, return_scalar_value=True)
+                pairs = [(o.latent_state, lat), (o.policy_logits, out["policy_logits"]), (o.value, out["value_logits"]),
+                         (o.value_scalar, out["value"])]
+            else:
+                o = cu.recurrent_inference(latent, action.to(torch.int32), return_scalars=True)
+                pairs = [(o.latent_state, lat), (o.policy_logits, out["policy_logits"]), (o.value, out["value_logits"]),
+                         (o.reward, out["reward_logits"]), (o.value_scalar, out["value"]), (o.reward_scalar, out["reward"])]
+            for i, (got, exp) in enumerate(pairs):
+                assert torch.equal(got.reshape(-1), exp.reshape(-1)), (which, i)

@@ -115,14 +115,14 @@ def ratios(ref, cu, which):
 NAME = None
 
 
-@pytest.mark.parametrize("name", ["cartpole", "lunarlander", "minigrid", "l96_h48"])
+@pytest.mark.parametrize("name", ["cartpole", "lunarlander", "minigrid", "l96_h48", "l32_o1", "l64_o4096", "l192"])
 @pytest.mark.parametrize("which", [1, 0], ids=["initial", "recurrent"])
 def test_layers_match_float64_and_tc1_fails(name, which):
     global NAME
     NAME = name
     ref, cu = make(name, 21)
     r3 = ratios(ref, cu, which)
-    print(f"\n[mlp-ez-layers] {name} which={which} tc3 " + " ".join(f"{k}={v:.3g}" for k, v in r3.items()))
+    print(f"\n[mlp-ez-layers] {name} NC={cu.latent_state_dim // 32} which={which} tc3 " + " ".join(f"{k}={v:.3g}" for k, v in r3.items()))
     assert all(v <= 1.0 for v in r3.values()), r3
     cu.set_math("tc1")
     r1 = ratios(ref, cu, which)
