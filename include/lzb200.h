@@ -123,6 +123,22 @@ int lz_tree_backpropagate(lz_tree *t, int latent_index, const float *d_reward, c
  * lz_tree_set_tiebreak, by default the first maximum, which is that draw with rand() == 0 (how the parity oracle builds the
  * reference). */
 int lz_tree_set_ez(lz_tree *t, int efficientzero, int lstm_horizon_len);
+/* ---- Stochastic MuZero tree (lzero/mcts/ctree/ctree_stochastic_muzero/lib/cnode.cpp, stochastic_mz_tree.pyx) ----
+ * lz_tree_set_stochastic puts a MuZero tree in stochastic mode before lz_tree_prepare: the root is a decision node, the children
+ * of a decision node are chance nodes and those of a chance node decision nodes (cnode.cpp:96-165), so a node is a chance node
+ * exactly when its depth is odd.  The tree must have been created with A = max(action_space_size, chance_space_size): every
+ * logits, noise, mask, legal and visit row of the tree has that width.  An inner decision node has action_space_size children,
+ * a chance node chance_space_size, and a chance node's reward is 0.  A chance node's child is drawn as
+ * std::discrete_distribution(priors) (cnode.cpp:610-630, libstdc++'s arithmetic in double) at a uniform u: every selection
+ * uses chance_u when it is in [0, 1) (the reference's draw from std::mt19937(s) when std::random_device returns s), and a fresh
+ * u from the counter-based RNG of the tie draws (seed, epoch, step, depth) when chance_u < 0.  Decision nodes select as a
+ * MuZero tree (lz_tree_traverse's deterministic flag).  The traverse's d_search_len is the leaf's depth: the leaf is a chance
+ * node (leaf_node_is_chance) when it is odd.  lz_tree_backpropagate takes, per tree, the afterstate program's chance logits
+ * (the first chance_space_size entries of the row) for a chance leaf and the dynamics program's action logits otherwise.
+ * chance_space_size = 0 turns the tree back into a MuZero tree (the other arguments are then ignored).  Refused on EfficientZero
+ * and Gumbel trees (LZ_ESTATE); the reuse descent, back-up and search (lz_search_run_with_reuse) are refused on a stochastic
+ * tree. */
+int lz_tree_set_stochastic(lz_tree *t, int action_space_size, int chance_space_size, double chance_u);
 /* Tie-breaking of the EfficientZero and reuse descents, which have no deterministic switch in the reference (they draw
  * rand() % len(ties) after reseeding from the wall clock, ctree_efficientzero/lib/cnode.cpp:691, ctree_muzero cnode.cpp:610-640):
  * first_maximum = 1 (default; the reference's draw with rand() == 0, what the parity tests pin) or 0 = a uniform draw from the same tie
@@ -231,6 +247,34 @@ typedef struct lz_mlp_ez_config {
     float support_min, support_max, support_step;
 } lz_mlp_ez_config;
 int lz_model_create_mlp_ez(const lz_mlp_ez_config *cfg, lz_model **out);
+/* StochasticMuZeroModelMLP (lzero/model/stochastic_muzero_model_mlp.py; vector observations): MuZeroModelMLP's representation,
+ * dynamics and prediction networks, the dynamics network over [afterstate | one-hot chance outcome], plus
+ * afterstate_dynamics_network (a MuZeroModelMLP dynamics network over [latent | one-hot action]) and
+ * afterstate_prediction_network (a prediction network with chance_space_size policy outputs).  State-dict names follow the
+ * reference class; chance_encoder.* and the SSL projection entries are ignored.  Runs on the tensor-core MLP kernel: latent_dim a
+ * multiple of 32 in [32, 256], obs_dim 1-4096, action_space_size and chance_space_size 1-608, head hidden sizes 1-32, support
+ * size <= 608; anything else is LZ_EINVAL.  Math modes tc3 / tc1.  initial_inference is lz_model_initial_inference;
+ * recurrent_inference is lz_model_recurrent_inference_stochastic.  Its searches run on stochastic trees
+ * (lz_tree_set_stochastic) through lz_search_run. */
+typedef struct lz_mlp_stochastic_config {
+    int obs_dim, action_space_size, chance_space_size, latent_dim;
+    int reward_hidden, value_hidden, policy_hidden;     /* one hidden layer each: 32 */
+    int res_connection_in_dynamics;
+    float support_min, support_max, support_step;
+} lz_mlp_stochastic_config;
+int lz_model_create_mlp_stochastic(const lz_mlp_stochastic_config *cfg, lz_model **out);
+/* StochasticMuZeroModel.recurrent_inference(state, option, afterstate) (stochastic_muzero_model.py:233-273) on B rows:
+ * afterstate = 0: afterstate dynamics over [latent d_state | one-hot action d_option] and the afterstate prediction, so
+ *   d_next_state is the afterstate and d_policy_logits f32 [B, chance_space_size] the chance logits;
+ * afterstate = 1: dynamics over [afterstate d_state | one-hot chance outcome d_option] and the prediction, so d_next_state is
+ *   the next latent and d_policy_logits f32 [B, action_space_size].
+ * Reward and value as lz_model_recurrent_inference (logits f32 [B, K], scalars f32 [B]); outputs may be NULL.  d_row_mask
+ * int32 [B] or NULL: row b is computed only when (d_row_mask[b] & 1) == (row_mask_on & 1), and the other rows are neither
+ * read nor written (the fused search splits its leaves this way).  Latent buffers 16-byte aligned. */
+int lz_model_recurrent_inference_stochastic(lz_model *m, int afterstate, int B, const float *d_state, const int32_t *d_option,
+                                            const int32_t *d_row_mask, int row_mask_on, float *d_next_state,
+                                            float *d_reward_logits, float *d_value_logits, float *d_policy_logits,
+                                            float *d_reward, float *d_value, lz_stream s);
 int lz_model_destroy(lz_model *m);
 /* Feed one tensor of the reference state_dict (names as produced by MuZeroModel.state_dict(),
  * SURVEY.md App. B.4; fp32, contiguous, HOST memory).  Unknown names are ignored (returns 1). */
@@ -334,7 +378,12 @@ int lz_search_destroy(lz_search *q);
  * On a Gumbel tree (lz_tree_set_gumbel) with a MuZero conv or MLP model: GumbelMuZeroMCTSCtree.search (mcts_ctree.py:1076-1172),
  * one CUDA graph of [Gumbel descent] + num_simulations x [recurrent_inference, Gumbel back-up + next descent]; `deterministic`
  * is ignored, the roots must be freshly prepared (no descent since lz_tree_prepare; LZ_ESTATE) and the search's
- * num_simulations may not exceed the tree's Gumbel num_simulations (LZ_EINVAL). */
+ * num_simulations may not exceed the tree's Gumbel num_simulations (LZ_EINVAL).
+ * On a stochastic tree (lz_tree_set_stochastic) with a StochasticMuZeroModelMLP: StochasticMuZeroMCTSCtree.search
+ * (mcts_ctree_stochastic.py:117-252), one CUDA graph of [descent] + num_simulations x [the afterstate program on the leaves that
+ * are chance nodes, the dynamics program on the others (one row mask, its two parities), back-up + next descent]; both programs
+ * write the same latent pool slot.  `deterministic` is the decision nodes' tie rule.  Stochastic searches are not collected on
+ * the device (lz_search_collect*: LZ_EINVAL). */
 int lz_search_run(lz_search *q, const float *d_latent_roots, int deterministic, lz_stream s);
 /* MuZeroMCTSCtree.search_with_reuse (mcts_ctree.py:370-468; ReZero) and EfficientZeroMCTSCtree.search_with_reuse (:878-1003).
  * d_true_action int32 [B], d_reuse_value f32 [B] as for the reuse lz_tree_traverse; d_infer_count int32 [num_simulations] or
@@ -343,7 +392,7 @@ int lz_search_run(lz_search *q, const float *d_latent_roots, int deterministic, 
  * An EfficientZero search takes the roots' LSTM state d_hidden{0,1}_roots as lz_search_run_ez (NULL = zeros); its graph has
  * 5 x num_simulations kernels and is_reset is taken per TREE from the descent (search_len % lstm_horizon_len; the
  * reference indexes a compacted list by tree at :1040-1046 / cnode.cpp:646, see DESIGN.md 4.6).  A MuZero search takes
- * NULL hidden pointers (LZ_EINVAL otherwise).  Refused on a Gumbel tree (LZ_ESTATE). */
+ * NULL hidden pointers (LZ_EINVAL otherwise).  Refused on a Gumbel or a stochastic tree (LZ_ESTATE). */
 int lz_search_run_with_reuse(lz_search *q, const float *d_latent_roots, const float *d_hidden0_roots, const float *d_hidden1_roots,
                              const int32_t *d_true_action, const float *d_reuse_value, int32_t *d_infer_count, lz_stream s);
 /* EfficientZeroMCTSCtree.search (mcts_ctree.py:671-876) for a search created from an EfficientZero model and a tree in
@@ -388,7 +437,8 @@ int lz_search_collect_host_u8(lz_search *q, const uint8_t *h_obs_u8, const uint8
  *   d_mask uint8 [N*L, A] (legal actions; an all-zero row is every action), d_to_play int32 [N*L] or NULL (-1),
  *   d_true_action int32 [N*L] (the reference's -2 for a segment's last step and for padding), d_policy_mask uint8 [N*L],
  *   d_noise f32 [N*L, A] in legal order or NULL (reanalyze_noise = False), noise_weight.
- * q may be a MuZero or an EfficientZero search (the LSTM state at every root is zero, as initial_inference returns it).
+ * q may be a MuZero or an EfficientZero search (the LSTM state at every root is zero, as initial_inference returns it); a
+ * Gumbel or a stochastic search is refused (LZ_ESTATE).
  * The searches run backward from position L - 1: a plain search (MuZero: ties by `deterministic`; EfficientZero: first maximum,
  * `deterministic` is ignored),
  * then, with reuse_search, L - 1 search_with_reuse calls each reusing the root values of the position searched before it (ties:

@@ -40,6 +40,14 @@ class MlpEzConfig(ctypes.Structure):
                 ("support_step", c_float)]
 
 
+class MlpStochasticConfig(ctypes.Structure):
+    """struct lz_mlp_stochastic_config (include/lzb200.h)"""
+    _fields_ = [("obs_dim", c_int), ("action_space_size", c_int), ("chance_space_size", c_int), ("latent_dim", c_int),
+                ("reward_hidden", c_int), ("value_hidden", c_int), ("policy_hidden", c_int),
+                ("res_connection_in_dynamics", c_int), ("support_min", c_float), ("support_max", c_float),
+                ("support_step", c_float)]
+
+
 class ValueTables(ctypes.Structure):
     """struct lz_value_tables (include/lzb200.h): host struct of device table pointers"""
     _fields_ = [("N", c_int), ("K1", c_int), ("W", c_int), ("P", c_int), ("value_prefix", c_int), ("fp32", c_int),
@@ -64,6 +72,7 @@ SIGNATURES = {
     "lz_tree_select_action": (c_int, [c_void_p, c_float, c_int, ctypes.c_uint64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lz_tree_set_ez": (c_int, [c_void_p, c_int, c_int]),
     "lz_tree_set_tiebreak": (c_int, [c_void_p, c_int]),
+    "lz_tree_set_stochastic": (c_int, [c_void_p, c_int, c_int, ctypes.c_double]),
     "lz_tree_results": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lz_tree_debug_rng": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "lz_tree_set_gumbel": (c_int, [c_void_p, c_int, c_int]),
@@ -73,6 +82,9 @@ SIGNATURES = {
     "lz_model_create": (c_int, [ctypes.POINTER(ModelConfig), ctypes.POINTER(c_void_p)]),
     "lz_model_create_mlp": (c_int, [ctypes.POINTER(MlpConfig), ctypes.POINTER(c_void_p)]),
     "lz_model_create_mlp_ez": (c_int, [ctypes.POINTER(MlpEzConfig), ctypes.POINTER(c_void_p)]),
+    "lz_model_create_mlp_stochastic": (c_int, [ctypes.POINTER(MlpStochasticConfig), ctypes.POINTER(c_void_p)]),
+    "lz_model_recurrent_inference_stochastic": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int] +
+                                                [c_void_p] * 7),
     "lz_model_destroy": (c_int, [c_void_p]),
     "lz_model_set_tensor": (c_int, [c_void_p, c_char_p, c_void_p, c_int64]),
     "lz_model_finalize": (c_int, [c_void_p]),

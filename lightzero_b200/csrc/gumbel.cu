@@ -484,6 +484,7 @@ int lz_tree_set_gumbel(lz_tree *t, int max_num_considered_actions, int num_simul
         return LZ_OK;
     }
     LZ_REQUIRE(!t->p.ez, LZ_ESTATE, "lz_tree_set_gumbel: tree is in EfficientZero mode (the Gumbel tree is a MuZero tree)");
+    LZ_REQUIRE(!t->p.nc, LZ_ESTATE, "lz_tree_set_gumbel: tree is in stochastic mode (the Gumbel tree is a MuZero tree)");
     LZ_REQUIRE(max_num_considered_actions >= 0 && num_simulations > 0, LZ_EINVAL,
                "lz_tree_set_gumbel: bad arguments max_num_considered_actions=%d num_simulations=%d",
                max_num_considered_actions, num_simulations);

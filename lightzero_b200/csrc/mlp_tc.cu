@@ -102,6 +102,12 @@ __global__ void __launch_bounds__(kMezThreads, 1) k_mez_tc(MezNet net, MezIO io,
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int root0 = blockIdx.x * R, nvalid = min(R, io.B - root0);
     const int sbytes = mez_stage_bytes(L);
+    auto sel = [&](int b) { return !io.row_mask || (io.row_mask[b] & 1) == io.row_mask_on; };
+    if (io.row_mask) {
+        bool any = false;
+        for (int m = tid; m < nvalid; m += kMezThreads) any |= sel(root0 + m);
+        if (!__syncthreads_or(any)) return;    // no selected row in this CTA: no weights streamed, nothing written
+    }
 
     int il = 0, ic = 0, issued = 0;            // thread 0: the next weight chunk of the program to stream
     auto issue_next = [&]() {
@@ -128,10 +134,10 @@ __global__ void __launch_bounds__(kMezThreads, 1) k_mez_tc(MezNet net, MezIO io,
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         const int m = 16 * warp + (lane >> 2) + 8 * h;
-        on[h] = m < nvalid;
+        on[h] = m < nvalid && sel(root0 + m);
         brow[h] = root0 + (on[h] ? m : 0);
-        zrow[h] = io.latent_base ? io.latent_base + (io.ix ? (size_t)io.ix[brow[h]] * io.slot_stride : 0) + (size_t)brow[h] * L : nullptr;
-        arow[h] = io.action ? net.abias + (size_t)min(max(io.action[brow[h]], 0), net.A - 1) * L : nullptr;
+        zrow[h] = (io.latent_base && on[h]) ? io.latent_base + (io.ix ? (size_t)io.ix[brow[h]] * io.slot_stride : 0) + (size_t)brow[h] * L : nullptr;
+        arow[h] = (io.action && on[h]) ? net.abias + (size_t)min(max(io.action[brow[h]], 0), net.nact - 1) * L : nullptr;
     }
 
     // ---- input latents (recurrent programs) -> slot 0, fp16 hi / lo
@@ -139,7 +145,7 @@ __global__ void __launch_bounds__(kMezThreads, 1) k_mez_tc(MezNet net, MezIO io,
         for (int i = tid; i < kMezRows * (L / 8); i += kMezThreads) {
             const int m = i % kMezRows, kg = i / kMezRows;
             float v[8];
-            if (m < nvalid) {
+            if (m < nvalid && sel(root0 + m)) {
                 const int b = root0 + m;
                 const float *src = io.latent_base + (io.ix ? (size_t)io.ix[b] * io.slot_stride : 0) + (size_t)b * L + 8 * kg;
                 const float4 x = *reinterpret_cast<const float4 *>(src), y = *reinterpret_cast<const float4 *>(src + 4);
@@ -177,7 +183,7 @@ __global__ void __launch_bounds__(kMezThreads, 1) k_mez_tc(MezNet net, MezIO io,
 #pragma unroll
                 for (int u = 0; u < 16; ++u) {
                     const int k = 32 * c + 16 * hf + u;
-                    v[u] = (m < nvalid && k < net.obs_dim) ? io.obs[(size_t)(root0 + m) * net.obs_dim + k] : 0.0f;
+                    v[u] = (m < nvalid && k < net.obs_dim && sel(root0 + m)) ? io.obs[(size_t)(root0 + m) * net.obs_dim + k] : 0.0f;
                 }
 #pragma unroll
                 for (int g = 0; g < 2; ++g) {
@@ -296,6 +302,7 @@ __global__ void __launch_bounds__(kMezThreads, 1) k_mez_tc(MezNet net, MezIO io,
         const bool rew = (f & MF_REWARD) != 0, cat = (f & (MF_VALUE | MF_REWARD)) != 0;   // cat: a categorical head's piece
         const bool head = (f & (MF_VALUE | MF_REWARD | MF_POLICY)) != 0;
         const int ncols = cat ? net.K : net.A, col0 = net.layer[l].col0;
+        const int rstride = (cat || !io.policy_stride) ? ncols : io.policy_stride;
         float *lg = rew ? io.reward_logits : (cat ? io.value_logits : io.policy_logits);
         unsigned char *ob = out == MB_NONE ? nullptr : smem + (out == MB_HID ? S.hid : (out == MB_SLOT1 ? S.slot1 : 0));
         const int opart = out == MB_HID ? 4 * kMezKgBytes : mez_slot_part(L);
@@ -315,8 +322,8 @@ __global__ void __launch_bounds__(kMezThreads, 1) k_mez_tc(MezNet net, MezIO io,
                         if ((f & MF_FEAT) && io.feat) *reinterpret_cast<float2 *>(io.feat + o) = make_float2(v0, v1);
                         if (head) {
                             const int k = col0 + col;
-                            if (lg && k < ncols) lg[(size_t)brow[h] * ncols + k] = v0;
-                            if (lg && k + 1 < ncols) lg[(size_t)brow[h] * ncols + k + 1] = v1;
+                            if (lg && k < ncols) lg[(size_t)brow[h] * rstride + k] = v0;
+                            if (lg && k + 1 < ncols) lg[(size_t)brow[h] * rstride + k + 1] = v1;
                             if (cat && k < ncols) softmax_push(sm_m[h], sm_s[h], sm_w[h], v0, support_at(net.support_min, net.support_step, k));
                             if (cat && k + 1 < ncols) softmax_push(sm_m[h], sm_s[h], sm_w[h], v1, support_at(net.support_min, net.support_step, k + 1));
                         }
@@ -474,10 +481,29 @@ struct MezPacker {
         return ok;
     }
 
-    // prediction network on the latent in `src` (common.py:1218-1292); the other slot is its work buffer
-    bool predict(MezNet &net, int src, int L, int A, int K, int vh, int ph)
+    // the dynamics MLP `D` over [z | one-hot of na] (muzero_model_mlp.py:428-440, efficientzero_model_mlp.py:440-468) and, for
+    // MuZeroModelMLP (mz), its reward head.  Slots: the input latent z in slot 0; fc_dynamics_1 (+ z) -> slot 0 = the next
+    // latent; fc_dynamics_2 -> slot 1, which the reward head reads.  Without res_connection_in_dynamics fc_dynamics -> slot 0 is
+    // both the next latent and the reward head's input.  EfficientZeroModelMLP writes the reward head's input as the LSTM
+    // input (MF_FEAT) of the value-prefix head (ez.cu) instead.
+    bool dynamics(MezNet &net, const std::string &D, int L, int na, int K, int rh, bool res, bool mz, std::vector<float> &act)
     {
-        const std::string Q = "prediction_network.";
+        if (res)     // next = fc_dynamics_1([z | a]) + z; LSTM / reward head input = fc_dynamics_2(next)
+            return layer(net, D + "fc_dynamics_1.0", D + "fc_dynamics_1.1", L + na, L, L, 0, L, L, MB_SLOT0, MB_SLOT1, MF_RELU | MF_ACT, &act) &&
+                   layer(net, D + "fc_dynamics_1.3", D + "fc_dynamics_1.4", L, L, L, 0, L, L, MB_SLOT1, MB_SLOT0, MF_RELU | MF_RES | MF_LATENT) &&
+                   layer(net, D + "fc_dynamics_2.0", D + "fc_dynamics_2.1", L, L, L, 0, L, L, MB_SLOT0, MB_SLOT1, MF_RELU) &&
+                   layer(net, D + "fc_dynamics_2.3", D + "fc_dynamics_2.4", L, L, L, 0, L, L, MB_SLOT1, mz ? MB_SLOT1 : MB_NONE,
+                         MF_RELU | (mz ? 0 : MF_FEAT)) &&
+                   (!mz || cat_head(net, D + "fc_reward_head", MB_SLOT1, L, rh, K, MF_REWARD));
+        // next = LSTM / reward head input = fc_dynamics([z | a])
+        return layer(net, D + "fc_dynamics.0", D + "fc_dynamics.1", L + na, L, L, 0, L, L, MB_SLOT0, MB_SLOT1, MF_RELU | MF_ACT, &act) &&
+               layer(net, D + "fc_dynamics.3", D + "fc_dynamics.4", L, L, L, 0, L, L, MB_SLOT1, MB_SLOT0, MF_RELU | MF_LATENT | (mz ? 0 : MF_FEAT)) &&
+               (!mz || cat_head(net, D + "fc_reward_head", MB_SLOT0, L, rh, K, MF_REWARD));
+    }
+
+    // prediction network `Q` with A policy outputs on the latent in `src` (common.py:1218-1292); the other slot is its work buffer
+    bool predict(MezNet &net, const std::string &Q, int src, int L, int A, int K, int vh, int ph)
+    {
         const int wk = src == MB_SLOT0 ? MB_SLOT1 : MB_SLOT0;
         bool ok = layer(net, Q + "fc_prediction_common.0", Q + "fc_prediction_common.1", L, L, L, 0, L, L, src, wk, MF_RELU) &&
                   layer(net, Q + "fc_prediction_common.3", Q + "fc_prediction_common.4", L, L, L, 0, L, L, wk, wk, MF_RELU) &&
@@ -490,43 +516,36 @@ struct MezPacker {
 
 }  // namespace
 
-// EfficientZeroModelMLP and MuZeroModelMLP share the programs up to what follows the dynamics MLP: EfficientZeroModelMLP writes
-// its output as the LSTM input (MF_FEAT) of the value-prefix head (ez.cu), MuZeroModelMLP runs the reward head on it
-// (muzero_model_mlp.py:428-440).  Slots of the
-// recurrent program: the input latent z in slot 0; fc_dynamics_1 (+ z) -> slot 0 = the next latent; fc_dynamics_2 -> slot 1,
-// which the reward head reads; the prediction network reads slot 0 and works in slot 1.  Without res_connection_in_dynamics
-// fc_dynamics -> slot 0 is both the next latent and the reward head's input.
+// EfficientZeroModelMLP, MuZeroModelMLP and StochasticMuZeroModelMLP share the representation and prediction programs and the
+// dynamics MLP (MezPacker::dynamics).  StochasticMuZeroModelMLP (stochastic_muzero_model_mlp.py) has two recurrent programs:
+// `after`, afterstate_dynamics_network over [latent | one-hot action] and afterstate_prediction_network with the C chance
+// outcomes as its policy outputs (recurrent_inference(afterstate=False), stochastic_muzero_model.py:266-271), and `rec`,
+// dynamics_network over [afterstate | one-hot chance outcome] and prediction_network (afterstate=True, :262-265).
 int mez_finalize(lz_model *m)
 {
     const MlpTcState &c = m->mez;
     const bool mz = !m->vp;
-    const int L = c.latent, A = m->A, K = m->K, kobs = (c.obs_dim + 31) / 32 * 32;
+    const int L = c.latent, A = m->A, C = c.chance, K = m->K, kobs = (c.obs_dim + 31) / 32 * 32;
     MezPacker P;
     P.m = m;
-    MezNet init, rec;
+    MezNet init, rec, after;
     memset(&init, 0, sizeof(init));
     memset(&rec, 0, sizeof(rec));
-    const std::string R = "representation_network.", D = "dynamics_network.";
-    std::vector<float> act;
+    memset(&after, 0, sizeof(after));
+    const std::string R = "representation_network.", Q = "prediction_network.";
+    std::vector<float> act, act_after;
     bool ok = P.layer(init, R + "fc_representation.0", R + "fc_representation.1", c.obs_dim, c.obs_dim, L, 0, L, kobs, MB_OBS, MB_SLOT0, MF_GELU) &&
               P.layer(init, R + "fc_representation.3", "", L, L, L, 0, L, L, MB_SLOT0, MB_SLOT0, MF_LN | MF_LATENT) &&
-              P.predict(init, MB_SLOT0, L, A, K, c.value_hidden, c.policy_hidden);
-    if (ok && c.res)     // next = fc_dynamics_1([z | a]) + z; LSTM / reward head input = fc_dynamics_2(next)
-        ok = P.layer(rec, D + "fc_dynamics_1.0", D + "fc_dynamics_1.1", L + A, L, L, 0, L, L, MB_SLOT0, MB_SLOT1, MF_RELU | MF_ACT, &act) &&
-             P.layer(rec, D + "fc_dynamics_1.3", D + "fc_dynamics_1.4", L, L, L, 0, L, L, MB_SLOT1, MB_SLOT0, MF_RELU | MF_RES | MF_LATENT) &&
-             P.layer(rec, D + "fc_dynamics_2.0", D + "fc_dynamics_2.1", L, L, L, 0, L, L, MB_SLOT0, MB_SLOT1, MF_RELU) &&
-             P.layer(rec, D + "fc_dynamics_2.3", D + "fc_dynamics_2.4", L, L, L, 0, L, L, MB_SLOT1, mz ? MB_SLOT1 : MB_NONE,
-                     MF_RELU | (mz ? 0 : MF_FEAT)) &&
-             (!mz || P.cat_head(rec, D + "fc_reward_head", MB_SLOT1, L, c.reward_hidden, K, MF_REWARD));
-    else if (ok)                                // next = LSTM / reward head input = fc_dynamics([z | a])
-        ok = P.layer(rec, D + "fc_dynamics.0", D + "fc_dynamics.1", L + A, L, L, 0, L, L, MB_SLOT0, MB_SLOT1, MF_RELU | MF_ACT, &act) &&
-             P.layer(rec, D + "fc_dynamics.3", D + "fc_dynamics.4", L, L, L, 0, L, L, MB_SLOT1, MB_SLOT0, MF_RELU | MF_LATENT | (mz ? 0 : MF_FEAT)) &&
-             (!mz || P.cat_head(rec, D + "fc_reward_head", MB_SLOT0, L, c.reward_hidden, K, MF_REWARD));
-    ok = ok && P.predict(rec, MB_SLOT0, L, A, K, c.value_hidden, c.policy_hidden);
+              P.predict(init, Q, MB_SLOT0, L, A, K, c.value_hidden, c.policy_hidden);
+    ok = ok && P.dynamics(rec, "dynamics_network.", L, C ? C : A, K, c.reward_hidden, c.res, mz, act) &&
+         P.predict(rec, Q, MB_SLOT0, L, A, K, c.value_hidden, c.policy_hidden);
+    if (C)
+        ok = ok && P.dynamics(after, "afterstate_dynamics_network.", L, A, K, c.reward_hidden, c.res, true, act_after) &&
+             P.predict(after, "afterstate_prediction_network.", MB_SLOT0, L, C, K, c.value_hidden, c.policy_hidden);
     if (!ok) return LZ_EINVAL;
     auto lw = find_tensor(m, R + "norm.weight", L), lb = find_tensor(m, R + "norm.bias", L);
     if (!lw || !lb) return LZ_EINVAL;
-    const size_t o_lw = P.tab.add(*lw), o_lb = P.tab.add(*lb), o_act = P.tab.add(act);
+    const size_t o_lw = P.tab.add(*lw), o_lb = P.tab.add(*lb), o_act = P.tab.add(act), o_act_after = P.tab.add(act_after);
     // one upload: the weight chunks, then the tables from the next 256-byte boundary
     const size_t wbytes = (P.w.size() + 255) & ~(size_t)255;
     P.w.resize(wbytes, 0);
@@ -535,13 +554,18 @@ int mez_finalize(lz_model *m)
     int rc = upload(&m->mez.d_mez, P.w.data(), P.w.size());
     if (rc != LZ_OK) return rc;
     const float *tab = reinterpret_cast<const float *>(m->mez.d_mez + wbytes);
-    for (MezNet *n : {&init, &rec}) {
+    for (MezNet *n : {&init, &rec, &after}) {
         n->w = m->mez.d_mez; n->tab = tab; n->abias = tab + o_act; n->ln_w = tab + o_lw; n->ln_b = tab + o_lb;
-        n->L = L; n->A = A; n->K = K; n->obs_dim = c.obs_dim;
+        n->L = L; n->A = A; n->K = K; n->obs_dim = c.obs_dim; n->nact = A;
         n->support_min = m->support_min; n->support_step = m->support_step;
+    }
+    if (C) {
+        rec.nact = C;
+        after.A = C; after.abias = tab + o_act_after;
     }
     m->mez.init = init;
     m->mez.rec = rec;
+    m->mez.after = after;
     if ((rc = mez_prepare_launch()) != LZ_OK) return rc;
     return m->vp ? ez_finalize(m, L, c.reward_hidden, false) : LZ_OK;
 }
@@ -563,13 +587,15 @@ int mez_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
         LZ_REQUIRE(io.B <= m->ez.B, LZ_ESTATE, "model_recurrent: EfficientZero scratch sized for %d roots, got %d (model_reserve)", m->ez.B, io.B);
         LZ_REQUIRE(io.h_base && io.c_base, LZ_EINVAL, "model_recurrent: EfficientZero needs the reward hidden state");
     }
+    LZ_REQUIRE(!io.after_program || m->mez.chance, LZ_EINVAL, "model_recurrent: the afterstate program is StochasticMuZeroModelMLP's");
     MezIO e = mez_io(m, io.B);
     e.latent_base = io.latent_base; e.ix = io.ix; e.slot_stride = io.slot_stride; e.action = io.action;
+    e.row_mask = io.row_mask; e.row_mask_on = io.row_mask_on; e.policy_stride = io.policy_stride;
     e.latent_out = io.next_latent;
     if (ez) e.feat = m->ez.feat;
     else { e.reward = io.reward; e.reward_logits = io.reward_logits; }
     e.value = io.value; e.policy_logits = io.policy_logits; e.value_logits = io.value_logits;
-    int rc = mez_launch(m->mez.rec, e, s);
+    int rc = mez_launch(io.after_program ? m->mez.after : m->mez.rec, e, s);
     if (rc || !ez) return rc;
     return ez_tail(m, io, s);
 }

@@ -42,6 +42,8 @@ struct MezNet {
     const float *abias;               // [A][L]
     const float *ln_w, *ln_b;         // [L]
     int L, A, K, obs_dim, nlayers, nchunks;
+    int nact;                         // width of the one-hot input of MF_ACT (A, or the chance outcomes of a StochasticMuZeroModelMLP
+                                      // dynamics program, whose policy head has A outputs and whose afterstate program has K = C)
     MezLayer layer[kMezMaxLayers];
     float support_min, support_step;
 };
@@ -58,8 +60,14 @@ struct MezIO {
     float *reward;                    // [B] or nullptr (MuZeroModelMLP's reward head)
     float *reward_logits;             // [B][K] or nullptr
     float *value;                     // [B] or nullptr
-    float *policy_logits;             // [B][A] or nullptr
+    float *policy_logits;             // [B][A] (row stride policy_stride) or nullptr
     float *value_logits;              // [B][K] or nullptr
+    // optional row mask: with row_mask, row b is computed only when (row_mask[b] & 1) == row_mask_on; any other row is not
+    // read and none of its outputs is written (the fused Stochastic MuZero search runs its two recurrent programs over the
+    // same leaf batch, split by the parity of the leaf depth)
+    const int *row_mask;
+    int row_mask_on;
+    int policy_stride;                // row stride of policy_logits (0: A)
 };
 
 // plan of a launch: roots per CTA, CTAs, roots of the last CTA, shared memory bytes, weight ring stages

@@ -91,6 +91,8 @@ int check_create(const char *fn, float support_min, float support_max, float sup
 // ---- the internal launch API (model.cuh) -------------------------------------------------------------------------------------
 int model_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
 {
+    LZ_REQUIRE((!io.after_program && !io.row_mask) || m->family == ModelFamily::MlpTc, LZ_EINVAL,
+               "model_recurrent: afterstate programs and row masks are StochasticMuZeroModelMLP's");
     switch (m->family) {
         case ModelFamily::Conv: return conv_recurrent(m, io, s);
         case ModelFamily::Board: return board_recurrent(m, io, s);
@@ -208,6 +210,36 @@ int lz_model_create_mlp_ez(const lz_mlp_ez_config *cfg, lz_model **out)
     return LZ_OK;
 }
 
+int lz_model_create_mlp_stochastic(const lz_mlp_stochastic_config *cfg, lz_model **out)
+{
+    LZ_REQUIRE(cfg && out, LZ_EINVAL, "lz_model_create_mlp_stochastic: null argument");
+    const lz_mlp_stochastic_config &c = *cfg;
+    LZ_REQUIRE(c.latent_dim >= 32 && c.latent_dim <= kMezMaxL && c.latent_dim % 32 == 0, LZ_EINVAL,
+               "lz_model_create_mlp_stochastic: latent_dim must be a multiple of 32 in [32, %d] (got %d)", kMezMaxL, c.latent_dim);
+    LZ_REQUIRE(c.obs_dim >= 1 && c.obs_dim <= kMezMaxObs, LZ_EINVAL,
+               "lz_model_create_mlp_stochastic: obs_dim must be in [1, %d] (got %d)", kMezMaxObs, c.obs_dim);
+    LZ_REQUIRE(c.action_space_size >= 1 && c.action_space_size <= kMezMaxOut, LZ_EINVAL,
+               "lz_model_create_mlp_stochastic: action_space_size must be in [1, %d] (got %d)", kMezMaxOut, c.action_space_size);
+    LZ_REQUIRE(c.chance_space_size >= 1 && c.chance_space_size <= kMezMaxOut, LZ_EINVAL,
+               "lz_model_create_mlp_stochastic: chance_space_size must be in [1, %d] (got %d)", kMezMaxOut, c.chance_space_size);
+    LZ_REQUIRE(c.reward_hidden >= 1 && c.reward_hidden <= kMezMaxHid && c.value_hidden >= 1 && c.value_hidden <= kMezMaxHid &&
+                   c.policy_hidden >= 1 && c.policy_hidden <= kMezMaxHid, LZ_EINVAL,
+               "lz_model_create_mlp_stochastic: head hidden sizes must be in [1, %d] (got %d, %d, %d)", kMezMaxHid, c.reward_hidden,
+               c.value_hidden, c.policy_hidden);
+    int K = 0;
+    int rc = check_create("lz_model_create_mlp_stochastic", c.support_min, c.support_max, c.support_step, kMezMaxOut, &K);
+    if (rc != LZ_OK) return rc;
+    lz_model *m = new lz_model();
+    m->family = ModelFamily::MlpTc;
+    m->A = c.action_space_size; m->K = K; m->support_min = c.support_min; m->support_step = c.support_step;
+    m->lat_c = m->latent_floats = c.latent_dim; m->lat_h = m->lat_w = 1;
+    m->obs_elems = c.obs_dim;
+    m->mez = MlpTcState{c.obs_dim, c.latent_dim, c.reward_hidden, c.value_hidden, c.policy_hidden, c.res_connection_in_dynamics,
+                        c.chance_space_size};
+    *out = m;
+    return LZ_OK;
+}
+
 int lz_model_destroy(lz_model *m)
 {
     if (!m) return LZ_OK;
@@ -226,9 +258,12 @@ int lz_model_set_tensor(lz_model *m, const char *name, const float *h_data, int6
     LZ_REQUIRE(m && name && h_data && numel >= 0, LZ_EINVAL, "lz_model_set_tensor: bad argument");
     std::string n(name);
     if (n.find("num_batches_tracked") != std::string::npos) return 1;
+    const bool stochastic = m->family == ModelFamily::MlpTc && m->mez.chance;     // StochasticMuZeroModelMLP's afterstate networks
     if (n.rfind("representation_network.", 0) != 0 && n.rfind("dynamics_network.", 0) != 0 &&
-        n.rfind("prediction_network.", 0) != 0)
-        return 1;   // e.g. the optional SSL projection heads (muzero_model.py:198-208), unused at inference
+        n.rfind("prediction_network.", 0) != 0 &&
+        !(stochastic && (n.rfind("afterstate_dynamics_network.", 0) == 0 || n.rfind("afterstate_prediction_network.", 0) == 0)))
+        return 1;   // e.g. the optional SSL projection heads (muzero_model.py:198-208) and Stochastic MuZero's chance_encoder,
+                    // unused at inference
     m->tensors[n].assign(h_data, h_data + numel);
     m->finalized = false;
     return LZ_OK;
@@ -325,6 +360,24 @@ int lz_model_recurrent_inference(lz_model *m, int B, const float *d_latent, cons
     io.B = B; io.latent_base = d_latent; io.ix = nullptr; io.slot_stride = 0; io.action = d_action;
     io.next_latent = d_next_latent; io.reward = d_reward; io.value = d_value; io.policy_logits = d_policy_logits;
     io.reward_logits = d_reward_logits; io.value_logits = d_value_logits;
+    return model_recurrent(m, io, (cudaStream_t)s);
+}
+
+int lz_model_recurrent_inference_stochastic(lz_model *m, int afterstate, int B, const float *d_state, const int32_t *d_option,
+                                            const int32_t *d_row_mask, int row_mask_on, float *d_next_state,
+                                            float *d_reward_logits, float *d_value_logits, float *d_policy_logits,
+                                            float *d_reward, float *d_value, lz_stream s)
+{
+    LZ_REQUIRE(m && d_state && d_option && B > 0, LZ_EINVAL, "lz_model_recurrent_inference_stochastic: bad argument");
+    LZ_REQUIRE(m->finalized && m->family == ModelFamily::MlpTc && m->mez.chance, LZ_ESTATE,
+               "lz_model_recurrent_inference_stochastic: not a finalized StochasticMuZeroModelMLP");
+    RecIO io;
+    memset(&io, 0, sizeof(io));
+    io.B = B; io.latent_base = d_state; io.action = d_option;
+    io.next_latent = d_next_state; io.reward = d_reward; io.value = d_value; io.policy_logits = d_policy_logits;
+    io.reward_logits = d_reward_logits; io.value_logits = d_value_logits;
+    io.after_program = !afterstate;      // afterstate = 0: the state is a latent, the afterstate program makes an afterstate of it
+    io.row_mask = d_row_mask; io.row_mask_on = row_mask_on & 1;
     return model_recurrent(m, io, (cudaStream_t)s);
 }
 

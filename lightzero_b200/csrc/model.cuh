@@ -56,6 +56,12 @@ struct RecIO {
     size_t hslot_stride;
     float *h_out, *c_out;
     const int *is_reset;
+    // StochasticMuZeroModelMLP (MlpTc family only): after_program != 0 runs the afterstate program (afterstate dynamics + afterstate
+    // prediction, C chance logits into policy_logits) instead of the dynamics program; row_mask / row_mask_on as MezIO's
+    int after_program;
+    const int *row_mask;
+    int row_mask_on;
+    int policy_stride;                // row stride of policy_logits (0: the program's policy outputs)
 };
 
 struct TailIO {
@@ -112,8 +118,10 @@ struct MlpFp32State {
 
 struct MlpTcState {
     int obs_dim, latent, reward_hidden, value_hidden, policy_hidden, res;   // res: res_connection_in_dynamics
+    int chance;                       // StochasticMuZeroModelMLP: chance_space_size (0: the other MLP models)
     unsigned char *d_mez;             // packed fp16 hi / lo weights and fp32 tables of the dense layers
     MezNet rec, init;                 // recurrent_inference (dense part) / initial_inference programs
+    MezNet after;                     // StochasticMuZeroModelMLP's afterstate program (rec is its dynamics program on afterstates)
 };
 
 // EfficientZero's value-prefix head (ez.cu) on the LSTM input features that the Conv or the MlpTc network writes into `feat`

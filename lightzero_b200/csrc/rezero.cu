@@ -150,6 +150,7 @@ static int sweep(lz_search *q, const SweepArgs &a, cudaStream_t s)
     LZ_REQUIRE(!a.obs || a.mini > 0, LZ_EINVAL, "lz_rezero_reanalyze: mini_infer_size %d must be > 0", a.mini);
     LZ_REQUIRE(!(a.reuse && L > 1) || a.infer_count, LZ_EINVAL, "lz_rezero_reanalyze: d_infer_count is needed when L > 1 with reuse");
     LZ_REQUIRE(!t->gumbel, LZ_ESTATE, "lz_rezero_reanalyze: Gumbel tree (the sweep runs MuZero and EfficientZero trees)");
+    LZ_REQUIRE(!t->p.nc, LZ_ESTATE, "lz_rezero_reanalyze: stochastic tree (the sweep runs MuZero and EfficientZero trees)");
     // search_with_reuse breaks ties with rand() only (cnode.cpp:610-640, ctree_efficientzero cnode.cpp:691): the first maximum, the
     // draw with rand() == 0.  Changing the rule re-captures the graphs once; a sweep keeps it.
     int rc = lz_tree_set_tiebreak(t, 1);

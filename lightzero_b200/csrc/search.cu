@@ -79,12 +79,41 @@ static int enqueue_gumbel(lz_search *q, cudaStream_t s)
     return LZ_OK;
 }
 
+// StochasticMuZeroMCTSCtree.search (mcts_ctree_stochastic.py:117-252): [descent] + S x [the afterstate program on the rows whose
+// leaf is a chance node (odd depth), the dynamics program on the others, back-up (+ next descent)].  The reference splits the
+// leaves on the host and backs up the two subsets one after the other; the trees are independent, so one back-up of every tree
+// is the same.  Both programs write pool slot sim + 1 and the same hand-off buffers, each only its own rows.
+static int enqueue_stochastic(lz_search *q, int deterministic, cudaStream_t s)
+{
+    int rc;
+    lz_tree *t = q->tree;
+    TreeStep descent = {};
+    descent.traverse = 1; descent.deterministic = deterministic;
+    descent.ix = q->d_ix; descent.act = q->d_action; descent.len = q->d_len;
+    if ((rc = tree_launch_step(t, descent, s))) return rc;
+    for (int sim = 0; sim < q->S; ++sim) {
+        RecIO io = rec_io(q, sim);
+        io.row_mask = q->d_len; io.policy_stride = q->A;
+        for (int chance = 1; chance >= 0; --chance) {
+            io.after_program = chance; io.row_mask_on = chance;
+            if ((rc = model_recurrent(q->model, io, s))) return rc;
+        }
+        TreeStep step = descent;
+        step.traverse = sim + 1 < q->S;
+        step.latent_index = sim + 1;
+        step.reward = q->d_reward; step.value = q->d_value; step.logits = q->d_policy;
+        if ((rc = tree_launch_step(t, step, s))) return rc;
+    }
+    return LZ_OK;
+}
+
 static int enqueue_search(lz_search *q, int deterministic, bool reuse, cudaStream_t s)
 {
     if (q->tree->gumbel) return enqueue_gumbel(q, s);
     int rc;
     lz_tree *t = q->tree;
     t->step_counter = 0;
+    if (t->p.nc) return enqueue_stochastic(q, deterministic, s);
     if (persistent_search(q, reuse)) return tc_launch(q->model->conv.tc_rec, persistent_io(q, deterministic), s, &t->p);
     TreeStep descent = {};
     descent.traverse = 1; descent.deterministic = deterministic;
@@ -195,6 +224,7 @@ static int collect_search(lz_search *q, const uint8_t *d_mask, const float *d_lo
 {
     int rc;
     lz_tree *t = q->tree;
+    LZ_REQUIRE(!t->p.nc, LZ_EINVAL, "lz_search_collect: stochastic trees are not collected on the device");
     if ((rc = lz_tree_reset_mask(t, d_mask, s))) return rc;                        // policy/muzero.py:760,769
     const float *values = t->gumbel ? d_values : nullptr;
     if ((rc = lz_tree_prepare(t, d_logits, d_noise, noise_weight, nullptr, values, d_to_play, s))) return rc;   // :774
@@ -212,7 +242,11 @@ int lz_search_create(lz_tree *t, lz_model *m, int num_simulations, lz_search **o
     LZ_REQUIRE(t && m && out && num_simulations > 0, LZ_EINVAL, "lz_search_create: bad argument");
     LZ_REQUIRE(m->finalized, LZ_ESTATE, "lz_search_create: model not finalized");
     LZ_REQUIRE(num_simulations <= t->max_sims, LZ_EINVAL, "lz_search_create: num_simulations %d > tree capacity %d", num_simulations, t->max_sims);
-    LZ_REQUIRE(t->p.A == m->A, LZ_EINVAL, "lz_search_create: tree has %d actions, model %d", t->p.A, m->A);
+    const int C = m->family == ModelFamily::MlpTc ? m->mez.chance : 0;
+    LZ_REQUIRE(C == t->p.nc, LZ_EINVAL, "lz_search_create: a StochasticMuZeroModelMLP needs a tree in stochastic mode with its "
+               "chance_space_size and any other model a tree without chance nodes (lz_tree_set_stochastic; model %d, tree %d)", C, t->p.nc);
+    LZ_REQUIRE(t->p.na == m->A && t->p.A == std::max(m->A, C), LZ_EINVAL, "lz_search_create: tree has %d actions (width %d), model %d",
+               t->p.na, t->p.A, m->A);
     const bool ez = m->vp;
     LZ_REQUIRE(ez == (t->p.ez != 0), LZ_EINVAL, "lz_search_create: %s model needs a tree in %s mode (lz_tree_set_ez)",
                ez ? "an EfficientZero" : "a MuZero", ez ? "EfficientZero" : "MuZero");
@@ -229,6 +263,7 @@ int lz_search_create(lz_tree *t, lz_model *m, int num_simulations, lz_search **o
     if (rc == LZ_OK) rc = dev_alloc(&q->d_root_logits, (size_t)q->B * q->A);
     if (rc == LZ_OK) rc = dev_alloc(&q->d_root_value, (size_t)q->B);
     if (rc == LZ_OK) rc = dev_alloc(&q->d_skip, q->slot_stride);
+    if (rc == LZ_OK && C) rc = dev_alloc(&q->d_len, (size_t)q->B);
     if (rc == LZ_OK && ez) {
         q->hslot_stride = (size_t)q->B * m->lstm_hidden;
         rc = dev_alloc(&q->hpool, q->hslot_stride * (size_t)(q->S + 1));
@@ -260,7 +295,7 @@ int lz_search_destroy(lz_search *q)
     cudaFree(q->d_obs_stage); cudaFree(q->d_noise_stage); cudaFree(q->d_pre_stage); cudaFree(q->d_mask_stage); cudaFree(q->d_tp_stage);
     cudaFree(q->pool); cudaFree(q->d_ix); cudaFree(q->d_action); cudaFree(q->d_reward); cudaFree(q->d_value);
     cudaFree(q->d_policy); cudaFree(q->d_root_logits); cudaFree(q->d_root_value); cudaFree(q->d_skip);
-    cudaFree(q->hpool); cudaFree(q->cpool); cudaFree(q->d_is_reset);
+    cudaFree(q->hpool); cudaFree(q->cpool); cudaFree(q->d_is_reset); cudaFree(q->d_len);
     cudaFree(q->d_true_action); cudaFree(q->d_reuse_value);
     cudaFree(q->rz_latent); cudaFree(q->rz_logits);
     delete q;
@@ -286,6 +321,7 @@ int lz_search_run_with_reuse(lz_search *q, const float *d_latent_roots, const fl
                "lz_search_run_with_reuse: LSTM state passed to a MuZero search");
     LZ_REQUIRE(q->tree->prepared, LZ_ESTATE, "lz_search_run_with_reuse: roots not prepared (call lz_tree_prepare first)");
     LZ_REQUIRE(!q->tree->gumbel, LZ_ESTATE, "lz_search_run_with_reuse: Gumbel tree (it has no reuse search)");
+    LZ_REQUIRE(!q->tree->p.nc, LZ_ESTATE, "lz_search_run_with_reuse: stochastic tree (it has no reuse search)");
     const cudaStream_t s = (cudaStream_t)s_;
     int rc = search_reuse_buffers(q);
     if (rc == LZ_OK) rc = copy_latent_roots(q, d_latent_roots, s);
@@ -305,6 +341,8 @@ int lz_search_run(lz_search *q, const float *d_latent_roots, int deterministic, 
     LZ_REQUIRE(q, LZ_EINVAL, "lz_search_run: null search");
     LZ_REQUIRE(!q->hpool, LZ_ESTATE, "lz_search_run: EfficientZero search, use lz_search_run_ez");
     LZ_REQUIRE(q->tree->prepared, LZ_ESTATE, "lz_search_run: roots not prepared (call lz_tree_prepare first)");
+    LZ_REQUIRE((q->d_len != nullptr) == (q->tree->p.nc != 0), LZ_ESTATE,
+               "lz_search_run: the tree's stochastic mode does not match the model (lz_tree_set_stochastic)");
     if (const lz_gumbel *gs = q->tree->gumbel) {
         LZ_REQUIRE(gs->prepared && gs->traversals == 0, LZ_ESTATE,
                    "lz_search_run: Gumbel roots not freshly prepared (call lz_tree_prepare first)");

@@ -26,6 +26,8 @@ struct lz_search {
     float *hpool, *cpool;
     size_t hslot_stride;
     int32_t *d_is_reset;
+    // Stochastic MuZero: the depth of each leaf the last descent reached; its parity selects the recurrent program of the row
+    int32_t *d_len;
     // ReZero search_with_reuse: library-owned copies of the caller's per-root true action / reuse value (graph-stable addresses)
     int32_t *d_true_action;
     float *d_reuse_value;

@@ -3,6 +3,7 @@
 #include <math.h>
 #include <stdarg.h>
 
+#include <algorithm>
 #include <atomic>
 #include <limits.h>
 #include <mutex>
@@ -253,6 +254,7 @@ int lz_tree_create(int B, int A, int max_sims, lz_tree **out)
     p.n_to_play = (int *)(base + o_ntp); p.n_best = (int *)(base + o_nbest); p.n_reset = (int *)(base + o_nreset);
     p.n_batch = (int *)(base + o_nbatch); p.reuse_state = (int *)(base + o_rstate); p.infer_count = (int *)(base + o_infer);
     p.ez = 0; p.lstm_horizon = 5; p.tie_first = 1;
+    p.na = A; p.nc = 0; p.chance_u = -1.0;
     p.legal = (int *)(base + o_legal); p.nlegal = (int *)(base + o_nlegal);
     p.root_visit = (int *)(base + o_rvis); p.root_vsum = (float *)(base + o_rvsum); p.root_reward = (float *)(base + o_rrew);
     p.mm_max = (float *)(base + o_mmax); p.mm_min = (float *)(base + o_mmin);
@@ -343,6 +345,7 @@ int lz_tree_traverse(lz_tree *t, int deterministic, const int32_t *d_true_action
     LZ_REQUIRE(!d_is_reset || t->p.ez, LZ_EINVAL, "lz_tree_traverse: d_is_reset is an output of EfficientZero trees only");
     LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_traverse: roots not prepared (call lz_tree_prepare first)");
     LZ_REQUIRE(!t->gumbel || !d_reuse_value, LZ_ESTATE, "lz_tree_traverse: Gumbel tree (it has no reuse descent)");
+    LZ_REQUIRE(!t->p.nc || !d_reuse_value, LZ_ESTATE, "lz_tree_traverse: stochastic tree (it has no reuse descent)");
     TreeStep a = {};
     a.traverse = 1; a.deterministic = deterministic; a.true_action = d_true_action; a.reuse_value = d_reuse_value;
     a.ix = d_ix; a.iy = d_iy; a.act = d_last_action; a.len = d_search_len; a.vtp = d_virtual_to_play; a.is_reset = d_is_reset;
@@ -359,6 +362,7 @@ int lz_tree_backpropagate(lz_tree *t, int latent_index, const float *d_reward, c
                                                           : "lz_tree_backpropagate: d_is_reset is for EfficientZero trees only");
     LZ_REQUIRE(t->prepared, LZ_ESTATE, "lz_tree_backpropagate: roots not prepared");
     LZ_REQUIRE(!t->gumbel || !d_reuse_value, LZ_ESTATE, "lz_tree_backpropagate: Gumbel tree (it has no reuse back-up)");
+    LZ_REQUIRE(!t->p.nc || !d_reuse_value, LZ_ESTATE, "lz_tree_backpropagate: stochastic tree (it has no reuse back-up)");
     LZ_REQUIRE(latent_index >= 1 && latent_index <= t->max_sims, LZ_EINVAL,
                "lz_tree_backpropagate: latent_index %d outside [1, %d]", latent_index, t->max_sims);
     TreeStep a = {};
@@ -372,10 +376,34 @@ int lz_tree_set_ez(lz_tree *t, int efficientzero, int lstm_horizon_len)
     LZ_REQUIRE(t, LZ_EINVAL, "lz_tree_set_ez: null tree");
     LZ_REQUIRE(!efficientzero || lstm_horizon_len > 0, LZ_EINVAL, "lz_tree_set_ez: lstm_horizon_len must be > 0 (mcts_ctree.py:857)");
     LZ_REQUIRE(!efficientzero || !t->gumbel, LZ_ESTATE, "lz_tree_set_ez: Gumbel tree (lz_tree_set_gumbel(t, m, 0) turns it back into a MuZero tree)");
+    LZ_REQUIRE(!efficientzero || !t->p.nc, LZ_ESTATE, "lz_tree_set_ez: stochastic tree (lz_tree_set_stochastic(t, A, 0, -1) turns it back into a MuZero tree)");
     const int ez = efficientzero ? 1 : 0, hor = efficientzero ? lstm_horizon_len : t->p.lstm_horizon;
     if (t->p.ez != ez || t->p.lstm_horizon != hor) ++t->generation;
     t->p.ez = ez;
     t->p.lstm_horizon = hor;
+    return LZ_OK;
+}
+
+int lz_tree_set_stochastic(lz_tree *t, int action_space_size, int chance_space_size, double chance_u)
+{
+    LZ_REQUIRE(t, LZ_EINVAL, "lz_tree_set_stochastic: null tree");
+    TreeParams &p = t->p;
+    int na = p.A, nc = 0;
+    double u = -1.0;
+    if (chance_space_size) {
+        LZ_REQUIRE(!p.ez && !t->gumbel, LZ_ESTATE, "lz_tree_set_stochastic: EfficientZero or Gumbel tree");
+        LZ_REQUIRE(action_space_size >= 1 && chance_space_size >= 1 && std::max(action_space_size, chance_space_size) == p.A, LZ_EINVAL,
+                   "lz_tree_set_stochastic: a tree of width %d takes max(action_space_size, chance_space_size) == %d (got %d, %d)",
+                   p.A, p.A, action_space_size, chance_space_size);
+        LZ_REQUIRE(chance_u < 1.0, LZ_EINVAL, "lz_tree_set_stochastic: chance_u %g must be < 1 (or < 0 to sample)", chance_u);
+        na = action_space_size;
+        nc = chance_space_size;
+        u = chance_u < 0.0 ? -1.0 : chance_u;
+    }
+    if (p.na != na || p.nc != nc || p.chance_u != u) ++t->generation;      // captured graphs bake TreeParams in
+    p.na = na;
+    p.nc = nc;
+    p.chance_u = u;
     return LZ_OK;
 }
 

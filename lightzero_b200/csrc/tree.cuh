@@ -54,6 +54,13 @@ struct TreeParams {
                                  //     on an unexpanded child (expand, back up the reuse value), 2 stopped on an expanded child
                                  //     (no inference, no expansion, back up the reuse value)
     int *infer_count;            // [N] per-simulation number of trees that needed the network (search_with_reuse statistics)
+    // Stochastic MuZero (ctree_stochastic_muzero/lib/cnode.cpp): the children of a decision node are chance nodes and the
+    // children of a chance node are decision nodes, so a node's is_chance is the parity of its depth (the root is a decision
+    // node).  A is the edge width max(na, nc); every other tree has na = A and nc = 0.
+    int na;                      // children of an inner decision node (the model's actions)
+    int nc;                      // children of a chance node (chance_space_size), 0: no chance nodes
+    double chance_u;             // >= 0: the uniform every chance selection draws (a pinned std::mt19937 seed); < 0: a fresh
+                                 // draw per selection from the counter-based RNG of the tie draws
 };
 
 __device__ __forceinline__ float u2f(uint32_t u) { return __uint_as_float(u); }
@@ -137,6 +144,23 @@ __device__ __forceinline__ float ucb_score(const uint32_t *nb, int A, int a, boo
     return __fadd_rn(prior_score, value_score);
 }
 
+// cselect_child of a chance node (ctree_stochastic_muzero cnode.cpp:610-630): std::discrete_distribution over the n children's
+// priors, in libstdc++'s arithmetic (param_type::_M_initialize: double sum, p / sum, partial sums, the last set to 1.0; fewer
+// than two outcomes draw 0), at the uniform u: the first child whose cumulative probability is >= u (std::lower_bound).
+// Not inlined: inside the descent the double division's slow path made ptxas spill.
+static __device__ __noinline__ int chance_outcome(const uint32_t *nb, int A, int n, double u)
+{
+    if (n < 2) return 0;
+    double sum = 0.0;
+    for (int k = 0; k < n; ++k) sum += (double)u2f(nb[F_PRIOR * A + k]);
+    double cp = 0.0;
+    for (int k = 0; k < n - 1; ++k) {
+        cp += (double)u2f(nb[F_PRIOR * A + k]) / sum;
+        if (cp >= u) return k;
+    }
+    return n - 1;
+}
+
 // One PUCT descent of tree b by the calling warp: cbatch_traverse body (cnode.cpp:783-824) with
 // compute_mean_q (169-203) and cselect_child (551-595).  Records the path for the backup, and search_len / vtp (/ reuse_state)
 // of the tree in p.
@@ -169,7 +193,8 @@ __device__ __forceinline__ void tree_traverse(const TreeParams &p, int b, int la
 
     while (true) {
         const uint32_t *nb = tree_edges + (size_t)slot * kEdgeFields * A;
-        const int n = is_root ? nl : A;
+        const bool chance = p.nc && (plen & 1);       // plen is the depth of the node being scanned
+        const int n = is_root ? nl : (chance ? p.nc : p.na);
         // ---- compute_mean_q: sequential fp32 sum over visited children in legal order
         float total = 0.0f;
         int tv = 0;
@@ -203,7 +228,19 @@ __device__ __forceinline__ void tree_traverse(const TreeParams &p, int b, int la
         const float sq = __fsqrt_rn(total_children);
         float best = kFloatMin;
         int best_k = -1;
-        for (int c0 = 0; c0 < n; c0 += 32) {
+        if (chance) {
+            // a chance node draws its outcome; the counter key is the tie draws' (a depth is either chance or decision)
+            int k = 0;
+            if (lane == 0) {
+                double u = p.chance_u;
+                if (u < 0.0)
+                    u = (double)(mix64(p.rng_seed ^ mix64(*p.rng_epoch) ^ mix64(((unsigned long long)b << 32) | step) ^ (unsigned)plen) >> 11) *
+                        (1.0 / 9007199254740992.0);
+                k = chance_outcome(nb, A, n, u);
+            }
+            best_k = __shfl_sync(0xffffffffu, k, 0);
+        }
+        for (int c0 = 0; !chance && c0 < n; c0 += 32) {
             int k = c0 + lane;
             bool act = k < n;
             int a = act ? (is_root ? lg[k] : k) : 0;
@@ -215,7 +252,7 @@ __device__ __forceinline__ void tree_traverse(const TreeParams &p, int b, int la
                 best_k = c0 + __ffs(__ballot_sync(0xffffffffu, act && sc == cmax)) - 1;
             }
         }
-        if (!deterministic && best_k >= 0) {
+        if (!deterministic && !chance && best_k >= 0) {
             // tie list of cnode.cpp:576-586: the arg-max position, then every LATER position whose
             // score >= max - 1e-6; draw uniformly (counter-based hash instead of rand()).
             const float thr = __fsub_rn(best, 0.000001f);
@@ -350,8 +387,8 @@ __device__ __forceinline__ void tree_reset_root(const TreeParams &p, int b, int 
         for (int k = lane; k < n; k += 32) lg[k] = legal[k];
     }
     if (n == 0) {
-        n = A;
-        for (int k = lane; k < A; k += 32) lg[k] = k;
+        n = p.na;
+        for (int k = lane; k < n; k += 32) lg[k] = k;
     }
     for (int k = n + lane; k < A; k += 32) lg[k] = -1;
     if (lane == 0) {
@@ -430,7 +467,9 @@ __device__ __forceinline__ void tree_backprop(const TreeParams &p, int b, int la
     const int rstate = REUSE ? p.reuse_state[b] : 0;
     const bool no_expand = REUSE && rstate == 2;
     if (REUSE && rstate != 0) value = reuse_value;
-    if (!no_expand) expand_block(tree_edges + (size_t)latent_index * kEdgeFields * A, A, logits, nullptr, A, lane);
+    const bool leaf_chance = p.nc && (plen & 1);    // a chance leaf: its children are the nc outcomes, its reward 0 (cnode.cpp:116-119)
+    if (leaf_chance) reward = 0.0f;
+    if (!no_expand) expand_block(tree_edges + (size_t)latent_index * kEdgeFields * A, A, logits, nullptr, leaf_chance ? p.nc : p.na, lane);
     const int leaf_ps = pslot[plen - 1], leaf_pa = pact[plen - 1];
     uint32_t *leaf_nb = tree_edges + (size_t)leaf_ps * kEdgeFields * A;
     if (EZ && no_expand && lane == 0)      // ctree_efficientzero cnode.cpp:646: is_reset lands on the reached node even without expansion

@@ -20,9 +20,10 @@ from typing import Any, List, Optional, Union
 import numpy as np
 import torch
 
-from . import cabi, ez_tree, gmz_tree, mz_tree
+from . import cabi, ez_tree, gmz_tree, mz_tree, stochastic_mz_tree
 from .model_base import LzModel
 from .scaling_transform import DiscreteSupport, InverseScalarTransform
+from .stochastic_muzero_model_mlp import StochasticMuZeroModelMLP
 
 
 def _dev_f32(x, dev):
@@ -392,3 +393,73 @@ class GumbelMuZeroMCTSCtree(MuZeroMCTSCtree):
         with torch.cuda.device(roots.device):
             cabi.check(t.lib.lz_search_run(q, lat.data_ptr(), 1, cabi.stream_ptr()), "lz_search_run")
         self.last_num_kernels = t.lib.lz_search_num_kernels(q)
+
+
+class StochasticMuZeroMCTSCtree(MuZeroMCTSCtree):
+    """Mirror of ``lzero.mcts.tree_search.mcts_ctree_stochastic.StochasticMuZeroMCTSCtree``: ``roots(n, legal_actions,
+    chance_space_size)`` and ``search(roots, model, latent_state_roots, to_play_batch)``.  With a
+    ``lightzero_b200.StochasticMuZeroModelMLP`` the whole search is one CUDA graph (``lz_search_run`` on a stochastic tree);
+    any other model is driven step by step on the same device trees.
+
+    Config key ``chance_seed``: an integer s makes every chance selection the draw of ``std::mt19937(s)``, which is what the
+    reference draws when ``std::random_device`` returns s (its chance draws are otherwise not reproducible); None (the
+    default) samples each selection from the tree's counter-based RNG.  ``deterministic`` is the decision nodes' tie rule,
+    as in MuZeroMCTSCtree."""
+    config = dict(MuZeroMCTSCtree.config, chance_seed=None)
+
+    @classmethod
+    def roots(cls, active_collect_env_num: int, legal_actions: List[Any], chance_space_size: int = 2) -> "stochastic_mz_tree.Roots":
+        """mcts_ctree_stochastic.py:72-85"""
+        return stochastic_mz_tree.Roots(active_collect_env_num, legal_actions, chance_space_size)
+
+    def search(self, roots: "stochastic_mz_tree.Roots", model, latent_state_roots, to_play_batch: Union[int, List[Any]]) -> None:
+        """mcts_ctree_stochastic.py:87-252.  ``latent_state_roots``: np.ndarray or CUDA tensor [B, latent_state_dim]."""
+        S = int(self._cfg.num_simulations)
+        roots.set_chance_seed(self._cfg.chance_seed)
+        roots._materialize(S, self._params(), self.deterministic)
+        t = roots._tree
+        lat = _dev_f32(latent_state_roots, roots.device)
+        if not isinstance(model, StochasticMuZeroModelMLP):
+            self._search_stepwise_stochastic(roots, model, lat, S)
+            return
+        q = t.search_for(model, S)
+        with torch.cuda.device(roots.device):
+            cabi.check(t.lib.lz_search_run(q, lat.data_ptr(), int(self.deterministic), cabi.stream_ptr()), "lz_search_run")
+        self.last_num_kernels = t.lib.lz_search_num_kernels(q)
+
+    def search_with_reuse(self, *args, **kwargs):
+        """Refused: the reference's Stochastic MuZero has no search_with_reuse, and stochastic trees have no reuse descent."""
+        raise NotImplementedError("StochasticMuZeroMCTSCtree has no search_with_reuse (stochastic trees have no reuse descent)")
+
+    def _search_stepwise_stochastic(self, roots, model, lat, S):
+        """The search driven one simulation at a time around any model with the reference's
+        ``recurrent_inference(state, option, afterstate)``: chance leaves (odd depth) take the afterstate program
+        (afterstate=False), the others the dynamics program (mcts_ctree_stochastic.py:171-212)."""
+        t, dev, B = roots._tree, roots.device, roots.num
+        self._make_inverse_transforms(dev)
+        pool = torch.empty((S + 1,) + tuple(lat.shape), device=dev, dtype=torch.float32)
+        pool[0] = lat
+        rows = torch.arange(B, device=dev)
+        with torch.no_grad(), torch.cuda.device(dev):
+            if hasattr(model, "eval"):
+                model.eval()
+            for sim in range(S):
+                cabi.check(t.lib.lz_tree_traverse(t.h, int(self.deterministic), None, None, t.ix.data_ptr(), t.iy.data_ptr(),
+                                                  t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(), None,
+                                                  cabi.stream_ptr()), "lz_tree_traverse")
+                states, options = pool[t.ix.long(), rows], t.action.long()
+                chance = (t.search_len & 1).bool()
+                reward, value = torch.zeros(B, device=dev), torch.zeros(B, device=dev)
+                pol = torch.zeros(B, t.A, device=dev)
+                for is_chance in (True, False):
+                    sel = torch.nonzero(chance == is_chance).reshape(-1)
+                    if sel.numel() == 0:
+                        continue
+                    out = model.recurrent_inference(states[sel], options[sel], afterstate=not is_chance)
+                    pool[sim + 1, sel] = out.latent_state.to(torch.float32)
+                    value[sel] = self._inv(out.value).reshape(-1)
+                    reward[sel] = self._inv_reward(out.reward).reshape(-1)
+                    logits = out.policy_logits.to(torch.float32)
+                    pol[sel, :logits.shape[1]] = logits
+                cabi.check(t.lib.lz_tree_backpropagate(t.h, sim + 1, reward.data_ptr(), value.data_ptr(), pol.data_ptr(), None,
+                                                       None, None, None, cabi.stream_ptr()), "lz_tree_backpropagate")

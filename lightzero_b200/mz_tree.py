@@ -59,18 +59,24 @@ class TreeHandle:
                 cabi.check(self.lib.lz_tree_set_params(self.h, *p), "lz_tree_set_params")
             self.params = p
 
-    def set_mode(self, mode=(), deterministic: bool = True, gumbel=(0, 0)):
+    def set_mode(self, mode=(), deterministic: bool = True, gumbel=(0, 0), stochastic=(0, 0, -1.0)):
         """Puts the tree in one holder's whole mode: ``mode`` () for MuZero or (1, lstm_horizon_len) for EfficientZero
         value-prefix trees (the ``search_for`` mode), ``gumbel`` (max_num_considered_actions, num_simulations) for a Gumbel
-        tree, and the tie rule of the EfficientZero and *_with_reuse descents (``deterministic``: the first maximum, else the
-        uniform draw).  The mode is C state that outlives its holder, so every acquirer sets all of it, once: a change bumps
-        the tree's generation and re-captures its search graphs (csrc/search.cu)."""
+        tree, ``stochastic`` (action_space_size, chance_space_size, chance_u) for a Stochastic MuZero tree
+        (lz_tree_set_stochastic), and the tie rule of the EfficientZero and *_with_reuse descents (``deterministic``: the first
+        maximum, else the uniform draw).  The mode is C state that outlives its holder, so every acquirer sets all of it,
+        once: a change bumps the tree's generation and re-captures its search graphs (csrc/search.cu)."""
+        if not stochastic[1]:       # first: the EfficientZero and Gumbel modes refuse a stochastic tree
+            cabi.check(self.lib.lz_tree_set_stochastic(self.h, 0, 0, -1.0), "lz_tree_set_stochastic")
         if gumbel[1]:       # a Gumbel tree is a MuZero tree
             cabi.check(self.lib.lz_tree_set_ez(self.h, 0, 5), "lz_tree_set_ez")
             cabi.check(self.lib.lz_tree_set_gumbel(self.h, int(gumbel[0]), int(gumbel[1])), "lz_tree_set_gumbel")
         else:
             cabi.check(self.lib.lz_tree_set_gumbel(self.h, 0, 0), "lz_tree_set_gumbel")
             cabi.check(self.lib.lz_tree_set_ez(self.h, *(mode or (0, 5))), "lz_tree_set_ez")
+        if stochastic[1]:
+            cabi.check(self.lib.lz_tree_set_stochastic(self.h, int(stochastic[0]), int(stochastic[1]), float(stochastic[2])),
+                       "lz_tree_set_stochastic")
         cabi.check(self.lib.lz_tree_set_tiebreak(self.h, int(bool(deterministic))), "lz_tree_set_tiebreak")
 
     def release(self):
@@ -207,6 +213,7 @@ class Roots:
         self._values = None       # root value estimates of a Gumbel tree's prepare (set by gmz_tree.Roots)
         self._ez, self._lstm_horizon = False, 5     # EfficientZero value-prefix semantics (set by ez_tree.Roots)
         self._deterministic = True     # tie rule of the EfficientZero / *_with_reuse descents (the mirrors: first maximum)
+        self._stochastic = (0, 0, -1.0)     # Stochastic MuZero tree mode (set by stochastic_mz_tree.Roots)
         self._tree: Optional[TreeHandle] = None
         self._delta_reset = None
 
@@ -331,7 +338,7 @@ class Roots:
         if params is not None:
             t.set_params(*params)
         with torch.cuda.device(self.device):
-            t.set_mode((1, int(self._lstm_horizon)) if self._ez else (), self._deterministic, gumbel)
+            t.set_mode((1, int(self._lstm_horizon)) if self._ez else (), self._deterministic, gumbel, self._stochastic)
         return t
 
     def _reset_tree(self, t, s):
