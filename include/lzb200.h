@@ -382,8 +382,8 @@ int lz_search_destroy(lz_search *q);
  * On a stochastic tree (lz_tree_set_stochastic) with a StochasticMuZeroModelMLP: StochasticMuZeroMCTSCtree.search
  * (mcts_ctree_stochastic.py:117-252), one CUDA graph of [descent] + num_simulations x [the afterstate program on the leaves that
  * are chance nodes, the dynamics program on the others (one row mask, its two parities), back-up + next descent]; both programs
- * write the same latent pool slot.  `deterministic` is the decision nodes' tie rule.  Stochastic searches are not collected on
- * the device (lz_search_collect*: LZ_EINVAL). */
+ * write the same latent pool slot.  `deterministic` is the decision nodes' tie rule.  lz_search_collect* runs the same graph
+ * (see there). */
 int lz_search_run(lz_search *q, const float *d_latent_roots, int deterministic, lz_stream s);
 /* MuZeroMCTSCtree.search_with_reuse (mcts_ctree.py:370-468; ReZero) and EfficientZeroMCTSCtree.search_with_reuse (:878-1003).
  * d_true_action int32 [B], d_reuse_value f32 [B] as for the reuse lz_tree_traverse; d_infer_count int32 [num_simulations] or
@@ -406,7 +406,15 @@ int lz_search_run_ez(lz_search *q, const float *d_latent_roots, const float *d_h
  * On a Gumbel tree (lz_tree_set_gumbel) lz_tree_prepare takes the root value prediction as the roots' values
  * (GumbelMuZeroPolicy._forward_collect, gumbel_muzero.py:560-571) and the search is the Gumbel graph of lz_search_run; the
  * search's num_simulations may not exceed the tree's Gumbel num_simulations (LZ_EINVAL).  The same holds for the three
- * entry points below.  Read the results with lz_tree_results and lz_tree_gumbel_select_action. */
+ * entry points below.  Read the results with lz_tree_results and lz_tree_gumbel_select_action.
+ * On a stochastic tree (lz_tree_set_stochastic) with a StochasticMuZeroModelMLP (StochasticMuZeroPolicy._forward_collect /
+ * _forward_eval, lzero/policy/stochastic_muzero.py:578-760) the search is the stochastic graph of lz_search_run, and every row
+ * of d_mask, d_noise and d_policy_logits is the tree's width W = max(action_space_size, chance_space_size) wide: d_policy_logits
+ * receives initial_inference's policy in the first action_space_size columns of each row (the others are not written), mask
+ * columns at action_space_size and beyond are ignored and noise columns past the legal count are not read.  The step's reset
+ * advances the tree's RNG epoch, so with chance_u < 0 successive collects (and replays of one captured graph) draw their chance
+ * outcomes independently; with chance_u in [0, 1) every draw is the pinned one.  lz_tree_select_action then reads the root's
+ * legal children and returns action ids < action_space_size.  The same holds for the host entry points below. */
 int lz_search_collect(lz_search *q, const float *d_obs, const uint8_t *d_mask, const float *d_noise,
                       float noise_weight, const int32_t *d_to_play, int deterministic,
                       float *d_pred_value, float *d_policy_logits, lz_stream s);

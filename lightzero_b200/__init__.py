@@ -11,8 +11,9 @@ from .muzero_model_mlp import MuZeroModelMLP  # noqa: F401
 from .stochastic_muzero_model_mlp import StochasticMuZeroModelMLP  # noqa: F401
 from .scaling_transform import DiscreteSupport, InverseScalarTransform  # noqa: F401
 from . import ez_tree, gmz_tree, mz_tree, stochastic_mz_tree  # noqa: F401
-from .collect import EfficientZeroCollectPolicy, GumbelMuZeroCollectPolicy, MuZeroCollectPolicy  # noqa: F401
+from .collect import (EfficientZeroCollectPolicy, GumbelMuZeroCollectPolicy, MuZeroCollectPolicy,  # noqa: F401
+                      StochasticMuZeroCollectPolicy)
 
 __all__ = ["MuZeroMCTSCtree", "EfficientZeroMCTSCtree", "GumbelMuZeroMCTSCtree", "gmz_tree", "UniZeroMCTSCtree", "EfficientZeroModel", "EfficientZeroModelMLP", "EZNetworkOutput", "ez_tree", "MuZeroModel", "MuZeroModelMLP", "MZNetworkOutput", "DiscreteSupport",
            "InverseScalarTransform", "mz_tree", "MuZeroCollectPolicy", "EfficientZeroCollectPolicy",
-           "GumbelMuZeroCollectPolicy", "StochasticMuZeroMCTSCtree", "StochasticMuZeroModelMLP", "stochastic_mz_tree"]
+           "GumbelMuZeroCollectPolicy", "StochasticMuZeroCollectPolicy", "StochasticMuZeroMCTSCtree", "StochasticMuZeroModelMLP", "stochastic_mz_tree"]

@@ -16,10 +16,12 @@ import torch
 from . import cabi, mz_tree
 from .efficientzero_model import EfficientZeroModel
 from .efficientzero_model_mlp import EfficientZeroModelMLP
-from .mcts_ctree import EfficientZeroMCTSCtree, GumbelMuZeroMCTSCtree, MuZeroMCTSCtree
+from .mcts_ctree import EfficientZeroMCTSCtree, GumbelMuZeroMCTSCtree, MuZeroMCTSCtree, StochasticMuZeroMCTSCtree
 from .model_base import LzModel
 from .muzero_model import MuZeroModel
 from .muzero_model_mlp import MuZeroModelMLP
+from .stochastic_muzero_model_mlp import StochasticMuZeroModelMLP
+from .stochastic_mz_tree import chance_uniform
 
 _NP = {torch.uint8: np.uint8, torch.float32: np.float32, torch.int32: np.int32}
 
@@ -96,7 +98,7 @@ class MuZeroCollectPolicy:
         runs select_action (policy/utils.py:637-661) on the device and returns 'action' / 'entropy' (GumbelMuZeroCollectPolicy: the
         Gumbel read-out, which adds 'improved_policy' / 'completed_values' [B, A])."""
         B = obs.shape[0]
-        A = self.model.action_space_size
+        A = self._width()
         S = int(self.cfg.num_simulations)
         bufs = self._bufs(B, A)
         dev = self.device
@@ -153,6 +155,10 @@ class MuZeroCollectPolicy:
                    pred_value=bufs["h_pred"], policy_logits=bufs["h_logits"])
         out.update({k: bufs["h_" + k] for k in selected})
         return out
+
+    def _width(self):
+        """The row width of the tree and of the mask, noise and logits buffers: the action count."""
+        return self.model.action_space_size
 
     def _held_tree(self, B, A, S, det):
         """A pooled tree in this policy's mode for one search_batch: the collect's tie rule is its ``deterministic``, which
@@ -298,3 +304,50 @@ class GumbelMuZeroCollectPolicy(MuZeroCollectPolicy):
             out['predicted_policy_logits'] = logits[i].tolist()
             output[env_id] = out
         return output
+
+
+def _pad_columns(x, W):
+    """A [B, n] mask or noise argument (tensor, array or list of rows) zero padded to [B, W], where it already lives."""
+    if isinstance(x, torch.Tensor):
+        return torch.nn.functional.pad(x, (0, W - x.shape[1]))
+    x = np.asarray(x)
+    return np.pad(x, ((0, 0), (0, W - x.shape[1])))
+
+
+class StochasticMuZeroCollectPolicy(MuZeroCollectPolicy):
+    """The same for ``StochasticMuZeroPolicy._forward_collect`` / ``_forward_eval`` (lzero/policy/stochastic_muzero.py:578-760)
+    with a ``StochasticMuZeroModelMLP``: the pooled tree is a stochastic tree W = max(action_space_size, chance_space_size)
+    wide, and one ``lz_search_collect*`` call runs initial_inference, the root reset and prepare and the stochastic search
+    graph.  The config key ``chance_seed`` is read as ``StochasticMuZeroMCTSCtree`` reads it: an integer pins every chance draw
+    to std::mt19937(chance_seed)'s, None samples each step's draws afresh.  Masks and noises are [B, action_space_size] as the
+    reference takes them; ``search_batch`` returns visits [B, W] (-1 padded, as ``stochastic_mz_tree.Roots``) and policy
+    logits [B, action_space_size].  Output dicts have the reference's keys."""
+
+    def __init__(self, model: StochasticMuZeroModelMLP, cfg: Optional[dict] = None):
+        if not isinstance(model, StochasticMuZeroModelMLP):
+            raise TypeError(f"StochasticMuZeroCollectPolicy: the stochastic search runs a StochasticMuZeroModelMLP, not a "
+                            f"{type(model).__name__}")
+        super().__init__(model, cfg)
+        self.mcts = StochasticMuZeroMCTSCtree(cfg or {})
+        self.cfg = self.mcts._cfg
+
+    def _width(self):
+        return max(self.model.action_space_size, self.model.chance_space_size)
+
+    def _held_tree(self, B, W, S, det):
+        """A stochastic tree; the decision nodes' tie rule is the collect's ``deterministic``."""
+        seed = self.cfg.chance_seed
+        u = -1.0 if seed is None else chance_uniform(seed)
+        return mz_tree.held_tree(self.device, B, W, S, self.mcts._params(), (), det,
+                                 stochastic=(self.model.action_space_size, self.model.chance_space_size, u))
+
+    def search_batch(self, obs: torch.Tensor, action_mask, noises, to_play=None, deterministic=None,
+                     read_back: bool = True, select=None):
+        """MuZeroCollectPolicy.search_batch on the stochastic tree: action_mask and noises [B, action_space_size] are padded
+        to the tree's width W with zero columns, and the returned policy logits are the first action_space_size columns of
+        the [B, W] rows the collect writes."""
+        W = self._width()
+        out = super().search_batch(obs, _pad_columns(action_mask, W), None if noises is None else _pad_columns(noises, W),
+                                   to_play, deterministic, read_back, select)
+        out["policy_logits"] = out["policy_logits"][:, :self.model.action_space_size]
+        return out

@@ -5,7 +5,8 @@ environment over PCIe and nothing comes back except the chosen actions.
 * ``FrameStack``     -- ``GameSegment.get_obs()`` / ``append()`` / the ``frame_stack_num`` seeding (game_segment.py:140-181,
                         muzero_collector.py:451-457): [B, stack, H, W] uint8 on the device, oldest frame first;
 * ``SegmentStats``   -- ``GameSegment.store_search_stats`` / ``reset`` (game_segment.py:241-263, 340-362): child-visit distributions
-                        and root values (and Gumbel MuZero's improved policies) appended per step for B segments of capacity T;
+                        and root values (and Gumbel MuZero's improved policies) appended per step for B segments of capacity T,
+                        from any search family's collect, Stochastic MuZero's wider tree rows included;
 * ``gather_segments``-- the all-gather of finished segments across ranks (one NCCL ``all_gather_into_tensor`` of a packed buffer).
 
 All compute is in ``csrc/collector.cu`` behind the C ABI (include/lzb200.h); there is no CPU fallback.
@@ -97,8 +98,13 @@ class SegmentStats:
     def store_search_stats(self, visit_counts: torch.Tensor, root_values: torch.Tensor, active=None, improved_policy=None) -> None:
         """game_segment.py:241-263 for every (active) environment: ``visit_counts`` int32 [B, A] (-1 beyond the legal list, as
         ``lz_tree_results`` / ``Roots`` deliver them on the device), ``root_values`` f32 [B], and for Gumbel MuZero
-        ``improved_policy`` f32 [B, A] by action id (``GumbelMuZeroCollectPolicy.search_batch``'s ``improved_policy``)."""
-        v = visit_counts.to(self.device, torch.int32).contiguous()
+        ``improved_policy`` f32 [B, A] by action id (``GumbelMuZeroCollectPolicy.search_batch``'s ``improved_policy``).  The
+        visits of a Stochastic MuZero tree are [B, max(A, chance_space_size)] wide: the first A columns, which hold every legal
+        root child, are stored."""
+        v = visit_counts.to(self.device, torch.int32)
+        if v.shape[1] > self.A:
+            v = v[:, :self.A]
+        v = v.contiguous()
         r = root_values.to(self.device, torch.float32).contiguous()
         a = None if active is None else torch.as_tensor(active).to(self.device, torch.uint8).contiguous()
         with torch.cuda.device(self.device):

@@ -605,6 +605,7 @@ int mez_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, cud
     MezIO e = mez_io(m, B);
     e.obs = d_obs; e.latent_out = io_in.latent; e.latent_out2 = io_in.latent2;
     e.value = io_in.value; e.policy_logits = io_in.policy_logits; e.value_logits = io_in.value_logits;
+    e.policy_stride = io_in.policy_stride;
     return mez_launch(m->mez.init, e, s);
 }
 

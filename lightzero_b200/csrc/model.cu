@@ -104,6 +104,8 @@ int model_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
 
 int model_initial(lz_model *m, int B, const float *d_obs, const TailIO &io, cudaStream_t s)
 {
+    LZ_REQUIRE(!io.policy_stride || io.policy_stride == m->A || m->family == ModelFamily::MlpTc, LZ_EINVAL,
+               "model_initial: policy logits at a row stride of %d other than the %d actions are the MlpTc programs'", io.policy_stride, m->A);
     switch (m->family) {
         case ModelFamily::Conv: return conv_initial(m, B, d_obs, io, s);
         case ModelFamily::Board: return board_initial(m, B, d_obs, io, s);

@@ -70,8 +70,9 @@ struct TailIO {
     float *latent;                    // [B][C][P] (NCHW) or nullptr
     float *latent2;                   // second copy (latent pool slot 0) or nullptr
     float *value;                     // [B] scalar or nullptr
-    float *policy_logits;             // [B][A] or nullptr
+    float *policy_logits;             // [B][A] (row stride policy_stride) or nullptr
     float *value_logits;              // [B][K] or nullptr
+    int policy_stride;                // row stride of policy_logits (0: A); only the MlpTc programs take a stride other than A
 };
 
 // The model families: each has its own state below and its own module; model.cu switches on the family at every lz_model_*

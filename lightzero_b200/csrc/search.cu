@@ -218,13 +218,16 @@ static int gumbel_sims_check(const lz_search *q, const char *fn)
 
 // lz_search_collect*: reset the roots to the legal mask, prepare them from the initial inference's logits (+ noise), then search.
 // A Gumbel tree also takes the initial inference's root values d_values (GumbelMuZeroPolicy._forward_collect,
-// lzero/policy/gumbel_muzero.py:560-571) and runs the Gumbel search graph.
+// lzero/policy/gumbel_muzero.py:560-571) and runs the Gumbel search graph.  A stochastic tree runs the stochastic search graph
+// (StochasticMuZeroPolicy._forward_collect, lzero/policy/stochastic_muzero.py:578-760); its logits, mask and noise rows are the
+// tree's width max(A, C) wide, and the reset bumps the RNG epoch that keys the sampled chance draws of the step.
 static int collect_search(lz_search *q, const uint8_t *d_mask, const float *d_logits, const float *d_values, const float *d_noise,
                           float noise_weight, const int32_t *d_to_play, int deterministic, cudaStream_t s)
 {
     int rc;
     lz_tree *t = q->tree;
-    LZ_REQUIRE(!t->p.nc, LZ_EINVAL, "lz_search_collect: stochastic trees are not collected on the device");
+    LZ_REQUIRE((q->d_len != nullptr) == (t->p.nc != 0), LZ_ESTATE,
+               "lz_search_collect: the tree's stochastic mode does not match the model (lz_tree_set_stochastic)");
     if ((rc = lz_tree_reset_mask(t, d_mask, s))) return rc;                        // policy/muzero.py:760,769
     const float *values = t->gumbel ? d_values : nullptr;
     if ((rc = lz_tree_prepare(t, d_logits, d_noise, noise_weight, nullptr, values, d_to_play, s))) return rc;   // :774
@@ -365,6 +368,7 @@ static int collect_device(lz_search *q, const float *d_obs, const uint8_t *d_obs
     io.latent2 = q->pool;                                   // latent roots go straight into pool slot 0
     io.policy_logits = d_policy_logits ? d_policy_logits : q->d_root_logits;
     io.value = d_pred_value ? d_pred_value : q->d_root_value;
+    io.policy_stride = q->A;                                // the tree's width: max(A, C) on a stochastic tree, else A
     if (d_obs_u8) {
         LZ_REQUIRE(q->model->family == ModelFamily::Conv, LZ_EINVAL, "lz_search_collect_u8: uint8 frames need the conv model");
         if (!q->d_pre_stage && (rc = dev_alloc(&q->d_pre_stage, (size_t)q->B * q->model->latent_floats))) return rc;
@@ -445,7 +449,8 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
             TailIO io;
             memset(&io, 0, sizeof(io));
             io.latent2 = q->pool + (size_t)b0 * q->model->latent_floats;
-            io.policy_logits = logits + (size_t)b0 * A;
+            io.policy_logits = logits + (size_t)b0 * A;     // rows of the tree's width
+            io.policy_stride = A;
             io.value = pred + b0;
             rc = model_initial(q->model, bc, q->d_obs_stage + (size_t)b0 * q->obs_elems, io, s);
         }
@@ -456,6 +461,7 @@ static int collect_host(lz_search *q, const void *h_obs, int obs_u8, const uint8
         memset(&io, 0, sizeof(io));
         io.latent2 = q->pool;
         io.policy_logits = logits;
+        io.policy_stride = A;
         io.value = pred;
         int rc = conv_initial_tail(q->model, B, q->d_pre_stage, io, s);
         if (rc) return rc;

@@ -366,7 +366,7 @@ __device__ __forceinline__ void expand_block(uint32_t *nb, int A, const float *l
 }
 
 // CRoots::CRoots (cnode.cpp:301-317) and a fresh MinMaxStats (cminimax.cpp:7-11) of tree b by the calling warp.  The root's legal
-// list comes from mask (uint8 [A], ascending ids == np.nonzero order, policy/muzero.py:760), else from legal[0, nlegal), else is
+// list comes from mask (uint8 [A], ascending ids < na == np.nonzero order, policy/muzero.py:760), else from legal[0, nlegal), else is
 // every action (as is an empty list, cnode.cpp:101-107).  The tree-wide words (players_max, rng_epoch) are the launch's job.
 __device__ __forceinline__ void tree_reset_root(const TreeParams &p, int b, int lane, const uint8_t *mask, const int32_t *legal,
                                                 int nlegal)
@@ -377,7 +377,7 @@ __device__ __forceinline__ void tree_reset_root(const TreeParams &p, int b, int 
     if (mask) {
         for (int c0 = 0; c0 < A; c0 += 32) {
             int a = c0 + lane;
-            bool on = a < A && mask[a] != 0;
+            bool on = a < p.na && mask[a] != 0;     // a stochastic root's row is A = max(na, nc) wide: columns >= na are no action
             unsigned m = __ballot_sync(0xffffffffu, on);
             if (on) lg[n + __popc(m & ((1u << lane) - 1u))] = a;
             n += __popc(m);

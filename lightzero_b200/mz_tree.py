@@ -128,13 +128,14 @@ def acquire_tree(device, B, A, max_sims) -> TreeHandle:
 
 
 @contextlib.contextmanager
-def held_tree(device, B, A, max_sims, params, mode=(), deterministic: bool = True, gumbel=(0, 0)):
+def held_tree(device, B, A, max_sims, params, mode=(), deterministic: bool = True, gumbel=(0, 0), stochastic=(0, 0, -1.0)):
     """A pooled tree with these parameters and this whole mode (TreeHandle.set_mode) for the length of one call, released
-    at its end even when the call raises."""
+    at its end even when the call raises.  ``A`` is the tree's width: max(action_space_size, chance_space_size) for a
+    ``stochastic`` (action_space_size, chance_space_size, chance_u) tree."""
     t = acquire_tree(device, B, A, max_sims)
     try:
         t.set_params(*params)
-        t.set_mode(mode, deterministic, gumbel)
+        t.set_mode(mode, deterministic, gumbel, stochastic)
         yield t
     finally:
         t.release()
