@@ -333,7 +333,13 @@ int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uin
  * fc_prediction_common.0 and .3, the value head's two layers, the policy head's two layers; every layer with its BN and
  * activation.  width is latent_dim, a head's hidden size, the support size or A.  stage == D runs the whole program and writes
  * latent [B, latent_dim], value logits [B,K], policy logits [B,A], value [B], and for `which` 0 reward logits [B,K], reward [B].
- * h_info: roots per CTA (4), CTA count, roots of the last CTA, D, width (0 for stage D), 0, 0, 0. */
+ * h_info: roots per CTA (4), CTA count, roots of the last CTA, D, width (0 for stage D), 0, 0, 0.
+ * MuZeroModelMLP and StochasticMuZeroModelMLP on the tensor cores: stages as for EfficientZeroModelMLP; stage == D writes latent
+ * [B, latent_dim], a zero section [B, latent_dim], value logits [B,K], policy logits [B,P], value [B], and for the recurrent
+ * programs reward logits [B,K], reward [B].  StochasticMuZeroModelMLP's `which` 0 is its dynamics program on afterstates
+ * d_latent and chance outcomes d_action (P = A); `which` 2 is its afterstate program on latents d_latent and actions d_action:
+ * the afterstate dynamics, its reward head and the afterstate prediction (P = chance_space_size).  Any other model refuses
+ * `which` 2 (LZ_EINVAL). */
 int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_latent, const int32_t *d_action, int stage,
                              void *d_out, size_t out_bytes, int32_t *h_info, lz_stream s);
 int lz_model_latent_hw(const lz_model *m);   /* 6 for 84/96, 8 for 64; a square board's side; 0 for a non-square board */

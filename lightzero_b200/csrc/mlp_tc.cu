@@ -609,14 +609,16 @@ int mez_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, cud
     return mez_launch(m->mez.init, e, s);
 }
 
-// lz_model_debug_net_stage of EfficientZeroModelMLP and of MuZeroModelMLP on the tensor cores: which 1 is initial_inference on
-// the observations d_in
+// lz_model_debug_net_stage of EfficientZeroModelMLP, MuZeroModelMLP and StochasticMuZeroModelMLP on the tensor cores: which 1
+// is initial_inference on the observations d_in, 0 the recurrent program, 2 StochasticMuZeroModelMLP's afterstate program (its
+// policy is chance_space_size wide)
 int mez_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out,
                            size_t out_bytes, int32_t *h_info, cudaStream_t st)
 {
-    MezNet net = which ? m->mez.init : m->mez.rec;          // a copy: the model's programs stay as they are
+    LZ_REQUIRE(which != 2 || m->mez.chance, LZ_EINVAL, "lz_model_debug_net_stage: which 2 is StochasticMuZeroModelMLP's afterstate program");
+    MezNet net = which == 2 ? m->mez.after : which ? m->mez.init : m->mez.rec;   // a copy: the model's programs stay as they are
     const int L = net.L, K = net.K, A = net.A;
-    const bool rew = !which && !m->vp;               // MuZeroModelMLP's recurrent program has the reward head
+    const bool rew = which != 1 && !m->vp;           // MuZeroModelMLP's recurrent programs have the reward head
     int dense[kMezMaxLayers], D = 0;                        // the program indices of the L-wide layers outside the heads
     for (int l = 0; l < net.nlayers; ++l)
         if (net.layer[l].N == L && !(net.layer[l].flags & (MF_VALUE | MF_REWARD | MF_POLICY)) && net.layer[l].out != MB_HID) dense[D++] = l;
@@ -625,7 +627,7 @@ int mez_debug_stage(lz_model *m, int which, int B, const float *d_in, const int3
     LZ_REQUIRE(out_bytes >= nfl * sizeof(float), LZ_EINVAL, "lz_model_debug_net_stage: stage %d needs %zu bytes, got %zu", stage,
                nfl * sizeof(float), out_bytes);
     MezIO io = mez_io(m, B);
-    if (which) io.obs = d_in;
+    if (which == 1) io.obs = d_in;
     else { io.latent_base = d_in; io.action = d_action; }
     float *o = reinterpret_cast<float *>(d_out);
     if (stage < D) {

@@ -334,9 +334,11 @@ int lz_model_initial_inference(lz_model *m, int B, const float *d_obs, float *d_
 int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_latent, const int32_t *d_action, int stage, void *d_out,
                              size_t out_bytes, int32_t *h_info, lz_stream s_)
 {
-    LZ_REQUIRE(m && (which == 0 || which == 1) && B > 0 && d_latent && (which == 1 || d_action) && d_out && h_info && stage >= 0,
+    LZ_REQUIRE(m && which >= 0 && which <= 2 && B > 0 && d_latent && (which == 1 || d_action) && d_out && h_info && stage >= 0,
                LZ_EINVAL, "lz_model_debug_net_stage: bad argument");
     LZ_REQUIRE(m->finalized, LZ_ESTATE, "lz_model_debug_net_stage: model not finalized");
+    LZ_REQUIRE(which != 2 || (m->family == ModelFamily::MlpTc && m->mez.chance), LZ_EINVAL,
+               "lz_model_debug_net_stage: which 2 (the afterstate program) is StochasticMuZeroModelMLP's");
     const cudaStream_t s = (cudaStream_t)s_;
     switch (m->family) {
         case ModelFamily::Conv: return conv_debug_stage(m, which, B, d_latent, d_action, stage, d_out, out_bytes, h_info, s);

@@ -164,10 +164,10 @@ class Roots:
 
     def tie_stats(self):
         """descents with more than one tie, hash draws other than the first tie, tie lists with unequal scores (near ties),
-        longest search path"""
-        out = np.zeros(4, np.int64)
+        longest search path, chance draws over two or more outcomes (Stochastic MuZero trees)"""
+        out = np.zeros(5, np.int64)
         lib().lzo_tree_tie_stats(self._h, _p(out))
-        return dict(ties=int(out[0]), draws=int(out[1]), near=int(out[2]), max_len=int(out[3]))
+        return dict(ties=int(out[0]), draws=int(out[1]), near=int(out[2]), max_len=int(out[3]), chance=int(out[4]))
 
     def clear(self):
         pass

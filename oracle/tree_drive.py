@@ -1,26 +1,32 @@
 """The reference search loops, written once, for every tree module the tests drive.  TEST INFRASTRUCTURE ONLY.
 
 `drive(mod, case, kind, leaves)` runs one search of the reference driver protocol on `mod`: the compiled reference
-(oracle/_ref), the C port (oracle.ctree_port / ctree_port_ez) or a device mirror (lightzero_b200.mz_tree / ez_tree /
-gmz_tree).  Kinds and the loops they restate:
+(oracle/_ref), the C port (oracle.ctree_port / ctree_port_ez / ctree_port_stoch) or a device mirror (lightzero_b200.mz_tree /
+ez_tree / gmz_tree / stochastic_mz_tree).  Kinds and the loops they restate:
   mz        MuZeroMCTSCtree.search                      mcts_ctree.py:267-368
   ez        EfficientZeroMCTSCtree.search               mcts_ctree.py:729-876    (is_reset = search_len % horizon == 0)
   reuse     MuZeroMCTSCtree.search_with_reuse           mcts_ctree.py:370-468    (compacted inference batch)
   ez_reuse  EfficientZeroMCTSCtree.search_with_reuse    mcts_ctree.py:878-1003
   gumbel    GumbelMuZeroMCTSCtree.search                mcts_ctree.py:1104-1172
+  stoch     StochasticMuZeroMCTSCtree.search            mcts_ctree_stochastic.py:117-252  (chance leaves backed up first,
+            then decision leaves, each call with its leaf_idx_list)
 
 A case is a dict with the key names of the committed fixtures (tests/golden), so `np.load(fixture)` is a case:
 B, A, S, legal (+ nlegal when padded), root_logits, to_play, and optionally use_noise / noise + noises, noise_w,
 pb_c_base, pb_c_init, discount, delta, lstm_horizon_len, true_action / reuse_value (reuse kinds), m / root_values
-(gumbel), and the recorded leaf outputs rewards / values_in / policies (gumbel: rewards / values / logits).
+(gumbel), C and chance_seed (stoch: None samples the chance draws from the tie hash key, which the port and the device
+mirror support, the compiled reference does not), and the recorded leaf outputs rewards / values_in / policies (gumbel:
+rewards / values / logits; stoch: policies max(A, C) wide).
 
-`leaves(s, ix, iy, last_action, keep, reset)` gives simulation s's (reward or value prefix, value, policy logits) for
-the batch rows `keep` (every row except the reuse kinds' no-inference ones); `reset` is the EfficientZero is_reset mask.
-Three sources: `recorded(case, kind)`, `Sampled(draw)` and `network(model, latent, hidden)`.
+`leaves(s, ix, iy, last_action, keep, mask)` gives simulation s's (reward or value prefix, value, policy logits) for
+the batch rows `keep` (every row except the reuse kinds' no-inference ones); `mask` is the EfficientZero is_reset mask, or
+for stoch the leaf_node_is_chance mask (the driver keeps the first C logits of a chance leaf's row, the first A of a
+decision leaf's).  Three sources: `recorded(case, kind)`, `Sampled(draw)` and `network(model, latent, hidden)`.
 """
 import numpy as np
 
-PER_SIM = ("ix", "iy", "last_action", "search_len", "virtual_to_play", "is_reset", "n_inferred", "no_inference", "reuse_list")
+PER_SIM = ("ix", "iy", "last_action", "search_len", "virtual_to_play", "is_reset", "n_inferred", "no_inference", "reuse_list",
+           "is_chance")
 
 
 def legal_lists(c):
@@ -33,15 +39,35 @@ def legal_lists(c):
 
 
 def fixture_kind(d):
+    if "C" in d:
+        return "stoch"
     if "m" in d:
         return "gumbel"
     H = int(d["lstm_horizon_len"]) if "lstm_horizon_len" in d else 0
     return ("ez_reuse" if H else "reuse") if "true_action" in d else ("ez" if H else "mz")
 
 
-def make_roots(mod, B, legal, A, S, horizon=5):
-    """Roots of any tree module: the port takes its action space and node budget, ez_tree.Roots the LSTM horizon."""
+def make_roots(mod, B, legal, A, S, horizon=5, C=None, chance_seed=None):
+    """Roots of any tree module: the port takes its action space and node budget, ez_tree.Roots the LSTM horizon, the
+    Stochastic MuZero modules the chance space (and the compiled reference the pinned random_device of chance_seed)."""
     name = mod.__name__
+    if C is not None:
+        if name == "oracle.ctree_port_stoch":
+            roots = mod.Roots(B, legal, C, max_sims=S, action_space_size=A)
+            if chance_seed is not None:
+                from lightzero_b200.stochastic_mz_tree import chance_uniform
+                roots.set_chance_u(chance_uniform(chance_seed))
+            return roots
+        if name == "lightzero_b200.stochastic_mz_tree":
+            return mod.Roots(B, legal, C, chance_seed=chance_seed, max_simulations=S)
+        if name != "stochastic_mz_tree":
+            raise ValueError(f"{name} has no chance nodes: a Stochastic MuZero case runs on oracle.ctree_port_stoch, "
+                             "lightzero_b200.stochastic_mz_tree or the compiled stochastic_mz_tree")
+        if chance_seed is None:
+            raise ValueError("the compiled reference tree draws its chance outcomes from a pinned random_device only")
+        from oracle import build_stoch_ref
+        build_stoch_ref.set_random_device(chance_seed)
+        return mod.Roots(B, legal, C)
     if name.startswith("oracle.ctree_port"):
         return mod.Roots(B, legal, action_space_size=A, max_sims=S)
     if name == "lightzero_b200.ez_tree":
@@ -67,10 +93,11 @@ def recorded(c, kind="mz"):
     return leaves
 
 
-def random_case(B, A, S, seed, masks, noise, two_player, scale, reuse=False, horizon=0):
+def random_case(B, A, S, seed, masks, noise, two_player, scale, reuse=False, horizon=0, C=None, chance_seed=None):
     """Seeded random inputs, drawn in this order: legal lists (60 % of the actions when masks, never empty), root
     logits, to_play, for ReZero the true actions and reuse values, then Dirichlet noise.  Returns the case and a Sampled
-    source that goes on drawing r, v, p (normal, times scale) per simulation from the same generator."""
+    source that goes on drawing r, v, p (normal, times scale) per simulation from the same generator.  C: a Stochastic
+    MuZero case, whose policies are max(A, C) wide."""
     rng = np.random.default_rng(seed)
     legal = []
     for _ in range(B):
@@ -90,7 +117,10 @@ def random_case(B, A, S, seed, masks, noise, two_player, scale, reuse=False, hor
     if noise:
         for b, l in enumerate(legal):
             c["noises"][b, :len(l)] = rng.dirichlet([0.3] * len(l)).astype(np.float32)
-    return c, Sampled(lambda: (normal(B), normal(B), normal((B, A))))
+    if C is not None:
+        c.update(C=C, chance_seed=chance_seed)
+    W = A if C is None else max(A, C)
+    return c, Sampled(lambda: (normal(B), normal(B), normal((B, W))))
 
 
 class Sampled:
@@ -106,16 +136,42 @@ class Sampled:
         return [x[:len(keep)].tolist() for x in out]
 
 
-def network(model, latent, hidden=None, zero_reset_state=True):
+def network(model, latent, hidden=None, zero_reset_state=True, stochastic=False):
     """A CUDA model evaluating the gathered leaves with return_scalars=True.  Latents (and for EfficientZero the LSTM
     state (h, c), each [B, H]) are kept per simulation and gathered at (ix, iy); the state stored for a reset leaf is
-    zeroed (mcts_ctree.py:856-863) unless zero_reset_state is False."""
+    zeroed (mcts_ctree.py:856-863) unless zero_reset_state is False.  stochastic: a StochasticMuZeroModelMLP, whose chance
+    leaves (odd depth) run recurrent_inference(afterstate=False) and the others afterstate=True
+    (mcts_ctree_stochastic.py:171-212)."""
     import torch
     pool = [latent]
     hpool = [hidden] if hidden is not None else None
 
     @torch.no_grad()
+    def stoch_leaves(s, ix, iy, la, keep, is_chance):
+        ixs, iys = np.asarray(ix)[keep], torch.as_tensor(np.asarray(iy)[keep], device=latent.device)
+        lat = torch.empty((len(keep),) + tuple(latent.shape[1:]), device=latent.device, dtype=latent.dtype)
+        for x in np.unique(ixs):            # gather the leaves' parents slot by slot
+            rows = torch.as_tensor(np.nonzero(ixs == x)[0], device=latent.device)
+            lat[rows] = pool[int(x)][iys[rows]]
+        act = torch.tensor([la[k] for k in keep], device=lat.device)
+        nxt = torch.zeros_like(lat)
+        r, v, p = [0.0] * len(keep), [0.0] * len(keep), [None] * len(keep)
+        for chance in (True, False):
+            sel = [k for k in keep if bool(is_chance[k]) == chance]
+            if not sel:
+                continue
+            o = model.recurrent_inference(lat[sel], act[sel], afterstate=not chance, return_scalars=True)
+            nxt[sel] = o.latent_state
+            for k, rk, vk, pk in zip(sel, o.reward_scalar.cpu().tolist(), o.value_scalar.cpu().tolist(),
+                                     o.policy_logits.cpu().tolist()):
+                r[k], v[k], p[k] = rk, vk, pk
+        pool.append(nxt)
+        return r, v, p
+
+    @torch.no_grad()
     def leaves(s, ix, iy, la, keep, reset):
+        if stochastic:
+            return stoch_leaves(s, ix, iy, la, keep, reset)
         if not keep:
             pool.append(None)
             if hpool is not None:
@@ -170,7 +226,12 @@ def drive(mod, c, kind, leaves, det=True, setup=None, reset_in_backup=True):
     is_reset (ez kinds) or n_inferred, no_inference, reuse_list (reuse kinds), each [S, B] ([S] / [S, B + 1]); then
     the readout()."""
     B, A, S = int(c["B"]), int(c["A"]), int(c["S"])
-    gumbel, ez, reuse = kind == "gumbel", kind in ("ez", "ez_reuse"), kind in ("reuse", "ez_reuse")
+    gumbel, ez, reuse, stoch = kind == "gumbel", kind in ("ez", "ez_reuse"), kind in ("reuse", "ez_reuse"), kind == "stoch"
+    C = int(c["C"]) if stoch else None
+    chance_seed = c.get("chance_seed") if stoch else None
+    if chance_seed is not None and np.ndim(chance_seed) == 0 and int(chance_seed) < 0:
+        chance_seed = None          # fixtures store a sampled case's chance_seed as -1
+    chance_seed = None if chance_seed is None else int(chance_seed)
     disc = float(c.get("discount", 0.997))
     horizon = int(c.get("lstm_horizon_len", 5))
     legal = legal_lists(c)
@@ -182,7 +243,7 @@ def drive(mod, c, kind, leaves, det=True, setup=None, reset_in_backup=True):
         noises = [_f32(c["noises"][b][:len(l)]).tolist() for b, l in enumerate(legal)]
     logits = _f32(c["root_logits"]).tolist()
     pre = [_f32(c["root_values"]).tolist()] if gumbel else []
-    roots = make_roots(mod, B, legal, A, S, horizon)
+    roots = make_roots(mod, B, legal, A, S, horizon, C, chance_seed)
     if noises is None:
         roots.prepare_no_noise([0.] * B, *pre, logits, tp)
     else:
@@ -205,13 +266,18 @@ def drive(mod, c, kind, leaves, det=True, setup=None, reset_in_backup=True):
             ix, iy, la, vtp = mod.batch_traverse_with_reuse(roots, *pbc, res, list(tp), ta, rv)
         elif ez:
             ix, iy, la, vtp = mod.batch_traverse(roots, *pbc, res, list(tp))
+        elif stoch:        # the compiled reference has no deterministic switch (rand() == 0: the first maximum)
+            kw = {} if mod.__name__ == "stochastic_mz_tree" else dict(deterministic=det)
+            ch, ix, iy, la, vtp = mod.batch_traverse(roots, *pbc, res, list(tp), **kw)
+            ch = np.asarray([bool(x) for x in ch])
+            t["is_chance"].append(ch.astype(np.int32))
         else:
             ix, iy, la, vtp = mod.batch_traverse(roots, *pbc, res, list(tp), det)
         ix, iy, la, vtp = list(ix), list(iy), list(la), list(vtp)
         slen = list(res.get_search_len())
         for k, v in zip(PER_SIM, (ix, iy, la, slen, vtp)):
             t[k].append(v)
-        reset = (np.asarray(slen) % horizon == 0) if ez else None
+        reset = (np.asarray(slen) % horizon == 0) if ez else (ch if stoch else None)
         keep = [k for k in range(B) if ix[k] != -1]
         r, v, p = leaves(s, ix, iy, la, keep, reset)
         args = (s + 1, disc, r, v, p, mm, res)
@@ -221,6 +287,13 @@ def drive(mod, c, kind, leaves, det=True, setup=None, reset_in_backup=True):
             rs = [(reset if reset_in_backup else np.zeros(B, bool)).astype(np.int32).tolist()]
         if gumbel:
             mod.batch_back_propagate(*args, vtp)
+        elif stoch:        # chance leaves first, then decision leaves (mcts_ctree_stochastic.py:229-252)
+            for chance in (True, False):
+                idx = [k for k in range(B) if ch[k] == chance]
+                if idx:
+                    rows = [list(p[k])[:C if chance else A] for k in idx]
+                    mod.batch_backpropagate(s + 1, disc, [r[k] for k in idx], [v[k] for k in idx], rows, mm, res, vtp,
+                                            [bool(x) for x in ch], idx)
         elif reuse:        # no_inference_lst / reuse_lst as the driver builds them, -1 terminated
             no_inf = [iy[k] for k in range(B) if ix[k] == -1]
             reuse_lst = [k for k in range(B) if ix[k] == 0 and la[k] == ta[k]]

@@ -30,6 +30,9 @@ CONFIGS = {
     "l256_c608": (10, 3, 608, 256, False, 32, (-300., 301., 1.)),
     # a chance space wider than the action space at a middle latent, hidden layers of 16
     "l64_c9_res": (5, 4, 9, 64, True, 16, (-300., 301., 1.)),
+    # the longest programs: residual dynamics, 608 actions, 608 outcomes and 608 support bins at L = 32, so the `after` and `rec`
+    # programs both cut each FC2 into 19 pieces and reach the kernel's 66 layers
+    "l32_a608_c608": (8, 608, 608, 32, True, 32, (-304., 304., 1.)),
 }
 
 

@@ -10,7 +10,6 @@ StochasticMuZeroMCTSCtree):
   sampled search repeats bit for bit for a fixed RNG key, and the draws of one descent are keyed by depth;
 - the fused search on a side stream next to a busy legacy default stream (tests/test_gpu_streams.py's harness);
 - the reuse search is refused on stochastic trees, and only the stochastic model keeps afterstate_* tensors."""
-import copy
 import hashlib
 import os
 
@@ -129,34 +128,14 @@ def test_masked_launch(afterstate):
 
 
 # ---- trees -------------------------------------------------------------------------------------------------------------
-def reference_loop(T, roots, model, lat, S, to_play, deterministic=None):
-    """mcts_ctree_stochastic.py:117-252 with the module T (the compiled reference or lightzero_b200.stochastic_mz_tree)
-    driving `model`; the network's own scalars (softmax . support -> h^-1 in the kernel) are what both trees back up"""
-    B = roots.num
-    mm = T.MinMaxStatsList(B)
-    mm.set_delta(0.01)
-    pool = [lat.cpu().numpy()]
-    kw = {} if deterministic is None else dict(deterministic=deterministic)
-    for sim in range(S):
-        res = T.ResultsWrapper(B)
-        is_chance, ix, iy, act, vtp = T.batch_traverse(roots, 19652, 1.25, 0.997, mm, res, copy.deepcopy(to_play), **kw)
-        states = torch.from_numpy(np.stack([pool[x][y] for x, y in zip(ix, iy)])).cuda()
-        acts = torch.as_tensor(act).cuda()
-        nxt = np.zeros_like(pool[0])
-        out = {}
-        for chance in (True, False):
-            idx = [i for i in range(B) if bool(is_chance[i]) == chance]
-            if not idx:
-                continue
-            o = model.recurrent_inference(states[idx], acts[idx], afterstate=not chance, return_scalars=True)
-            nxt[idx] = o.latent_state.cpu().numpy()
-            out[chance] = (idx, o.reward_scalar.cpu().tolist(), o.value_scalar.cpu().tolist(), o.policy_logits.cpu().tolist())
-        pool.append(nxt)
-        for chance in (True, False):
-            if chance in out:
-                idx, rw, vl, pl = out[chance]
-                T.batch_backpropagate(sim + 1, 0.997, rw, vl, pl, mm, res, vtp, list(is_chance), idx)
-    return readout(roots)
+def reference_loop(T, model, lat, legal, logits, noises, to_play, S, chance_seed):
+    """mcts_ctree_stochastic.py:117-252 (oracle/tree_drive.py, kind "stoch") with the module T (the compiled reference or
+    lightzero_b200.stochastic_mz_tree) driving `model`; the network's own scalars (softmax . support -> h^-1 in the kernel) are
+    what both trees back up.  Decision ties take the first maximum.  Returns (the drive's trace, roots)."""
+    from oracle.tree_drive import drive, network
+    c = dict(B=len(to_play), A=model.action_space_size, C=model.chance_space_size, S=S, legal=legal, root_logits=logits,
+             noises=noises, to_play=to_play, chance_seed=chance_seed)
+    return drive(T, c, "stoch", network(model, lat, stochastic=True), det=True)
 
 
 def readout(roots):
@@ -208,11 +187,13 @@ def test_tree_parity(name, B, two_player, masked, noise, seed, S):
             roots.prepare_no_noise([0.] * B, logits, to_play)
         return roots
 
-    build_stoch_ref.set_random_device(chance_seed)
-    want = reference_loop(oracle, prepare(oracle.Roots(B, legal, C)), cu, o.latent_state, S, to_play)
-    got = reference_loop(T, prepare(T.Roots(B, legal, C, chance_seed=chance_seed, max_simulations=S)), cu, o.latent_state, S,
-                         to_play, True)
-    assert_equal(got, want)
+    from oracle.tree_drive import assert_same
+    want, ref_roots = reference_loop(oracle, cu, o.latent_state, legal, logits, noises, to_play, S, chance_seed)
+    got, step_roots = reference_loop(T, cu, o.latent_state, legal, logits, noises, to_play, S, chance_seed)
+    assert_same(got, want)                  # per simulation is_chance, ix, iy, last_action, search_len, vtp, then the read-outs
+    want = readout(ref_roots)
+    assert_equal(readout(step_roots), want)
+    step_roots.clear()
     mcts = lzb.StochasticMuZeroMCTSCtree(dict(num_simulations=S, deterministic=True, chance_seed=chance_seed))
     roots = prepare(mcts.roots(B, legal, C))
     mcts.search(roots, cu, o.latent_state, to_play)
@@ -279,9 +260,8 @@ def test_sampled_search_repeats():
     name, B, S = "l64_c9_res", 77, 30        # a shape no other test pools: both trees are fresh
     cu, o, legal, noises, to_play, C = case(name, B, False, True, True, 9)
     logits = o.policy_logits.cpu().tolist()
-    step = T.Roots(B, legal, C, max_simulations=S)
-    step.prepare(0.25, noises, [0.] * B, logits, to_play)
-    got = reference_loop(T, step, cu, o.latent_state, S, to_play, True)
+    _, step = reference_loop(T, cu, o.latent_state, legal, logits, noises, to_play, S, None)
+    got = readout(step)
     mcts = lzb.StochasticMuZeroMCTSCtree(dict(num_simulations=S, deterministic=True, chance_seed=None))
     fused = mcts.roots(B, legal, C)
     fused.prepare(0.25, noises, [0.] * B, logits, to_play)

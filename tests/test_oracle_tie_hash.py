@@ -125,3 +125,108 @@ def test_near_ties_are_counted():
         port.batch_backpropagate(s + 1, 0.997, [0.] * B, [0.] * B, np.zeros((B, A), np.float32).tolist(), mm, res, vtp)
     st = roots.tie_stats()
     assert st["near"] == B and st["ties"] == 2 * B
+
+
+# ---- Stochastic MuZero chance draws --------------------------------------------------------------------------------------
+_LIBM = None
+
+
+def expf(x):
+    """glibc's expf, the one the port's expand calls"""
+    global _LIBM
+    if _LIBM is None:
+        import ctypes
+        _LIBM = ctypes.CDLL("libm.so.6")
+        _LIBM.expf.restype, _LIBM.expf.argtypes = ctypes.c_float, [ctypes.c_float]
+    return np.float32(_LIBM.expf(float(x)))
+
+
+def priors_of(logits):
+    """CNode::expand's softmax in float32, sequential in key order (ctree_stochastic_muzero cnode.cpp:143-166)"""
+    logits = np.asarray(logits, np.float32)
+    m = np.float32(np.max(logits))
+    temp = [expf(np.float32(x - m)) for x in logits]
+    s = np.float32(0.0)
+    for x in temp:
+        s = np.float32(s + x)
+    return [np.float32(x / s) for x in temp]
+
+
+def chance_u(seed, epoch, b, step, depth):
+    """the uniform of a hashed chance draw: the tie hash key, >> 11, times 2^-53"""
+    h = mix64(seed ^ mix64(epoch) ^ mix64(((b << 32) | step) & M64) ^ depth)
+    return float(h >> 11) * 2.0 ** -53
+
+
+def discrete_draw(priors, u):
+    """std::discrete_distribution<>(priors) at the uniform u in libstdc++: double sum, p / sum, partial sums with the last
+    set to 1.0, lower_bound; fewer than two outcomes draw 0"""
+    if len(priors) < 2:
+        return 0
+    s = 0.0
+    for p in priors:
+        s += float(p)
+    cp, acc = [], 0.0
+    for p in priors:
+        acc += float(p) / s
+        cp.append(acc)
+    cp[-1] = 1.0
+    return int(np.searchsorted(np.asarray(cp), u, side="left"))
+
+
+def _chance_chains(C, B, S, seed, key, variant=0):
+    """B trees whose decision nodes have one action, so every descent alternates action 0 and a chance draw; the chance
+    leaves get random logits (some far below the rest: zero priors).  Returns the port's per-simulation paths and the
+    logits of every chance node, keyed by its path."""
+    from oracle import ctree_port_stoch as ps
+    rng = np.random.default_rng(seed)
+    roots = ps.Roots(B, [[0]] * B, C, max_sims=S, action_space_size=1)
+    roots.prepare_no_noise([0.] * B, np.zeros((B, 1), np.float32).tolist(), [-1] * B)
+    roots.set_tie_hash(*key)
+    roots.set_chance_variant(variant)
+    mm = ps.MinMaxStatsList(B)
+    mm.set_delta(0.01)
+    nodes, paths = {}, []
+    for s in range(S):
+        res = ps.ResultsWrapper(B)
+        ch, _, _, _, vtp = ps.batch_traverse(roots, 19652, 1.25, 0.997, mm, res, [-1] * B, False)
+        traj = roots.get_trajectories()
+        paths.append(traj)
+        logits = (rng.standard_normal((B, C)) * 2).astype(np.float32)
+        logits[rng.random((B, C)) < 0.2] = -200.0
+        for b in range(B):
+            if ch[b]:
+                nodes[(b,) + tuple(traj[b])] = logits[b]
+        pol = [logits[b].tolist() if ch[b] else [0.0] for b in range(B)]
+        ps.batch_backpropagate(s + 1, 0.997, rng.standard_normal(B).tolist(), rng.standard_normal(B).tolist(), pol, mm, res,
+                               vtp, ch, list(range(B)))
+    return paths, nodes, roots.tie_stats()
+
+
+@pytest.mark.parametrize("C", [2, 7, 40])
+def test_chance_draw_is_the_device_formula(C):
+    """Hash mode (no pinned u): every chance outcome of the port is lower_bound(partial sums of the node's priors, u) with
+    u = (mix64(seed ^ mix64(epoch) ^ mix64((b << 32) | step) ^ depth) >> 11) * 2^-53, restated here in Python, for every
+    (tree, step, depth) of a few thousand draws; the chance draw counter counts them"""
+    B, S, key = 150, 14, (0xdeadbeefcafe, 5, 3)
+    paths, nodes, st = _chance_chains(C, B, S, 100 + C, key)
+    n = 0
+    for s, traj in enumerate(paths):
+        for b in range(B):
+            for d in range(1, len(traj[b]), 2):
+                pri = priors_of(nodes[(b,) + tuple(traj[b][:d])])
+                assert traj[b][d] == discrete_draw(pri, chance_u(key[0], key[1], b, key[2] + s, d)), (b, s, d)
+                n += 1
+    assert n > 2000 and st["chance"] == n and st["ties"] == 0
+    assert max(len(t) for p in paths for t in p) >= 5
+
+
+@pytest.mark.parametrize("variant", [1, 2, 3, 4])
+def test_chance_draw_mutants_change_the_outcomes(variant):
+    """The sensitivity mutants of the chance key (epoch + 1, step + 1, depth - 1) and the modulo draw h % C give other
+    outcomes on most draws where the priors leave a choice"""
+    C, B, S, key = 5, 150, 8, (77, 2, 0)
+    base, _, _ = _chance_chains(C, B, S, 7, key)
+    mut, _, _ = _chance_chains(C, B, S, 7, key, variant)
+    first = [next((s for s in range(S) if base[s][b] != mut[s][b]), None) for b in range(B)]
+    assert sum(f is not None for f in first) > 0.8 * B, variant
