@@ -263,10 +263,26 @@ typedef struct lz_mlp_stochastic_config {
     float support_min, support_max, support_step;
 } lz_mlp_stochastic_config;
 int lz_model_create_mlp_stochastic(const lz_mlp_stochastic_config *cfg, lz_model **out);
-/* StochasticMuZeroModel.recurrent_inference(state, option, afterstate) (stochastic_muzero_model.py:233-273) on B rows:
- * afterstate = 0: afterstate dynamics over [latent d_state | one-hot action d_option] and the afterstate prediction, so
+/* StochasticMuZeroModel with downsample=False (lzero/model/stochastic_muzero_model.py; board observations, the 2048 config):
+ * the board network of lz_model_create (representation_network, prediction_network) plus dynamics_network over [afterstate |
+ * one plane of value chance / chance_space_size], afterstate_dynamics_network over [latent | one plane of value
+ * action / action_space_size] and afterstate_prediction_network (chance_space_size policy outputs), all on the board
+ * tensor-core kernel.  State-dict names follow the reference class; chance_encoder.* and the SSL projection entries are
+ * ignored.  base takes the board envelope of lz_model_create (downsample = 0, efficientzero = 0, num_channels 16 / 32 / 64,
+ * boards up to 8x8, 1-16 observation planes, 1-64 actions) and chance_space_size is 1-64; anything else is LZ_EINVAL
+ * (downsample = 1, the Atari Stochastic MuZero network, is not supported).  Latents are f32 [B, num_channels, obs_h, obs_w].
+ * initial_inference is lz_model_initial_inference, recurrent_inference lz_model_recurrent_inference_stochastic; its searches
+ * run on stochastic trees through lz_search_run and lz_search_collect as StochasticMuZeroModelMLP's. */
+typedef struct lz_stochastic_config {
+    lz_model_config base;
+    int chance_space_size;
+} lz_stochastic_config;
+int lz_model_create_stochastic(const lz_stochastic_config *cfg, lz_model **out);
+/* StochasticMuZeroModel.recurrent_inference(state, option, afterstate) (stochastic_muzero_model.py:233-273) on B rows, for
+ * either Stochastic MuZero model (StochasticMuZeroModelMLP: one-hot encodings; StochasticMuZeroModel: one scalar plane):
+ * afterstate = 0: afterstate dynamics over [latent d_state | action d_option] and the afterstate prediction, so
  *   d_next_state is the afterstate and d_policy_logits f32 [B, chance_space_size] the chance logits;
- * afterstate = 1: dynamics over [afterstate d_state | one-hot chance outcome d_option] and the prediction, so d_next_state is
+ * afterstate = 1: dynamics over [afterstate d_state | chance outcome d_option] and the prediction, so d_next_state is
  *   the next latent and d_policy_logits f32 [B, action_space_size].
  * Reward and value as lz_model_recurrent_inference (logits f32 [B, K], scalars f32 [B]); outputs may be NULL.  d_row_mask
  * int32 [B] or NULL: row b is computed only when (d_row_mask[b] & 1) == (row_mask_on & 1), and the other rows are neither
@@ -338,8 +354,10 @@ int lz_model_debug_tower_stage(lz_model *m, int B, const float *d_obs, const uin
  * [B, latent_dim], a zero section [B, latent_dim], value logits [B,K], policy logits [B,P], value [B], and for the recurrent
  * programs reward logits [B,K], reward [B].  StochasticMuZeroModelMLP's `which` 0 is its dynamics program on afterstates
  * d_latent and chance outcomes d_action (P = A); `which` 2 is its afterstate program on latents d_latent and actions d_action:
- * the afterstate dynamics, its reward head and the afterstate prediction (P = chance_space_size).  Any other model refuses
- * `which` 2 (LZ_EINVAL). */
+ * the afterstate dynamics, its reward head and the afterstate prediction (P = chance_space_size).
+ * StochasticMuZeroModel (board): `which` 0 and 1 as for the board models (`which` 0 its dynamics program on afterstates and
+ * chance outcomes); `which` 2 its afterstate program on latents and actions, with the board models' stages and outputs and
+ * policy logits [B, chance_space_size] in both policy sections.  Any other model refuses `which` 2 (LZ_EINVAL). */
 int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_latent, const int32_t *d_action, int stage,
                              void *d_out, size_t out_bytes, int32_t *h_info, lz_stream s);
 int lz_model_latent_hw(const lz_model *m);   /* 6 for 84/96, 8 for 64; a square board's side; 0 for a non-square board */
@@ -385,7 +403,7 @@ int lz_search_destroy(lz_search *q);
  * one CUDA graph of [Gumbel descent] + num_simulations x [recurrent_inference, Gumbel back-up + next descent]; `deterministic`
  * is ignored, the roots must be freshly prepared (no descent since lz_tree_prepare; LZ_ESTATE) and the search's
  * num_simulations may not exceed the tree's Gumbel num_simulations (LZ_EINVAL).
- * On a stochastic tree (lz_tree_set_stochastic) with a StochasticMuZeroModelMLP: StochasticMuZeroMCTSCtree.search
+ * On a stochastic tree (lz_tree_set_stochastic) with a Stochastic MuZero model: StochasticMuZeroMCTSCtree.search
  * (mcts_ctree_stochastic.py:117-252), one CUDA graph of [descent] + num_simulations x [the afterstate program on the leaves that
  * are chance nodes, the dynamics program on the others (one row mask, its two parities), back-up + next descent]; both programs
  * write the same latent pool slot.  `deterministic` is the decision nodes' tie rule.  lz_search_collect* runs the same graph
@@ -413,7 +431,7 @@ int lz_search_run_ez(lz_search *q, const float *d_latent_roots, const float *d_h
  * (GumbelMuZeroPolicy._forward_collect, gumbel_muzero.py:560-571) and the search is the Gumbel graph of lz_search_run; the
  * search's num_simulations may not exceed the tree's Gumbel num_simulations (LZ_EINVAL).  The same holds for the three
  * entry points below.  Read the results with lz_tree_results and lz_tree_gumbel_select_action.
- * On a stochastic tree (lz_tree_set_stochastic) with a StochasticMuZeroModelMLP (StochasticMuZeroPolicy._forward_collect /
+ * On a stochastic tree (lz_tree_set_stochastic) with a Stochastic MuZero model (StochasticMuZeroPolicy._forward_collect /
  * _forward_eval, lzero/policy/stochastic_muzero.py:578-760) the search is the stochastic graph of lz_search_run, and every row
  * of d_mask, d_noise and d_policy_logits is the tree's width W = max(action_space_size, chance_space_size) wide: d_policy_logits
  * receives initial_inference's policy in the first action_space_size columns of each row (the others are not written), mask

@@ -48,6 +48,11 @@ class MlpStochasticConfig(ctypes.Structure):
                 ("support_step", c_float)]
 
 
+class StochasticConfig(ctypes.Structure):
+    """struct lz_stochastic_config (include/lzb200.h)"""
+    _fields_ = [("base", ModelConfig), ("chance_space_size", c_int)]
+
+
 class ValueTables(ctypes.Structure):
     """struct lz_value_tables (include/lzb200.h): host struct of device table pointers"""
     _fields_ = [("N", c_int), ("K1", c_int), ("W", c_int), ("P", c_int), ("value_prefix", c_int), ("fp32", c_int),
@@ -83,6 +88,7 @@ SIGNATURES = {
     "lz_model_create_mlp": (c_int, [ctypes.POINTER(MlpConfig), ctypes.POINTER(c_void_p)]),
     "lz_model_create_mlp_ez": (c_int, [ctypes.POINTER(MlpEzConfig), ctypes.POINTER(c_void_p)]),
     "lz_model_create_mlp_stochastic": (c_int, [ctypes.POINTER(MlpStochasticConfig), ctypes.POINTER(c_void_p)]),
+    "lz_model_create_stochastic": (c_int, [ctypes.POINTER(StochasticConfig), ctypes.POINTER(c_void_p)]),
     "lz_model_recurrent_inference_stochastic": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int] +
                                                 [c_void_p] * 7),
     "lz_model_destroy": (c_int, [c_void_p]),

@@ -17,10 +17,9 @@ from . import cabi, mz_tree
 from .efficientzero_model import EfficientZeroModel
 from .efficientzero_model_mlp import EfficientZeroModelMLP
 from .mcts_ctree import EfficientZeroMCTSCtree, GumbelMuZeroMCTSCtree, MuZeroMCTSCtree, StochasticMuZeroMCTSCtree
-from .model_base import LzModel
+from .model_base import LzModel, StochasticLzModel
 from .muzero_model import MuZeroModel
 from .muzero_model_mlp import MuZeroModelMLP
-from .stochastic_muzero_model_mlp import StochasticMuZeroModelMLP
 from .stochastic_mz_tree import chance_uniform
 
 _NP = {torch.uint8: np.uint8, torch.float32: np.float32, torch.int32: np.int32}
@@ -316,16 +315,16 @@ def _pad_columns(x, W):
 
 class StochasticMuZeroCollectPolicy(MuZeroCollectPolicy):
     """The same for ``StochasticMuZeroPolicy._forward_collect`` / ``_forward_eval`` (lzero/policy/stochastic_muzero.py:578-760)
-    with a ``StochasticMuZeroModelMLP``: the pooled tree is a stochastic tree W = max(action_space_size, chance_space_size)
-    wide, and one ``lz_search_collect*`` call runs initial_inference, the root reset and prepare and the stochastic search
-    graph.  The config key ``chance_seed`` is read as ``StochasticMuZeroMCTSCtree`` reads it: an integer pins every chance draw
+    with a Stochastic MuZero model (``StochasticMuZeroModelMLP`` or ``StochasticMuZeroModel``): the pooled tree is a
+    stochastic tree W = max(action_space_size, chance_space_size) wide, and one ``lz_search_collect*`` call runs
+    initial_inference, the root reset and prepare and the stochastic search graph.  The config key ``chance_seed`` is read as ``StochasticMuZeroMCTSCtree`` reads it: an integer pins every chance draw
     to std::mt19937(chance_seed)'s, None samples each step's draws afresh.  Masks and noises are [B, action_space_size] as the
     reference takes them; ``search_batch`` returns visits [B, W] (-1 padded, as ``stochastic_mz_tree.Roots``) and policy
     logits [B, action_space_size].  Output dicts have the reference's keys."""
 
-    def __init__(self, model: StochasticMuZeroModelMLP, cfg: Optional[dict] = None):
-        if not isinstance(model, StochasticMuZeroModelMLP):
-            raise TypeError(f"StochasticMuZeroCollectPolicy: the stochastic search runs a StochasticMuZeroModelMLP, not a "
+    def __init__(self, model: StochasticLzModel, cfg: Optional[dict] = None):
+        if not isinstance(model, StochasticLzModel):
+            raise TypeError(f"StochasticMuZeroCollectPolicy: the stochastic search runs a StochasticMuZeroModelMLP or StochasticMuZeroModel, not a "
                             f"{type(model).__name__}")
         super().__init__(model, cfg)
         self.mcts = StochasticMuZeroMCTSCtree(cfg or {})

@@ -20,6 +20,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <array>
 
 #include "board_tc.cuh"
 #include "model.cuh"
@@ -61,21 +62,28 @@ __host__ __device__ inline BoardSmem board_smem(int NT, int R, int H, int W)
     return s;
 }
 
-// row m of a CTA's padded grid -> (root slot r, pixel p); false for pad rows and absent roots
-__device__ __forceinline__ bool board_row(int m, int nvalid, int H, int W, int &r, int &p)
+// root b is computed: no row mask, or its mask bit selects it
+__device__ __forceinline__ bool board_root_on(const BoardIO &io, int b)
+{
+    return !io.row_mask || (__ldg(io.row_mask + b) & 1) == io.row_mask_on;
+}
+
+// row m of a CTA's padded grid -> (root slot r, pixel p); false for pad rows and absent roots (past the batch, or masked off)
+__device__ __forceinline__ bool board_row(const BoardIO &io, int m, int root0, int nvalid, int H, int W, int &r, int &p)
 {
     const int pitch = W + 1, rpr = (H + 1) * pitch;
     r = m / rpr;
     const int q = m - r * rpr, y = q / pitch, x = q - y * pitch;
     p = y * W + x;
-    return r < nvalid && y < H && x < W;
+    return r < nvalid && y < H && x < W && board_root_on(io, root0 + r);
 }
 
 // one head for the CTA's roots from the fp32 latent rows in skip: 1x1 conv + BN + ReLU -> feat, FC1 + BN1d + ReLU -> hid, FC2 ->
-// logits (one warp per root), the categorical heads' scalar through categorical_to_scalar
+// logits (one warp per root, rows ld apart in glog), the categorical heads' scalar through categorical_to_scalar; masked-off
+// roots are computed on their zero rows and not written
 template <int C>
-__device__ void board_head(const BoardNet &net, const BoardHead &hd, const float *skip, float *feat, float *hidb, float *lbuf, int nvalid,
-                           int root0, float *glog, float *gscal, bool categorical)
+__device__ void board_head(const BoardNet &net, const BoardIO &io, const BoardHead &hd, const float *skip, float *feat, float *hidb,
+                           float *lbuf, int nvalid, int root0, float *glog, int ld, float *gscal, bool categorical)
 {
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int H = net.H, W = net.W, P = H * W, pitch = W + 1, rpr = (H + 1) * pitch;
@@ -102,13 +110,14 @@ __device__ void board_head(const BoardNet &net, const BoardHead &hd, const float
     for (int r = warp; r < nvalid; r += kBoardThreads / 32) {
         const float *hv = hidb + r * hid;
         const int b = root0 + r;
+        if (!board_root_on(io, b)) continue;
         for (int k = lane; k < K; k += 32) {
             const float *w = hd.fc2 + (size_t)k * hid;
             float a = 0.0f;
             for (int j = 0; j < hid; ++j) a = fmaf(__ldg(w + j), hv[j], a);
             a += __ldg(hd.b2 + k);
             lrow[k] = a;
-            if (glog) glog[(size_t)b * K + k] = a;
+            if (glog) glog[(size_t)b * ld + k] = a;
         }
         __syncwarp();
         if (categorical) {
@@ -158,6 +167,11 @@ __global__ void __launch_bounds__(kBoardThreads, 1) k_board_tc(BoardNet net, Boa
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int root0 = blockIdx.x * R, nvalid = min(R, io.B - root0);
     const int nl = net.nlayers, total = nl * 9;
+    if (io.row_mask) {
+        bool any = false;
+        for (int r = tid; r < nvalid; r += kBoardThreads) any |= board_root_on(io, root0 + r);
+        if (!__syncthreads_or(any)) return;    // no selected root in this CTA: no weights streamed, nothing written
+    }
 
     auto issue = [&](int pos) {        // thread 0: tap pos of the program's weight stream into its ring stage
         const int layer = pos / 9, tap = pos - layer * 9;
@@ -183,7 +197,7 @@ __global__ void __launch_bounds__(kBoardThreads, 1) k_board_tc(BoardNet net, Boa
             const int c = i / (NT * 64), m = i - c * (NT * 64);
             int r, p;
             float v = 0.0f;
-            if (board_row(m, nvalid, H, W, r, p)) {
+            if (board_row(io, m, root0, nvalid, H, W, r, p)) {
                 const int b = root0 + r;
                 if (obs) v = c < io.obs_c ? io.obs[((size_t)b * io.obs_c + c) * P + p] : 0.0f;
                 else v = io.latent_base[(io.ix ? (size_t)io.ix[b] * io.slot_stride : 0) + ((size_t)b * C + c) * P + p];
@@ -206,7 +220,7 @@ __global__ void __launch_bounds__(kBoardThreads, 1) k_board_tc(BoardNet net, Boa
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             int r, p;
-            rinfo[t][h] = board_row(t * 64 + 16 * warp + (lane >> 2) + 8 * h, nvalid, H, W, r, p) ? ((r << 8) | p) : -1;
+            rinfo[t][h] = board_row(io, t * 64 + 16 * warp + (lane >> 2) + 8 * h, root0, nvalid, H, W, r, p) ? ((r << 8) | p) : -1;
         }
 
     const uint32_t act_s = smem_u32(act), ring_s = smem_u32(ring);
@@ -260,7 +274,7 @@ __global__ void __launch_bounds__(kBoardThreads, 1) k_board_tc(BoardNet net, Boa
                 const int m = t * 64 + 16 * warp + (lane >> 2) + 8 * h, info = rinfo[t][h];
                 const int r = info >> 8, p = info & 255, b = root0 + r;
                 const float *abr = nullptr;
-                if (ab && info >= 0) abr = net.abias + (size_t)min(max(io.action[b], 0), net.A - 1) * C * P + p;
+                if (ab && info >= 0) abr = net.abias + (size_t)min(max(io.action[b], 0), net.nopt - 1) * C * P + p;
 #pragma unroll
                 for (int j = 0; j < C / 8; ++j) {
                     const int c = 8 * j + 2 * (lane & 3);
@@ -295,13 +309,14 @@ __global__ void __launch_bounds__(kBoardThreads, 1) k_board_tc(BoardNet net, Boa
 
         if (flags & BF_HOOK_REWARD) {
             if (io.reward_logits || io.reward)
-                board_head<C>(net, net.head[0], skip, feat, hidb, lbuf, nvalid, root0, io.reward_logits, io.reward, true);
+                board_head<C>(net, io, net.head[0], skip, feat, hidb, lbuf, nvalid, root0, io.reward_logits, net.head[0].K, io.reward, true);
         }
         if (flags & BF_HOOK_VALPOL) {
             if (io.value_logits || io.value)
-                board_head<C>(net, net.head[1], skip, feat, hidb, lbuf, nvalid, root0, io.value_logits, io.value, true);
+                board_head<C>(net, io, net.head[1], skip, feat, hidb, lbuf, nvalid, root0, io.value_logits, net.head[1].K, io.value, true);
             if (io.policy_logits)
-                board_head<C>(net, net.head[2], skip, feat, hidb, lbuf, nvalid, root0, io.policy_logits, nullptr, false);
+                board_head<C>(net, io, net.head[2], skip, feat, hidb, lbuf, nvalid, root0, io.policy_logits,
+                              io.policy_stride ? io.policy_stride : net.head[2].K, nullptr, false);
         }
     }
 }
@@ -392,30 +407,79 @@ float board_pack_conv3(const float *w, int C, int cin_total, int cin_used, int c
     return scale;
 }
 
+// The encoding planes' share of a dynamics conv (torch [C][C + planes][3][3]) for each of n options: border-aware tap sums of the
+// option's plane, times its plane value, times the BN scale.  One-hot encoding (muzero_model.py:341-369): option o is plane o at
+// value 1.  Scalar plane (stochastic_muzero_model.py:354-377, 408-431): option o is plane 0 at value o / n in fp32, as the
+// reference computes it.  The tap sum accumulates in double and is rounded once.
+static void board_option_table(const std::vector<float> &w, int C, int cin_total, int H, int W, int n, bool onehot,
+                               const std::vector<float> &scale, float *dst)
+{
+    const int P = H * W;
+    for (int o = 0; o < n; ++o) {
+        const int plane = onehot ? o : 0;
+        const double v = onehot ? 1.0 : (double)((float)o / (float)n);
+        for (int co = 0; co < C; ++co)
+            for (int y = 0; y < H; ++y)
+                for (int x = 0; x < W; ++x) {
+                    double acc = 0.0;
+                    for (int t = 0; t < 9; ++t) {
+                        const int yy = y + t / 3 - 1, xx = x + t % 3 - 1;
+                        if (yy >= 0 && yy < H && xx >= 0 && xx < W) acc += w[((size_t)co * cin_total + C + plane) * 9 + t];
+                    }
+                    dst[((size_t)o * C + co) * P + y * W + x] = (float)(acc * v) * scale[co];
+                }
+    }
+}
+
 // ---- the Board family (lz_model::board) ----------------------------------------------------------------------------------
-// tables of the board network: fp16 hi/lo conv weights, folded BN, action planes, fp32 heads ----
+// tables of the board network: fp16 hi/lo conv weights, folded BN, option planes, fp32 heads.  MuZeroModel has two programs,
+// StochasticMuZeroModel (m->chance != 0, stochastic_muzero_model.py) three: `init` (representation + prediction), `rec`
+// (dynamics_network over [afterstate | chance plane] + prediction_network, recurrent_inference(afterstate=True)) and `after`
+// (afterstate_dynamics_network over [latent | action plane] + afterstate_prediction_network with chance_space_size policy
+// outputs, recurrent_inference(afterstate=False)).  Its dynamics networks name their BNs bn / bn_reward where MuZeroModel's
+// has norm_common / norm_reward, and its afterstate prediction network bn_value / bn_policy where prediction_network has
+// norm_value / norm_policy.
 int board_finalize(lz_model *m)
 {
     const lz_model_config &c = m->board.cfg;
     const int C = c.num_channels, A = c.action_space_size, n = c.num_res_blocks, H = c.obs_h, W = c.obs_w, P = H * W;
+    const int NC = m->chance;
+    const bool stoch = NC != 0;
     const std::string D = "dynamics_network.", Q = "prediction_network.", R = "representation_network.";
+    const std::string AD = "afterstate_dynamics_network.", AQ = "afterstate_prediction_network.";
+    const std::string dyn_bn = stoch ? "bn" : "norm_common", rew_bn = stoch ? "bn_reward" : "norm_reward";
     struct Conv { std::string w, bn; int cin_total, cin_used, cin_pad; };
-    // conv indices: 0 dyn conv | 1..2n dyn blocks | 2n+1..4n pred blocks | 4n+1..6n rep blocks | 6n+1 rep conv
+    // conv indices: 0 dyn conv | 1..2n dyn blocks | 2n+1..4n pred blocks | 4n+1..6n rep blocks | 6n+1 rep conv, and for
+    // StochasticMuZeroModel 6n+2 afterstate dyn conv | 6n+3..8n+2 its blocks | 8n+3..10n+2 afterstate pred blocks
     std::vector<Conv> convs;
-    convs.push_back({D + "conv.weight", D + "norm_common", C + A, C, C});
-    for (const std::string &pre : {D, Q, R})
+    auto blocks_of = [&](const std::string &pre) {
         for (int i = 0; i < n; ++i) {
             const std::string b = pre + "resblocks." + std::to_string(i);
             convs.push_back({b + ".conv1.0.weight", b + ".conv1.1", C, C, C});
             convs.push_back({b + ".conv2.0.weight", b + ".conv2.1", C, C, C});
         }
+    };
+    convs.push_back({D + "conv.weight", D + dyn_bn, C + (stoch ? 1 : A), C, C});
+    for (const std::string &pre : {D, Q, R}) blocks_of(pre);
     convs.push_back({R + "conv.weight", R + "norm", c.obs_c, c.obs_c, 16});   // observation planes padded to 16 with zero weights
+    const int after_conv = 6 * n + 2;
+    if (stoch) {
+        convs.push_back({AD + "conv.weight", AD + "bn", C + 1, C, C});
+        blocks_of(AD);
+        blocks_of(AQ);
+    }
+    // option tables of the recurrent programs' dynamics convs: rec (actions one-hot, or chance outcomes on a scalar plane),
+    // after (actions on a scalar plane)
+    struct OptTable { int conv, n; bool onehot; size_t off; };
+    std::vector<OptTable> tables = {{0, stoch ? NC : A, !stoch, 0}};
+    if (stoch) tables.push_back({after_conv, A, false, (size_t)NC * C * P});
+    const size_t ab_floats = tables.back().off + (size_t)tables.back().n * C * P;
     const int nconv = (int)convs.size();
     auto align = [](size_t v) { return (v + 127) & ~(size_t)127; };
     std::vector<size_t> woff(nconv);
     size_t off = 0;
     for (int i = 0; i < nconv; ++i) { woff[i] = off; off += (size_t)9 * convs[i].cin_pad * C * 4; }
-    const size_t off_bn = align(off), off_ab = align(off_bn + (size_t)nconv * 2 * C * 4), off_heads = align(off_ab + (size_t)A * C * P * 4);
+    const size_t off_bn = align(off), off_ab = align(off_bn + (size_t)nconv * 2 * C * 4), off_heads = align(off_ab + ab_floats * 4);
     std::vector<unsigned char> host(off_heads, 0);
     float *bn = reinterpret_cast<float *>(host.data() + off_bn), *ab = reinterpret_cast<float *>(host.data() + off_ab);
     for (int ci = 0; ci < nconv; ++ci) {
@@ -425,27 +489,24 @@ int board_finalize(lz_model *m)
         if (!w || !fold_bn(m, cv.bn, C, scale, shift)) return LZ_EINVAL;
         const float ws = board_pack_conv3(w->data(), C, cv.cin_total, cv.cin_used, cv.cin_pad, host.data() + woff[ci]);
         for (int k = 0; k < C; ++k) { bn[ci * 2 * C + k] = scale[k] / ws; bn[ci * 2 * C + C + k] = shift[k]; }
-        if (ci == 0)      // one-hot action planes (muzero_model.py:341-369): border-aware tap sums, times the BN scale
-            for (int a = 0; a < A; ++a)
-                for (int co = 0; co < C; ++co)
-                    for (int y = 0; y < H; ++y)
-                        for (int x = 0; x < W; ++x) {
-                            double acc = 0.0;
-                            for (int t = 0; t < 9; ++t) {
-                                const int yy = y + t / 3 - 1, xx = x + t % 3 - 1;
-                                if (yy >= 0 && yy < H && xx >= 0 && xx < W) acc += (*w)[((size_t)co * cv.cin_total + C + a) * 9 + t];
-                            }
-                            ab[((size_t)a * C + co) * P + y * W + x] = (float)acc * scale[co];
-                        }
+        for (const OptTable &t : tables)
+            if (t.conv == ci) board_option_table(*w, C, cv.cin_total, H, W, t.n, t.onehot, scale, ab + t.off);
     }
-    // heads: fp32 tables (conv bias folded into the 1x1 BN shift, Linear bias into the BN1d shift)
+    // heads: fp32 tables (conv bias folded into the 1x1 BN shift, Linear bias into the BN1d shift); reward, value, policy of
+    // rec and init, then of after
     struct HD { std::string conv, norm, fc; int hc, hid, K; };
-    const HD heads[3] = {{D + "conv1x1_reward", D + "norm_reward", D + "fc_reward_head", c.reward_head_channels, c.reward_hidden, m->K},
-                         {Q + "conv1x1_value", Q + "norm_value", Q + "fc_value", c.value_head_channels, c.value_hidden, m->K},
-                         {Q + "conv1x1_policy", Q + "norm_policy", Q + "fc_policy", c.policy_head_channels, c.policy_hidden, A}};
+    std::vector<HD> heads = {{D + "conv1x1_reward", D + rew_bn, D + "fc_reward_head", c.reward_head_channels, c.reward_hidden, m->K},
+                             {Q + "conv1x1_value", Q + "norm_value", Q + "fc_value", c.value_head_channels, c.value_hidden, m->K},
+                             {Q + "conv1x1_policy", Q + "norm_policy", Q + "fc_policy", c.policy_head_channels, c.policy_hidden, A}};
+    if (stoch) {
+        heads.push_back({AD + "conv1x1_reward", AD + "bn_reward", AD + "fc_reward_head", c.reward_head_channels, c.reward_hidden, m->K});
+        heads.push_back({AQ + "conv1x1_value", AQ + "bn_value", AQ + "fc_value", c.value_head_channels, c.value_hidden, m->K});
+        heads.push_back({AQ + "conv1x1_policy", AQ + "bn_policy", AQ + "fc_policy", c.policy_head_channels, c.policy_hidden, NC});
+    }
+    const int nheads = (int)heads.size();
     TablePacker hp;
-    size_t hoff[3][8];
-    for (int h = 0; h < 3; ++h) {
+    std::vector<std::array<size_t, 8>> hoff(nheads);
+    for (int h = 0; h < nheads; ++h) {
         const HD &d = heads[h];
         const int nin = d.hc * P;
         auto w1 = find_tensor(m, d.conv + ".weight", (size_t)d.hc * C), b1 = find_tensor(m, d.conv + ".bias", d.hc);
@@ -467,18 +528,26 @@ int board_finalize(lz_model *m)
     memset(&base, 0, sizeof(base));
     base.convw = m->board.d_board;
     base.bn = reinterpret_cast<const float *>(m->board.d_board + off_bn);
-    base.abias = reinterpret_cast<const float *>(m->board.d_board + off_ab);
+    const float *abd = reinterpret_cast<const float *>(m->board.d_board + off_ab);
     const float *hb = reinterpret_cast<const float *>(m->board.d_board + off_heads);
-    for (int h = 0; h < 3; ++h) {
-        BoardHead &o = base.head[h];
-        o.w1 = hb + hoff[h][0]; o.s1 = hb + hoff[h][1]; o.t1 = hb + hoff[h][2];
-        o.fc1 = hb + hoff[h][3]; o.s2 = hb + hoff[h][4]; o.t2 = hb + hoff[h][5];
-        o.fc2 = hb + hoff[h][6]; o.b2 = hb + hoff[h][7];
-        o.hc = heads[h].hc; o.hid = heads[h].hid; o.K = heads[h].K;
-    }
-    base.C = C; base.H = H; base.W = W; base.A = A;
+    base.C = C; base.H = H; base.W = W;
     base.support_min = c.support_min; base.support_step = c.support_step;
-    BoardNet rec = base, init = base;
+    // a program's three heads from heads[h0 ..], its option table from tables[t]
+    auto program = [&](int h0, int t) {
+        BoardNet net = base;
+        for (int h = 0; h < 3; ++h) {
+            BoardHead &o = net.head[h];
+            const std::array<size_t, 8> &q = hoff[h0 + h];
+            o.w1 = hb + q[0]; o.s1 = hb + q[1]; o.t1 = hb + q[2];
+            o.fc1 = hb + q[3]; o.s2 = hb + q[4]; o.t2 = hb + q[5];
+            o.fc2 = hb + q[6]; o.b2 = hb + q[7];
+            o.hc = heads[h0 + h].hc; o.hid = heads[h0 + h].hid; o.K = heads[h0 + h].K;
+        }
+        net.abias = abd + tables[t].off;
+        net.nopt = tables[t].n;
+        return net;
+    };
+    BoardNet rec = program(0, 0), init = program(0, 0), after = stoch ? program(3, 1) : base;
     auto add = [&](BoardNet &net, int ci, int flags) {
         net.layer_woff[net.nlayers] = (uint32_t)woff[ci];
         net.layer_bn[net.nlayers] = ci * 2 * C;
@@ -496,7 +565,12 @@ int board_finalize(lz_model *m)
     add(init, 6 * n + 1, BF_OBS | BF_STORE_RES);
     blocks(init, 4 * n + 1, BF_WRITE_LATENT);
     blocks(init, 2 * n + 1, BF_HOOK_VALPOL);
-    m->board.rec = rec; m->board.init = init;
+    if (stoch) {
+        add(after, after_conv, BF_RES | BF_STORE_RES | BF_ACT_BIAS);
+        blocks(after, after_conv + 1, BF_WRITE_LATENT | BF_HOOK_REWARD);
+        blocks(after, after_conv + 1 + 2 * n, BF_HOOK_VALPOL);
+    }
+    m->board.rec = rec; m->board.init = init; m->board.after = after;
     return board_prepare_launch();
 }
 
@@ -514,7 +588,8 @@ int board_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
     b.latent_base = io.latent_base; b.ix = io.ix; b.slot_stride = io.slot_stride; b.action = io.action;
     b.latent_out = io.next_latent; b.reward = io.reward; b.value = io.value; b.policy_logits = io.policy_logits;
     b.reward_logits = io.reward_logits; b.value_logits = io.value_logits;
-    return board_launch(m->board.rec, b, s);
+    b.policy_stride = io.policy_stride; b.row_mask = io.row_mask; b.row_mask_on = io.row_mask_on;
+    return board_launch(io.after_program ? m->board.after : m->board.rec, b, s);
 }
 
 int board_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, cudaStream_t s)
@@ -522,15 +597,19 @@ int board_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, c
     BoardIO b = board_io(m, B);
     b.obs = d_obs; b.latent_out = io_in.latent; b.latent_out2 = io_in.latent2;
     b.value = io_in.value; b.policy_logits = io_in.policy_logits; b.value_logits = io_in.value_logits;
+    b.policy_stride = io_in.policy_stride;
     return board_launch(m->board.init, b, s);
 }
 
-// lz_model_debug_net_stage of the board network: which 1 is the whole initial_inference program, d_latent the observations
+// lz_model_debug_net_stage of the board network: which 1 is the whole initial_inference program, d_latent the observations;
+// which 2 StochasticMuZeroModel's afterstate program (policy logits chance_space_size wide)
 int board_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out,
                              size_t out_bytes, int32_t *h_info, cudaStream_t st)
 {
-    BoardNet net = which ? m->board.init : m->board.rec;      // a copy: the model's programs stay as they are
-    const int nl = net.nlayers, K = m->K, A = m->A;
+    // a copy: the model's programs stay as they are
+    BoardNet net = which == 2 ? m->board.after : which ? m->board.init : m->board.rec;
+    const int nl = net.nlayers, K = m->K, A = net.head[2].K;
+    const bool obs = which == 1;
     LZ_REQUIRE(stage <= nl, LZ_EINVAL, "lz_model_debug_net_stage: stage %d past the %d layers of the program", stage, nl);
     const size_t nfl = stage < nl ? (size_t)B * m->latent_floats : (size_t)B * (2 * K + 2 * A + 4);
     LZ_REQUIRE(out_bytes >= nfl * sizeof(float), LZ_EINVAL, "lz_model_debug_net_stage: stage %d needs %zu bytes, got %zu", stage,
@@ -540,7 +619,7 @@ int board_debug_stage(lz_model *m, int which, int B, const float *d_in, const in
     memcpy(h_info, info, sizeof(info));
     float *o = reinterpret_cast<float *>(d_out);
     BoardIO io = board_io(m, B);
-    if (which) io.obs = d_in;
+    if (obs) io.obs = d_in;
     else { io.latent_base = d_in; io.action = d_action; }
     if (stage < nl) {
         // the program cut after layer `stage`, whose output is the only latent written; no head runs
@@ -555,11 +634,11 @@ int board_debug_stage(lz_model *m, int which, int B, const float *d_in, const in
     float *rl = o, *vl = rl + (size_t)B * K, *pl = vl + (size_t)B * K, *r = pl + (size_t)B * A, *v = r + B;
     float *pl2 = v + B, *r2 = pl2 + (size_t)B * A, *v2 = r2 + B;
     io.policy_logits = pl; io.value_logits = vl; io.value = v;
-    if (!which) { io.reward_logits = rl; io.reward = r; }
+    if (!obs) { io.reward_logits = rl; io.reward = r; }
     int rc = board_launch(net, io, st);
     if (rc) return rc;
     io.policy_logits = pl2; io.value_logits = nullptr; io.value = v2;
-    io.reward_logits = nullptr; io.reward = which ? nullptr : r2;
+    io.reward_logits = nullptr; io.reward = obs ? nullptr : r2;
     return board_launch(net, io, st);
 }
 

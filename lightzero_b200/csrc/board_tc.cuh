@@ -1,5 +1,6 @@
 // board_tc.cuh -- interface of the board-grid tensor-core network (board_tc.cu): MuZeroModel with downsample=False, the network of
-// the board-game configs (tictactoe, connect4, gomoku): every layer at the board's own H x W, C in {16, 32, 64} channels.
+// the board-game configs (tictactoe, connect4, gomoku), and StochasticMuZeroModel with downsample=False (2048): every layer at
+// the board's own H x W, C in {16, 32, 64} channels.
 #pragma once
 #include "lz_common.cuh"
 
@@ -21,9 +22,10 @@ struct BoardHead {                 // conv1x1 -> BN -> ReLU -> Linear(hc*P -> hi
 struct BoardNet {
     const unsigned char *convw;    // per conv: [9 taps][cin / 8 k-groups][C hi rows | C lo rows][8] fp16, K-major core matrices
     const float *bn;               // per conv: [scale C | shift C] (the weights' power-of-two scale folded into scale)
-    const float *abias;            // [A][C][P]: the one-hot action planes' share of the dynamics conv, times its BN scale
-    BoardHead head[3];             // reward, value, policy
-    int C, H, W, A;
+    const float *abias;            // [nopt][C][P]: the option encoding planes' share of the dynamics conv, times its BN scale
+    BoardHead head[3];             // reward, value, policy (the policy head is K = chance_space_size wide in the afterstate program)
+    int C, H, W;
+    int nopt;                      // options of the program's dynamics conv (actions, or chance outcomes): rows of abias
     int nlayers;
     uint32_t layer_woff[kBoardMaxLayers];   // byte offset of the layer's conv weights in convw
     int layer_bn[kBoardMaxLayers];          // float offset of its [scale | shift] in bn
@@ -38,11 +40,16 @@ struct BoardIO {
     const float *latent_base;      // input latents: base + ix[b] * slot_stride + b * C * P (NCHW)
     const int *ix;                 // or nullptr
     size_t slot_stride;
-    const int *action;             // [B]
+    const int *action;             // [B] options (actions or chance outcomes)
     float *latent_out, *latent_out2;   // [B][C][P] or nullptr
     float *reward, *value;         // [B] or nullptr
-    float *policy_logits;          // [B][A] or nullptr
+    float *policy_logits;          // [B][policy_stride] or nullptr
     float *reward_logits, *value_logits;   // [B][K] or nullptr
+    int policy_stride;             // row stride of policy_logits (0: the policy head's width)
+    // optional row mask: with row_mask, root b is computed only when (row_mask[b] & 1) == row_mask_on; any other root is an
+    // absent root (its latent and option are not read, none of its outputs is written)
+    const int *row_mask;
+    int row_mask_on;
 };
 
 // plan of a launch: roots per CTA, 64-row tiles per CTA, CTAs, roots of the last CTA, shared memory bytes

@@ -525,7 +525,7 @@ int mez_finalize(lz_model *m)
 {
     const MlpTcState &c = m->mez;
     const bool mz = !m->vp;
-    const int L = c.latent, A = m->A, C = c.chance, K = m->K, kobs = (c.obs_dim + 31) / 32 * 32;
+    const int L = c.latent, A = m->A, C = m->chance, K = m->K, kobs = (c.obs_dim + 31) / 32 * 32;
     MezPacker P;
     P.m = m;
     MezNet init, rec, after;
@@ -587,7 +587,7 @@ int mez_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
         LZ_REQUIRE(io.B <= m->ez.B, LZ_ESTATE, "model_recurrent: EfficientZero scratch sized for %d roots, got %d (model_reserve)", m->ez.B, io.B);
         LZ_REQUIRE(io.h_base && io.c_base, LZ_EINVAL, "model_recurrent: EfficientZero needs the reward hidden state");
     }
-    LZ_REQUIRE(!io.after_program || m->mez.chance, LZ_EINVAL, "model_recurrent: the afterstate program is StochasticMuZeroModelMLP's");
+    LZ_REQUIRE(!io.after_program || m->chance, LZ_EINVAL, "model_recurrent: the afterstate program is StochasticMuZeroModelMLP's");
     MezIO e = mez_io(m, io.B);
     e.latent_base = io.latent_base; e.ix = io.ix; e.slot_stride = io.slot_stride; e.action = io.action;
     e.row_mask = io.row_mask; e.row_mask_on = io.row_mask_on; e.policy_stride = io.policy_stride;
@@ -615,7 +615,7 @@ int mez_initial(lz_model *m, int B, const float *d_obs, const TailIO &io_in, cud
 int mez_debug_stage(lz_model *m, int which, int B, const float *d_in, const int32_t *d_action, int stage, void *d_out,
                            size_t out_bytes, int32_t *h_info, cudaStream_t st)
 {
-    LZ_REQUIRE(which != 2 || m->mez.chance, LZ_EINVAL, "lz_model_debug_net_stage: which 2 is StochasticMuZeroModelMLP's afterstate program");
+    LZ_REQUIRE(which != 2 || m->chance, LZ_EINVAL, "lz_model_debug_net_stage: which 2 is StochasticMuZeroModelMLP's afterstate program");
     MezNet net = which == 2 ? m->mez.after : which ? m->mez.init : m->mez.rec;   // a copy: the model's programs stay as they are
     const int L = net.L, K = net.K, A = net.A;
     const bool rew = which != 1 && !m->vp;           // MuZeroModelMLP's recurrent programs have the reward head

@@ -91,8 +91,8 @@ int check_create(const char *fn, float support_min, float support_max, float sup
 // ---- the internal launch API (model.cuh) -------------------------------------------------------------------------------------
 int model_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
 {
-    LZ_REQUIRE((!io.after_program && !io.row_mask) || m->family == ModelFamily::MlpTc, LZ_EINVAL,
-               "model_recurrent: afterstate programs and row masks are StochasticMuZeroModelMLP's");
+    LZ_REQUIRE((!io.after_program && !io.row_mask) || m->chance, LZ_EINVAL,
+               "model_recurrent: afterstate programs and row masks are the Stochastic MuZero models'");
     switch (m->family) {
         case ModelFamily::Conv: return conv_recurrent(m, io, s);
         case ModelFamily::Board: return board_recurrent(m, io, s);
@@ -104,8 +104,9 @@ int model_recurrent(lz_model *m, const RecIO &io, cudaStream_t s)
 
 int model_initial(lz_model *m, int B, const float *d_obs, const TailIO &io, cudaStream_t s)
 {
-    LZ_REQUIRE(!io.policy_stride || io.policy_stride == m->A || m->family == ModelFamily::MlpTc, LZ_EINVAL,
-               "model_initial: policy logits at a row stride of %d other than the %d actions are the MlpTc programs'", io.policy_stride, m->A);
+    LZ_REQUIRE(!io.policy_stride || io.policy_stride == m->A || m->chance, LZ_EINVAL,
+               "model_initial: policy logits at a row stride of %d other than the %d actions are the Stochastic MuZero models'",
+               io.policy_stride, m->A);
     switch (m->family) {
         case ModelFamily::Conv: return conv_initial(m, B, d_obs, io, s);
         case ModelFamily::Board: return board_initial(m, B, d_obs, io, s);
@@ -181,6 +182,20 @@ int lz_model_create(const lz_model_config *cfg, lz_model **out)
     return LZ_OK;
 }
 
+int lz_model_create_stochastic(const lz_stochastic_config *cfg, lz_model **out)
+{
+    LZ_REQUIRE(cfg && out, LZ_EINVAL, "lz_model_create_stochastic: null argument");
+    LZ_REQUIRE(cfg->base.downsample == 0, LZ_EINVAL,
+               "lz_model_create_stochastic: downsample=True (the Atari Stochastic MuZero network) is not supported; the board "
+               "network (downsample=False) is");
+    LZ_REQUIRE(!cfg->base.efficientzero, LZ_EINVAL, "lz_model_create_stochastic: efficientzero must be 0");
+    LZ_REQUIRE(cfg->chance_space_size >= 1 && cfg->chance_space_size <= 64, LZ_EINVAL,
+               "lz_model_create_stochastic: chance_space_size must be in [1, 64] (got %d)", cfg->chance_space_size);
+    const int rc = lz_model_create(&cfg->base, out);      // the board network's envelope
+    if (rc == LZ_OK) (*out)->chance = cfg->chance_space_size;
+    return rc;
+}
+
 int lz_model_create_mlp_ez(const lz_mlp_ez_config *cfg, lz_model **out)
 {
     LZ_REQUIRE(cfg && out, LZ_EINVAL, "lz_model_create_mlp_ez: null argument");
@@ -236,8 +251,8 @@ int lz_model_create_mlp_stochastic(const lz_mlp_stochastic_config *cfg, lz_model
     m->A = c.action_space_size; m->K = K; m->support_min = c.support_min; m->support_step = c.support_step;
     m->lat_c = m->latent_floats = c.latent_dim; m->lat_h = m->lat_w = 1;
     m->obs_elems = c.obs_dim;
-    m->mez = MlpTcState{c.obs_dim, c.latent_dim, c.reward_hidden, c.value_hidden, c.policy_hidden, c.res_connection_in_dynamics,
-                        c.chance_space_size};
+    m->chance = c.chance_space_size;
+    m->mez = MlpTcState{c.obs_dim, c.latent_dim, c.reward_hidden, c.value_hidden, c.policy_hidden, c.res_connection_in_dynamics};
     *out = m;
     return LZ_OK;
 }
@@ -260,7 +275,7 @@ int lz_model_set_tensor(lz_model *m, const char *name, const float *h_data, int6
     LZ_REQUIRE(m && name && h_data && numel >= 0, LZ_EINVAL, "lz_model_set_tensor: bad argument");
     std::string n(name);
     if (n.find("num_batches_tracked") != std::string::npos) return 1;
-    const bool stochastic = m->family == ModelFamily::MlpTc && m->mez.chance;     // StochasticMuZeroModelMLP's afterstate networks
+    const bool stochastic = m->chance != 0;     // the Stochastic MuZero models' afterstate networks
     if (n.rfind("representation_network.", 0) != 0 && n.rfind("dynamics_network.", 0) != 0 &&
         n.rfind("prediction_network.", 0) != 0 &&
         !(stochastic && (n.rfind("afterstate_dynamics_network.", 0) == 0 || n.rfind("afterstate_prediction_network.", 0) == 0)))
@@ -337,8 +352,7 @@ int lz_model_debug_net_stage(lz_model *m, int which, int B, const float *d_laten
     LZ_REQUIRE(m && which >= 0 && which <= 2 && B > 0 && d_latent && (which == 1 || d_action) && d_out && h_info && stage >= 0,
                LZ_EINVAL, "lz_model_debug_net_stage: bad argument");
     LZ_REQUIRE(m->finalized, LZ_ESTATE, "lz_model_debug_net_stage: model not finalized");
-    LZ_REQUIRE(which != 2 || (m->family == ModelFamily::MlpTc && m->mez.chance), LZ_EINVAL,
-               "lz_model_debug_net_stage: which 2 (the afterstate program) is StochasticMuZeroModelMLP's");
+    LZ_REQUIRE(which != 2 || m->chance, LZ_EINVAL, "lz_model_debug_net_stage: which 2 (the afterstate program) is the Stochastic MuZero models'");
     const cudaStream_t s = (cudaStream_t)s_;
     switch (m->family) {
         case ModelFamily::Conv: return conv_debug_stage(m, which, B, d_latent, d_action, stage, d_out, out_bytes, h_info, s);
@@ -373,8 +387,8 @@ int lz_model_recurrent_inference_stochastic(lz_model *m, int afterstate, int B, 
                                             float *d_reward, float *d_value, lz_stream s)
 {
     LZ_REQUIRE(m && d_state && d_option && B > 0, LZ_EINVAL, "lz_model_recurrent_inference_stochastic: bad argument");
-    LZ_REQUIRE(m->finalized && m->family == ModelFamily::MlpTc && m->mez.chance, LZ_ESTATE,
-               "lz_model_recurrent_inference_stochastic: not a finalized StochasticMuZeroModelMLP");
+    LZ_REQUIRE(m->finalized && m->chance, LZ_ESTATE,
+               "lz_model_recurrent_inference_stochastic: not a finalized Stochastic MuZero model");
     RecIO io;
     memset(&io, 0, sizeof(io));
     io.B = B; io.latent_base = d_state; io.action = d_option;

@@ -56,8 +56,8 @@ struct RecIO {
     size_t hslot_stride;
     float *h_out, *c_out;
     const int *is_reset;
-    // StochasticMuZeroModelMLP (MlpTc family only): after_program != 0 runs the afterstate program (afterstate dynamics + afterstate
-    // prediction, C chance logits into policy_logits) instead of the dynamics program; row_mask / row_mask_on as MezIO's
+    // Stochastic MuZero models (lz_model::chance != 0): after_program != 0 runs the afterstate program (afterstate dynamics +
+    // afterstate prediction, C chance logits into policy_logits) instead of the dynamics program; row_mask / row_mask_on as MezIO's
     int after_program;
     const int *row_mask;
     int row_mask_on;
@@ -72,7 +72,7 @@ struct TailIO {
     float *value;                     // [B] scalar or nullptr
     float *policy_logits;             // [B][A] (row stride policy_stride) or nullptr
     float *value_logits;              // [B][K] or nullptr
-    int policy_stride;                // row stride of policy_logits (0: A); only the MlpTc programs take a stride other than A
+    int policy_stride;                // row stride of policy_logits (0: A); only the Stochastic MuZero models take a stride other than A
 };
 
 // The model families: each has its own state below and its own module; model.cu switches on the family at every lz_model_*
@@ -109,6 +109,7 @@ struct BoardState {
     lz_model_config cfg;
     unsigned char *d_board;           // packed conv weights, BN / action-plane tables and fp32 head tables
     BoardNet rec, init;               // recurrent_inference / initial_inference programs
+    BoardNet after;                   // StochasticMuZeroModel's afterstate program (rec is its dynamics program on afterstates)
 };
 
 struct MlpFp32State {
@@ -119,7 +120,6 @@ struct MlpFp32State {
 
 struct MlpTcState {
     int obs_dim, latent, reward_hidden, value_hidden, policy_hidden, res;   // res: res_connection_in_dynamics
-    int chance;                       // StochasticMuZeroModelMLP: chance_space_size (0: the other MLP models)
     unsigned char *d_mez;             // packed fp16 hi / lo weights and fp32 tables of the dense layers
     MezNet rec, init;                 // recurrent_inference (dense part) / initial_inference programs
     MezNet after;                     // StochasticMuZeroModelMLP's afterstate program (rec is its dynamics program on afterstates)
@@ -141,6 +141,8 @@ struct lz_model {
     bool vp;                          // EfficientZero: the reward is a value prefix from the LSTM head in `ez`
     int lstm_hidden;                  // its LSTM width (0 without the head)
     int A, K;                         // actions, support size
+    int chance;                       // Stochastic MuZero models (StochasticMuZeroModelMLP, StochasticMuZeroModel): chance_space_size;
+                                      // 0 for every other model
     float support_min, support_step;
     int lat_c, lat_h, lat_w;          // latent shape of one root ([latent_dim][1][1] for the MLP families)
     int latent_floats;                // lat_c * lat_h * lat_w

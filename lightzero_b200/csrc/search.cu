@@ -245,8 +245,8 @@ int lz_search_create(lz_tree *t, lz_model *m, int num_simulations, lz_search **o
     LZ_REQUIRE(t && m && out && num_simulations > 0, LZ_EINVAL, "lz_search_create: bad argument");
     LZ_REQUIRE(m->finalized, LZ_ESTATE, "lz_search_create: model not finalized");
     LZ_REQUIRE(num_simulations <= t->max_sims, LZ_EINVAL, "lz_search_create: num_simulations %d > tree capacity %d", num_simulations, t->max_sims);
-    const int C = m->family == ModelFamily::MlpTc ? m->mez.chance : 0;
-    LZ_REQUIRE(C == t->p.nc, LZ_EINVAL, "lz_search_create: a StochasticMuZeroModelMLP needs a tree in stochastic mode with its "
+    const int C = m->chance;
+    LZ_REQUIRE(C == t->p.nc, LZ_EINVAL, "lz_search_create: a Stochastic MuZero model needs a tree in stochastic mode with its "
                "chance_space_size and any other model a tree without chance nodes (lz_tree_set_stochastic; model %d, tree %d)", C, t->p.nc);
     LZ_REQUIRE(t->p.na == m->A && t->p.A == std::max(m->A, C), LZ_EINVAL, "lz_search_create: tree has %d actions (width %d), model %d",
                t->p.na, t->p.A, m->A);

@@ -21,9 +21,8 @@ import numpy as np
 import torch
 
 from . import cabi, ez_tree, gmz_tree, mz_tree, stochastic_mz_tree
-from .model_base import LzModel
+from .model_base import LzModel, StochasticLzModel
 from .scaling_transform import DiscreteSupport, InverseScalarTransform
-from .stochastic_muzero_model_mlp import StochasticMuZeroModelMLP
 
 
 def _dev_f32(x, dev):
@@ -398,8 +397,8 @@ class GumbelMuZeroMCTSCtree(MuZeroMCTSCtree):
 class StochasticMuZeroMCTSCtree(MuZeroMCTSCtree):
     """Mirror of ``lzero.mcts.tree_search.mcts_ctree_stochastic.StochasticMuZeroMCTSCtree``: ``roots(n, legal_actions,
     chance_space_size)`` and ``search(roots, model, latent_state_roots, to_play_batch)``.  With a
-    ``lightzero_b200.StochasticMuZeroModelMLP`` the whole search is one CUDA graph (``lz_search_run`` on a stochastic tree);
-    any other model is driven step by step on the same device trees.
+    ``lightzero_b200`` Stochastic MuZero model (``StochasticMuZeroModelMLP`` or ``StochasticMuZeroModel``) the whole search is
+    one CUDA graph (``lz_search_run`` on a stochastic tree); any other model is driven step by step on the same device trees.
 
     Config key ``chance_seed``: an integer s makes every chance selection the draw of ``std::mt19937(s)``, which is what the
     reference draws when ``std::random_device`` returns s (its chance draws are otherwise not reproducible); None (the
@@ -413,13 +412,13 @@ class StochasticMuZeroMCTSCtree(MuZeroMCTSCtree):
         return stochastic_mz_tree.Roots(active_collect_env_num, legal_actions, chance_space_size)
 
     def search(self, roots: "stochastic_mz_tree.Roots", model, latent_state_roots, to_play_batch: Union[int, List[Any]]) -> None:
-        """mcts_ctree_stochastic.py:87-252.  ``latent_state_roots``: np.ndarray or CUDA tensor [B, latent_state_dim]."""
+        """mcts_ctree_stochastic.py:87-252.  ``latent_state_roots``: np.ndarray or CUDA tensor [B, latent_state_dim] or [B, C, H, W]."""
         S = int(self._cfg.num_simulations)
         roots.set_chance_seed(self._cfg.chance_seed)
         roots._materialize(S, self._params(), self.deterministic)
         t = roots._tree
         lat = _dev_f32(latent_state_roots, roots.device)
-        if not isinstance(model, StochasticMuZeroModelMLP):
+        if not isinstance(model, StochasticLzModel):
             self._search_stepwise_stochastic(roots, model, lat, S)
             return
         q = t.search_for(model, S)

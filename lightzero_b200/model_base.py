@@ -1,8 +1,8 @@
-"""What the four CUDA model wrappers (``MuZeroModel``, ``EfficientZeroModel``, ``MuZeroModelMLP``, ``EfficientZeroModelMLP``)
-share: one ``lz_model`` handle and its lifecycle, the weights from a reference ``state_dict``, the math mode, and the two
-inference bodies.  The model family is the class-level ``value_prefix`` flag: the EfficientZero models carry the LSTM
-value-prefix head, their ``recurrent_inference`` takes and returns the reward hidden state and their searches run on
-value-prefix trees."""
+"""What the CUDA model wrappers (``MuZeroModel``, ``EfficientZeroModel``, ``MuZeroModelMLP``, ``EfficientZeroModelMLP`` and
+the two Stochastic MuZero models) share: one ``lz_model`` handle and its lifecycle, the weights from a reference
+``state_dict``, the math mode, and the inference bodies.  The model family is the class-level ``value_prefix`` flag: the
+EfficientZero models carry the LSTM value-prefix head, their ``recurrent_inference`` takes and returns the reward hidden state
+and their searches run on value-prefix trees; the Stochastic MuZero models (``StochasticLzModel``) run on stochastic trees."""
 import itertools
 from dataclasses import dataclass
 from typing import Dict, Tuple
@@ -163,3 +163,38 @@ class LzModel:
                 self._lib.lz_model_destroy(self._h)
         except Exception:
             pass
+
+
+class StochasticLzModel(LzModel):
+    """Base of the Stochastic MuZero wrappers (``StochasticMuZeroModelMLP``, ``StochasticMuZeroModel``): a subclass sets
+    ``chance_space_size``.  Their searches run on stochastic trees, and ``recurrent_inference`` takes the reference's
+    ``afterstate`` flag."""
+    chance_space_size = 0
+
+    def recurrent_inference(self, state: torch.Tensor, option: torch.Tensor, afterstate: bool = False,
+                            return_scalars: bool = False) -> MZNetworkOutput:
+        """stochastic_muzero_model.py:233-273.  ``afterstate=False``: ``state`` is a latent and ``option`` an action; returns
+        the afterstate and its chance logits [B, chance_space_size].  ``afterstate=True``: ``state`` is an afterstate and
+        ``option`` a chance outcome; returns the next latent and its policy logits [B, action_space_size]."""
+        self._check()
+        d = self.device
+        state = state.to(d, torch.float32).contiguous()
+        if self._align_latents and state.data_ptr() % 16:
+            state = state.clone()
+        option = option.to(d).reshape(-1).to(torch.int32).contiguous()
+        B = state.shape[0]
+        nxt = torch.empty((B,) + self._latent, device=d)
+        policy = torch.empty(B, self.action_space_size if afterstate else self.chance_space_size, device=d)
+        value = torch.empty(B, self.value_support_size, device=d)
+        reward = torch.empty(B, self.reward_support_size, device=d)
+        rs = torch.empty(B, device=d) if return_scalars else None
+        vs = torch.empty(B, device=d) if return_scalars else None
+        with torch.cuda.device(d):
+            cabi.check(self._lib.lz_model_recurrent_inference_stochastic(
+                self._h, int(bool(afterstate)), B, state.data_ptr(), option.data_ptr(), None, 0, nxt.data_ptr(),
+                reward.data_ptr(), value.data_ptr(), policy.data_ptr(), cabi.ptr(rs), cabi.ptr(vs), cabi.stream_ptr()),
+                "lz_model_recurrent_inference_stochastic")
+        out = MZNetworkOutput(value, reward, policy, nxt)
+        if return_scalars:
+            out.reward_scalar, out.value_scalar = rs, vs
+        return out

@@ -315,7 +315,8 @@ def compute_target_reward_value(
     """Mirror of ``MuZeroGameBuffer._compute_target_reward_value`` (lzero/mcts/buffer/game_buffer_muzero.py:467-575) and, with
     ``efficientzero=True``, ``EfficientZeroGameBuffer._compute_target_reward_value`` (game_buffer_efficientzero.py:167-323), as
     one device call (``lz_value_targets`` / ``lz_value_targets_root``).  The ReZero, Gumbel MuZero and Stochastic MuZero buffers
-    inherit these (a StochasticMuZeroModelMLP gives the MuZero buffer's targets from its initial_inference values).
+    inherit these (a StochasticMuZeroModelMLP or StochasticMuZeroModel gives the MuZero buffer's targets from its
+    initial_inference values).
 
     The arguments are the fields of the reference's ``reward_value_context``: value_obs [N * (K + 1), ...] (host or device; row =
     segment * (K + 1) + position), value_mask, pos_in_game_segment_list [N], rewards_list (per segment the reward segment,
@@ -341,7 +342,7 @@ def compute_target_reward_value(
         raise ValueError(f"compute_target_reward_value: {T} rows, got value_obs {tuple(value_obs.shape)}")
     if not isinstance(model, LzModel):
         raise TypeError(f"compute_target_reward_value: {type(model).__name__} has no CUDA initial_inference (MuZeroModel, "
-                        "MuZeroModelMLP, StochasticMuZeroModelMLP, EfficientZeroModel or EfficientZeroModelMLP)")
+                        "MuZeroModelMLP, StochasticMuZeroModelMLP, StochasticMuZeroModel, EfficientZeroModel or EfficientZeroModelMLP)")
     if bool(efficientzero) != model.value_prefix:
         raise TypeError(f"compute_target_reward_value: the {'EfficientZero' if efficientzero else 'MuZero'} buffer's targets need "
                         f"{'an EfficientZero' if efficientzero else 'a MuZero'} model, not a {type(model).__name__}")

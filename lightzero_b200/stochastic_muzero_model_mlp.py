@@ -9,10 +9,10 @@ from typing import Optional, Sequence
 import torch
 
 from . import cabi
-from .model_base import LzModel, MZNetworkOutput
+from .model_base import StochasticLzModel
 
 
-class StochasticMuZeroModelMLP(LzModel):
+class StochasticMuZeroModelMLP(StochasticLzModel):
     _align_latents = True
 
     def __init__(self, observation_shape: int = 2, action_space_size: int = 6, chance_space_size: int = 2,
@@ -44,31 +44,3 @@ class StochasticMuZeroModelMLP(LzModel):
                                        policy_head_hidden_channels[0], int(bool(res_connection_in_dynamics)),
                                        value_support_range[0], value_support_range[1], value_support_range[2])
         self._create(device, "lz_model_create_mlp_stochastic", cfg, value_support_range)
-
-    def recurrent_inference(self, state: torch.Tensor, option: torch.Tensor, afterstate: bool = False,
-                            return_scalars: bool = False) -> MZNetworkOutput:
-        """stochastic_muzero_model.py:233-273.  ``afterstate=False``: ``state`` is a latent and ``option`` an action; returns
-        the afterstate and its chance logits [B, chance_space_size].  ``afterstate=True``: ``state`` is an afterstate and
-        ``option`` a chance outcome; returns the next latent and its policy logits [B, action_space_size]."""
-        self._check()
-        d = self.device
-        state = state.to(d, torch.float32).contiguous()
-        if state.data_ptr() % 16:
-            state = state.clone()
-        option = option.to(d).reshape(-1).to(torch.int32).contiguous()
-        B = state.shape[0]
-        nxt = torch.empty((B,) + self._latent, device=d)
-        policy = torch.empty(B, self.action_space_size if afterstate else self.chance_space_size, device=d)
-        value = torch.empty(B, self.value_support_size, device=d)
-        reward = torch.empty(B, self.reward_support_size, device=d)
-        rs = torch.empty(B, device=d) if return_scalars else None
-        vs = torch.empty(B, device=d) if return_scalars else None
-        with torch.cuda.device(d):
-            cabi.check(self._lib.lz_model_recurrent_inference_stochastic(
-                self._h, int(bool(afterstate)), B, state.data_ptr(), option.data_ptr(), None, 0, nxt.data_ptr(),
-                reward.data_ptr(), value.data_ptr(), policy.data_ptr(), cabi.ptr(rs), cabi.ptr(vs), cabi.stream_ptr()),
-                "lz_model_recurrent_inference_stochastic")
-        out = MZNetworkOutput(value, reward, policy, nxt)
-        if return_scalars:
-            out.reward_scalar, out.value_scalar = rs, vs
-        return out
