@@ -378,13 +378,6 @@ static int gumbel_readout(lz_tree *t, const GumbelReadout &o, cudaStream_t s)
     return LZ_OK;
 }
 
-int gumbel_launch_step(lz_tree *t, const TreeStep &a, cudaStream_t s)
-{
-    k_gumbel_step<<<gumbel_grid(t->p.B), kGumbelBlock, 0, s>>>(t->p, t->gumbel->g, a);
-    LZ_KERNEL_CHECK();
-    return LZ_OK;
-}
-
 int gumbel_prepare(lz_tree *t, const float *d_values, cudaStream_t s)
 {
     lz_gumbel *gs = t->gumbel;
@@ -407,8 +400,8 @@ int gumbel_step(lz_tree *t, const TreeStep &a, cudaStream_t s)
     } else {
         LZ_REQUIRE(gs->pending, LZ_ESTATE, "lz_tree_backpropagate: no Gumbel descent to back up (call lz_tree_traverse first)");
     }
-    int rc = gumbel_launch_step(t, a, s);
-    if (rc != LZ_OK) return rc;
+    k_gumbel_step<<<gumbel_grid(t->p.B), kGumbelBlock, 0, s>>>(t->p, gs->g, a);
+    LZ_KERNEL_CHECK();
     if (a.traverse) ++gs->traversals;
     gs->pending = a.traverse != 0;
     return LZ_OK;

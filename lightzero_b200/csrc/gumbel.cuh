@@ -16,13 +16,12 @@ struct GumbelParams {
 // the same float / double overloads as the reference binary.
 void gumbel_host_tables(int m, int S, int A, int *seq, float *gumbel);
 
-// One k_gumbel_step launch: back-up of latent_index (> 0), then the next Gumbel descent (a.traverse).
-int gumbel_launch_step(lz_tree *t, const TreeStep &a, cudaStream_t s);
 // lz_tree_prepare of a Gumbel tree after the MuZero prepare: the roots' value estimates d_values f32 [B] (CRoots::prepare,
 // cnode.cpp:418-455) and a fresh round of at most num_simulations descents.
 int gumbel_prepare(lz_tree *t, const float *d_values, cudaStream_t s);
-// lz_tree_traverse (a.traverse) / lz_tree_backpropagate (a.latent_index) of a Gumbel tree: gumbel_launch_step behind the checks
-// that every back-up follows a descent and that one prepare allows at most num_simulations descents.
+// tree_launch_step of a Gumbel tree: one k_gumbel_step launch, the back-up of latent_index (> 0) then the next Gumbel descent
+// (a.traverse), behind the checks that every back-up follows a descent and that one prepare allows at most num_simulations
+// descents.  The Gumbel descent draws no random numbers: a.deterministic and a.step are not read.
 int gumbel_step(lz_tree *t, const TreeStep &a, cudaStream_t s);
 void gumbel_free(lz_tree *t);
 

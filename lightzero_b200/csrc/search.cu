@@ -32,10 +32,6 @@ static RecIO rec_io(const lz_search *q, int sim)
     return io;
 }
 
-// MuZeroMCTSCtree.search (mcts_ctree.py:267-368), EfficientZeroMCTSCtree.search (:671-876) and their search_with_reuse variants
-// (:370-468, :878-1003): [descent] + S x [recurrent_inference, back-up (+ next descent)].  Under reuse every tree goes through the
-// network every simulation (the reference compacts the batch on the host; here the rows of "no inference" trees are computed and
-// ignored, which keeps the loop one static CUDA graph).
 // Persistent search: roots never interact, so the CTA that owns up to 8 roots can run their whole search -- tree
 // back-up / descent and the network -- for all num_simulations inside ONE launch of the tensor-core kernel.
 // EfficientZero stays a multi-kernel graph: its LSTM step is a GEMM over all roots (several launches per simulation).
@@ -58,66 +54,37 @@ static TcIO persistent_io(const lz_search *q, int deterministic)
     return io;
 }
 
-// GumbelMuZeroMCTSCtree.search (mcts_ctree.py:1076-1172): [Gumbel descent] + S x [recurrent_inference, Gumbel back-up + next
-// descent] with the non-persistent network kernels.
-static int enqueue_gumbel(lz_search *q, cudaStream_t s)
+// recurrent_inference of simulation sim.  A Stochastic MuZero model runs two programs, each on its own rows and into the same
+// pool slot and hand-off buffers: the afterstate program on the rows whose leaf is a chance node (odd depth, search_len in
+// d_len), then the dynamics program on the others (mcts_ctree_stochastic.py:171-212).
+static int recurrent_step(const lz_search *q, int sim, cudaStream_t s)
 {
-    int rc;
-    lz_tree *t = q->tree;
-    TreeStep descent = {};
-    descent.traverse = 1;
-    descent.ix = q->d_ix; descent.act = q->d_action;
-    if ((rc = gumbel_launch_step(t, descent, s))) return rc;
-    for (int sim = 0; sim < q->S; ++sim) {
-        if ((rc = model_recurrent(q->model, rec_io(q, sim), s))) return rc;
-        TreeStep step = descent;
-        step.traverse = sim + 1 < q->S;
-        step.latent_index = sim + 1;
-        step.reward = q->d_reward; step.value = q->d_value; step.logits = q->d_policy;
-        if ((rc = gumbel_launch_step(t, step, s))) return rc;
+    RecIO io = rec_io(q, sim);
+    if (!q->d_len) return model_recurrent(q->model, io, s);
+    io.row_mask = q->d_len; io.policy_stride = q->A;
+    for (int chance = 1; chance >= 0; --chance) {
+        io.after_program = chance; io.row_mask_on = chance;
+        if (int rc = model_recurrent(q->model, io, s)) return rc;
     }
     return LZ_OK;
 }
 
-// StochasticMuZeroMCTSCtree.search (mcts_ctree_stochastic.py:117-252): [descent] + S x [the afterstate program on the rows whose
-// leaf is a chance node (odd depth), the dynamics program on the others, back-up (+ next descent)].  The reference splits the
-// leaves on the host and backs up the two subsets one after the other; the trees are independent, so one back-up of every tree
-// is the same.  Both programs write pool slot sim + 1 and the same hand-off buffers, each only its own rows.
-static int enqueue_stochastic(lz_search *q, int deterministic, cudaStream_t s)
-{
-    int rc;
-    lz_tree *t = q->tree;
-    TreeStep descent = {};
-    descent.traverse = 1; descent.deterministic = deterministic;
-    descent.ix = q->d_ix; descent.act = q->d_action; descent.len = q->d_len;
-    if ((rc = tree_launch_step(t, descent, s))) return rc;
-    for (int sim = 0; sim < q->S; ++sim) {
-        RecIO io = rec_io(q, sim);
-        io.row_mask = q->d_len; io.policy_stride = q->A;
-        for (int chance = 1; chance >= 0; --chance) {
-            io.after_program = chance; io.row_mask_on = chance;
-            if ((rc = model_recurrent(q->model, io, s))) return rc;
-        }
-        TreeStep step = descent;
-        step.traverse = sim + 1 < q->S;
-        step.latent_index = sim + 1;
-        step.reward = q->d_reward; step.value = q->d_value; step.logits = q->d_policy;
-        if ((rc = tree_launch_step(t, step, s))) return rc;
-    }
-    return LZ_OK;
-}
-
+// MuZeroMCTSCtree.search (mcts_ctree.py:267-368), EfficientZeroMCTSCtree.search (:671-876) and their search_with_reuse variants
+// (:370-468, :878-1003), GumbelMuZeroMCTSCtree.search (:1076-1172) and StochasticMuZeroMCTSCtree.search
+// (mcts_ctree_stochastic.py:117-252): [descent] + S x [recurrent_inference, back-up (+ next descent)], each tree step the
+// kernel of the tree's mode (tree_launch_step).  Under reuse every tree goes through the network every simulation (the
+// reference compacts the batch on the host; here the rows of "no inference" trees are computed and ignored, which keeps the
+// loop one static CUDA graph).  The stochastic reference splits the leaves on the host and backs up the two subsets one
+// after the other; the trees are independent, so one back-up of every tree is the same.
 static int enqueue_search(lz_search *q, int deterministic, bool reuse, cudaStream_t s)
 {
-    if (q->tree->gumbel) return enqueue_gumbel(q, s);
     int rc;
     lz_tree *t = q->tree;
-    t->step_counter = 0;
-    if (t->p.nc) return enqueue_stochastic(q, deterministic, s);
+    if (!t->gumbel) t->step_counter = 0;      // the Gumbel descent takes no RNG step and leaves the counter as it is
     if (persistent_search(q, reuse)) return tc_launch(q->model->conv.tc_rec, persistent_io(q, deterministic), s, &t->p);
     TreeStep descent = {};
     descent.traverse = 1; descent.deterministic = deterministic;
-    descent.act = q->d_action; descent.is_reset = q->d_is_reset;
+    descent.act = q->d_action; descent.is_reset = q->d_is_reset; descent.len = q->d_len;
     if (reuse) {
         descent.true_action = q->d_true_action; descent.reuse_value = q->d_reuse_value;
         descent.ix_net = q->d_ix;
@@ -128,7 +95,7 @@ static int enqueue_search(lz_search *q, int deterministic, bool reuse, cudaStrea
     const bool fuse = !(reuse && q->hpool);
     if ((rc = tree_launch_step(t, descent, s))) return rc;
     for (int sim = 0; sim < q->S; ++sim) {
-        if ((rc = model_recurrent(q->model, rec_io(q, sim), s))) return rc;
+        if ((rc = recurrent_step(q, sim, s))) return rc;
         const bool next = sim + 1 < q->S;
         TreeStep step = descent;
         step.traverse = next && fuse;

@@ -195,6 +195,7 @@ static inline dim3 tree_grid(int B) { return dim3(ceil_div(B, kTreeBlock / 32));
 
 int tree_launch_step(lz_tree *t, const TreeStep &a_in, cudaStream_t s)
 {
+    if (t->gumbel) return gumbel_step(t, a_in, s);      // takes no step of the RNG counter
     TreeStep a = a_in;
     const bool reuse = a.reuse_value != nullptr;
     if (a.traverse) {
@@ -349,7 +350,7 @@ int lz_tree_traverse(lz_tree *t, int deterministic, const int32_t *d_true_action
     TreeStep a = {};
     a.traverse = 1; a.deterministic = deterministic; a.true_action = d_true_action; a.reuse_value = d_reuse_value;
     a.ix = d_ix; a.iy = d_iy; a.act = d_last_action; a.len = d_search_len; a.vtp = d_virtual_to_play; a.is_reset = d_is_reset;
-    return t->gumbel ? gumbel_step(t, a, (cudaStream_t)s) : tree_launch_step(t, a, (cudaStream_t)s);
+    return tree_launch_step(t, a, (cudaStream_t)s);
 }
 
 int lz_tree_backpropagate(lz_tree *t, int latent_index, const float *d_reward, const float *d_value, const float *d_logits,
@@ -368,7 +369,7 @@ int lz_tree_backpropagate(lz_tree *t, int latent_index, const float *d_reward, c
     TreeStep a = {};
     a.latent_index = latent_index; a.reward = d_reward; a.value = d_value; a.logits = d_logits; a.to_play = d_to_play;
     a.leaf_reset = d_is_reset; a.batch_rank = d_batch_rank; a.reuse_value = d_reuse_value;
-    return t->gumbel ? gumbel_step(t, a, (cudaStream_t)s) : tree_launch_step(t, a, (cudaStream_t)s);
+    return tree_launch_step(t, a, (cudaStream_t)s);
 }
 
 int lz_tree_set_ez(lz_tree *t, int efficientzero, int lstm_horizon_len)

@@ -603,7 +603,8 @@ struct TreeStep {
     int32_t *is_reset;                      // [B] EfficientZero: search_len % lstm_horizon == 0 of the reached node
 };
 
-// Launches one k_tree_step on s.  The MuZero descent takes a.deterministic; the EfficientZero and reuse descents take
-// p.tie_first.  Each descent consumes one step of the tree's RNG counter.
+// Launches the step kernel of the tree's mode on s: k_gumbel_step on a Gumbel tree (gumbel_step), else k_tree_step.  The
+// MuZero descent takes a.deterministic; the EfficientZero and reuse descents take p.tie_first.  Each k_tree_step descent
+// consumes one step of the tree's RNG counter.
 int tree_launch_step(lz_tree *t, const TreeStep &a, cudaStream_t s);
 }  // namespace lz

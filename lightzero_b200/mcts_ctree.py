@@ -110,15 +110,11 @@ class MuZeroMCTSCtree(object):
             raise TypeError(f"MuZeroMCTSCtree.search: an {type(model).__name__} needs EfficientZeroMCTSCtree")
         S = int(self._cfg.num_simulations)
         roots._materialize(S, self._params(), self.deterministic)     # reset + prepare on device, MinMax stats fresh (:291-292)
-        t = roots._tree
         lat = _dev_f32(latent_state_roots, roots.device)
         if family is None:
-            self._search_stepwise(roots, model, lat, S)
-            return
-        q = t.search_for(model, S)
-        with torch.cuda.device(roots.device):
-            cabi.check(t.lib.lz_search_run(q, lat.data_ptr(), int(self.deterministic), cabi.stream_ptr()), "lz_search_run")
-        self.last_num_kernels = t.lib.lz_search_num_kernels(q)
+            self._search_stepwise(roots, model, S, lat)
+        else:
+            self._run_fused(roots, model, S, (), "lz_search_run", lat.data_ptr(), int(self.deterministic))
 
     def search_with_reuse(self, roots: "mz_tree.Roots", model, latent_state_roots, to_play_batch: Union[int, List[Any]],
                           true_action_list=None, reuse_value_list=None):
@@ -136,17 +132,23 @@ class MuZeroMCTSCtree(object):
         """The fused search_with_reuse (lz_search_run_with_reuse) of either tree family from ``roots_state`` = (latents, LSTM
         h, LSTM c; None for MuZero); returns the reference's ``(length, average_infer)``."""
         roots._materialize(S, self._params(), self.deterministic)     # the reference draws rand() % len(ties) (cnode.cpp:610-640)
-        t, dev, B = roots._tree, roots.device, roots.num
+        dev, B = roots.device, roots.num
         ta = mz_tree._to_dev(true_action_list, torch.int32, dev, (B,))
         rv = mz_tree._to_dev(reuse_value_list, torch.float32, dev, (B,))
         counts = torch.empty(S, dtype=torch.int32, device=dev)
-        q = t.search_for(model, S, mode)
-        with torch.cuda.device(dev):
-            cabi.check(t.lib.lz_search_run_with_reuse(q, *(cabi.ptr(x) for x in roots_state), ta.data_ptr(), rv.data_ptr(),
-                                                      counts.data_ptr(), cabi.stream_ptr()), "lz_search_run_with_reuse")
-        self.last_num_kernels = t.lib.lz_search_num_kernels(q)
+        self._run_fused(roots, model, S, mode, "lz_search_run_with_reuse", *(cabi.ptr(x) for x in roots_state), ta.data_ptr(),
+                        rv.data_ptr(), counts.data_ptr())
         c = counts.cpu().numpy()
         return int(c[-1]), float(c.sum()) / S
+
+    def _run_fused(self, roots, model, S, mode, fn, *args):
+        """One fused search on the roots' tree: the lz_search handle of (model, S, mode), then the library call
+        ``fn(handle, *args, stream)``; records the kernel count of its search graph in ``last_num_kernels``."""
+        t = roots._tree
+        q = t.search_for(model, S, mode)
+        with torch.cuda.device(roots.device):
+            cabi.check(getattr(t.lib, fn)(q, *args, cabi.stream_ptr()), fn)
+        self.last_num_kernels = t.lib.lz_search_num_kernels(q)
 
     def _make_inverse_transforms(self, dev):
         """mcts_ctree.py:249-253: separate value and reward supports, both categorical (the only representation the CUDA
@@ -163,31 +165,42 @@ class MuZeroMCTSCtree(object):
         vr, rr = rng("value_support_range"), rng("reward_support_range")
         self._inv_reward = self._inv if vr == rr else InverseScalarTransform(DiscreteSupport(*rr, device=dev))
 
-    def _search_stepwise(self, roots, model, lat, S):
-        """The search driven one simulation at a time around any model object, on the descent and back-up of the tree's mode
-        (MuZero or Gumbel)."""
-        t = roots._tree
-        dev = roots.device
+    def _search_stepwise(self, roots, model, S, *states):
+        """The search driven one simulation at a time around any model object, on the descent and back-up of the tree's mode:
+        per simulation one descent, the model call ``_recurrent`` on the leaves it reached and one back-up.  ``states``: the
+        roots' latents, then an EfficientZero search's LSTM state h and c [B, lstm_hidden_size]; each has a pool of S + 1
+        slots, slot sim + 1 written by simulation sim.  An EfficientZero tree also hands the leaves' is_reset to the model
+        call and the back-up."""
+        t, dev, B = roots._tree, roots.device, roots.num
         self._make_inverse_transforms(dev)
-        B = roots.num
-        pool = torch.empty((S + 1,) + tuple(lat.shape), device=dev, dtype=torch.float32)
-        pool[0] = lat
+        pools = [torch.empty((S + 1,) + tuple(x.shape), device=dev, dtype=torch.float32) for x in states]
+        for pool, x in zip(pools, states):
+            pool[0] = x
         rows = torch.arange(B, device=dev)
+        reset = torch.empty(B, dtype=torch.int32, device=dev) if len(states) > 1 else None
         with torch.no_grad(), torch.cuda.device(dev):
             if hasattr(model, "eval"):
                 model.eval()
             for sim in range(S):
                 cabi.check(t.lib.lz_tree_traverse(t.h, int(self.deterministic), None, None, t.ix.data_ptr(), t.iy.data_ptr(),
-                                                  t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(), None,
-                                                  cabi.stream_ptr()), "lz_tree_traverse")
-                latent_states = pool[t.ix.long(), rows]                       # mcts_ctree.py:323-324 on device
-                out = model.recurrent_inference(latent_states, t.action.long())
-                pool[sim + 1] = out.latent_state
-                value = self._inv(out.value).reshape(-1).contiguous()        # :349 (value support)
-                reward = self._inv_reward(out.reward).reshape(-1).contiguous()      # :350 (reward support)
-                pol = out.policy_logits.to(torch.float32).contiguous()
+                                                  t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(),
+                                                  cabi.ptr(reset), cabi.stream_ptr()), "lz_tree_traverse")
+                ix = t.ix.long()
+                new_states, reward, value, logits = self._recurrent(model, t, [pool[ix, rows] for pool in pools],  # :323-324
+                                                                    t.action.long(), reset)
+                for pool, x in zip(pools, new_states):
+                    pool[sim + 1] = x
+                value = self._inv(value).reshape(-1).contiguous()            # :349 (value support)
+                reward = self._inv_reward(reward).reshape(-1).contiguous()   # :350 (reward support)
+                pol = logits.to(torch.float32).contiguous()
                 cabi.check(t.lib.lz_tree_backpropagate(t.h, sim + 1, reward.data_ptr(), value.data_ptr(), pol.data_ptr(), None,
-                                                       None, None, None, cabi.stream_ptr()), "lz_tree_backpropagate")
+                                                       None, cabi.ptr(reset), None, cabi.stream_ptr()), "lz_tree_backpropagate")
+
+    def _recurrent(self, model, t, states, action, reset):
+        """One simulation's model call on the gathered states of the leaves; returns (their new states, reward logits, value
+        logits, policy logits), every row of the batch."""
+        out = model.recurrent_inference(states[0], action)
+        return (out.latent_state,), out.reward, out.value, out.policy_logits
 
 
 class EfficientZeroMCTSCtree(MuZeroMCTSCtree):
@@ -219,15 +232,11 @@ class EfficientZeroMCTSCtree(MuZeroMCTSCtree):
         assert H > 0                                   # mcts_ctree.py:857
         roots._ez, roots._lstm_horizon = True, H
         roots._materialize(S, self._params(), self.deterministic)
-        t = roots._tree
         lat, h0, h1 = self._ez_inputs(roots, latent_state_roots, reward_hidden_state_roots)
         if not _value_prefix_model(model):
-            self._search_stepwise_ez(roots, model, lat, h0, h1, S, H)
-            return
-        q = t.search_for(model, S, (1, H))
-        with torch.cuda.device(roots.device):
-            cabi.check(t.lib.lz_search_run_ez(q, lat.data_ptr(), h0.data_ptr(), h1.data_ptr(), cabi.stream_ptr()), "lz_search_run_ez")
-        self.last_num_kernels = t.lib.lz_search_num_kernels(q)
+            self._search_stepwise(roots, model, S, lat, h0, h1)
+        else:
+            self._run_fused(roots, model, S, (1, H), "lz_search_run_ez", lat.data_ptr(), h0.data_ptr(), h1.data_ptr())
 
     def search_with_reuse(self, roots: "ez_tree.Roots", model, latent_state_roots, reward_hidden_state_roots,
                           to_play_batch: Union[int, List[Any]], true_action_list=None, reuse_value_list=None):
@@ -250,36 +259,14 @@ class EfficientZeroMCTSCtree(MuZeroMCTSCtree):
         return (_dev_f32(latent_state_roots, dev), _dev_f32(reward_hidden_state_roots[0], dev).reshape(B, -1),
                 _dev_f32(reward_hidden_state_roots[1], dev).reshape(B, -1))
 
-    def _search_stepwise_ez(self, roots, model, lat, h0, h1, S, H):
-        t = roots._tree
-        dev = roots.device
-        self._make_inverse_transforms(dev)
-        B = roots.num
-        pool = torch.empty((S + 1,) + tuple(lat.shape), device=dev, dtype=torch.float32)
-        hp0 = torch.zeros((S + 1, B, h0.shape[1]), device=dev)
-        hp1 = torch.zeros((S + 1, B, h1.shape[1]), device=dev)
-        pool[0], hp0[0], hp1[0] = lat, h0, h1
-        rows = torch.arange(B, device=dev)
-        reset = torch.empty(B, dtype=torch.int32, device=dev)
-        with torch.no_grad(), torch.cuda.device(dev):
-            if hasattr(model, "eval"):
-                model.eval()
-            for sim in range(S):
-                cabi.check(t.lib.lz_tree_traverse(t.h, 0, None, None, t.ix.data_ptr(), t.iy.data_ptr(), t.action.data_ptr(),
-                                                  t.search_len.data_ptr(), t.vtp.data_ptr(), reset.data_ptr(),
-                                                  cabi.stream_ptr()), "lz_tree_traverse")
-                ix = t.ix.long()
-                hidden = (hp0[ix, rows].unsqueeze(0), hp1[ix, rows].unsqueeze(0))          # mcts_ctree.py:819-831
-                out = model.recurrent_inference(pool[ix, rows], hidden, t.action.long())
-                pool[sim + 1] = out.latent_state
-                keep = (reset == 0).to(torch.float32).unsqueeze(1)                          # :856-863
-                hp0[sim + 1] = out.reward_hidden_state[0].reshape(B, -1) * keep
-                hp1[sim + 1] = out.reward_hidden_state[1].reshape(B, -1) * keep
-                value = self._inv(out.value).reshape(-1).contiguous()
-                vprefix = self._inv_reward(out.value_prefix).reshape(-1).contiguous()
-                pol = out.policy_logits.to(torch.float32).contiguous()
-                cabi.check(t.lib.lz_tree_backpropagate(t.h, sim + 1, vprefix.data_ptr(), value.data_ptr(), pol.data_ptr(), None,
-                                                       None, reset.data_ptr(), None, cabi.stream_ptr()), "lz_tree_backpropagate")
+    def _recurrent(self, model, t, states, action, reset):
+        """mcts_ctree.py:819-863: the leaves' LSTM state goes in, and the new state comes out zeroed where the leaf is reset."""
+        latent, h, c = states
+        out = model.recurrent_inference(latent, (h.unsqueeze(0), c.unsqueeze(0)), action)
+        keep = (reset == 0).to(torch.float32).unsqueeze(1)
+        B = latent.shape[0]
+        hidden = tuple(x.reshape(B, -1) * keep for x in out.reward_hidden_state)
+        return (out.latent_state,) + hidden, out.value_prefix, out.value, out.policy_logits
 
 
 class UniZeroMCTSCtree(MuZeroMCTSCtree):
@@ -383,15 +370,11 @@ class GumbelMuZeroMCTSCtree(MuZeroMCTSCtree):
         m = self._cfg.get("max_num_considered_actions", None)
         m = roots._pending["A"] if m is None else int(m)
         roots._materialize_gumbel((m, S), self._params())   # reset + prepare on device: a fresh search
-        t = roots._tree
         lat = _dev_f32(latent_state_roots, roots.device)
         if family is None:
-            self._search_stepwise(roots, model, lat, S)
-            return
-        q = t.search_for(model, S, ("gumbel",))
-        with torch.cuda.device(roots.device):
-            cabi.check(t.lib.lz_search_run(q, lat.data_ptr(), 1, cabi.stream_ptr()), "lz_search_run")
-        self.last_num_kernels = t.lib.lz_search_num_kernels(q)
+            self._search_stepwise(roots, model, S, lat)
+        else:
+            self._run_fused(roots, model, S, ("gumbel",), "lz_search_run", lat.data_ptr(), 1)
 
 
 class StochasticMuZeroMCTSCtree(MuZeroMCTSCtree):
@@ -416,49 +399,32 @@ class StochasticMuZeroMCTSCtree(MuZeroMCTSCtree):
         S = int(self._cfg.num_simulations)
         roots.set_chance_seed(self._cfg.chance_seed)
         roots._materialize(S, self._params(), self.deterministic)
-        t = roots._tree
         lat = _dev_f32(latent_state_roots, roots.device)
         if not isinstance(model, StochasticLzModel):
-            self._search_stepwise_stochastic(roots, model, lat, S)
-            return
-        q = t.search_for(model, S)
-        with torch.cuda.device(roots.device):
-            cabi.check(t.lib.lz_search_run(q, lat.data_ptr(), int(self.deterministic), cabi.stream_ptr()), "lz_search_run")
-        self.last_num_kernels = t.lib.lz_search_num_kernels(q)
+            self._search_stepwise(roots, model, S, lat)
+        else:
+            self._run_fused(roots, model, S, (), "lz_search_run", lat.data_ptr(), int(self.deterministic))
 
     def search_with_reuse(self, *args, **kwargs):
         """Refused: the reference's Stochastic MuZero has no search_with_reuse, and stochastic trees have no reuse descent."""
         raise NotImplementedError("StochasticMuZeroMCTSCtree has no search_with_reuse (stochastic trees have no reuse descent)")
 
-    def _search_stepwise_stochastic(self, roots, model, lat, S):
-        """The search driven one simulation at a time around any model with the reference's
-        ``recurrent_inference(state, option, afterstate)``: chance leaves (odd depth) take the afterstate program
-        (afterstate=False), the others the dynamics program (mcts_ctree_stochastic.py:171-212)."""
-        t, dev, B = roots._tree, roots.device, roots.num
-        self._make_inverse_transforms(dev)
-        pool = torch.empty((S + 1,) + tuple(lat.shape), device=dev, dtype=torch.float32)
-        pool[0] = lat
-        rows = torch.arange(B, device=dev)
-        with torch.no_grad(), torch.cuda.device(dev):
-            if hasattr(model, "eval"):
-                model.eval()
-            for sim in range(S):
-                cabi.check(t.lib.lz_tree_traverse(t.h, int(self.deterministic), None, None, t.ix.data_ptr(), t.iy.data_ptr(),
-                                                  t.action.data_ptr(), t.search_len.data_ptr(), t.vtp.data_ptr(), None,
-                                                  cabi.stream_ptr()), "lz_tree_traverse")
-                states, options = pool[t.ix.long(), rows], t.action.long()
-                chance = (t.search_len & 1).bool()
-                reward, value = torch.zeros(B, device=dev), torch.zeros(B, device=dev)
-                pol = torch.zeros(B, t.A, device=dev)
-                for is_chance in (True, False):
-                    sel = torch.nonzero(chance == is_chance).reshape(-1)
-                    if sel.numel() == 0:
-                        continue
-                    out = model.recurrent_inference(states[sel], options[sel], afterstate=not is_chance)
-                    pool[sim + 1, sel] = out.latent_state.to(torch.float32)
-                    value[sel] = self._inv(out.value).reshape(-1)
-                    reward[sel] = self._inv_reward(out.reward).reshape(-1)
-                    logits = out.policy_logits.to(torch.float32)
-                    pol[sel, :logits.shape[1]] = logits
-                cabi.check(t.lib.lz_tree_backpropagate(t.h, sim + 1, reward.data_ptr(), value.data_ptr(), pol.data_ptr(), None,
-                                                       None, None, None, cabi.stream_ptr()), "lz_tree_backpropagate")
+    def _recurrent(self, model, t, states, action, reset):
+        """The model with the reference's ``recurrent_inference(state, option, afterstate)``: chance leaves (odd depth) take
+        the afterstate program (afterstate=False), the others the dynamics program (mcts_ctree_stochastic.py:171-212); the
+        policy logits are padded to the tree's width max(A, C)."""
+        latent = states[0]
+        B, dev = latent.shape[0], latent.device
+        new = torch.empty_like(latent)
+        reward = torch.empty(B, self._inv_reward.support.size, device=dev)
+        value = torch.empty(B, self._inv.support.size, device=dev)
+        logits = torch.zeros(B, t.A, device=dev)
+        chance = (t.search_len & 1).bool()
+        for is_chance in (True, False):
+            sel = torch.nonzero(chance == is_chance).reshape(-1)
+            if sel.numel() == 0:
+                continue
+            out = model.recurrent_inference(latent[sel], action[sel], afterstate=not is_chance)
+            new[sel], reward[sel], value[sel] = out.latent_state, out.reward, out.value
+            logits[sel, :out.policy_logits.shape[1]] = out.policy_logits.to(torch.float32)
+        return (new,), reward, value, logits
